@@ -50,7 +50,7 @@ typedef enum {
   b200collFloat32 = 0,
   b200collFloat16 = 1,
   b200collBfloat16 = 2,
-  b200collFloat8e4m3 = 3,   /* output / wire type only */
+  b200collFloat8e4m3 = 3,   /* OCP FP8 E4M3 (finite max 448) */
   /* the types below take the generic reduction path (src/generic.cu): same type in and out, no scale, any operator but avg */
   b200collInt8 = 4,
   b200collUint8 = 5,
@@ -59,11 +59,22 @@ typedef enum {
   b200collInt64 = 8,
   b200collUint64 = 9,
   b200collFloat64 = 10,
-  b200collNumTypes = 11
+  b200collFloat8e5m2 = 11,  /* OCP FP8 E5M2 (finite max 57344) */
+  b200collNumTypes = 12
 } b200collDataType_t;
 
-/* sum and avg of fp16 / bf16 / fp32 run on the fused fast paths (Lamport, two-shot, NVLS); prod, min, max — and every operator on the
- * integer types and fp64 — run on one barrier-based P2P kernel that accumulates in the element type. */
+/* Fused-epilogue types are fp32, fp16, bf16, e4m3 and e5m2. Supported (in_dtype, out_dtype) pairs:
+ *   f32 -> f32, f16, bf16, e4m3, e5m2      f16 -> f16, f32, e4m3, e5m2      bf16 -> bf16, f32, e4m3, e5m2
+ *   e4m3 / e5m2 -> e4m3, e5m2, f16, bf16   (FP8 -> f32 is refused with InvalidArgument)
+ * Every input element is widened to fp32 and summed in rank order, multiplied by scale (avg: times the fp32 value 1/nranks) and rounded
+ * ONCE to the output type, so every rank holds bit-identical results. Rounding to FP8 is round-to-nearest-even with saturation to the
+ * finite range: +-inf becomes +-max, NaN stays NaN. The same scale and cast apply to all-gather, broadcast and all-to-all(v): e4m3 in,
+ * bf16 out, scale = inverse quantisation scale is a dequantising all-gather. The NVLS switch of an H100 cannot reduce FP8 (sm_90a has
+ * no FP8 multimem.ld_reduce), so FP8 reductions run on the P2P algorithms; FP8 data movement may still use multimem.st. */
+
+/* sum and avg of fp16 / bf16 / fp32 / e4m3 / e5m2 run on the fused fast paths (Lamport, two-shot, NVLS for the 16- and 32-bit types);
+ * prod, min, max — and every operator on the integer types and fp64 — run on one barrier-based P2P kernel that accumulates in the
+ * element type (fp16 / bf16 / FP8 in fp32). */
 typedef enum { b200collSum = 0, b200collAvg = 1, b200collProd = 2, b200collMin = 3, b200collMax = 4 } b200collRedOp_t;
 
 typedef enum {

@@ -18,8 +18,12 @@ namespace b200coll {
 template <typename T> struct Tag { using type = T; };
 using bf16 = __nv_bfloat16;
 using f8 = __nv_fp8_e4m3;
+using e5m2 = __nv_fp8_e5m2;
 
-// Supported (in, out) pairs: same type, widen to f32, narrow f32 to 16-bit, quantise to e4m3.
+static bool is_fp8(b200collDataType_t t) { return t == b200collFloat8e4m3 || t == b200collFloat8e5m2; }
+
+// Supported (in, out) pairs: same type, widen to f32, narrow f32 to 16-bit, quantise to e4m3 / e5m2; FP8 in, FP8 or 16-bit out
+// (FP8 -> f32 would need a 64-byte store per input vector and is refused).
 template <typename F>
 static b200collResult_t dispatch_types(b200collDataType_t in, b200collDataType_t out, F&& f) {
   if (in == b200collFloat32) {
@@ -28,6 +32,7 @@ static b200collResult_t dispatch_types(b200collDataType_t in, b200collDataType_t
       case b200collBfloat16: return f(Tag<float>{}, Tag<bf16>{});
       case b200collFloat16: return f(Tag<float>{}, Tag<__half>{});
       case b200collFloat8e4m3: return f(Tag<float>{}, Tag<f8>{});
+      case b200collFloat8e5m2: return f(Tag<float>{}, Tag<e5m2>{});
       default: break;
     }
   } else if (in == b200collBfloat16) {
@@ -35,6 +40,7 @@ static b200collResult_t dispatch_types(b200collDataType_t in, b200collDataType_t
       case b200collBfloat16: return f(Tag<bf16>{}, Tag<bf16>{});
       case b200collFloat32: return f(Tag<bf16>{}, Tag<float>{});
       case b200collFloat8e4m3: return f(Tag<bf16>{}, Tag<f8>{});
+      case b200collFloat8e5m2: return f(Tag<bf16>{}, Tag<e5m2>{});
       default: break;
     }
   } else if (in == b200collFloat16) {
@@ -42,6 +48,23 @@ static b200collResult_t dispatch_types(b200collDataType_t in, b200collDataType_t
       case b200collFloat16: return f(Tag<__half>{}, Tag<__half>{});
       case b200collFloat32: return f(Tag<__half>{}, Tag<float>{});
       case b200collFloat8e4m3: return f(Tag<__half>{}, Tag<f8>{});
+      case b200collFloat8e5m2: return f(Tag<__half>{}, Tag<e5m2>{});
+      default: break;
+    }
+  } else if (in == b200collFloat8e4m3) {
+    switch (out) {
+      case b200collFloat8e4m3: return f(Tag<f8>{}, Tag<f8>{});
+      case b200collFloat8e5m2: return f(Tag<f8>{}, Tag<e5m2>{});
+      case b200collBfloat16: return f(Tag<f8>{}, Tag<bf16>{});
+      case b200collFloat16: return f(Tag<f8>{}, Tag<__half>{});
+      default: break;
+    }
+  } else if (in == b200collFloat8e5m2) {
+    switch (out) {
+      case b200collFloat8e5m2: return f(Tag<e5m2>{}, Tag<e5m2>{});
+      case b200collFloat8e4m3: return f(Tag<e5m2>{}, Tag<f8>{});
+      case b200collBfloat16: return f(Tag<e5m2>{}, Tag<bf16>{});
+      case b200collFloat16: return f(Tag<e5m2>{}, Tag<__half>{});
       default: break;
     }
   }
@@ -128,7 +151,8 @@ static size_t out_align(size_t in_sz, size_t out_sz) { return std::min<size_t>(1
 
 static b200collResult_t check_common(b200collComm* c, const void* send, void* recv, const b200collEpilogue* ep) {
   if (!c || !send || !recv || !ep) { set_last_error("null argument"); return b200collInvalidArgument; }
-  if ((int)ep->in_dtype < 0 || (int)ep->in_dtype >= (int)b200collFloat8e4m3 || (int)ep->out_dtype < 0 || (int)ep->out_dtype > (int)b200collFloat8e4m3) { set_last_error("bad dtype (fp32 / fp16 / bf16 in, those or e4m3 out; integer and fp64 payloads: reductions take the generic path, data movement takes them as words)"); return b200collInvalidArgument; }
+  auto fused = [](b200collDataType_t t) { return ((int)t >= 0 && (int)t <= (int)b200collFloat8e4m3) || t == b200collFloat8e5m2; };
+  if (!fused(ep->in_dtype) || !fused(ep->out_dtype)) { set_last_error("bad dtype (fp32 / fp16 / bf16 / e4m3 / e5m2; integer and fp64 payloads: reductions take the generic path, data movement takes them as words)"); return b200collInvalidArgument; }
   const size_t is = b200collTypeSize(ep->in_dtype), os = b200collTypeSize(ep->out_dtype);
   if (!aligned(send, 16) || !aligned(recv, out_align(is, os))) { set_last_error("send must be 16-byte aligned and recv aligned to one output vector"); return b200collInvalidArgument; }
   if (c->fault_host && *const_cast<volatile uint32_t*>(&c->fault_host->code) != 0) { set_last_error("communicator is poisoned by an earlier watchdog fault"); return b200collRemoteError; }
@@ -282,7 +306,11 @@ static b200collResult_t launch_ll2(b200collComm* c, const void* send, void* recv
   if (i == b200collFloat32 && o == b200collFloat32) return launch_ll2_typed<float, float>(c, send, recv, count, scale, st);
   if (i == b200collBfloat16 && o == b200collBfloat16) return launch_ll2_typed<bf16, bf16>(c, send, recv, count, scale, st);
   if (i == b200collFloat16 && o == b200collFloat16) return launch_ll2_typed<__half, __half>(c, send, recv, count, scale, st);
-  set_last_error("two-shot LL needs in_dtype == out_dtype");
+  if (i == b200collFloat8e4m3 && o == b200collFloat8e4m3) return launch_ll2_typed<f8, f8>(c, send, recv, count, scale, st);
+  if (i == b200collFloat8e4m3 && o == b200collFloat8e5m2) return launch_ll2_typed<f8, e5m2>(c, send, recv, count, scale, st);
+  if (i == b200collFloat8e5m2 && o == b200collFloat8e5m2) return launch_ll2_typed<e5m2, e5m2>(c, send, recv, count, scale, st);
+  if (i == b200collFloat8e5m2 && o == b200collFloat8e4m3) return launch_ll2_typed<e5m2, f8>(c, send, recv, count, scale, st);
+  set_last_error("two-shot LL needs in_dtype == out_dtype (or two FP8 types)");
   return b200collInvalidArgument;
 }
 
@@ -300,6 +328,9 @@ static b200collResult_t ar_symmetric(b200collComm* c, b200collAlgo_t algo, const
     } else if (algo == b200collAlgoTwoShot) {
       Grid g = pick_grid(c, kShapeP2p, nvec / c->nranks + 1, 2);
       launch_k(k_ar_twoshot<InT, OutT>, g.blocks, g.threads, st, c->dev, in_off, arena_off(c, recv), count, scale, b200collOpAllReduce);
+    } else if constexpr (kIsFp8<InT>) {
+      set_last_error("internal: NVLS all-reduce requested for an FP8 input");     // b200collAllReduce never picks it
+      return b200collInternalError;
     } else {
       static const int forced_u = [] { const char* e = getenv("B200COLL_NVLS_UNROLL"); return e ? atoi(e) : 0; }();
       const size_t slice = nvec / c->nranks + 1;
@@ -484,13 +515,14 @@ b200collResult_t b200collAllReduce(const void* send, void* recv, size_t count, c
   if (c->nranks == 1) { account(c, b200collOpAllReduce, bytes, b200collAlgoCopy); return copy_scale(c, send, recv, count, ep, scale, st); }
   const bool sym_in = b200collIsSymmetric(c, send, bytes), sym_out = b200collIsSymmetric(c, recv, count * os);
   b200collAlgo_t algo = c->forced_algo != b200collAlgoAuto ? c->forced_algo : b200collTunerPick(b200collOpAllReduce, bytes, c->nranks, c->nvls);
+  const bool fp8_in = is_fp8(ep->in_dtype);
   auto feasible = [&](b200collAlgo_t a) {
     switch (a) {
       case b200collAlgoLL: return bytes <= kLLOneShotMaxBytes;
       case b200collAlgoLL2: return is == os && bytes <= kLLOneShotMaxBytes * (size_t)c->nranks;
       case b200collAlgoOneShot: return sym_in && !inplace;
       case b200collAlgoTwoShot: return sym_in && sym_out;
-      case b200collAlgoNvls: return c->nvls && sym_in && sym_out;
+      case b200collAlgoNvls: return c->nvls && sym_in && sym_out && !fp8_in;      // no FP8 multimem.ld_reduce on sm_90a
       default: return false;
     }
   };
@@ -509,7 +541,7 @@ b200collResult_t b200collAllReduce(const void* send, void* recv, size_t count, c
   }
   // ---- staged: buffers outside the arena and too big for LL. Chunk through the two staging halves.
   c->stats.staged_calls++;
-  b200collAlgo_t inner = (c->nvls && c->nranks > 2) ? b200collAlgoNvls : b200collAlgoTwoShot;
+  b200collAlgo_t inner = (c->nvls && c->nranks > 2 && !fp8_in) ? b200collAlgoNvls : b200collAlgoTwoShot;
   const size_t chunk = std::min(kStageHalfBytes / is, kStageHalfBytes / os) / 64 * 64;
   for (size_t done = 0; done < count; done += chunk) {
     const size_t n = std::min(chunk, count - done);
@@ -597,15 +629,17 @@ b200collResult_t b200collReduceScatter(const void* send, void* recv, size_t recv
   if (algo == b200collAlgoOneShot) algo = b200collAlgoTwoShot;
   if (algo == b200collAlgoLL2) algo = b200collAlgoLL;
   if (algo == b200collAlgoLL && bytes > kLLOneShotMaxBytes) algo = b200collAlgoTwoShot;
-  if (algo == b200collAlgoNvls && !c->nvls) algo = b200collAlgoTwoShot;
+  if (algo == b200collAlgoNvls && (!c->nvls || is_fp8(ep->in_dtype))) algo = b200collAlgoTwoShot;     // no FP8 multimem.ld_reduce on sm_90a
   if (algo == b200collAlgoLL) { account(c, b200collOpReduceScatter, bytes, algo); return launch_ll(c, b200collOpReduceScatter, send, recv, recvcount, ep, scale, st); }
   auto pull = [&](const void* s_slice_of_mine, void* r, size_t n) -> b200collResult_t {
     account(c, b200collOpReduceScatter, n * is, algo);
     return dispatch_types(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
       using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
       Grid g = pick_grid(c, algo == b200collAlgoNvls ? kShapeNvlsRs : kShapeP2p, n / Epv<InT>::value, 2);
-      if (algo == b200collAlgoNvls) launch_k(k_pull_reduce<InT, OutT, false, true>, g.blocks, g.threads, st, c->dev, arena_off(c, s_slice_of_mine), static_cast<OutT*>(r), n, scale, b200collOpReduceScatter);
-      else launch_k(k_pull_reduce<InT, OutT, false, false>, g.blocks, g.threads, st, c->dev, arena_off(c, s_slice_of_mine), static_cast<OutT*>(r), n, scale, b200collOpReduceScatter);
+      if constexpr (!kIsFp8<InT>) {
+        if (algo == b200collAlgoNvls) launch_k(k_pull_reduce<InT, OutT, false, true>, g.blocks, g.threads, st, c->dev, arena_off(c, s_slice_of_mine), static_cast<OutT*>(r), n, scale, b200collOpReduceScatter);
+        else launch_k(k_pull_reduce<InT, OutT, false, false>, g.blocks, g.threads, st, c->dev, arena_off(c, s_slice_of_mine), static_cast<OutT*>(r), n, scale, b200collOpReduceScatter);
+      } else launch_k(k_pull_reduce<InT, OutT, false, false>, g.blocks, g.threads, st, c->dev, arena_off(c, s_slice_of_mine), static_cast<OutT*>(r), n, scale, b200collOpReduceScatter);
       LAUNCH_CHECK(c);
       return b200collSuccess;
     });
@@ -806,14 +840,16 @@ b200collResult_t b200collReduce(const void* send, void* recv, size_t count, cons
   if (c->nranks == 1) { account(c, b200collOpReduce, count * is, b200collAlgoCopy); return copy_scale(c, send, recv, count, ep, scale, st); }
   if (send == recv && is != os) { set_last_error("in-place reduce needs in_dtype and out_dtype of equal size"); return b200collInvalidArgument; }
   b200collAlgo_t algo = c->forced_algo != b200collAlgoAuto ? c->forced_algo : b200collTunerPick(b200collOpReduce, count * is, c->nranks, c->nvls);
-  if (algo != b200collAlgoNvls || !c->nvls) algo = b200collAlgoTwoShot;     // multimem.ld_reduce by the root, or the root pulls from every peer
+  if (algo != b200collAlgoNvls || !c->nvls || is_fp8(ep->in_dtype)) algo = b200collAlgoTwoShot;     // multimem.ld_reduce by the root (not for FP8), or the root pulls from every peer
   auto pull = [&](const void* s_sym, void* r, size_t n) -> b200collResult_t {
     account(c, b200collOpReduce, n * is, algo);
     return dispatch_types(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
       using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
       Grid g = pick_grid(c, algo == b200collAlgoNvls ? kShapeRooted : kShapeP2p, std::max<size_t>(1, n / Epv<InT>::value), algo == b200collAlgoNvls ? 4 : 2);
-      if (algo == b200collAlgoNvls) launch_k(k_reduce_root<InT, OutT, true>, g.blocks, g.threads, st, c->dev, arena_off(c, s_sym), static_cast<OutT*>(r), n, scale, root, b200collOpReduce);
-      else launch_k(k_reduce_root<InT, OutT, false>, g.blocks, g.threads, st, c->dev, arena_off(c, s_sym), static_cast<OutT*>(r), n, scale, root, b200collOpReduce);
+      if constexpr (!kIsFp8<InT>) {
+        if (algo == b200collAlgoNvls) launch_k(k_reduce_root<InT, OutT, true>, g.blocks, g.threads, st, c->dev, arena_off(c, s_sym), static_cast<OutT*>(r), n, scale, root, b200collOpReduce);
+        else launch_k(k_reduce_root<InT, OutT, false>, g.blocks, g.threads, st, c->dev, arena_off(c, s_sym), static_cast<OutT*>(r), n, scale, root, b200collOpReduce);
+      } else launch_k(k_reduce_root<InT, OutT, false>, g.blocks, g.threads, st, c->dev, arena_off(c, s_sym), static_cast<OutT*>(r), n, scale, root, b200collOpReduce);
       LAUNCH_CHECK(c);
       return b200collSuccess;
     });

@@ -3,7 +3,7 @@
 //   * epoch barrier over per-block flags in each rank's control page (monotonic, never reset)
 //   * Lamport (flag-in-payload) slot protocol for the zero-barrier small-message path
 //   * multimem.{ld_reduce,st} wrappers (NVLS: reduce / broadcast inside the NVSwitch)
-//   * 16-byte vector load/convert/store for {f32,f16,bf16} in and {f32,f16,bf16,e4m3} out
+//   * 16-byte vector load/convert/store for {f32,f16,bf16,e4m3,e5m2} in and out
 // Every cross-GPU spin carries a globaltimer watchdog that records a b200collFault and bails
 // out instead of hanging the GPU (SURVEY §5.3).
 #pragma once
@@ -155,6 +155,11 @@ __device__ __forceinline__ void mc_st_words(void* a, const uint32_t* w, int nwor
 
 // ---------------------------------------------------------------- type handling
 template <typename T> struct Epv { static constexpr int value = 16 / (int)sizeof(T); };
+// FP8 inputs: sm_90a has no FP8 multimem.ld_reduce, so the NVLS reduction kernels are never instantiated for them, and they are
+// summed in rank order on every P2P kernel (an e5m2 sum in fp32 is not exact, so the order is part of the result).
+template <typename T> constexpr bool kIsFp8 = false;
+template <> constexpr bool kIsFp8<__nv_fp8_e4m3> = true;
+template <> constexpr bool kIsFp8<__nv_fp8_e5m2> = true;
 
 template <typename InT> __device__ __forceinline__ void unpack_add(float* acc, const uint4& v);
 template <> __device__ __forceinline__ void unpack_add<float>(float* acc, const uint4& v) {
@@ -174,6 +179,22 @@ template <> __device__ __forceinline__ void unpack_add<__half>(float* acc, const
     acc[2 * i] += f.x; acc[2 * i + 1] += f.y;
   }
 }
+// FP8: the hardware fp8x2 -> f16x2 unpack (F2FP.F16.E4M3.UNPACK_B / .E5M2.UNPACK_B), then f16x2 -> f32. Every e4m3 and e5m2 value is
+// exact in fp16, so the widening is exact.
+template <__nv_fp8_interpretation_t I> __device__ __forceinline__ void unpack_add_fp8(float* acc, const uint4& v) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const __half2_raw r = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w[i] >> (16 * h)), I);
+      const float2 f = __half22float2(__half2(r));
+      acc[4 * i + 2 * h] += f.x; acc[4 * i + 2 * h + 1] += f.y;
+    }
+  }
+}
+template <> __device__ __forceinline__ void unpack_add<__nv_fp8_e4m3>(float* acc, const uint4& v) { unpack_add_fp8<__NV_E4M3>(acc, v); }
+template <> __device__ __forceinline__ void unpack_add<__nv_fp8_e5m2>(float* acc, const uint4& v) { unpack_add_fp8<__NV_E5M2>(acc, v); }
 
 // pack E floats into E*sizeof(OutT)/4 words
 template <typename OutT, int E> struct Pack;
@@ -209,6 +230,17 @@ template <int E> struct Pack<__nv_fp8_e4m3, E> {
     }
   }
 };
+template <int E> struct Pack<__nv_fp8_e5m2, E> {
+  static constexpr int W = E / 4;
+  static __device__ __forceinline__ void run(const float* f, uint32_t* w) {
+#pragma unroll
+    for (int i = 0; i < E / 4; i++) {
+      uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(f[4 * i], f[4 * i + 1]), __NV_SATFINITE, __NV_E5M2);
+      uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(f[4 * i + 2], f[4 * i + 3]), __NV_SATFINITE, __NV_E5M2);
+      w[i] = lo | (hi << 16);
+    }
+  }
+};
 
 template <int W> __device__ __forceinline__ void st_words(void* p, const uint32_t* w) {
   if (W == 8) {
@@ -231,10 +263,13 @@ template <typename T> __device__ __forceinline__ float to_float(T v);
 template <> __device__ __forceinline__ float to_float<float>(float v) { return v; }
 template <> __device__ __forceinline__ float to_float<__half>(__half v) { return __half2float(v); }
 template <> __device__ __forceinline__ float to_float<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <> __device__ __forceinline__ float to_float<__nv_fp8_e4m3>(__nv_fp8_e4m3 v) { return __half2float(__half(__nv_cvt_fp8_to_halfraw(v.__x, __NV_E4M3))); }
+template <> __device__ __forceinline__ float to_float<__nv_fp8_e5m2>(__nv_fp8_e5m2 v) { return __half2float(__half(__nv_cvt_fp8_to_halfraw(v.__x, __NV_E5M2))); }
 template <typename T> __device__ __forceinline__ T from_float(float v);
 template <> __device__ __forceinline__ float from_float<float>(float v) { return v; }
 template <> __device__ __forceinline__ __half from_float<__half>(float v) { return __float2half_rn(v); }
 template <> __device__ __forceinline__ __nv_bfloat16 from_float<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
-template <> __device__ __forceinline__ __nv_fp8_e4m3 from_float<__nv_fp8_e4m3>(float v) { return __nv_fp8_e4m3(v); }
+template <> __device__ __forceinline__ __nv_fp8_e4m3 from_float<__nv_fp8_e4m3>(float v) { return __nv_fp8_e4m3(v); }   // satfinite, round to nearest even
+template <> __device__ __forceinline__ __nv_fp8_e5m2 from_float<__nv_fp8_e5m2>(float v) { return __nv_fp8_e5m2(v); }
 
 }  // namespace b200coll

@@ -180,9 +180,11 @@ __global__ void __launch_bounds__(kThreads) k_ll(COMM_PARAM, const InT* __restri
   }
   __syncthreads();
   if (threadIdx.x == 0 && last_block_ticket(c)) {
-    c.state[kLLUsedLo0 + buf] = (uint32_t)nv;
-    c.state[kLLUsedHi0 + buf] = 0;
-    c.state[kSeqLL] = k + 1;
+    // FP8 (16 accumulators per vector): read the sequence number again instead of keeping it live across the loop, where it spilled
+    const uint32_t kk = (kIsFp8<InT> || kIsFp8<OutT>) ? load_seq(c, kSeqLL) : k;
+    c.state[kLLUsedLo0 + kk % 3] = (uint32_t)nv;
+    c.state[kLLUsedHi0 + kk % 3] = 0;
+    c.state[kSeqLL] = kk + 1;
   }
 }
 
@@ -294,7 +296,7 @@ __device__ __forceinline__ void ar_tail_rank0(const CommDev& c, size_t in_off, s
 }
 
 // out_local[i] = scale * sum_r peer_r[in_off + i]   (one-shot all-reduce; reduce-scatter with in_off pointing at my slice)
-// FIXED_ORDER: sum in rank order so every rank computes bit-identical results (one-shot AR).
+// FIXED_ORDER: sum in rank order so every rank computes bit-identical results (one-shot AR). FP8 inputs always sum in rank order.
 template <typename InT, typename OutT, bool FIXED_ORDER, bool MC>
 __global__ void __launch_bounds__(kThreads) k_pull_reduce(COMM_PARAM, size_t in_off, OutT* __restrict__ out, size_t count, float scale, uint32_t op) {
   pdl_prologue();
@@ -323,7 +325,7 @@ __global__ void __launch_bounds__(kThreads) k_pull_reduce(COMM_PARAM, size_t in_
 #pragma unroll
           for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
             int r = j;
-            if (!FIXED_ORDER) { r = c.rank + j; if (r >= c.nranks) r -= c.nranks; }
+            if (!FIXED_ORDER && !kIsFp8<InT>) { r = c.rank + j; if (r >= c.nranks) r -= c.nranks; }
             d[u][j] = ld_vec(c.peer[r] + in_off + v * 16);
           }
         }
@@ -355,7 +357,8 @@ __global__ void __launch_bounds__(kThreads) k_pull_reduce(COMM_PARAM, size_t in_
 // ------------------------------------------------------------------------------------------------
 // Two-shot fused into one pass: rank r owns vector slice r; pulls it from every peer, reduces in fp32,
 // applies scale/cast and pushes the finished vector into every peer's out. Bytes per GPU and direction:
-// S(N-1)/N pulled + S(N-1)/N pushed -> bus bandwidth bound = link bandwidth.
+// S(N-1)/N pulled + S(N-1)/N pushed -> bus bandwidth bound = link bandwidth. Peers are visited starting after my own rank (spreads
+// the pulls over the links); FP8 inputs are pulled and summed in rank order instead, the order the FP8 semantics promise.
 template <typename InT, typename OutT>
 __global__ void __launch_bounds__(kThreads) k_ar_twoshot(COMM_PARAM, size_t in_off, size_t out_off, size_t count, float scale, uint32_t op) {
   pdl_prologue();
@@ -375,7 +378,8 @@ __global__ void __launch_bounds__(kThreads) k_ar_twoshot(COMM_PARAM, size_t in_o
       if (v < v1) {
 #pragma unroll
         for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
-          int r = c.rank + j; if (r >= c.nranks) r -= c.nranks;
+          int r = j;
+          if (!kIsFp8<InT>) { r = c.rank + j; if (r >= c.nranks) r -= c.nranks; }
           d[u][j] = ld_vec(c.peer[r] + in_off + v * 16);
         }
       }

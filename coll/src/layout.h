@@ -21,8 +21,9 @@ constexpr size_t kLLBytes = 3 * (size_t)kMaxRanks * kLLMaxBytes;
 constexpr size_t kOffStage = kOffLL + kLLBytes;         // staging for buffers outside the arena (2 halves)
 constexpr size_t kStageHalfBytes = 32u << 20;
 constexpr size_t kOffHeap = kOffStage + 2 * kStageHalfBytes;   // user heap starts here (77 MiB)
-constexpr uint32_t kLLSentinel = 0xFFFFFFFFu;           // a NaN pattern in f32/f16x2/bf16x2; payload words equal to it are rewritten
-constexpr uint32_t kLLSanitized = 0x7FFF7FFFu;          // still NaN in every supported type
+constexpr uint32_t kLLSentinel = 0xFFFFFFFFu;           // a NaN pattern in f32/f16x2/bf16x2 (four NaNs in e4m3x4 and e5m2x4); payload words equal to it are rewritten
+constexpr uint32_t kLLSanitized = 0x7FFF7FFFu;          // still NaN in every supported type (e4m3 / e5m2: 0x7F and 0xFF bytes are NaN), so
+                                                        // bit-exact movement of arbitrary bytes uses the barrier-based kernels instead
 
 // Point-to-point mailboxes, in the zero-initialised part of the first megabyte that the flag matrix does not use.
 //   post: u64 [receiver rank][CTA][2 slots][2 words], written by the RECEIVER into the SENDER's arena ("write n bytes at this offset of mine")

@@ -5,6 +5,7 @@
 // User buffers are ordinary cudaMalloc memory here, so calls take the Lamport path (<= 512 KiB) or the staged path;
 // ncclMemAlloc hands out symmetric-arena memory once a communicator exists (zero-copy + NVLS).
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -20,7 +21,7 @@ extern "C" {
 typedef struct ncclComm* ncclComm_t;
 typedef struct { char internal[128]; } ncclUniqueId;
 typedef enum { ncclSuccess = 0, ncclUnhandledCudaError = 1, ncclSystemError = 2, ncclInternalError = 3, ncclInvalidArgument = 4, ncclInvalidUsage = 5, ncclRemoteError = 6, ncclInProgress = 7 } ncclResult_t;
-typedef enum { ncclInt8 = 0, ncclUint8 = 1, ncclInt32 = 2, ncclUint32 = 3, ncclInt64 = 4, ncclUint64 = 5, ncclFloat16 = 6, ncclFloat32 = 7, ncclFloat64 = 8, ncclBfloat16 = 9 } ncclDataType_t;
+typedef enum { ncclInt8 = 0, ncclUint8 = 1, ncclInt32 = 2, ncclUint32 = 3, ncclInt64 = 4, ncclUint64 = 5, ncclFloat16 = 6, ncclFloat32 = 7, ncclFloat64 = 8, ncclBfloat16 = 9, ncclFloat8e4m3 = 10, ncclFloat8e5m2 = 11 } ncclDataType_t;
 typedef enum { ncclSum = 0, ncclProd = 1, ncclMax = 2, ncclMin = 3, ncclAvg = 4 } ncclRedOp_t;
 typedef enum { ncclScalarDevice = 0, ncclScalarHostImmediate = 1 } ncclScalarResidence_t;
 typedef struct ncclWindow_vidmem* ncclWindow_t;
@@ -59,9 +60,12 @@ bool map_dt(ncclDataType_t dt, b200collDataType_t* out) {
   }
 }
 
-// Every NCCL element type that libb200coll can reduce (fp8 is a wire / output format only, as in NCCL before 2.24).
+// Every NCCL element type that libb200coll can reduce. FP8 (as in NCCL 2.24 and later) reduces in fp32 with one satfinite rounding;
+// it is deliberately not in map_dt, so FP8 data movement stays on the bit-exact word path (the Lamport path would rewrite NaN bytes).
 bool map_dt_reduce(ncclDataType_t dt, b200collDataType_t* out) {
   switch (dt) {
+    case ncclFloat8e4m3: *out = b200collFloat8e4m3; return true;
+    case ncclFloat8e5m2: *out = b200collFloat8e5m2; return true;
     case ncclInt8: *out = b200collInt8; return true;
     case ncclUint8: *out = b200collUint8; return true;
     case ncclInt32: *out = b200collInt32; return true;
@@ -93,7 +97,7 @@ bool map_op(ncclRedOp_t op, b200collRedOp_t* rop, float* scale) {
 
 size_t nccl_type_size(ncclDataType_t dt) {
   switch ((int)dt) {
-    case ncclInt8: case ncclUint8: case 10 /* ncclFloat8e4m3 */: case 11 /* ncclFloat8e5m2 */: return 1;
+    case ncclInt8: case ncclUint8: case ncclFloat8e4m3: case ncclFloat8e5m2: return 1;
     case ncclFloat16: case ncclBfloat16: return 2;
     case ncclInt32: case ncclUint32: case ncclFloat32: return 4;
     case ncclInt64: case ncclUint64: case ncclFloat64: return 8;
@@ -217,13 +221,15 @@ ncclResult_t ncclCommDeregister(const ncclComm_t, void*) { return ncclSuccess; }
 ncclResult_t ncclRedOpCreatePreMulSum(ncclRedOp_t* op, void* scalar, ncclDataType_t dt, ncclScalarResidence_t residence, ncclComm_t comm) {
   if (!op || !scalar || !comm) return ncclInvalidArgument;
   unsigned char raw[8] = {};
-  const size_t sz = dt == ncclFloat64 ? 8 : dt == ncclFloat32 ? 4 : (dt == ncclFloat16 || dt == ncclBfloat16) ? 2 : 0;
+  const size_t sz = dt == ncclFloat64 ? 8 : dt == ncclFloat32 ? 4 : (dt == ncclFloat16 || dt == ncclBfloat16) ? 2 : (dt == ncclFloat8e4m3 || dt == ncclFloat8e5m2) ? 1 : 0;
   if (!sz) return ncclInvalidArgument;
   if (residence == ncclScalarHostImmediate) memcpy(raw, scalar, sz);
   else if (cudaMemcpy(raw, scalar, sz, cudaMemcpyDeviceToHost) != cudaSuccess) return ncclUnhandledCudaError;
   float v;
   if (dt == ncclFloat64) { double d; memcpy(&d, raw, 8); v = (float)d; }
   else if (dt == ncclFloat32) memcpy(&v, raw, 4);
+  else if (dt == ncclFloat8e4m3) v = __half2float(__half(__nv_cvt_fp8_to_halfraw(raw[0], __NV_E4M3)));
+  else if (dt == ncclFloat8e5m2) v = __half2float(__half(__nv_cvt_fp8_to_halfraw(raw[0], __NV_E5M2)));
   else { unsigned short h; memcpy(&h, raw, 2); if (dt == ncclBfloat16) { unsigned int w = (unsigned int)h << 16; memcpy(&v, &w, 4); } else { __half hh; memcpy(&hh, &h, 2); v = __half2float(hh); } }
   std::lock_guard<std::mutex> lk(g_mu);
   size_t slot = 0;
@@ -302,7 +308,7 @@ ncclResult_t ncclReduceScatter(const void* send, void* recv, size_t recvcount, n
 // (scale 1, same type in and out = the bit-exact identity path).
 static bool map_dt_as_words(ncclDataType_t dt, size_t count, b200collDataType_t* t, size_t* n) {
   switch (dt) {
-    case ncclInt8: case ncclUint8: if (count % 2) return false; *t = b200collFloat16; *n = count / 2; return true;
+    case ncclInt8: case ncclUint8: case ncclFloat8e4m3: case ncclFloat8e5m2: if (count % 2) return false; *t = b200collFloat16; *n = count / 2; return true;
     case ncclFloat16: case ncclBfloat16: *t = b200collFloat16; *n = count; return true;
     case ncclInt32: case ncclUint32: case ncclFloat32: *t = b200collFloat32; *n = count; return true;
     case ncclInt64: case ncclUint64: case ncclFloat64: *t = b200collFloat32; *n = count * 2; return true;
