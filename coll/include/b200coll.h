@@ -211,6 +211,41 @@ b200collResult_t b200collReduce(const void* send, void* recv, size_t count, cons
                                 b200collRedOp_t op, int root, b200collComm_t comm, b200collStream_t stream);
 b200collResult_t b200collBarrier(b200collComm_t comm, b200collStream_t stream);
 
+/* --- block-scaled FP8 (src/blockscaled.cu): per-block dequantisation fused into all-gather, reduce-scatter and all-reduce.
+ * Each rank's send buffer is a row-major matrix [rows, row_len] of e4m3 or e5m2 (rows = count / row_len) with one fp32 scale per
+ * block_rows x block_cols block of THAT rank's matrix: ceil(rows / block_rows) x ceil(row_len / block_cols) scales, row-major, the last
+ * block row and column may be partial. Element (i, j) of rank r has the value v = float(q) * s[i / block_rows][j / block_cols] (one fp32
+ * multiply, round to nearest even).
+ *   all-reduce, reduce-scatter:  out = round_once(((0 + v_0) + v_1 + ... + v_{N-1}) * scale), summed in fp32 in rank order; avg multiplies
+ *                                scale by the fp32 value 1/N; other operators are refused (InvalidArgument)
+ *   all-gather:                  out[shard r] = round_once((0 + v_r) * scale)   (so -0 comes out as +0)
+ * ep->in_dtype is e4m3 or e5m2, ep->out_dtype bf16, fp16 or fp32 (FP8 -> fp32 is allowed here), ep->scale the global multiplier.
+ * Rounding is RNE; NaN and inf in q or in a scale propagate as the fp32 arithmetic produces them.
+ * Constraints (InvalidArgument unless noted, message in b200collGetLastError): row_len % 16 == 0; block_cols % 16 == 0 and block_rows >= 1
+ * (so each 16-byte FP8 vector lies in one block); count % row_len == 0; reduce-scatter: rows % nranks == 0 (every slice is whole rows);
+ * send and scales in the symmetric arena at the same offsets on every rank, else InvalidUsage (there is no staging path); recv any
+ * 16-byte aligned device buffer that does not overlap send.
+ * FP8 crosses NVLink (receivers pull FP8 and scales and dequantise in registers). All-gather and reduce-scatter count as oneshot in
+ * b200collStats; all-reduce maps the tuner's pick (or the forced algorithm): ll / ll2 / oneshot -> oneshot (pull the whole matrix),
+ * twoshot / nvls -> twoshot (pull my slice, push the result into every recv), and twoshot falls back to oneshot when recv is outside the
+ * arena. Each rank makes that choice from its own recv, so all-reduce recv must be placed alike on every rank: in the arena at the same
+ * offset everywhere, or outside it everywhere (ranks that disagree run different kernels and end in a watchdog fault; B200COLL_CHECK=1
+ * turns the disagreement into InvalidUsage before the launch on multi-process communicators). One rank: a local dequantising copy, counted as copy.
+ * bytes = FP8 input bytes (per rank; reduce-scatter: recvcount). At most 2^35 - 16 elements per rank. */
+typedef struct {
+  const float* scales;   /* ceil(rows/block_rows) x ceil(row_len/block_cols) fp32, row-major, in the symmetric arena */
+  size_t row_len;        /* elements per row of the send matrix */
+  int block_rows, block_cols;
+} b200collBlockScale;
+/* recv holds nranks*sendcount elements of out_dtype; shard r is rank r's matrix dequantised with rank r's scales. */
+b200collResult_t b200collAllGatherBlockScaled(const void* send, void* recv, size_t sendcount, const b200collBlockScale* bs,
+                                              const b200collEpilogue* ep, b200collComm_t comm, b200collStream_t stream);
+/* send holds nranks*recvcount elements (rows whole rows); rank r receives the reduction of row slice r. */
+b200collResult_t b200collReduceScatterBlockScaled(const void* send, void* recv, size_t recvcount, const b200collBlockScale* bs,
+                                                  const b200collEpilogue* ep, b200collRedOp_t op, b200collComm_t comm, b200collStream_t stream);
+b200collResult_t b200collAllReduceBlockScaled(const void* send, void* recv, size_t count, const b200collBlockScale* bs,
+                                              const b200collEpilogue* ep, b200collRedOp_t op, b200collComm_t comm, b200collStream_t stream);
+
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.
  * AllReduceHost is the end-to-end step "pinned host -> GPU -> all-reduce -> pinned host" as one asynchronous call on `stream`:

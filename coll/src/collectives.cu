@@ -12,6 +12,7 @@
 
 #include "comm.h"
 #include "kernels.cuh"
+#include "launch.cuh"
 
 namespace b200coll {
 
@@ -72,81 +73,8 @@ static b200collResult_t dispatch_types(b200collDataType_t in, b200collDataType_t
   return b200collInvalidArgument;
 }
 
-#define LAUNCH_CHECK(c)                                                                                  \
-  do {                                                                                                   \
-    cudaError_t e__ = cudaGetLastError();                                                                \
-    if (e__ != cudaSuccess) { set_last_error(std::string("kernel launch failed: ") + cudaGetErrorString(e__)); return b200collUnhandledCudaError; } \
-    (c)->stats.kernel_launches++;                                                                        \
-  } while (0)
-
-struct Grid { int blocks, threads; };
-
-// Every kernel goes through cudaLaunchKernelEx so that back-to-back collectives can use programmatic dependent launch
-// (on by default, B200COLL_PDL=0 disables): the next kernel's launch latency overlaps the current kernel's execution; each kernel starts with
-// griddepcontrol.launch_dependents + griddepcontrol.wait, so it still observes its predecessor's completed memory.
-// Never with virtual ranks (several communicators on one GPU): a pre-launched dependent grid parks its CTAs on SMs
-// that another rank's current kernel still needs, and ranks that spin on each other then deadlock (seen at 1 MiB with
-// 4 ranks on one GPU). With one rank per GPU every CTA of kernel i is resident before kernel i+1 may start.
-// The overlap pays for tiny messages and costs time for larger ones (the early-launched grid sits on the SMs while its predecessor
-// still needs them, and its griddepcontrol.wait returns only after the predecessor's memory flush). So only launches whose message is
-// at most B200COLL_PDL_MAX_KB (default 8) carry the attribute; the cut-off has not been re-measured on multi-GPU H100 systems. launch_ll sets the flag for the launch it is about to make.
-static thread_local bool t_pdl_small = false;
-static size_t pdl_max_bytes() {
-  static const size_t v = [] { const char* e = getenv("B200COLL_PDL_MAX_KB"); return (size_t)(e && *e ? atol(e) : 8) << 10; }();
-  return v;
-}
-static bool pdl_enabled() {
-  static const bool on = [] { const char* e = getenv("B200COLL_PDL"); return !(e && *e == '0'); }();      // on unless B200COLL_PDL=0
-  return on && t_pdl_small && g_loopback_comms.load(std::memory_order_relaxed) == 0;
-}
-template <typename... KArgs, typename... Args>
-static void launch_k_smem(void (*kernel)(KArgs...), int blocks, int threads, size_t smem, cudaStream_t st, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)blocks); cfg.blockDim = dim3((unsigned)threads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr;
-  if (pdl_enabled()) {
-    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr.val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = &attr; cfg.numAttrs = 1;
-  }
-  (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-template <typename... KArgs, typename... Args>
-static void launch_k(void (*kernel)(KArgs...), int blocks, int threads, cudaStream_t st, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)blocks); cfg.blockDim = dim3((unsigned)threads); cfg.dynamicSmemBytes = 0; cfg.stream = st;
-  cudaLaunchAttribute attr;
-  if (pdl_enabled()) {
-    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr.val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = &attr; cfg.numAttrs = 1;
-  }
-  (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);   // the error is picked up by LAUNCH_CHECK's cudaGetLastError
-}
-
-// Pick the smallest block size that still covers `vecs` with <= max_ctas blocks (small work spreads over more SMs),
-// unless the family's shape pins the thread count.
-enum { kShapeNvls = 0, kShapeP2p = 1, kShapeLL = 2, kShapeNvlsRs = 3, kShapeRooted = 4 };
-static Grid pick_grid(const b200collComm* c, int kind, size_t vecs, int unroll) {
-  static const int forced = [] { const char* e = getenv("B200COLL_FORCE_THREADS"); return e ? atoi(e) : 0; }();
-  const int max_ctas = std::max(1, std::min(c->shape[kind].max_ctas > 0 ? c->shape[kind].max_ctas : c->max_ctas, c->max_ctas));
-  int pinned = c->shape[kind].threads;
-  if (forced >= 32 && forced <= 512) pinned = forced;
-  if (pinned) {
-    size_t b = (vecs + (size_t)pinned * unroll - 1) / ((size_t)pinned * unroll);
-    return Grid{(int)std::max<size_t>(1, std::min<size_t>(b, (size_t)max_ctas)), pinned};
-  }
-  for (int t : {128, 256, 512}) {
-    size_t b = (vecs + (size_t)t * unroll - 1) / ((size_t)t * unroll);
-    if (b <= (size_t)max_ctas || t == 512) return Grid{(int)std::max<size_t>(1, std::min<size_t>(b, (size_t)max_ctas)), t};
-  }
-  return Grid{1, 128};
-}
-
-static size_t arena_off(b200collComm* c, const void* p) { return reinterpret_cast<CUdeviceptr>(p) - c->peer_va[c->rank]; }
 static char* stage_ptr(b200collComm* c, int half) { return reinterpret_cast<char*>(c->peer_va[c->rank]) + kOffStage + (size_t)half * kStageHalfBytes; }
 
-static bool aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) % a) == 0; }
 static size_t out_align(size_t in_sz, size_t out_sz) { return std::min<size_t>(16, 16 / in_sz * out_sz); }
 
 static b200collResult_t check_common(b200collComm* c, const void* send, void* recv, const b200collEpilogue* ep) {
@@ -161,7 +89,7 @@ static b200collResult_t check_common(b200collComm* c, const void* send, void* re
 
 // B200COLL_NVTX=1: one NVTX mark per collective ("b200coll all_reduce nvls 67108864 B") so timelines show which algorithm
 // a call took (SURVEY §5.1: the reference only passes NCCL_DEBUG through to opaque payloads).
-static void account(b200collComm* c, b200collOp_t op, size_t bytes, b200collAlgo_t algo) {
+void account(b200collComm* c, b200collOp_t op, size_t bytes, b200collAlgo_t algo) {
   c->stats.calls[op]++; c->stats.bytes[op] += bytes; c->stats.algo_calls[algo]++;
   if ((c->stats_tick++ & 0xFF) == 0) stats_page_publish(c);      // keep the exported counters fresh without the application polling
   static const bool nvtx = [] { const char* e = getenv("B200COLL_NVTX"); return e && *e && *e != '0'; }();
@@ -179,7 +107,7 @@ static void account(b200collComm* c, b200collOp_t op, size_t bytes, b200collAlgo
 // offsets (allocation order drifted), counts or placements would read and write wrong peer addresses or run different kernels with
 // different barrier counts. B200COLL_CHECK=1 compares (op, algorithm, count, offsets) across ranks over the bootstrap channel before
 // every such launch and fails the call with InvalidUsage instead (host-synchronous, multi-process communicators only: a debugging aid).
-static b200collResult_t cross_check(b200collComm* c, b200collOp_t op, b200collAlgo_t algo, size_t count, size_t off_a, size_t off_b) {
+b200collResult_t cross_check(b200collComm* c, b200collOp_t op, b200collAlgo_t algo, size_t count, size_t off_a, size_t off_b) {
   static const bool on = [] { const char* e = getenv("B200COLL_CHECK"); return e && *e && *e != '0'; }();
   if (!on || !c->boot || c->nranks == 1) return b200collSuccess;
   struct Sig { unsigned long long op, algo, count, a, b; } mine = {(unsigned long long)op, (unsigned long long)algo, count, off_a, off_b};

@@ -1,0 +1,91 @@
+// Host-side launch helpers shared by the collective entry points (collectives.cu, blockscaled.cu): kernel launch through
+// cudaLaunchKernelEx with optional programmatic dependent launch, the launch-shape picker, and call accounting.
+#pragma once
+#include <stdlib.h>
+
+#include <algorithm>
+#include <string>
+
+#include "comm.h"
+
+namespace b200coll {
+
+#define LAUNCH_CHECK(c)                                                                                  \
+  do {                                                                                                   \
+    cudaError_t e__ = cudaGetLastError();                                                                \
+    if (e__ != cudaSuccess) { set_last_error(std::string("kernel launch failed: ") + cudaGetErrorString(e__)); return b200collUnhandledCudaError; } \
+    (c)->stats.kernel_launches++;                                                                        \
+  } while (0)
+
+struct Grid { int blocks, threads; };
+
+// Every kernel goes through cudaLaunchKernelEx so that back-to-back collectives can use programmatic dependent launch
+// (on by default, B200COLL_PDL=0 disables): the next kernel's launch latency overlaps the current kernel's execution; each kernel starts with
+// griddepcontrol.launch_dependents + griddepcontrol.wait, so it still observes its predecessor's completed memory.
+// Never with virtual ranks (several communicators on one GPU): a pre-launched dependent grid parks its CTAs on SMs
+// that another rank's current kernel still needs, and ranks that spin on each other then deadlock (seen at 1 MiB with
+// 4 ranks on one GPU). With one rank per GPU every CTA of kernel i is resident before kernel i+1 may start.
+// The overlap pays for tiny messages and costs time for larger ones (the early-launched grid sits on the SMs while its predecessor
+// still needs them, and its griddepcontrol.wait returns only after the predecessor's memory flush). So only launches whose message is
+// at most B200COLL_PDL_MAX_KB (default 8) carry the attribute; the cut-off has not been re-measured on multi-GPU H100 systems. launch_ll sets the flag for the launch it is about to make.
+inline thread_local bool t_pdl_small = false;
+inline size_t pdl_max_bytes() {
+  static const size_t v = [] { const char* e = getenv("B200COLL_PDL_MAX_KB"); return (size_t)(e && *e ? atol(e) : 8) << 10; }();
+  return v;
+}
+inline bool pdl_enabled() {
+  static const bool on = [] { const char* e = getenv("B200COLL_PDL"); return !(e && *e == '0'); }();      // on unless B200COLL_PDL=0
+  return on && t_pdl_small && g_loopback_comms.load(std::memory_order_relaxed) == 0;
+}
+template <typename... KArgs, typename... Args>
+static void launch_k_smem(void (*kernel)(KArgs...), int blocks, int threads, size_t smem, cudaStream_t st, Args&&... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)blocks); cfg.blockDim = dim3((unsigned)threads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cudaLaunchAttribute attr;
+  if (pdl_enabled()) {
+    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr.val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = &attr; cfg.numAttrs = 1;
+  }
+  (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+template <typename... KArgs, typename... Args>
+static void launch_k(void (*kernel)(KArgs...), int blocks, int threads, cudaStream_t st, Args&&... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)blocks); cfg.blockDim = dim3((unsigned)threads); cfg.dynamicSmemBytes = 0; cfg.stream = st;
+  cudaLaunchAttribute attr;
+  if (pdl_enabled()) {
+    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr.val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = &attr; cfg.numAttrs = 1;
+  }
+  (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);   // the error is picked up by LAUNCH_CHECK's cudaGetLastError
+}
+
+// Pick the smallest block size that still covers `vecs` with <= max_ctas blocks (small work spreads over more SMs),
+// unless the family's shape pins the thread count.
+enum { kShapeNvls = 0, kShapeP2p = 1, kShapeLL = 2, kShapeNvlsRs = 3, kShapeRooted = 4 };
+inline Grid pick_grid(const b200collComm* c, int kind, size_t vecs, int unroll) {
+  static const int forced = [] { const char* e = getenv("B200COLL_FORCE_THREADS"); return e ? atoi(e) : 0; }();
+  const int max_ctas = std::max(1, std::min(c->shape[kind].max_ctas > 0 ? c->shape[kind].max_ctas : c->max_ctas, c->max_ctas));
+  int pinned = c->shape[kind].threads;
+  if (forced >= 32 && forced <= 512) pinned = forced;
+  if (pinned) {
+    size_t b = (vecs + (size_t)pinned * unroll - 1) / ((size_t)pinned * unroll);
+    return Grid{(int)std::max<size_t>(1, std::min<size_t>(b, (size_t)max_ctas)), pinned};
+  }
+  for (int t : {128, 256, 512}) {
+    size_t b = (vecs + (size_t)t * unroll - 1) / ((size_t)t * unroll);
+    if (b <= (size_t)max_ctas || t == 512) return Grid{(int)std::max<size_t>(1, std::min<size_t>(b, (size_t)max_ctas)), t};
+  }
+  return Grid{1, 128};
+}
+
+inline size_t arena_off(b200collComm* c, const void* p) { return reinterpret_cast<CUdeviceptr>(p) - c->peer_va[c->rank]; }
+inline bool aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) % a) == 0; }
+
+// collectives.cu: count a call in the stats (and mark it for NVTX / debug traces); B200COLL_CHECK=1 cross-check of a symmetric launch
+void account(b200collComm* c, b200collOp_t op, size_t bytes, b200collAlgo_t algo);
+b200collResult_t cross_check(b200collComm* c, b200collOp_t op, b200collAlgo_t algo, size_t count, size_t off_a, size_t off_b);
+
+}  // namespace b200coll

@@ -51,7 +51,31 @@ struct Opts {
   int skew_us = 0;   // delay rank 0's launches (race hunting)
   struct Shape { int kind, ctas, threads; };
   std::vector<Shape> shapes;   // --sweep kind:ctas:threads,... (launch-shape tuning inside one process)
+  int bs_rows = 0, bs_cols = 0;   // --block-scale RxC: block-scaled FP8 collectives (0 = off)
+  size_t row_len = 2048;          // --row-len N: columns of the block-scaled matrix
 };
+
+// Block-scaled mode: each rank's send buffer is a [rows, row_len] FP8 matrix with one fp32 scale per bs_rows x bs_cols block. Scales are
+// seeded (hash of rank and block index): mantissas use all 23 bits, exponents span 2^-8..2^8, so products round and the check below,
+// which repeats the library's arithmetic on the host, is bit for bit.
+static size_t bs_max_scales(const Opts& o) {
+  const size_t rows = o.max_bytes / o.row_len + 1;
+  return (rows / o.bs_rows + 1) * (o.row_len / o.bs_cols + 1);
+}
+static float bs_scale(int rank, size_t idx) {
+  uint32_t h = (uint32_t)(idx * 2654435761u) ^ (uint32_t)(rank * 40503u + 0x9E3779B9u);
+  h ^= h >> 15; h *= 0x2C1B3C6Du; h ^= h >> 12;
+  return ldexpf(1.0f + (float)(h & 0x7FFFFF) * 0x1p-23f, (int)((h >> 23) % 17) - 8);
+}
+static uint32_t out_bits(float v, b200collDataType_t dt) {
+  if (dt == b200collFloat32) { uint32_t u; memcpy(&u, &v, 4); return u; }
+  if (dt == b200collFloat16) { __half h = __float2half_rn(v); uint16_t u; memcpy(&u, &h, 2); return u; }
+  __nv_bfloat16 b = __float2bfloat16_rn(v); uint16_t u; memcpy(&u, &b, 2); return u;
+}
+static uint32_t got_bits(const void* p, size_t i, b200collDataType_t dt) {
+  if (dt == b200collFloat32) { uint32_t u; memcpy(&u, (const char*)p + 4 * i, 4); return u; }
+  uint16_t u; memcpy(&u, (const char*)p + 2 * i, 2); return u;
+}
 
 static size_t parse_size(const char* s) {
   char* end; double v = strtod(s, &end);
@@ -152,6 +176,13 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
   void *send = nullptr, *recv = nullptr;
   CC(b200collMemAlloc(ctx.comm, &send, send_cap + 4096));
   CC(b200collMemAlloc(ctx.comm, &recv, recv_cap + 4096));
+  const bool bs_mode = o.bs_rows > 0;
+  float* scales = nullptr;
+  std::vector<float> host_scales;
+  if (bs_mode) {
+    if (o.op != "all_gather" && o.op != "reduce_scatter" && o.op != "all_reduce") { fprintf(stderr, "--block-scale takes --op all_gather, reduce_scatter or all_reduce\n"); return 2; }
+    CC(b200collMemAlloc(ctx.comm, (void**)&scales, bs_max_scales(o) * 4));
+  }
   b200collEpilogue ep{o.in_dt, o.out_dt, o.scale};
   int gen_ctr[4] = {0, 0, 0, 0};
   std::vector<char> host;
@@ -159,6 +190,7 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
   if (rank == 0) {
     printf("# b200coll_perf op=%s nranks=%d in=%s out=%s scale=%g algo=%s nvls=%d loopback=%d mode=%s\n", o.op.c_str(), n, dt_name(o.in_dt), dt_name(o.out_dt), o.scale, o.algo.c_str(),
            info.nvls, info.same_device_loopback, o.procs ? "procs" : "threads");
+    if (bs_mode) printf("# block-scaled: row_len=%zu block=%dx%d (one fp32 scale per block, seeded)\n", o.row_len, o.bs_rows, o.bs_cols);
     printf("#%13s %12s %6s %8s | %10s %8s %8s %6s | %10s %8s %8s %6s\n", "size(B)", "count", "type", "algo", "oop us", "algbw", "busbw", "#wrong", "ip us", "algbw", "busbw", "#wrong");
     fflush(stdout);
   }
@@ -175,7 +207,19 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
     else { count = bytes / is / n; in_elems = out_elems = count * n; }
     const size_t E = 16 / is;
     if (!is_ar) count = count / E * E;
+    if (bs_mode) count = count / o.row_len * o.row_len;      // whole rows on every rank (reduce-scatter: rows = n * count / row_len)
     if (count == 0) continue;
+    const size_t bs_rows_total = bs_mode ? (is_rs ? count * n : count) / o.row_len : 0;
+    const size_t bs_ncb = bs_mode ? (o.row_len + o.bs_cols - 1) / o.bs_cols : 0;
+    const size_t bs_nscales = bs_mode ? (bs_rows_total + o.bs_rows - 1) / o.bs_rows * bs_ncb : 0;
+    if (bs_mode) {
+      host_scales.resize(bs_nscales);
+      for (size_t k = 0; k < bs_nscales; k++) host_scales[k] = bs_scale(rank, k);
+      RT(cudaMemcpy(scales, host_scales.data(), bs_nscales * 4, cudaMemcpyHostToDevice));
+    }
+    const b200collBlockScale bsd{scales, o.row_len, o.bs_rows, o.bs_cols};
+    // value of element i of rank r's send matrix, dequantised (one fp32 multiply)
+    auto bs_val = [&](int r, size_t i) { return gen(r, i) * bs_scale(r, (i / o.row_len / o.bs_rows) * bs_ncb + (i % o.row_len) / o.bs_cols); };
     if (!is_ar) { in_elems = is_ag ? count : count * n; out_elems = is_rs ? count : count * n; }
     const size_t in_b = in_elems * is, out_b = out_elems * os;
     const size_t slot_b = (std::max(in_b, out_b / os * is) + 4095) / 4096 * 4096;
@@ -226,6 +270,9 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
           CC(b200collRecv(rbuf(slot), count * is, (rank + n - 1) % n, ctx.comm, st));
           CC(b200collGroupEnd());
         }
+        else if (bs_mode && is_ar) CC(b200collAllReduceBlockScaled(sbuf(slot), rbuf(slot), count, &bsd, &ep, b200collSum, ctx.comm, st));
+        else if (bs_mode && is_ag) CC(b200collAllGatherBlockScaled(sbuf(slot), rbuf(slot), count, &bsd, &ep, ctx.comm, st));
+        else if (bs_mode && is_rs) CC(b200collReduceScatterBlockScaled(sbuf(slot), rbuf(slot), count, &bsd, &ep, b200collSum, ctx.comm, st));
         else if (is_bc) CC(b200collBroadcast(sbuf(slot), rbuf(slot), count, &ep, kRoot, ctx.comm, st));
         else if (is_rd) CC(b200collReduce(sbuf(slot), rbuf(slot), count, &ep, b200collSum, kRoot, ctx.comm, st));
         else if (is_ar) CC(b200collAllReduce(sbuf(slot), rbuf(slot), count, &ep, b200collSum, ctx.comm, st));
@@ -253,7 +300,14 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
         host.resize(check_elems * os);
         RT(cudaMemcpy(host.data(), outp, check_elems * os, cudaMemcpyDeviceToHost));
         const size_t stride = check_elems > (1u << 22) ? 61 : 1;   // sample large buffers
-        for (size_t e = 0; e < check_elems; e += stride) {
+        for (size_t e = 0; e < check_elems && bs_mode; e += stride) {      // bit for bit: ((0 + v_0) + v_1 + ...) * scale, rounded once
+          float acc = 0.0f;
+          if (is_ag) acc += bs_val((int)(e / count), e % count);
+          else for (int r = 0; r < n; r++) acc += bs_val(r, is_rs ? (size_t)rank * count + e : e);
+          const uint32_t want = out_bits(acc * o.scale, o.out_dt), got = got_bits(host.data(), e, o.out_dt);
+          if (got != want) { if (errs < 4) fprintf(stderr, "rank %d %s block-scaled size %zu elem %zu: got bits 0x%x want 0x%x\n", rank, o.op.c_str(), bytes, e, got, want); errs++; }
+        }
+        for (size_t e = 0; e < check_elems && !bs_mode; e += stride) {
           const float want = expected(o, rank, n, e, count), got = to_f(host.data(), e, o.out_dt);
           // FP8 outputs round once: half an ulp is 2^-4 (e4m3) or 2^-3 (e5m2) of the value
           const float tol = o.out_dt == b200collFloat8e4m3 ? fabsf(want) * 0.0725f + 0.002f : o.out_dt == b200collFloat8e5m2 ? fabsf(want) * 0.135f + 0.002f : 0.0f;
@@ -305,6 +359,7 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
     printf("# launches=%llu staged_calls=%llu errors=%ld\n", (unsigned long long)s.kernel_launches, (unsigned long long)s.staged_calls, total_errors);
     fflush(stdout);      // --procs children leave through _exit(): nothing buffered survives it
   }
+  if (scales) CC(b200collMemFree(ctx.comm, scales));
   CC(b200collMemFree(ctx.comm, recv));
   CC(b200collMemFree(ctx.comm, send));
   RT(cudaStreamDestroy(st));
@@ -362,6 +417,8 @@ int main(int argc, char** argv) {
     else if (a == "-t" || a == "--nthreads" || a == "-m" || a == "--agg_iters" || a == "-p" || a == "--parallel_init" || a == "-z" || a == "--blocking" || a == "-a" || a == "--average" ||
              a == "-G" || a == "--cudagraph" || a == "-C" || a == "--report_cputime" || a == "-R" || a == "--local_register" || a == "-T" || a == "--timeout" || a == "-r" || a == "--root") (void)next();   // accepted, no effect here
     else if (a == "--out-dtype") o.out_dt = parse_dt(next());
+    else if (a == "--block-scale") { if (sscanf(next(), "%dx%d", &o.bs_rows, &o.bs_cols) != 2 || o.bs_rows < 1 || o.bs_cols < 16 || o.bs_cols % 16) { fprintf(stderr, "--block-scale RxC: R >= 1, C a multiple of 16\n"); return 1; } }
+    else if (a == "--row-len") o.row_len = (size_t)atoll(next());
     else if (a == "--scale") o.scale = (float)atof(next());
     else if (a == "--algo") o.algo = next();
     else if (a == "--iters" || a == "-n") o.iters = atoi(next());
@@ -389,6 +446,9 @@ int main(int argc, char** argv) {
            "  under mpirun / torchrun (OMPI_COMM_WORLD_*, PMI_*, RANK/WORLD_SIZE/LOCAL_RANK) each process is one rank; B200COLL_JOB_ID names the job\n"
            "  -w N -n/--iters N -c 0|1  warm-up, timed iterations, check results against the host reference\n"
            "  -d float|half|bfloat16|e4m3|e5m2 (fp8 = e4m3)   input type; --out-dtype T and --scale X fuse a cast / scale into the collective\n"
+           "  --block-scale RxC         block-scaled FP8 (all_gather, reduce_scatter, all_reduce): -d e4m3|e5m2 [R x C]-blocked matrices, one seeded\n"
+           "                            fp32 scale per block, --out-dtype bfloat16|half|float; -c 1 checks bit for bit against the host\n"
+           "  --row-len N               columns of the block-scaled matrix (default 2048; N and C multiples of 16)\n"
            "  --algo auto|ll|ll2|oneshot|twoshot|nvls   --inplace 0|1|2   --max-ctas N   --sweep kind:ctas:threads,...   --json FILE   --window SIZE\n"
            "  --selfcheck               report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;
@@ -396,6 +456,7 @@ int main(int argc, char** argv) {
     else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 1; }
   }
   if (o.factor < 2) o.factor = 2;
+  if (o.bs_rows && (o.row_len == 0 || o.row_len % 16)) { fprintf(stderr, "--row-len must be a positive multiple of 16\n"); return 1; }
   const LauncherRank lr = launcher_rank();
   if (lr.size > 1 && o.devs.empty() && !o.procs) {
     // one rank of an mpirun / torchrun job (nccl-tests' -g 1 layout): rendezvous on the job id, timing page in /dev/shm
@@ -413,7 +474,7 @@ int main(int argc, char** argv) {
     o.nranks = lr.size; o.procs = true;
     b200collConfig cfg; b200collConfigDefault(&cfg);
     const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
-    if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20);
+    if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0);
     b200collUniqueId id; CC(b200collUniqueIdFromString(("perf/" + lr.job).c_str(), &id));
     RT(cudaSetDevice(dev));
     b200collComm_t comm;
@@ -441,7 +502,7 @@ int main(int argc, char** argv) {
   b200collConfig cfg; b200collConfigDefault(&cfg);
   // arena: two windows (+ max buffers) and slack
   const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
-  size_t need = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20);
+  size_t need = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0);
   if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = need;
   if (o.procs) {
     b200collUniqueId id; CC(b200collGetUniqueId(&id));

@@ -41,6 +41,10 @@ class Epilogue(C.Structure):
     _fields_ = [("in_dtype", C.c_int), ("out_dtype", C.c_int), ("scale", C.c_float)]
 
 
+class BlockScale(C.Structure):
+    _fields_ = [("scales", C.c_void_p), ("row_len", C.c_size_t), ("block_rows", C.c_int), ("block_cols", C.c_int)]
+
+
 class Config(C.Structure):
     _fields_ = [("arena_bytes", C.c_size_t), ("enable_nvls", C.c_int), ("max_ctas", C.c_int), ("timeout_ms", C.c_int), ("debug", C.c_int)]
 
@@ -125,6 +129,9 @@ def load() -> C.CDLL:
     L.b200collBroadcast.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
     L.b200collReduce.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, ci, vp, vp]
     L.b200collBarrier.argtypes = [vp, vp]
+    L.b200collAllGatherBlockScaled.argtypes = [vp, vp, sz, C.POINTER(BlockScale), C.POINTER(Epilogue), vp, vp]
+    L.b200collReduceScatterBlockScaled.argtypes = [vp, vp, sz, C.POINTER(BlockScale), C.POINTER(Epilogue), ci, vp, vp]
+    L.b200collAllReduceBlockScaled.argtypes = [vp, vp, sz, C.POINTER(BlockScale), C.POINTER(Epilogue), ci, vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -181,6 +188,41 @@ def torch_dtype_code(dtype) -> int:
     import torch
     return {torch.float32: F32, torch.float16: F16, torch.bfloat16: BF16, torch.float8_e4m3fn: FP8_E4M3, torch.float8_e5m2: FP8_E5M2, torch.int8: I8, torch.uint8: U8, torch.int32: I32,
             torch.int64: I64, torch.float64: F64, torch.bool: U8}[dtype]
+
+
+def check_block_scaled(op: str, nranks: int, q, scales, out, block=(1, 128)) -> tuple[int, int]:
+    """Shape and dtype rules of the block-scaled collectives ("all_gather", "reduce_scatter", "all_reduce"), checked on the tensors'
+    metadata only (no device, no communicator): raises ValueError, returns (block_rows, block_cols).
+    q: 2-D contiguous float8_e4m3fn / float8_e5m2 [rows, row_len]; scales: contiguous float32 (ceil(rows/br), ceil(row_len/bc));
+    out: bfloat16 / float16 / float32 of shape (nranks*rows, row_len) for all-gather, (rows/nranks, row_len) for reduce-scatter,
+    (rows, row_len) for all-reduce."""
+    import torch
+    if op not in ("all_gather", "reduce_scatter", "all_reduce"):
+        raise ValueError(f"unknown block-scaled op {op!r}")
+    if q.dtype not in (torch.float8_e4m3fn, torch.float8_e5m2):
+        raise ValueError(f"q must be float8_e4m3fn or float8_e5m2, not {q.dtype}")
+    if q.dim() != 2 or not q.is_contiguous():
+        raise ValueError(f"q must be a contiguous 2-D [rows, row_len] tensor, got shape {tuple(q.shape)}")
+    try:
+        br, bc = (int(b) for b in block)
+    except (TypeError, ValueError):
+        raise ValueError(f"block must be (block_rows, block_cols), got {block!r}") from None
+    if br < 1 or bc < 16 or bc % 16:
+        raise ValueError(f"block {block!r}: block_rows must be >= 1 and block_cols a positive multiple of 16")
+    rows, row_len = q.shape
+    if row_len % 16:
+        raise ValueError(f"row_len {row_len} must be a multiple of 16")
+    want = (-(-rows // br), -(-row_len // bc))
+    if scales.dtype != torch.float32 or tuple(scales.shape) != want or not scales.is_contiguous():
+        raise ValueError(f"scales must be a contiguous float32 tensor of shape {want}, got {scales.dtype} {tuple(scales.shape)}")
+    if out.dtype not in (torch.bfloat16, torch.float16, torch.float32) or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous bfloat16, float16 or float32 tensor, got {out.dtype}")
+    if op == "reduce_scatter" and rows % nranks:
+        raise ValueError(f"reduce_scatter: rows ({rows}) must be a multiple of nranks ({nranks})")
+    out_shape = {"all_gather": (nranks * rows, row_len), "reduce_scatter": (rows // nranks, row_len), "all_reduce": (rows, row_len)}[op]
+    if tuple(out.shape) != out_shape:
+        raise ValueError(f"{op}: out must have shape {out_shape}, got {tuple(out.shape)}")
+    return br, bc
 
 
 class _CudaArray:
@@ -410,6 +452,28 @@ class Comm:
         ep = self._ep(src, dst, scale)
         _check(load().b200collReduceScatter(C.c_void_p(src.data_ptr()), C.c_void_p(dst.data_ptr()), dst.numel(), C.byref(ep), op, self._h, self._stream(stream)), "ReduceScatter")
         return dst
+
+    def _block_scaled(self, what, fn, op_name, q, scales, out, block, scale, extra, count, stream):
+        br, bc = check_block_scaled(op_name, self.nranks, q, scales, out, block)
+        bs = BlockScale(scales.data_ptr(), q.shape[1], br, bc)
+        ep = self._ep(q, out, scale)
+        _check(fn(C.c_void_p(q.data_ptr()), C.c_void_p(out.data_ptr()), count, C.byref(bs), C.byref(ep), *extra, self._h, self._stream(stream)), what)
+        return out
+
+    def all_gather_block_scaled(self, q, scales, out, block=(1, 128), scale: float = 1.0, stream=None):
+        """out[r-th shard] = round(scale * dequant(q of rank r)), dequant = float(q) times the fp32 scale of its block_rows x block_cols
+        block. q [rows, row_len] FP8 and scales (ceil(rows/br), ceil(row_len/bc)) fp32 must be arena tensors (`empty()`); out is bf16,
+        fp16 or fp32 of shape (nranks*rows, row_len). FP8 and scales cross NVLink; the receiver dequantises (b200collAllGatherBlockScaled)."""
+        return self._block_scaled("AllGatherBlockScaled", load().b200collAllGatherBlockScaled, "all_gather", q, scales, out, block, scale, (), q.numel(), stream)
+
+    def reduce_scatter_block_scaled(self, q, scales, out, block=(1, 128), scale: float = 1.0, op: int = SUM, stream=None):
+        """out = round(scale * sum over ranks, in rank order, of dequant(row slice `rank` of q)); op SUM or AVG; out (rows/nranks, row_len)."""
+        return self._block_scaled("ReduceScatterBlockScaled", load().b200collReduceScatterBlockScaled, "reduce_scatter", q, scales, out, block, scale, (op,),
+                                  q.numel() // self.nranks, stream)
+
+    def all_reduce_block_scaled(self, q, scales, out, block=(1, 128), scale: float = 1.0, op: int = SUM, stream=None):
+        """out = round(scale * sum over ranks, in rank order, of dequant(q)); op SUM or AVG; out (rows, row_len). Two-shot needs out in the arena."""
+        return self._block_scaled("AllReduceBlockScaled", load().b200collAllReduceBlockScaled, "all_reduce", q, scales, out, block, scale, (op,), q.numel(), stream)
 
     def all_to_all(self, src, dst, scale: float = 1.0, stream=None):
         ep = self._ep(src, dst, scale)
