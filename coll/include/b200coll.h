@@ -66,15 +66,31 @@ typedef enum {
 /* Fused-epilogue types are fp32, fp16, bf16, e4m3 and e5m2. Supported (in_dtype, out_dtype) pairs:
  *   f32 -> f32, f16, bf16, e4m3, e5m2      f16 -> f16, f32, e4m3, e5m2      bf16 -> bf16, f32, e4m3, e5m2
  *   e4m3 / e5m2 -> e4m3, e5m2, f16, bf16   (FP8 -> f32 is refused with InvalidArgument)
- * Every input element is widened to fp32 and summed in rank order, multiplied by scale (avg: times the fp32 value 1/nranks) and rounded
- * ONCE to the output type, so every rank holds bit-identical results. Rounding to FP8 is round-to-nearest-even with saturation to the
- * finite range: +-inf becomes +-max, NaN stays NaN. The same scale and cast apply to all-gather, broadcast and all-to-all(v): e4m3 in,
- * bf16 out, scale = inverse quantisation scale is a dequantising all-gather. The NVLS switch of an H100 cannot reduce FP8 (sm_90a has
- * no FP8 multimem.ld_reduce), so FP8 reductions run on the P2P algorithms; FP8 data movement may still use multimem.st. */
+ * Sum and avg: every input element is widened to fp32, accumulated from +0 (so -0 inputs give +0) in a fixed order, multiplied once
+ * by scale (avg: the fp32 product scale * (1/nranks)) and rounded ONCE, to nearest even, to the output type, so every rank holds
+ * bit-identical results. The order depends on the kernel:
+ *   FP8 inputs, every P2P kernel                            ranks 0 .. N-1
+ *   LL and LL2 all-reduce, LL reduce-scatter                ranks 0 .. N-1
+ *   one-shot all-reduce, P2P rooted reduce                  ranks 0 .. N-1
+ *   two-shot all-reduce (16- and 32-bit inputs)             vector v lies in slice o where nvec*o/N <= v < nvec*(o+1)/N (nvec = count /
+ *                                                           (16 / sizeof(in))); it is summed o, o+1, .., N-1, 0, .., o-1. Elements past
+ *                                                           the last whole vector are summed in rank order. A staged all-reduce (buffers
+ *                                                           outside the arena) runs this per staging chunk, slices taken from the chunk.
+ *   P2P reduce-scatter (16- and 32-bit inputs)              receiving rank r sums r, r+1, .., N-1, 0, .., r-1
+ *   NVLS (multimem.ld_reduce)                               the switch's order: within an ulp of the exact sum, not bit-reproducible
+ * Rounding to FP8 saturates to the finite range (+-inf becomes +-max, NaN stays NaN); fp16 overflows to inf.
+ * All-gather, broadcast and all-to-all(v) apply the same epilogue per element: round((0 + x) * scale) (e4m3 in, bf16 out, scale =
+ * inverse quantisation scale is a dequantising all-gather). With the identity epilogue (same type, scale 1) they are bit copies, -0
+ * and NaN payloads included, on the barrier-based and copy-engine kernels; the Lamport (ll) path carries values through fp32 registers
+ * (-0 becomes +0, NaN payloads may be quieted), which is why bit-exact payloads force the two-shot family. With one rank every op is a
+ * copy with this epilogue, and the identity is a bit copy at every size (in place: nothing is launched).
+ * The NVLS switch of an H100 cannot reduce FP8 (sm_90a has no FP8 multimem.ld_reduce), so FP8 reductions run on the P2P algorithms;
+ * FP8 data movement may still use multimem.st. */
 
 /* sum and avg of fp16 / bf16 / fp32 / e4m3 / e5m2 run on the fused fast paths (Lamport, two-shot, NVLS for the 16- and 32-bit types);
  * prod, min, max — and every operator on the integer types and fp64 — run on one barrier-based P2P kernel that accumulates in the
- * element type (fp16 / bf16 / FP8 in fp32). */
+ * element type (fp16 / bf16 / FP8 in fp32), starting from rank 0's value (not +0) and going through ranks 1 .. N-1; integer sums wrap.
+ * min / max propagate a NaN from any rank (as torch.minimum / maximum do) and keep the lower rank's value on a tie (-0 against +0). */
 typedef enum { b200collSum = 0, b200collAvg = 1, b200collProd = 2, b200collMin = 3, b200collMax = 4 } b200collRedOp_t;
 
 typedef enum {

@@ -168,10 +168,12 @@ static b200collResult_t launch_bulk(b200collComm* c, BulkArgs& a, bool sync, b20
 }
 
 // ------------------------------------------------------------------------------------------------ nranks == 1
+// The identity epilogue is a bit copy at every size (in place: nothing to do); anything else is round((0 + x) * scale).
 static b200collResult_t copy_scale(b200collComm* c, const void* send, void* recv, size_t count, const b200collEpilogue* ep, float scale, cudaStream_t st) {
-  if (send == recv && ep->in_dtype == ep->out_dtype && scale == 1.0f) return b200collSuccess;
+  const int identity = (ep->in_dtype == ep->out_dtype && scale == 1.0f) ? 1 : 0;
+  if (send == recv && identity) return b200collSuccess;
   const size_t nbytes = count * b200collTypeSize(ep->in_dtype);
-  if (bulk_enabled() && ep->in_dtype == ep->out_dtype && scale == 1.0f && nbytes >= bulk_min_bytes() && nbytes % 16 == 0 && aligned(recv, 16)) {
+  if (bulk_enabled() && identity && nbytes >= bulk_min_bytes() && nbytes % 16 == 0 && aligned(recv, 16)) {
     BulkArgs a = {};
     a.nseg = 1; a.src[0] = static_cast<const char*>(send); a.bytes[0] = nbytes; a.dst_local = static_cast<char*>(recv);
     return launch_bulk(c, a, false, b200collOpAllReduce, st);
@@ -181,7 +183,7 @@ static b200collResult_t copy_scale(b200collComm* c, const void* send, void* recv
     // streaming copy: no peers to wait for, so oversubscribe the chip (8 CTAs of 256 threads per SM) instead of the collective cap
     const size_t vecs = count / Epv<InT>::value + 1;
     Grid g{(int)std::max<size_t>(1, std::min<size_t>((vecs + 1023) / 1024, (size_t)std::max(1, c->sm_count) * 8)), 256};
-    launch_k(k_copy_scale<InT, OutT>, g.blocks, g.threads, st, static_cast<const InT*>(send), static_cast<OutT*>(recv), count, scale);
+    launch_k(k_copy_scale<InT, OutT>, g.blocks, g.threads, st, static_cast<const InT*>(send), static_cast<OutT*>(recv), count, scale, identity);
     LAUNCH_CHECK(c);
     return b200collSuccess;
   });

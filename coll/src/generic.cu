@@ -35,11 +35,13 @@ template <> __device__ __forceinline__ __nv_bfloat16 g_store<__nv_bfloat16>(floa
 template <> __device__ __forceinline__ __nv_fp8_e4m3 g_store<__nv_fp8_e4m3>(float v) { return from_float<__nv_fp8_e4m3>(v); }   // satfinite
 template <> __device__ __forceinline__ __nv_fp8_e5m2 g_store<__nv_fp8_e5m2>(float v) { return from_float<__nv_fp8_e5m2>(v); }
 
+// min / max: a NaN from any rank propagates (as torch.minimum / maximum do); on a tie (+0 vs -0 included) the lower rank's value stays.
+// `b != b` is false for integers and compiles away.
 template <int OP, typename A> __device__ __forceinline__ A g_apply(A a, A b) {
   if (OP == b200collSum) return a + b;
   if (OP == b200collProd) return a * b;
-  if (OP == b200collMin) return b < a ? b : a;
-  return b > a ? b : a;
+  if (OP == b200collMin) return (b < a || b != b) ? b : a;
+  return (b > a || b != b) ? b : a;
 }
 
 template <typename T, int OP>
@@ -167,12 +169,12 @@ b200collResult_t generic_reduce(b200collComm* c, b200collOp_t which, const void*
   if (count == 0) return b200collSuccess;
   const int n = c->nranks;
   const size_t in_elems = which == b200collOpReduceScatter ? count * n : count;
+  if (n > 1 && which == b200collOpReduceScatter && (count * es) % 16 != 0) { set_last_error("reduce-scatter recvcount must be a multiple of 16 bytes / sizeof(dtype)"); return b200collInvalidArgument; }
   c->stats.calls[which]++; c->stats.bytes[which] += count * es; c->stats.algo_calls[b200collAlgoTwoShot]++;
   if (n == 1) {
     if (send != recv) { cudaError_t e = cudaMemcpyAsync(recv, send, count * es, cudaMemcpyDeviceToDevice, st); if (e != cudaSuccess) { set_last_error(cudaGetErrorString(e)); return b200collUnhandledCudaError; } }
     return b200collSuccess;
   }
-  if (which == b200collOpReduceScatter && (count * es) % 16 != 0) { set_last_error("reduce-scatter recvcount must be a multiple of 16 bytes / sizeof(dtype)"); return b200collInvalidArgument; }
   char* const base = reinterpret_cast<char*>(c->peer_va[c->rank]);
   auto off = [&](const void* p) { return (size_t)(static_cast<const char*>(p) - base); };
   const bool sym_in = b200collIsSymmetric(c, send, in_elems * es);

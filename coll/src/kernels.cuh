@@ -32,11 +32,14 @@ __device__ __forceinline__ void finish_store_local(OutT* dst, const float* acc, 
 }
 
 // ------------------------------------------------------------------------------------------------
+// identity (same type, scale 1): a bit copy, so -0 and NaN payloads survive as they do in the copy-engine path of larger copies.
+// Otherwise out = round((0 + x) * scale) in the vector body and the tail alike (-0 becomes +0).
 template <typename InT, typename OutT>
-__global__ void __launch_bounds__(kThreads) k_copy_scale(const InT* __restrict__ in, OutT* __restrict__ out, size_t count, float scale) {
+__global__ void __launch_bounds__(kThreads) k_copy_scale(const InT* __restrict__ in, OutT* __restrict__ out, size_t count, float scale, int identity) {
   pdl_prologue();
   constexpr int E = Epv<InT>::value;
   constexpr int U = 4;                       // 4 x 16 B loads in flight per thread: HBM-latency hiding for a pure streaming kernel
+  constexpr bool kSameSize = sizeof(InT) == sizeof(OutT);
   const size_t nvec = count / E;
   const size_t stride = (size_t)gridDim.x * blockDim.x * U;
   for (size_t base = (size_t)blockIdx.x * blockDim.x * U + threadIdx.x; base < nvec; base += stride) {
@@ -46,12 +49,21 @@ __global__ void __launch_bounds__(kThreads) k_copy_scale(const InT* __restrict__
 #pragma unroll
     for (int u = 0; u < U; u++) {
       const size_t v = base + (size_t)u * blockDim.x;
-      if (v < nvec) { float acc[E] = {}; unpack_add<InT>(acc, d[u]); finish_store_local<InT, OutT, E>(out + v * E, acc, scale); }
+      if (v < nvec) {
+        if (kSameSize && identity) { st_vec(out + v * E, d[u]); continue; }
+        float acc[E] = {}; unpack_add<InT>(acc, d[u]); finish_store_local<InT, OutT, E>(out + v * E, acc, scale);
+      }
     }
   }
   if (blockIdx.x == 0) {
     const size_t e = nvec * E + threadIdx.x;
-    if (e < count) out[e] = from_float<OutT>(to_float<InT>(in[e]) * scale);
+    if (e < count) {
+      OutT o = from_float<OutT>((0.f + to_float<InT>(in[e])) * scale);
+      if constexpr (kSameSize) {
+        if (identity) { const InT x = in[e]; memcpy(&o, &x, sizeof(o)); }
+      }
+      out[e] = o;
+    }
   }
 }
 
@@ -357,8 +369,9 @@ __global__ void __launch_bounds__(kThreads) k_pull_reduce(COMM_PARAM, size_t in_
 // ------------------------------------------------------------------------------------------------
 // Two-shot fused into one pass: rank r owns vector slice r; pulls it from every peer, reduces in fp32,
 // applies scale/cast and pushes the finished vector into every peer's out. Bytes per GPU and direction:
-// S(N-1)/N pulled + S(N-1)/N pushed -> bus bandwidth bound = link bandwidth. Peers are visited starting after my own rank (spreads
-// the pulls over the links); FP8 inputs are pulled and summed in rank order instead, the order the FP8 semantics promise.
+// S(N-1)/N pulled + S(N-1)/N pushed -> bus bandwidth bound = link bandwidth. The slice owner sums its own copy first, then ranks
+// owner+1, ..., N-1, 0, ..., owner-1 (spreads the pulls over the links); FP8 inputs are pulled and summed in rank order instead, the
+// order the FP8 semantics promise.
 template <typename InT, typename OutT>
 __global__ void __launch_bounds__(kThreads) k_ar_twoshot(COMM_PARAM, size_t in_off, size_t out_off, size_t count, float scale, uint32_t op) {
   pdl_prologue();
@@ -613,7 +626,7 @@ __global__ void __launch_bounds__(kThreads) k_bcast(COMM_PARAM, const InT* __res
     if (blockIdx.x == 0) {                          // scalar tail (count not a multiple of one vector)
       const size_t e = nvec * E + threadIdx.x;
       if (e < count) {
-        OutT o = from_float<OutT>(to_float<InT>(in[e]) * scale);
+        OutT o = from_float<OutT>((0.f + to_float<InT>(in[e])) * scale);   // +0 accumulator, as in the vector path
         if constexpr (sizeof(InT) == sizeof(OutT)) {
           if (identity) { const InT x = in[e]; memcpy(&o, &x, sizeof(o)); }   // bit-exact, like the vector path (payload may not be a float at all)
         }
