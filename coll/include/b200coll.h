@@ -80,10 +80,11 @@ typedef enum {
  *   NVLS (multimem.ld_reduce)                               the switch's order: within an ulp of the exact sum, not bit-reproducible
  * Rounding to FP8 saturates to the finite range (+-inf becomes +-max, NaN stays NaN); fp16 overflows to inf.
  * All-gather, broadcast and all-to-all(v) apply the same epilogue per element: round((0 + x) * scale) (e4m3 in, bf16 out, scale =
- * inverse quantisation scale is a dequantising all-gather). With the identity epilogue (same type, scale 1) they are bit copies, -0
- * and NaN payloads included, on the barrier-based and copy-engine kernels; the Lamport (ll) path carries values through fp32 registers
- * (-0 becomes +0, NaN payloads may be quieted), which is why bit-exact payloads force the two-shot family. With one rank every op is a
- * copy with this epilogue, and the identity is a bit copy at every size (in place: nothing is launched).
+ * inverse quantisation scale is a dequantising all-gather). With the identity epilogue (same type, scale 1) they are bit copies, -0,
+ * +-inf and NaN payloads included, on the barrier-based and copy-engine kernels. The Lamport (ll) path stores the received words too,
+ * with one exception: a 4-byte word equal to its empty-slot marker 0xFFFFFFFF (bytes FF FF FF FF) arrives as 0x7FFF7FFF (FF 7F FF 7F),
+ * which is still NaN in every type; payloads that are not floating point must therefore force the two-shot family. With one rank every
+ * op is a copy with this epilogue, and the identity is a bit copy at every size (in place: nothing is launched).
  * The NVLS switch of an H100 cannot reduce FP8 (sm_90a has no FP8 multimem.ld_reduce), so FP8 reductions run on the P2P algorithms;
  * FP8 data movement may still use multimem.st. */
 

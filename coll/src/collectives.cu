@@ -198,21 +198,22 @@ static b200collResult_t launch_ll(b200collComm* c, b200collOp_t op, const void* 
     Grid g = pick_grid(c, kShapeLL, nv, 1);
     const InT* in = static_cast<const InT*>(send); OutT* out = static_cast<OutT*>(recv);
     const bool mc = c->nvls;
+    const int identity = (ep->in_dtype == ep->out_dtype && scale == 1.0f) ? 1 : 0;     // movement only (SUM=false): store the words as received
     struct PdlScope { PdlScope(bool v) { t_pdl_small = v; } ~PdlScope() { t_pdl_small = false; } } pdl_scope(count * sizeof(InT) <= pdl_max_bytes());
     switch (op) {
       case b200collOpAllReduce:
-        if (mc) launch_k(k_ll<InT, OutT, false, true, true>, g.blocks, g.threads, st, c->dev, in, out, count, scale, op);
-        else launch_k(k_ll<InT, OutT, false, true, false>, g.blocks, g.threads, st, c->dev, in, out, count, scale, op);
+        if (mc) launch_k(k_ll<InT, OutT, false, true, true>, g.blocks, g.threads, st, c->dev, in, out, count, scale, identity, op);
+        else launch_k(k_ll<InT, OutT, false, true, false>, g.blocks, g.threads, st, c->dev, in, out, count, scale, identity, op);
         break;
       case b200collOpAllGather:
-        if (mc) launch_k(k_ll<InT, OutT, false, false, true>, g.blocks, g.threads, st, c->dev, in, out, count, scale, op);
-        else launch_k(k_ll<InT, OutT, false, false, false>, g.blocks, g.threads, st, c->dev, in, out, count, scale, op);
+        if (mc) launch_k(k_ll<InT, OutT, false, false, true>, g.blocks, g.threads, st, c->dev, in, out, count, scale, identity, op);
+        else launch_k(k_ll<InT, OutT, false, false, false>, g.blocks, g.threads, st, c->dev, in, out, count, scale, identity, op);
         break;
       case b200collOpReduceScatter:
-        launch_k(k_ll<InT, OutT, true, true, false>, g.blocks, g.threads, st, c->dev, in, out, count, scale, op);
+        launch_k(k_ll<InT, OutT, true, true, false>, g.blocks, g.threads, st, c->dev, in, out, count, scale, identity, op);
         break;
       default:
-        launch_k(k_ll<InT, OutT, true, false, false>, g.blocks, g.threads, st, c->dev, in, out, count, scale, op);
+        launch_k(k_ll<InT, OutT, true, false, false>, g.blocks, g.threads, st, c->dev, in, out, count, scale, identity, op);
         break;
     }
     LAUNCH_CHECK(c);

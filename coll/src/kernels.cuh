@@ -124,10 +124,21 @@ __device__ __forceinline__ void store_out_guarded(OutT* out, size_t i, size_t co
   }
 }
 
+template <typename OutT, int E>
+__device__ __forceinline__ void store_raw_guarded(OutT* out, size_t vec, size_t count, const uint4& w) {
+  if ((vec + 1) * E <= count) { st_vec(out + vec * E, w); return; }
+  union { OutT e[E]; uint4 v; } u;
+  u.v = w;
+#pragma unroll
+  for (int k = 0; k < E; k++) if (vec * E + k < count) out[vec * E + k] = u.e[k];
+}
+
 // SLICED=false: every peer gets my whole `count`-element input (AR, AG). SLICED=true: peer p gets block p (RS, A2A).
-// SUM=true: out[i] = sum over sources (AR, RS). SUM=false: out[src*count + i] = source's data (AG, A2A).
+// SUM=true: out[i] = sum over sources (AR, RS). SUM=false: out[src*count + i] = source's data (AG, A2A); with the identity epilogue
+// (same type, scale 1) the received words are stored as they arrived, so the only change is the sentinel word, which ll_sanitize
+// rewrote to kLLSanitized (still NaN in every type).
 template <typename InT, typename OutT, bool SLICED, bool SUM, bool MC>
-__global__ void __launch_bounds__(kThreads) k_ll(COMM_PARAM, const InT* __restrict__ in, OutT* __restrict__ out, size_t count, float scale, uint32_t op) {
+__global__ void __launch_bounds__(kThreads) k_ll(COMM_PARAM, const InT* __restrict__ in, OutT* __restrict__ out, size_t count, float scale, int identity, uint32_t op) {
   pdl_prologue();
   constexpr int E = Epv<InT>::value;
   const uint32_t k = load_seq(c, kSeqLL);
@@ -183,6 +194,9 @@ __global__ void __launch_bounds__(kThreads) k_ll(COMM_PARAM, const InT* __restri
 #pragma unroll
         for (int r = 0; r < kMaxRanks; r++) if (r < c.nranks) {
           uint4 d = (r == c.rank) ? own : ll_wait(c, ll_slot(me, buf, r, i), r, op);
+          if constexpr (sizeof(InT) == sizeof(OutT)) {
+            if (identity) { store_raw_guarded<OutT, E>(out + (size_t)r * count, i, count, d); continue; }
+          }
           float acc[E] = {};
           unpack_add<InT>(acc, d);
           store_out_guarded<OutT, E>(out + (size_t)r * count, i, count, acc, scale);
@@ -207,15 +221,6 @@ __global__ void __launch_bounds__(kThreads) k_ll(COMM_PARAM, const InT* __restri
 // everybody's hi slot (buf, p, i) — one multimem.st when MC — and every rank copies the N slices into out.
 // One thread owns vector i of *every* slice end to end, so there is no intra-kernel dependency between threads
 // and in-place is safe (a thread reads all its inputs before its first write). Needs sizeof(OutT) == sizeof(InT).
-template <typename OutT, int E>
-__device__ __forceinline__ void store_raw_guarded(OutT* out, size_t vec, size_t count, const uint4& w) {
-  if ((vec + 1) * E <= count) { st_vec(out + vec * E, w); return; }
-  union { OutT e[E]; uint4 v; } u;
-  u.v = w;
-#pragma unroll
-  for (int k = 0; k < E; k++) if (vec * E + k < count) out[vec * E + k] = u.e[k];
-}
-
 template <typename InT, typename OutT, bool MC>
 __global__ void __launch_bounds__(kThreads) k_ll_twoshot(COMM_PARAM, const InT* __restrict__ in, OutT* __restrict__ out, size_t count, float scale, uint32_t op) {
   pdl_prologue();

@@ -525,8 +525,8 @@ class Comm:
 
     class _BitExact:
         """Payloads that are not floating point (token ids, masks) must not take the Lamport path: it recognises empty slots by a NaN bit
-        pattern and rewrites payload words that collide with it (harmless for floats, fatal for an int64 -1), and it passes data through
-        fp32 registers. The barrier-based push kernels forward 16-byte vectors untouched when the epilogue is the identity."""
+        pattern and rewrites payload words that collide with it (0xFFFFFFFF becomes 0x7FFF7FFF: harmless for floats, which stay NaN,
+        fatal for an int64 -1). The barrier-based push kernels forward 16-byte vectors untouched when the epilogue is the identity."""
 
         def __init__(self, comm):
             self.comm = comm

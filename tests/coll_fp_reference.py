@@ -1,4 +1,5 @@
-"""Order-exact fp32 reference for the fp32 / fp16 / bf16 collectives of libb200coll, and seeded data that can tell orders apart.
+"""Order-exact fp32 reference for the fp32 / fp16 / bf16 / e4m3 / e5m2 collectives of libb200coll, and seeded data that can tell
+orders apart.
 
 Every fused sum / avg path widens each input to fp32, accumulates from +0 in a fixed order, multiplies once by the fp32 scale (avg: the
 fp32 product scale * (1/N)) and rounds once, to nearest even, to the output type (FP8 saturates, fp16 overflows to inf). The order is
@@ -10,11 +11,17 @@ a property of the kernel that ran, so the reference takes it as an argument:
                                   o, o+1, ..., o-1; elements past the last whole vector are summed in rank order (ar_tail_rank0)
     ("staged", N, E, count, chunk)  the staged all-reduce: two-shot on each chunk of `chunk` elements, slices from the chunk's nvec
 
-Not collected by pytest (no test_ prefix); imported by test_coll_fp_numerics_cpu.py and test_coll_fp_numerics_gpu.py."""
+FP8 inputs are summed in rank order on every P2P kernel (the two-shot all-reduce and the P2P reduce-scatter included), so their
+order model is always [0, 1, ..., N-1].
+
+Not collected by pytest (no test_ prefix); imported by the test_coll_fp_numerics_* and test_coll_fp8_numerics_* files."""
 import torch
 
 STAGE_HALF_BYTES = 32 << 20          # coll/src/layout.h kStageHalfBytes
 LL_ONESHOT_MAX_BYTES = 512 << 10     # kLLOneShotMaxBytes: per source
+HOST_ZEROCOPY_BYTES = 4096 << 10     # hostpath.cu defaults: B200COLL_HOST_ZEROCOPY_KB
+HOST_PIPELINE_BYTES = 8192 << 10     # B200COLL_HOST_PIPELINE_KB
+LL_SENTINEL, LL_SANITIZED = 0xFFFFFFFF, 0x7FFF7FFF    # layout.h kLLSentinel / kLLSanitized
 
 FP8_MAX = {torch.float8_e4m3fn: 448.0, torch.float8_e5m2: 57344.0}
 # significand bits (implicit bit included) and exponent of the smallest normal
@@ -91,6 +98,24 @@ def staged_chunk(in_size, out_size, nranks, op):
     raise ValueError(op)
 
 
+def host_chunks(count, in_size, out_size, nranks):
+    """b200collAllReduceHost with its default knobs (they are read once per process): the regime and the element count of each
+    b200collAllReduce it makes, in order. "zero_copy" is one call on the mapped host pointers; "single" and "pipelined" run on arena
+    staging buffers, so each chunk is an all-reduce of its own, with its own algorithm choice and (two-shot) its own slices."""
+    nbytes = count * in_size
+    zc_feasible = nranks == 1 or nbytes <= LL_ONESHOT_MAX_BYTES or (in_size == out_size and nbytes <= LL_ONESHOT_MAX_BYTES * nranks)
+    if nbytes <= HOST_ZEROCOPY_BYTES and zc_feasible:
+        return "zero_copy", [count]
+    chunk = min(16 << 20, max(4 << 20, nbytes // 6))
+    if nbytes < HOST_PIPELINE_BYTES:
+        chunk = nbytes
+    chunk = (chunk + 1023) // 1024 * 1024
+    if chunk >= nbytes:
+        return "single", [count]
+    ce = chunk // in_size
+    return "pipelined", [min(ce, count - d) for d in range(0, count, ce)]
+
+
 def staged_owner_map(count, n, e, chunk, device="cpu"):
     parts = [owner_map(min(chunk, count - d), n, e, device) for d in range(0, count, chunk)]
     return torch.cat(parts)
@@ -138,6 +163,16 @@ def ref_move(x, s, out_dtype, identity):
     return ref_reduce([x], [0], s, out_dtype)
 
 
+def ll_move(x):
+    """The identity epilogue on the Lamport (ll) path: a bit copy except that every 4-byte word equal to the empty-slot sentinel
+    (0xFFFFFFFF, NaN in every type) arrives as its sanitized form 0x7FFF7FFF (bytes FF 7F FF 7F, still NaN in every type). Words are
+    counted from the start of the buffer, which is 16-byte aligned."""
+    u = x.contiguous().view(torch.uint8).clone()
+    w = u[:u.numel() // 4 * 4].view(torch.int32)                              # a partial last word is padded with zeros: never the sentinel
+    w[w == -1] = LL_SANITIZED
+    return u.view(x.dtype)
+
+
 # ------------------------------------------------------------------------------------------------- data
 def _exp2(e):
     return torch.exp2(e.float())
@@ -152,6 +187,8 @@ def gen_inputs(n, count, in_dt, seed, device="cuda"):
         one small value (just above or below the tie) or two tiny values that tip it only when they meet before B,
       * input-type subnormals, -0 on every rank at some positions and at the last one, values near 65504 for fp16 (sums overflow),
       * NaN and +-inf at fixed positions."""
+    if in_dt in FP8_MAX:
+        return _gen_fp8(n, count, in_dt, seed, device)
     g = torch.Generator(device=device).manual_seed(seed)
     dev = device
     rnd = lambda *shape: torch.rand(shape, generator=g, device=dev)
@@ -215,7 +252,102 @@ def gen_inputs(n, count, in_dt, seed, device="cuda"):
     return [out[r].clone() for r in range(n)]                                 # own allocations: 16-byte aligned like any buffer
 
 
-NAN_PAYLOADS = {torch.float32: (0x7F800001, -0x3FFEDD), torch.bfloat16: (0x7F81, -0x3D), torch.float16: (0x7C01, -0x1C9)}
+NAN_PAYLOADS = {torch.float32: (0x7F800001, -0x3FFEDD), torch.bfloat16: (0x7F81, -0x3D), torch.float16: (0x7C01, -0x1C9),
+                torch.float8_e4m3fn: (0x7F, 0xFF), torch.float8_e5m2: (0x7D, 0xFE)}
+# FP8 bytes at fixed positions (position, rank or None for every rank, byte). e4m3 has no inf: 0x7F and 0xFF are its only NaNs.
+FP8_SPECIAL = {
+    torch.float8_e4m3fn: [(3, 1, 0x7F), (35, -1, 0xFF)],
+    torch.float8_e5m2: [(3, 1, 0x7E), (11, 0, 0x7C), (19, -1, 0xFC), (27, 0, 0x7C), (27, 1, 0xFC), (35, -1, 0xFF)],
+}
+LL_WORDS = ((48, LL_SENTINEL), (52, LL_SANITIZED))     # element (byte) offset of a 4-byte word on rank 1 % N
+
+
+def _gen_fp8(n, count, in_dt, seed, device):
+    """gen_inputs for e4m3 / e5m2 inputs; every value is built exactly in the input type (no rounding on the way in):
+      * random signs, 4 (e4m3) or 3 (e5m2) significant bits and a spread of exponents,
+      * cancellation: +B and -B on two ranks (B in 2^12 .. 2^15 for e5m2, 2^6 .. 2^8 for e4m3) and small values down to 2^-16 (e5m2) or
+        2^-9 (e4m3) elsewhere; for e5m2 the small ones survive only in some orders, for e4m3 every sum is exact in fp32 in any order,
+      * rounding ties of bf16, fp16, e4m3 and e5m2 outputs: B (with as many significant bits as the input type has) on one rank and half
+        an output ulp of B on another, plus nothing (an exact tie), a nudge just above or below it by less than half an fp16 ulp (rounding
+        through fp16 removes it), or, for e5m2 with B >= 2^8, a tiny value of half an fp32 ulp of B on every other rank: lost one by one,
+        a whole ulp when two meet before B,
+      * same-sign values near the maximum: sums past 448 (e4m3) and past 57344 and 65504 (e5m2), so FP8 outputs saturate and fp16
+        outputs overflow to inf,
+      * input-type subnormals, -0 on every rank at positions 7 mod 61 and at the last one (a scalar tail),
+      * FP8_SPECIAL bytes (NaN, and for e5m2 +-inf, with payloads), NAN_PAYLOADS at positions 41 and 43 on every rank, and on rank 1 % N
+        the words LL_WORDS: the Lamport sentinel FF FF FF FF at byte 48 and its sanitized form FF 7F FF 7F at byte 52."""
+    g = torch.Generator(device=device).manual_seed(seed)
+    dev = device
+    e5 = in_dt == torch.float8_e5m2
+    p = MANT[in_dt]
+    rnd = lambda *shape: torch.rand(shape, generator=g, device=dev)
+    rint = lambda lo, hi, *shape: torch.randint(lo, hi, shape, generator=g, device=dev)
+    frac = lambda k: 1 + k.float() / (1 << (p - 1))                               # 1.m with p - 1 fraction bits
+    sign = torch.where(rnd(n, count) < 0.5, -1.0, 1.0)
+    x = sign * _exp2(rint(-12, 13, n, count) if e5 else rint(-6, 8, n, count)) * frac(rint(0, 1 << (p - 1), n, count))
+    cls = rint(0, 100, count)
+    ranks = torch.arange(n, device=dev).unsqueeze(1)
+    a = rint(0, n, count)
+    b = (a + 1 + (rint(0, max(1, n - 1), count) if n > 1 else 0)) % n
+    is_a, is_b = ranks == a, ranks == b
+    rest = ~(is_a | is_b)
+    psign = torch.where(rnd(count) < 0.5, -1.0, 1.0)
+
+    # cancellation
+    big = psign * (_exp2(rint(12, 16, count)) * frac(rint(0, 3, count)) if e5 else _exp2(rint(6, 9, count)) * frac(rint(0, 7, count)))
+    se = rint(-16, -8, n, count) if e5 else rint(-9, -3, n, count)
+    small = sign * _exp2(se) * torch.where(se >= EMIN[in_dt], frac(rint(0, 1 << (p - 1), n, count)), torch.ones_like(sign))
+    x = torch.where((cls >= 50) & (cls < 65), torch.where(is_a, big, torch.where(is_b, -big, small)), x)
+
+    # ties of an output type (chosen per position)
+    tie_types = [torch.bfloat16, torch.float16, torch.float8_e4m3fn, torch.float8_e5m2]
+    tsel = cls % 4
+    pout = torch.tensor([MANT[t] for t in tie_types], device=dev)[tsel]
+    q = torch.minimum(pout, torch.tensor(p, device=dev))                         # significant bits of B: exact in input and output
+    if e5:
+        # e4m3 output: B + half must stay below 448, so B is 256, 320 or 384 (half = 16); otherwise B in 2^8 .. 2^13
+        eb = torch.where(tsel == 2, torch.full_like(cls, 8), rint(8, 14, count))
+        kmax = torch.where(tsel == 2, torch.full_like(cls, 3), _exp2(q - 1).long())
+    else:
+        eb = rint(3, 8, count)                                                    # half an fp16 ulp of B (2^(eb-11)) is still >= 2^-9
+        kmax = _exp2(q - 1).long()
+    k = (rnd(count) * kmax).floor()
+    bval = psign * _exp2(eb) * (1 + k / _exp2(q - 1))
+    half = psign * _exp2(eb - pout)
+    variant = rint(0, 4, count)
+    if not e5:
+        variant = torch.where(variant >= 2, variant - 2, variant)                 # no tiny pairs for e4m3: exact ties and nudges
+    first_rest = (ranks == (b + 1) % n) & rest
+    tiny = psign * _exp2(eb - 24)                                                 # half an fp32 ulp of B: lost alone (B is even), not in pairs
+    nudge = torch.where(rnd(count) < 0.5, -1.0, 1.0) * psign * _exp2(eb - (13 if e5 else 12))   # < half an fp16 ulp of B
+    eps = torch.where(variant == 0, torch.zeros_like(tiny), torch.where(variant == 1, nudge, tiny))
+    eps_r = torch.where(variant == 1, first_rest, rest)
+    negz = torch.where(rnd(n, count) < 0.5, -0.0, 0.0)
+    tie = torch.where(is_a, bval, torch.where(is_b, half, torch.where(eps_r, eps, negz)))
+    x = torch.where((cls >= 65) & (cls < 85), tie, x)
+
+    # saturation: one sign per position, magnitudes near the maximum on every rank
+    top = _exp2(rint(14, 16, n, count)) * frac(rint(0, 4, n, count)) if e5 else _exp2(rint(7, 9, n, count)) * frac(rint(0, 7, n, count))
+    x = torch.where((cls >= 85) & (cls < 92), psign * top.clamp(max=FP8_MAX[in_dt]), x)
+
+    # input-type subnormals: k * 2^(emin - p + 1)
+    sub = sign * rint(1, 1 << (p - 1), n, count).float() * _exp2(torch.tensor(EMIN[in_dt] - p + 1, device=dev))
+    x = torch.where((cls >= 92) & (cls < 99), sub, x)
+
+    idx = torch.arange(count, device=dev)
+    x = torch.where((idx % 61 == 7) | (idx == count - 1), torch.full_like(x, -0.0), x)
+    out = x.to(in_dt)
+    bits = out.view(torch.uint8)
+    for pos, r, v in FP8_SPECIAL[in_dt]:
+        if pos < count:
+            bits[r % n, pos] = v
+    for pos, v in zip((41, 43), NAN_PAYLOADS[in_dt]):
+        if pos < count:
+            bits[:, pos] = v
+    for pos, word in LL_WORDS:
+        if pos + 4 <= count:
+            bits[1 % n, pos:pos + 4] = torch.tensor(list(word.to_bytes(4, "little")), dtype=torch.uint8, device=dev)
+    return [out[r].clone() for r in range(n)]
 
 
 # ------------------------------------------------------------------------------------------------- comparison

@@ -348,8 +348,8 @@ MOVES = [("float32", "bfloat16", 0.1), ("bfloat16", "float32", 0.1), ("float16",
 @pytest.mark.parametrize("group", [3, 5], indirect=True)
 def test_data_movement(torch_cuda, coll_mod, group):
     """All-gather, broadcast, all-to-all and all-to-all-v: round((0 + x) * scale) with a cast or a scale, a bit copy (-0 and NaN
-    payloads included) with the identity epilogue. The Lamport path carries values through fp32, so identity copies force the
-    barrier-based kernels, as Comm.bit_exact does."""
+    payloads included) with the identity epilogue. The Lamport path rewrites a word equal to its empty-slot marker, so identity copies
+    force the barrier-based kernels, as Comm.bit_exact does (test_coll_fp8_numerics_gpu.py checks the Lamport identity model)."""
     torch, coll = torch_cuda, coll_mod
     comms, streams = group
     n = len(comms)
