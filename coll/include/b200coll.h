@@ -263,6 +263,42 @@ b200collResult_t b200collReduceScatterBlockScaled(const void* send, void* recv, 
 b200collResult_t b200collAllReduceBlockScaled(const void* send, void* recv, size_t count, const b200collBlockScale* bs,
                                               const b200collEpilogue* ep, b200collRedOp_t op, b200collComm_t comm, b200collStream_t stream);
 
+/* --- quantising collectives (src/quantized.cu): bf16, fp16 or fp32 in, block-scaled FP8 over NVLink, one kernel per call.
+ * Each rank quantises its own send buffer, cut into blocks of `block` consecutive elements, to wire_dtype (e4m3 or e5m2) with one fp32
+ * scale per block; peers pull the FP8 data and scales, dequantise in registers, sum in fp32 in rank order and store out_dtype.
+ * Per block, with x widened exactly to fp32 and FMAX = 448 (e4m3) or 57344 (e5m2):
+ *   amax = max |x| over the block (a NaN anywhere makes amax NaN)
+ *   inv = FMAX / amax, s = amax / FMAX     IEEE fp32 divisions rounded to nearest; inv = s = 1 if amax == 0 or inv is +inf
+ *   q = fp8_rne_satfinite(x * inv)         the product rounded to fp32 first; NaN stays NaN
+ *   v = float(q) * s                       one fp32 multiply, rounded to nearest even
+ * From there the block-scaled rules above apply, v_r being rank r's v:
+ *   all-reduce, reduce-scatter:  out = round_once(((0 + v_0) + v_1 + ... + v_{N-1}) * scale); sum or avg only (avg multiplies scale by
+ *                                the fp32 value 1/N)
+ *   all-gather:                  out[shard r] = round_once((0 + v_r) * scale)
+ * So a block holding +-inf or NaN comes out NaN in every element (q = 0 and s = inf, or NaN throughout), -0 comes out as +0, every rank
+ * holds bit-identical results (a rank's own all-gather shard is the round trip of its input, not a copy of it), one-shot and two-shot
+ * give the same bits, and one rank computes the same formula with N = 1 (a local round trip, counted as copy).
+ * Arguments (InvalidArgument unless noted, message in b200collGetLastError): ep->in_dtype and ep->out_dtype bf16, fp16 or fp32;
+ * wire_dtype e4m3 or e5m2; block 16, 32, 64, 128, 256 or 512; the per-rank count (reduce-scatter: recvcount) a multiple of block;
+ * send and recv 16-byte aligned. send may be any device buffer (only the local rank reads it). recv may be any device buffer; the
+ * two-shot all-reduce needs it in the arena (peers write into it) and falls back to one-shot otherwise, with the algorithm chosen as in
+ * b200collAllReduceBlockScaled (the tuner's pick for an FP8 all-reduce of count bytes), so recv must be placed alike on every rank.
+ * The all-reduce may run in place (send == recv, with in_dtype and out_dtype of one size); any other overlap of send and recv is refused.
+ * A poisoned communicator gives RemoteError.
+ * Scratch: the FP8 copy and its scales (count + 4 * count / block bytes per rank) live in a library-owned buffer taken from the symmetric
+ * heap with b200collMemAlloc on first use and grown on demand, so these calls are a collective contract like MemAlloc (same calls in the
+ * same order on every rank); OutOfMemory when the arena cannot hold it. A superseded scratch is kept until CommDestroy, so a CUDA graph
+ * captured before a later call grew the scratch stays valid.
+ * b200collStats count the input bytes (reduce-scatter: recvcount elements) under oneshot, twoshot or copy. At most 2^35 - 16 elements per rank. */
+/* recv holds nranks*sendcount elements of out_dtype; shard r is rank r's send buffer quantised and dequantised. */
+b200collResult_t b200collAllGatherQuantized(const void* send, void* recv, size_t sendcount, b200collDataType_t wire_dtype, int block,
+                                            const b200collEpilogue* ep, b200collComm_t comm, b200collStream_t stream);
+/* send holds nranks*recvcount elements; rank r receives the reduction of slice r. */
+b200collResult_t b200collReduceScatterQuantized(const void* send, void* recv, size_t recvcount, b200collDataType_t wire_dtype, int block,
+                                                const b200collEpilogue* ep, b200collRedOp_t op, b200collComm_t comm, b200collStream_t stream);
+b200collResult_t b200collAllReduceQuantized(const void* send, void* recv, size_t count, b200collDataType_t wire_dtype, int block,
+                                            const b200collEpilogue* ep, b200collRedOp_t op, b200collComm_t comm, b200collStream_t stream);
+
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.
  * AllReduceHost is the end-to-end step "pinned host -> GPU -> all-reduce -> pinned host" as one asynchronous call on `stream`:

@@ -53,6 +53,8 @@ struct Opts {
   std::vector<Shape> shapes;   // --sweep kind:ctas:threads,... (launch-shape tuning inside one process)
   int bs_rows = 0, bs_cols = 0;   // --block-scale RxC: block-scaled FP8 collectives (0 = off)
   size_t row_len = 2048;          // --row-len N: columns of the block-scaled matrix
+  int q_block = 0;                // --quantize WIRE:BLOCK: quantising collectives (0 = off)
+  b200collDataType_t q_wire = b200collFloat8e4m3;
 };
 
 // Block-scaled mode: each rank's send buffer is a [rows, row_len] FP8 matrix with one fp32 scale per bs_rows x bs_cols block. Scales are
@@ -77,6 +79,14 @@ static uint32_t got_bits(const void* p, size_t i, b200collDataType_t dt) {
   uint16_t u; memcpy(&u, (const char*)p + 2 * i, 2); return u;
 }
 
+// The library's quantisation scratch (FP8 copy plus scales per rank) grows with the sweep and keeps every superseded buffer: reserve
+// twice the largest one.
+static size_t q_scratch_bytes(const Opts& o) {
+  if (!o.q_block) return 0;
+  const size_t elems = o.max_bytes / b200collTypeSize(o.in_dt);
+  return 2 * (elems + elems / o.q_block * 4) + (4u << 20);
+}
+
 static size_t parse_size(const char* s) {
   char* end; double v = strtod(s, &end);
   if (*end == 'K' || *end == 'k') v *= 1024; else if (*end == 'M' || *end == 'm') v *= 1 << 20; else if (*end == 'G' || *end == 'g') v *= 1 << 30;
@@ -94,6 +104,35 @@ static const char* dt_name(b200collDataType_t t) { return t == b200collFloat32 ?
 
 // deterministic input: multiples of 0.25 in [-2, 2] (exact in e4m3 and e5m2 too) so sums over <= 8 ranks are exact in bf16/f16/f32
 static inline float gen(int rank, size_t i) { return (float)((int)((i * 7 + (size_t)rank * 13 + (i >> 9)) % 17) - 8) * 0.25f; }
+
+// Quantising mode: rank r's input element i is gen(r, i) times a power of two that changes from block to block (2^-6 .. 2^6, exact in
+// bf16, fp16 and fp32), so blocks have different amax values. The check repeats the library's per-block rule on the host (amax, two
+// IEEE divisions, RNE saturating pack, one multiply) and the rank-order fp32 sum, bit for bit.
+static float q_in(const Opts& o, int rank, size_t i) { return gen(rank, i) * ldexpf(1.0f, (int)(((i / o.q_block) * 5 + (size_t)rank * 3) % 13) - 6); }
+template <typename T> __global__ void k_fill_q(T* p, size_t n, int rank, int block) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float v = (float)((int)((i * 7 + (size_t)rank * 13 + (i >> 9)) % 17) - 8) * 0.25f;
+    p[i] = T(v * ldexpf(1.0f, (int)(((i / block) * 5 + (size_t)rank * 3) % 13) - 6));
+  }
+}
+// The dequantised value of rank r's element i; `memo` keeps the last block's (index, inv, s), as the check walks elements in order.
+struct QMemo { size_t blk = SIZE_MAX; float inv = 1.0f, s = 1.0f; };
+static float q_val(const Opts& o, int rank, size_t i, QMemo* memo) {
+  const size_t blk = i / o.q_block;
+  const float fmax = o.q_wire == b200collFloat8e4m3 ? 448.0f : 57344.0f;
+  if (memo->blk != blk) {
+    float amax = 0.0f;
+    for (size_t k = blk * o.q_block; k < (blk + 1) * o.q_block; k++) amax = std::max(amax, fabsf(q_in(o, rank, k)));
+    volatile float a = amax;                                     // keep both divisions as written: IEEE, rounded to nearest
+    float inv = fmax / a, s = a / fmax;
+    if (amax == 0.0f || isinf(inv)) inv = s = 1.0f;
+    *memo = QMemo{blk, inv, s};
+  }
+  const float y = q_in(o, rank, i) * memo->inv;
+  const __nv_fp8_interpretation_t I = o.q_wire == b200collFloat8e4m3 ? __NV_E4M3 : __NV_E5M2;
+  const __nv_fp8_storage_t q = __nv_cvt_float_to_fp8(y, __NV_SATFINITE, I);
+  return __half2float(__half(__nv_cvt_fp8_to_halfraw(q, I))) * memo->s;
+}
 
 template <typename T> __global__ void k_fill(T* p, size_t n, int rank, size_t base) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -176,7 +215,13 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
   void *send = nullptr, *recv = nullptr;
   CC(b200collMemAlloc(ctx.comm, &send, send_cap + 4096));
   CC(b200collMemAlloc(ctx.comm, &recv, recv_cap + 4096));
-  const bool bs_mode = o.bs_rows > 0;
+  const bool bs_mode = o.bs_rows > 0, q_mode = o.q_block > 0;
+  if (q_mode && ((o.op != "all_gather" && o.op != "reduce_scatter" && o.op != "all_reduce") || bs_mode ||
+                 (o.in_dt != b200collBfloat16 && o.in_dt != b200collFloat16 && o.in_dt != b200collFloat32) ||
+                 (o.out_dt != b200collBfloat16 && o.out_dt != b200collFloat16 && o.out_dt != b200collFloat32))) {
+    fprintf(stderr, "--quantize takes --op all_gather, reduce_scatter or all_reduce, -d and --out-dtype bfloat16|half|float, and no --block-scale\n");
+    return 2;
+  }
   float* scales = nullptr;
   std::vector<float> host_scales;
   if (bs_mode) {
@@ -191,6 +236,7 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
     printf("# b200coll_perf op=%s nranks=%d in=%s out=%s scale=%g algo=%s nvls=%d loopback=%d mode=%s\n", o.op.c_str(), n, dt_name(o.in_dt), dt_name(o.out_dt), o.scale, o.algo.c_str(),
            info.nvls, info.same_device_loopback, o.procs ? "procs" : "threads");
     if (bs_mode) printf("# block-scaled: row_len=%zu block=%dx%d (one fp32 scale per block, seeded)\n", o.row_len, o.bs_rows, o.bs_cols);
+    if (q_mode) printf("# quantised: wire=%s block=%d (each rank quantises its input, one fp32 scale per block)\n", dt_name(o.q_wire), o.q_block);
     printf("#%13s %12s %6s %8s | %10s %8s %8s %6s | %10s %8s %8s %6s\n", "size(B)", "count", "type", "algo", "oop us", "algbw", "busbw", "#wrong", "ip us", "algbw", "busbw", "#wrong");
     fflush(stdout);
   }
@@ -208,6 +254,7 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
     const size_t E = 16 / is;
     if (!is_ar) count = count / E * E;
     if (bs_mode) count = count / o.row_len * o.row_len;      // whole rows on every rank (reduce-scatter: rows = n * count / row_len)
+    if (q_mode) count = count / o.q_block * o.q_block;       // whole blocks on every rank (reduce-scatter: every slice)
     if (count == 0) continue;
     const size_t bs_rows_total = bs_mode ? (is_rs ? count * n : count) / o.row_len : 0;
     const size_t bs_ncb = bs_mode ? (o.row_len + o.bs_cols - 1) / o.bs_cols : 0;
@@ -232,6 +279,7 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
     for (int ip = 0; ip < 2; ip++) {
       if ((ip == 0 && o.inplace == 1) || (ip == 1 && o.inplace == 0)) continue;
       if (ip == 1 && (o.op == "alltoall" || is_sr || is_ga || is_sc || is != os)) continue;
+      if (ip == 1 && q_mode && !is_ar) continue;              // the quantising all-gather and reduce-scatter refuse overlapping buffers
       auto sbuf = [&](int slot) -> char* {
         char* base = ip ? (char*)recv : (char*)send;
         size_t off = (size_t)slot * slot_b;
@@ -270,6 +318,9 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
           CC(b200collRecv(rbuf(slot), count * is, (rank + n - 1) % n, ctx.comm, st));
           CC(b200collGroupEnd());
         }
+        else if (q_mode && is_ar) CC(b200collAllReduceQuantized(sbuf(slot), rbuf(slot), count, o.q_wire, o.q_block, &ep, b200collSum, ctx.comm, st));
+        else if (q_mode && is_ag) CC(b200collAllGatherQuantized(sbuf(slot), rbuf(slot), count, o.q_wire, o.q_block, &ep, ctx.comm, st));
+        else if (q_mode && is_rs) CC(b200collReduceScatterQuantized(sbuf(slot), rbuf(slot), count, o.q_wire, o.q_block, &ep, b200collSum, ctx.comm, st));
         else if (bs_mode && is_ar) CC(b200collAllReduceBlockScaled(sbuf(slot), rbuf(slot), count, &bsd, &ep, b200collSum, ctx.comm, st));
         else if (bs_mode && is_ag) CC(b200collAllGatherBlockScaled(sbuf(slot), rbuf(slot), count, &bsd, &ep, ctx.comm, st));
         else if (bs_mode && is_rs) CC(b200collReduceScatterBlockScaled(sbuf(slot), rbuf(slot), count, &bsd, &ep, b200collSum, ctx.comm, st));
@@ -284,7 +335,14 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
       long errs = 0;
       if (o.check) {
         if (!ip) RT(cudaMemsetAsync(rbuf(0), 0x5A, out_b, st));
-        if (ip && is_ag) fill(sbuf(0), in_elems, o.in_dt, rank, 0, st);
+        if (q_mode) {
+          void* p = sbuf(0);
+          if (o.in_dt == b200collFloat32) k_fill_q<float><<<256, 256, 0, st>>>((float*)p, in_elems, rank, o.q_block);
+          else if (o.in_dt == b200collFloat16) k_fill_q<__half><<<256, 256, 0, st>>>((__half*)p, in_elems, rank, o.q_block);
+          else k_fill_q<__nv_bfloat16><<<256, 256, 0, st>>>((__nv_bfloat16*)p, in_elems, rank, o.q_block);
+          RT(cudaGetLastError());
+        }
+        else if (ip && is_ag) fill(sbuf(0), in_elems, o.in_dt, rank, 0, st);
         else if (ip && is_rs) fill((char*)recv, in_elems, o.in_dt, rank, 0, st);
         else fill(sbuf(0), in_elems, o.in_dt, rank, 0, st);
         RT(cudaStreamSynchronize(st));
@@ -307,7 +365,15 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
           const uint32_t want = out_bits(acc * o.scale, o.out_dt), got = got_bits(host.data(), e, o.out_dt);
           if (got != want) { if (errs < 4) fprintf(stderr, "rank %d %s block-scaled size %zu elem %zu: got bits 0x%x want 0x%x\n", rank, o.op.c_str(), bytes, e, got, want); errs++; }
         }
-        for (size_t e = 0; e < check_elems && !bs_mode; e += stride) {
+        std::vector<QMemo> memo(n);
+        for (size_t e = 0; e < check_elems && q_mode; e += stride) {      // bit for bit: ((0 + v_0) + v_1 + ...) * scale, rounded once
+          float acc = 0.0f;
+          if (is_ag) acc += q_val(o, (int)(e / count), e % count, &memo[e / count]);
+          else for (int r = 0; r < n; r++) acc += q_val(o, r, is_rs ? (size_t)rank * count + e : e, &memo[r]);
+          const uint32_t want = out_bits(acc * o.scale, o.out_dt), got = got_bits(host.data(), e, o.out_dt);
+          if (got != want) { if (errs < 4) fprintf(stderr, "rank %d %s quantised size %zu %s elem %zu: got bits 0x%x want 0x%x\n", rank, o.op.c_str(), bytes, ip ? "ip" : "oop", e, got, want); errs++; }
+        }
+        for (size_t e = 0; e < check_elems && !bs_mode && !q_mode; e += stride) {
           const float want = expected(o, rank, n, e, count), got = to_f(host.data(), e, o.out_dt);
           // FP8 outputs round once: half an ulp is 2^-4 (e4m3) or 2^-3 (e5m2) of the value
           const float tol = o.out_dt == b200collFloat8e4m3 ? fabsf(want) * 0.0725f + 0.002f : o.out_dt == b200collFloat8e5m2 ? fabsf(want) * 0.135f + 0.002f : 0.0f;
@@ -419,6 +485,14 @@ int main(int argc, char** argv) {
     else if (a == "--out-dtype") o.out_dt = parse_dt(next());
     else if (a == "--block-scale") { if (sscanf(next(), "%dx%d", &o.bs_rows, &o.bs_cols) != 2 || o.bs_rows < 1 || o.bs_cols < 16 || o.bs_cols % 16) { fprintf(stderr, "--block-scale RxC: R >= 1, C a multiple of 16\n"); return 1; } }
     else if (a == "--row-len") o.row_len = (size_t)atoll(next());
+    else if (a == "--quantize") {
+      char wire[16] = {};
+      if (sscanf(next(), "%15[a-z0-9]:%d", wire, &o.q_block) != 2 || (strcmp(wire, "e4m3") && strcmp(wire, "e5m2")) || o.q_block < 16 || o.q_block > 512 ||
+          (o.q_block & (o.q_block - 1))) {
+        fprintf(stderr, "--quantize WIRE:BLOCK: WIRE e4m3 or e5m2, BLOCK 16, 32, 64, 128, 256 or 512\n"); return 1;
+      }
+      o.q_wire = parse_dt(wire);
+    }
     else if (a == "--scale") o.scale = (float)atof(next());
     else if (a == "--algo") o.algo = next();
     else if (a == "--iters" || a == "-n") o.iters = atoi(next());
@@ -449,6 +523,9 @@ int main(int argc, char** argv) {
            "  --block-scale RxC         block-scaled FP8 (all_gather, reduce_scatter, all_reduce): -d e4m3|e5m2 [R x C]-blocked matrices, one seeded\n"
            "                            fp32 scale per block, --out-dtype bfloat16|half|float; -c 1 checks bit for bit against the host\n"
            "  --row-len N               columns of the block-scaled matrix (default 2048; N and C multiples of 16)\n"
+           "  --quantize WIRE:BLOCK     quantising collectives (all_gather, reduce_scatter, all_reduce): -d bfloat16|half|float in, each rank\n"
+           "                            quantises to WIRE (e4m3|e5m2) with one fp32 scale per BLOCK (16..512) elements, --out-dtype bfloat16|half|float;\n"
+           "                            seeded inputs whose blocks differ in amax; -c 1 checks bit for bit against the host\n"
            "  --algo auto|ll|ll2|oneshot|twoshot|nvls   --inplace 0|1|2   --max-ctas N   --sweep kind:ctas:threads,...   --json FILE   --window SIZE\n"
            "  --selfcheck               report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;
@@ -474,7 +551,7 @@ int main(int argc, char** argv) {
     o.nranks = lr.size; o.procs = true;
     b200collConfig cfg; b200collConfigDefault(&cfg);
     const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
-    if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0);
+    if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o);
     b200collUniqueId id; CC(b200collUniqueIdFromString(("perf/" + lr.job).c_str(), &id));
     RT(cudaSetDevice(dev));
     b200collComm_t comm;
@@ -502,7 +579,7 @@ int main(int argc, char** argv) {
   b200collConfig cfg; b200collConfigDefault(&cfg);
   // arena: two windows (+ max buffers) and slack
   const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
-  size_t need = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0);
+  size_t need = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o);
   if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = need;
   if (o.procs) {
     b200collUniqueId id; CC(b200collGetUniqueId(&id));

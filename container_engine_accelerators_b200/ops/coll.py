@@ -132,6 +132,9 @@ def load() -> C.CDLL:
     L.b200collAllGatherBlockScaled.argtypes = [vp, vp, sz, C.POINTER(BlockScale), C.POINTER(Epilogue), vp, vp]
     L.b200collReduceScatterBlockScaled.argtypes = [vp, vp, sz, C.POINTER(BlockScale), C.POINTER(Epilogue), ci, vp, vp]
     L.b200collAllReduceBlockScaled.argtypes = [vp, vp, sz, C.POINTER(BlockScale), C.POINTER(Epilogue), ci, vp, vp]
+    L.b200collAllGatherQuantized.argtypes = [vp, vp, sz, ci, ci, C.POINTER(Epilogue), vp, vp]
+    L.b200collReduceScatterQuantized.argtypes = [vp, vp, sz, ci, ci, C.POINTER(Epilogue), ci, vp, vp]
+    L.b200collAllReduceQuantized.argtypes = [vp, vp, sz, ci, ci, C.POINTER(Epilogue), ci, vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -223,6 +226,45 @@ def check_block_scaled(op: str, nranks: int, q, scales, out, block=(1, 128)) -> 
     if tuple(out.shape) != out_shape:
         raise ValueError(f"{op}: out must have shape {out_shape}, got {tuple(out.shape)}")
     return br, bc
+
+
+QUANT_BLOCKS = (16, 32, 64, 128, 256, 512)
+
+
+def check_quantized(op: str, nranks: int, src, out, block: int = 128, wire=None) -> int:
+    """Rules of the quantising collectives ("all_gather", "reduce_scatter", "all_reduce"), checked on the tensors' metadata only (no
+    communicator, no library call): raises ValueError, returns the wire type's library code. src and out: contiguous bfloat16, float16
+    or float32; wire: torch.float8_e4m3fn (default) or torch.float8_e5m2; block one of QUANT_BLOCKS. out has nranks * src.numel()
+    elements for all-gather, src.numel() / nranks for reduce-scatter and src.numel() for all-reduce, and every rank's share is whole
+    blocks. Only the all-reduce may run in place (out is src, or a tensor with the same data pointer and element size)."""
+    import torch
+    wire = torch.float8_e4m3fn if wire is None else wire
+    if op not in ("all_gather", "reduce_scatter", "all_reduce"):
+        raise ValueError(f"unknown quantised op {op!r}")
+    wide = (torch.bfloat16, torch.float16, torch.float32)
+    if src.dtype not in wide or not src.is_contiguous():
+        raise ValueError(f"src must be a contiguous bfloat16, float16 or float32 tensor, got {src.dtype}")
+    if out.dtype not in wide or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous bfloat16, float16 or float32 tensor, got {out.dtype}")
+    if wire not in (torch.float8_e4m3fn, torch.float8_e5m2):
+        raise ValueError(f"wire must be torch.float8_e4m3fn or torch.float8_e5m2, not {wire}")
+    if isinstance(block, bool) or not isinstance(block, int) or block not in QUANT_BLOCKS:
+        raise ValueError(f"block must be one of {QUANT_BLOCKS}, got {block!r}")
+    n = src.numel()
+    if op == "reduce_scatter" and n % nranks:
+        raise ValueError(f"reduce_scatter: src.numel() ({n}) must be a multiple of nranks ({nranks})")
+    want = {"all_gather": nranks * n, "reduce_scatter": n // nranks, "all_reduce": n}[op]
+    if out.numel() != want:
+        raise ValueError(f"{op}: out must have {want} elements, got {out.numel()}")
+    share = n // nranks if op == "reduce_scatter" else n
+    if share % block:
+        raise ValueError(f"{op}: {'the per-rank slice' if op == 'reduce_scatter' else 'src.numel()'} ({share}) must be a multiple of block ({block})")
+    a, na = src.data_ptr(), n * src.element_size()
+    b, nb = out.data_ptr(), out.numel() * out.element_size()
+    in_place = op == "all_reduce" and a == b and src.element_size() == out.element_size()
+    if n and not in_place and a < b + nb and b < a + na:
+        raise ValueError(f"{op}: out must not overlap src" + (" (in place needs out to be src, with a dtype of the same size)" if op == "all_reduce" else ""))
+    return torch_dtype_code(wire)
 
 
 class _CudaArray:
@@ -474,6 +516,35 @@ class Comm:
     def all_reduce_block_scaled(self, q, scales, out, block=(1, 128), scale: float = 1.0, op: int = SUM, stream=None):
         """out = round(scale * sum over ranks, in rank order, of dequant(q)); op SUM or AVG; out (rows, row_len). Two-shot needs out in the arena."""
         return self._block_scaled("AllReduceBlockScaled", load().b200collAllReduceBlockScaled, "all_reduce", q, scales, out, block, scale, (op,), q.numel(), stream)
+
+    def all_gather_quantized(self, src, out, block: int = 128, wire=None, scale: float = 1.0, stream=None):
+        """out[r-th shard] = round(scale * dequant(quant(src of rank r))): src (bf16, fp16 or fp32, any device tensor) is quantised on
+        this rank to `wire` FP8 with one fp32 scale per `block` elements, and FP8 and scales cross NVLink (b200collAllGatherQuantized).
+        out: bf16, fp16 or fp32 with nranks * src.numel() elements. The scratch comes from the arena: the same calls on every rank."""
+        w = check_quantized("all_gather", self.nranks, src, out, block, wire)
+        ep = self._ep(src, out, scale)
+        _check(load().b200collAllGatherQuantized(C.c_void_p(src.data_ptr()), C.c_void_p(out.data_ptr()), src.numel(), w, block, C.byref(ep), self._h,
+                                                 self._stream(stream)), "AllGatherQuantized")
+        return out
+
+    def reduce_scatter_quantized(self, src, out, block: int = 128, wire=None, scale: float = 1.0, op: int = SUM, stream=None):
+        """out = round(scale * sum over ranks, in rank order, of dequant(quant(slice `rank` of src))); op SUM or AVG; out has
+        src.numel() / nranks elements, a multiple of block."""
+        w = check_quantized("reduce_scatter", self.nranks, src, out, block, wire)
+        ep = self._ep(src, out, scale)
+        _check(load().b200collReduceScatterQuantized(C.c_void_p(src.data_ptr()), C.c_void_p(out.data_ptr()), out.numel(), w, block, C.byref(ep), op, self._h,
+                                                     self._stream(stream)), "ReduceScatterQuantized")
+        return out
+
+    def all_reduce_quantized(self, src, out=None, block: int = 128, wire=None, scale: float = 1.0, op: int = SUM, stream=None):
+        """out = round(scale * sum over ranks, in rank order, of dequant(quant(src))); op SUM or AVG; out=None runs in place. Two-shot
+        needs out in the arena (`empty()`), else the call runs one-shot."""
+        out = src if out is None else out
+        w = check_quantized("all_reduce", self.nranks, src, out, block, wire)
+        ep = self._ep(src, out, scale)
+        _check(load().b200collAllReduceQuantized(C.c_void_p(src.data_ptr()), C.c_void_p(out.data_ptr()), src.numel(), w, block, C.byref(ep), op, self._h,
+                                                 self._stream(stream)), "AllReduceQuantized")
+        return out
 
     def all_to_all(self, src, dst, scale: float = 1.0, stream=None):
         ep = self._ep(src, dst, scale)
