@@ -228,7 +228,7 @@ b200collResult_t b200collReduce(const void* send, void* recv, size_t count, cons
                                 b200collRedOp_t op, int root, b200collComm_t comm, b200collStream_t stream);
 b200collResult_t b200collBarrier(b200collComm_t comm, b200collStream_t stream);
 
-/* --- block-scaled FP8 (src/blockscaled.cu): per-block dequantisation fused into all-gather, reduce-scatter and all-reduce.
+/* --- block-scaled FP8 (src/blockscaled.cu, with the quantising collectives below): per-block dequantisation fused into all-gather, reduce-scatter and all-reduce.
  * Each rank's send buffer is a row-major matrix [rows, row_len] of e4m3 or e5m2 (rows = count / row_len) with one fp32 scale per
  * block_rows x block_cols block of THAT rank's matrix: ceil(rows / block_rows) x ceil(row_len / block_cols) scales, row-major, the last
  * block row and column may be partial. Element (i, j) of rank r has the value v = float(q) * s[i / block_rows][j / block_cols] (one fp32
@@ -263,7 +263,7 @@ b200collResult_t b200collReduceScatterBlockScaled(const void* send, void* recv, 
 b200collResult_t b200collAllReduceBlockScaled(const void* send, void* recv, size_t count, const b200collBlockScale* bs,
                                               const b200collEpilogue* ep, b200collRedOp_t op, b200collComm_t comm, b200collStream_t stream);
 
-/* --- quantising collectives (src/quantized.cu): bf16, fp16 or fp32 in, block-scaled FP8 over NVLink, one kernel per call.
+/* --- quantising collectives (src/blockscaled.cu, sharing the block-scaled pull): bf16, fp16 or fp32 in, block-scaled FP8 over NVLink, one kernel per call.
  * Each rank quantises its own send buffer, cut into blocks of `block` consecutive elements, to wire_dtype (e4m3 or e5m2) with one fp32
  * scale per block; peers pull the FP8 data and scales, dequantise in registers, sum in fp32 in rank order and store out_dtype.
  * Per block, with x widened exactly to fp32 and FMAX = 448 (e4m3) or 57344 (e5m2):

@@ -1,6 +1,9 @@
-// libb200coll block-scaled FP8 collectives: e4m3 / e5m2 matrices with one fp32 scale per block_rows x block_cols block (1x128 activation
-// and gradient blocks, 128x128 weight blocks), dequantised in registers and delivered as bf16, fp16 or fp32. FP8 crosses NVLink, the
-// wider type is only ever written locally (or, in the two-shot all-reduce, pushed once as the finished result):
+// libb200coll block-scaled FP8 collectives, in two families that share one pull-and-dequantise core. FP8 and fp32 block scales cross
+// NVLink; receivers pull them from every peer, dequantise in registers, sum in fp32 in rank order, round once and store bf16, fp16 or
+// fp32 locally (or, in the two-shot all-reduce, push the finished result once).
+//
+// Block-scaled: e4m3 / e5m2 matrices with one fp32 scale per block_rows x block_cols block (1x128 activation and gradient blocks,
+// 128x128 weight blocks), written by the caller into the arena:
 //
 //   k_bsq_ag_pull<InT, OutT>              all-gather: barrier, pull every rank's FP8 shard and scales, dequantise, store locally, barrier
 //   k_bsq_pull_reduce<InT, OutT, false>   reduce-scatter (my row slice) / one-shot all-reduce (whole matrix): pull from every rank in
@@ -8,15 +11,48 @@
 //   k_bsq_pull_reduce<InT, OutT, true>    two-shot all-reduce: the same over my vector slice, the result pushed into every rank's recv
 //   k_bsq_copy<InT, OutT>                 one rank: local dequantising copy, no barrier
 //
-// Scales: a 16-byte FP8 vector lies in exactly one block (row_len and block_cols are multiples of 16), so a vector needs one scale per
-// rank. Lanes of a warp hold consecutive vectors and usually share scales (8 lanes per 1x128 block, whole warps per 128x128 block):
-// __match_any_sync groups the lanes by scale index, the lowest lane of each group loads the scale and __shfl_sync hands it to the rest,
-// so each distinct scale is read once per warp and rank. The vector -> (row, column) -> block arithmetic is 32-bit multiply-high
-// division by host-computed constants: no integer division in the loops.
+// Quantising: bf16, fp16 or fp32 in, one kernel per call. Each rank quantises its own send buffer to e4m3 / e5m2 with one fp32 scale
+// per `block` consecutive elements, into a library-owned symmetric scratch; from there the block-scaled pull applies:
+//
+//   k_quant_ag<InT, WireT, OutT>                  all-gather: quantise my shard, barrier, pull and dequantise every rank's shard, barrier
+//   k_quant_pull_reduce<InT, WireT, OutT, false>  reduce-scatter (my slice) / one-shot all-reduce (whole buffer): quantise, barrier,
+//                                                 pull from every rank in rank order, sum in fp32, scale, round once, store locally
+//   k_quant_pull_reduce<InT, WireT, OutT, true>   two-shot all-reduce: the same over my block slice, the result pushed into every recv
+//   k_quant_copy<InT, WireT, OutT>                one rank: the quantise / dequantise round trip in registers, no scratch, no barrier
+//
+// Scales: a 16-byte FP8 vector lies in exactly one block (row_len and block_cols are multiples of 16; a quantising block is a whole
+// number of vectors), so a vector needs one scale per rank. Lanes of a warp hold consecutive vectors and usually share scales (8 lanes
+// per 1x128 block, whole warps per 128x128 block): __match_any_sync groups the lanes by scale index, the lowest lane of each group loads
+// the scale and __shfl_sync hands it to the rest, so each distinct scale is read once per warp and rank. Each family's geometry maps a
+// vector to its scale: the block-scaled vector -> (row, column) -> block arithmetic is 32-bit multiply-high division by host-computed
+// constants (no integer division in the loops), a quantising block is a shift.
+//
+// Quantising, per block: amax = max |x| (the largest unsigned bit pattern of |x|, so a NaN anywhere makes amax NaN); inv = FMAX / amax
+// and s = amax / FMAX, both IEEE divisions rounded to nearest, inv = s = 1 when amax == 0 or inv overflows; q = fp8_satfinite(x * inv);
+// the dequantised value is float(q) * s. FMAX is 448 (e4m3) or 57344 (e5m2).
+//
+// Fusing the quantise phase into the pull kernel is sound because of three properties, which the code below keeps:
+//   * Same-index CTAs only. The epoch barrier orders CTA b of this rank against CTA b of every peer, nothing else. Every vector loop in
+//     this file is warp_walk, so the quantise loop walks each rank-slice exactly as the pull loop walks it (same grid, same start per slice,
+//     same stride): every vector CTA b pulls from a peer after the barrier was quantised by CTA b on that peer before it. All-gather
+//     walks the whole shard; reduce-scatter and two-shot walk each of the N slices in turn; one-shot walks the whole buffer once.
+//   * Blocks stay inside one warp iteration. block is a power of two from 16 to 512 elements (1 to 32 vectors), a warp's first vector
+//     is the slice start plus a multiple of 32, and slice starts and ends fall on whole blocks (the two-shot slices are cut at
+//     nblk*r/N blocks, not nvec*r/N vectors). So the lanes of one block are consecutive lanes of one warp, all active or all idle, and
+//     the amax is a butterfly over those lanes: no shared memory, no cross-warp step.
+//   * The first barrier releases. The block-scaled kernels take it relaxed because their inputs were written by earlier kernels; here
+//     this CTA's own scratch stores must be visible to the peers that pull them, so it is barrier_blocks<true>.
+// The same argument makes the in-place all-reduce safe on both algorithms: vector v of send is read only by the CTA that walks it, and
+// is overwritten (by that CTA locally in one-shot, by CTA b of the slice owner in two-shot) only after that CTA has passed the first
+// barrier, which follows the read.
+//
+// The final barrier keeps the scratch safe to reuse: no rank's kernel ends before every peer's CTAs have finished pulling from it.
 #include <limits.h>
+#include <math.h>
 #include <stdint.h>
 
-#include "blockscale.cuh"
+#include <type_traits>
+
 #include "comm.h"
 #include "launch.cuh"
 
@@ -28,90 +64,137 @@ using e5m2 = __nv_fp8_e5m2;
 
 constexpr int kBsqThreads = 512;
 
-// What every kernel needs to find vector v of a rank's send matrix and its scale. Vector indices are 32-bit (the host refuses larger).
+// q = floor(n / d) for every 32-bit n as (umulhi(n, m) + n) >> l, l = ceil(log2 d), m = floor(2^32 (2^l - d) / d) + 1 (Granlund and
+// Montgomery, "Division by invariant integers using multiplication", 1994). The sum needs 33 bits, so it is formed in 64.
+struct FastDiv {
+  uint32_t d, m, l;
+  __device__ __forceinline__ uint32_t div(uint32_t n) const { return (uint32_t)(((unsigned long long)__umulhi(n, m) + n) >> l); }
+};
+inline FastDiv make_fastdiv(uint32_t d) {
+  uint32_t l = 0;
+  while (l < 32 && (1ull << l) < d) l++;
+  return FastDiv{d, (uint32_t)(((1ull << 32) * ((1ull << l) - d)) / d + 1), l};
+}
+
+// What every kernel needs to find vector v of a rank's FP8 data and its scale. Vector indices are 32-bit (the host refuses larger).
 struct BsqGeom {
-  size_t send_off, scale_off;     // arena offsets of the FP8 matrix and of its scales (the same on every rank)
+  size_t data_off, scale_off;     // arena offsets of the caller's FP8 matrix and of its scales (the same on every rank)
   uint32_t nvec;                  // 16-element vectors in one rank's matrix
   uint32_t ncb;                   // block columns (scales per block row)
   FastDiv vpr, br, vpb;           // vectors per row, rows per block, vectors per block column
+  __device__ __forceinline__ uint32_t scale_index(uint32_t v) const {
+    const uint32_t row = vpr.div(v), cv = v - row * vpr.d;
+    return br.div(row) * ncb + vpb.div(cv);
+  }
 };
 
-__device__ __forceinline__ uint32_t bsq_scale_index(const BsqGeom& g, uint32_t v) {
-  const uint32_t row = g.vpr.div(v), cv = v - row * g.vpr.d;
-  return g.br.div(row) * g.ncb + g.vpb.div(cv);
+struct QuantGeom {
+  size_t data_off, scale_off;     // arena offsets of the scratch FP8 copy and of its scales (the same on every rank)
+  uint32_t nvec;                  // 16-element vectors in one rank's send buffer
+  uint32_t nblk;                  // blocks in one rank's send buffer
+  uint32_t lvpb;                  // log2(vectors per block)
+  __device__ __forceinline__ uint32_t scale_index(uint32_t v) const { return v >> lvpb; }
+};
+
+// The one walk over vectors [v0, v1): a warp takes 32 consecutive vectors starting at v0 plus a multiple of 32, the grid strides
+// over the range, and all 32 lanes run every iteration (f(v, active), active = v < v1), so the full-mask warp intrinsics below always
+// see whole warps. 32-bit indices: the host keeps nvec below 2^31, so b + stride cannot wrap.
+template <typename F>
+__device__ __forceinline__ void warp_walk(uint32_t v0, uint32_t v1, F&& f) {
+  const uint32_t lane = threadIdx.x & 31;
+  for (uint32_t b = v0 + blockIdx.x * blockDim.x + (threadIdx.x & ~31u); b < v1; b += gridDim.x * blockDim.x) f(b + lane, b + lane < v1);
 }
 
-// Dequantise vectors [0, nvec) of one rank's matrix into dst. Loops run on the warp's first vector so that whole warps stay together
-// for the scale exchange.
-template <typename InT, typename OutT>
-__device__ __forceinline__ void bsq_dequant_range(const BsqGeom& g, const char* src, const char* scales, OutT* dst, float scale) {
-  const uint32_t lane = threadIdx.x & 31;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t b = (size_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); b < g.nvec; b += stride) {
-    const size_t v = b + lane;
-    const bool act = v < g.nvec;
-    uint4 q = make_uint4(0, 0, 0, 0);
-    if (act) q = ld_vec(src + v * 16);
-    const uint32_t idx = act ? bsq_scale_index(g, (uint32_t)v) : 0u;
-    const WarpScale ws(idx, act);
-    const float s = ws.get(scales, idx);
-    if (act) {
-      float acc[16] = {};
-      bsq_dequant_add<InT>(acc, q, s);
-      bsq_store<OutT>(dst + v * 16, acc, scale);
+// The scale of every lane's vector, one load per distinct index in the warp. All 32 lanes call it; `active` lanes have a vector.
+struct WarpScale {
+  unsigned leader;
+  bool loads;
+  __device__ __forceinline__ WarpScale(uint32_t idx, bool active) {
+    const unsigned same = __match_any_sync(0xFFFFFFFFu, active ? idx : 0xFFFFFFFFu);
+    leader = __ffs(same) - 1;
+    loads = active && (threadIdx.x & 31) == leader;
+  }
+  __device__ __forceinline__ float get(const char* scales, uint32_t idx) const {
+    float s = 0.f;
+    if (loads) s = *reinterpret_cast<const float*>(scales + (size_t)idx * 4);
+    return __shfl_sync(0xFFFFFFFFu, s, leader);
+  }
+};
+
+// acc[i] += float(q[i]) * s, both roundings kept (no fused multiply-add): the value of an element is the rounded product.
+template <typename WireT> __device__ __forceinline__ void bsq_dequant_add(float* acc, const uint4& v, float s) {
+  constexpr __nv_fp8_interpretation_t I = std::is_same<WireT, __nv_fp8_e4m3>::value ? __NV_E4M3 : __NV_E5M2;
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const __half2_raw r = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w[i] >> (16 * h)), I);   // F2FP.F16.E4M3 / E5M2.UNPACK_B
+      const float2 f = __half22float2(__half2(r));
+      acc[4 * i + 2 * h] = __fadd_rn(acc[4 * i + 2 * h], __fmul_rn(f.x, s));
+      acc[4 * i + 2 * h + 1] = __fadd_rn(acc[4 * i + 2 * h + 1], __fmul_rn(f.y, s));
     }
   }
 }
 
-template <typename InT, typename OutT>
-__global__ void __launch_bounds__(kBsqThreads) k_bsq_copy(const __grid_constant__ BsqGeom g, const char* __restrict__ in, const char* __restrict__ scales,
-                                                       OutT* __restrict__ out, float scale) {
-  pdl_prologue();
-  bsq_dequant_range<InT, OutT>(g, in, scales, out, scale);
+// out = round_once(acc * scale): 16 elements, 32 (bf16 / fp16) or 64 (fp32) bytes
+template <typename OutT> __device__ __forceinline__ void bsq_store(void* dst, const float* acc, float scale) {
+  constexpr int W = Pack<OutT, 16>::W;
+  float f[16];
+#pragma unroll
+  for (int i = 0; i < 16; i++) f[i] = __fmul_rn(acc[i], scale);
+  uint32_t w[W];
+  Pack<OutT, 16>::run(f, w);
+  if constexpr (W == 16) {
+#pragma unroll
+    for (int k = 0; k < 4; k++) st_vec(reinterpret_cast<char*>(dst) + 16 * k, make_uint4(w[4 * k], w[4 * k + 1], w[4 * k + 2], w[4 * k + 3]));
+  } else {
+    st_words<W>(dst, w);
+  }
 }
 
-// out holds nranks shards of nvec*16 elements; shard r is rank r's matrix dequantised with rank r's scales
-template <typename InT, typename OutT>
-__global__ void __launch_bounds__(kBsqThreads) k_bsq_ag_pull(COMM_PARAM, const __grid_constant__ BsqGeom g, OutT* __restrict__ out, float scale, uint32_t op) {
-  pdl_prologue();
-  const uint32_t s = load_seq(c, kSeqBarrier);
-  if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;          // every rank's shard and scales are written
+// Dequantise vectors [0, nvec) of one rank's FP8 data into dst.
+template <typename WireT, typename OutT, typename Geom>
+__device__ __forceinline__ void dequant_range(const Geom& g, const char* src, const char* scales, OutT* dst, float scale) {
+  warp_walk(0, g.nvec, [&](uint32_t v, bool act) {
+    uint4 q = make_uint4(0, 0, 0, 0);
+    if (act) q = ld_vec(src + (size_t)v * 16);
+    const uint32_t idx = act ? g.scale_index(v) : 0u;
+    const WarpScale ws(idx, act);
+    const float s = ws.get(scales, idx);
+    if (act) {
+      float acc[16] = {};
+      bsq_dequant_add<WireT>(acc, q, s);
+      bsq_store<OutT>(dst + (size_t)v * 16, acc, scale);
+    }
+  });
+}
+
+// All-gather: out holds nranks shards of nvec*16 elements; shard r is rank r's FP8 data dequantised with rank r's scales
+template <typename WireT, typename OutT, typename Geom>
+__device__ __forceinline__ void ag_pull(const CommDev& c, const Geom& g, OutT* out, float scale) {
   for (int j = 0; j < c.nranks; j++) {                          // peers visited starting with myself: spreads the pulls over the links
     int r = c.rank + j; if (r >= c.nranks) r -= c.nranks;
-    bsq_dequant_range<InT, OutT>(g, c.peer[r] + g.send_off, c.peer[r] + g.scale_off, out + (size_t)r * g.nvec * 16, scale);
+    dequant_range<WireT, OutT>(g, c.peer[r] + g.data_off, c.peer[r] + g.scale_off, out + (size_t)r * g.nvec * 16, scale);
   }
-  if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // nobody reads my shard any more: I may overwrite it
-  if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
 }
 
 // Vectors [v0, v1) summed over ranks in rank order: acc = ((0 + v_0) + v_1 + ...), then round_once(acc * scale).
 // PUSH=false: stored at out_local[(v - v0) * 16] (reduce-scatter: my slice; one-shot all-reduce: v0 = 0, v1 = nvec).
 // PUSH=true: stored at arena offset out_off + v * 16 * sizeof(OutT) of every rank (two-shot all-reduce, my vector slice).
-// One 512-thread CTA per SM, like the other P2P reduction kernels (k_pull_reduce, k_ar_twoshot: about 100 registers): with eight pulled
-// vectors and 16 accumulators live, squeezing the kernel into the 64 registers of two CTAs per SM made ptxas spill the loop state.
-template <typename InT, typename OutT, bool PUSH>
-__global__ void __launch_bounds__(kBsqThreads, 1) k_bsq_pull_reduce(COMM_PARAM, const __grid_constant__ BsqGeom g, OutT* __restrict__ out_local, size_t out_off,
-                                                              uint32_t v0, uint32_t v1, float scale, uint32_t op) {
-  pdl_prologue();
-  {
-    const uint32_t s = load_seq(c, kSeqBarrier);
-    if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;
-  }
-  // 32-bit vector indices: the host keeps nvec below 2^31, so b + stride cannot wrap
-  const uint32_t lane = threadIdx.x & 31;
-  for (uint32_t b = v0 + blockIdx.x * blockDim.x + (threadIdx.x & ~31u); b < v1; b += gridDim.x * blockDim.x) {
-    const uint32_t v = b + lane;
-    const bool act = v < v1;
+template <typename WireT, typename OutT, bool PUSH, typename Geom>
+__device__ __forceinline__ void pull_reduce_range(const CommDev& c, const Geom& g, OutT* out_local, size_t out_off, uint32_t v0, uint32_t v1, float scale) {
+  warp_walk(v0, v1, [&](uint32_t v, bool act) {
     uint4 d[kMaxRanks];
 #pragma unroll
-    for (int r = 0; r < kMaxRanks; r++) if (r < c.nranks) d[r] = act ? ld_vec(c.peer[r] + g.send_off + (size_t)v * 16) : make_uint4(0, 0, 0, 0);
-    const uint32_t idx = act ? bsq_scale_index(g, v) : 0u;
+    for (int r = 0; r < kMaxRanks; r++) if (r < c.nranks) d[r] = act ? ld_vec(c.peer[r] + g.data_off + (size_t)v * 16) : make_uint4(0, 0, 0, 0);
+    const uint32_t idx = act ? g.scale_index(v) : 0u;
     const WarpScale ws(idx, act);
     float acc[16] = {};
 #pragma unroll
     for (int r = 0; r < kMaxRanks; r++) if (r < c.nranks) {
       const float sr = ws.get(c.peer[r] + g.scale_off, idx);
-      bsq_dequant_add<InT>(acc, d[r], sr);
+      bsq_dequant_add<WireT>(acc, d[r], sr);
     }
     if (act) {
       if (PUSH) {
@@ -124,90 +207,286 @@ __global__ void __launch_bounds__(kBsqThreads, 1) k_bsq_pull_reduce(COMM_PARAM, 
         bsq_store<OutT>(out_local + (size_t)(v - v0) * 16, acc, scale);
       }
     }
+  });
+}
+
+// Block-scaled kernels.
+template <typename InT, typename OutT>
+__global__ void __launch_bounds__(kBsqThreads) k_bsq_copy(const __grid_constant__ BsqGeom g, const char* __restrict__ in, const char* __restrict__ scales,
+                                                       OutT* __restrict__ out, float scale) {
+  pdl_prologue();
+  dequant_range<InT, OutT>(g, in, scales, out, scale);
+}
+
+template <typename InT, typename OutT>
+__global__ void __launch_bounds__(kBsqThreads) k_bsq_ag_pull(COMM_PARAM, const __grid_constant__ BsqGeom g, OutT* __restrict__ out, float scale, uint32_t op) {
+  pdl_prologue();
+  const uint32_t s = load_seq(c, kSeqBarrier);
+  if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;          // every rank's shard and scales are written
+  ag_pull<InT, OutT>(c, g, out, scale);
+  if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // nobody reads my shard any more: I may overwrite it
+  if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
+}
+
+// One 512-thread CTA per SM, like the other P2P reduction kernels (k_pull_reduce, k_ar_twoshot: about 100 registers): with eight pulled
+// vectors and 16 accumulators live, squeezing the kernel into the 64 registers of two CTAs per SM made ptxas spill the loop state.
+template <typename InT, typename OutT, bool PUSH>
+__global__ void __launch_bounds__(kBsqThreads, 1) k_bsq_pull_reduce(COMM_PARAM, const __grid_constant__ BsqGeom g, OutT* __restrict__ out_local, size_t out_off,
+                                                              uint32_t v0, uint32_t v1, float scale, uint32_t op) {
+  pdl_prologue();
+  {
+    const uint32_t s = load_seq(c, kSeqBarrier);
+    if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;
   }
+  pull_reduce_range<InT, OutT, PUSH>(c, g, out_local, out_off, v0, v1, scale);
   // the sequence number is read again rather than kept live across the loop: only the last block, after the barrier below, bumps it
   const uint32_t s = load_seq(c, kSeqBarrier);
   if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;
   if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
 }
 
-// ------------------------------------------------------------------------------------------------ host side
-template <typename T> struct Tag { using type = T; };
+// Quantising kernels.
+template <typename WireT> constexpr float kWireMax = 448.0f;
+template <> constexpr float kWireMax<__nv_fp8_e5m2> = 57344.0f;
 
+// the first vector of slice s of n: slices are cut at whole blocks
+__device__ __forceinline__ uint32_t quant_slice_start(const QuantGeom& g, uint32_t s, uint32_t n) {
+  return (uint32_t)((unsigned long long)g.nblk * s / n) << g.lvpb;
+}
+
+// 16 elements of InT at p, widened (exactly) to fp32
+template <typename InT> __device__ __forceinline__ void quant_load16(const char* p, float* x) {
+  if constexpr (std::is_same<InT, float>::value) {
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+      const uint4 v = ld_vec(p + 16 * k);
+      x[4 * k] = __uint_as_float(v.x); x[4 * k + 1] = __uint_as_float(v.y); x[4 * k + 2] = __uint_as_float(v.z); x[4 * k + 3] = __uint_as_float(v.w);
+    }
+  } else {
+#pragma unroll
+    for (int k = 0; k < 2; k++) {
+      const uint4 v = ld_vec(p + 16 * k);
+      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int i = 0; i < 4; i++) {
+        if constexpr (std::is_same<InT, __nv_bfloat16>::value) {
+          x[8 * k + 2 * i] = __uint_as_float(w[i] << 16); x[8 * k + 2 * i + 1] = __uint_as_float(w[i] & 0xFFFF0000u);
+        } else {
+          const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
+          x[8 * k + 2 * i] = f.x; x[8 * k + 2 * i + 1] = f.y;
+        }
+      }
+    }
+  }
+}
+
+// Quantise this lane's 16 elements with the amax of its block, whose vectors are held by the aligned group of `gl` lanes (a power of
+// two up to 32) this lane belongs to. All 32 lanes call it; idle lanes pass zeros, and their groups are wholly idle. Returns the FP8
+// vector; *scale receives s.
+template <typename WireT> __device__ __forceinline__ uint4 quant_vec(const float* x, uint32_t gl, float* scale) {
+  uint32_t m = 0;
+#pragma unroll
+  for (int i = 0; i < 16; i++) m = max(m, __float_as_uint(x[i]) & 0x7FFFFFFFu);
+  for (uint32_t o = 1; o < gl; o <<= 1) m = max(m, __shfl_xor_sync(0xFFFFFFFFu, m, o));
+  const float amax = __uint_as_float(m);
+  float inv = __fdiv_rn(kWireMax<WireT>, amax), s = __fdiv_rn(amax, kWireMax<WireT>);
+  if (amax == 0.0f || inv == INFINITY) { inv = 1.0f; s = 1.0f; }
+  float y[16];
+#pragma unroll
+  for (int i = 0; i < 16; i++) y[i] = __fmul_rn(x[i], inv);
+  uint32_t w[4];
+  Pack<WireT, 16>::run(y, w);                                     // cvt.rn.satfinite: F2FP.SATFINITE.E4M3 / .E5M2
+  *scale = s;
+  return make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+// Quantise vectors [v0, v1) of my send buffer into my scratch, walked as the pull loops walk a slice.
+template <typename InT, typename WireT>
+__device__ __forceinline__ void quant_range(const QuantGeom& g, const char* in, char* q, char* scales, uint32_t v0, uint32_t v1) {
+  const uint32_t lane = threadIdx.x & 31, gl = 1u << g.lvpb;
+  warp_walk(v0, v1, [&](uint32_t v, bool act) {
+    float x[16] = {};
+    if (act) quant_load16<InT>(in + (size_t)v * (16 * sizeof(InT)), x);
+    float s;
+    const uint4 w = quant_vec<WireT>(x, gl, &s);
+    if (act) {
+      st_vec(q + (size_t)v * 16, w);
+      if ((lane & (gl - 1)) == 0) *reinterpret_cast<float*>(scales + (size_t)g.scale_index(v) * 4) = s;
+    }
+  });
+}
+
+template <typename InT, typename WireT, typename OutT>
+__global__ void __launch_bounds__(kBsqThreads) k_quant_copy(const char* in, OutT* out, uint32_t nvec, uint32_t lvpb, float scale) {
+  pdl_prologue();
+  const uint32_t gl = 1u << lvpb;
+  warp_walk(0, nvec, [&](uint32_t v, bool act) {
+    float x[16] = {};
+    if (act) quant_load16<InT>(in + (size_t)v * (16 * sizeof(InT)), x);
+    float s;
+    const uint4 w = quant_vec<WireT>(x, gl, &s);
+    if (act) {
+      float acc[16] = {};
+      bsq_dequant_add<WireT>(acc, w, s);
+      bsq_store<OutT>(out + (size_t)v * 16, acc, scale);
+    }
+  });
+}
+
+template <typename InT, typename WireT, typename OutT>
+__global__ void __launch_bounds__(kBsqThreads) k_quant_ag(COMM_PARAM, const __grid_constant__ QuantGeom g, const char* __restrict__ in, OutT* __restrict__ out,
+                                                          float scale, uint32_t op) {
+  pdl_prologue();
+  quant_range<InT, WireT>(g, in, c.peer[c.rank] + g.data_off, c.peer[c.rank] + g.scale_off, 0, g.nvec);
+  const uint32_t s = load_seq(c, kSeqBarrier);
+  if (!barrier_blocks<true>(c, 2 * s + 1, op)) return;           // every rank's CTA b has quantised the vectors CTA b pulls below
+  ag_pull<WireT, OutT>(c, g, out, scale);
+  if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // nobody reads my scratch any more: the next call may overwrite it
+  if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
+}
+
+// nslices == 1: one-shot all-reduce, the whole buffer is quantised and reduced. nslices == N: reduce-scatter (PUSH=false) or two-shot
+// all-reduce (PUSH=true) of my block slice. in and out_local may be the same buffer (in-place all-reduce).
+template <typename InT, typename WireT, typename OutT, bool PUSH>
+__global__ void __launch_bounds__(kBsqThreads, 1) k_quant_pull_reduce(COMM_PARAM, const __grid_constant__ QuantGeom g, const char* in, OutT* out_local, size_t out_off,
+                                                                      uint32_t nslices, float scale, uint32_t op) {
+  pdl_prologue();
+  for (uint32_t sl = 0; sl < nslices; sl++)
+    quant_range<InT, WireT>(g, in, c.peer[c.rank] + g.data_off, c.peer[c.rank] + g.scale_off, quant_slice_start(g, sl, nslices), quant_slice_start(g, sl + 1, nslices));
+  {
+    const uint32_t s = load_seq(c, kSeqBarrier);
+    if (!barrier_blocks<true>(c, 2 * s + 1, op)) return;
+  }
+  const uint32_t me = nslices == 1 ? 0u : (uint32_t)c.rank;
+  pull_reduce_range<WireT, OutT, PUSH>(c, g, out_local, out_off, quant_slice_start(g, me, nslices), quant_slice_start(g, me + 1, nslices), scale);
+  const uint32_t s = load_seq(c, kSeqBarrier);
+  if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;
+  if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
+}
+
+// ------------------------------------------------------------------------------------------------ host side
+// (wire, out) -> f(Tag<WireT>, Tag<OutT>); the argument checks have refused every other type
 template <typename F>
-static b200collResult_t dispatch_bsq(b200collDataType_t in, b200collDataType_t out, F&& f) {
-  auto outs = [&](auto ti) -> b200collResult_t {
+static b200collResult_t dispatch_wire_out(b200collDataType_t wire, b200collDataType_t out, F&& f) {
+  auto outs = [&](auto tw) -> b200collResult_t {
     switch (out) {
-      case b200collBfloat16: return f(ti, Tag<bf16>{});
-      case b200collFloat16: return f(ti, Tag<__half>{});
-      case b200collFloat32: return f(ti, Tag<float>{});
-      default: set_last_error("block-scaled collectives: out_dtype must be bf16, fp16 or fp32"); return b200collInvalidArgument;
+      case b200collBfloat16: return f(tw, Tag<bf16>{});
+      case b200collFloat16: return f(tw, Tag<__half>{});
+      default: return f(tw, Tag<float>{});
     }
   };
-  if (in == b200collFloat8e4m3) return outs(Tag<f8>{});
-  if (in == b200collFloat8e5m2) return outs(Tag<e5m2>{});
-  set_last_error("block-scaled collectives: in_dtype must be e4m3 or e5m2");
-  return b200collInvalidArgument;
+  return wire == b200collFloat8e4m3 ? outs(Tag<f8>{}) : outs(Tag<e5m2>{});
 }
 
-static bool overlaps(const void* a, size_t na, const void* b, size_t nb) {
-  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
-  return x < y + nb && y < x + na;
+// the quantising kernels: one more level for the input type
+template <typename F>
+static b200collResult_t dispatch_quant(b200collDataType_t in, b200collDataType_t wire, b200collDataType_t out, F&& f) {
+  auto wires_outs = [&](auto ti) -> b200collResult_t { return dispatch_wire_out(wire, out, [&](auto tw, auto to) { return f(ti, tw, to); }); };
+  switch (in) {
+    case b200collBfloat16: return wires_outs(Tag<bf16>{});
+    case b200collFloat16: return wires_outs(Tag<__half>{});
+    default: return wires_outs(Tag<float>{});
+  }
 }
 
-struct BsqCall {
+static bool is_fp8(b200collDataType_t t) { return t == b200collFloat8e4m3 || t == b200collFloat8e5m2; }
+static bool wide_type(b200collDataType_t t) { return t == b200collBfloat16 || t == b200collFloat16 || t == b200collFloat32; }
+
+template <typename Geom> struct Fp8Call {
   b200collComm* c;
-  size_t count;                   // elements of one rank's send matrix
+  size_t count;                   // elements of one rank's send buffer
+  size_t in_bytes;                // bytes of my send
   size_t out_bytes;               // bytes of my recv
-  size_t nscales;
   float scale;                    // ep->scale, times 1/nranks for avg
-  BsqGeom g;
+  Geom g;
 };
+
+// The argument rules both families share; `family_check` returns the message of the first family rule the call breaks, or nullptr.
+// Every refusal comes before the poisoned-communicator check. On success `call` is filled in except for its geometry.
+template <typename Check, typename Geom>
+static b200collResult_t fp8_prepare(b200collComm* c, b200collOp_t which, const void* send, const void* recv, size_t count, const b200collEpilogue* ep,
+                                    b200collRedOp_t rop, const char* family, Check&& family_check, Fp8Call<Geom>* call) {
+  auto refuse = [](const std::string& msg) { set_last_error(msg); return b200collInvalidArgument; };
+  if (!c || !send || !recv || !ep) return refuse("null argument");
+  if (const char* e = family_check()) return refuse(e);
+  if (!wide_type(ep->out_dtype)) return refuse(std::string(family) + " collectives: out_dtype must be bf16, fp16 or fp32");
+  if (which != b200collOpAllGather && rop != b200collSum && rop != b200collAvg) return refuse(std::string(family) + " reductions take sum or avg only");
+  if (count / 16 >= ((size_t)1 << 31)) return refuse(std::string(family) + " collectives: fewer than 2^35 elements per rank");
+  if (!aligned(send, 16) || !aligned(recv, 16)) return refuse("send and recv must be 16-byte aligned");
+  if (comm_poisoned(c)) return b200collRemoteError;
+  call->c = c;
+  call->count = count;
+  call->in_bytes = count * b200collTypeSize(ep->in_dtype);
+  call->out_bytes = (which == b200collOpAllGather ? count * c->nranks : which == b200collOpReduceScatter ? count / c->nranks : count) * b200collTypeSize(ep->out_dtype);
+  call->scale = ep->scale * (rop == b200collAvg && which != b200collOpAllGather ? 1.0f / (float)c->nranks : 1.0f);
+  return b200collSuccess;
+}
+
+// The all-reduce algorithm of both families: the table's pick for an FP8 all-reduce of `count` bytes, or the forced algorithm. The
+// Lamport paths and one-shot become the one-shot pull, two-shot and NVLS the two-shot pull + push, which needs recv in the arena (peers
+// write into it) and falls back to one-shot otherwise.
+static b200collAlgo_t fp8_all_reduce_algo(b200collComm* c, size_t count, const void* recv, size_t out_bytes) {
+  const b200collAlgo_t want = c->forced_algo != b200collAlgoAuto ? c->forced_algo : b200collTunerPick(b200collOpAllReduce, count, c->nranks, c->nvls);
+  const bool two = (want == b200collAlgoTwoShot || want == b200collAlgoNvls) && b200collIsSymmetric(c, recv, out_bytes);
+  return two ? b200collAlgoTwoShot : b200collAlgoOneShot;
+}
+
+// Whole warps: WarpScale and the amax butterfly are full-mask warp intrinsics, and pick_grid takes a forced thread count as given.
+static Grid warp_grid(const b200collComm* c, size_t vecs) {
+  Grid gr = pick_grid(c, kShapeP2p, vecs, 1);
+  gr.threads = std::max(32, gr.threads & ~31);
+  return gr;
+}
+
+// the pull-reduce grid: sized to my slice (reduce-scatter, two-shot) or to the whole buffer (one-shot)
+static Grid reduce_grid(const b200collComm* c, b200collOp_t which, b200collAlgo_t algo, uint32_t nvec) {
+  const uint32_t n = (uint32_t)c->nranks;
+  return warp_grid(c, algo == b200collAlgoTwoShot ? nvec / n + 1 : which == b200collOpReduceScatter ? nvec / n : nvec);
+}
+
+// nranks == 1: no peers, no barrier; grid as for the fused copy (streaming, 8 CTAs of 256 threads per SM at most)
+static int copy_blocks(const b200collComm* c, uint32_t nvec) {
+  return (int)std::max<size_t>(1, std::min<size_t>(((size_t)nvec + 255) / 256, (size_t)std::max(1, c->sm_count) * 8));
+}
+
+// ---- block-scaled
+using BsqCall = Fp8Call<BsqGeom>;
 
 // Everything the three entry points check before they launch. On success `call` is filled in; count == 0 is left to the caller.
 static b200collResult_t bsq_prepare(b200collComm* c, b200collOp_t which, const void* send, void* recv, size_t count, const b200collBlockScale* bs,
                                     const b200collEpilogue* ep, b200collRedOp_t rop, BsqCall* call) {
-  if (!c || !send || !recv || !bs || !ep || !bs->scales) { set_last_error("null argument"); return b200collInvalidArgument; }
-  if (ep->in_dtype != b200collFloat8e4m3 && ep->in_dtype != b200collFloat8e5m2) { set_last_error("block-scaled collectives: in_dtype must be e4m3 or e5m2"); return b200collInvalidArgument; }
-  if (ep->out_dtype != b200collBfloat16 && ep->out_dtype != b200collFloat16 && ep->out_dtype != b200collFloat32) { set_last_error("block-scaled collectives: out_dtype must be bf16, fp16 or fp32"); return b200collInvalidArgument; }
-  if (which != b200collOpAllGather && rop != b200collSum && rop != b200collAvg) { set_last_error("block-scaled reductions take sum or avg only"); return b200collInvalidArgument; }
-  if (bs->row_len == 0 || bs->row_len % 16 != 0) { set_last_error("block-scaled collectives: row_len must be a positive multiple of 16"); return b200collInvalidArgument; }
-  if (bs->block_rows < 1 || bs->block_cols < 16 || bs->block_cols % 16 != 0) { set_last_error("block-scaled collectives: block_rows must be >= 1 and block_cols a positive multiple of 16"); return b200collInvalidArgument; }
-  if (count % bs->row_len != 0) { set_last_error("block-scaled collectives: the send count must be a multiple of row_len"); return b200collInvalidArgument; }
-  if (count / 16 >= ((size_t)1 << 31)) { set_last_error("block-scaled collectives: fewer than 2^35 elements per rank"); return b200collInvalidArgument; }
-  const size_t rows = count / bs->row_len;
-  if (which == b200collOpReduceScatter && rows % (size_t)c->nranks != 0) { set_last_error("block-scaled reduce-scatter: the number of rows must be a multiple of nranks"); return b200collInvalidArgument; }
-  if (!aligned(send, 16) || !aligned(recv, 16) || !aligned(bs->scales, 4)) { set_last_error("send and recv must be 16-byte aligned, scales 4-byte aligned"); return b200collInvalidArgument; }
-  if (c->fault_host && *const_cast<volatile uint32_t*>(&c->fault_host->code) != 0) { set_last_error("communicator is poisoned by an earlier watchdog fault"); return b200collRemoteError; }
-  const size_t os = b200collTypeSize(ep->out_dtype);
-  const size_t vpr = bs->row_len / 16, vpb = (size_t)bs->block_cols / 16;
+  b200collResult_t rc = fp8_prepare(c, which, send, recv, count, ep, rop, "block-scaled", [&]() -> const char* {
+    if (!bs || !bs->scales) return "null argument";
+    if (!is_fp8(ep->in_dtype)) return "block-scaled collectives: in_dtype must be e4m3 or e5m2";
+    if (bs->row_len == 0 || bs->row_len % 16 != 0) return "block-scaled collectives: row_len must be a positive multiple of 16";
+    if (bs->block_rows < 1 || bs->block_cols < 16 || bs->block_cols % 16 != 0) return "block-scaled collectives: block_rows must be >= 1 and block_cols a positive multiple of 16";
+    if (count % bs->row_len != 0) return "block-scaled collectives: the send count must be a multiple of row_len";
+    if (which == b200collOpReduceScatter && (count / bs->row_len) % (size_t)c->nranks != 0) return "block-scaled reduce-scatter: the number of rows must be a multiple of nranks";
+    if (!aligned(bs->scales, 4)) return "block-scaled collectives: scales must be 4-byte aligned";
+    return nullptr;
+  }, call);
+  if (rc != b200collSuccess || count == 0) return rc;
+  const size_t rows = count / bs->row_len, vpr = bs->row_len / 16, vpb = (size_t)bs->block_cols / 16;
   const size_t nbr = (rows + bs->block_rows - 1) / bs->block_rows, ncb = (vpr + vpb - 1) / vpb;
-  call->c = c;
-  call->count = count;
-  call->out_bytes = (which == b200collOpAllGather ? count * c->nranks : which == b200collOpReduceScatter ? count / c->nranks : count) * os;
-  call->nscales = nbr * ncb;
-  call->scale = ep->scale * (rop == b200collAvg && which != b200collOpAllGather ? 1.0f / (float)c->nranks : 1.0f);
-  if (count == 0) return b200collSuccess;
-  if (overlaps(send, count, recv, call->out_bytes)) { set_last_error("block-scaled collectives: recv must not overlap send"); return b200collInvalidArgument; }
+  if (overlaps(send, call->in_bytes, recv, call->out_bytes)) { set_last_error("block-scaled collectives: recv must not overlap send"); return b200collInvalidArgument; }
   // peers read my matrix and scales at MY arena offsets: both must be arena memory (there is no staging path for these ops)
-  if (!b200collIsSymmetric(c, send, count) || !b200collIsSymmetric(c, bs->scales, call->nscales * 4)) {
+  if (!b200collIsSymmetric(c, send, count) || !b200collIsSymmetric(c, bs->scales, nbr * ncb * 4)) {
     set_last_error("block-scaled collectives: send and scales must lie in the symmetric arena (b200collMemAlloc), at the same offsets on every rank");
     return b200collInvalidUsage;
   }
   BsqGeom& g = call->g;
-  g.send_off = arena_off(c, send); g.scale_off = arena_off(c, bs->scales);
+  g.data_off = arena_off(c, send); g.scale_off = arena_off(c, bs->scales);
   g.nvec = (uint32_t)(count / 16); g.ncb = (uint32_t)ncb;
   g.vpr = make_fastdiv((uint32_t)vpr); g.br = make_fastdiv((uint32_t)bs->block_rows); g.vpb = make_fastdiv((uint32_t)vpb);
   return b200collSuccess;
 }
 
-// nranks == 1: no peers, no barrier; grid as for the fused copy (streaming, 8 CTAs of 256 threads per SM at most)
 static b200collResult_t bsq_copy(const BsqCall& k, const void* send, const b200collBlockScale* bs, void* recv, const b200collEpilogue* ep, cudaStream_t st) {
   b200collComm* c = k.c;
-  return dispatch_bsq(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
+  return dispatch_wire_out(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
     using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
-    const int blocks = (int)std::max<size_t>(1, std::min<size_t>(((size_t)k.g.nvec + 255) / 256, (size_t)std::max(1, c->sm_count) * 8));
-    launch_k(k_bsq_copy<InT, OutT>, blocks, 256, st, k.g, static_cast<const char*>(send), reinterpret_cast<const char*>(bs->scales), static_cast<OutT*>(recv), k.scale);
+    launch_k(k_bsq_copy<InT, OutT>, copy_blocks(c, k.g.nvec), 256, st, k.g, static_cast<const char*>(send), reinterpret_cast<const char*>(bs->scales),
+             static_cast<OutT*>(recv), k.scale);
     LAUNCH_CHECK(c);
     return b200collSuccess;
   });
@@ -220,15 +499,98 @@ static b200collResult_t bsq_reduce(const BsqCall& k, b200collOp_t which, b200col
   if (which == b200collOpReduceScatter || algo == b200collAlgoTwoShot) {
     v0 = (uint32_t)((unsigned long long)k.g.nvec * me / n); v1 = (uint32_t)((unsigned long long)k.g.nvec * (me + 1) / n);
   }
-  return dispatch_bsq(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
+  const Grid gr = reduce_grid(c, which, algo, k.g.nvec);
+  return dispatch_wire_out(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
     using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
-    if (algo == b200collAlgoTwoShot) {
-      const Grid gr = pick_grid(c, kShapeP2p, k.g.nvec / n + 1, 1);
+    if (algo == b200collAlgoTwoShot)
       launch_k(k_bsq_pull_reduce<InT, OutT, true>, gr.blocks, gr.threads, st, c->dev, k.g, static_cast<OutT*>(nullptr), arena_off(c, recv), v0, v1, k.scale, (uint32_t)which);
-    } else {
-      const Grid gr = pick_grid(c, kShapeP2p, which == b200collOpReduceScatter ? k.g.nvec / n : k.g.nvec, 1);
+    else
       launch_k(k_bsq_pull_reduce<InT, OutT, false>, gr.blocks, gr.threads, st, c->dev, k.g, static_cast<OutT*>(recv), (size_t)0, v0, v1, k.scale, (uint32_t)which);
+    LAUNCH_CHECK(c);
+    return b200collSuccess;
+  });
+}
+
+// ---- quantising
+using QuantCall = Fp8Call<QuantGeom>;
+
+// Everything the three entry points check before they touch the scratch or launch; count == 0 is left to the caller.
+static b200collResult_t quant_prepare(b200collComm* c, b200collOp_t which, const void* send, void* recv, size_t count, b200collDataType_t wire, int block,
+                                      const b200collEpilogue* ep, b200collRedOp_t rop, QuantCall* call) {
+  b200collResult_t rc = fp8_prepare(c, which, send, recv, count, ep, rop, "quantised", [&]() -> const char* {
+    if (!wide_type(ep->in_dtype)) return "quantised collectives: in_dtype must be bf16, fp16 or fp32";
+    if (!is_fp8(wire)) return "quantised collectives: wire_dtype must be e4m3 or e5m2";
+    if (block < 16 || block > 512 || (block & (block - 1)) != 0) return "quantised collectives: block must be 16, 32, 64, 128, 256 or 512";
+    const bool rs = which == b200collOpReduceScatter;
+    if ((rs ? count / (size_t)c->nranks : count) % (size_t)block != 0)
+      return rs ? "quantised reduce-scatter: recvcount must be a multiple of block" : "quantised collectives: the count must be a multiple of block";
+    return nullptr;
+  }, call);
+  if (rc != b200collSuccess || count == 0) return rc;
+  // in place (all-reduce only): every vector is read and rewritten at the same position, so the element sizes must agree
+  const bool in_place = which == b200collOpAllReduce && send == recv && call->in_bytes == call->out_bytes;
+  if (!in_place && overlaps(send, call->in_bytes, recv, call->out_bytes)) {
+    set_last_error(which == b200collOpAllReduce ? "quantised all-reduce: recv must be send (with in_dtype and out_dtype of one size) or not overlap it"
+                                                : "quantised collectives: recv must not overlap send");
+    return b200collInvalidArgument;
+  }
+  QuantGeom& g = call->g;
+  g.nvec = (uint32_t)(count / 16);
+  g.nblk = (uint32_t)(count / (size_t)block);
+  g.lvpb = 0;
+  while ((16u << g.lvpb) < (uint32_t)block) g.lvpb++;
+  return b200collSuccess;
+}
+
+// The FP8 copy (count bytes) and its scales (count / block fp32) of one call, in the symmetric heap. Taken with b200collMemAlloc on first
+// use and grown on demand: a collective contract like MemAlloc (every rank makes the same quantised calls in the same order, so every
+// rank gets the same offsets). A superseded scratch is never given back before CommDestroy: a CUDA graph captured earlier still
+// addresses it, and must stay valid when a later, larger call moves the scratch.
+static b200collResult_t quant_scratch(b200collComm* c, QuantCall* k) {
+  const size_t qbytes = k->count, need = qbytes + (size_t)k->g.nblk * 4;
+  if (c->quant_scratch_bytes < need) {
+    void* p = nullptr;
+    size_t bytes = std::max(need, 2 * c->quant_scratch_bytes);
+    b200collResult_t rc = b200collMemAlloc(c, &p, bytes);
+    if (rc != b200collSuccess && bytes != need) rc = b200collMemAlloc(c, &p, bytes = need);
+    if (rc != b200collSuccess) {
+      set_last_error("quantised collectives: the symmetric arena cannot hold the " + std::to_string(need) + "-byte FP8 scratch (raise B200COLL_ARENA_MB)");
+      return rc;
     }
+    if (c->quant_scratch) c->quant_scratch_retired.push_back(c->quant_scratch);
+    c->quant_scratch = p;
+    c->quant_scratch_bytes = bytes;
+  }
+  k->g.data_off = arena_off(c, c->quant_scratch);
+  k->g.scale_off = k->g.data_off + qbytes;                        // count is a multiple of 16: the scales are 16-byte aligned
+  return b200collSuccess;
+}
+
+// nranks == 1: the round trip in registers
+static b200collResult_t quant_copy(const QuantCall& k, const void* send, void* recv, b200collDataType_t wire, const b200collEpilogue* ep, cudaStream_t st) {
+  b200collComm* c = k.c;
+  return dispatch_quant(ep->in_dtype, wire, ep->out_dtype, [&](auto ti, auto tw, auto to) -> b200collResult_t {
+    using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type; using OutT = typename decltype(to)::type;
+    launch_k(k_quant_copy<InT, WireT, OutT>, copy_blocks(c, k.g.nvec), 256, st, static_cast<const char*>(send), static_cast<OutT*>(recv), k.g.nvec, k.g.lvpb, k.scale);
+    LAUNCH_CHECK(c);
+    return b200collSuccess;
+  });
+}
+
+static b200collResult_t quant_reduce(const QuantCall& k, b200collOp_t which, b200collAlgo_t algo, const void* send, void* recv, b200collDataType_t wire,
+                                     const b200collEpilogue* ep, cudaStream_t st) {
+  b200collComm* c = k.c;
+  const uint32_t nslices = (which == b200collOpReduceScatter || algo == b200collAlgoTwoShot) ? (uint32_t)c->nranks : 1u;
+  const Grid gr = reduce_grid(c, which, algo, k.g.nvec);
+  return dispatch_quant(ep->in_dtype, wire, ep->out_dtype, [&](auto ti, auto tw, auto to) -> b200collResult_t {
+    using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type; using OutT = typename decltype(to)::type;
+    const char* in = static_cast<const char*>(send);
+    if (algo == b200collAlgoTwoShot)
+      launch_k(k_quant_pull_reduce<InT, WireT, OutT, true>, gr.blocks, gr.threads, st, c->dev, k.g, in, static_cast<OutT*>(nullptr), arena_off(c, recv), nslices, k.scale,
+               (uint32_t)which);
+    else
+      launch_k(k_quant_pull_reduce<InT, WireT, OutT, false>, gr.blocks, gr.threads, st, c->dev, k.g, in, static_cast<OutT*>(recv), (size_t)0, nslices, k.scale,
+               (uint32_t)which);
     LAUNCH_CHECK(c);
     return b200collSuccess;
   });
@@ -247,12 +609,12 @@ b200collResult_t b200collAllGatherBlockScaled(const void* send, void* recv, size
   if (rc != b200collSuccess || sendcount == 0) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (c->nranks == 1) { account(c, b200collOpAllGather, sendcount, b200collAlgoCopy); return bsq_copy(k, send, bs, recv, ep, st); }
-  rc = cross_check(c, b200collOpAllGather, b200collAlgoOneShot, sendcount, k.g.send_off, k.g.scale_off);
+  rc = cross_check(c, b200collOpAllGather, b200collAlgoOneShot, sendcount, k.g.data_off, k.g.scale_off);
   if (rc != b200collSuccess) return rc;
   account(c, b200collOpAllGather, sendcount, b200collAlgoOneShot);
-  return dispatch_bsq(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
+  return dispatch_wire_out(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
     using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
-    const Grid gr = pick_grid(c, kShapeP2p, k.g.nvec, 1);
+    const Grid gr = warp_grid(c, k.g.nvec);
     launch_k(k_bsq_ag_pull<InT, OutT>, gr.blocks, gr.threads, st, c->dev, k.g, static_cast<OutT*>(recv), k.scale, (uint32_t)b200collOpAllGather);
     LAUNCH_CHECK(c);
     return b200collSuccess;
@@ -267,7 +629,7 @@ b200collResult_t b200collReduceScatterBlockScaled(const void* send, void* recv, 
   if (rc != b200collSuccess || recvcount == 0) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (c->nranks == 1) { account(c, b200collOpReduceScatter, recvcount, b200collAlgoCopy); return bsq_copy(k, send, bs, recv, ep, st); }
-  rc = cross_check(c, b200collOpReduceScatter, b200collAlgoOneShot, recvcount, k.g.send_off, k.g.scale_off);
+  rc = cross_check(c, b200collOpReduceScatter, b200collAlgoOneShot, recvcount, k.g.data_off, k.g.scale_off);
   if (rc != b200collSuccess) return rc;
   account(c, b200collOpReduceScatter, recvcount, b200collAlgoOneShot);
   return bsq_reduce(k, b200collOpReduceScatter, b200collAlgoOneShot, recv, ep, st);
@@ -280,15 +642,63 @@ b200collResult_t b200collAllReduceBlockScaled(const void* send, void* recv, size
   if (rc != b200collSuccess || count == 0) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (c->nranks == 1) { account(c, b200collOpAllReduce, count, b200collAlgoCopy); return bsq_copy(k, send, bs, recv, ep, st); }
-  // the table's pick for an FP8 all-reduce of this many bytes (or the forced algorithm): the Lamport paths and one-shot become the
-  // one-shot pull, two-shot and NVLS the two-shot pull + push, which needs recv in the arena (peers write into it)
-  const b200collAlgo_t want = c->forced_algo != b200collAlgoAuto ? c->forced_algo : b200collTunerPick(b200collOpAllReduce, count, c->nranks, c->nvls);
-  b200collAlgo_t algo = (want == b200collAlgoTwoShot || want == b200collAlgoNvls) ? b200collAlgoTwoShot : b200collAlgoOneShot;
-  if (algo == b200collAlgoTwoShot && !b200collIsSymmetric(c, recv, k.out_bytes)) algo = b200collAlgoOneShot;
-  rc = cross_check(c, b200collOpAllReduce, algo, count, k.g.send_off, algo == b200collAlgoTwoShot ? arena_off(c, recv) : k.g.scale_off);
+  const b200collAlgo_t algo = fp8_all_reduce_algo(c, count, recv, k.out_bytes);
+  rc = cross_check(c, b200collOpAllReduce, algo, count, k.g.data_off, algo == b200collAlgoTwoShot ? arena_off(c, recv) : k.g.scale_off);
   if (rc != b200collSuccess) return rc;
   account(c, b200collOpAllReduce, count, algo);
   return bsq_reduce(k, b200collOpAllReduce, algo, recv, ep, st);
+}
+
+b200collResult_t b200collAllGatherQuantized(const void* send, void* recv, size_t sendcount, b200collDataType_t wire_dtype, int block,
+                                            const b200collEpilogue* ep, b200collComm_t c, b200collStream_t stream) {
+  QuantCall k;
+  b200collResult_t rc = quant_prepare(c, b200collOpAllGather, send, recv, sendcount, wire_dtype, block, ep, b200collSum, &k);
+  if (rc != b200collSuccess || sendcount == 0) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (c->nranks == 1) { account(c, b200collOpAllGather, k.in_bytes, b200collAlgoCopy); return quant_copy(k, send, recv, wire_dtype, ep, st); }
+  if ((rc = quant_scratch(c, &k)) != b200collSuccess) return rc;
+  rc = cross_check(c, b200collOpAllGather, b200collAlgoOneShot, sendcount, k.g.data_off, k.g.scale_off);
+  if (rc != b200collSuccess) return rc;
+  account(c, b200collOpAllGather, k.in_bytes, b200collAlgoOneShot);
+  return dispatch_quant(ep->in_dtype, wire_dtype, ep->out_dtype, [&](auto ti, auto tw, auto to) -> b200collResult_t {
+    using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type; using OutT = typename decltype(to)::type;
+    const Grid gr = warp_grid(c, k.g.nvec);
+    launch_k(k_quant_ag<InT, WireT, OutT>, gr.blocks, gr.threads, st, c->dev, k.g, static_cast<const char*>(send), static_cast<OutT*>(recv), k.scale,
+             (uint32_t)b200collOpAllGather);
+    LAUNCH_CHECK(c);
+    return b200collSuccess;
+  });
+}
+
+b200collResult_t b200collReduceScatterQuantized(const void* send, void* recv, size_t recvcount, b200collDataType_t wire_dtype, int block,
+                                                const b200collEpilogue* ep, b200collRedOp_t op, b200collComm_t c, b200collStream_t stream) {
+  if (c && recvcount > SIZE_MAX / B200COLL_MAX_RANKS) { set_last_error("recvcount too large"); return b200collInvalidArgument; }
+  QuantCall k;
+  b200collResult_t rc = quant_prepare(c, b200collOpReduceScatter, send, recv, c ? recvcount * c->nranks : 0, wire_dtype, block, ep, op, &k);
+  if (rc != b200collSuccess || recvcount == 0) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t bytes = recvcount * b200collTypeSize(ep->in_dtype);
+  if (c->nranks == 1) { account(c, b200collOpReduceScatter, bytes, b200collAlgoCopy); return quant_copy(k, send, recv, wire_dtype, ep, st); }
+  if ((rc = quant_scratch(c, &k)) != b200collSuccess) return rc;
+  rc = cross_check(c, b200collOpReduceScatter, b200collAlgoOneShot, recvcount, k.g.data_off, k.g.scale_off);
+  if (rc != b200collSuccess) return rc;
+  account(c, b200collOpReduceScatter, bytes, b200collAlgoOneShot);
+  return quant_reduce(k, b200collOpReduceScatter, b200collAlgoOneShot, send, recv, wire_dtype, ep, st);
+}
+
+b200collResult_t b200collAllReduceQuantized(const void* send, void* recv, size_t count, b200collDataType_t wire_dtype, int block,
+                                            const b200collEpilogue* ep, b200collRedOp_t op, b200collComm_t c, b200collStream_t stream) {
+  QuantCall k;
+  b200collResult_t rc = quant_prepare(c, b200collOpAllReduce, send, recv, count, wire_dtype, block, ep, op, &k);
+  if (rc != b200collSuccess || count == 0) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (c->nranks == 1) { account(c, b200collOpAllReduce, k.in_bytes, b200collAlgoCopy); return quant_copy(k, send, recv, wire_dtype, ep, st); }
+  const b200collAlgo_t algo = fp8_all_reduce_algo(c, count, recv, k.out_bytes);
+  if ((rc = quant_scratch(c, &k)) != b200collSuccess) return rc;
+  rc = cross_check(c, b200collOpAllReduce, algo, count, k.g.data_off, algo == b200collAlgoTwoShot ? arena_off(c, recv) : k.g.scale_off);
+  if (rc != b200collSuccess) return rc;
+  account(c, b200collOpAllReduce, k.in_bytes, algo);
+  return quant_reduce(k, b200collOpAllReduce, algo, send, recv, wire_dtype, ep, st);
 }
 
 }  // extern "C"

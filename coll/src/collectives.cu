@@ -16,7 +16,6 @@
 
 namespace b200coll {
 
-template <typename T> struct Tag { using type = T; };
 using bf16 = __nv_bfloat16;
 using f8 = __nv_fp8_e4m3;
 using e5m2 = __nv_fp8_e5m2;
@@ -83,7 +82,7 @@ static b200collResult_t check_common(b200collComm* c, const void* send, void* re
   if (!fused(ep->in_dtype) || !fused(ep->out_dtype)) { set_last_error("bad dtype (fp32 / fp16 / bf16 / e4m3 / e5m2; integer and fp64 payloads: reductions take the generic path, data movement takes them as words)"); return b200collInvalidArgument; }
   const size_t is = b200collTypeSize(ep->in_dtype), os = b200collTypeSize(ep->out_dtype);
   if (!aligned(send, 16) || !aligned(recv, out_align(is, os))) { set_last_error("send must be 16-byte aligned and recv aligned to one output vector"); return b200collInvalidArgument; }
-  if (c->fault_host && *const_cast<volatile uint32_t*>(&c->fault_host->code) != 0) { set_last_error("communicator is poisoned by an earlier watchdog fault"); return b200collRemoteError; }
+  if (comm_poisoned(c)) return b200collRemoteError;
   return b200collSuccess;
 }
 
@@ -373,7 +372,7 @@ b200collResult_t p2p_flush(std::vector<PendingP2p>& all) {
     std::vector<PendingP2p> mine, rest;
     for (const PendingP2p& o : all) (o.comm == c ? mine : rest).push_back(o);
     all.swap(rest);
-    if (c->fault_host && *const_cast<volatile uint32_t*>(&c->fault_host->code) != 0) { set_last_error("communicator is poisoned by an earlier watchdog fault"); return b200collRemoteError; }
+    if (comm_poisoned(c)) return b200collRemoteError;
     // a group may span communicators on several GPUs of this process (nccl-tests -g N): launch each on its own device
     struct DeviceGuard {
       int prev = -1; bool switched = false;

@@ -105,7 +105,7 @@ struct b200collComm {
   bool affinity_changed = false;
   b200coll::HostPath host;
   std::map<void*, size_t> host_allocs;  // HostAlloc: base -> mapped length
-  // quantising collectives (quantized.cu): the symmetric scratch for the FP8 copy and its scales, grown on demand. Superseded scratch
+  // quantising collectives (blockscaled.cu): the symmetric scratch for the FP8 copy and its scales, grown on demand. Superseded scratch
   // buffers stay allocated until CommDestroy (a captured CUDA graph may still address them).
   void* quant_scratch = nullptr;
   size_t quant_scratch_bytes = 0;

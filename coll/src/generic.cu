@@ -14,6 +14,7 @@
 
 #include "comm.h"
 #include "device.cuh"
+#include "launch.cuh"
 
 namespace b200coll {
 
@@ -165,7 +166,7 @@ b200collResult_t generic_reduce(b200collComm* c, b200collOp_t which, const void*
   const size_t es = b200collTypeSize(ep->in_dtype);
   if (es == 0) { set_last_error("bad dtype"); return b200collInvalidArgument; }
   if (reinterpret_cast<uintptr_t>(send) % 16 || reinterpret_cast<uintptr_t>(recv) % 16) { set_last_error("send and recv must be 16-byte aligned"); return b200collInvalidArgument; }
-  if (c->fault_host && *const_cast<volatile uint32_t*>(&c->fault_host->code) != 0) { set_last_error("communicator is poisoned by an earlier watchdog fault"); return b200collRemoteError; }
+  if (comm_poisoned(c)) return b200collRemoteError;
   if (count == 0) return b200collSuccess;
   const int n = c->nranks;
   const size_t in_elems = which == b200collOpReduceScatter ? count * n : count;

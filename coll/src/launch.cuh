@@ -1,5 +1,6 @@
-// Host-side launch helpers shared by the collective entry points (collectives.cu, blockscaled.cu): kernel launch through
-// cudaLaunchKernelEx with optional programmatic dependent launch, the launch-shape picker, and call accounting.
+// Host-side launch helpers shared by the collective entry points (collectives.cu, generic.cu, and blockscaled.cu for the block-scaled
+// and quantising FP8 collectives): kernel launch through cudaLaunchKernelEx with optional programmatic dependent launch, the
+// launch-shape picker, argument and communicator checks, the type tag, and call accounting.
 #pragma once
 #include <stdlib.h>
 
@@ -83,6 +84,20 @@ inline Grid pick_grid(const b200collComm* c, int kind, size_t vecs, int unroll) 
 
 inline size_t arena_off(b200collComm* c, const void* p) { return reinterpret_cast<CUdeviceptr>(p) - c->peer_va[c->rank]; }
 inline bool aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) % a) == 0; }
+inline bool overlaps(const void* a, size_t na, const void* b, size_t nb) {
+  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+  return x < y + nb && y < x + na;
+}
+
+// A kernel that hit its watchdog deadline poisons the communicator: every later call is refused (the caller returns RemoteError).
+inline bool comm_poisoned(const b200collComm* c) {
+  if (!c->fault_host || *const_cast<volatile uint32_t*>(&c->fault_host->code) == 0) return false;
+  set_last_error("communicator is poisoned by an earlier watchdog fault");
+  return true;
+}
+
+// type dispatch: f(Tag<InT>{}, Tag<OutT>{}) instantiates a launch for the element types
+template <typename T> struct Tag { using type = T; };
 
 // collectives.cu: count a call in the stats (and mark it for NVTX / debug traces); B200COLL_CHECK=1 cross-check of a symmetric launch
 void account(b200collComm* c, b200collOp_t op, size_t bytes, b200collAlgo_t algo);

@@ -92,7 +92,10 @@ def test_sass_unpacks_in_hardware_uses_no_multimem_and_no_64bit_division(coll_li
 def test_source_moves_data_without_multimem():
     """The data path is plain loads and stores over NVLink; the only multicast operation is the shared epoch barrier's counter."""
     src = open(os.path.join(ROOT, "coll", "src", "blockscaled.cu")).read()
-    assert "multimem" not in src.split("// ---", 1)[0].split("#include", 1)[1]
+    device = src.split("// ---", 1)[0].split("#include", 1)[1]
+    for loop in ("warp_walk", "dequant_range", "pull_reduce_range", "quant_range", "k_bsq_pull_reduce", "k_quant_pull_reduce"):
+        assert f" {loop}(" in device, loop                        # the device section the check covers holds every loop
+    assert "multimem" not in device
     for helper in ("mc_ld_reduce", "mc_st_words", "c.mc"):
         assert helper not in src, helper
 

@@ -254,11 +254,12 @@ def test_sass_reduces_amax_across_lanes_packs_saturating_and_unpacks_in_hardware
             assert "MATCH.ANY" in body, name                              # pulled scales shared by the lanes that need them
 
 
-def test_ptxas_reports_no_spill_bytes(tmp_path):
-    """The compiler's own account, with the library's flags: no stack frame and no spill stores or loads for any k_quant_ kernel."""
-    src = os.path.join(ROOT, "coll", "src", "quantized.cu")
+def test_ptxas_reports_no_spill_bytes_in_the_shared_fp8_unit(tmp_path):
+    """The compiler's own account, with the library's flags: no stack frame and no spill stores or loads for any k_quant_ kernel of
+    blockscaled.cu, the translation unit the quantising kernels share with the block-scaled ones."""
+    src = os.path.join(ROOT, "coll", "src", "blockscaled.cu")
     r = subprocess.run([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
-                        "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-c", src, "-o", str(tmp_path / "quantized.o")],
+                        "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-c", src, "-o", str(tmp_path / "blockscaled.o")],
                        capture_output=True, text=True, check=True)
     report, cur = {}, None
     for line in r.stderr.splitlines():
