@@ -331,6 +331,10 @@ b200collResult_t b200collRecv(void* buf, size_t bytes, int peer, b200collComm_t 
  * launches it would make as text: CTA ranges per operation, direct or staged receive, window layout, follow-up kernels. */
 b200collResult_t b200collDebugPlanP2p(int rank, int nranks, int loopback, size_t window, int nops, const int* is_send, const int* peer,
                                       const size_t* bytes, const int* in_arena, char* out, size_t outlen);
+/* Test hook (no GPU needed): the launch plan of the one-rank copy-engine copy of `bytes` (a multiple of 16) on a GPU with `sm_count`
+ * SMs. [0, bytes) is cut into chunks of `chunk` bytes (the last one shorter) and CTA b of `blocks` copies chunks b, b + blocks, ...:
+ * `rounds` of them, or one fewer. `max_resident` is how many of its CTAs fit on the GPU at once, which `blocks` never exceeds. */
+b200collResult_t b200collDebugPlanCopy(size_t bytes, int sm_count, int* blocks, unsigned* chunk, unsigned* rounds, int* max_resident);
 
 /* --- tuner (libnccl-tuner.so analogue). */
 b200collAlgo_t b200collTunerPick(b200collOp_t op, size_t bytes, int nranks, int nvls_available);

@@ -167,16 +167,47 @@ static b200collResult_t launch_bulk(b200collComm* c, BulkArgs& a, bool sync, b20
 }
 
 // ------------------------------------------------------------------------------------------------ nranks == 1
+// The one-rank copy-engine copy (kernels.cuh k_copy_bulk) is planned from the size and the SM count alone: as many CTAs as are resident
+// at once (2 of 96 KiB shared memory per SM) unless that would leave a CTA less than kCopyMinPerCta, and a chunk size (whole 128-byte
+// lines, at most one ring slot) that makes the round-robin deal of chunks fill whole rounds of the grid: every CTA moves `rounds`
+// chunks, or one fewer for the few that the line rounding leaves short. Fixed 16 KiB chunks left a ragged last round (at 16 MiB, 232
+// of 396 CTAs moved 3 chunks and 164 moved 2). Chunks rounded to 16 bytes only cut a line in two at every chunk boundary and cost
+// 5-7% of the copy rate from 256 MiB up on an H100; from there on the chunk comes out at 16 KiB again.
+struct CopyPlan { int blocks; uint32_t chunk; uint32_t rounds; };
+constexpr unsigned long long kCopyMinPerCta = 4096;
+constexpr unsigned long long kCopyAlign = 128;
+constexpr int kCopyCtasPerSm = 2;      // 2 x (96 KiB ring + 1 KiB reserved) fits the 228 KiB of shared memory of an H100 SM
+static CopyPlan plan_copy(unsigned long long bytes, int sm_count) {
+  const unsigned long long cap = (unsigned long long)kCopyCtasPerSm * (unsigned long long)std::max(1, sm_count);
+  const unsigned long long blocks = std::max(1ull, std::min(cap, (bytes + kCopyMinPerCta - 1) / kCopyMinPerCta));
+  const unsigned long long rounds = std::max(1ull, (bytes + blocks * kCopySlot - 1) / (blocks * kCopySlot));
+  const unsigned long long per = (bytes + blocks * rounds - 1) / (blocks * rounds);
+  const unsigned long long chunk = std::min<unsigned long long>(kCopySlot, std::max(kCopyAlign, (per + kCopyAlign - 1) / kCopyAlign * kCopyAlign));
+  return CopyPlan{(int)std::max(1ull, std::min(blocks, (bytes + chunk - 1) / chunk)), (uint32_t)chunk, (uint32_t)rounds};
+}
+static b200collResult_t launch_copy_bulk(b200collComm* c, const void* send, void* recv, size_t nbytes, cudaStream_t st) {
+  static std::atomic<unsigned long long> attr_done{0};      // per device, as in launch_bulk
+  const unsigned long long bit = 1ull << (c->device & 63);
+  if (!(attr_done.load(std::memory_order_acquire) & bit)) {
+    cudaFuncSetAttribute(k_copy_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCopySmemBytes);
+    attr_done.fetch_or(bit, std::memory_order_release);
+  }
+  const CopyPlan p = plan_copy(nbytes, c->sm_count);
+  PdlScope pdl_scope(true);
+  launch_k_smem(k_copy_bulk, p.blocks, kBulkThreads, kCopySmemBytes, st, c->dev, static_cast<const char*>(send), static_cast<char*>(recv),
+                (unsigned long long)nbytes, p.chunk);
+  LAUNCH_CHECK(c);
+  c->stats.bulk_launches++;
+  return b200collSuccess;
+}
+
 // The identity epilogue is a bit copy at every size (in place: nothing to do); anything else is round((0 + x) * scale).
 static b200collResult_t copy_scale(b200collComm* c, const void* send, void* recv, size_t count, const b200collEpilogue* ep, float scale, cudaStream_t st) {
   const int identity = (ep->in_dtype == ep->out_dtype && scale == 1.0f) ? 1 : 0;
   if (send == recv && identity) return b200collSuccess;
   const size_t nbytes = count * b200collTypeSize(ep->in_dtype);
-  if (bulk_enabled() && identity && nbytes >= bulk_min_bytes() && nbytes % 16 == 0 && aligned(recv, 16)) {
-    BulkArgs a = {};
-    a.nseg = 1; a.src[0] = static_cast<const char*>(send); a.bytes[0] = nbytes; a.dst_local = static_cast<char*>(recv);
-    return launch_bulk(c, a, false, b200collOpAllReduce, st);
-  }
+  if (bulk_enabled() && identity && nbytes >= bulk_min_bytes() && nbytes % 16 == 0 && aligned(send, 16) && aligned(recv, 16))
+    return launch_copy_bulk(c, send, recv, nbytes, st);
   return dispatch_types(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
     using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
     // streaming copy: no peers to wait for, so oversubscribe the chip (8 CTAs of 256 threads per SM) instead of the collective cap
@@ -198,7 +229,7 @@ static b200collResult_t launch_ll(b200collComm* c, b200collOp_t op, const void* 
     const InT* in = static_cast<const InT*>(send); OutT* out = static_cast<OutT*>(recv);
     const bool mc = c->nvls;
     const int identity = (ep->in_dtype == ep->out_dtype && scale == 1.0f) ? 1 : 0;     // movement only (SUM=false): store the words as received
-    struct PdlScope { PdlScope(bool v) { t_pdl_small = v; } ~PdlScope() { t_pdl_small = false; } } pdl_scope(count * sizeof(InT) <= pdl_max_bytes());
+    PdlScope pdl_scope(count * sizeof(InT) <= pdl_max_bytes());
     switch (op) {
       case b200collOpAllReduce:
         if (mc) launch_k(k_ll<InT, OutT, false, true, true>, g.blocks, g.threads, st, c->dev, in, out, count, scale, identity, op);
@@ -837,6 +868,14 @@ b200collResult_t b200collDebugPlanP2p(int rank, int nranks, int loopback, size_t
   g_p2p_dry = nullptr;
   snprintf(out, outlen, "%s", text.c_str());
   return rc;
+}
+
+b200collResult_t b200collDebugPlanCopy(size_t bytes, int sm_count, int* blocks, unsigned* chunk, unsigned* rounds, int* max_resident) {
+  if (!blocks || !chunk || !rounds || !max_resident || sm_count < 1) return b200collInvalidArgument;
+  const CopyPlan p = plan_copy(bytes, sm_count);
+  *blocks = p.blocks; *chunk = p.chunk; *rounds = p.rounds;
+  *max_resident = kCopyCtasPerSm * sm_count;
+  return b200collSuccess;
 }
 
 b200collResult_t b200collBarrier(b200collComm_t c, b200collStream_t stream) {

@@ -11,7 +11,8 @@
 //   k_a2av_push       all-to-all(v)                per-peer row ranges, flattened for load balance
 //   k_bcast           broadcast                    root pushes (P2P or one multimem.st per vector); the others only synchronise
 //   k_reduce_root     reduce                       the root pulls (or multimem.ld_reduce) the whole buffer; the others only synchronise
-//   k_bulk            identity epilogue, >= 1 MiB   all-gather / broadcast / all-to-all(v) / one-rank copy through the copy engine (cp.async.bulk ring)
+//   k_bulk            identity epilogue, >= 1 MiB   all-gather / broadcast / all-to-all(v) through the copy engine (cp.async.bulk ring)
+//   k_copy_bulk       nranks==1, identity, >= 1 MiB a deeper ring of the same kind, chunks planned on the host to fill whole rounds, PDL
 //   k_p2p             send / recv (grouped)        receiver posts where to write, sender pushes over NVLink and signals; no all-rank barrier
 //   k_barrier
 #pragma once
@@ -704,15 +705,15 @@ __global__ void __launch_bounds__(kThreads) k_reduce_root(COMM_PARAM, size_t in_
 }
 
 // ------------------------------------------------------------------------------------------------
-// Copy-engine data movement (TMA bulk copies): all-gather, broadcast, all-to-all(v) and the one-rank copy when the epilogue is the
-// identity (same dtype, scale 1) — the bytes are never looked at, so no register ever holds them. One elected thread per CTA drives a
+// Copy-engine data movement (TMA bulk copies): all-gather, broadcast, all-to-all(v) and (k_copy_bulk below) the one-rank copy when the
+// epilogue is the identity (same dtype, scale 1) — the bytes are never looked at, so no register ever holds them. One elected thread per CTA drives a
 // shared-memory ring:   cp.async.bulk global -> shared (completion counted on an mbarrier)      [SASS: UBLKCP.S.G + SYNCS.ARRIVE.TRANS64]
 //                       cp.async.bulk shared -> (peer) global, one per destination, one bulk group per chunk            [UBLKCP.G.S]
 // Loads run kStages-1 chunks ahead of the stores; a slot is reloaded once the group that stored from it has finished READING it
 // (cp.async.bulk.wait_group.read), so up to (kStages-1) loads and 2 store groups per CTA are in flight — enough outstanding bytes per SM
 // for HBM (one rank) and for NVLink (peers) without spending registers or issue slots on the payload.
 // The work is a list of segments (source range -> set of destinations), flattened into chunks and dealt round-robin to the CTAs:
-//   one-rank copy   1 segment, local destination            all-gather   1 segment -> every rank's out[rank]
+//   all-gather      1 segment -> every rank's out[rank]
 //   broadcast       root: 1 segment -> every rank; others: none (barriers only)
 //   all-to-all(v)   one segment per peer (staggered start so that all ranks do not hit the same peer at once)
 struct BulkArgs {
@@ -722,7 +723,6 @@ struct BulkArgs {
   unsigned long long chunk_prefix[kMaxRanks + 1]; // chunks before segment g
   unsigned long long dst_off[kMaxRanks];          // arena offset at the destination rank(s)
   unsigned dst_mask[kMaxRanks];                   // bit r: copy to rank r (peer[r] + dst_off)
-  char* dst_local;                                // one-rank copy: plain local destination instead of arena destinations (nseg == 1)
 };
 constexpr int kBulkStages = 4;
 constexpr uint32_t kBulkChunk = 16384;
@@ -778,15 +778,11 @@ __global__ void __launch_bounds__(kBulkThreads) k_bulk(COMM_PARAM, const __grid_
       if (dead) break;
       int seg; unsigned long long off; uint32_t n;
       locate(k, &seg, &off, &n);
-      if (a.dst_local) {
-        asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(a.dst_local + off), "r"(src_s), "r"(n) : "memory");
-      } else {
-        const unsigned mask = a.dst_mask[seg];
+      const unsigned mask = a.dst_mask[seg];
 #pragma unroll
-        for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
-          int r = c.rank + j; if (r >= c.nranks) r -= c.nranks;
-          if (mask & (1u << r)) asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(c.peer[r] + a.dst_off[seg] + off), "r"(src_s), "r"(n) : "memory");
-        }
+      for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
+        int r = c.rank + j; if (r >= c.nranks) r -= c.nranks;
+        if (mask & (1u << r)) asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(c.peer[r] + a.dst_off[seg] + off), "r"(src_s), "r"(n) : "memory");
       }
       asm volatile("cp.async.bulk.commit_group;" ::: "memory");
       if (k + ahead < mine) {
@@ -801,6 +797,71 @@ __global__ void __launch_bounds__(kBulkThreads) k_bulk(COMM_PARAM, const __grid_
     if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;
     if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
   }
+}
+
+// One-rank identity copy through a deeper ring of the same kind (6 slots of 16 KiB, 2 CTAs per SM), planned on the host (collectives.cu plan_copy): CTA b copies chunks b, b + gridDim.x,
+// ... of `chunk` bytes, a size chosen so that the chunks fill whole rounds of the grid and no CTA runs a ragged last round. No segment
+// search, no destination loop, no proxy fence (no flag store follows the copy), and the watchdog clock is read only once a wait has
+// spun past the first check interval. Loads and stores carry an L2 evict-first policy. Launched with programmatic dependent launch (launch.cuh says when that is safe): the next grid is
+// released at entry and this grid's loads start only after griddepcontrol.wait, so a chain of copies observes each predecessor's
+// completed stores.
+constexpr int kCopyStages = 6;                  // 96 KiB ring: 2 CTAs per SM (collectives.cu kCopyCtasPerSm)
+constexpr uint32_t kCopySlot = 16384;
+constexpr size_t kCopySmemBytes = (size_t)kCopyStages * kCopySlot;
+__global__ void __launch_bounds__(kBulkThreads) k_copy_bulk(COMM_PARAM, const char* __restrict__ src, char* __restrict__ dst,
+                                                            unsigned long long bytes, uint32_t chunk) {
+  asm volatile("griddepcontrol.launch_dependents;");
+  if (threadIdx.x != 0) return;
+  extern __shared__ __align__(128) char ring[];                  // [kCopyStages][kCopySlot]
+  __shared__ __align__(8) unsigned long long full[kCopyStages];
+  for (int i = 0; i < kCopyStages; i++) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&full[i])));
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  unsigned long long pol;                                        // every byte is read once and written once: evict it from L2 first
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  const unsigned long long nchunks = (bytes + chunk - 1) / chunk;
+  const uint32_t mine = nchunks > blockIdx.x ? (uint32_t)((nchunks - blockIdx.x + gridDim.x - 1) / gridDim.x) : 0u;
+  auto span = [&](uint32_t k, unsigned long long* off) {
+    *off = (blockIdx.x + (unsigned long long)k * gridDim.x) * chunk;
+    return (uint32_t)(bytes - *off < chunk ? bytes - *off : chunk);
+  };
+  auto load = [&](uint32_t k) {
+    unsigned long long off;
+    const uint32_t n = span(k, &off);
+    const uint32_t slot = k % kCopyStages;
+    const uint32_t bar = smem_u32(&full[slot]), dst_s = smem_u32(ring + (size_t)slot * kCopySlot);
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(n) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst_s), "l"(src + off), "r"(n), "r"(bar), "l"(pol) : "memory");
+  };
+  asm volatile("griddepcontrol.wait;" ::: "memory");             // the previous grid's stores (possibly our source) are visible
+  constexpr uint32_t ahead = kCopyStages - 1;
+  for (uint32_t k = 0; k < mine && k < ahead; k++) load(k);
+  bool dead = false;
+  for (uint32_t k = 0; k < mine && !dead; k++) {
+    const uint32_t slot = k % kCopyStages, parity = (k / kCopyStages) & 1u;
+    const uint32_t bar = smem_u32(&full[slot]), src_s = smem_u32(ring + (size_t)slot * kCopySlot);
+    uint32_t done = 0, spins = 0;
+    unsigned long long t0 = 0;
+    while (true) {
+      asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }" : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+      if (done) break;
+      if (((++spins) & 0x3FF) == 0) {                             // slow path: the deadline counts from the first check
+        const unsigned long long now = globaltimer_ns();
+        if (t0 == 0) t0 = now;
+        else if (now - t0 > c.timeout_ns) { record_fault(c, 5, (uint32_t)c.rank, k, slot, b200collOpAllReduce); dead = true; break; }   // the copy engine never delivered: report, do not hang
+      }
+    }
+    if (dead) break;
+    unsigned long long off;
+    const uint32_t n = span(k, &off);
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(dst + off), "r"(src_s), "r"(n), "l"(pol) : "memory");
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    if (k + ahead < mine) {
+      asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // every group but the one just committed has finished reading its slot
+      load(k + ahead);
+    }
+  }
+  // The ring must outlive the reads of the last stores; their writes complete with the grid, before any dependent's griddepcontrol.wait returns.
+  asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 
 }  // namespace b200coll

@@ -29,14 +29,21 @@ struct Grid { int blocks, threads; };
 // The overlap pays for tiny messages and costs time for larger ones (the early-launched grid sits on the SMs while its predecessor
 // still needs them, and its griddepcontrol.wait returns only after the predecessor's memory flush). So only launches whose message is
 // at most B200COLL_PDL_MAX_KB (default 8) carry the attribute; the cut-off has not been re-measured on multi-GPU H100 systems. launch_ll sets the flag for the launch it is about to make.
-inline thread_local bool t_pdl_small = false;
+// One exception, at every size: the one-rank copy-engine copy (k_copy_bulk). Its grid never exceeds what is resident at once (2 CTAs of
+// 96 KiB per SM), so every one of its CTAs already holds its slot when a dependent grid is released, and a dependent can only take
+// slots the copy does not need; what PDL saves there is the launch gap between back-to-back copies.
+inline thread_local bool t_pdl = false;
+struct PdlScope {           // the launches made while it lives carry the attribute (if pdl_enabled() allows it)
+  explicit PdlScope(bool v) { t_pdl = v; }
+  ~PdlScope() { t_pdl = false; }
+};
 inline size_t pdl_max_bytes() {
   static const size_t v = [] { const char* e = getenv("B200COLL_PDL_MAX_KB"); return (size_t)(e && *e ? atol(e) : 8) << 10; }();
   return v;
 }
 inline bool pdl_enabled() {
   static const bool on = [] { const char* e = getenv("B200COLL_PDL"); return !(e && *e == '0'); }();      // on unless B200COLL_PDL=0
-  return on && t_pdl_small && g_loopback_comms.load(std::memory_order_relaxed) == 0;
+  return on && t_pdl && g_loopback_comms.load(std::memory_order_relaxed) == 0;
 }
 template <typename... KArgs, typename... Args>
 static void launch_k_smem(void (*kernel)(KArgs...), int blocks, int threads, size_t smem, cudaStream_t st, Args&&... args) {
