@@ -5,7 +5,8 @@
 
 For each (tokens per rank, hidden, skew): device-timed dispatch of bf16 token rows to the ranks that own their experts, with
 (a) libb200coll all_to_all_v, bf16 on the wire; (b) the same with the fp8-e4m3 quantise fused into the dispatch kernel (half the
-bytes on NVLink, no separate cast kernel); (c) NCCL all_to_all_single with split sizes (torch.distributed, the way MoE stacks call it).
+bytes on NVLink, no separate cast kernel); (c) NCCL all_to_all_single with split sizes (torch.distributed, the way MoE stacks call it);
+(d) all_to_all_v_quantized, the block-scaled dispatch FP8 recipes use: e4m3 rows with one fp32 scale per 1x128 block, one kernel.
 Bus bandwidth = (bytes a rank sends off-chip, max over ranks) / time. Rank 0 prints one JSON line per shape."""
 from __future__ import annotations
 
@@ -32,6 +33,7 @@ def main() -> int:
     send = comm.empty(cap_rows * cap_hidden, torch.bfloat16)
     recv = comm.empty(cap_rows * cap_hidden, torch.bfloat16)
     recv8 = comm.empty(cap_rows * cap_hidden, torch.float8_e4m3fn)
+    recv_scales = comm.empty(cap_rows * cap_hidden // 128, torch.float32)
     send.copy_((torch.arange(send.numel(), device="cuda") % 251).to(torch.bfloat16) * 0.01)
     nccl_recv = torch.empty(cap_rows * cap_hidden, dtype=torch.bfloat16, device="cuda")
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -61,6 +63,8 @@ def main() -> int:
         torch.cuda.synchronize()
         ok = bool(torch.equal(recv[:n_recv], nccl_recv[:n_recv]))
         us_fp8 = timed(lambda: comm.all_to_all_v(send, recv8, hidden, rows, so, ro, scale=1.0))
+        q_rows = plan.max_rows                                   # the same on every rank, as the symmetric recv needs
+        us_bsq = timed(lambda: comm.all_to_all_v_quantized(send, recv8[:q_rows * hidden], recv_scales[:q_rows * hidden // 128], hidden, rows, so, ro, block=128))
         us_nccl = timed(lambda: dist.all_to_all_single(nccl_recv[:n_recv], send[:n_send], out_split, in_split))
         offchip = max(int(plan.rows[s].sum() - plan.rows[s, s]) for s in range(world)) * hidden * 2
         oks = torch.tensor([1.0 if ok else 0.0], device="cuda"); dist.all_reduce(oks, op=dist.ReduceOp.MIN)
@@ -69,7 +73,8 @@ def main() -> int:
                               "max_offchip_bytes_per_rank": offchip, "imbalance_max_over_mean": round(float(plan.rows.sum(axis=0).max() / plan.rows.sum(axis=0).mean()), 3),
                               "ours_us": round(us_ours, 2), "ours_busbw": round(offchip / us_ours / 1e3, 2), "ours_fused_fp8_us": round(us_fp8, 2),
                               "nccl_us": round(us_nccl, 2), "nccl_busbw": round(offchip / us_nccl / 1e3, 2), "speedup": round(us_nccl / us_ours, 2),
-                              "fp8_speedup_vs_nccl_bf16": round(us_nccl / us_fp8, 2), "matches_nccl": bool(oks.item() == 1.0)}), flush=True)
+                              "fp8_speedup_vs_nccl_bf16": round(us_nccl / us_fp8, 2), "matches_nccl": bool(oks.item() == 1.0),
+                              "ours_block_fp8_us": round(us_bsq, 2)}), flush=True)
     comm.destroy()
     dist.destroy_process_group()
     return 0

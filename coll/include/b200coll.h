@@ -298,6 +298,32 @@ b200collResult_t b200collReduceScatterQuantized(const void* send, void* recv, si
                                                 const b200collEpilogue* ep, b200collRedOp_t op, b200collComm_t comm, b200collStream_t stream);
 b200collResult_t b200collAllReduceQuantized(const void* send, void* recv, size_t count, b200collDataType_t wire_dtype, int block,
                                             const b200collEpilogue* ep, b200collRedOp_t op, b200collComm_t comm, b200collStream_t stream);
+/* Quantising all-to-all-v (expert dispatch): bf16, fp16 or fp32 rows in, FP8 rows and their block scales out, one kernel per call. The
+ * row geometry is b200collAllToAllv's: send_rows[p] rows of row_elems elements, starting at row send_row_off[p] of send, go to peer p and
+ * land at row recv_row_off_at_peer[p] of that peer's recv and recv_scales (host arrays of length nranks). The sender quantises in
+ * registers and pushes FP8 and scales straight into each receiver's buffers: row_elems * (1 + 4 / block) bytes per row cross NVLink.
+ *   Per-row blocks: every row is cut into blocks of `block` consecutive elements (row_elems % block == 0), each quantised by the rule
+ *   above (amax the largest bit pattern of |x|; inv and s IEEE divisions, inv = s = 1 when amax == 0 or inv is +inf; q = satfinite
+ *   RNE(x * inv)), so a row's q and s are the bits b200collAllGatherQuantized writes into its scratch for the same block.
+ *   recv: [recv_rows, row_elems] of wire_dtype. recv_scales: [recv_rows, row_elems / block] fp32, row-major: the block_rows = 1,
+ *   block_cols = block layout of b200collBlockScale, so the result is also an input of the block-scaled collectives. Rows outside the
+ *   received ranges are not written.
+ *   in_dtype bf16, fp16 or fp32; wire_dtype e4m3 or e5m2; block 16, 32, 64, 128, 256 or 512.
+ *   recv_rows: the rows recv and recv_scales hold, the same on every rank (they are symmetric allocations). Every destination range
+ *   [recv_row_off_at_peer[p], + send_rows[p]) must lie inside it, else InvalidArgument before anything is launched.
+ * Placement: send any 16-byte aligned device buffer (only its own rank reads it). With more than one rank, recv and recv_scales must be
+ * arena memory at the same offsets on every rank, else InvalidUsage; with B200COLL_CHECK=1 on multi-process communicators, ranks that
+ * disagree on (recv_rows, recv, recv_scales) get InvalidUsage instead of a watchdog fault. send overlapping recv or recv_scales, or recv
+ * overlapping recv_scales, is InvalidArgument.
+ * Other arguments (InvalidArgument, message in b200collGetLastError): null pointers, negative counts or offsets, send or recv not 16-byte
+ * aligned or recv_scales not 4-byte aligned, more than 2^31 - 1 16-element vectors sent per rank. A poisoned communicator gives RemoteError.
+ * Every rank launches on every call, a rank that sends nothing included (its peers' barriers wait for it), as with b200collAllToAllv.
+ * One rank: a local quantising copy with no barrier, recv and recv_scales any device buffers, counted as copy.
+ * b200collStats count the input bytes sent under alltoall, algorithm twoshot (or copy). */
+b200collResult_t b200collAllToAllvQuantized(const void* send, void* recv, float* recv_scales, size_t row_elems, size_t recv_rows,
+                                            const int64_t* send_rows, const int64_t* send_row_off, const int64_t* recv_row_off_at_peer,
+                                            b200collDataType_t in_dtype, b200collDataType_t wire_dtype, int block,
+                                            b200collComm_t comm, b200collStream_t stream);
 
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.

@@ -20,6 +20,11 @@
 //   k_quant_pull_reduce<InT, WireT, OutT, true>   two-shot all-reduce: the same over my block slice, the result pushed into every recv
 //   k_quant_copy<InT, WireT, OutT>                one rank: the quantise / dequantise round trip in registers, no scratch, no barrier
 //
+// Quantising all-to-all-v (expert dispatch): bf16, fp16 or fp32 rows in, FP8 rows and their per-row block scales out, one kernel:
+//
+//   k_a2av_quant_push<InT, WireT>   barrier, quantise my rows for every peer and push FP8 and scales into its recv, barrier (releases)
+//   k_a2av_quant_copy<InT, WireT>   one rank: a local quantising copy, no barrier
+//
 // Scales: a 16-byte FP8 vector lies in exactly one block (row_len and block_cols are multiples of 16; a quantising block is a whole
 // number of vectors), so a vector needs one scale per rank. Lanes of a warp hold consecutive vectors and usually share scales (8 lanes
 // per 1x128 block, whole warps per 128x128 block): __match_any_sync groups the lanes by scale index, the lowest lane of each group loads
@@ -53,6 +58,7 @@
 
 #include <type_traits>
 
+#include "a2av.h"
 #include "comm.h"
 #include "launch.cuh"
 
@@ -364,6 +370,50 @@ __global__ void __launch_bounds__(kBsqThreads, 1) k_quant_pull_reduce(COMM_PARAM
   if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
 }
 
+// Quantising all-to-all-v. A2AvArgs counts 16-element vectors here: src_vec[p] of my send, dst_vec[p] of peer p's recv (FP8, 16 bytes
+// per vector), and the prefix over the staggered peer order. The scale of destination vector d is fp32 element d >> lvpb of the peer's
+// recv_scales. Blocks never straddle a warp or a peer's segment: every prefix entry and every destination offset is whole rows, a row is
+// whole blocks, and a block is a power of two of at most 32 vectors. So warp_walk's 32-aligned warps hold whole blocks of one segment
+// (a block's lanes are one aligned lane group, all active or all idle), and quant_vec's butterfly sees exactly the block's lanes.
+template <typename InT, typename WireT>
+__global__ void __launch_bounds__(kBsqThreads) k_a2av_quant_push(COMM_PARAM, const char* __restrict__ in, size_t q_off, size_t s_off,
+                                                                 const __grid_constant__ A2AvArgs a, uint32_t lvpb, uint32_t op) {
+  pdl_prologue();
+  const uint32_t s = load_seq(c, kSeqBarrier);
+  if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;          // every peer has entered the call: its recv is free to overwrite
+  const uint32_t lane = threadIdx.x & 31, gl = 1u << lvpb;
+  warp_walk(0, (uint32_t)a.prefix[c.nranks], [&](uint32_t v, bool act) {
+    int p = 0;
+    uint32_t lv = 0;
+    float x[16] = {};
+    if (act) {
+      int j = 0;
+#pragma unroll
+      for (int q = 1; q < kMaxRanks; q++) if (q < c.nranks && v >= a.prefix[q]) j = q;
+      p = c.rank + 1 + j; if (p >= c.nranks) p -= c.nranks;
+      lv = v - (uint32_t)a.prefix[j];
+      quant_load16<InT>(in + (a.src_vec[p] + lv) * (16 * sizeof(InT)), x);
+    }
+    float sc;
+    const uint4 w = quant_vec<WireT>(x, gl, &sc);
+    if (act) {
+      const unsigned long long d = a.dst_vec[p] + lv;
+      st_vec(c.peer[p] + q_off + d * 16, w);
+      if ((lane & (gl - 1)) == 0) *reinterpret_cast<float*>(c.peer[p] + s_off + (d >> lvpb) * 4) = sc;
+    }
+  });
+  if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // releases my stores to their receivers
+  if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
+}
+
+// One rank: vectors [0, g.nvec) of in quantised into q and scales (all three already offset to the first row), no barrier
+template <typename InT, typename WireT>
+__global__ void __launch_bounds__(kBsqThreads) k_a2av_quant_copy(const __grid_constant__ QuantGeom g, const char* __restrict__ in, char* __restrict__ q,
+                                                                 char* __restrict__ scales) {
+  pdl_prologue();
+  quant_range<InT, WireT>(g, in, q, scales, 0, g.nvec);
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 // (wire, out) -> f(Tag<WireT>, Tag<OutT>); the argument checks have refused every other type
 template <typename F>
@@ -596,6 +646,59 @@ static b200collResult_t quant_reduce(const QuantCall& k, b200collOp_t which, b20
   });
 }
 
+// ---- quantising all-to-all-v
+// (in, wire) -> f(Tag<InT>, Tag<WireT>)
+template <typename F>
+static b200collResult_t dispatch_in_wire(b200collDataType_t in, b200collDataType_t wire, F&& f) {
+  return dispatch_quant(in, wire, b200collFloat32, [&](auto ti, auto tw, auto) { return f(ti, tw); });
+}
+
+// Everything b200collAllToAllvQuantized checks before it launches; on success `a` holds the vector geometry (prefix not yet filled),
+// `nv` the vectors per peer and `in_bytes` the input bytes sent.
+static b200collResult_t a2aq_prepare(b200collComm* c, const void* send, void* recv, float* recv_scales, size_t row_elems, size_t recv_rows,
+                                     const int64_t* send_rows, const int64_t* send_row_off, const int64_t* recv_row_off_at_peer,
+                                     b200collDataType_t in_dtype, b200collDataType_t wire, int block, A2AvArgs* a, unsigned long long* nv,
+                                     size_t* in_bytes) {
+  auto refuse = [](const std::string& msg) { set_last_error("quantised all-to-all-v: " + msg); return b200collInvalidArgument; };
+  if (!c || !send || !recv || !recv_scales || !send_rows || !send_row_off || !recv_row_off_at_peer) return refuse("null argument");
+  if (!wide_type(in_dtype)) return refuse("in_dtype must be bf16, fp16 or fp32");
+  if (!is_fp8(wire)) return refuse("wire_dtype must be e4m3 or e5m2");
+  if (block < 16 || block > 512 || (block & (block - 1)) != 0) return refuse("block must be 16, 32, 64, 128, 256 or 512");
+  if (row_elems == 0 || row_elems % (size_t)block != 0) return refuse("row_elems must be a positive multiple of block");
+  if (!aligned(send, 16) || !aligned(recv, 16) || !aligned(recv_scales, 4)) return refuse("send and recv must be 16-byte aligned, recv_scales 4-byte aligned");
+  const size_t is = b200collTypeSize(in_dtype);
+  const size_t max_rows = (SIZE_MAX >> 4) / (row_elems * is);     // every byte offset below then fits in size_t with room to spare
+  if (recv_rows > max_rows) return refuse("recv_rows * row_elems is too large");
+  const unsigned long long row_vecs = row_elems / 16, max_vecs = (1ull << 31) - 1;
+  unsigned long long total = 0;
+  size_t send_end = 0;                                            // the bytes of send that are read
+  *in_bytes = 0;
+  for (int p = 0; p < c->nranks; p++) {
+    if (send_rows[p] < 0 || send_row_off[p] < 0 || recv_row_off_at_peer[p] < 0) return refuse("negative row count or offset");
+    const size_t rows = (size_t)send_rows[p], src = (size_t)send_row_off[p], dst = (size_t)recv_row_off_at_peer[p];
+    if (rows > recv_rows || dst > recv_rows - rows)
+      return refuse("rows for peer " + std::to_string(p) + " land at [" + std::to_string(dst) + ", +" + std::to_string(rows) + "), past recv_rows = " + std::to_string(recv_rows));
+    if (src > max_rows || rows > max_rows - src) return refuse("the send range of peer " + std::to_string(p) + " is too large");
+    if (rows > (max_vecs - total) / row_vecs) return refuse("at most 2^31 - 1 16-element vectors may be sent per rank");
+    total += rows * row_vecs;
+    a->src_vec[p] = src * row_vecs;
+    a->dst_vec[p] = dst * row_vecs;
+    nv[p] = rows * row_vecs;
+    *in_bytes += rows * row_elems * is;
+    if (rows) send_end = std::max(send_end, (src + rows) * row_elems * is);
+  }
+  if (comm_poisoned(c)) return b200collRemoteError;
+  const size_t q_bytes = recv_rows * row_elems, s_bytes = recv_rows * (row_elems / (size_t)block) * 4;
+  if (overlaps(send, send_end, recv, q_bytes) || overlaps(send, send_end, recv_scales, s_bytes)) return refuse("send must not overlap recv or recv_scales");
+  if (overlaps(recv, q_bytes, recv_scales, s_bytes)) return refuse("recv and recv_scales must not overlap");
+  // peers store into my recv and recv_scales at MY arena offsets: both must be arena memory
+  if (c->nranks > 1 && (!b200collIsSymmetric(c, recv, std::max<size_t>(q_bytes, 1)) || !b200collIsSymmetric(c, recv_scales, std::max<size_t>(s_bytes, 1)))) {
+    set_last_error("quantised all-to-all-v: recv and recv_scales must lie in the symmetric arena (b200collMemAlloc), at the same offsets on every rank");
+    return b200collInvalidUsage;
+  }
+  return b200collSuccess;
+}
+
 }  // namespace b200coll
 
 using namespace b200coll;
@@ -699,6 +802,50 @@ b200collResult_t b200collAllReduceQuantized(const void* send, void* recv, size_t
   if (rc != b200collSuccess) return rc;
   account(c, b200collOpAllReduce, k.in_bytes, algo);
   return quant_reduce(k, b200collOpAllReduce, algo, send, recv, wire_dtype, ep, st);
+}
+
+b200collResult_t b200collAllToAllvQuantized(const void* send, void* recv, float* recv_scales, size_t row_elems, size_t recv_rows,
+                                            const int64_t* send_rows, const int64_t* send_row_off, const int64_t* recv_row_off_at_peer,
+                                            b200collDataType_t in_dtype, b200collDataType_t wire_dtype, int block,
+                                            b200collComm_t c, b200collStream_t stream) {
+  A2AvArgs a = {};
+  unsigned long long nv[kMaxRanks] = {};
+  size_t in_bytes = 0;
+  b200collResult_t rc = a2aq_prepare(c, send, recv, recv_scales, row_elems, recv_rows, send_rows, send_row_off, recv_row_off_at_peer, in_dtype, wire_dtype,
+                                     block, &a, nv, &in_bytes);
+  if (rc != b200collSuccess) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  uint32_t lvpb = 0;
+  while ((16u << lvpb) < (uint32_t)block) lvpb++;
+  if (c->nranks == 1) {
+    account(c, b200collOpAllToAll, in_bytes, b200collAlgoCopy);
+    if (nv[0] == 0) return b200collSuccess;
+    QuantGeom g = {};
+    g.nvec = (uint32_t)nv[0];
+    g.lvpb = lvpb;
+    const char* in = static_cast<const char*>(send) + a.src_vec[0] * 16 * b200collTypeSize(in_dtype);
+    char* q = static_cast<char*>(recv) + a.dst_vec[0] * 16;
+    char* s = reinterpret_cast<char*>(recv_scales) + (a.dst_vec[0] >> lvpb) * 4;
+    return dispatch_in_wire(in_dtype, wire_dtype, [&](auto ti, auto tw) -> b200collResult_t {
+      using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type;
+      launch_k(k_a2av_quant_copy<InT, WireT>, copy_blocks(c, g.nvec), 256, st, g, in, q, s);
+      LAUNCH_CHECK(c);
+      return b200collSuccess;
+    });
+  }
+  rc = cross_check(c, b200collOpAllToAll, b200collAlgoTwoShot, recv_rows, arena_off(c, recv), arena_off(c, recv_scales));
+  if (rc != b200collSuccess) return rc;
+  a2av_prefix(c->rank, c->nranks, nv, &a);
+  account(c, b200collOpAllToAll, in_bytes, b200collAlgoTwoShot);
+  // the full P2P grid on every rank, whatever it sends: CTA b meets CTA b of every peer in the barriers (see a2av_launch)
+  const Grid gr = warp_grid(c, ~(size_t)0 >> 8);
+  return dispatch_in_wire(in_dtype, wire_dtype, [&](auto ti, auto tw) -> b200collResult_t {
+    using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type;
+    launch_k(k_a2av_quant_push<InT, WireT>, gr.blocks, gr.threads, st, c->dev, static_cast<const char*>(send), arena_off(c, recv), arena_off(c, recv_scales), a,
+             lvpb, (uint32_t)b200collOpAllToAll);
+    LAUNCH_CHECK(c);
+    return b200collSuccess;
+  });
 }
 
 }  // extern "C"

@@ -639,16 +639,6 @@ static b200collResult_t a2av_launch(b200collComm* c, const void* send, void* rec
   });
 }
 
-// Fill the flattened prefix in the kernel's staggered order (j -> peer rank+1+j).
-static void a2av_prefix(const b200collComm* c, const unsigned long long* nvec_by_peer, A2AvArgs* a) {
-  a->prefix[0] = 0;
-  for (int j = 0; j < c->nranks; j++) {
-    int p = c->rank + 1 + j; if (p >= c->nranks) p -= c->nranks;
-    a->prefix[j + 1] = a->prefix[j] + nvec_by_peer[p];
-  }
-  for (int j = c->nranks + 1; j <= kMaxRanks; j++) a->prefix[j] = a->prefix[c->nranks];
-}
-
 b200collResult_t b200collAllToAll(const void* send, void* recv, size_t count, const b200collEpilogue* ep, b200collComm_t c, b200collStream_t stream) {
   b200collResult_t rc = check_common(c, send, recv, ep);
   if (rc != b200collSuccess) return rc;
@@ -670,7 +660,7 @@ b200collResult_t b200collAllToAll(const void* send, void* recv, size_t count, co
     A2AvArgs a = {};
     unsigned long long nv[kMaxRanks] = {};
     for (int p = 0; p < c->nranks; p++) { a.src_vec[p] = (unsigned long long)p * s_stride_elems / E; a.dst_vec[p] = (unsigned long long)c->rank * n / E; nv[p] = n / E; }
-    a2av_prefix(c, nv, &a);
+    a2av_prefix(c->rank, c->nranks, nv, &a);
     account(c, b200collOpAllToAll, n * is * c->nranks, algo);
     return a2av_launch(c, s, r_sym, a, ep, st, true);
   };
@@ -733,7 +723,7 @@ b200collResult_t b200collAllToAllv(const void* send, void* recv, size_t row_elem
     nv[p] = (unsigned long long)send_rows[p] * row_vecs;
     total_bytes += (size_t)send_rows[p] * row_elems * is;
   }
-  a2av_prefix(c, nv, &a);
+  a2av_prefix(c->rank, c->nranks, nv, &a);
   account(c, b200collOpAllToAll, total_bytes, b200collAlgoTwoShot);
   return a2av_launch(c, send, recv, a, ep, st, false);
 }

@@ -16,6 +16,7 @@
 //   k_p2p             send / recv (grouped)        receiver posts where to write, sender pushes over NVLink and signals; no all-rank barrier
 //   k_barrier
 #pragma once
+#include "a2av.h"
 #include "device.cuh"
 
 namespace b200coll {
@@ -522,14 +523,9 @@ __global__ void __launch_bounds__(kThreads) k_ag_push(COMM_PARAM, const InT* __r
 }
 
 // ------------------------------------------------------------------------------------------------
-// All-to-all(v) push. Per destination p: nvec[p] input vectors starting at vector src_vec[p] of my send
+// All-to-all(v) push (A2AvArgs in a2av.h). Per destination p: nvec[p] input vectors starting at vector src_vec[p] of my send
 // buffer go to output-vector offset dst_vec[p] (units of E*sizeof(OutT) bytes) of peer p's recv buffer.
 // The (peer, vector) space is flattened with a prefix table so skewed expert loads still spread over all CTAs.
-struct A2AvArgs {
-  unsigned long long src_vec[kMaxRanks];
-  unsigned long long dst_vec[kMaxRanks];
-  unsigned long long prefix[kMaxRanks + 1];   // prefix over the staggered order j = 0..nranks-1 (peer = rank+1+j)
-};
 template <typename InT, typename OutT>
 __global__ void __launch_bounds__(kThreads) k_a2av_push(COMM_PARAM, const InT* __restrict__ in, size_t out_off, A2AvArgs a, float scale, int identity, uint32_t op) {
   pdl_prologue();

@@ -79,10 +79,16 @@ static uint32_t got_bits(const void* p, size_t i, b200collDataType_t dt) {
   uint16_t u; memcpy(&u, (const char*)p + 2 * i, 2); return u;
 }
 
+// The quantising all-to-all-v receives one fp32 scale per block of its FP8 rows, into an arena buffer that holds the scales of a whole
+// window or of the largest message.
+static size_t q_a2a_scale_bytes(const Opts& o) {
+  return (std::max(o.window, o.max_bytes) + 4096) / b200collTypeSize(o.in_dt) / o.q_block * 4 + 4096;
+}
 // The library's quantisation scratch (FP8 copy plus scales per rank) grows with the sweep and keeps every superseded buffer: reserve
-// twice the largest one.
+// twice the largest one. The all-to-all-v takes no scratch, only its scale buffer.
 static size_t q_scratch_bytes(const Opts& o) {
   if (!o.q_block) return 0;
+  if (o.op == "alltoall") return q_a2a_scale_bytes(o);
   const size_t elems = o.max_bytes / b200collTypeSize(o.in_dt);
   return 2 * (elems + elems / o.q_block * 4) + (4u << 20);
 }
@@ -115,9 +121,9 @@ template <typename T> __global__ void k_fill_q(T* p, size_t n, int rank, int blo
     p[i] = T(v * ldexpf(1.0f, (int)(((i / block) * 5 + (size_t)rank * 3) % 13) - 6));
   }
 }
-// The dequantised value of rank r's element i; `memo` keeps the last block's (index, inv, s), as the check walks elements in order.
+// The FP8 code of rank r's element i; `memo` keeps the last block's (index, inv, s), as the check walks elements in order.
 struct QMemo { size_t blk = SIZE_MAX; float inv = 1.0f, s = 1.0f; };
-static float q_val(const Opts& o, int rank, size_t i, QMemo* memo) {
+static __nv_fp8_storage_t q_code(const Opts& o, int rank, size_t i, QMemo* memo) {
   const size_t blk = i / o.q_block;
   const float fmax = o.q_wire == b200collFloat8e4m3 ? 448.0f : 57344.0f;
   if (memo->blk != blk) {
@@ -129,9 +135,12 @@ static float q_val(const Opts& o, int rank, size_t i, QMemo* memo) {
     *memo = QMemo{blk, inv, s};
   }
   const float y = q_in(o, rank, i) * memo->inv;
-  const __nv_fp8_interpretation_t I = o.q_wire == b200collFloat8e4m3 ? __NV_E4M3 : __NV_E5M2;
-  const __nv_fp8_storage_t q = __nv_cvt_float_to_fp8(y, __NV_SATFINITE, I);
-  return __half2float(__half(__nv_cvt_fp8_to_halfraw(q, I))) * memo->s;
+  return __nv_cvt_float_to_fp8(y, __NV_SATFINITE, o.q_wire == b200collFloat8e4m3 ? __NV_E4M3 : __NV_E5M2);
+}
+// ... and its dequantised value
+static float q_val(const Opts& o, int rank, size_t i, QMemo* memo) {
+  const __nv_fp8_storage_t q = q_code(o, rank, i, memo);
+  return __half2float(__half(__nv_cvt_fp8_to_halfraw(q, o.q_wire == b200collFloat8e4m3 ? __NV_E4M3 : __NV_E5M2))) * memo->s;
 }
 
 template <typename T> __global__ void k_fill(T* p, size_t n, int rank, size_t base) {
@@ -215,13 +224,17 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
   void *send = nullptr, *recv = nullptr;
   CC(b200collMemAlloc(ctx.comm, &send, send_cap + 4096));
   CC(b200collMemAlloc(ctx.comm, &recv, recv_cap + 4096));
-  const bool bs_mode = o.bs_rows > 0, q_mode = o.q_block > 0;
-  if (q_mode && ((o.op != "all_gather" && o.op != "reduce_scatter" && o.op != "all_reduce") || bs_mode ||
-                 (o.in_dt != b200collBfloat16 && o.in_dt != b200collFloat16 && o.in_dt != b200collFloat32) ||
-                 (o.out_dt != b200collBfloat16 && o.out_dt != b200collFloat16 && o.out_dt != b200collFloat32))) {
-    fprintf(stderr, "--quantize takes --op all_gather, reduce_scatter or all_reduce, -d and --out-dtype bfloat16|half|float, and no --block-scale\n");
+  const bool bs_mode = o.bs_rows > 0, q_mode = o.q_block > 0, is_a2a = o.op == "alltoall";
+  const bool wide_in = o.in_dt == b200collBfloat16 || o.in_dt == b200collFloat16 || o.in_dt == b200collFloat32;
+  const bool wide_out = o.out_dt == b200collBfloat16 || o.out_dt == b200collFloat16 || o.out_dt == b200collFloat32;
+  if (q_mode && ((o.op != "all_gather" && o.op != "reduce_scatter" && o.op != "all_reduce" && !is_a2a) || bs_mode || !wide_in ||
+                 (is_a2a ? o.out_dt != o.q_wire || o.row_len % o.q_block != 0 : !wide_out))) {
+    fprintf(stderr, "--quantize takes --op all_gather, reduce_scatter or all_reduce with -d and --out-dtype bfloat16|half|float, or --op alltoall with\n"
+                    "-d bfloat16|half|float, --out-dtype WIRE (or none) and a --row-len that is a multiple of BLOCK; and no --block-scale\n");
     return 2;
   }
+  float* q_scales = nullptr;                                     // quantising alltoall: the received scales, one window of them
+  if (q_mode && is_a2a) CC(b200collMemAlloc(ctx.comm, (void**)&q_scales, q_a2a_scale_bytes(o)));
   float* scales = nullptr;
   std::vector<float> host_scales;
   if (bs_mode) {
@@ -237,6 +250,7 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
            info.nvls, info.same_device_loopback, o.procs ? "procs" : "threads");
     if (bs_mode) printf("# block-scaled: row_len=%zu block=%dx%d (one fp32 scale per block, seeded)\n", o.row_len, o.bs_rows, o.bs_cols);
     if (q_mode) printf("# quantised: wire=%s block=%d (each rank quantises its input, one fp32 scale per block)\n", dt_name(o.q_wire), o.q_block);
+    if (q_mode && is_a2a) printf("# all-to-all-v: an even split of whole %zu-element rows to every peer; FP8 rows and scales are checked\n", o.row_len);
     printf("#%13s %12s %6s %8s | %10s %8s %8s %6s | %10s %8s %8s %6s\n", "size(B)", "count", "type", "algo", "oop us", "algbw", "busbw", "#wrong", "ip us", "algbw", "busbw", "#wrong");
     fflush(stdout);
   }
@@ -255,7 +269,12 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
     if (!is_ar) count = count / E * E;
     if (bs_mode) count = count / o.row_len * o.row_len;      // whole rows on every rank (reduce-scatter: rows = n * count / row_len)
     if (q_mode) count = count / o.q_block * o.q_block;       // whole blocks on every rank (reduce-scatter: every slice)
+    if (q_mode && is_a2a) count = count / o.row_len * o.row_len;      // whole rows to every peer
     if (count == 0) continue;
+    // quantising alltoall: rpp rows to every peer; rank r's rows for p start at row p * rpp and land at row r * rpp of p's recv
+    const size_t rpp = count / o.row_len;
+    std::vector<int64_t> a2a_rows(n, (int64_t)rpp), a2a_soff(n), a2a_roff(n, (int64_t)(rank * rpp));
+    for (int p = 0; p < n; p++) a2a_soff[p] = (int64_t)(p * rpp);
     const size_t bs_rows_total = bs_mode ? (is_rs ? count * n : count) / o.row_len : 0;
     const size_t bs_ncb = bs_mode ? (o.row_len + o.bs_cols - 1) / o.bs_cols : 0;
     const size_t bs_nscales = bs_mode ? (bs_rows_total + o.bs_rows - 1) / o.bs_rows * bs_ncb : 0;
@@ -291,6 +310,7 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
         if (ip && is_rs) off += (size_t)rank * count * is;     // in-place reduce-scatter: recv = send + rank*count
         return (char*)recv + off;
       };
+      auto qsbuf = [&](int slot) -> float* { return q_scales + (size_t)slot * (slot_b / is / o.q_block); };   // the scales of rbuf(slot)
       auto launch = [&](int slot) {
         if (is_hc) {
           RT(cudaMemcpyAsync(rbuf(slot) + (size_t)rank * count * is, sbuf(slot), count * is, cudaMemcpyDeviceToDevice, st));
@@ -321,6 +341,9 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
         else if (q_mode && is_ar) CC(b200collAllReduceQuantized(sbuf(slot), rbuf(slot), count, o.q_wire, o.q_block, &ep, b200collSum, ctx.comm, st));
         else if (q_mode && is_ag) CC(b200collAllGatherQuantized(sbuf(slot), rbuf(slot), count, o.q_wire, o.q_block, &ep, ctx.comm, st));
         else if (q_mode && is_rs) CC(b200collReduceScatterQuantized(sbuf(slot), rbuf(slot), count, o.q_wire, o.q_block, &ep, b200collSum, ctx.comm, st));
+        else if (q_mode && is_a2a)
+          CC(b200collAllToAllvQuantized(sbuf(slot), rbuf(slot), qsbuf(slot), o.row_len, rpp * n, a2a_rows.data(), a2a_soff.data(), a2a_roff.data(), o.in_dt, o.q_wire,
+                                        o.q_block, ctx.comm, st));
         else if (bs_mode && is_ar) CC(b200collAllReduceBlockScaled(sbuf(slot), rbuf(slot), count, &bsd, &ep, b200collSum, ctx.comm, st));
         else if (bs_mode && is_ag) CC(b200collAllGatherBlockScaled(sbuf(slot), rbuf(slot), count, &bsd, &ep, ctx.comm, st));
         else if (bs_mode && is_rs) CC(b200collReduceScatterBlockScaled(sbuf(slot), rbuf(slot), count, &bsd, &ep, b200collSum, ctx.comm, st));
@@ -335,6 +358,7 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
       long errs = 0;
       if (o.check) {
         if (!ip) RT(cudaMemsetAsync(rbuf(0), 0x5A, out_b, st));
+        if (q_mode && is_a2a) RT(cudaMemsetAsync(qsbuf(0), 0x5A, out_elems / o.q_block * 4, st));
         if (q_mode) {
           void* p = sbuf(0);
           if (o.in_dt == b200collFloat32) k_fill_q<float><<<256, 256, 0, st>>>((float*)p, in_elems, rank, o.q_block);
@@ -366,7 +390,25 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
           if (got != want) { if (errs < 4) fprintf(stderr, "rank %d %s block-scaled size %zu elem %zu: got bits 0x%x want 0x%x\n", rank, o.op.c_str(), bytes, e, got, want); errs++; }
         }
         std::vector<QMemo> memo(n);
-        for (size_t e = 0; e < check_elems && q_mode; e += stride) {      // bit for bit: ((0 + v_0) + v_1 + ...) * scale, rounded once
+        if (q_mode && is_a2a) {      // bit for bit: my recv element e is rank e / count's element rank * count + e % count, quantised
+          for (size_t e = 0; e < check_elems; e += stride) {
+            const int src = (int)(e / count);
+            const uint32_t want = q_code(o, src, (size_t)rank * count + e % count, &memo[src]), got = (unsigned char)host[e];
+            if (got != want) { if (errs < 4) fprintf(stderr, "rank %d alltoall quantised size %zu elem %zu: got FP8 0x%x want 0x%x\n", rank, bytes, e, got, want); errs++; }
+          }
+          const size_t nsc = out_elems / o.q_block, sstride = nsc > (1u << 18) ? 61 : 1;
+          std::vector<float> got_s(nsc);
+          RT(cudaMemcpy(got_s.data(), qsbuf(0), nsc * 4, cudaMemcpyDeviceToHost));
+          std::vector<QMemo> smemo(n);
+          for (size_t j = 0; j < nsc; j += sstride) {
+            const size_t e = j * o.q_block;
+            const int src = (int)(e / count);
+            q_code(o, src, (size_t)rank * count + e % count, &smemo[src]);
+            const uint32_t want = out_bits(smemo[src].s, b200collFloat32), got = out_bits(got_s[j], b200collFloat32);
+            if (got != want) { if (errs < 4) fprintf(stderr, "rank %d alltoall quantised size %zu scale %zu: got bits 0x%x want 0x%x\n", rank, bytes, j, got, want); errs++; }
+          }
+        }
+        for (size_t e = 0; e < check_elems && q_mode && !is_a2a; e += stride) {      // bit for bit: ((0 + v_0) + v_1 + ...) * scale, rounded once
           float acc = 0.0f;
           if (is_ag) acc += q_val(o, (int)(e / count), e % count, &memo[e / count]);
           else for (int r = 0; r < n; r++) acc += q_val(o, r, is_rs ? (size_t)rank * count + e : e, &memo[r]);
@@ -402,6 +444,7 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
       size_t tb = is_ar ? count * is : count * is * n;   // nccl-tests "size"
       b200collOp_t opid = is_bc ? b200collOpBroadcast : is_rd ? b200collOpReduce : is_ar ? b200collOpAllReduce : is_ag ? b200collOpAllGather : is_rs ? b200collOpReduceScatter : b200collOpAllToAll;
       if (is_sr || is_ga || is_sc) algo_used = "p2p";
+      else if (q_mode && is_a2a) algo_used = n > 1 ? "twoshot" : "copy";
       else if (o.algo == "auto") algo_used = b200collAlgoName(b200collTunerPick(opid, is_ar ? count * is : count * is, n, info.nvls)); else algo_used = o.algo.c_str();
       const double factor = (is_bc || is_rd || is_sr) ? 1.0 : is_ar ? 2.0 * (n - 1) / n : (double)(n - 1) / n;
       double ab[2], bb[2];
@@ -426,6 +469,7 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
     fflush(stdout);      // --procs children leave through _exit(): nothing buffered survives it
   }
   if (scales) CC(b200collMemFree(ctx.comm, scales));
+  if (q_scales) CC(b200collMemFree(ctx.comm, q_scales));
   CC(b200collMemFree(ctx.comm, recv));
   CC(b200collMemFree(ctx.comm, send));
   RT(cudaStreamDestroy(st));
@@ -466,6 +510,7 @@ static LauncherRank launcher_rank() {
 int main(int argc, char** argv) {
   Opts o;
   int gpus_per_proc = 0;
+  bool out_given = false;
   if (const char* op = op_from_argv0(argv[0])) o.op = op;
   for (int i = 1; i < argc; i++) {
     std::string a = argv[i];
@@ -477,12 +522,12 @@ int main(int argc, char** argv) {
     else if (a == "-b" || a == "--min") o.min_bytes = parse_size(next());
     else if (a == "-e" || a == "--max") o.max_bytes = parse_size(next());
     else if (a == "-f" || a == "--factor") o.factor = atoi(next());
-    else if (a == "--dtype" || a == "-d" || a == "--datatype") o.in_dt = o.out_dt = parse_dt(next());
+    else if (a == "--dtype" || a == "-d" || a == "--datatype") { o.in_dt = o.out_dt = parse_dt(next()); out_given = false; }
     else if (a == "-g" || a == "--ngpus") gpus_per_proc = atoi(next());
     else if (a == "-o" || a == "--redop") { std::string v = next(); if (v != "sum") { fprintf(stderr, "only -o sum is benchmarked (avg is a fused scale: use --scale)\n"); return 1; } }
     else if (a == "-t" || a == "--nthreads" || a == "-m" || a == "--agg_iters" || a == "-p" || a == "--parallel_init" || a == "-z" || a == "--blocking" || a == "-a" || a == "--average" ||
              a == "-G" || a == "--cudagraph" || a == "-C" || a == "--report_cputime" || a == "-R" || a == "--local_register" || a == "-T" || a == "--timeout" || a == "-r" || a == "--root") (void)next();   // accepted, no effect here
-    else if (a == "--out-dtype") o.out_dt = parse_dt(next());
+    else if (a == "--out-dtype") { o.out_dt = parse_dt(next()); out_given = true; }
     else if (a == "--block-scale") { if (sscanf(next(), "%dx%d", &o.bs_rows, &o.bs_cols) != 2 || o.bs_rows < 1 || o.bs_cols < 16 || o.bs_cols % 16) { fprintf(stderr, "--block-scale RxC: R >= 1, C a multiple of 16\n"); return 1; } }
     else if (a == "--row-len") o.row_len = (size_t)atoll(next());
     else if (a == "--quantize") {
@@ -522,10 +567,14 @@ int main(int argc, char** argv) {
            "  -d float|half|bfloat16|e4m3|e5m2 (fp8 = e4m3)   input type; --out-dtype T and --scale X fuse a cast / scale into the collective\n"
            "  --block-scale RxC         block-scaled FP8 (all_gather, reduce_scatter, all_reduce): -d e4m3|e5m2 [R x C]-blocked matrices, one seeded\n"
            "                            fp32 scale per block, --out-dtype bfloat16|half|float; -c 1 checks bit for bit against the host\n"
-           "  --row-len N               columns of the block-scaled matrix (default 2048; N and C multiples of 16)\n"
-           "  --quantize WIRE:BLOCK     quantising collectives (all_gather, reduce_scatter, all_reduce): -d bfloat16|half|float in, each rank\n"
+           "  --row-len N               columns of the block-scaled matrix, or row length of the quantising alltoall (default 2048; N and C\n"
+           "                            multiples of 16, N a multiple of BLOCK)\n"
+           "  --quantize WIRE:BLOCK     quantising collectives (all_gather, reduce_scatter, all_reduce, alltoall): -d bfloat16|half|float in, each rank\n"
            "                            quantises to WIRE (e4m3|e5m2) with one fp32 scale per BLOCK (16..512) elements, --out-dtype bfloat16|half|float;\n"
            "                            seeded inputs whose blocks differ in amax; -c 1 checks bit for bit against the host\n"
+           "                            --op alltoall: the quantising all-to-all-v, -d bfloat16|half|float in, --out-dtype WIRE (the default); each rank\n"
+           "                            sends an even split of whole --row-len rows to every peer and receives FP8 rows plus one fp32 scale per\n"
+           "                            BLOCK; -c 1 checks every FP8 byte and scale bit for bit against the host quantiser\n"
            "  --algo auto|ll|ll2|oneshot|twoshot|nvls   --inplace 0|1|2   --max-ctas N   --sweep kind:ctas:threads,...   --json FILE   --window SIZE\n"
            "  --selfcheck               report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;
@@ -533,6 +582,7 @@ int main(int argc, char** argv) {
     else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 1; }
   }
   if (o.factor < 2) o.factor = 2;
+  if (o.q_block && o.op == "alltoall" && !out_given) o.out_dt = o.q_wire;     // the quantising alltoall receives the wire type
   if (o.bs_rows && (o.row_len == 0 || o.row_len % 16)) { fprintf(stderr, "--row-len must be a positive multiple of 16\n"); return 1; }
   const LauncherRank lr = launcher_rank();
   if (lr.size > 1 && o.devs.empty() && !o.procs) {

@@ -135,6 +135,8 @@ def load() -> C.CDLL:
     L.b200collAllGatherQuantized.argtypes = [vp, vp, sz, ci, ci, C.POINTER(Epilogue), vp, vp]
     L.b200collReduceScatterQuantized.argtypes = [vp, vp, sz, ci, ci, C.POINTER(Epilogue), ci, vp, vp]
     L.b200collAllReduceQuantized.argtypes = [vp, vp, sz, ci, ci, C.POINTER(Epilogue), ci, vp, vp]
+    i64p = C.POINTER(C.c_int64)
+    L.b200collAllToAllvQuantized.argtypes = [vp, vp, C.POINTER(C.c_float), sz, sz, i64p, i64p, i64p, ci, ci, ci, vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -265,6 +267,56 @@ def check_quantized(op: str, nranks: int, src, out, block: int = 128, wire=None)
     if n and not in_place and a < b + nb and b < a + na:
         raise ValueError(f"{op}: out must not overlap src" + (" (in place needs out to be src, with a dtype of the same size)" if op == "all_reduce" else ""))
     return torch_dtype_code(wire)
+
+
+def check_all_to_all_v_quantized(nranks: int, src, out, out_scales, row_elems: int, block: int, send_rows, send_row_off,
+                                 recv_row_off_at_peer) -> tuple[int, int]:
+    """Rules of the quantising all-to-all-v, checked on the tensors' metadata and the host lists only (no communicator, no library call):
+    raises ValueError, returns the library codes of (src's type, the wire type). src: contiguous bfloat16, float16 or float32; out:
+    contiguous float8_e4m3fn or float8_e5m2 (the wire type), out.numel() a multiple of row_elems; out_scales: contiguous float32 with
+    out.numel() // block elements; block one of QUANT_BLOCKS and row_elems a positive multiple of it. The three lists have nranks
+    non-negative entries; every send range [send_row_off[p], + send_rows[p]) lies inside src and every destination range
+    [recv_row_off_at_peer[p], + send_rows[p]) inside out, in rows of row_elems elements. src must not overlap out or out_scales."""
+    import operator
+
+    import torch
+    if src.dtype not in (torch.bfloat16, torch.float16, torch.float32) or not src.is_contiguous():
+        raise ValueError(f"src must be a contiguous bfloat16, float16 or float32 tensor, got {src.dtype}")
+    if out.dtype not in (torch.float8_e4m3fn, torch.float8_e5m2) or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous float8_e4m3fn or float8_e5m2 tensor (the wire type), got {out.dtype}")
+    if out_scales.dtype != torch.float32 or not out_scales.is_contiguous():
+        raise ValueError(f"out_scales must be a contiguous float32 tensor, got {out_scales.dtype}")
+    if isinstance(block, bool) or not isinstance(block, int) or block not in QUANT_BLOCKS:
+        raise ValueError(f"block must be one of {QUANT_BLOCKS}, got {block!r}")
+    if isinstance(row_elems, bool) or not isinstance(row_elems, int) or row_elems <= 0 or row_elems % block:
+        raise ValueError(f"row_elems must be a positive multiple of block ({block}), got {row_elems!r}")
+    if out.numel() % row_elems:
+        raise ValueError(f"out.numel() ({out.numel()}) must be a multiple of row_elems ({row_elems})")
+    if out_scales.numel() != out.numel() // block:
+        raise ValueError(f"out_scales must hold out.numel() // block = {out.numel() // block} floats, got {out_scales.numel()}")
+    lists = {"send_rows": send_rows, "send_row_off": send_row_off, "recv_row_off_at_peer": recv_row_off_at_peer}
+    vals = {}
+    for name, xs in lists.items():
+        try:
+            vals[name] = [operator.index(x) for x in xs]
+        except TypeError:
+            raise ValueError(f"{name} must be a sequence of integers") from None
+        if len(vals[name]) != nranks:
+            raise ValueError(f"{name} must have nranks = {nranks} entries, got {len(vals[name])}")
+        if any(x < 0 for x in vals[name]):
+            raise ValueError(f"{name} must not hold negative entries: {vals[name]}")
+    src_rows, out_rows = src.numel() // row_elems, out.numel() // row_elems
+    for p, (rows, so, ro) in enumerate(zip(vals["send_rows"], vals["send_row_off"], vals["recv_row_off_at_peer"])):
+        if so + rows > src_rows:
+            raise ValueError(f"peer {p}: send rows [{so}, {so + rows}) lie past the {src_rows} whole rows of src")
+        if ro + rows > out_rows:
+            raise ValueError(f"peer {p}: destination rows [{ro}, {ro + rows}) lie past the {out_rows} rows of out")
+    a, na = src.data_ptr(), src.numel() * src.element_size()
+    for t in (out, out_scales):
+        b, nb = t.data_ptr(), t.numel() * t.element_size()
+        if na and nb and a < b + nb and b < a + na:
+            raise ValueError("src must not overlap out or out_scales")
+    return torch_dtype_code(src.dtype), torch_dtype_code(out.dtype)
 
 
 class _CudaArray:
@@ -558,6 +610,21 @@ class Comm:
         _check(load().b200collAllToAllv(C.c_void_p(src.data_ptr()), C.c_void_p(dst.data_ptr()), row_elems, arr(send_rows), arr(send_row_off), arr(recv_row_off_at_peer),
                                         C.byref(ep), self._h, self._stream(stream)), "AllToAllv")
         return dst
+
+    def all_to_all_v_quantized(self, src, out, out_scales, row_elems: int, send_rows, send_row_off, recv_row_off_at_peer, block: int = 128,
+                               stream=None):
+        """Expert dispatch with FP8 on the wire (b200collAllToAllvQuantized): send_rows[p] rows of row_elems elements of src (bf16, fp16
+        or fp32, any device tensor), starting at row send_row_off[p], are quantised on this rank in blocks of `block` elements with one
+        fp32 scale per block, and land at row recv_row_off_at_peer[p] of peer p's out (FP8: its dtype is the wire type) and out_scales
+        ([rows, row_elems // block] fp32). Returns (out, out_scales). With more than one rank, out and out_scales must be arena tensors
+        (`empty()`) of the same size on every rank; every rank calls, a rank that sends nothing included."""
+        ic, wc = check_all_to_all_v_quantized(self.nranks, src, out, out_scales, row_elems, block, send_rows, send_row_off, recv_row_off_at_peer)
+        n = self.nranks
+        arr = lambda xs: (C.c_int64 * n)(*[int(x) for x in xs])
+        _check(load().b200collAllToAllvQuantized(C.c_void_p(src.data_ptr()), C.c_void_p(out.data_ptr()), C.cast(C.c_void_p(out_scales.data_ptr()), C.POINTER(C.c_float)),
+                                                 row_elems, out.numel() // row_elems, arr(send_rows), arr(send_row_off), arr(recv_row_off_at_peer), ic, wc, block,
+                                                 self._h, self._stream(stream)), "AllToAllvQuantized")
+        return out, out_scales
 
     def broadcast(self, src, dst=None, root: int = 0, scale: float = 1.0, stream=None):
         """dst on every rank = cast(scale * src of `root`). src is read on the root only (ncclBroadcast)."""
