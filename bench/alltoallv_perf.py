@@ -7,6 +7,9 @@ For each (tokens per rank, hidden, skew): device-timed dispatch of bf16 token ro
 (a) libb200coll all_to_all_v, bf16 on the wire; (b) the same with the fp8-e4m3 quantise fused into the dispatch kernel (half the
 bytes on NVLink, no separate cast kernel); (c) NCCL all_to_all_single with split sizes (torch.distributed, the way MoE stacks call it);
 (d) all_to_all_v_quantized, the block-scaled dispatch FP8 recipes use: e4m3 rows with one fp32 scale per 1x128 block, one kernel.
+Then the combine back, with the dispatched rows standing in for the expert outputs: (e) all_to_all_v_combine, each rank pulling its
+tokens' top-k rows and summing them with the gate weights in one kernel, against (f) NCCL all_to_all_single back plus the PyTorch
+gather and weighted sum a MoE stack runs; combine_matches says ours equals an explicit slot-order fp32 sum bit for bit.
 Bus bandwidth = (bytes a rank sends off-chip, max over ranks) / time. Rank 0 prints one JSON line per shape."""
 from __future__ import annotations
 
@@ -36,6 +39,7 @@ def main() -> int:
     recv_scales = comm.empty(cap_rows * cap_hidden // 128, torch.float32)
     send.copy_((torch.arange(send.numel(), device="cuda") % 251).to(torch.bfloat16) * 0.01)
     nccl_recv = torch.empty(cap_rows * cap_hidden, dtype=torch.bfloat16, device="cuda")
+    nccl_back = torch.empty(cap_rows * cap_hidden, dtype=torch.bfloat16, device="cuda")
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 
     def timed(fn) -> float:
@@ -66,15 +70,35 @@ def main() -> int:
         q_rows = plan.max_rows                                   # the same on every rank, as the symmetric recv needs
         us_bsq = timed(lambda: comm.all_to_all_v_quantized(send, recv8[:q_rows * hidden], recv_scales[:q_rows * hidden // 128], hidden, rows, so, ro, block=128))
         us_nccl = timed(lambda: dist.all_to_all_single(nccl_recv[:n_recv], send[:n_send], out_split, in_split))
+        # combine: recv holds the bf16 dispatch result (the expert outputs' stand-in), so dispatch row i's expert row is send row i
+        comm.all_to_all_v(send, recv, hidden, rows, so, ro)
+        idx = torch.from_numpy(plan.index[rank]).cuda()
+        gate = torch.from_numpy(plan.weights[rank]).cuda()
+        out = torch.empty(tokens, hidden, dtype=torch.bfloat16, device="cuda")
+        eo = recv[:q_rows * hidden]
+        us_comb = timed(lambda: comm.all_to_all_v_combine(eo, out, hidden, rows, so, ro, idx, gate))
+        comm.check_async_error()
+        y = send[:n_send].view(-1, hidden)
+        acc = torch.zeros(tokens, hidden, device="cuda")
+        for j in range(idx.shape[1]):
+            acc = acc + gate[:, j:j + 1] * y[idx[:, j].long()].float()
+        comb_ok = bool(torch.equal(out.view(torch.int16), acc.to(torch.bfloat16).view(torch.int16)))
+        idx_l = idx.long()
+
+        def nccl_combine():
+            dist.all_to_all_single(nccl_back[:n_send], nccl_recv[:n_recv], in_split, out_split)
+            return (nccl_back[:n_send].view(-1, hidden)[idx_l].float() * gate.unsqueeze(-1)).sum(dim=1).to(torch.bfloat16)
+        us_nccl_comb = timed(nccl_combine)
         offchip = max(int(plan.rows[s].sum() - plan.rows[s, s]) for s in range(world)) * hidden * 2
-        oks = torch.tensor([1.0 if ok else 0.0], device="cuda"); dist.all_reduce(oks, op=dist.ReduceOp.MIN)
+        oks = torch.tensor([1.0 if ok else 0.0, 1.0 if comb_ok else 0.0], device="cuda"); dist.all_reduce(oks, op=dist.ReduceOp.MIN)
         if rank == 0:
             print(json.dumps({"bench": "alltoallv_perf", "n_gpus": world, "tokens_per_rank": tokens, "hidden": hidden, "skew": skew, "top_k": 2,
                               "max_offchip_bytes_per_rank": offchip, "imbalance_max_over_mean": round(float(plan.rows.sum(axis=0).max() / plan.rows.sum(axis=0).mean()), 3),
                               "ours_us": round(us_ours, 2), "ours_busbw": round(offchip / us_ours / 1e3, 2), "ours_fused_fp8_us": round(us_fp8, 2),
                               "nccl_us": round(us_nccl, 2), "nccl_busbw": round(offchip / us_nccl / 1e3, 2), "speedup": round(us_nccl / us_ours, 2),
-                              "fp8_speedup_vs_nccl_bf16": round(us_nccl / us_fp8, 2), "matches_nccl": bool(oks.item() == 1.0),
-                              "ours_block_fp8_us": round(us_bsq, 2)}), flush=True)
+                              "fp8_speedup_vs_nccl_bf16": round(us_nccl / us_fp8, 2), "matches_nccl": bool(oks[0].item() == 1.0),
+                              "ours_block_fp8_us": round(us_bsq, 2), "ours_combine_us": round(us_comb, 2), "nccl_combine_us": round(us_nccl_comb, 2),
+                              "combine_matches": bool(oks[1].item() == 1.0)}), flush=True)
     comm.destroy()
     dist.destroy_process_group()
     return 0

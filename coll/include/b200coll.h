@@ -324,6 +324,40 @@ b200collResult_t b200collAllToAllvQuantized(const void* send, void* recv, float*
                                             const int64_t* send_rows, const int64_t* send_row_off, const int64_t* recv_row_off_at_peer,
                                             b200collDataType_t in_dtype, b200collDataType_t wire_dtype, int block,
                                             b200collComm_t comm, b200collStream_t stream);
+/* Expert combine: the reverse of b200collAllToAllv / b200collAllToAllvQuantized with the top-k weighted sum fused, one kernel per call.
+ * Each rank pulls the expert output rows its tokens need straight from the peers' expert_out, sums them in registers in slot order and
+ * writes [tokens, row_elems] once: no landing buffer, no second kernel, no atomics, the same bits on every run.
+ *   send_rows, send_row_off, recv_row_off_at_peer: the host arrays (length nranks) this rank passed to its dispatch call, same meaning.
+ *   Dispatch row i belongs to peer p when send_row_off[p] <= i < send_row_off[p] + send_rows[p]; its expert output is row
+ *   recv_row_off_at_peer[p] + (i - send_row_off[p]) of peer p's expert_out.
+ *   expert_out: [recv_rows, row_elems] of ep->in_dtype on every rank, written by the experts before the call.
+ *   index: device [tokens, top_k] int32 dispatch rows, -1 for a dropped slot. weights: device [tokens, top_k] fp32, or NULL for all ones.
+ *   out: [tokens, row_elems] of ep->out_dtype.
+ * Result, per token t and element e: out[t, e] = round_once(scale * acc), acc = ((+0 + w[t,0]*y(index[t,0])[e]) + w[t,1]*y(index[t,1])[e])
+ * + ... for j = 0 .. top_k-1, every product and every sum rounded to fp32 on its own (no fused multiply-add), slots in slot order. A
+ * slot whose index names no dispatch row (negative, in a gap between ranges, or past every range) is skipped; weights == NULL gives the
+ * bits of all-ones weights. scale = ep->scale; rounding RNE, fp16 overflows to inf; NaN and inf propagate as the fp32 arithmetic makes
+ * them; -0 comes out as +0; a token whose slots are all dropped gets +0 (times scale). The result depends only on the expert_out values
+ * and the weights, not on the number of ranks or on which rank held a row.
+ *   in_dtype and out_dtype: each bf16, fp16 or fp32 (9 pairs); FP8 on either side is InvalidArgument.
+ * Refused with InvalidArgument before anything is launched (message in b200collGetLastError): null pointers (index and out may be NULL
+ * only when tokens == 0), row_elems == 0 or row_elems % 16 != 0, top_k < 1, negative counts or offsets, a destination range
+ * [recv_row_off_at_peer[p], + send_rows[p]) past recv_rows, two non-empty send ranges that overlap (the row -> peer map must be unique),
+ * expert_out or out not 16-byte aligned, index or weights not 4-byte aligned, out overlapping expert_out, index or weights, more than
+ * 2^31 - 1 16-element vectors of out, tokens * top_k > 2^31 - 1.
+ * Placement: with more than one rank, expert_out must be arena memory at the same offset on every rank (else InvalidUsage) and recv_rows
+ * the same on every rank; with B200COLL_CHECK=1 on multi-process communicators, (recv_rows, arena offset of expert_out) is compared across
+ * ranks. out, index and weights may be any device buffers. A poisoned communicator gives RemoteError.
+ * The kernel never reads outside a destination range of a peer, whatever index holds (index is device data the host cannot check).
+ * Every rank launches on every call, a rank with tokens == 0 or no rows included (its peers' barriers wait for it). The call returns
+ * (on its stream) only after every peer has finished reading this rank's expert_out, so the caller may overwrite it right after.
+ * One rank: a local gather and sum with no barrier, expert_out any device buffer.
+ * b200collStats count the call under alltoall, algorithm oneshot (copy with one rank), sum_p send_rows[p] * row_elems * sizeof(in) bytes,
+ * and one kernel launch. */
+b200collResult_t b200collAllToAllvCombine(const void* expert_out, void* out, size_t row_elems, size_t recv_rows,
+                                          const int64_t* send_rows, const int64_t* send_row_off, const int64_t* recv_row_off_at_peer,
+                                          const int32_t* index, const float* weights, size_t tokens, int top_k,
+                                          const b200collEpilogue* ep, b200collComm_t comm, b200collStream_t stream);
 
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.

@@ -143,22 +143,6 @@ template <typename WireT> __device__ __forceinline__ void bsq_dequant_add(float*
   }
 }
 
-// out = round_once(acc * scale): 16 elements, 32 (bf16 / fp16) or 64 (fp32) bytes
-template <typename OutT> __device__ __forceinline__ void bsq_store(void* dst, const float* acc, float scale) {
-  constexpr int W = Pack<OutT, 16>::W;
-  float f[16];
-#pragma unroll
-  for (int i = 0; i < 16; i++) f[i] = __fmul_rn(acc[i], scale);
-  uint32_t w[W];
-  Pack<OutT, 16>::run(f, w);
-  if constexpr (W == 16) {
-#pragma unroll
-    for (int k = 0; k < 4; k++) st_vec(reinterpret_cast<char*>(dst) + 16 * k, make_uint4(w[4 * k], w[4 * k + 1], w[4 * k + 2], w[4 * k + 3]));
-  } else {
-    st_words<W>(dst, w);
-  }
-}
-
 // Dequantise vectors [0, nvec) of one rank's FP8 data into dst.
 template <typename WireT, typename OutT, typename Geom>
 __device__ __forceinline__ void dequant_range(const Geom& g, const char* src, const char* scales, OutT* dst, float scale) {
@@ -171,7 +155,7 @@ __device__ __forceinline__ void dequant_range(const Geom& g, const char* src, co
     if (act) {
       float acc[16] = {};
       bsq_dequant_add<WireT>(acc, q, s);
-      bsq_store<OutT>(dst + (size_t)v * 16, acc, scale);
+      store16_scaled<OutT>(dst + (size_t)v * 16, acc, scale);
     }
   });
 }
@@ -207,10 +191,10 @@ __device__ __forceinline__ void pull_reduce_range(const CommDev& c, const Geom& 
 #pragma unroll
         for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
           int r = c.rank + j; if (r >= c.nranks) r -= c.nranks;
-          bsq_store<OutT>(c.peer[r] + out_off + (size_t)v * (16 * sizeof(OutT)), acc, scale);
+          store16_scaled<OutT>(c.peer[r] + out_off + (size_t)v * (16 * sizeof(OutT)), acc, scale);
         }
       } else {
-        bsq_store<OutT>(out_local + (size_t)(v - v0) * 16, acc, scale);
+        store16_scaled<OutT>(out_local + (size_t)(v - v0) * 16, acc, scale);
       }
     }
   });
@@ -334,7 +318,7 @@ __global__ void __launch_bounds__(kBsqThreads) k_quant_copy(const char* in, OutT
     if (act) {
       float acc[16] = {};
       bsq_dequant_add<WireT>(acc, w, s);
-      bsq_store<OutT>(out + (size_t)v * 16, acc, scale);
+      store16_scaled<OutT>(out + (size_t)v * 16, acc, scale);
     }
   });
 }
@@ -673,12 +657,11 @@ static b200collResult_t a2aq_prepare(b200collComm* c, const void* send, void* re
   unsigned long long total = 0;
   size_t send_end = 0;                                            // the bytes of send that are read
   *in_bytes = 0;
+  A2AvRows rg;
+  const std::string bad = a2av_rows(c->nranks, send_rows, send_row_off, recv_row_off_at_peer, recv_rows, max_rows, &rg);
+  if (!bad.empty()) return refuse(bad);
   for (int p = 0; p < c->nranks; p++) {
-    if (send_rows[p] < 0 || send_row_off[p] < 0 || recv_row_off_at_peer[p] < 0) return refuse("negative row count or offset");
-    const size_t rows = (size_t)send_rows[p], src = (size_t)send_row_off[p], dst = (size_t)recv_row_off_at_peer[p];
-    if (rows > recv_rows || dst > recv_rows - rows)
-      return refuse("rows for peer " + std::to_string(p) + " land at [" + std::to_string(dst) + ", +" + std::to_string(rows) + "), past recv_rows = " + std::to_string(recv_rows));
-    if (src > max_rows || rows > max_rows - src) return refuse("the send range of peer " + std::to_string(p) + " is too large");
+    const size_t rows = rg.rows[p], src = rg.src_row[p], dst = rg.dst_row[p];
     if (rows > (max_vecs - total) / row_vecs) return refuse("at most 2^31 - 1 16-element vectors may be sent per rank");
     total += rows * row_vecs;
     a->src_vec[p] = src * row_vecs;

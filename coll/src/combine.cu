@@ -1,0 +1,245 @@
+// libb200coll expert combine: the reverse of the all-to-all-v dispatch with the top-k weighted sum fused, one kernel per call.
+//
+//   k_a2av_combine_pull<InT, OutT>    barrier, pull each token's top_k expert rows from the peers' expert_out, sum in slot order in
+//                                     fp32, round once, store locally, barrier
+//   k_a2av_combine_local<InT, OutT>   one rank: the same gather and sum from a local expert_out, no barrier
+//
+// Each rank walks (token, 16-element vector) pairs of its own out. For slot j of token t, index[t, j] is a row of the dispatch send
+// buffer; the segment table (A2AvRows, the rows of the dispatch call) maps it to (peer p, row of p's expert_out). A row in no segment
+// is a dropped slot. So every load lies inside a destination range [dst_row[p], + rows[p]) of a peer, which the host has checked against
+// recv_rows: whatever the device-side index holds, the kernel reads nothing else.
+//
+// Per thread, up to kSlots slots are loaded before the first of them is added, so several NVLink (or HBM) reads are in flight; the adds
+// then run in slot order, acc = (acc + w_j * y_j) with both roundings kept, so the batching does not change the result.
+#include <stdint.h>
+
+#include <algorithm>
+#include <type_traits>
+#include <vector>
+
+#include "a2av.h"
+#include "comm.h"
+#include "launch.cuh"
+
+namespace b200coll {
+
+using bf16 = __nv_bfloat16;
+
+constexpr int kCombineThreads = 512;
+
+// The (peer, expert_out row) of dispatch row i, or false when i names no dispatch row. The host refuses overlapping send ranges, so at
+// most one segment matches.
+__device__ __forceinline__ bool combine_row(const A2AvRows& g, int nranks, int32_t i, int* peer, unsigned long long* row) {
+  bool hit = false;
+#pragma unroll
+  for (int q = 0; q < kMaxRanks; q++) {
+    const unsigned long long d = (unsigned long long)((long long)i - (long long)g.src_row[q]);     // negative -> huge -> no match
+    if (q < nranks && d < g.rows[q]) { *peer = q; *row = g.dst_row[q] + d; hit = true; }
+  }
+  return hit;
+}
+
+// 16 elements of InT held as sizeof(InT) 16-byte words, widened (exactly) to fp32
+template <typename InT> __device__ __forceinline__ void combine_widen(const uint4* raw, float* x) {
+#pragma unroll
+  for (int k = 0; k < (int)sizeof(InT); k++) {
+    const uint32_t w[4] = {raw[k].x, raw[k].y, raw[k].z, raw[k].w};
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      if constexpr (std::is_same<InT, float>::value) {
+        x[4 * k + i] = __uint_as_float(w[i]);
+      } else if constexpr (std::is_same<InT, bf16>::value) {
+        x[8 * k + 2 * i] = __uint_as_float(w[i] << 16); x[8 * k + 2 * i + 1] = __uint_as_float(w[i] & 0xFFFF0000u);
+      } else {
+        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
+        x[8 * k + 2 * i] = f.x; x[8 * k + 2 * i + 1] = f.y;
+      }
+    }
+  }
+}
+
+// Vectors [0, tokens * vpr) of out, vpr = row_elems / 16. base(p) is the address of peer p's expert_out. Consecutive threads take
+// consecutive vectors of a row, so the loads of a warp are coalesced; lanes of one token read index and weights at one address
+// (a broadcast). 32-bit indices: the host keeps tokens * vpr below 2^31, so v + stride cannot wrap.
+template <typename InT, typename OutT, typename Base>
+__device__ __forceinline__ void combine_range(const A2AvRows& g, int nranks, Base&& base, const int32_t* __restrict__ index,
+                                              const float* __restrict__ weights, OutT* __restrict__ out, uint32_t tokens, uint32_t top_k,
+                                              uint32_t vpr, float scale) {
+  constexpr int NW = (int)sizeof(InT);                           // 16-byte words per 16 elements: 2 (bf16, fp16) or 4 (fp32)
+  constexpr int kSlots = 16 / (int)sizeof(InT);                  // slots in flight per thread: 8 or 4, 64 registers of raw data
+  const uint32_t nvec = tokens * vpr;
+  for (uint32_t v = blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += gridDim.x * blockDim.x) {
+    const uint32_t t = v / vpr, col = v - t * vpr;
+    const int32_t* it = index + (size_t)t * top_k;
+    const float* wt = weights + (size_t)t * top_k;
+    float acc[16];
+#pragma unroll
+    for (int e = 0; e < 16; e++) acc[e] = 0.0f;
+    for (uint32_t j0 = 0; j0 < top_k; j0 += kSlots) {
+      uint4 raw[kSlots][NW];
+      float w[kSlots];
+      bool hit[kSlots];
+#pragma unroll
+      for (int b = 0; b < kSlots; b++) {
+        hit[b] = false;
+        w[b] = 1.0f;
+        int p = 0;
+        unsigned long long row = 0;
+        if (j0 + b < top_k && combine_row(g, nranks, it[j0 + b], &p, &row)) {
+          hit[b] = true;
+          if (weights) w[b] = wt[j0 + b];
+          const char* src = base(p) + (row * vpr + col) * (16 * sizeof(InT));
+#pragma unroll
+          for (int k = 0; k < NW; k++) raw[b][k] = ld_vec(src + 16 * k);
+        }
+      }
+#pragma unroll
+      for (int b = 0; b < kSlots; b++) {
+        if (!hit[b]) continue;
+        float x[16];
+        combine_widen<InT>(raw[b], x);
+#pragma unroll
+        for (int e = 0; e < 16; e++) acc[e] = __fadd_rn(acc[e], __fmul_rn(w[b], x[e]));
+      }
+    }
+    store16_scaled<OutT>(out + (size_t)v * 16, acc, scale);
+  }
+}
+
+// The grid is the full P2P shape on every rank, whatever its tokens (see b200collAllToAllvCombine). The epoch barrier pairs CTA b of
+// this rank with CTA b of every peer and nothing else; each rank knows only its own tokens, so a grid sized to them would differ from
+// rank to rank, and a CTA missing on one rank would leave CTA b of its peers waiting. With one grid everywhere, the first barrier
+// (relaxed: expert_out was written by earlier kernels on each peer's stream) means every peer's expert_out is complete before any CTA
+// pulls, and the closing barrier means no rank's kernel ends before every CTA of every peer has finished its pulls, so the caller may
+// overwrite expert_out right after the call on its own stream. CTAs with no vectors take only the two barriers.
+template <typename InT, typename OutT>
+__global__ void __launch_bounds__(kCombineThreads, 1) k_a2av_combine_pull(COMM_PARAM, size_t eo_off, const __grid_constant__ A2AvRows g,
+                                                                          const int32_t* __restrict__ index, const float* __restrict__ weights,
+                                                                          OutT* __restrict__ out, uint32_t tokens, uint32_t top_k, uint32_t vpr,
+                                                                          float scale, uint32_t op) {
+  pdl_prologue();
+  {
+    const uint32_t s = load_seq(c, kSeqBarrier);
+    if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every peer's expert_out is written
+  }
+  combine_range<InT, OutT>(g, c.nranks, [&](int p) -> const char* { return c.peer[p] + eo_off; }, index, weights, out, tokens, top_k, vpr, scale);
+  // the sequence number is read again rather than kept live across the loop: only the last block, after the barrier below, bumps it
+  const uint32_t s = load_seq(c, kSeqBarrier);
+  if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // nobody reads my expert_out any more: the caller may overwrite it
+  if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
+}
+
+template <typename InT, typename OutT>
+__global__ void __launch_bounds__(kCombineThreads, 1) k_a2av_combine_local(const __grid_constant__ A2AvRows g, const char* __restrict__ expert_out,
+                                                                           const int32_t* __restrict__ index, const float* __restrict__ weights,
+                                                                           OutT* __restrict__ out, uint32_t tokens, uint32_t top_k, uint32_t vpr,
+                                                                           float scale) {
+  pdl_prologue();
+  combine_range<InT, OutT>(g, 1, [&](int) { return expert_out; }, index, weights, out, tokens, top_k, vpr, scale);
+}
+
+// ------------------------------------------------------------------------------------------------ host side
+static bool combine_type(b200collDataType_t t) { return t == b200collBfloat16 || t == b200collFloat16 || t == b200collFloat32; }
+
+// (in, out) -> f(Tag<InT>, Tag<OutT>); the argument checks have refused every other type
+template <typename F>
+static b200collResult_t dispatch_combine(b200collDataType_t in, b200collDataType_t out, F&& f) {
+  auto outs = [&](auto ti) -> b200collResult_t {
+    switch (out) {
+      case b200collBfloat16: return f(ti, Tag<bf16>{});
+      case b200collFloat16: return f(ti, Tag<__half>{});
+      default: return f(ti, Tag<float>{});
+    }
+  };
+  switch (in) {
+    case b200collBfloat16: return outs(Tag<bf16>{});
+    case b200collFloat16: return outs(Tag<__half>{});
+    default: return outs(Tag<float>{});
+  }
+}
+
+// Everything b200collAllToAllvCombine checks before it launches; on success `g` holds the segment table and `in_bytes` the bytes of
+// expert_out the dispatch rows cover.
+static b200collResult_t combine_prepare(b200collComm* c, const void* expert_out, void* out, size_t row_elems, size_t recv_rows, const int64_t* send_rows,
+                                        const int64_t* send_row_off, const int64_t* recv_row_off_at_peer, const int32_t* index, const float* weights,
+                                        size_t tokens, int top_k, const b200collEpilogue* ep, A2AvRows* g, size_t* in_bytes) {
+  auto refuse = [](const std::string& msg) { set_last_error("all-to-all-v combine: " + msg); return b200collInvalidArgument; };
+  if (!c || !expert_out || !ep || !send_rows || !send_row_off || !recv_row_off_at_peer || ((!index || !out) && tokens > 0)) return refuse("null argument");
+  if (!combine_type(ep->in_dtype) || !combine_type(ep->out_dtype)) return refuse("in_dtype and out_dtype must be bf16, fp16 or fp32");
+  if (row_elems == 0 || row_elems % 16 != 0) return refuse("row_elems must be a positive multiple of 16");
+  if (top_k < 1) return refuse("top_k must be at least 1");
+  if (!aligned(expert_out, 16) || !aligned(out, 16)) return refuse("expert_out and out must be 16-byte aligned");
+  if (!aligned(index, 4) || !aligned(weights, 4)) return refuse("index and weights must be 4-byte aligned");
+  const size_t max_vecs = ((size_t)1 << 31) - 1;
+  if (tokens > max_vecs / (row_elems / 16)) return refuse("at most 2^31 - 1 16-element vectors of out");
+  if (tokens > max_vecs / (size_t)top_k) return refuse("tokens * top_k must be at most 2^31 - 1");
+  const size_t is = b200collTypeSize(ep->in_dtype), os = b200collTypeSize(ep->out_dtype);
+  const size_t max_rows = (SIZE_MAX >> 4) / (row_elems * is);     // every byte offset below then fits in size_t with room to spare
+  if (recv_rows > max_rows) return refuse("recv_rows * row_elems is too large");
+  const std::string bad = a2av_rows(c->nranks, send_rows, send_row_off, recv_row_off_at_peer, recv_rows, max_rows, g);
+  if (!bad.empty()) return refuse(bad);
+  std::vector<std::pair<unsigned long long, unsigned long long>> ranges;     // non-empty send ranges [lo, hi)
+  *in_bytes = 0;
+  for (int p = 0; p < c->nranks; p++) {
+    if (g->rows[p]) ranges.emplace_back(g->src_row[p], g->src_row[p] + g->rows[p]);
+    *in_bytes += g->rows[p] * row_elems * is;
+  }
+  std::sort(ranges.begin(), ranges.end());
+  for (size_t k = 1; k < ranges.size(); k++)
+    if (ranges[k].first < ranges[k - 1].second) return refuse("two send ranges overlap: a dispatch row must belong to one peer");
+  const size_t eo_bytes = recv_rows * row_elems * is, out_bytes = tokens * row_elems * os, idx_bytes = tokens * (size_t)top_k * 4;
+  if (overlaps(out, out_bytes, expert_out, eo_bytes) || (index && overlaps(out, out_bytes, index, idx_bytes)) ||
+      (weights && overlaps(out, out_bytes, weights, idx_bytes)))
+    return refuse("out must not overlap expert_out, index or weights");
+  if (comm_poisoned(c)) return b200collRemoteError;
+  // peers pull from my expert_out at MY arena offset: it must be arena memory
+  if (c->nranks > 1 && !b200collIsSymmetric(c, expert_out, std::max<size_t>(eo_bytes, 1))) {
+    set_last_error("all-to-all-v combine: expert_out must lie in the symmetric arena (b200collMemAlloc), at the same offset on every rank");
+    return b200collInvalidUsage;
+  }
+  return b200collSuccess;
+}
+
+}  // namespace b200coll
+
+using namespace b200coll;
+
+extern "C" {
+
+b200collResult_t b200collAllToAllvCombine(const void* expert_out, void* out, size_t row_elems, size_t recv_rows,
+                                          const int64_t* send_rows, const int64_t* send_row_off, const int64_t* recv_row_off_at_peer,
+                                          const int32_t* index, const float* weights, size_t tokens, int top_k,
+                                          const b200collEpilogue* ep, b200collComm_t c, b200collStream_t stream) {
+  A2AvRows g;
+  size_t in_bytes = 0;
+  b200collResult_t rc = combine_prepare(c, expert_out, out, row_elems, recv_rows, send_rows, send_row_off, recv_row_off_at_peer, index, weights, tokens,
+                                        top_k, ep, &g, &in_bytes);
+  if (rc != b200collSuccess) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const uint32_t vpr = (uint32_t)(row_elems / 16), nvec = (uint32_t)(tokens * vpr);
+  if (c->nranks == 1) {
+    account(c, b200collOpAllToAll, in_bytes, b200collAlgoCopy);
+    const int blocks = (int)std::max<size_t>(1, std::min<size_t>(((size_t)nvec + kCombineThreads - 1) / kCombineThreads, (size_t)std::max(1, c->sm_count)));
+    return dispatch_combine(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
+      using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
+      launch_k(k_a2av_combine_local<InT, OutT>, blocks, kCombineThreads, st, g, static_cast<const char*>(expert_out), index, weights, static_cast<OutT*>(out),
+               (uint32_t)tokens, (uint32_t)top_k, vpr, ep->scale);
+      LAUNCH_CHECK(c);
+      return b200collSuccess;
+    });
+  }
+  rc = cross_check(c, b200collOpAllToAll, b200collAlgoOneShot, recv_rows, arena_off(c, expert_out), 0);
+  if (rc != b200collSuccess) return rc;
+  account(c, b200collOpAllToAll, in_bytes, b200collAlgoOneShot);
+  // the full P2P grid on every rank, whatever its tokens: CTA b meets CTA b of every peer in both barriers (see k_a2av_combine_pull)
+  const Grid gr = pick_grid(c, kShapeP2p, ~(size_t)0 >> 8, 1);
+  return dispatch_combine(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
+    using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
+    launch_k(k_a2av_combine_pull<InT, OutT>, gr.blocks, gr.threads, st, c->dev, arena_off(c, expert_out), g, index, weights, static_cast<OutT*>(out),
+             (uint32_t)tokens, (uint32_t)top_k, vpr, ep->scale, (uint32_t)b200collOpAllToAll);
+    LAUNCH_CHECK(c);
+    return b200collSuccess;
+  });
+}
+
+}  // extern "C"

@@ -254,6 +254,21 @@ template <int W> __device__ __forceinline__ void st_words(void* p, const uint32_
     asm volatile("st.global.u32 [%0], %1;" ::"l"(p), "r"(w[0]) : "memory");
   }
 }
+// out = round_once(acc * scale): 16 elements, 32 (bf16 / fp16) or 64 (fp32) bytes
+template <typename OutT> __device__ __forceinline__ void store16_scaled(void* dst, const float* acc, float scale) {
+  constexpr int W = Pack<OutT, 16>::W;
+  float f[16];
+#pragma unroll
+  for (int i = 0; i < 16; i++) f[i] = __fmul_rn(acc[i], scale);
+  uint32_t w[W];
+  Pack<OutT, 16>::run(f, w);
+  if constexpr (W == 16) {
+#pragma unroll
+    for (int k = 0; k < 4; k++) st_vec(reinterpret_cast<char*>(dst) + 16 * k, make_uint4(w[4 * k], w[4 * k + 1], w[4 * k + 2], w[4 * k + 3]));
+  } else {
+    st_words<W>(dst, w);
+  }
+}
 template <int W> __device__ __forceinline__ void mc_st_wordsW(void* p, const uint32_t* w) {
   if (W == 8) { mc_st_words(p, w, 4); mc_st_words(reinterpret_cast<char*>(p) + 16, w + 4, 4); }
   else mc_st_words(p, w, W);

@@ -55,6 +55,7 @@ struct Opts {
   size_t row_len = 2048;          // --row-len N: columns of the block-scaled matrix
   int q_block = 0;                // --quantize WIRE:BLOCK: quantising collectives (0 = off)
   b200collDataType_t q_wire = b200collFloat8e4m3;
+  int combine_k = 0;              // --combine K: the expert combine with top_k = K (0 = off)
 };
 
 // Block-scaled mode: each rank's send buffer is a [rows, row_len] FP8 matrix with one fp32 scale per bs_rows x bs_cols block. Scales are
@@ -188,6 +189,117 @@ constexpr int kRoot = 0;   // rooted ops (broadcast, reduce) are driven from ran
 
 struct RankCtx { int rank, nranks; b200collComm_t comm; int dev; };
 
+// Expert-combine mode (--combine K). Per size, every rank's expert_out holds `bytes` of whole --row-len rows, an even split: rpp rows
+// came from every rank. So rank r's dispatch rows for peer p are rows [p * rpp, + rpp) of its (notional) send buffer and their expert
+// outputs are rows [r * rpp, + rpp) of p's expert_out. tokens = n * rpp / K, and token t's slot j goes to range (t + j + h(t)) % n
+// (K different ranges where n >= K), to the next unused row of that range, or is dropped (-1) when the range is used up. Weights are
+// seeded in [0.25, 1.25). Expert-out values are exact in every input type and the weights have full mantissas, so products and sums
+// round; -c 1 repeats the slot-order fp32 arithmetic on the host and compares every output element bit for bit.
+static uint32_t co_hash(uint32_t x) { x ^= x >> 16; x *= 0x7FEB352Du; x ^= x >> 15; x *= 0x846CA68Bu; x ^= x >> 16; return x; }
+static float co_val(int rank, size_t i) { return gen(rank, i) * ldexpf(1.0f, (int)((i / 16 * 5 + (size_t)rank * 3) % 13) - 6); }
+template <typename T> __global__ void k_fill_co(T* p, size_t n, int rank) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float v = (float)((int)((i * 7 + (size_t)rank * 13 + (i >> 9)) % 17) - 8) * 0.25f;
+    p[i] = T(v * ldexpf(1.0f, (int)((i / 16 * 5 + (size_t)rank * 3) % 13) - 6));
+  }
+}
+static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out, void* out, cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1) {
+  const int n = ctx.nranks, rank = ctx.rank, K = o.combine_k;
+  const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt), row = o.row_len;
+  const b200collEpilogue ep{o.in_dt, o.out_dt, o.scale};
+  int gen_ctr[4] = {0, 0, 0, 0};
+  long total_errors = 0;
+  if (rank == 0) {
+    printf("# b200coll_perf op=alltoall combine top_k=%d nranks=%d in=%s out=%s scale=%g row_len=%zu: size = expert_out bytes read per rank\n", K, n, dt_name(o.in_dt),
+           dt_name(o.out_dt), o.scale, row);
+    printf("#%13s %12s %6s %8s | %10s %8s %6s\n", "size(B)", "tokens", "type", "algo", "us", "algbw", "#wrong");
+    fflush(stdout);
+  }
+  for (size_t bytes = o.min_bytes; bytes <= o.max_bytes; bytes *= o.factor) {
+    const size_t rpp = bytes / is / row / n, recv_rows = rpp * n, tokens = recv_rows / K;
+    if (tokens == 0) continue;
+    std::vector<int64_t> rows(n, (int64_t)rpp), soff(n), roff(n, (int64_t)(rank * rpp));
+    for (int p = 0; p < n; p++) soff[p] = (int64_t)(p * rpp);
+    std::vector<int32_t> idx(tokens * K);
+    std::vector<float> w(tokens * K);
+    std::vector<size_t> used(n, 0);
+    for (size_t t = 0; t < tokens; t++) {
+      const uint32_t h = co_hash((uint32_t)t * 2654435761u ^ (uint32_t)rank * 97u);
+      for (int j = 0; j < K; j++) {
+        const int p = (int)((t + j + h) % n);
+        idx[t * K + j] = used[p] < rpp ? (int32_t)(soff[p] + used[p]++) : -1;
+        w[t * K + j] = 0.25f + (float)(co_hash(h + 31u * j) & 0xFFFFFF) * 0x1p-24f;
+      }
+    }
+    int32_t* d_idx = nullptr; float* d_w = nullptr;
+    RT(cudaMalloc(&d_idx, idx.size() * 4)); RT(cudaMalloc(&d_w, w.size() * 4));
+    RT(cudaMemcpy(d_idx, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice));
+    RT(cudaMemcpy(d_w, w.data(), w.size() * 4, cudaMemcpyHostToDevice));
+    const size_t eo_elems = recv_rows * row, out_elems = tokens * row;
+    if (o.in_dt == b200collFloat32) k_fill_co<float><<<256, 256, 0, st>>>((float*)expert_out, eo_elems, rank);
+    else if (o.in_dt == b200collFloat16) k_fill_co<__half><<<256, 256, 0, st>>>((__half*)expert_out, eo_elems, rank);
+    else k_fill_co<__nv_bfloat16><<<256, 256, 0, st>>>((__nv_bfloat16*)expert_out, eo_elems, rank);
+    RT(cudaGetLastError());
+    RT(cudaMemsetAsync(out, 0x5A, out_elems * os, st));
+    auto launch = [&] {
+      CC(b200collAllToAllvCombine(expert_out, out, row, recv_rows, rows.data(), soff.data(), roff.data(), d_idx, d_w, tokens, K, &ep, ctx.comm, st));
+    };
+    long errs = 0;
+    if (o.check) {
+      RT(cudaStreamSynchronize(st));
+      spin_barrier(sh, 0, n, &gen_ctr[0]);
+      launch();
+      RT(cudaStreamSynchronize(st));
+      spin_barrier(sh, 1, n, &gen_ctr[1]);
+      std::vector<char> host(out_elems * os);
+      RT(cudaMemcpy(host.data(), out, host.size(), cudaMemcpyDeviceToHost));
+      for (size_t t = 0; t < tokens; t++) {
+        for (size_t e = 0; e < row; e++) {
+          float acc = 0.0f;
+          for (int j = 0; j < K; j++) {
+            const int32_t i = idx[t * K + j];
+            if (i < 0) continue;
+            const int p = (int)(i / (int64_t)rpp);                      // the range row i lies in, and its row of p's expert_out
+            const size_t r = (size_t)rank * rpp + (size_t)(i - soff[p]);
+            volatile float prod = w[t * K + j] * co_val(p, r * row + e);
+            acc = acc + prod;
+          }
+          const uint32_t want = out_bits(acc * o.scale, o.out_dt), got = got_bits(host.data(), t * row + e, o.out_dt);
+          if (got != want) { if (errs < 4) fprintf(stderr, "rank %d combine size %zu token %zu elem %zu: got bits 0x%x want 0x%x\n", rank, bytes, t, e, got, want); errs++; }
+        }
+      }
+    }
+    for (int i = 0; i < o.warmup; i++) launch();
+    RT(cudaStreamSynchronize(st));
+    spin_barrier(sh, 2, n, &gen_ctr[2]);
+    RT(cudaEventRecord(e0, st));
+    for (int i = 0; i < o.iters; i++) launch();
+    RT(cudaEventRecord(e1, st));
+    RT(cudaEventSynchronize(e1));
+    float ms = 0; RT(cudaEventElapsedTime(&ms, e0, e1));
+    sh->ms[rank] = ms / o.iters; sh->errors[rank] = errs;
+    spin_barrier(sh, 3, n, &gen_ctr[3]);
+    float worst = 0; long es = 0;
+    for (int r = 0; r < n; r++) { worst = std::max(worst, sh->ms[r]); es += sh->errors[r]; }
+    total_errors += es;
+    spin_barrier(sh, 0, n, &gen_ctr[0]);   // keep ms[] stable until everyone has read it
+    b200collFault f;
+    if (b200collCommGetAsyncError(ctx.comm, &f) != b200collSuccess) { fprintf(stderr, "rank %d WATCHDOG code=%u peer=%u block=%u expected=%u observed=%u\n", rank, f.code, f.peer, f.block, f.expected, f.observed); _exit(5); }
+    if (rank == 0) {
+      const size_t eo_bytes = recv_rows * row * is;
+      printf("%14zu %12zu %6s %8s | %10.2f %8.2f %6ld\n", eo_bytes, tokens, dt_name(o.in_dt), n > 1 ? "oneshot" : "copy", worst * 1e3, eo_bytes / (worst * 1e3) / 1e3, es);
+      fflush(stdout);
+    }
+    RT(cudaFree(d_idx)); RT(cudaFree(d_w));
+  }
+  b200collStats s; CC(b200collCommStatsGet(ctx.comm, &s));
+  if (rank == 0) {
+    printf("# launches=%llu errors=%ld\n", (unsigned long long)s.kernel_launches, total_errors);
+    fflush(stdout);
+  }
+  return total_errors ? 1 : 0;
+}
+
 // expected value of output element e (element index in the op's output) for this rank
 static float expected(const Opts& o, int rank, int n, size_t e, size_t count) {
   if (o.op == "all_reduce" || o.op == "reduce") { float s = 0; for (int r = 0; r < n; r++) s += gen(r, e); return s * o.scale; }
@@ -224,6 +336,15 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
   void *send = nullptr, *recv = nullptr;
   CC(b200collMemAlloc(ctx.comm, &send, send_cap + 4096));
   CC(b200collMemAlloc(ctx.comm, &recv, recv_cap + 4096));
+  if (o.combine_k) {
+    if (o.op != "alltoall" || o.q_block || o.bs_rows || o.row_len == 0 || o.row_len % 16 ||
+        [](b200collDataType_t t) { return t != b200collBfloat16 && t != b200collFloat16 && t != b200collFloat32; }(o.in_dt) ||
+        [](b200collDataType_t t) { return t != b200collBfloat16 && t != b200collFloat16 && t != b200collFloat32; }(o.out_dt)) {
+      fprintf(stderr, "--combine K takes --op alltoall, -d and --out-dtype bfloat16|half|float, a --row-len that is a multiple of 16, and no --quantize or --block-scale\n");
+      return 2;
+    }
+    return run_combine(o, ctx, sh, send, recv, st, e0, e1);
+  }
   const bool bs_mode = o.bs_rows > 0, q_mode = o.q_block > 0, is_a2a = o.op == "alltoall";
   const bool wide_in = o.in_dt == b200collBfloat16 || o.in_dt == b200collFloat16 || o.in_dt == b200collFloat32;
   const bool wide_out = o.out_dt == b200collBfloat16 || o.out_dt == b200collFloat16 || o.out_dt == b200collFloat32;
@@ -538,6 +659,7 @@ int main(int argc, char** argv) {
       }
       o.q_wire = parse_dt(wire);
     }
+    else if (a == "--combine") { o.combine_k = atoi(next()); if (o.combine_k < 1) { fprintf(stderr, "--combine K: K >= 1\n"); return 1; } }
     else if (a == "--scale") o.scale = (float)atof(next());
     else if (a == "--algo") o.algo = next();
     else if (a == "--iters" || a == "-n") o.iters = atoi(next());
@@ -575,6 +697,11 @@ int main(int argc, char** argv) {
            "                            --op alltoall: the quantising all-to-all-v, -d bfloat16|half|float in, --out-dtype WIRE (the default); each rank\n"
            "                            sends an even split of whole --row-len rows to every peer and receives FP8 rows plus one fp32 scale per\n"
            "                            BLOCK; -c 1 checks every FP8 byte and scale bit for bit against the host quantiser\n"
+           "  --combine K               --op alltoall: the expert combine (all-to-all-v back, top-K weighted sum fused), -d bfloat16|half|float the\n"
+           "                            expert_out type, --out-dtype bfloat16|half|float the out type, --row-len a multiple of 16; every rank returns\n"
+           "                            an even split of whole rows, each token takes K slots from K different ranges where there are enough (seeded\n"
+           "                            routing and weights); size = expert_out bytes read per rank; -c 1 checks every output element bit for bit\n"
+           "                            against the slot-order host reference\n"
            "  --algo auto|ll|ll2|oneshot|twoshot|nvls   --inplace 0|1|2   --max-ctas N   --sweep kind:ctas:threads,...   --json FILE   --window SIZE\n"
            "  --selfcheck               report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;

@@ -6,7 +6,7 @@ Comm.all_to_all_v(). Routing is drawn from a Zipf-like popularity so some expert
 §7.3-7 warns about)."""
 from __future__ import annotations
 
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 
 import numpy as np
 
@@ -19,6 +19,11 @@ class DispatchPlan:
     send_off: np.ndarray        # send_off[s, d]: first row of that block in s's send buffer
     recv_off: np.ndarray        # recv_off[d, s]: first row of s's block in d's recv buffer
     max_rows: int               # buffer capacity (rows) that fits every rank's send and recv side
+    # index[s]: [tokens, top_k] int32, the row of rank s's send buffer each (token, slot) is dispatched as (within a destination's
+    # range, rows in row-major (token, slot) order); weights[s]: [tokens, top_k] float32 gate weights summing to 1 per token. Together
+    # with rows / send_off / recv_off they are the arguments of Comm.all_to_all_v_combine().
+    index: list = field(default_factory=list)
+    weights: list = field(default_factory=list)
 
     def bytes_sent(self, rank: int, itemsize: int = 2) -> int:
         return int(self.rows[rank].sum()) * self.hidden * itemsize
@@ -30,16 +35,30 @@ def expert_dispatch_plan(nranks: int, tokens_per_rank: int, hidden: int, experts
     pop = 1.0 / np.arange(1, n_experts + 1) ** skew if skew > 0 else np.ones(n_experts)
     pop = rng.permutation(pop / pop.sum())
     rows = np.zeros((nranks, nranks), dtype=np.int64)
+    dests = []
     for s in range(nranks):
         choice = rng.choice(n_experts, size=(tokens_per_rank, top_k), p=pop)
         dest = choice // experts_per_rank
+        dests.append(dest)
         rows[s] = np.bincount(dest.ravel(), minlength=nranks)
     send_off = np.zeros_like(rows)
     send_off[:, 1:] = np.cumsum(rows, axis=1)[:, :-1]
+    index = []
+    for s, dest in enumerate(dests):
+        flat = dest.ravel()
+        order = np.argsort(flat, kind="stable")                  # row-major (token, slot) order within each destination
+        idx = np.empty(flat.size, dtype=np.int64)
+        idx[order] = np.arange(flat.size)                        # rank among all slots sorted by destination = row in s's send buffer
+        index.append(idx.reshape(tokens_per_rank, top_k).astype(np.int32))
+    wrng = np.random.default_rng([seed, 0x6A7E])                 # its own generator: the routing above stays what it was
+    weights = []
+    for s in range(nranks):
+        w = wrng.random((tokens_per_rank, top_k)) + 0.05
+        weights.append((w / w.sum(axis=1, keepdims=True)).astype(np.float32))
     recv_off = np.zeros_like(rows)                       # recv_off[d, s]
     recv_off[:, 1:] = np.cumsum(rows.T, axis=1)[:, :-1]
     max_rows = int(max(rows.sum(axis=1).max(), rows.sum(axis=0).max()))
-    return DispatchPlan(nranks, hidden, rows, send_off, recv_off, max_rows)
+    return DispatchPlan(nranks, hidden, rows, send_off, recv_off, max_rows, index, weights)
 
 
 def uniform_plan(nranks: int, rows_per_peer: int, hidden: int) -> DispatchPlan:

@@ -137,6 +137,8 @@ def load() -> C.CDLL:
     L.b200collAllReduceQuantized.argtypes = [vp, vp, sz, ci, ci, C.POINTER(Epilogue), ci, vp, vp]
     i64p = C.POINTER(C.c_int64)
     L.b200collAllToAllvQuantized.argtypes = [vp, vp, C.POINTER(C.c_float), sz, sz, i64p, i64p, i64p, ci, ci, ci, vp, vp]
+    L.b200collAllToAllvCombine.argtypes = [vp, vp, sz, sz, i64p, i64p, i64p, C.POINTER(C.c_int32), C.POINTER(C.c_float), sz, ci,
+                                           C.POINTER(Epilogue), vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -317,6 +319,64 @@ def check_all_to_all_v_quantized(nranks: int, src, out, out_scales, row_elems: i
         if na and nb and a < b + nb and b < a + na:
             raise ValueError("src must not overlap out or out_scales")
     return torch_dtype_code(src.dtype), torch_dtype_code(out.dtype)
+
+
+def check_all_to_all_v_combine(nranks: int, expert_out, out, row_elems: int, send_rows, send_row_off, recv_row_off_at_peer, index,
+                               weights) -> tuple[int, int]:
+    """Rules of the expert combine, checked on the tensors' metadata and the host lists only (no communicator, no library call): raises
+    ValueError, returns the library codes of (expert_out's type, out's type). expert_out and out: contiguous bfloat16, float16 or float32;
+    row_elems a positive multiple of 16 dividing expert_out.numel(); index: contiguous int32 [tokens, top_k] with top_k >= 1; weights:
+    None or contiguous float32 of index's shape; out.numel() == tokens * row_elems. The three lists have nranks non-negative entries,
+    the non-empty send ranges [send_row_off[p], + send_rows[p]) are disjoint, and every destination range [recv_row_off_at_peer[p],
+    + send_rows[p]) lies inside expert_out, in rows of row_elems elements. out must not overlap expert_out, index or weights."""
+    import operator
+
+    import torch
+    wide = (torch.bfloat16, torch.float16, torch.float32)
+    for name, t in (("expert_out", expert_out), ("out", out)):
+        if t.dtype not in wide or not t.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous bfloat16, float16 or float32 tensor, got {t.dtype}")
+    if isinstance(row_elems, bool) or not isinstance(row_elems, int) or row_elems <= 0 or row_elems % 16:
+        raise ValueError(f"row_elems must be a positive multiple of 16, got {row_elems!r}")
+    if expert_out.numel() % row_elems:
+        raise ValueError(f"expert_out.numel() ({expert_out.numel()}) must be a multiple of row_elems ({row_elems})")
+    if index.dtype != torch.int32 or index.dim() != 2 or not index.is_contiguous() or index.shape[1] < 1:
+        raise ValueError(f"index must be a contiguous int32 [tokens, top_k] tensor with top_k >= 1, got {index.dtype}{list(index.shape)}")
+    tokens, top_k = index.shape
+    if weights is not None and (weights.dtype != torch.float32 or tuple(weights.shape) != (tokens, top_k) or not weights.is_contiguous()):
+        raise ValueError(f"weights must be None or a contiguous float32 [{tokens}, {top_k}] tensor, got {weights.dtype}{list(weights.shape)}")
+    if out.numel() != tokens * row_elems:
+        raise ValueError(f"out must hold tokens * row_elems = {tokens * row_elems} elements, got {out.numel()}")
+    lists = {"send_rows": send_rows, "send_row_off": send_row_off, "recv_row_off_at_peer": recv_row_off_at_peer}
+    vals = {}
+    for name, xs in lists.items():
+        try:
+            vals[name] = [operator.index(x) for x in xs]
+        except TypeError:
+            raise ValueError(f"{name} must be a sequence of integers") from None
+        if len(vals[name]) != nranks:
+            raise ValueError(f"{name} must have nranks = {nranks} entries, got {len(vals[name])}")
+        if any(x < 0 for x in vals[name]):
+            raise ValueError(f"{name} must not hold negative entries: {vals[name]}")
+    eo_rows = expert_out.numel() // row_elems
+    ranges = []
+    for p, (rows, so, ro) in enumerate(zip(vals["send_rows"], vals["send_row_off"], vals["recv_row_off_at_peer"])):
+        if ro + rows > eo_rows:
+            raise ValueError(f"peer {p}: destination rows [{ro}, {ro + rows}) lie past the {eo_rows} rows of expert_out")
+        if rows:
+            ranges.append((so, so + rows, p))
+    ranges.sort()
+    for (lo0, hi0, p0), (lo1, hi1, p1) in zip(ranges, ranges[1:]):
+        if lo1 < hi0:
+            raise ValueError(f"the send ranges of peers {p0} [{lo0}, {hi0}) and {p1} [{lo1}, {hi1}) overlap: a dispatch row must belong to one peer")
+    a, na = out.data_ptr(), out.numel() * out.element_size()
+    for name, t in (("expert_out", expert_out), ("index", index), ("weights", weights)):
+        if t is None:
+            continue
+        b, nb = t.data_ptr(), t.numel() * t.element_size()
+        if na and nb and a < b + nb and b < a + na:
+            raise ValueError(f"out must not overlap {name}")
+    return torch_dtype_code(expert_out.dtype), torch_dtype_code(out.dtype)
 
 
 class _CudaArray:
@@ -625,6 +685,26 @@ class Comm:
                                                  row_elems, out.numel() // row_elems, arr(send_rows), arr(send_row_off), arr(recv_row_off_at_peer), ic, wc, block,
                                                  self._h, self._stream(stream)), "AllToAllvQuantized")
         return out, out_scales
+
+    def all_to_all_v_combine(self, expert_out, out, row_elems: int, send_rows, send_row_off, recv_row_off_at_peer, index, weights=None,
+                             scale: float = 1.0, stream=None):
+        """Expert combine (b200collAllToAllvCombine), the reverse of all_to_all_v with the top-k weighted sum fused: the three lists are
+        the ones this rank passed to its dispatch call; index [tokens, top_k] int32 names, per token and slot, a row of that dispatch's
+        send buffer (-1: dropped); weights [tokens, top_k] float32 or None (all ones). out[t] = round(scale * sum over slots in slot
+        order of weights[t, j] * (expert output of row index[t, j])), pulled from the expert_out of the peer that row went to. Returns
+        out. With more than one rank, expert_out must be an arena tensor (`empty()`) of the same size on every rank; every rank calls,
+        a rank with no tokens included."""
+        ic, oc = check_all_to_all_v_combine(self.nranks, expert_out, out, row_elems, send_rows, send_row_off, recv_row_off_at_peer, index, weights)
+        n = self.nranks
+        arr = lambda xs: (C.c_int64 * n)(*[int(x) for x in xs])
+        tokens, top_k = index.shape
+        ep = Epilogue(ic, oc, float(scale))
+        w = C.cast(C.c_void_p(weights.data_ptr() if weights is not None else None), C.POINTER(C.c_float))
+        _check(load().b200collAllToAllvCombine(C.c_void_p(expert_out.data_ptr()), C.c_void_p(out.data_ptr()), row_elems, expert_out.numel() // row_elems,
+                                               arr(send_rows), arr(send_row_off), arr(recv_row_off_at_peer),
+                                               C.cast(C.c_void_p(index.data_ptr()), C.POINTER(C.c_int32)), w, tokens, top_k, C.byref(ep),
+                                               self._h, self._stream(stream)), "AllToAllvCombine")
+        return out
 
     def broadcast(self, src, dst=None, root: int = 0, scale: float = 1.0, stream=None):
         """dst on every rank = cast(scale * src of `root`). src is read on the root only (ncclBroadcast)."""
