@@ -15,9 +15,13 @@ library's generic kernel; FP8 reductions (every operator) accumulate in fp32 and
 all-gather and all-to-all move the bytes untouched, as words. Everything else (CPU tensors, odd shapes) is executed by an
 internal Gloo group over host copies: slow but correct, which keeps DDP's bookkeeping collectives and object broadcasts working.
 
-Status: the fallback and dispatch logic is exercised on CPU (tests/test_process_group.py); the CUDA fast paths reuse the calls the GPU
-suite covers through `ops.coll.Comm`, but the process group itself has not run on a GPU box yet (tests/test_process_group.py has the
-two-process GPU test, opt-in until it has).
+Which route a collective takes (a fused kernel, the generic kernel, a word view, Gloo) depends only on what every rank shares: device
+type, dtype, element counts, operator, split lists being given or not. Never on layout: a tensor that is not contiguous or not 16-byte
+aligned on one rank travels through an aligned contiguous temporary on that rank, and a rank that sends no rows to an uneven all-to-all
+still enters it. Ranks that chose different transports for one collective would wait for each other until the watchdog fires.
+
+Status: the dispatch logic is exercised on CPU (tests/test_process_group.py, including that the route is the same whatever the layout);
+tests/test_process_group_numerics_gpu.py runs every route at 2, 3 and 4 ranks on a GPU, bit for bit against tests/coll_fp_reference.py.
 """
 from __future__ import annotations
 
@@ -81,7 +85,27 @@ class _P2pWork(_Work):
 
 
 def _fast(t: torch.Tensor) -> bool:
-    return t.is_cuda and t.is_contiguous() and t.dtype in _FAST_DTYPES and t.data_ptr() % 16 == 0 and t.numel() > 0
+    return t.is_cuda and t.dtype in _FAST_DTYPES and t.numel() > 0
+
+
+# The kernels take contiguous, 16-byte aligned buffers. Layout is a per-rank fact, so it never picks the route (see the module
+# docstring): a tensor the kernel cannot take as it is goes through a temporary on this rank only.
+def _direct(t: torch.Tensor) -> bool:
+    return t.is_contiguous() and t.data_ptr() % 16 == 0
+
+
+def _src(t: torch.Tensor) -> torch.Tensor:
+    return t if _direct(t) else t.detach().clone(memory_format=torch.contiguous_format)      # a fresh allocation is aligned
+
+
+def _dst(t: torch.Tensor) -> torch.Tensor:
+    """Where the kernel writes: `t` itself, or a temporary the caller copies into `t` afterwards (`_finish`)."""
+    return t if _direct(t) else torch.empty_like(t, memory_format=torch.contiguous_format)
+
+
+def _finish(t: torch.Tensor, d: torch.Tensor) -> None:
+    if d is not t:
+        t.copy_(d)
 
 
 _GENERIC_DTYPES = (torch.int8, torch.uint8, torch.int32, torch.int64, torch.float64)      # any operator but AVG, on the generic P2P kernel
@@ -108,7 +132,7 @@ def _red_op(op) -> Optional[int]:
 
 
 def _reducible(t: torch.Tensor, op: Optional[int]) -> bool:
-    if op is None or not (t.is_cuda and t.is_contiguous() and t.data_ptr() % 16 == 0 and t.numel() > 0):
+    if op is None or not (t.is_cuda and t.numel() > 0):
         return False
     if t.dtype in _FAST_DTYPES or t.dtype in _FP8_DTYPES:
         return True
@@ -136,6 +160,7 @@ class B200CollProcessGroup(dist.ProcessGroup):
         self._last_stream = None          # stream and completion event of the previous device collective (see _ordered)
         self._last_event = None
         self._pending: list = []          # queued point-to-point operations: (kind, tensor, peer), launched as one group
+        self._no_rows = None              # a small aligned tensor: the send buffer of a rank with no rows in an uneven all-to-all
         self.fast_calls = 0               # collectives that ran on libb200coll
         self.fallback_calls = 0           # collectives that ran on the Gloo group
 
@@ -229,7 +254,9 @@ class B200CollProcessGroup(dist.ProcessGroup):
         if op is not None and all(_reducible(t, op) for t in tensors):
             with self._ordered(self):
                 for t in tensors:
-                    self.comm.all_reduce(t, op=op)
+                    d = _src(t)
+                    self.comm.all_reduce(d, op=op)
+                    _finish(t, d)
             self.fast_calls += 1
             return self._work(tensors)
         gopts = dist.AllreduceOptions()
@@ -241,7 +268,7 @@ class B200CollProcessGroup(dist.ProcessGroup):
         self._via_gloo(tensors, lambda h: self.gloo.allreduce(h, gopts))
         if avg:
             for t in tensors:
-                t.div_(self._size)
+                t.div_(self._size, rounding_mode=None if t.is_floating_point() else "trunc")     # integers: the quotient toward zero, as NCCL's avg
         return self._work(tensors)
 
     def allreduce_coalesced(self, tensors, opts=None):
@@ -251,11 +278,12 @@ class B200CollProcessGroup(dist.ProcessGroup):
         root = opts.rootRank if opts is not None else 0
         done = []
         for t in tensors:
-            words = self._as_words(t)
-            if words is None:
+            if not self._has_words(t):
                 break
+            d = _src(t)
             with self._ordered(self):
-                self.comm.broadcast(words, root=root)
+                self.comm.broadcast(self._as_words(d), root=root)
+            _finish(t, d)
             done.append(t)
         if len(done) == len(tensors):
             self.fast_calls += 1
@@ -269,9 +297,14 @@ class B200CollProcessGroup(dist.ProcessGroup):
         return self._work(tensors)
 
     @staticmethod
+    def _has_words(t: torch.Tensor) -> bool:
+        """Can this tensor's bytes travel as fp16 / fp32 words? Decided from device type, dtype and byte count only."""
+        return t.is_cuda and t.numel() > 0 and (t.dtype in _FAST_DTYPES or (t.numel() * t.element_size()) % 2 == 0)
+
+    @staticmethod
     def _as_words(t: torch.Tensor) -> Optional[torch.Tensor]:
-        """View any contiguous CUDA tensor as fp16/fp32 words for bit-exact movement (broadcast does not care about the dtype)."""
-        if not (t.is_cuda and t.is_contiguous() and t.numel() > 0 and t.data_ptr() % 16 == 0):
+        """View a contiguous, aligned CUDA tensor as fp16/fp32 words for bit-exact movement (broadcast does not care about the dtype)."""
+        if not (t.is_cuda and t.numel() > 0 and _direct(t)):
             return None
         if t.dtype in _FAST_DTYPES:
             return t.view(-1)
@@ -301,7 +334,10 @@ class B200CollProcessGroup(dist.ProcessGroup):
         if op is not None and all(_reducible(t, op) for t in tensors):
             with self._ordered(self):
                 for t in tensors:
-                    self.comm.reduce(t, root=root, op=op)
+                    d = _src(t)
+                    self.comm.reduce(d, root=root, op=op)
+                    if self._rank == root:
+                        _finish(t, d)
             self.fast_calls += 1
             return self._work(tensors)
         gopts = dist.ReduceOptions()
@@ -312,21 +348,22 @@ class B200CollProcessGroup(dist.ProcessGroup):
         return self._work(tensors)
 
     def _allgather_base(self, output, input, opts=None):
-        if _fast(output) and _fast(input) and output.dtype == input.dtype and (input.numel() * input.element_size()) % 16 == 0 \
+        if output.is_cuda and input.is_cuda and output.dtype == input.dtype and input.numel() > 0 and (input.numel() * input.element_size()) % 16 == 0 \
                 and output.numel() == input.numel() * self._size:
-            with self._ordered(self):
-                self.comm.all_gather(input.view(-1), output.view(-1))
+            o, i = _dst(output), _src(input)
+            if input.dtype in _FAST_DTYPES:
+                with self._ordered(self):
+                    self.comm.all_gather(i.view(-1), o.view(-1))
+            else:                                               # integer / bool / fp8 payloads (token ids, masks): moved as raw words
+                words = self._word_views(o, i)
+                with self._ordered(self), self.comm.bit_exact():
+                    self.comm.all_gather(words[1], words[0])
+            _finish(output, o)
             self.fast_calls += 1
             return self._work(output)
-        words = self._word_views(output, input) if output.dtype == input.dtype and output.numel() == input.numel() * self._size \
-            and (input.numel() * input.element_size()) % 16 == 0 else None
-        if words is not None:                                   # integer / bool / fp8 payloads (token ids, masks): moved as raw words
-            with self._ordered(self), self.comm.bit_exact():
-                self.comm.all_gather(words[1], words[0])
-            self.fast_calls += 1
-            return self._work(output)
-        chunks = list(output.view(-1).chunk(self._size))
-        self.allgather([chunks], [input.view(-1)])
+        o = output if output.is_contiguous() else torch.empty(output.shape, dtype=output.dtype, device=output.device)
+        self.allgather([list(o.view(-1).chunk(self._size))], [input.reshape(-1)])
+        _finish(output, o)
         return self._work(output)
 
     def allgather(self, output_tensors, input_tensors, opts=None):
@@ -335,7 +372,7 @@ class B200CollProcessGroup(dist.ProcessGroup):
             if same and _fast(inp) and all(o.is_cuda for o in outs) and (inp.numel() * inp.element_size()) % 16 == 0:
                 flat = torch.empty(inp.numel() * self._size, dtype=inp.dtype, device=inp.device)
                 with self._ordered(self):
-                    self.comm.all_gather(inp.view(-1), flat)
+                    self.comm.all_gather(_src(inp).view(-1), flat)
                 for o, piece in zip(outs, flat.chunk(self._size)):
                     o.copy_(piece.view_as(o))
                 self.fast_calls += 1
@@ -355,17 +392,19 @@ class B200CollProcessGroup(dist.ProcessGroup):
 
     def _reduce_scatter_base(self, output, input, opts=None):
         op = _sum_or_avg(opts.reduceOp) if opts is not None else coll.SUM
-        fp8 = output.dtype in _FP8_DTYPES and _reducible(output, op) and _reducible(input, op)
-        if op is not None and (fp8 or (_fast(output) and _fast(input))) and output.dtype == input.dtype and (output.numel() * output.element_size()) % 16 == 0 \
-                and input.numel() == output.numel() * self._size:
+        fused = output.dtype in _FAST_DTYPES or output.dtype in _FP8_DTYPES
+        if op is not None and fused and output.is_cuda and input.is_cuda and output.dtype == input.dtype and output.numel() > 0 \
+                and (output.numel() * output.element_size()) % 16 == 0 and input.numel() == output.numel() * self._size:
+            o, i = _dst(output), _src(input)
             with self._ordered(self):
-                self.comm.reduce_scatter(input.view(-1), output.view(-1), op=op)
+                self.comm.reduce_scatter(i.view(-1), o.view(-1), op=op)
+            _finish(output, o)
             self.fast_calls += 1
             return self._work(output)
         # generic: all-reduce a copy, keep my slice
-        tmp = input.detach().clone().view(-1)
+        tmp = input.detach().clone().reshape(-1)
         self.allreduce([tmp], opts)
-        output.view(-1).copy_(tmp.chunk(self._size)[self._rank])
+        output.copy_(tmp.chunk(self._size)[self._rank].view_as(output))
         return self._work(output)
 
     def reduce_scatter(self, output_tensors, input_tensors, opts=None):
@@ -382,27 +421,34 @@ class B200CollProcessGroup(dist.ProcessGroup):
     def alltoall_base(self, output, input, output_split_sizes, input_split_sizes, opts=None):
         n = self._size
         even = not output_split_sizes and not input_split_sizes
-        if even and _fast(output) and _fast(input) and output.dtype == input.dtype and output.data_ptr() != input.data_ptr() \
+        # in place (refused by the library) is the caller's choice of arguments, made alike on every rank
+        if even and output.is_cuda and input.is_cuda and output.dtype == input.dtype and output.data_ptr() != input.data_ptr() and input.numel() > 0 \
                 and input.numel() % n == 0 and (input.numel() // n * input.element_size()) % 16 == 0 and output.numel() == input.numel():
-            with self._ordered(self):
-                self.comm.all_to_all(input.view(-1), output.view(-1))
+            o, i = _dst(output), _src(input)
+            if input.dtype in _FAST_DTYPES:
+                with self._ordered(self):
+                    self.comm.all_to_all(i.view(-1), o.view(-1))
+            else:
+                words = self._word_views(o, i)
+                with self._ordered(self), self.comm.bit_exact():
+                    self.comm.all_to_all(words[1], words[0])
+            _finish(output, o)
             self.fast_calls += 1
             return self._work(output)
-        words = self._word_views(output, input) if even and output.dtype == input.dtype and output.data_ptr() != input.data_ptr() and input.numel() % n == 0 \
-            and (input.numel() // n * input.element_size()) % 16 == 0 and output.numel() == input.numel() else None
-        if words is not None:
-            with self._ordered(self), self.comm.bit_exact():
-                self.comm.all_to_all(words[1], words[0])
-            self.fast_calls += 1
-            return self._work(output)
-        row_elems = input[0].numel() if input.dim() > 0 and input.shape[0] > 0 else 0
-        if not even and row_elems and _fast(input) and output.is_cuda and output.is_contiguous() and output.dtype == input.dtype \
-                and (row_elems * input.element_size()) % 16 == 0:
-            return self._alltoallv_rows(output, input, list(input_split_sizes), row_elems)
+        # uneven: the row width comes from the trailing shape, which every rank shares; the number of rows (none at all for a rank that
+        # sends nothing) does not pick the route
+        row_elems = 1
+        for d in input.shape[1:]:
+            row_elems *= d
+        if not even and input.dim() > 0 and output.dim() > 0 and input.is_cuda and output.is_cuda and input.dtype in _FAST_DTYPES and output.dtype == input.dtype \
+                and row_elems > 0 and (row_elems * input.element_size()) % 16 == 0:
+            # a split list left out means equal blocks (c10d's rule); each rank's own row of the split matrix is all the route below needs
+            in_splits = list(input_split_sizes) or [input.shape[0] // n] * n
+            return self._alltoallv_rows(output, input, in_splits, row_elems)
         # Gloo: works on host copies for any layout
         self.fallback_calls += 1
-        host_in = input.detach().cpu() if input.is_cuda else input
-        host_out = torch.empty_like(output, device="cpu")
+        host_in = (input.detach().cpu() if input.is_cuda else input).contiguous()
+        host_out = torch.empty(output.shape, dtype=output.dtype)
         self.gloo.alltoall_base(host_out, host_in, list(output_split_sizes or []), list(input_split_sizes or [])).wait()
         output.copy_(host_out)
         return self._work(output)
@@ -423,10 +469,16 @@ class B200CollProcessGroup(dist.ProcessGroup):
         if scratch is None:
             scratch = self._scratch[cls] = self.comm.empty(cls, torch.uint8)
         recv = scratch[:need].view(input.dtype)
+        if input.numel() == 0:                               # no rows to send: the library still wants a real, aligned send pointer
+            if self._no_rows is None:
+                self._no_rows = torch.zeros(16, dtype=torch.uint8, device=output.device)
+            src = self._no_rows.view(input.dtype)
+        else:
+            src = _src(input).view(-1)
         with self._ordered(self):
-            self.comm.all_to_all_v(input.view(-1), recv, row_elems, send_rows, send_off, recv_off_at_peer)
+            self.comm.all_to_all_v(src, recv, row_elems, send_rows, send_off, recv_off_at_peer)
         got_rows = sum(matrix[s][self._rank] for s in range(n))
-        output.view(-1)[:got_rows * row_elems].copy_(recv[:got_rows * row_elems])
+        output[:got_rows].copy_(recv[:got_rows * row_elems].view(got_rows, *output.shape[1:]))
         self.fast_calls += 1
         return self._work(output)
 
@@ -530,17 +582,16 @@ class B200CollProcessGroup(dist.ProcessGroup):
         if not ops:
             return
         comm, copy_out, keep = self.comm, [], []
-        direct = lambda t: t.is_contiguous() and t.data_ptr() % 16 == 0
         with coll.group():
             for kind, t, peer in ops:
                 if t.numel() == 0:
                     continue
                 if kind == "send":
-                    if not direct(t):
+                    if not _direct(t):
                         t = t.contiguous().clone()      # clone(): a fresh allocation is aligned
                         keep.append(t)                  # Comm.send only records the pointer; the kernel is launched when the group closes,
                     comm.send(t, peer)                  # so the temporary must stay allocated (and un-reused) until then
-                elif direct(t):
+                elif _direct(t):
                     comm.recv(t, peer)
                 else:
                     tmp = torch.empty(t.shape, dtype=t.dtype, device=t.device)

@@ -209,7 +209,7 @@ def _gpu_pair(rank, world):
         with torch.cuda.stream(side):
             dist.all_reduce(b)
     torch.cuda.synchronize()
-    assert torch.isfinite(a).all() and torch.isfinite(b).all() and a[0].item() == a[-1].item() and b[0].item() == b[-1].item()
+    assert a.eq(3.0 * 2 ** 19).all() and b.eq(30.0 * 2 ** 19).all()              # 1 + 2, then doubled by each of the 19 later rounds
     # point to point: blocking pair, then a ring step as isend + irecv (queued, one grouped kernel at the first wait), a strided tensor,
     # and batch_isend_irecv
     other = 1 - rank
@@ -394,3 +394,171 @@ def test_integer_payloads_move_as_words_and_never_take_the_lamport_path(monkeypa
     del log[:]
     flt = _DeviceLike.of(torch.zeros(64)); pg._allgather_base(_DeviceLike.of(torch.zeros(128)), flt)      # real floats keep the tuner's choice
     assert log == [("all_gather", torch.float32, 64, 128)] and pg.fast_calls == 3 and pg.fallback_calls == 0
+
+
+# ------------------------------------------------------------------------------------------------- the route is the same on every rank (no GPU)
+class _RouteComm:
+    """Stands in for the communicator: logs which library call was made, refuses a buffer the kernels could not take, and writes 7s
+    where the kernel would write."""
+    nranks = 2
+    _algo = "auto"
+
+    def __init__(self, log):
+        self.log = log
+
+    def _call(self, name, *bufs, out=None):
+        assert all(b.is_contiguous() and b.data_ptr() % 16 == 0 and b.data_ptr() != 0 for b in bufs), f"{name}: a buffer the kernel cannot take"
+        self.log.append("lib." + name)
+        if out is not None:
+            out.fill_(7)
+
+    def check_async_error(self): pass
+    def set_algo(self, name): self._algo = name
+    def bit_exact(self): self.log.append("bit_exact"); return pgmod.coll.Comm._BitExact(self)
+    def empty(self, numel, dtype): return torch.zeros(numel, dtype=dtype)
+    def all_reduce(self, t, op=None): self._call("all_reduce", t, out=t)
+    def reduce(self, t, root=0, op=None): self._call("reduce", t, out=t)
+    def broadcast(self, t, root=0): self._call("broadcast", t, out=t)
+    def all_gather(self, src, dst): self._call("all_gather", src, dst, out=dst)
+    def reduce_scatter(self, src, dst, op=None): self._call("reduce_scatter", src, dst, out=dst)
+    def all_to_all(self, src, dst): self._call("all_to_all", src, dst, out=dst)
+    def all_to_all_v(self, src, dst, row_elems, send_rows, send_off, recv_off): self._call("all_to_all_v", src, dst, out=dst)
+
+
+class _RouteGloo:
+    """Stands in for the Gloo group: logs the call; its all-gather hands back the split matrix of the uneven all-to-all."""
+    class _Done:
+        def wait(self): return True
+
+    def __init__(self, log, matrix):
+        self.log, self.matrix = log, matrix
+
+    def allgather(self, outs, ins, *a):
+        self.log.append("gloo.allgather")
+        for o, row in zip(outs[0], self.matrix):
+            if o.numel() == len(row):
+                o.copy_(torch.tensor(row))
+        return self._Done()
+
+    def __getattr__(self, name):
+        def call(*a, **k):
+            self.log.append("gloo." + name)
+            return self._Done()
+        return call
+
+
+def _route_group(monkeypatch, rank, matrix=((0, 0), (0, 0))):
+    class _Stream:
+        def wait_event(self, e): pass
+        def synchronize(self): pass
+    class _Event:
+        def record(self, s): pass
+    stream = _Stream()
+    monkeypatch.setattr(torch.cuda, "current_stream", lambda *a, **k: stream)
+    monkeypatch.setattr(torch.cuda, "Event", _Event)
+    log = []
+    pg = pgmod.B200CollProcessGroup(store=None, rank=rank, size=2)
+    pg._comm, pg._gloo = _RouteComm(log), _RouteGloo(log, [list(r) for r in matrix])
+    return pg, log
+
+
+def _laid_out(layout, numel, dtype=torch.float32, cols=None):
+    """A device-like tensor of `numel` elements (rows of `cols`): as the allocator gives it, starting 4 or 8 bytes past a 16-byte
+    boundary, or a column slice of a wider tensor."""
+    shape = (numel,) if cols is None else (numel // cols, cols)
+    if layout == "misaligned":
+        return _DeviceLike.of(torch.zeros(numel + 1, dtype=dtype))[1:].view(shape)
+    if layout == "strided":
+        return _DeviceLike.of(torch.zeros(*shape, 2, dtype=dtype))[..., 0]
+    return _DeviceLike.of(torch.zeros(shape, dtype=dtype))
+
+
+def _ar_opts(op):
+    o = dist.AllreduceOptions(); o.reduceOp = op
+    return o
+
+
+def _rs_opts(op):
+    o = dist.ReduceScatterOptions(); o.reduceOp = op
+    return o
+
+
+# name -> (call(pg, make) -> the tensor that must have been written, or None; the route every rank must take)
+_ROUTE_CASES = {
+    "all_reduce fp32 sum": (lambda pg, mk: (lambda t: (pg.allreduce([t], _ar_opts(dist.ReduceOp.SUM)), t)[1])(mk(64)), ["lib.all_reduce"]),
+    "all_reduce int64 max": (lambda pg, mk: (lambda t: (pg.allreduce([t], _ar_opts(dist.ReduceOp.MAX)), t)[1])(mk(64, torch.int64)), ["lib.all_reduce"]),
+    "all_reduce int32 avg": (lambda pg, mk: (pg.allreduce([mk(64, torch.int32)], _ar_opts(dist.ReduceOp.AVG)), None)[1], ["gloo.allreduce"]),
+    "reduce bf16 (root)": (lambda pg, mk: (lambda t: (pg.reduce([t]), t)[1])(mk(64, torch.bfloat16)), ["lib.reduce"]),
+    "broadcast int64": (lambda pg, mk: (lambda t: (pg.broadcast([t]), t)[1])(mk(33, torch.int64)), ["lib.broadcast"]),
+    "broadcast uint8, odd bytes": (lambda pg, mk: (pg.broadcast([mk(33, torch.uint8)]), None)[1], ["gloo.broadcast"]),
+    "all_gather_into_tensor fp32": (lambda pg, mk: (lambda o: (pg._allgather_base(o, mk(64)), o)[1])(mk(128)), ["lib.all_gather"]),
+    "all_gather_into_tensor int64": (lambda pg, mk: (lambda o: (pg._allgather_base(o, mk(64, torch.int64)), o)[1])(mk(128, torch.int64)),
+                                     ["bit_exact", "lib.all_gather"]),
+    "all_gather list fp32": (lambda pg, mk: (lambda outs: (pg.allgather([outs], [mk(64)]), outs[1])[1])([mk(64), mk(64)]), ["lib.all_gather"]),
+    "reduce_scatter_tensor bf16 avg": (lambda pg, mk: (lambda o: (pg._reduce_scatter_base(o, mk(128, torch.bfloat16), _rs_opts(dist.ReduceOp.AVG)), o)[1])(mk(64, torch.bfloat16)),
+                                       ["lib.reduce_scatter"]),
+    "reduce_scatter_tensor fp32 max": (lambda pg, mk: (lambda o: (pg._reduce_scatter_base(o, mk(128), _rs_opts(dist.ReduceOp.MAX)), o)[1])(mk(64)),
+                                       ["lib.all_reduce"]),
+    "all_to_all_single even fp32": (lambda pg, mk: (lambda o: (pg.alltoall_base(o, mk(128), [], []), o)[1])(mk(128)), ["lib.all_to_all"]),
+    "all_to_all_single even int64": (lambda pg, mk: (lambda o: (pg.alltoall_base(o, mk(128, torch.int64), [], []), o)[1])(mk(128, torch.int64)),
+                                     ["bit_exact", "lib.all_to_all"]),
+}
+
+
+@pytest.mark.parametrize("case", sorted(_ROUTE_CASES))
+def test_the_route_does_not_depend_on_this_ranks_layout(monkeypatch, case):
+    """Every rank must take the same route, so the route may depend only on what the ranks share (device type, dtype, counts, operator).
+    The same call with this rank's tensors misaligned or strided takes the route the plain call takes, the kernel still only sees
+    aligned contiguous buffers (_RouteComm checks), and the result reaches the caller's tensor."""
+    call, want = _ROUTE_CASES[case]
+    for layout in ("plain", "misaligned", "strided"):
+        pg, log = _route_group(monkeypatch, rank=0)
+        written = call(pg, lambda numel, dtype=torch.float32: _laid_out(layout, numel, dtype))
+        assert log == want, (case, layout, log)
+        assert (pg.fast_calls, pg.fallback_calls) == ((1, 0) if want[-1].startswith("lib.") else (0, 1)), (case, layout)
+        if written is not None and want[-1].startswith("lib."):
+            assert bool((written != 0).all()), (case, layout, "the result never reached the caller's tensor")
+
+
+def _uneven(pg, rows_in, rows_out, in_splits, out_splits, layout="plain", cols=8, dtype=torch.float32):
+    src = _laid_out(layout, rows_in * cols, dtype, cols) if rows_in else _DeviceLike.of(torch.zeros(0, cols, dtype=dtype))
+    dst = _laid_out(layout, rows_out * cols, dtype, cols) if rows_out else _DeviceLike.of(torch.zeros(0, cols, dtype=dtype))
+    pg.alltoall_base(dst, src, out_splits, in_splits)
+    return dst
+
+
+def test_uneven_all_to_all_route_is_the_same_on_a_rank_without_rows(monkeypatch):
+    """Expert dispatch: rank 0 sends 2 + 3 rows, rank 1 sends nothing (a silent sender) and rank 0 receives nothing from it. Both must
+    enter the all-to-all-v (the split matrix over Gloo, then the library call); the silent rank hands the library a real send pointer."""
+    matrix = ((2, 3), (0, 0))
+    want = ["gloo.allgather", "lib.all_to_all_v"]
+    pg0, log0 = _route_group(monkeypatch, 0, matrix)
+    out0 = _uneven(pg0, 5, 2, [2, 3], [2, 0])
+    pg1, log1 = _route_group(monkeypatch, 1, matrix)
+    out1 = _uneven(pg1, 0, 3, [0, 0], [3, 0])
+    assert log0 == want and log1 == want, (log0, log1)
+    assert out0.eq(7).all() and out1.eq(7).all() and pg1.fallback_calls == 0
+    # nothing to receive either: still the same route
+    pg1, log1 = _route_group(monkeypatch, 1, ((2, 0), (0, 0)))
+    _uneven(pg1, 0, 0, [0, 0], [0, 0])
+    assert log1 == want
+    # layout of this rank's rows does not matter, and spare output rows are left alone
+    for layout in ("misaligned", "strided"):
+        pg0, log0 = _route_group(monkeypatch, 0, matrix)
+        out = _uneven(pg0, 5, 4, [2, 3], [2, 0], layout)
+        assert log0 == want and out[:2].eq(7).all() and out[2:].eq(0).all(), layout
+    # rows that are not whole 16-byte vectors, or an integer payload: Gloo, on the silent rank too
+    for cols, dtype in ((3, torch.float32), (8, torch.int64)):
+        for rank, rows_in, splits in ((0, 5, [2, 3]), (1, 0, [0, 0])):
+            pg, log = _route_group(monkeypatch, rank, matrix)
+            _uneven(pg, rows_in, 2, splits, [2, 0], cols=cols, dtype=dtype)
+            assert log == ["gloo.alltoall_base"], (cols, dtype, rank, log)
+
+
+def test_uneven_all_to_all_with_one_split_list_left_out(monkeypatch):
+    """c10d: a split list left out means equal blocks. The rank's row of the split matrix is then the even split, not an empty list."""
+    sent = []
+    pg, log = _route_group(monkeypatch, 0, ((2, 2), (1, 3)))
+    pg._gloo.allgather = lambda outs, ins, *a: (sent.append(ins[0].tolist()), _RouteGloo.allgather(pg._gloo, outs, ins))[1]
+    out = _uneven(pg, 4, 3, [], [2, 1])
+    assert sent == [[2, 2]] and log == ["gloo.allgather", "lib.all_to_all_v"] and out.eq(7).all()
