@@ -10,6 +10,10 @@ bytes on NVLink, no separate cast kernel); (c) NCCL all_to_all_single with split
 Then the combine back, with the dispatched rows standing in for the expert outputs: (e) all_to_all_v_combine, each rank pulling its
 tokens' top-k rows and summing them with the gate weights in one kernel, against (f) NCCL all_to_all_single back plus the PyTorch
 gather and weighted sum a MoE stack runs; combine_matches says ours equals an explicit slot-order fp32 sum bit for bit.
+Then the same routing from the router's device-side expert ids: (g) expert_dispatch, layout, count exchange and push with no host sync,
+and (h) expert_combine over its route, against (i) what a caller writes today to reach all_to_all_v from device ids: a device bincount,
+a .cpu(), an all-gather of the counts, the offsets on the host, an argsort permute of the rows, then all_to_all_v. routed_matches says
+nothing was dropped, the counts add up to the plan's rows, and the routed combine equals the slot-order fp32 sum bit for bit.
 Bus bandwidth = (bytes a rank sends off-chip, max over ranks) / time. Rank 0 prints one JSON line per shape."""
 from __future__ import annotations
 
@@ -89,8 +93,38 @@ def main() -> int:
             dist.all_to_all_single(nccl_back[:n_send], nccl_recv[:n_recv], in_split, out_split)
             return (nccl_back[:n_send].view(-1, hidden)[idx_l].float() * gate.unsqueeze(-1)).sum(dim=1).to(torch.bfloat16)
         us_nccl_comb = timed(nccl_combine)
+        # device-routed dispatch and combine from the plan's expert ids (4 experts per rank), into the same symmetric recv
+        n_exp, x = world * 4, send[:tokens * hidden].view(tokens, hidden)
+        topk = torch.from_numpy(plan.experts[rank]).cuda()
+        rrecv = recv[:q_rows * hidden]
+        _, counts, route, dropped = comm.expert_dispatch(x, topk, n_exp, rrecv)
+        us_routed = timed(lambda: comm.expert_dispatch(x, topk, n_exp, rrecv, counts, route, dropped))
+        us_routed_comb = timed(lambda: comm.expert_combine(rrecv.view(-1, hidden), route, gate, out))
+        comm.check_async_error()
+        # recv holds every rank's rows (plan.max_rows >= any rank's load): nothing dropped, this rank's counts add up to the rows the
+        # plan sends it, every slot routed, and the combine of the returned rows is the slot-order sum of each token's own row
+        xr = x.float()
+        acc = torch.zeros(tokens, hidden, device="cuda")
+        for j in range(topk.shape[1]):
+            acc = acc + gate[:, j:j + 1] * xr
+        routed_ok = (int(dropped.item()) == 0 and int(counts.sum().item()) == int(plan.rows[:, rank].sum()) and bool((route >= 0).all())
+                     and bool(torch.equal(out.view(torch.int16), acc.to(torch.bfloat16).view(torch.int16))))
+        all_counts = torch.empty(world * world, dtype=torch.int64, device="cuda")
+
+        def host_plan():
+            dest = (topk // 4).view(-1).long()
+            mine = torch.bincount(dest, minlength=world)
+            dist.all_gather_into_tensor(all_counts, mine)
+            m = all_counts.cpu().view(world, world).tolist()             # m[s][d]: rows s sends to d
+            h_rows = m[rank]
+            h_so = [sum(h_rows[:d]) for d in range(world)]
+            h_ro = [sum(m[s][d] for s in range(rank)) for d in range(world)]
+            order = torch.argsort(dest, stable=True)
+            permuted = x[order // topk.shape[1]]
+            comm.all_to_all_v(permuted, recv, hidden, h_rows, h_so, h_ro)
+        us_host_plan = timed(host_plan)
         offchip = max(int(plan.rows[s].sum() - plan.rows[s, s]) for s in range(world)) * hidden * 2
-        oks = torch.tensor([1.0 if ok else 0.0, 1.0 if comb_ok else 0.0], device="cuda"); dist.all_reduce(oks, op=dist.ReduceOp.MIN)
+        oks = torch.tensor([1.0 if ok else 0.0, 1.0 if comb_ok else 0.0, 1.0 if routed_ok else 0.0], device="cuda"); dist.all_reduce(oks, op=dist.ReduceOp.MIN)
         if rank == 0:
             print(json.dumps({"bench": "alltoallv_perf", "n_gpus": world, "tokens_per_rank": tokens, "hidden": hidden, "skew": skew, "top_k": 2,
                               "max_offchip_bytes_per_rank": offchip, "imbalance_max_over_mean": round(float(plan.rows.sum(axis=0).max() / plan.rows.sum(axis=0).mean()), 3),
@@ -98,7 +132,9 @@ def main() -> int:
                               "nccl_us": round(us_nccl, 2), "nccl_busbw": round(offchip / us_nccl / 1e3, 2), "speedup": round(us_nccl / us_ours, 2),
                               "fp8_speedup_vs_nccl_bf16": round(us_nccl / us_fp8, 2), "matches_nccl": bool(oks[0].item() == 1.0),
                               "ours_block_fp8_us": round(us_bsq, 2), "ours_combine_us": round(us_comb, 2), "nccl_combine_us": round(us_nccl_comb, 2),
-                              "combine_matches": bool(oks[1].item() == 1.0)}), flush=True)
+                              "combine_matches": bool(oks[1].item() == 1.0), "ours_routed_us": round(us_routed, 2),
+                              "ours_routed_combine_us": round(us_routed_comb, 2), "host_plan_us": round(us_host_plan, 2),
+                              "routed_matches": bool(oks[2].item() == 1.0)}), flush=True)
     comm.destroy()
     dist.destroy_process_group()
     return 0

@@ -358,6 +358,49 @@ b200collResult_t b200collAllToAllvCombine(const void* expert_out, void* out, siz
                                           const int64_t* send_rows, const int64_t* send_row_off, const int64_t* recv_row_off_at_peer,
                                           const int32_t* index, const float* weights, size_t tokens, int top_k,
                                           const b200collEpilogue* ep, b200collComm_t comm, b200collStream_t stream);
+/* Device-routed expert dispatch: the router's top-k expert ids in (device), rows grouped by expert out, with no host sync. Two kernels
+ * per call: a one-CTA layout kernel (per-expert counts, exchanged between ranks through a mailbox in the arena, and each slot's row),
+ * then a push of the rows over NVLink. Nothing the host must know depends on device data, so the call can be captured in a CUDA graph.
+ *   Experts: num_experts (E) experts, 1 <= E <= 1024, E a multiple of nranks; rank d owns experts [d*E/N, (d+1)*E/N).
+ *   topk_idx: device [tokens, top_k] int32. Slot (t, j) sends row t of x to expert topk_idx[t, j]; an id outside [0, E) drops the slot.
+ *   A token may name one expert twice: it is then sent twice.
+ *   x: [tokens, row_elems] of dtype (bf16, fp16 or fp32), any 16-byte aligned device buffer (only its own rank reads it). Rows move as
+ *   raw bits: NaN payloads and -0 survive.
+ *   recv: [recv_rows, row_elems] of dtype. On rank d it holds d's experts in ascending order; within an expert, rows by source rank
+ *   ascending; within a source, in row-major (token, slot) order. The row of slot (t, j) of rank s sent to expert e is
+ *   base_d(e) + sum_{s' < s} cnt[s'][e] + #{(t', j') < (t, j) on rank s with topk_idx = e}, base_d(e) the total rows of d's experts
+ *   below e over all sources. A row at or past recv_rows is dropped; rows not stored keep their previous bytes.
+ *   expert_counts: device [E/N] int32, rows stored per local expert: clamp(recv_rows - base_d(e), 0, total[e]).
+ *   route: device [tokens, top_k] int32, peer * recv_rows + row for a stored slot, -1 for a dropped one (what b200collExpertCombine reads).
+ *   dropped: device [1] int32, rows addressed to this rank that did not fit (saturating at 2^31 - 1).
+ * Refused with InvalidArgument before anything is launched: null pointers (x, topk_idx and route may be NULL only when tokens == 0),
+ * a dtype other than bf16, fp16 or fp32, row_elems == 0 or row_elems % 16 != 0, top_k < 1, E outside [1, 1024] or not a multiple of
+ * nranks, x or recv not 16-byte aligned, topk_idx, expert_counts, route or dropped not 4-byte aligned, recv overlapping x, an output
+ * array overlapping another, topk_idx, x or recv, tokens * top_k > 2^31 - 1, nranks * recv_rows > 2^31 - 1, more than 2^31 - 1 16-byte
+ * vectors offered (tokens * top_k * row_bytes / 16).
+ * Placement: with more than one rank, recv must be arena memory at the same offset on every rank (else InvalidUsage), and recv_rows the
+ * same on every rank; with B200COLL_CHECK=1 on multi-process communicators (E, row_elems, recv_rows, arena offset of recv) is compared
+ * across ranks. A poisoned communicator gives RemoteError.
+ * Every rank launches on every call, a rank with tokens == 0 included (its peers' barriers wait for it). One rank: no barriers, recv any
+ * device buffer, counted as copy. b200collStats count the call under alltoall, algorithm twoshot (copy with one rank), two kernel
+ * launches, and tokens * top_k * row_elems * sizeof(dtype) bytes: the slots offered, which the host knows, not the rows stored. */
+b200collResult_t b200collExpertDispatch(const void* x, void* recv, size_t row_elems, size_t recv_rows, const int32_t* topk_idx, size_t tokens,
+                                        int top_k, int num_experts, int32_t* expert_counts, int32_t* route, int32_t* dropped,
+                                        b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
+/* Expert combine from a device route: b200collAllToAllvCombine's result and rules, with each slot's (peer, row) read from the route
+ * b200collExpertDispatch wrote instead of the dispatch's host arrays. Slot j of token t reads row route % recv_rows of peer
+ * route / recv_rows's expert_out ([recv_rows, row_elems] of ep->in_dtype); a route outside [0, nranks * recv_rows) is a dropped slot, and
+ * the kernel reads nothing else whatever the device array holds. out[t] = round_once(scale * ((+0 + w0*y0) + w1*y1 + ...)) in slot order,
+ * no fused multiply-add, 9 type pairs; weights NULL gives all ones.
+ * Refused with InvalidArgument before anything is launched: null pointers (route and out may be NULL only when tokens == 0), in or out
+ * type not bf16, fp16 or fp32, row_elems == 0 or row_elems % 16 != 0, top_k < 1, expert_out or out not 16-byte aligned, route or weights
+ * not 4-byte aligned, out overlapping expert_out, route or weights, more than 2^31 - 1 16-element vectors of out, tokens * top_k > 2^31 - 1,
+ * nranks * recv_rows > 2^31 - 1. Placement, the closing barrier (the caller may overwrite expert_out right after the call), the one-rank
+ * path and RemoteError are those of b200collAllToAllvCombine. b200collStats count the call under alltoall, algorithm oneshot (copy with
+ * one rank), one kernel launch, and tokens * top_k * row_elems * sizeof(in) bytes (the slots offered). */
+b200collResult_t b200collExpertCombine(const void* expert_out, void* out, size_t row_elems, size_t recv_rows, const int32_t* route,
+                                       const float* weights, size_t tokens, int top_k, const b200collEpilogue* ep, b200collComm_t comm,
+                                       b200collStream_t stream);
 
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.

@@ -3,6 +3,8 @@
 //   k_a2av_combine_pull<InT, OutT>    barrier, pull each token's top_k expert rows from the peers' expert_out, sum in slot order in
 //                                     fp32, round once, store locally, barrier
 //   k_a2av_combine_local<InT, OutT>   one rank: the same gather and sum from a local expert_out, no barrier
+//   k_routed_combine_pull / _local    b200collExpertCombine: the same two, each slot's (peer, row) read from the device route that
+//                                     b200collExpertDispatch wrote (RouteMap) instead of the segment table
 //
 // Each rank walks (token, 16-element vector) pairs of its own out. For slot j of token t, index[t, j] is a row of the dispatch send
 // buffer; the segment table (A2AvRows, the rows of the dispatch call) maps it to (peer p, row of p's expert_out). A row in no segment
@@ -58,11 +60,25 @@ template <typename InT> __device__ __forceinline__ void combine_widen(const uint
   }
 }
 
-// Vectors [0, tokens * vpr) of out, vpr = row_elems / 16. base(p) is the address of peer p's expert_out. Consecutive threads take
-// consecutive vectors of a row, so the loads of a warp are coalesced; lanes of one token read index and weights at one address
-// (a broadcast). 32-bit indices: the host keeps tokens * vpr below 2^31, so v + stride cannot wrap.
-template <typename InT, typename OutT, typename Base>
-__device__ __forceinline__ void combine_range(const A2AvRows& g, int nranks, Base&& base, const int32_t* __restrict__ index,
+// The (peer, expert_out row) of a route written by b200collExpertDispatch (peer * recv_rows + row), or false for any value outside
+// [0, limit), limit = nranks * recv_rows <= 2^31 - 1 (the host checks it): negative values are >= 2^31 as unsigned.
+struct RouteMap {
+  uint32_t limit, recv_rows;
+  __device__ __forceinline__ bool operator()(int32_t i, int* peer, unsigned long long* row) const {
+    if ((uint32_t)i >= limit) return false;
+    const uint32_t p = (uint32_t)i / recv_rows;
+    *peer = (int)p;
+    *row = (uint32_t)i - p * recv_rows;
+    return true;
+  }
+};
+
+// Vectors [0, tokens * vpr) of out, vpr = row_elems / 16. map(index value, &peer, &row) names the expert_out row of a slot (false: a
+// dropped slot) and base(p) is the address of peer p's expert_out. Consecutive threads take consecutive vectors of a row, so the loads
+// of a warp are coalesced; lanes of one token read index and weights at one address (a broadcast). 32-bit indices: the host keeps
+// tokens * vpr below 2^31, so v + stride cannot wrap.
+template <typename InT, typename OutT, typename Map, typename Base>
+__device__ __forceinline__ void combine_range(Map&& map, Base&& base, const int32_t* __restrict__ index,
                                               const float* __restrict__ weights, OutT* __restrict__ out, uint32_t tokens, uint32_t top_k,
                                               uint32_t vpr, float scale) {
   constexpr int NW = (int)sizeof(InT);                           // 16-byte words per 16 elements: 2 (bf16, fp16) or 4 (fp32)
@@ -85,7 +101,7 @@ __device__ __forceinline__ void combine_range(const A2AvRows& g, int nranks, Bas
         w[b] = 1.0f;
         int p = 0;
         unsigned long long row = 0;
-        if (j0 + b < top_k && combine_row(g, nranks, it[j0 + b], &p, &row)) {
+        if (j0 + b < top_k && map(it[j0 + b], &p, &row)) {
           hit[b] = true;
           if (weights) w[b] = wt[j0 + b];
           const char* src = base(p) + (row * vpr + col) * (16 * sizeof(InT));
@@ -122,7 +138,8 @@ __global__ void __launch_bounds__(kCombineThreads, 1) k_a2av_combine_pull(COMM_P
     const uint32_t s = load_seq(c, kSeqBarrier);
     if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every peer's expert_out is written
   }
-  combine_range<InT, OutT>(g, c.nranks, [&](int p) -> const char* { return c.peer[p] + eo_off; }, index, weights, out, tokens, top_k, vpr, scale);
+  combine_range<InT, OutT>([&](int32_t i, int* p, unsigned long long* row) { return combine_row(g, c.nranks, i, p, row); },
+                           [&](int p) -> const char* { return c.peer[p] + eo_off; }, index, weights, out, tokens, top_k, vpr, scale);
   // the sequence number is read again rather than kept live across the loop: only the last block, after the barrier below, bumps it
   const uint32_t s = load_seq(c, kSeqBarrier);
   if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // nobody reads my expert_out any more: the caller may overwrite it
@@ -135,7 +152,33 @@ __global__ void __launch_bounds__(kCombineThreads, 1) k_a2av_combine_local(const
                                                                            OutT* __restrict__ out, uint32_t tokens, uint32_t top_k, uint32_t vpr,
                                                                            float scale) {
   pdl_prologue();
-  combine_range<InT, OutT>(g, 1, [&](int) { return expert_out; }, index, weights, out, tokens, top_k, vpr, scale);
+  combine_range<InT, OutT>([&](int32_t i, int* p, unsigned long long* row) { return combine_row(g, 1, i, p, row); },
+                           [&](int) { return expert_out; }, index, weights, out, tokens, top_k, vpr, scale);
+}
+
+// The combine of b200collExpertCombine: the same kernels with the slot's (peer, row) taken from the dispatch's device route. The
+// barriers and the grid follow k_a2av_combine_pull, for the same reasons.
+template <typename InT, typename OutT>
+__global__ void __launch_bounds__(kCombineThreads, 1) k_routed_combine_pull(COMM_PARAM, size_t eo_off, RouteMap m, const int32_t* __restrict__ route,
+                                                                            const float* __restrict__ weights, OutT* __restrict__ out, uint32_t tokens,
+                                                                            uint32_t top_k, uint32_t vpr, float scale, uint32_t op) {
+  pdl_prologue();
+  {
+    const uint32_t s = load_seq(c, kSeqBarrier);
+    if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every peer's expert_out is written
+  }
+  combine_range<InT, OutT>(m, [&](int p) -> const char* { return c.peer[p] + eo_off; }, route, weights, out, tokens, top_k, vpr, scale);
+  const uint32_t s = load_seq(c, kSeqBarrier);
+  if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // nobody reads my expert_out any more: the caller may overwrite it
+  if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
+}
+
+template <typename InT, typename OutT>
+__global__ void __launch_bounds__(kCombineThreads, 1) k_routed_combine_local(RouteMap m, const char* __restrict__ expert_out, const int32_t* __restrict__ route,
+                                                                             const float* __restrict__ weights, OutT* __restrict__ out, uint32_t tokens,
+                                                                             uint32_t top_k, uint32_t vpr, float scale) {
+  pdl_prologue();
+  combine_range<InT, OutT>(m, [&](int) { return expert_out; }, route, weights, out, tokens, top_k, vpr, scale);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -158,6 +201,43 @@ static b200collResult_t dispatch_combine(b200collDataType_t in, b200collDataType
   }
 }
 
+// The argument rules both combines share, after their null checks ("" or why the call is refused); max_rows bounds recv_rows so that
+// every byte offset fits in size_t with room to spare. `index` is the index (b200collAllToAllvCombine) or the route (b200collExpertCombine).
+static std::string combine_shape(const void* expert_out, const void* out, size_t row_elems, size_t recv_rows, const int32_t* index, const float* weights,
+                                 size_t tokens, int top_k, const b200collEpilogue* ep, const char* index_name, size_t* max_rows) {
+  if (!combine_type(ep->in_dtype) || !combine_type(ep->out_dtype)) return "in_dtype and out_dtype must be bf16, fp16 or fp32";
+  if (row_elems == 0 || row_elems % 16 != 0) return "row_elems must be a positive multiple of 16";
+  if (top_k < 1) return "top_k must be at least 1";
+  if (!aligned(expert_out, 16) || !aligned(out, 16)) return "expert_out and out must be 16-byte aligned";
+  if (!aligned(index, 4) || !aligned(weights, 4)) return std::string(index_name) + " and weights must be 4-byte aligned";
+  const size_t max_vecs = ((size_t)1 << 31) - 1;
+  if (tokens > max_vecs / (row_elems / 16)) return "at most 2^31 - 1 16-element vectors of out";
+  if (tokens > max_vecs / (size_t)top_k) return "tokens * top_k must be at most 2^31 - 1";
+  *max_rows = (SIZE_MAX >> 4) / (row_elems * b200collTypeSize(ep->in_dtype));
+  if (recv_rows > *max_rows) return "recv_rows * row_elems is too large";
+  return "";
+}
+
+// The placement rules both combines share: out overlapping expert_out, index or weights (InvalidArgument), a poisoned communicator
+// (RemoteError), a multi-rank expert_out outside the arena (InvalidUsage).
+static b200collResult_t combine_place(b200collComm* c, const void* expert_out, void* out, size_t row_elems, size_t recv_rows, const int32_t* index,
+                                      const float* weights, size_t tokens, int top_k, const b200collEpilogue* ep, const char* what, const char* index_name) {
+  const size_t is = b200collTypeSize(ep->in_dtype), os = b200collTypeSize(ep->out_dtype);
+  const size_t eo_bytes = recv_rows * row_elems * is, out_bytes = tokens * row_elems * os, idx_bytes = tokens * (size_t)top_k * 4;
+  if (overlaps(out, out_bytes, expert_out, eo_bytes) || (index && overlaps(out, out_bytes, index, idx_bytes)) ||
+      (weights && overlaps(out, out_bytes, weights, idx_bytes))) {
+    set_last_error(std::string(what) + ": out must not overlap expert_out, " + index_name + " or weights");
+    return b200collInvalidArgument;
+  }
+  if (comm_poisoned(c)) return b200collRemoteError;
+  // peers pull from my expert_out at MY arena offset: it must be arena memory
+  if (c->nranks > 1 && !b200collIsSymmetric(c, expert_out, std::max<size_t>(eo_bytes, 1))) {
+    set_last_error(std::string(what) + ": expert_out must lie in the symmetric arena (b200collMemAlloc), at the same offset on every rank");
+    return b200collInvalidUsage;
+  }
+  return b200collSuccess;
+}
+
 // Everything b200collAllToAllvCombine checks before it launches; on success `g` holds the segment table and `in_bytes` the bytes of
 // expert_out the dispatch rows cover.
 static b200collResult_t combine_prepare(b200collComm* c, const void* expert_out, void* out, size_t row_elems, size_t recv_rows, const int64_t* send_rows,
@@ -165,17 +245,10 @@ static b200collResult_t combine_prepare(b200collComm* c, const void* expert_out,
                                         size_t tokens, int top_k, const b200collEpilogue* ep, A2AvRows* g, size_t* in_bytes) {
   auto refuse = [](const std::string& msg) { set_last_error("all-to-all-v combine: " + msg); return b200collInvalidArgument; };
   if (!c || !expert_out || !ep || !send_rows || !send_row_off || !recv_row_off_at_peer || ((!index || !out) && tokens > 0)) return refuse("null argument");
-  if (!combine_type(ep->in_dtype) || !combine_type(ep->out_dtype)) return refuse("in_dtype and out_dtype must be bf16, fp16 or fp32");
-  if (row_elems == 0 || row_elems % 16 != 0) return refuse("row_elems must be a positive multiple of 16");
-  if (top_k < 1) return refuse("top_k must be at least 1");
-  if (!aligned(expert_out, 16) || !aligned(out, 16)) return refuse("expert_out and out must be 16-byte aligned");
-  if (!aligned(index, 4) || !aligned(weights, 4)) return refuse("index and weights must be 4-byte aligned");
-  const size_t max_vecs = ((size_t)1 << 31) - 1;
-  if (tokens > max_vecs / (row_elems / 16)) return refuse("at most 2^31 - 1 16-element vectors of out");
-  if (tokens > max_vecs / (size_t)top_k) return refuse("tokens * top_k must be at most 2^31 - 1");
-  const size_t is = b200collTypeSize(ep->in_dtype), os = b200collTypeSize(ep->out_dtype);
-  const size_t max_rows = (SIZE_MAX >> 4) / (row_elems * is);     // every byte offset below then fits in size_t with room to spare
-  if (recv_rows > max_rows) return refuse("recv_rows * row_elems is too large");
+  size_t max_rows = 0;
+  const std::string shape = combine_shape(expert_out, out, row_elems, recv_rows, index, weights, tokens, top_k, ep, "index", &max_rows);
+  if (!shape.empty()) return refuse(shape);
+  const size_t is = b200collTypeSize(ep->in_dtype);
   const std::string bad = a2av_rows(c->nranks, send_rows, send_row_off, recv_row_off_at_peer, recv_rows, max_rows, g);
   if (!bad.empty()) return refuse(bad);
   std::vector<std::pair<unsigned long long, unsigned long long>> ranges;     // non-empty send ranges [lo, hi)
@@ -187,17 +260,32 @@ static b200collResult_t combine_prepare(b200collComm* c, const void* expert_out,
   std::sort(ranges.begin(), ranges.end());
   for (size_t k = 1; k < ranges.size(); k++)
     if (ranges[k].first < ranges[k - 1].second) return refuse("two send ranges overlap: a dispatch row must belong to one peer");
-  const size_t eo_bytes = recv_rows * row_elems * is, out_bytes = tokens * row_elems * os, idx_bytes = tokens * (size_t)top_k * 4;
-  if (overlaps(out, out_bytes, expert_out, eo_bytes) || (index && overlaps(out, out_bytes, index, idx_bytes)) ||
-      (weights && overlaps(out, out_bytes, weights, idx_bytes)))
-    return refuse("out must not overlap expert_out, index or weights");
-  if (comm_poisoned(c)) return b200collRemoteError;
-  // peers pull from my expert_out at MY arena offset: it must be arena memory
-  if (c->nranks > 1 && !b200collIsSymmetric(c, expert_out, std::max<size_t>(eo_bytes, 1))) {
-    set_last_error("all-to-all-v combine: expert_out must lie in the symmetric arena (b200collMemAlloc), at the same offset on every rank");
-    return b200collInvalidUsage;
+  return combine_place(c, expert_out, out, row_elems, recv_rows, index, weights, tokens, top_k, ep, "all-to-all-v combine", "index");
+}
+
+// (in, out) -> one launch of k_routed_combine_pull (more than one rank) or k_routed_combine_local
+static b200collResult_t routed_combine_launch(b200collComm* c, const void* expert_out, void* out, size_t row_elems, size_t recv_rows, const int32_t* route,
+                                              const float* weights, size_t tokens, int top_k, const b200collEpilogue* ep, cudaStream_t st) {
+  const uint32_t vpr = (uint32_t)(row_elems / 16), nvec = (uint32_t)(tokens * vpr);
+  const RouteMap m{(uint32_t)(c->nranks * recv_rows), (uint32_t)recv_rows};
+  if (c->nranks == 1) {
+    const int blocks = (int)std::max<size_t>(1, std::min<size_t>(((size_t)nvec + kCombineThreads - 1) / kCombineThreads, (size_t)std::max(1, c->sm_count)));
+    return dispatch_combine(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
+      using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
+      launch_k(k_routed_combine_local<InT, OutT>, blocks, kCombineThreads, st, m, static_cast<const char*>(expert_out), route, weights, static_cast<OutT*>(out),
+               (uint32_t)tokens, (uint32_t)top_k, vpr, ep->scale);
+      LAUNCH_CHECK(c);
+      return b200collSuccess;
+    });
   }
-  return b200collSuccess;
+  const Grid gr = pick_grid(c, kShapeP2p, ~(size_t)0 >> 8, 1);     // the full P2P grid on every rank, as in b200collAllToAllvCombine
+  return dispatch_combine(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
+    using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
+    launch_k(k_routed_combine_pull<InT, OutT>, gr.blocks, gr.threads, st, c->dev, arena_off(c, expert_out), m, route, weights, static_cast<OutT*>(out),
+             (uint32_t)tokens, (uint32_t)top_k, vpr, ep->scale, (uint32_t)b200collOpAllToAll);
+    LAUNCH_CHECK(c);
+    return b200collSuccess;
+  });
 }
 
 }  // namespace b200coll
@@ -240,6 +328,29 @@ b200collResult_t b200collAllToAllvCombine(const void* expert_out, void* out, siz
     LAUNCH_CHECK(c);
     return b200collSuccess;
   });
+}
+
+b200collResult_t b200collExpertCombine(const void* expert_out, void* out, size_t row_elems, size_t recv_rows, const int32_t* route,
+                                       const float* weights, size_t tokens, int top_k, const b200collEpilogue* ep, b200collComm_t c,
+                                       b200collStream_t stream) {
+  auto refuse = [](const std::string& msg) { set_last_error("expert combine: " + msg); return b200collInvalidArgument; };
+  if (!c || !expert_out || !ep || ((!route || !out) && tokens > 0)) return refuse("null argument");
+  size_t max_rows = 0;
+  const std::string shape = combine_shape(expert_out, out, row_elems, recv_rows, route, weights, tokens, top_k, ep, "route", &max_rows);
+  if (!shape.empty()) return refuse(shape);
+  if (recv_rows > (((size_t)1 << 31) - 1) / (size_t)c->nranks) return refuse("nranks * recv_rows must be at most 2^31 - 1 (a route is an int32)");
+  b200collResult_t rc = combine_place(c, expert_out, out, row_elems, recv_rows, route, weights, tokens, top_k, ep, "expert combine", "route");
+  if (rc != b200collSuccess) return rc;
+  const size_t offered = tokens * (size_t)top_k * row_elems * b200collTypeSize(ep->in_dtype);
+  if (c->nranks == 1) {
+    account(c, b200collOpAllToAll, offered, b200collAlgoCopy);
+  } else {
+    rc = cross_check(c, b200collOpAllToAll, b200collAlgoOneShot, recv_rows, arena_off(c, expert_out), 0);
+    if (rc != b200collSuccess) return rc;
+    account(c, b200collOpAllToAll, offered, b200collAlgoOneShot);
+  }
+  const DeviceScope on_device(c->device);
+  return routed_combine_launch(c, expert_out, out, row_elems, recv_rows, route, weights, tokens, top_k, ep, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -89,6 +89,15 @@ inline Grid pick_grid(const b200collComm* c, int kind, size_t vecs, int unroll) 
   return Grid{1, 128};
 }
 
+// Makes the communicator's GPU current while it lives and restores the caller's: a process may drive communicators on several GPUs,
+// and a launch onto a stream of another device than the current one fails (after the peers' kernels are already waiting for it).
+struct DeviceScope {
+  int prev = -1;
+  bool switched = false;
+  explicit DeviceScope(int want) { if (cudaGetDevice(&prev) == cudaSuccess && prev != want) switched = cudaSetDevice(want) == cudaSuccess; }
+  ~DeviceScope() { if (switched) cudaSetDevice(prev); }
+};
+
 inline size_t arena_off(b200collComm* c, const void* p) { return reinterpret_cast<CUdeviceptr>(p) - c->peer_va[c->rank]; }
 inline bool aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) % a) == 0; }
 inline bool overlaps(const void* a, size_t na, const void* b, size_t nb) {

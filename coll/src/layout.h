@@ -36,6 +36,14 @@ constexpr size_t kP2pDoneBytes = (size_t)kMaxRanks * kP2pMaxBlocks * 4;
 static_assert(kOffP2pDone + kP2pDoneBytes <= kOffLL, "p2p mailboxes must fit below the Lamport scratch");
 constexpr int kP2pTagBits = 24, kP2pValueBits = 40;     // each post word = (chunk sequence number mod 2^24) << 40 | value
 
+// Routed expert dispatch (routed.cu): the count mailbox, int32 [source rank][kRouteMaxExperts]. Before the dispatch's exchange barrier
+// every rank writes its per-expert slot counts into row [its rank] of every rank's mailbox; after it each rank reads the whole matrix.
+constexpr int kRouteMaxExperts = 1024;
+constexpr size_t kOffRouteCounts = 512 << 10;
+constexpr size_t kRouteCountsBytes = (size_t)kMaxRanks * kRouteMaxExperts * 4;
+static_assert(kOffRouteCounts >= kOffP2pDone + kP2pDoneBytes, "the route count mailbox must lie clear of the p2p mailboxes");
+static_assert(kOffRouteCounts + kRouteCountsBytes <= kOffLL, "the route count mailbox must fit below the Lamport scratch");
+
 // local (non-symmetric) per-comm state words
 enum { kSeqBarrier = 0, kSeqLL = 1, kTicket = 2, kLLUsedLo0 = 3 /* 3,4,5 */, kLLUsedHi0 = 6 /* 6,7,8 */,
        kP2pSendSeq0 = 16 /* [peer][CTA]: chunks sent so far */, kP2pRecvSeq0 = kP2pSendSeq0 + kMaxRanks * kP2pMaxBlocks /* chunks received so far */,

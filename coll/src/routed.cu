@@ -1,0 +1,274 @@
+// libb200coll device-routed expert dispatch: the router's top-k expert ids in, rows grouped by expert out, no host sync. Two kernels
+// per call:
+//
+//   k_routed_layout   one CTA: each slot's rank among this rank's slots to the same expert, the per-expert counts, the count exchange
+//                     through the mailbox (layout.h, kOffRouteCounts) and one releasing barrier, then every slot's route
+//   k_routed_push<P>  every (slot, 16-byte vector) pair with a route is copied to its row of the owner's recv; P: over NVLink into the
+//                     peers' arenas, closing releasing barrier; !P (one rank): into a local buffer, no barrier
+//
+// Layout. The slots [0, tokens * top_k) are cut into 32 contiguous segments, one per warp of the layout CTA. A warp walks its segment
+// 32 slots at a time: __match_any_sync groups the lanes that name one expert, a lane's rank in the group is the popcount of the lower
+// lanes in it, and the group's lowest lane adds the group's size to the warp's running count of that expert in shared memory. So a slot's
+// rank is the number of earlier slots of its segment with the same expert; a prefix over the warps' counts (segment order is slot order)
+// makes it the rank among all of this rank's slots. No atomic hands out a position: the layout is the same on every run.
+//
+// Ordering argument (rank s, call k; "A" is the layout kernel's barrier, "B" the push kernel's closing barrier; both release, and CTA b
+// of every rank meets CTA b of every other rank in them):
+// - A peer's mailbox row [s] is free when s writes it in call k: the peer read its mailbox in its layout kernel of call k - 1, which
+//   ended before its push kernel of call k - 1 began, and s only starts call k after passing B of call k - 1, which waits for every peer
+//   to arrive there. Collectives between the two calls only add barriers (or none: LL takes no barrier and uses no mailbox).
+// - A peer's recv is free when s pushes into it in call k: s passed A of call k first, and a peer arrives at A only once its own stream
+//   has reached call k, so everything the peer's stream did before (an expert GEMM reading recv) is complete. That is why the push kernel
+//   takes no entry barrier: A, one kernel earlier on the same stream, already orders it. Receivers see the rows after their push kernel
+//   ends because of B (released by every sender after its stores).
+// - Sender and receiver agree on every row: both compute it from the same [nranks][E] count matrix, read after A, and the same rule.
+// - The grids cannot differ between ranks: the layout kernel is one CTA everywhere, and the push kernel is the full P2P launch shape of
+//   the communicator on every rank whatever its tokens (as in k_a2av_push), so a CTA without work only takes the barrier.
+// - Graph replay: both kernels read the epoch from the communicator's state word (load_seq) and bump it once, the counts travel in
+//   device memory, and the host passes only shapes and pointers: nothing about the epoch or the routing lives in kernel arguments.
+#include <stdint.h>
+
+#include <algorithm>
+#include <atomic>
+#include <string>
+
+#include "comm.h"
+#include "launch.cuh"
+
+namespace b200coll {
+
+constexpr int kLayoutThreads = 1024, kLayoutWarps = kLayoutThreads / 32;
+constexpr int kRoutedPushThreads = 512, kRoutedPushUnroll = 4;
+
+// Shared memory of k_routed_layout: int32 counts [warp][E], int64 bases [E], int64 warp sums [kLayoutWarps + 1].
+constexpr size_t layout_smem(int E) { return (size_t)kLayoutWarps * E * 4 + (size_t)E * 8 + (kLayoutWarps + 1) * 8; }
+
+__global__ void __launch_bounds__(kLayoutThreads, 1) k_routed_layout(COMM_PARAM, const int32_t* __restrict__ topk_idx, uint32_t slots, int E,
+                                                                     uint32_t recv_rows, int32_t* __restrict__ route, int32_t* __restrict__ expert_counts,
+                                                                     int32_t* __restrict__ dropped, uint32_t op) {
+  pdl_prologue();
+  extern __shared__ __align__(16) unsigned char smem[];
+  int* cnt = reinterpret_cast<int*>(smem);
+  long long* base = reinterpret_cast<long long*>(smem + (size_t)kLayoutWarps * E * 4);
+  long long* wsum = base + E;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const uint32_t per = (slots + kLayoutWarps - 1) / kLayoutWarps;
+  const uint32_t lo = min(slots, (uint32_t)w * per), hi = min(slots, lo + per);
+  for (int i = threadIdx.x; i < kLayoutWarps * E; i += blockDim.x) cnt[i] = 0;
+  __syncthreads();
+
+  // 1. each slot's rank within its warp's segment, kept in route until step 4
+  int* mine = cnt + w * E;
+  for (uint32_t b = lo; b < hi; b += 32) {
+    const uint32_t i = b + lane;
+    int e = -1;
+    if (i < hi) { const int32_t id = topk_idx[i]; if ((uint32_t)id < (uint32_t)E) e = id; }
+    const unsigned same = __match_any_sync(0xFFFFFFFFu, e);
+    const int lower = __popc(same & ((1u << lane) - 1u));
+    const int r = e >= 0 ? mine[e] + lower : 0;
+    __syncwarp();
+    if (e >= 0 && lower == 0) mine[e] += __popc(same);
+    __syncwarp();
+    if (i < hi) route[i] = r;
+  }
+  __syncthreads();
+
+  // 2. per expert: the exclusive prefix of the warps' counts, and this rank's count of it
+  for (int e = threadIdx.x; e < E; e += blockDim.x) {
+    int run = 0;
+    for (int v = 0; v < kLayoutWarps; v++) { const int x = cnt[v * E + e]; cnt[v * E + e] = run; run += x; }
+    base[e] = run;
+  }
+  __syncthreads();
+
+  // 3. the exchange: my counts into row [my rank] of every rank's mailbox, one releasing barrier, then the whole matrix. E <= blockDim:
+  // thread e owns expert e from here on.
+  const int e = threadIdx.x;
+  const bool exchange = c.nranks > 1;
+  const uint32_t s = load_seq(c, kSeqBarrier);
+  if (exchange) {
+    if (e < E)
+      for (int p = 0; p < c.nranks; p++) reinterpret_cast<int*>(c.peer[p] + kOffRouteCounts)[c.rank * kRouteMaxExperts + e] = (int)base[e];
+    if (!barrier_blocks<true>(c, 2 * s + 1, op)) {               // watchdog: route no row, so the push kernel moves nothing
+      for (uint32_t i = threadIdx.x; i < slots; i += blockDim.x) route[i] = -1;
+      return;
+    }
+  }
+  long long total = 0, before_me = 0;                            // rows of expert e over all ranks, and from ranks below mine
+  if (e < E) {
+    if (exchange) {
+      const uint32_t* box = reinterpret_cast<const uint32_t*>(c.peer[c.rank] + kOffRouteCounts) + e;
+      for (int q = 0; q < c.nranks; q++) {
+        const long long m = (int)ld_relaxed_sys(box + (size_t)q * kRouteMaxExperts);
+        total += m;
+        if (q < c.rank) before_me += m;
+      }
+    } else {
+      total = base[e];
+    }
+  }
+  // exclusive prefix of total over the experts: a warp scan, then the warps' sums
+  long long x = total;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) { const long long y = __shfl_up_sync(0xFFFFFFFFu, x, d); if (lane >= d) x += y; }
+  if (lane == 31) wsum[w] = x;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    long long run = 0;
+    for (int v = 0; v < kLayoutWarps; v++) { const long long t = wsum[v]; wsum[v] = run; run += t; }
+    wsum[kLayoutWarps] = 0;                                      // the dropped rows, summed below
+  }
+  __syncthreads();
+  const long long below = x - total + wsum[w];                   // rows of all experts below e
+  if (e < E) base[e] = below;
+  __syncthreads();
+  const int epr = E / c.nranks;
+  long long first = 0;                                           // base_d(e): rows of the owner's experts below e
+  if (e < E) first = below - base[e / epr * epr];
+  __syncthreads();
+  if (e < E) {
+    base[e] = first + before_me;                                 // my first row for expert e in its owner's recv
+    if (e / epr == c.rank) {
+      const long long stored = min(max((long long)recv_rows - first, 0ll), total);
+      expert_counts[e - c.rank * epr] = (int32_t)stored;
+      if (total > stored) atomicAdd(reinterpret_cast<unsigned long long*>(&wsum[kLayoutWarps]), (unsigned long long)(total - stored));
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) *dropped = (int32_t)min(wsum[kLayoutWarps], (long long)INT32_MAX);
+
+  // 4. every slot's route: its owner and row, or -1 when the id is invalid or the row falls at or past recv_rows
+  for (uint32_t i = lo + lane; i < hi; i += 32) {
+    const int32_t id = topk_idx[i];
+    int32_t r = -1;
+    if ((uint32_t)id < (uint32_t)E) {
+      const long long row = base[id] + mine[id] + route[i];
+      if (row < (long long)recv_rows) r = (int32_t)((long long)(id / epr) * recv_rows + row);
+    }
+    route[i] = r;
+  }
+  if (exchange && threadIdx.x == 0) c.state[kSeqBarrier] = s + 1;   // one CTA: every thread read s before the barrier
+}
+
+// Vectors [0, nvec) = (slot, 16-byte vector of its row), vpr vectors per row. A slot's route names (peer, row) or is outside
+// [0, nranks * recv_rows) and moves nothing. The host keeps nvec and nranks * recv_rows below 2^31, so 32-bit indices cannot wrap.
+template <bool kPeers>
+__global__ void __launch_bounds__(kRoutedPushThreads) k_routed_push(COMM_PARAM, const char* __restrict__ x, char* __restrict__ recv, size_t recv_off,
+                                                                    const int32_t* __restrict__ route, uint32_t top_k, uint32_t vpr, uint32_t nvec,
+                                                                    uint32_t recv_rows, uint32_t op) {
+  pdl_prologue();
+  constexpr int U = kRoutedPushUnroll;
+  const uint32_t limit = (uint32_t)c.nranks * recv_rows;
+  for (uint32_t b = blockIdx.x * blockDim.x * U + threadIdx.x; b < nvec; b += gridDim.x * blockDim.x * U) {
+    uint4 d[U];
+    char* dst[U];
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+      const uint32_t v = b + u * blockDim.x;
+      dst[u] = nullptr;
+      if (v < nvec) {
+        const uint32_t slot = v / vpr, col = v - slot * vpr;
+        const uint32_t r = (uint32_t)route[slot];
+        if (r < limit) {
+          const uint32_t p = r / recv_rows, row = r - p * recv_rows;
+          dst[u] = (kPeers ? c.peer[p] + recv_off : recv) + ((size_t)row * vpr + col) * 16;
+          d[u] = ld_vec(x + ((size_t)(slot / top_k) * vpr + col) * 16);
+        }
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < U; u++)
+      if (dst[u]) st_vec(dst[u], d[u]);
+  }
+  if constexpr (kPeers) {
+    const uint32_t s = load_seq(c, kSeqBarrier);
+    if (!barrier_blocks<true>(c, 2 * s + 1, op)) return;         // my rows are in every receiver's recv before its kernel ends
+    if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
+  }
+}
+
+static bool routed_type(b200collDataType_t t) { return t == b200collBfloat16 || t == b200collFloat16 || t == b200collFloat32; }
+
+}  // namespace b200coll
+
+using namespace b200coll;
+
+extern "C" {
+
+b200collResult_t b200collExpertDispatch(const void* x, void* recv, size_t row_elems, size_t recv_rows, const int32_t* topk_idx, size_t tokens,
+                                        int top_k, int num_experts, int32_t* expert_counts, int32_t* route, int32_t* dropped,
+                                        b200collDataType_t dtype, b200collComm_t c, b200collStream_t stream) {
+  auto refuse = [](const std::string& msg) { set_last_error("expert dispatch: " + msg); return b200collInvalidArgument; };
+  if (!c || !recv || !expert_counts || !dropped || ((!x || !topk_idx || !route) && tokens > 0)) return refuse("null argument");
+  if (!routed_type(dtype)) return refuse("dtype must be bf16, fp16 or fp32");
+  if (row_elems == 0 || row_elems % 16 != 0) return refuse("row_elems must be a positive multiple of 16");
+  if (top_k < 1) return refuse("top_k must be at least 1");
+  if (num_experts < 1 || num_experts > kRouteMaxExperts || num_experts % c->nranks != 0)
+    return refuse("num_experts must be in [1, 1024] and a multiple of nranks");
+  const size_t max31 = ((size_t)1 << 31) - 1;
+  if (tokens > max31 / (size_t)top_k) return refuse("tokens * top_k must be at most 2^31 - 1");
+  if (recv_rows > max31 / (size_t)c->nranks) return refuse("nranks * recv_rows must be at most 2^31 - 1 (a route is an int32)");
+  const size_t row_bytes = row_elems * b200collTypeSize(dtype), vpr = row_bytes / 16, slots = tokens * (size_t)top_k;
+  if (slots > max31 / vpr) return refuse("at most 2^31 - 1 16-byte vectors offered (tokens * top_k * row_bytes / 16)");
+  if (!aligned(x, 16) || !aligned(recv, 16)) return refuse("x and recv must be 16-byte aligned");
+  if (!aligned(topk_idx, 4) || !aligned(expert_counts, 4) || !aligned(route, 4) || !aligned(dropped, 4))
+    return refuse("topk_idx, expert_counts, route and dropped must be 4-byte aligned");
+  const size_t x_bytes = tokens * row_bytes, recv_bytes = recv_rows * row_bytes, idx_bytes = slots * 4, counts_bytes = (size_t)(num_experts / c->nranks) * 4;
+  if (x && overlaps(recv, recv_bytes, x, x_bytes)) return refuse("recv must not overlap x");
+  const struct { const void* p; size_t n; } outs[] = {{expert_counts, counts_bytes}, {route, idx_bytes}, {dropped, 4}},
+                                         others[] = {{topk_idx, idx_bytes}, {x, x_bytes}, {recv, recv_bytes}};
+  for (size_t i = 0; i < 3; i++) {
+    if (!outs[i].p) continue;
+    for (size_t j = i + 1; j < 3; j++)
+      if (outs[j].p && overlaps(outs[i].p, outs[i].n, outs[j].p, outs[j].n)) return refuse("expert_counts, route and dropped must not overlap each other");
+    for (const auto& o : others)
+      if (o.p && overlaps(outs[i].p, outs[i].n, o.p, o.n)) return refuse("expert_counts, route and dropped must not overlap topk_idx, x or recv");
+  }
+  if (comm_poisoned(c)) return b200collRemoteError;
+  const DeviceScope on_device(c->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool peers = c->nranks > 1;
+  if (peers) {
+    // peers push into my recv at MY arena offset: it must be arena memory
+    if (!b200collIsSymmetric(c, recv, std::max<size_t>(recv_bytes, 1))) {
+      set_last_error("expert dispatch: recv must lie in the symmetric arena (b200collMemAlloc), at the same offset on every rank");
+      return b200collInvalidUsage;
+    }
+    // (E, row_elems) travel as one number: E < 2048
+    const b200collResult_t rc = cross_check(c, b200collOpAllToAll, b200collAlgoTwoShot, recv_rows, arena_off(c, recv), row_elems * 2048 + (size_t)num_experts);
+    if (rc != b200collSuccess) return rc;
+  }
+  account(c, b200collOpAllToAll, slots * row_bytes, peers ? b200collAlgoTwoShot : b200collAlgoCopy);
+
+  // Once per device, before the first layout kernel: its shared-memory limit, and both push kernels loaded. With lazy module loading
+  // the first launch of a kernel loads it, and the load waits for kernels already running: a push launched for the first time behind
+  // a layout kernel that waits at its barrier for a rank driven by the same host thread would wait for a launch that never comes.
+  static std::atomic<unsigned long long> attr_done{0};          // per device, as in launch_bulk
+  const unsigned long long bit = 1ull << (c->device & 63);
+  if (!(attr_done.load(std::memory_order_acquire) & bit)) {
+    cudaFuncSetAttribute(k_routed_layout, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)layout_smem(kRouteMaxExperts));
+    cudaFuncAttributes fa;
+    cudaFuncGetAttributes(&fa, k_routed_push<true>);
+    cudaFuncGetAttributes(&fa, k_routed_push<false>);
+    attr_done.fetch_or(bit, std::memory_order_acq_rel);
+  }
+  launch_k_smem(k_routed_layout, 1, kLayoutThreads, layout_smem(num_experts), st, c->dev, topk_idx, (uint32_t)slots, num_experts, (uint32_t)recv_rows,
+                route, expert_counts, dropped, (uint32_t)b200collOpAllToAll);
+  LAUNCH_CHECK(c);
+  const uint32_t nvec = (uint32_t)(slots * vpr);
+  if (peers) {
+    // the full P2P grid on every rank, whatever its tokens: CTA b meets CTA b of every peer in the closing barrier
+    const Grid gr = pick_grid(c, kShapeP2p, ~(size_t)0 >> 8, kRoutedPushUnroll);
+    launch_k(k_routed_push<true>, gr.blocks, gr.threads, st, c->dev, static_cast<const char*>(x), static_cast<char*>(nullptr), arena_off(c, recv), route,
+             (uint32_t)top_k, (uint32_t)vpr, nvec, (uint32_t)recv_rows, (uint32_t)b200collOpAllToAll);
+  } else {
+    const size_t per_cta = (size_t)kRoutedPushThreads * kRoutedPushUnroll;
+    const int blocks = (int)std::max<size_t>(1, std::min<size_t>((nvec + per_cta - 1) / per_cta, (size_t)4 * std::max(1, c->sm_count)));
+    launch_k(k_routed_push<false>, blocks, kRoutedPushThreads, st, c->dev, static_cast<const char*>(x), static_cast<char*>(recv), (size_t)0, route,
+             (uint32_t)top_k, (uint32_t)vpr, nvec, (uint32_t)recv_rows, (uint32_t)b200collOpAllToAll);
+  }
+  LAUNCH_CHECK(c);
+  return b200collSuccess;
+}
+
+}  // extern "C"

@@ -56,6 +56,7 @@ struct Opts {
   int q_block = 0;                // --quantize WIRE:BLOCK: quantising collectives (0 = off)
   b200collDataType_t q_wire = b200collFloat8e4m3;
   int combine_k = 0;              // --combine K: the expert combine with top_k = K (0 = off)
+  int route_e = 0, route_k = 0;   // --route E:K: the device-routed dispatch and combine, E experts, top-K (0 = off)
 };
 
 // Block-scaled mode: each rank's send buffer is a [rows, row_len] FP8 matrix with one fp32 scale per bs_rows x bs_cols block. Scales are
@@ -300,6 +301,165 @@ static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out,
   return total_errors ? 1 : 0;
 }
 
+// Routed mode (--route E:K). Per size, every rank holds tokens = size / row bytes tokens of x (k_fill values) and routes slot (t, j) to
+// expert h(rank, t, j) % E, or drops it (id -1) every 61st slot; the hash is seeded, so every rank can draw every rank's ids on the host.
+// recv holds tokens * K rows on every rank, the mean load, so some receivers clip and some do not. -c 1 repeats the layout on the host
+// (per-expert counts, then each slot's row) and checks every byte of recv (stored rows, and the 0x5A poison elsewhere), every count,
+// every route and dropped; then the combine (recv as the expert output, seeded weights) bit for bit against the slot-order reference.
+static int32_t ro_id(int rank, size_t t, int j, int E) {
+  const uint32_t h = co_hash((uint32_t)(t * 0x9E3779B1u) ^ (uint32_t)(rank * 0x85EBCA77u) ^ (uint32_t)(j * 0xC2B2AE3Du));
+  return h % 61 == 7 ? -1 : (int32_t)(h % (uint32_t)E);
+}
+static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1) {
+  const int n = ctx.nranks, rank = ctx.rank, E = o.route_e, K = o.route_k, epr = E / n;
+  const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt), row = o.row_len;
+  const b200collEpilogue ep{o.in_dt, o.out_dt, o.scale};
+  void* recv = nullptr;
+  CC(b200collMemAlloc(ctx.comm, &recv, o.max_bytes * K + 4096));     // tokens * K rows at the largest size, the same on every rank
+  int32_t* small = nullptr;
+  RT(cudaMalloc(&small, (size_t)(epr + 1) * 4));
+  int32_t *d_counts = small, *d_dropped = small + epr;
+  int gen_ctr[4] = {0, 0, 0, 0};
+  long total_errors = 0;
+  if (rank == 0) {
+    printf("# b200coll_perf op=alltoall routed dispatch + combine experts=%d top_k=%d nranks=%d in=%s out=%s scale=%g row_len=%zu: size = x bytes per rank\n", E, K,
+           n, dt_name(o.in_dt), dt_name(o.out_dt), o.scale, row);
+    printf("#%13s %12s %6s %8s | %12s %12s %6s\n", "size(B)", "tokens", "type", "algo", "dispatch us", "combine us", "#wrong");
+    fflush(stdout);
+  }
+  for (size_t bytes = o.min_bytes; bytes <= o.max_bytes; bytes *= o.factor) {
+    const size_t tokens = bytes / is / row, slots = tokens * K, recv_rows = slots;
+    if (tokens == 0) continue;
+    // every rank's ids, counts and layout on the host
+    std::vector<std::vector<int32_t>> ids(n, std::vector<int32_t>(slots));
+    std::vector<std::vector<long long>> cnt(n, std::vector<long long>(E, 0));
+    for (int s = 0; s < n; s++)
+      for (size_t i = 0; i < slots; i++) { const int32_t e = ro_id(s, i / K, (int)(i % K), E); ids[s][i] = e; if (e >= 0) cnt[s][e]++; }
+    std::vector<long long> total(E, 0), below(E, 0), base(E, 0);
+    for (int e = 0; e < E; e++) for (int s = 0; s < n; s++) total[e] += cnt[s][e];
+    for (int e = 1; e < E; e++) below[e] = below[e - 1] + total[e - 1];
+    for (int e = 0; e < E; e++) base[e] = below[e] - below[e / epr * epr];
+    // the row of every slot of every rank (-1: invalid id or past recv_rows)
+    std::vector<std::vector<long long>> rowof(n, std::vector<long long>(slots, -1));
+    for (int s = 0; s < n; s++) {
+      std::vector<long long> seen(E, 0);
+      for (size_t i = 0; i < slots; i++) {
+        const int32_t e = ids[s][i];
+        if (e < 0) continue;
+        long long r = base[e] + seen[e]++;
+        for (int q = 0; q < s; q++) r += cnt[q][e];
+        if (r < (long long)recv_rows) rowof[s][i] = r;
+      }
+    }
+    std::vector<float> w(slots);
+    for (size_t i = 0; i < slots; i++) w[i] = 0.25f + (float)(co_hash((uint32_t)i * 31u + (uint32_t)rank) & 0xFFFFFF) * 0x1p-24f;
+    int32_t *d_idx = nullptr, *d_route = nullptr; float* d_w = nullptr; void* out = nullptr;
+    RT(cudaMalloc(&d_idx, slots * 4)); RT(cudaMalloc(&d_route, slots * 4)); RT(cudaMalloc(&d_w, slots * 4)); RT(cudaMalloc(&out, tokens * row * os));
+    RT(cudaMemcpy(d_idx, ids[rank].data(), slots * 4, cudaMemcpyHostToDevice));
+    RT(cudaMemcpy(d_w, w.data(), slots * 4, cudaMemcpyHostToDevice));
+    fill(x, tokens * row, o.in_dt, rank, 0, st);
+    RT(cudaMemsetAsync(recv, 0x5A, recv_rows * row * is, st));
+    auto dispatch = [&] {
+      CC(b200collExpertDispatch(x, recv, row, recv_rows, d_idx, tokens, K, E, d_counts, d_route, d_dropped, o.in_dt, ctx.comm, st));
+    };
+    auto combine = [&] { CC(b200collExpertCombine(recv, out, row, recv_rows, d_route, d_w, tokens, K, &ep, ctx.comm, st)); };
+    long errs = 0;
+    auto bad = [&](const char* what, size_t a, long long got, long long want) {
+      if (errs < 4) fprintf(stderr, "rank %d route size %zu %s %zu: got %lld want %lld\n", rank, bytes, what, a, got, want);
+      errs++;
+    };
+    if (o.check) {
+      RT(cudaStreamSynchronize(st));
+      spin_barrier(sh, 0, n, &gen_ctr[0]);
+      dispatch();
+      combine();
+      RT(cudaStreamSynchronize(st));
+      spin_barrier(sh, 1, n, &gen_ctr[1]);
+      std::vector<unsigned char> h_recv(recv_rows * row * is);
+      std::vector<int32_t> h_route(slots), h_small(epr + 1);
+      std::vector<char> h_out(tokens * row * os);
+      RT(cudaMemcpy(h_recv.data(), recv, h_recv.size(), cudaMemcpyDeviceToHost));
+      RT(cudaMemcpy(h_route.data(), d_route, slots * 4, cudaMemcpyDeviceToHost));
+      RT(cudaMemcpy(h_small.data(), small, h_small.size() * 4, cudaMemcpyDeviceToHost));
+      RT(cudaMemcpy(h_out.data(), out, h_out.size(), cudaMemcpyDeviceToHost));
+      // recv: which (source, token) each of my rows holds
+      std::vector<long long> src(recv_rows, -1);
+      for (int s = 0; s < n; s++)
+        for (size_t i = 0; i < slots; i++)
+          if (rowof[s][i] >= 0 && ids[s][i] / epr == rank) src[rowof[s][i]] = (long long)s * tokens + (long long)(i / K);
+      for (size_t r = 0; r < recv_rows; r++) {
+        for (size_t e = 0; e < row; e++) {
+          const size_t at = r * row + e;
+          long long got = 0, want = 0;
+          memcpy(&got, h_recv.data() + at * is, is);
+          if (src[r] < 0) { want = is == 4 ? 0x5A5A5A5All : 0x5A5All; }
+          else want = out_bits(gen((int)(src[r] / (long long)tokens), (size_t)(src[r] % (long long)tokens) * row + e), o.in_dt);
+          if (got != want) bad("recv element", at, got, want);
+        }
+      }
+      long long dropped = 0;
+      for (int e = rank * epr; e < (rank + 1) * epr; e++) {
+        const long long stored = std::min(std::max((long long)recv_rows - base[e], 0ll), total[e]);
+        dropped += total[e] - stored;
+        if (h_small[e - rank * epr] != stored) bad("expert_counts", (size_t)e, h_small[e - rank * epr], stored);
+      }
+      if (h_small[epr] != dropped) bad("dropped", 0, h_small[epr], dropped);
+      for (size_t i = 0; i < slots; i++) {
+        const long long want = rowof[rank][i] < 0 ? -1 : (long long)(ids[rank][i] / epr) * (long long)recv_rows + rowof[rank][i];
+        if (h_route[i] != want) bad("route", i, h_route[i], want);
+      }
+      // the combine of identity experts: every stored slot of token t brings back t's own row
+      for (size_t t = 0; t < tokens; t++) {
+        for (size_t e = 0; e < row; e++) {
+          float acc = 0.0f;
+          for (int j = 0; j < K; j++) {
+            if (rowof[rank][t * K + j] < 0) continue;
+            volatile float prod = w[t * K + j] * gen(rank, t * row + e);
+            acc = acc + prod;
+          }
+          const uint32_t want = out_bits(acc * o.scale, o.out_dt), got = got_bits(h_out.data(), t * row + e, o.out_dt);
+          if (got != want) bad("combine element", t * row + e, got, want);
+        }
+      }
+    }
+    float ms[2] = {0, 0};
+    for (int phase = 0; phase < 2; phase++) {
+      for (int i = 0; i < o.warmup; i++) { if (phase == 0) dispatch(); else combine(); }
+      RT(cudaStreamSynchronize(st));
+      spin_barrier(sh, 2, n, &gen_ctr[2]);
+      RT(cudaEventRecord(e0, st));
+      for (int i = 0; i < o.iters; i++) { if (phase == 0) dispatch(); else combine(); }
+      RT(cudaEventRecord(e1, st));
+      RT(cudaEventSynchronize(e1));
+      RT(cudaEventElapsedTime(&ms[phase], e0, e1));
+      ms[phase] /= o.iters;
+    }
+    float worst[2] = {0, 0};
+    long es = 0;
+    for (int phase = 0; phase < 2; phase++) {
+      sh->ms[rank] = ms[phase]; sh->errors[rank] = errs;
+      spin_barrier(sh, 3, n, &gen_ctr[3]);
+      for (int r = 0; r < n; r++) { worst[phase] = std::max(worst[phase], sh->ms[r]); if (phase == 0) es += sh->errors[r]; }
+      spin_barrier(sh, 0, n, &gen_ctr[0]);   // keep ms[] stable until everyone has read it
+    }
+    total_errors += es;
+    b200collFault f;
+    if (b200collCommGetAsyncError(ctx.comm, &f) != b200collSuccess) { fprintf(stderr, "rank %d WATCHDOG code=%u peer=%u block=%u expected=%u observed=%u\n", rank, f.code, f.peer, f.block, f.expected, f.observed); _exit(5); }
+    if (rank == 0) {
+      printf("%14zu %12zu %6s %8s | %12.2f %12.2f %6ld\n", tokens * row * is, tokens, dt_name(o.in_dt), n > 1 ? "twoshot" : "copy", worst[0] * 1e3, worst[1] * 1e3, es);
+      fflush(stdout);
+    }
+    RT(cudaFree(d_idx)); RT(cudaFree(d_route)); RT(cudaFree(d_w)); RT(cudaFree(out));
+  }
+  RT(cudaFree(small));
+  b200collStats s; CC(b200collCommStatsGet(ctx.comm, &s));
+  if (rank == 0) {
+    printf("# launches=%llu errors=%ld\n", (unsigned long long)s.kernel_launches, total_errors);
+    fflush(stdout);
+  }
+  return total_errors ? 1 : 0;
+}
+
 // expected value of output element e (element index in the op's output) for this rank
 static float expected(const Opts& o, int rank, int n, size_t e, size_t count) {
   if (o.op == "all_reduce" || o.op == "reduce") { float s = 0; for (int r = 0; r < n; r++) s += gen(r, e); return s * o.scale; }
@@ -344,6 +504,15 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
       return 2;
     }
     return run_combine(o, ctx, sh, send, recv, st, e0, e1);
+  }
+  if (o.route_e) {
+    const auto wide = [](b200collDataType_t t) { return t == b200collBfloat16 || t == b200collFloat16 || t == b200collFloat32; };
+    if (o.op != "alltoall" || o.q_block || o.bs_rows || o.row_len == 0 || o.row_len % 16 || !wide(o.in_dt) || !wide(o.out_dt) || o.route_e % n != 0) {
+      fprintf(stderr, "--route E:K takes --op alltoall, -d and --out-dtype bfloat16|half|float, a --row-len that is a multiple of 16, E a multiple of the\n"
+                      "number of ranks, and no --quantize, --block-scale or --combine\n");
+      return 2;
+    }
+    return run_route(o, ctx, sh, send, st, e0, e1);
   }
   const bool bs_mode = o.bs_rows > 0, q_mode = o.q_block > 0, is_a2a = o.op == "alltoall";
   const bool wide_in = o.in_dt == b200collBfloat16 || o.in_dt == b200collFloat16 || o.in_dt == b200collFloat32;
@@ -660,6 +829,9 @@ int main(int argc, char** argv) {
       o.q_wire = parse_dt(wire);
     }
     else if (a == "--combine") { o.combine_k = atoi(next()); if (o.combine_k < 1) { fprintf(stderr, "--combine K: K >= 1\n"); return 1; } }
+    else if (a == "--route") {
+      if (sscanf(next(), "%d:%d", &o.route_e, &o.route_k) != 2 || o.route_e < 1 || o.route_e > 1024 || o.route_k < 1) { fprintf(stderr, "--route E:K: 1 <= E <= 1024, K >= 1\n"); return 1; }
+    }
     else if (a == "--scale") o.scale = (float)atof(next());
     else if (a == "--algo") o.algo = next();
     else if (a == "--iters" || a == "-n") o.iters = atoi(next());
@@ -702,6 +874,11 @@ int main(int argc, char** argv) {
            "                            an even split of whole rows, each token takes K slots from K different ranges where there are enough (seeded\n"
            "                            routing and weights); size = expert_out bytes read per rank; -c 1 checks every output element bit for bit\n"
            "                            against the slot-order host reference\n"
+           "  --route E:K               --op alltoall: the device-routed expert dispatch and its combine, E experts (a multiple of the ranks, at most\n"
+           "                            1024) sharded over the ranks, seeded top-K expert ids per token on the device, -d bfloat16|half|float rows,\n"
+           "                            --out-dtype the combine's out type, recv sized to the mean load (tokens * K rows); size = x bytes per rank;\n"
+           "                            reports the dispatch (layout, count exchange and push) and the combine; -c 1 checks every received byte,\n"
+           "                            count, route and dropped, and the combine bit for bit, against the host layout\n"
            "  --algo auto|ll|ll2|oneshot|twoshot|nvls   --inplace 0|1|2   --max-ctas N   --sweep kind:ctas:threads,...   --json FILE   --window SIZE\n"
            "  --selfcheck               report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;
@@ -728,7 +905,8 @@ int main(int argc, char** argv) {
     o.nranks = lr.size; o.procs = true;
     b200collConfig cfg; b200collConfigDefault(&cfg);
     const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
-    if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o);
+    if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o) +
+                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0);     // --route: recv holds K rows per token
     b200collUniqueId id; CC(b200collUniqueIdFromString(("perf/" + lr.job).c_str(), &id));
     RT(cudaSetDevice(dev));
     b200collComm_t comm;
@@ -756,7 +934,8 @@ int main(int argc, char** argv) {
   b200collConfig cfg; b200collConfigDefault(&cfg);
   // arena: two windows (+ max buffers) and slack
   const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
-  size_t need = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o);
+  size_t need = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o) +
+                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0);     // --route: recv holds K rows per token
   if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = need;
   if (o.procs) {
     b200collUniqueId id; CC(b200collGetUniqueId(&id));

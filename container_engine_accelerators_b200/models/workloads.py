@@ -24,6 +24,9 @@ class DispatchPlan:
     # with rows / send_off / recv_off they are the arguments of Comm.all_to_all_v_combine().
     index: list = field(default_factory=list)
     weights: list = field(default_factory=list)
+    # experts[s]: [tokens, top_k] int32, the expert each (token, slot) of rank s is routed to (experts [d * experts_per_rank, + experts_per_rank)
+    # live on rank d): the topk_idx argument of Comm.expert_dispatch(), from the same draw as rows and index.
+    experts: list = field(default_factory=list)
 
     def bytes_sent(self, rank: int, itemsize: int = 2) -> int:
         return int(self.rows[rank].sum()) * self.hidden * itemsize
@@ -35,9 +38,10 @@ def expert_dispatch_plan(nranks: int, tokens_per_rank: int, hidden: int, experts
     pop = 1.0 / np.arange(1, n_experts + 1) ** skew if skew > 0 else np.ones(n_experts)
     pop = rng.permutation(pop / pop.sum())
     rows = np.zeros((nranks, nranks), dtype=np.int64)
-    dests = []
+    dests, experts = [], []
     for s in range(nranks):
         choice = rng.choice(n_experts, size=(tokens_per_rank, top_k), p=pop)
+        experts.append(choice.astype(np.int32))
         dest = choice // experts_per_rank
         dests.append(dest)
         rows[s] = np.bincount(dest.ravel(), minlength=nranks)
@@ -58,7 +62,7 @@ def expert_dispatch_plan(nranks: int, tokens_per_rank: int, hidden: int, experts
     recv_off = np.zeros_like(rows)                       # recv_off[d, s]
     recv_off[:, 1:] = np.cumsum(rows.T, axis=1)[:, :-1]
     max_rows = int(max(rows.sum(axis=1).max(), rows.sum(axis=0).max()))
-    return DispatchPlan(nranks, hidden, rows, send_off, recv_off, max_rows, index, weights)
+    return DispatchPlan(nranks, hidden, rows, send_off, recv_off, max_rows, index, weights, experts)
 
 
 def uniform_plan(nranks: int, rows_per_peer: int, hidden: int) -> DispatchPlan:

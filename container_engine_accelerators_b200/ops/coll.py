@@ -139,6 +139,9 @@ def load() -> C.CDLL:
     L.b200collAllToAllvQuantized.argtypes = [vp, vp, C.POINTER(C.c_float), sz, sz, i64p, i64p, i64p, ci, ci, ci, vp, vp]
     L.b200collAllToAllvCombine.argtypes = [vp, vp, sz, sz, i64p, i64p, i64p, C.POINTER(C.c_int32), C.POINTER(C.c_float), sz, ci,
                                            C.POINTER(Epilogue), vp, vp]
+    i32p = C.POINTER(C.c_int32)
+    L.b200collExpertDispatch.argtypes = [vp, vp, sz, sz, i32p, sz, ci, ci, i32p, i32p, i32p, ci, vp, vp]
+    L.b200collExpertCombine.argtypes = [vp, vp, sz, sz, i32p, C.POINTER(C.c_float), sz, ci, C.POINTER(Epilogue), vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -375,6 +378,94 @@ def check_all_to_all_v_combine(nranks: int, expert_out, out, row_elems: int, sen
             continue
         b, nb = t.data_ptr(), t.numel() * t.element_size()
         if na and nb and a < b + nb and b < a + na:
+            raise ValueError(f"out must not overlap {name}")
+    return torch_dtype_code(expert_out.dtype), torch_dtype_code(out.dtype)
+
+
+MAX_EXPERTS = 1024
+_I31 = 2 ** 31 - 1
+
+
+def _numel(shape) -> int:
+    n = 1
+    for d in shape:
+        n *= d
+    return n
+
+
+def _overlap(t, u) -> bool:
+    a, na = t.data_ptr(), t.numel() * t.element_size()
+    b, nb = u.data_ptr(), u.numel() * u.element_size()
+    return bool(na and nb and a < b + nb and b < a + na)
+
+
+def check_expert_dispatch(nranks: int, x, topk_idx, num_experts: int, recv, expert_counts=None, route=None, dropped=None) -> int:
+    """Rules of the device-routed expert dispatch, checked on the tensors' metadata only (no communicator, no library call, no device
+    read): raises ValueError, returns the library code of x's type. x: contiguous bfloat16, float16 or float32 [tokens, row_elems] with
+    row_elems a positive multiple of 16; topk_idx: contiguous int32 [tokens, top_k], top_k >= 1; num_experts in [1, MAX_EXPERTS] and a
+    multiple of nranks; recv: contiguous, x's dtype, a whole number of rows; expert_counts (num_experts // nranks), route (tokens, top_k)
+    and dropped (1 element): contiguous int32 when given. tokens * top_k, nranks * recv rows and tokens * top_k * row bytes / 16 are at
+    most 2^31 - 1. recv must not overlap x, and no output may overlap another output, topk_idx, x or recv."""
+    import torch
+    if x.dtype not in (torch.bfloat16, torch.float16, torch.float32) or x.dim() != 2 or not x.is_contiguous():
+        raise ValueError(f"x must be a contiguous bfloat16, float16 or float32 [tokens, row_elems] tensor, got {x.dtype}{list(x.shape)}")
+    tokens, row_elems = x.shape
+    if row_elems <= 0 or row_elems % 16:
+        raise ValueError(f"row_elems (x.shape[1] = {row_elems}) must be a positive multiple of 16")
+    if topk_idx.dtype != torch.int32 or topk_idx.dim() != 2 or not topk_idx.is_contiguous() or topk_idx.shape[1] < 1:
+        raise ValueError(f"topk_idx must be a contiguous int32 [tokens, top_k] tensor with top_k >= 1, got {topk_idx.dtype}{list(topk_idx.shape)}")
+    if topk_idx.shape[0] != tokens:
+        raise ValueError(f"topk_idx has {topk_idx.shape[0]} tokens, x has {tokens}")
+    top_k = topk_idx.shape[1]
+    if isinstance(num_experts, bool) or not isinstance(num_experts, int) or not 1 <= num_experts <= MAX_EXPERTS or num_experts % nranks:
+        raise ValueError(f"num_experts must be an int in [1, {MAX_EXPERTS}] and a multiple of nranks ({nranks}), got {num_experts!r}")
+    if recv.dtype != x.dtype or not recv.is_contiguous() or recv.numel() % row_elems:
+        raise ValueError(f"recv must be a contiguous {x.dtype} tensor of whole {row_elems}-element rows, got {recv.dtype} with {recv.numel()} elements")
+    if tokens * top_k > _I31:
+        raise ValueError(f"tokens * top_k ({tokens * top_k}) must be at most 2^31 - 1")
+    if nranks * (recv.numel() // row_elems) > _I31:
+        raise ValueError("nranks * recv rows must be at most 2^31 - 1 (a route is an int32)")
+    if tokens * top_k * (row_elems * x.element_size() // 16) > _I31:
+        raise ValueError("at most 2^31 - 1 16-byte vectors may be offered (tokens * top_k * row bytes / 16)")
+    if _overlap(recv, x):
+        raise ValueError("recv must not overlap x")
+    outs = [(n, t, shape) for n, t, shape in (("expert_counts", expert_counts, (num_experts // nranks,)), ("route", route, (tokens, top_k)),
+                                              ("dropped", dropped, (1,))) if t is not None]
+    for name, t, shape in outs:
+        if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != _numel(shape):
+            raise ValueError(f"{name} must be a contiguous int32 tensor of shape {shape}, got {t.dtype}{list(t.shape)}")
+    for k, (name, t, _) in enumerate(outs):
+        for other, u in [(n, o) for n, o, _ in outs[k + 1:]] + [("topk_idx", topk_idx), ("x", x), ("recv", recv)]:
+            if _overlap(t, u):
+                raise ValueError(f"{name} must not overlap {other}")
+    return torch_dtype_code(x.dtype)
+
+
+def check_expert_combine(nranks: int, expert_out, route, weights, out) -> tuple[int, int]:
+    """Rules of the expert combine from a device route, checked on the tensors' metadata only: raises ValueError, returns the library
+    codes of (expert_out's type, out's type). out: contiguous bfloat16, float16 or float32 [tokens, row_elems], row_elems a positive
+    multiple of 16; expert_out: contiguous bfloat16, float16 or float32 of whole rows; route: contiguous int32 [tokens, top_k], top_k >= 1;
+    weights: None or contiguous float32 of route's shape. nranks * expert_out rows is at most 2^31 - 1. out must not overlap expert_out,
+    route or weights."""
+    import torch
+    wide = (torch.bfloat16, torch.float16, torch.float32)
+    if out.dtype not in wide or out.dim() != 2 or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous bfloat16, float16 or float32 [tokens, row_elems] tensor, got {out.dtype}{list(out.shape)}")
+    tokens, row_elems = out.shape
+    if row_elems <= 0 or row_elems % 16:
+        raise ValueError(f"row_elems (out.shape[1] = {row_elems}) must be a positive multiple of 16")
+    if expert_out.dtype not in wide or not expert_out.is_contiguous() or expert_out.numel() % row_elems:
+        raise ValueError(f"expert_out must be a contiguous bfloat16, float16 or float32 tensor of whole {row_elems}-element rows, got {expert_out.dtype}")
+    if route.dtype != torch.int32 or route.dim() != 2 or not route.is_contiguous() or route.shape[1] < 1 or route.shape[0] != tokens:
+        raise ValueError(f"route must be a contiguous int32 [{tokens}, top_k] tensor with top_k >= 1, got {route.dtype}{list(route.shape)}")
+    if weights is not None and (weights.dtype != torch.float32 or weights.shape != route.shape or not weights.is_contiguous()):
+        raise ValueError(f"weights must be None or a contiguous float32 {list(route.shape)} tensor, got {weights.dtype}{list(weights.shape)}")
+    if tokens * route.shape[1] > _I31:
+        raise ValueError("tokens * top_k must be at most 2^31 - 1")
+    if nranks * (expert_out.numel() // row_elems) > _I31:
+        raise ValueError("nranks * expert_out rows must be at most 2^31 - 1 (a route is an int32)")
+    for name, t in (("expert_out", expert_out), ("route", route), ("weights", weights)):
+        if t is not None and _overlap(out, t):
             raise ValueError(f"out must not overlap {name}")
     return torch_dtype_code(expert_out.dtype), torch_dtype_code(out.dtype)
 
@@ -704,6 +795,47 @@ class Comm:
                                                arr(send_rows), arr(send_row_off), arr(recv_row_off_at_peer),
                                                C.cast(C.c_void_p(index.data_ptr()), C.POINTER(C.c_int32)), w, tokens, top_k, C.byref(ep),
                                                self._h, self._stream(stream)), "AllToAllvCombine")
+        return out
+
+    def expert_dispatch(self, x, topk_idx, num_experts: int, recv, expert_counts=None, route=None, dropped=None, stream=None):
+        """Device-routed expert dispatch (b200collExpertDispatch): slot (t, j) sends row t of x ([tokens, row_elems] bf16, fp16 or fp32)
+        to expert topk_idx[t, j] (int32 on the device; an id outside [0, num_experts) drops the slot). Rank d owns experts
+        [d * E / N, (d + 1) * E / N); its recv holds them in ascending order, each expert's rows by source rank, then in (token, slot)
+        order, and rows past recv's end are dropped. Returns (recv, expert_counts [E / N] int32: rows stored per local expert,
+        route [tokens, top_k] int32: peer * recv_rows + row or -1, dropped [1] int32: rows for this rank that did not fit). The small
+        outputs are allocated on the call's stream when not given. Nothing is read back to the host. A program that drives several ranks
+        from one thread (virtual ranks sharing a GPU) passes them, allocated before the first rank's call: an allocation between two
+        ranks' calls can wait for the device (a cache flush frees memory, and freeing synchronises), while the earlier rank's layout
+        kernel waits at its barrier for the next rank's call. With more than one rank, recv
+        must be an arena tensor (`empty()`) of the same size on every rank; every rank calls, a rank with no tokens included."""
+        import torch
+        code = check_expert_dispatch(self.nranks, x, topk_idx, num_experts, recv, expert_counts, route, dropped)
+        tokens, row_elems = x.shape
+        top_k = topk_idx.shape[1]
+        if expert_counts is None or route is None or dropped is None:
+            with torch.cuda.device(x.device), torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream(x.device)):
+                expert_counts = torch.empty(num_experts // self.nranks, dtype=torch.int32, device=x.device) if expert_counts is None else expert_counts
+                route = torch.empty(tokens, top_k, dtype=torch.int32, device=x.device) if route is None else route
+                dropped = torch.empty(1, dtype=torch.int32, device=x.device) if dropped is None else dropped
+            check_expert_dispatch(self.nranks, x, topk_idx, num_experts, recv, expert_counts, route, dropped)
+        i32 = lambda t: C.cast(C.c_void_p(t.data_ptr()), C.POINTER(C.c_int32))
+        _check(load().b200collExpertDispatch(C.c_void_p(x.data_ptr()), C.c_void_p(recv.data_ptr()), row_elems, recv.numel() // row_elems, i32(topk_idx),
+                                             tokens, top_k, num_experts, i32(expert_counts), i32(route), i32(dropped), code, self._h,
+                                             self._stream(stream)), "ExpertDispatch")
+        return recv, expert_counts, route, dropped
+
+    def expert_combine(self, expert_out, route, weights, out, scale: float = 1.0, stream=None):
+        """Expert combine from the dispatch's device route (b200collExpertCombine): out[t] ([tokens, row_elems]) = round(scale * sum
+        over slots in slot order of weights[t, j] * row route[t, j] % recv_rows of peer route[t, j] // recv_rows's expert_out); a route
+        outside [0, nranks * recv_rows) is a dropped slot, weights None means all ones. Returns out. With more than one rank, expert_out
+        must be an arena tensor (`empty()`) of the same size on every rank; every rank calls."""
+        ic, oc = check_expert_combine(self.nranks, expert_out, route, weights, out)
+        tokens, row_elems = out.shape
+        ep = Epilogue(ic, oc, float(scale))
+        w = C.cast(C.c_void_p(weights.data_ptr() if weights is not None else None), C.POINTER(C.c_float))
+        _check(load().b200collExpertCombine(C.c_void_p(expert_out.data_ptr()), C.c_void_p(out.data_ptr()), row_elems, expert_out.numel() // row_elems,
+                                            C.cast(C.c_void_p(route.data_ptr()), C.POINTER(C.c_int32)), w, tokens, route.shape[1], C.byref(ep),
+                                            self._h, self._stream(stream)), "ExpertCombine")
         return out
 
     def broadcast(self, src, dst=None, root: int = 0, scale: float = 1.0, stream=None):
