@@ -14,6 +14,9 @@ Then the same routing from the router's device-side expert ids: (g) expert_dispa
 and (h) expert_combine over its route, against (i) what a caller writes today to reach all_to_all_v from device ids: a device bincount,
 a .cpu(), an all-gather of the counts, the offsets on the host, an argsort permute of the rows, then all_to_all_v. routed_matches says
 nothing was dropped, the counts add up to the plan's rows, and the routed combine equals the slot-order fp32 sum bit for bit.
+Then (j) expert_dispatch_quantized, the same routing with e4m3 rows and 1x128 block scales on the wire, into recv8 / recv_scales;
+routed_fp8_matches says its counts, route and dropped equal the bf16 routed dispatch's and every stored row, dequantised, lies within
+amax * 2^-4 of its source token's row (amax of the element's block: half an e4m3 ulp at the block's largest value).
 Bus bandwidth = (bytes a rank sends off-chip, max over ranks) / time. Rank 0 prints one JSON line per shape."""
 from __future__ import annotations
 
@@ -101,6 +104,23 @@ def main() -> int:
         us_routed = timed(lambda: comm.expert_dispatch(x, topk, n_exp, rrecv, counts, route, dropped))
         us_routed_comb = timed(lambda: comm.expert_combine(rrecv.view(-1, hidden), route, gate, out))
         comm.check_async_error()
+        # the same routing with FP8 on the wire; x is the same on every rank (send is filled the same way everywhere), so a stored row
+        # only needs its source token, which the gathered routes give
+        q8, s8 = recv8[:q_rows * hidden], recv_scales[:q_rows * hidden // 128]
+        c8, r8, d8 = torch.empty_like(counts), torch.empty_like(route), torch.empty_like(dropped)
+        us_routed_fp8 = timed(lambda: comm.expert_dispatch_quantized(x, topk, n_exp, q8, s8, 128, c8, r8, d8))
+        comm.check_async_error()
+        routes = torch.empty(world, *route.shape, dtype=route.dtype, device="cuda")
+        dist.all_gather_into_tensor(routes, r8)
+        mine = (routes >= rank * q_rows) & (routes < (rank + 1) * q_rows)
+        rows_at = (routes[mine] - rank * q_rows).long()
+        src_tok = torch.nonzero(mine)[:, 1]                                # slot (s, t, j) -> token t
+        deq = q8.view(q_rows, -1, 128).float() * s8.view(q_rows, -1, 1)
+        ref = x[src_tok].float().view(len(src_tok), -1, 128)
+        amax = ref.abs().amax(dim=-1, keepdim=True)
+        # e4m3 keeps 3 mantissa bits: half an ulp is at most 2^-4 of the value; the slack covers the fp32 roundings of x * inv and q * s
+        fp8_ok = (torch.equal(c8, counts) and torch.equal(r8, route) and torch.equal(d8, dropped)
+                  and bool(((deq[rows_at] - ref).abs() <= amax * (2.0 ** -4 + 2.0 ** -20)).all()))
         # recv holds every rank's rows (plan.max_rows >= any rank's load): nothing dropped, this rank's counts add up to the rows the
         # plan sends it, every slot routed, and the combine of the returned rows is the slot-order sum of each token's own row
         xr = x.float()
@@ -124,7 +144,8 @@ def main() -> int:
             comm.all_to_all_v(permuted, recv, hidden, h_rows, h_so, h_ro)
         us_host_plan = timed(host_plan)
         offchip = max(int(plan.rows[s].sum() - plan.rows[s, s]) for s in range(world)) * hidden * 2
-        oks = torch.tensor([1.0 if ok else 0.0, 1.0 if comb_ok else 0.0, 1.0 if routed_ok else 0.0], device="cuda"); dist.all_reduce(oks, op=dist.ReduceOp.MIN)
+        oks = torch.tensor([1.0 if ok else 0.0, 1.0 if comb_ok else 0.0, 1.0 if routed_ok else 0.0, 1.0 if fp8_ok else 0.0], device="cuda")
+        dist.all_reduce(oks, op=dist.ReduceOp.MIN)
         if rank == 0:
             print(json.dumps({"bench": "alltoallv_perf", "n_gpus": world, "tokens_per_rank": tokens, "hidden": hidden, "skew": skew, "top_k": 2,
                               "max_offchip_bytes_per_rank": offchip, "imbalance_max_over_mean": round(float(plan.rows.sum(axis=0).max() / plan.rows.sum(axis=0).mean()), 3),
@@ -134,7 +155,8 @@ def main() -> int:
                               "ours_block_fp8_us": round(us_bsq, 2), "ours_combine_us": round(us_comb, 2), "nccl_combine_us": round(us_nccl_comb, 2),
                               "combine_matches": bool(oks[1].item() == 1.0), "ours_routed_us": round(us_routed, 2),
                               "ours_routed_combine_us": round(us_routed_comb, 2), "host_plan_us": round(us_host_plan, 2),
-                              "routed_matches": bool(oks[2].item() == 1.0)}), flush=True)
+                              "routed_matches": bool(oks[2].item() == 1.0), "ours_routed_fp8_us": round(us_routed_fp8, 2),
+                              "routed_fp8_matches": bool(oks[3].item() == 1.0)}), flush=True)
     comm.destroy()
     dist.destroy_process_group()
     return 0

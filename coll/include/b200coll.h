@@ -387,6 +387,33 @@ b200collResult_t b200collAllToAllvCombine(const void* expert_out, void* out, siz
 b200collResult_t b200collExpertDispatch(const void* x, void* recv, size_t row_elems, size_t recv_rows, const int32_t* topk_idx, size_t tokens,
                                         int top_k, int num_experts, int32_t* expert_counts, int32_t* route, int32_t* dropped,
                                         b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
+/* Device-routed expert dispatch with FP8 on the wire: b200collExpertDispatch's layout, b200collAllToAllvQuantized's rows. Two kernels per
+ * call, the same layout kernel, then a push that quantises every token's row once and stores the FP8 row and its block scales to every
+ * stored slot of the token: row_elems * (1 + 4 / block) bytes per row cross NVLink instead of row_elems * sizeof(in_dtype). No host sync,
+ * so the call can be captured in a CUDA graph.
+ *   Layout: exactly b200collExpertDispatch's for the same arguments: expert ownership, the row of every slot, expert_counts, route,
+ *   dropped and the capacity rule (rows at or past recv_rows are dropped) are the same, bit for bit.
+ *   x: [tokens, row_elems] of in_dtype (bf16, fp16 or fp32), any 16-byte aligned device buffer.
+ *   recv: [recv_rows, row_elems] of wire_dtype (e4m3 or e5m2). Row r holds the quantisation of its source token's row, by the rule of
+ *   b200collAllToAllvQuantized (amax the largest bit pattern of |x| per block of `block` elements; inv and s IEEE divisions, inv = s = 1
+ *   when amax == 0 or inv is +inf; q = satfinite RNE(x * inv)). recv_scales: [recv_rows, row_elems / block] fp32, row r's scales (the
+ *   block_rows = 1, block_cols = block layout of b200collBlockScale). Every stored slot of one token gets the same bytes and scales; rows
+ *   not stored keep their previous bytes in both buffers. block: 16, 32, 64, 128, 256 or 512, dividing row_elems.
+ * Refused with InvalidArgument before anything is launched: everything b200collExpertDispatch refuses, and in_dtype other than bf16,
+ * fp16 or fp32, wire_dtype other than e4m3 or e5m2, a block not in the list, row_elems % block != 0, recv_scales NULL or not 4-byte
+ * aligned, any overlap among x, recv and recv_scales, an output array overlapping recv_scales, more than 2^31 - 1 16-element vectors
+ * of x (tokens * row_elems / 16).
+ * Placement: with more than one rank, recv and recv_scales must be arena memory at the same offsets on every rank (else InvalidUsage), and
+ * recv_rows the same on every rank; with B200COLL_CHECK=1 on multi-process communicators, recv_rows, both arena offsets and (E, row_elems,
+ * block, wire_dtype) are compared across ranks. A poisoned communicator gives RemoteError.
+ * Every rank launches on every call, a rank with tokens == 0 included. One rank: no barriers, recv and recv_scales any device buffers,
+ * counted as copy. b200collStats count the call under alltoall, algorithm twoshot (copy with one rank), two kernel launches, and
+ * tokens * top_k * row_elems * sizeof(in_dtype) bytes. */
+b200collResult_t b200collExpertDispatchQuantized(const void* x, void* recv, float* recv_scales, size_t row_elems, size_t recv_rows,
+                                                 const int32_t* topk_idx, size_t tokens, int top_k, int num_experts,
+                                                 int32_t* expert_counts, int32_t* route, int32_t* dropped,
+                                                 b200collDataType_t in_dtype, b200collDataType_t wire_dtype, int block,
+                                                 b200collComm_t comm, b200collStream_t stream);
 /* Expert combine from a device route: b200collAllToAllvCombine's result and rules, with each slot's (peer, row) read from the route
  * b200collExpertDispatch wrote instead of the dispatch's host arrays. Slot j of token t reads row route % recv_rows of peer
  * route / recv_rows's expert_out ([recv_rows, row_elems] of ep->in_dtype); a route outside [0, nranks * recv_rows) is a dropped slot, and

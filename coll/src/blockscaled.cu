@@ -25,6 +25,11 @@
 //   k_a2av_quant_push<InT, WireT>   barrier, quantise my rows for every peer and push FP8 and scales into its recv, barrier (releases)
 //   k_a2av_quant_copy<InT, WireT>   one rank: a local quantising copy, no barrier
 //
+// Routed FP8 dispatch (the push half of b200collExpertDispatchQuantized; its layout kernel lives in routed.cu):
+//
+//   k_expert_quant_push<InT, WireT, P>   quantise each token's row once, store FP8 and scales to every routed row of the owners' recv;
+//                                        P: closing barrier (releases), !P (one rank): local, no barrier
+//
 // Scales: a 16-byte FP8 vector lies in exactly one block (row_len and block_cols are multiples of 16; a quantising block is a whole
 // number of vectors), so a vector needs one scale per rank. Lanes of a warp hold consecutive vectors and usually share scales (8 lanes
 // per 1x128 block, whole warps per 128x128 block): __match_any_sync groups the lanes by scale index, the lowest lane of each group loads
@@ -398,6 +403,46 @@ __global__ void __launch_bounds__(kBsqThreads) k_a2av_quant_copy(const __grid_co
   quant_range<InT, WireT>(g, in, q, scales, 0, g.nvec);
 }
 
+// Routed FP8 dispatch (b200collExpertDispatchQuantized; routed.cu launches k_routed_layout before it on the same stream). Vectors
+// [0, nvec) of x are (token, 16-element vector of its row), vpr vectors per row. Each is loaded, widened and quantised once, then stored
+// to every stored slot of its token: the FP8 vector to row `row` of the owner's recv, and the block's scale, by the block's lowest lane,
+// to the same row of the owner's recv_scales. A route outside [0, nranks * recv_rows) stores nothing, so a token's slots all get the
+// same bytes and scales. quant_vec's butterfly sees exactly one block's lanes: a row is whole blocks, a token's first vector t * vpr is a
+// multiple of the vectors per block, and a block is a power of two of at most 32 vectors; so with warp_walk's 32-aligned warps a block's
+// lanes are one aligned lane group of one warp, all active or all idle (and, being one token's, they read the same routes).
+// kPeers: stores into the owners' arenas at q_off / s_off. No entry barrier: layout barrier A, one kernel earlier on this stream, already
+// freed every peer's recv and recv_scales (the ordering argument in routed.cu, as for k_routed_push); one closing releasing barrier.
+// !kPeers (one rank): stores into recv and scales, no barrier.
+template <typename InT, typename WireT, bool kPeers>
+__global__ void __launch_bounds__(kBsqThreads) k_expert_quant_push(COMM_PARAM, const char* __restrict__ x, char* __restrict__ recv, char* __restrict__ scales,
+                                                                   size_t q_off, size_t s_off, const int32_t* __restrict__ route, uint32_t top_k,
+                                                                   uint32_t vpr, uint32_t nvec, uint32_t recv_rows, uint32_t lvpb, uint32_t op) {
+  pdl_prologue();
+  const uint32_t lane = threadIdx.x & 31, gl = 1u << lvpb, limit = (uint32_t)c.nranks * recv_rows;
+  warp_walk(0, nvec, [&](uint32_t v, bool act) {
+    float xv[16] = {};
+    if (act) quant_load16<InT>(x + (size_t)v * (16 * sizeof(InT)), xv);
+    float sc;
+    const uint4 w = quant_vec<WireT>(xv, gl, &sc);
+    if (act) {
+      const uint32_t t = v / vpr, col = v - t * vpr;
+      for (uint32_t j = 0; j < top_k; j++) {
+        const uint32_t r = (uint32_t)route[(size_t)t * top_k + j];
+        if (r >= limit) continue;
+        const uint32_t p = r / recv_rows, row = r - p * recv_rows;
+        const size_t d = (size_t)row * vpr + col;                   // FP8 vector d of the owner's recv; its scale is element d >> lvpb
+        st_vec((kPeers ? c.peer[p] + q_off : recv) + d * 16, w);
+        if ((lane & (gl - 1)) == 0) *reinterpret_cast<float*>((kPeers ? c.peer[p] + s_off : scales) + (d >> lvpb) * 4) = sc;
+      }
+    }
+  });
+  if constexpr (kPeers) {
+    const uint32_t s = load_seq(c, kSeqBarrier);
+    if (!barrier_blocks<true>(c, 2 * s + 1, op)) return;         // my rows and scales are in every owner's buffers before its kernel ends
+    if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 // (wire, out) -> f(Tag<WireT>, Tag<OutT>); the argument checks have refused every other type
 template <typename F>
@@ -680,6 +725,41 @@ static b200collResult_t a2aq_prepare(b200collComm* c, const void* send, void* re
     return b200collInvalidUsage;
   }
   return b200collSuccess;
+}
+
+// ---- routed FP8 dispatch: the push after the layout kernel (routed.cu checks the arguments and launches the layout first)
+void load_expert_quant_push() {
+  cudaFuncAttributes fa;
+  for (b200collDataType_t in : {b200collBfloat16, b200collFloat16, b200collFloat32})
+    for (b200collDataType_t wire : {b200collFloat8e4m3, b200collFloat8e5m2})
+      dispatch_in_wire(in, wire, [&](auto ti, auto tw) -> b200collResult_t {
+        using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type;
+        cudaFuncGetAttributes(&fa, k_expert_quant_push<InT, WireT, true>);
+        cudaFuncGetAttributes(&fa, k_expert_quant_push<InT, WireT, false>);
+        return b200collSuccess;
+      });
+}
+
+b200collResult_t launch_expert_quant_push(b200collComm* c, const void* x, void* recv, float* recv_scales, const int32_t* route, size_t tokens, int top_k,
+                                          size_t row_elems, size_t recv_rows, b200collDataType_t in_dtype, b200collDataType_t wire, int block, cudaStream_t st) {
+  uint32_t lvpb = 0;
+  while ((16u << lvpb) < (uint32_t)block) lvpb++;
+  const uint32_t vpr = (uint32_t)(row_elems / 16), nvec = (uint32_t)(tokens * vpr);
+  const char* in = static_cast<const char*>(x);
+  return dispatch_in_wire(in_dtype, wire, [&](auto ti, auto tw) -> b200collResult_t {
+    using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type;
+    if (c->nranks > 1) {
+      // the full P2P grid on every rank, whatever its tokens: CTA b meets CTA b of every peer in the closing barrier
+      const Grid gr = warp_grid(c, ~(size_t)0 >> 8);
+      launch_k(k_expert_quant_push<InT, WireT, true>, gr.blocks, gr.threads, st, c->dev, in, static_cast<char*>(nullptr), static_cast<char*>(nullptr),
+               arena_off(c, recv), arena_off(c, recv_scales), route, (uint32_t)top_k, vpr, nvec, (uint32_t)recv_rows, lvpb, (uint32_t)b200collOpAllToAll);
+    } else {
+      launch_k(k_expert_quant_push<InT, WireT, false>, copy_blocks(c, nvec), 256, st, c->dev, in, static_cast<char*>(recv), reinterpret_cast<char*>(recv_scales),
+               (size_t)0, (size_t)0, route, (uint32_t)top_k, vpr, nvec, (uint32_t)recv_rows, lvpb, (uint32_t)b200collOpAllToAll);
+    }
+    LAUNCH_CHECK(c);
+    return b200collSuccess;
+  });
 }
 
 }  // namespace b200coll

@@ -6,6 +6,11 @@
 //   k_routed_push<P>  every (slot, 16-byte vector) pair with a route is copied to its row of the owner's recv; P: over NVLink into the
 //                     peers' arenas, closing releasing barrier; !P (one rank): into a local buffer, no barrier
 //
+// b200collExpertDispatchQuantized runs the same layout kernel, then k_expert_quant_push<InT, WireT, P> (in blockscaled.cu, beside the
+// quantise helpers it shares) in place of k_routed_push: it walks (token, 16-element vector) pairs of x, quantises each vector once and
+// stores the FP8 vector and its block scale to every routed row of the owners' recv and recv_scales, with the same barriers as
+// k_routed_push. The ordering argument below covers it word for word, with "recv" read as "recv and recv_scales".
+//
 // Layout. The slots [0, tokens * top_k) are cut into 32 contiguous segments, one per warp of the layout CTA. A warp walks its segment
 // 32 slots at a time: __match_any_sync groups the lanes that name one expert, a lane's rank in the group is the popcount of the lower
 // lanes in it, and the group's lowest lane adds the group's size to the warp's running count of that expert in shared memory. So a slot's
@@ -189,6 +194,99 @@ __global__ void __launch_bounds__(kRoutedPushThreads) k_routed_push(COMM_PARAM, 
 
 static bool routed_type(b200collDataType_t t) { return t == b200collBfloat16 || t == b200collFloat16 || t == b200collFloat32; }
 
+// What the FP8 dispatch adds to the bf16 one: the scales buffer, the wire type and the quantising block.
+struct RoutedQuant {
+  float* recv_scales;
+  b200collDataType_t wire;
+  int block;
+};
+
+// The argument and placement rules of both routed dispatches (q == nullptr: b200collExpertDispatch, whose messages and codes these are).
+// InvalidArgument before anything else, then RemoteError for a poisoned communicator, then InvalidUsage for buffers outside the arena
+// and the B200COLL_CHECK=1 cross-check. Host only: nothing is launched.
+static b200collResult_t routed_prepare(b200collComm* c, const void* x, const void* recv, size_t row_elems, size_t recv_rows, const int32_t* topk_idx,
+                                       size_t tokens, int top_k, int num_experts, const int32_t* expert_counts, const int32_t* route,
+                                       const int32_t* dropped, b200collDataType_t dtype, const RoutedQuant* q) {
+  const std::string who = q ? "quantised expert dispatch: " : "expert dispatch: ";
+  auto refuse = [&](const std::string& msg) { set_last_error(who + msg); return b200collInvalidArgument; };
+  if (!c || !recv || !expert_counts || !dropped || (q && !q->recv_scales) || ((!x || !topk_idx || !route) && tokens > 0)) return refuse("null argument");
+  if (!routed_type(dtype)) return refuse(q ? "in_dtype must be bf16, fp16 or fp32" : "dtype must be bf16, fp16 or fp32");
+  if (q && q->wire != b200collFloat8e4m3 && q->wire != b200collFloat8e5m2) return refuse("wire_dtype must be e4m3 or e5m2");
+  if (q && (q->block < 16 || q->block > 512 || (q->block & (q->block - 1)) != 0)) return refuse("block must be 16, 32, 64, 128, 256 or 512");
+  if (q ? row_elems == 0 || row_elems % (size_t)q->block != 0 : row_elems == 0 || row_elems % 16 != 0)
+    return refuse(q ? "row_elems must be a positive multiple of block" : "row_elems must be a positive multiple of 16");
+  if (top_k < 1) return refuse("top_k must be at least 1");
+  if (num_experts < 1 || num_experts > kRouteMaxExperts || num_experts % c->nranks != 0)
+    return refuse("num_experts must be in [1, 1024] and a multiple of nranks");
+  const size_t max31 = ((size_t)1 << 31) - 1;
+  if (tokens > max31 / (size_t)top_k) return refuse("tokens * top_k must be at most 2^31 - 1");
+  if (recv_rows > max31 / (size_t)c->nranks) return refuse("nranks * recv_rows must be at most 2^31 - 1 (a route is an int32)");
+  // the FP8 push walks (token, 16-element vector) pairs of x with 32-bit indices
+  if (q && tokens > max31 / (row_elems / 16)) return refuse("at most 2^31 - 1 16-element vectors of x (tokens * row_elems / 16)");
+  const size_t row_bytes = row_elems * b200collTypeSize(dtype), vpr = row_bytes / 16, slots = tokens * (size_t)top_k;
+  if (slots > max31 / vpr) return refuse("at most 2^31 - 1 16-byte vectors offered (tokens * top_k * row_bytes / 16)");
+  if (!aligned(x, 16) || !aligned(recv, 16)) return refuse("x and recv must be 16-byte aligned");
+  if (q && !aligned(q->recv_scales, 4)) return refuse("recv_scales must be 4-byte aligned");
+  if (!aligned(topk_idx, 4) || !aligned(expert_counts, 4) || !aligned(route, 4) || !aligned(dropped, 4))
+    return refuse("topk_idx, expert_counts, route and dropped must be 4-byte aligned");
+  // recv holds FP8 rows in the quantised call
+  const size_t x_bytes = tokens * row_bytes, recv_bytes = recv_rows * (q ? row_elems : row_bytes), idx_bytes = slots * 4,
+               counts_bytes = (size_t)(num_experts / c->nranks) * 4, scale_bytes = q ? recv_rows * (row_elems / (size_t)q->block) * 4 : 0;
+  if (x && overlaps(recv, recv_bytes, x, x_bytes)) return refuse("recv must not overlap x");
+  if (q && x && overlaps(q->recv_scales, scale_bytes, x, x_bytes)) return refuse("recv_scales must not overlap x");
+  if (q && overlaps(q->recv_scales, scale_bytes, recv, recv_bytes)) return refuse("recv and recv_scales must not overlap");
+  const struct { const void* p; size_t n; } outs[] = {{expert_counts, counts_bytes}, {route, idx_bytes}, {dropped, 4}},
+                                         others[] = {{topk_idx, idx_bytes}, {x, x_bytes}, {recv, recv_bytes}, {q ? q->recv_scales : nullptr, scale_bytes}};
+  for (size_t i = 0; i < 3; i++) {
+    if (!outs[i].p) continue;
+    for (size_t j = i + 1; j < 3; j++)
+      if (outs[j].p && overlaps(outs[i].p, outs[i].n, outs[j].p, outs[j].n)) return refuse("expert_counts, route and dropped must not overlap each other");
+    for (const auto& o : others)
+      if (o.p && overlaps(outs[i].p, outs[i].n, o.p, o.n))
+        return refuse(q ? "expert_counts, route and dropped must not overlap topk_idx, x, recv or recv_scales"
+                        : "expert_counts, route and dropped must not overlap topk_idx, x or recv");
+  }
+  if (comm_poisoned(c)) return b200collRemoteError;
+  if (c->nranks == 1) return b200collSuccess;
+  // peers push into my recv (and recv_scales) at MY arena offsets: they must be arena memory
+  if (!b200collIsSymmetric(c, recv, std::max<size_t>(recv_bytes, 1)) || (q && !b200collIsSymmetric(c, q->recv_scales, std::max<size_t>(scale_bytes, 1)))) {
+    set_last_error(q ? "quantised expert dispatch: recv and recv_scales must lie in the symmetric arena (b200collMemAlloc), at the same offsets on every rank"
+                     : "expert dispatch: recv must lie in the symmetric arena (b200collMemAlloc), at the same offset on every rank");
+    return b200collInvalidUsage;
+  }
+  // (E, row_elems) travel as one number: E < 2048
+  if (!q) return cross_check(c, b200collOpAllToAll, b200collAlgoTwoShot, recv_rows, arena_off(c, recv), row_elems * 2048 + (size_t)num_experts);
+  // the FP8 call has one more offset, so two exchanges: (recv_rows, both offsets), then (row_elems, E, block and wire)
+  const b200collResult_t rc = cross_check(c, b200collOpAllToAll, b200collAlgoTwoShot, recv_rows, arena_off(c, recv), arena_off(c, q->recv_scales));
+  if (rc != b200collSuccess) return rc;
+  return cross_check(c, b200collOpAllToAll, b200collAlgoTwoShot, row_elems, (size_t)num_experts, (size_t)q->block * 2 + (q->wire == b200collFloat8e5m2));
+}
+
+// Once per device, before the first layout kernel of either dispatch: its shared-memory limit, and every push kernel that can follow it
+// loaded. With lazy module loading the first launch of a kernel loads it, and the load waits for kernels already running: a push
+// launched for the first time behind a layout kernel that waits at its barrier for a rank driven by the same host thread would wait for
+// a launch that never comes. Whichever dispatch runs first on a device loads the other's push kernels too.
+static void routed_preload(const b200collComm* c) {
+  static std::atomic<unsigned long long> attr_done{0};          // per device, as in launch_bulk
+  const unsigned long long bit = 1ull << (c->device & 63);
+  if (attr_done.load(std::memory_order_acquire) & bit) return;
+  cudaFuncSetAttribute(k_routed_layout, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)layout_smem(kRouteMaxExperts));
+  cudaFuncAttributes fa;
+  cudaFuncGetAttributes(&fa, k_routed_push<true>);
+  cudaFuncGetAttributes(&fa, k_routed_push<false>);
+  load_expert_quant_push();
+  attr_done.fetch_or(bit, std::memory_order_acq_rel);
+}
+
+static b200collResult_t launch_layout(b200collComm* c, const int32_t* topk_idx, size_t slots, int num_experts, size_t recv_rows, int32_t* route,
+                                      int32_t* expert_counts, int32_t* dropped, cudaStream_t st) {
+  routed_preload(c);
+  launch_k_smem(k_routed_layout, 1, kLayoutThreads, layout_smem(num_experts), st, c->dev, topk_idx, (uint32_t)slots, num_experts, (uint32_t)recv_rows,
+                route, expert_counts, dropped, (uint32_t)b200collOpAllToAll);
+  LAUNCH_CHECK(c);
+  return b200collSuccess;
+}
+
 }  // namespace b200coll
 
 using namespace b200coll;
@@ -198,63 +296,14 @@ extern "C" {
 b200collResult_t b200collExpertDispatch(const void* x, void* recv, size_t row_elems, size_t recv_rows, const int32_t* topk_idx, size_t tokens,
                                         int top_k, int num_experts, int32_t* expert_counts, int32_t* route, int32_t* dropped,
                                         b200collDataType_t dtype, b200collComm_t c, b200collStream_t stream) {
-  auto refuse = [](const std::string& msg) { set_last_error("expert dispatch: " + msg); return b200collInvalidArgument; };
-  if (!c || !recv || !expert_counts || !dropped || ((!x || !topk_idx || !route) && tokens > 0)) return refuse("null argument");
-  if (!routed_type(dtype)) return refuse("dtype must be bf16, fp16 or fp32");
-  if (row_elems == 0 || row_elems % 16 != 0) return refuse("row_elems must be a positive multiple of 16");
-  if (top_k < 1) return refuse("top_k must be at least 1");
-  if (num_experts < 1 || num_experts > kRouteMaxExperts || num_experts % c->nranks != 0)
-    return refuse("num_experts must be in [1, 1024] and a multiple of nranks");
-  const size_t max31 = ((size_t)1 << 31) - 1;
-  if (tokens > max31 / (size_t)top_k) return refuse("tokens * top_k must be at most 2^31 - 1");
-  if (recv_rows > max31 / (size_t)c->nranks) return refuse("nranks * recv_rows must be at most 2^31 - 1 (a route is an int32)");
-  const size_t row_bytes = row_elems * b200collTypeSize(dtype), vpr = row_bytes / 16, slots = tokens * (size_t)top_k;
-  if (slots > max31 / vpr) return refuse("at most 2^31 - 1 16-byte vectors offered (tokens * top_k * row_bytes / 16)");
-  if (!aligned(x, 16) || !aligned(recv, 16)) return refuse("x and recv must be 16-byte aligned");
-  if (!aligned(topk_idx, 4) || !aligned(expert_counts, 4) || !aligned(route, 4) || !aligned(dropped, 4))
-    return refuse("topk_idx, expert_counts, route and dropped must be 4-byte aligned");
-  const size_t x_bytes = tokens * row_bytes, recv_bytes = recv_rows * row_bytes, idx_bytes = slots * 4, counts_bytes = (size_t)(num_experts / c->nranks) * 4;
-  if (x && overlaps(recv, recv_bytes, x, x_bytes)) return refuse("recv must not overlap x");
-  const struct { const void* p; size_t n; } outs[] = {{expert_counts, counts_bytes}, {route, idx_bytes}, {dropped, 4}},
-                                         others[] = {{topk_idx, idx_bytes}, {x, x_bytes}, {recv, recv_bytes}};
-  for (size_t i = 0; i < 3; i++) {
-    if (!outs[i].p) continue;
-    for (size_t j = i + 1; j < 3; j++)
-      if (outs[j].p && overlaps(outs[i].p, outs[i].n, outs[j].p, outs[j].n)) return refuse("expert_counts, route and dropped must not overlap each other");
-    for (const auto& o : others)
-      if (o.p && overlaps(outs[i].p, outs[i].n, o.p, o.n)) return refuse("expert_counts, route and dropped must not overlap topk_idx, x or recv");
-  }
-  if (comm_poisoned(c)) return b200collRemoteError;
+  b200collResult_t rc = routed_prepare(c, x, recv, row_elems, recv_rows, topk_idx, tokens, top_k, num_experts, expert_counts, route, dropped, dtype, nullptr);
+  if (rc != b200collSuccess) return rc;
   const DeviceScope on_device(c->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool peers = c->nranks > 1;
-  if (peers) {
-    // peers push into my recv at MY arena offset: it must be arena memory
-    if (!b200collIsSymmetric(c, recv, std::max<size_t>(recv_bytes, 1))) {
-      set_last_error("expert dispatch: recv must lie in the symmetric arena (b200collMemAlloc), at the same offset on every rank");
-      return b200collInvalidUsage;
-    }
-    // (E, row_elems) travel as one number: E < 2048
-    const b200collResult_t rc = cross_check(c, b200collOpAllToAll, b200collAlgoTwoShot, recv_rows, arena_off(c, recv), row_elems * 2048 + (size_t)num_experts);
-    if (rc != b200collSuccess) return rc;
-  }
+  const size_t row_bytes = row_elems * b200collTypeSize(dtype), vpr = row_bytes / 16, slots = tokens * (size_t)top_k;
   account(c, b200collOpAllToAll, slots * row_bytes, peers ? b200collAlgoTwoShot : b200collAlgoCopy);
-
-  // Once per device, before the first layout kernel: its shared-memory limit, and both push kernels loaded. With lazy module loading
-  // the first launch of a kernel loads it, and the load waits for kernels already running: a push launched for the first time behind
-  // a layout kernel that waits at its barrier for a rank driven by the same host thread would wait for a launch that never comes.
-  static std::atomic<unsigned long long> attr_done{0};          // per device, as in launch_bulk
-  const unsigned long long bit = 1ull << (c->device & 63);
-  if (!(attr_done.load(std::memory_order_acquire) & bit)) {
-    cudaFuncSetAttribute(k_routed_layout, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)layout_smem(kRouteMaxExperts));
-    cudaFuncAttributes fa;
-    cudaFuncGetAttributes(&fa, k_routed_push<true>);
-    cudaFuncGetAttributes(&fa, k_routed_push<false>);
-    attr_done.fetch_or(bit, std::memory_order_acq_rel);
-  }
-  launch_k_smem(k_routed_layout, 1, kLayoutThreads, layout_smem(num_experts), st, c->dev, topk_idx, (uint32_t)slots, num_experts, (uint32_t)recv_rows,
-                route, expert_counts, dropped, (uint32_t)b200collOpAllToAll);
-  LAUNCH_CHECK(c);
+  if ((rc = launch_layout(c, topk_idx, slots, num_experts, recv_rows, route, expert_counts, dropped, st)) != b200collSuccess) return rc;
   const uint32_t nvec = (uint32_t)(slots * vpr);
   if (peers) {
     // the full P2P grid on every rank, whatever its tokens: CTA b meets CTA b of every peer in the closing barrier
@@ -269,6 +318,22 @@ b200collResult_t b200collExpertDispatch(const void* x, void* recv, size_t row_el
   }
   LAUNCH_CHECK(c);
   return b200collSuccess;
+}
+
+b200collResult_t b200collExpertDispatchQuantized(const void* x, void* recv, float* recv_scales, size_t row_elems, size_t recv_rows,
+                                                 const int32_t* topk_idx, size_t tokens, int top_k, int num_experts,
+                                                 int32_t* expert_counts, int32_t* route, int32_t* dropped,
+                                                 b200collDataType_t in_dtype, b200collDataType_t wire_dtype, int block,
+                                                 b200collComm_t c, b200collStream_t stream) {
+  const RoutedQuant q{recv_scales, wire_dtype, block};
+  b200collResult_t rc = routed_prepare(c, x, recv, row_elems, recv_rows, topk_idx, tokens, top_k, num_experts, expert_counts, route, dropped, in_dtype, &q);
+  if (rc != b200collSuccess) return rc;
+  const DeviceScope on_device(c->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t slots = tokens * (size_t)top_k;
+  account(c, b200collOpAllToAll, slots * row_elems * b200collTypeSize(in_dtype), c->nranks > 1 ? b200collAlgoTwoShot : b200collAlgoCopy);
+  if ((rc = launch_layout(c, topk_idx, slots, num_experts, recv_rows, route, expert_counts, dropped, st)) != b200collSuccess) return rc;
+  return launch_expert_quant_push(c, x, recv, recv_scales, route, tokens, top_k, row_elems, recv_rows, in_dtype, wire_dtype, block, st);
 }
 
 }  // extern "C"

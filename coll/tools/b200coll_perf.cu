@@ -306,24 +306,38 @@ static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out,
 // recv holds tokens * K rows on every rank, the mean load, so some receivers clip and some do not. -c 1 repeats the layout on the host
 // (per-expert counts, then each slot's row) and checks every byte of recv (stored rows, and the 0x5A poison elsewhere), every count,
 // every route and dropped; then the combine (recv as the expert output, seeded weights) bit for bit against the slot-order reference.
+// With --quantize WIRE:BLOCK it runs the FP8 routed dispatch instead: x holds the quantising mode's values (k_fill_q), recv FP8 rows
+// and recv_scales one fp32 scale per block; -c 1 checks every FP8 byte and scale against the host quantiser (q_code) and the 0x5A
+// poison of rows not stored in both, besides counts, routes and dropped. The combine needs a wide expert_out, so only the dispatch is timed.
+static size_t route_scale_bytes(const Opts& o) {
+  return o.route_e && o.q_block ? o.max_bytes / b200collTypeSize(o.in_dt) * o.route_k / o.q_block * 4 + 4096 : 0;
+}
 static int32_t ro_id(int rank, size_t t, int j, int E) {
   const uint32_t h = co_hash((uint32_t)(t * 0x9E3779B1u) ^ (uint32_t)(rank * 0x85EBCA77u) ^ (uint32_t)(j * 0xC2B2AE3Du));
   return h % 61 == 7 ? -1 : (int32_t)(h % (uint32_t)E);
 }
 static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1) {
   const int n = ctx.nranks, rank = ctx.rank, E = o.route_e, K = o.route_k, epr = E / n;
-  const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt), row = o.row_len;
+  const bool quant = o.q_block > 0;
+  const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt), row = o.row_len, rs = quant ? 1 : is;   // rs: bytes of a recv element
   const b200collEpilogue ep{o.in_dt, o.out_dt, o.scale};
   void* recv = nullptr;
   CC(b200collMemAlloc(ctx.comm, &recv, o.max_bytes * K + 4096));     // tokens * K rows at the largest size, the same on every rank
+  float* recv_scales = nullptr;
+  if (quant) CC(b200collMemAlloc(ctx.comm, (void**)&recv_scales, route_scale_bytes(o)));
   int32_t* small = nullptr;
   RT(cudaMalloc(&small, (size_t)(epr + 1) * 4));
   int32_t *d_counts = small, *d_dropped = small + epr;
   int gen_ctr[4] = {0, 0, 0, 0};
   long total_errors = 0;
-  if (rank == 0) {
+  if (rank == 0 && quant) {
+    printf("# b200coll_perf op=alltoall routed FP8 dispatch experts=%d top_k=%d nranks=%d in=%s wire=%s block=%d row_len=%zu: size = x bytes per rank; combine not run\n",
+           E, K, n, dt_name(o.in_dt), dt_name(o.q_wire), o.q_block, row);
+  } else if (rank == 0) {
     printf("# b200coll_perf op=alltoall routed dispatch + combine experts=%d top_k=%d nranks=%d in=%s out=%s scale=%g row_len=%zu: size = x bytes per rank\n", E, K,
            n, dt_name(o.in_dt), dt_name(o.out_dt), o.scale, row);
+  }
+  if (rank == 0) {
     printf("#%13s %12s %6s %8s | %12s %12s %6s\n", "size(B)", "tokens", "type", "algo", "dispatch us", "combine us", "#wrong");
     fflush(stdout);
   }
@@ -357,10 +371,20 @@ static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream
     RT(cudaMalloc(&d_idx, slots * 4)); RT(cudaMalloc(&d_route, slots * 4)); RT(cudaMalloc(&d_w, slots * 4)); RT(cudaMalloc(&out, tokens * row * os));
     RT(cudaMemcpy(d_idx, ids[rank].data(), slots * 4, cudaMemcpyHostToDevice));
     RT(cudaMemcpy(d_w, w.data(), slots * 4, cudaMemcpyHostToDevice));
-    fill(x, tokens * row, o.in_dt, rank, 0, st);
-    RT(cudaMemsetAsync(recv, 0x5A, recv_rows * row * is, st));
+    const size_t nsc = quant ? recv_rows * row / o.q_block : 0;     // scales in recv_scales
+    if (!quant) fill(x, tokens * row, o.in_dt, rank, 0, st);
+    else if (o.in_dt == b200collFloat32) k_fill_q<float><<<256, 256, 0, st>>>((float*)x, tokens * row, rank, o.q_block);
+    else if (o.in_dt == b200collFloat16) k_fill_q<__half><<<256, 256, 0, st>>>((__half*)x, tokens * row, rank, o.q_block);
+    else k_fill_q<__nv_bfloat16><<<256, 256, 0, st>>>((__nv_bfloat16*)x, tokens * row, rank, o.q_block);
+    RT(cudaGetLastError());
+    RT(cudaMemsetAsync(recv, 0x5A, recv_rows * row * rs, st));
+    if (quant) RT(cudaMemsetAsync(recv_scales, 0x5A, nsc * 4, st));
     auto dispatch = [&] {
-      CC(b200collExpertDispatch(x, recv, row, recv_rows, d_idx, tokens, K, E, d_counts, d_route, d_dropped, o.in_dt, ctx.comm, st));
+      if (quant)
+        CC(b200collExpertDispatchQuantized(x, recv, recv_scales, row, recv_rows, d_idx, tokens, K, E, d_counts, d_route, d_dropped, o.in_dt, o.q_wire, o.q_block,
+                                           ctx.comm, st));
+      else
+        CC(b200collExpertDispatch(x, recv, row, recv_rows, d_idx, tokens, K, E, d_counts, d_route, d_dropped, o.in_dt, ctx.comm, st));
     };
     auto combine = [&] { CC(b200collExpertCombine(recv, out, row, recv_rows, d_route, d_w, tokens, K, &ep, ctx.comm, st)); };
     long errs = 0;
@@ -372,22 +396,39 @@ static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream
       RT(cudaStreamSynchronize(st));
       spin_barrier(sh, 0, n, &gen_ctr[0]);
       dispatch();
-      combine();
+      if (!quant) combine();
       RT(cudaStreamSynchronize(st));
       spin_barrier(sh, 1, n, &gen_ctr[1]);
-      std::vector<unsigned char> h_recv(recv_rows * row * is);
+      std::vector<unsigned char> h_recv(recv_rows * row * rs);
       std::vector<int32_t> h_route(slots), h_small(epr + 1);
       std::vector<char> h_out(tokens * row * os);
       RT(cudaMemcpy(h_recv.data(), recv, h_recv.size(), cudaMemcpyDeviceToHost));
       RT(cudaMemcpy(h_route.data(), d_route, slots * 4, cudaMemcpyDeviceToHost));
       RT(cudaMemcpy(h_small.data(), small, h_small.size() * 4, cudaMemcpyDeviceToHost));
       RT(cudaMemcpy(h_out.data(), out, h_out.size(), cudaMemcpyDeviceToHost));
+      std::vector<float> h_scales(nsc);
+      if (quant) RT(cudaMemcpy(h_scales.data(), recv_scales, nsc * 4, cudaMemcpyDeviceToHost));
       // recv: which (source, token) each of my rows holds
       std::vector<long long> src(recv_rows, -1);
       for (int s = 0; s < n; s++)
         for (size_t i = 0; i < slots; i++)
           if (rowof[s][i] >= 0 && ids[s][i] / epr == rank) src[rowof[s][i]] = (long long)s * tokens + (long long)(i / K);
-      for (size_t r = 0; r < recv_rows; r++) {
+      for (size_t r = 0; r < recv_rows && quant; r++) {      // FP8 bytes and scales from the host quantiser, or the poison
+        QMemo memo;
+        const int s = src[r] < 0 ? -1 : (int)(src[r] / (long long)tokens);
+        const size_t t = src[r] < 0 ? 0 : (size_t)(src[r] % (long long)tokens);
+        for (size_t e = 0; e < row; e++) {
+          const size_t at = r * row + e;
+          const long long got = h_recv[at], want = s < 0 ? 0x5A : (long long)q_code(o, s, t * row + e, &memo);
+          if (got != want) bad("recv FP8 byte", at, got, want);
+          if (e % o.q_block == 0) {
+            const size_t j = at / o.q_block;
+            const long long gs = out_bits(h_scales[j], b200collFloat32), ws = s < 0 ? 0x5A5A5A5All : (long long)out_bits(memo.s, b200collFloat32);
+            if (gs != ws) bad("recv scale bits", j, gs, ws);
+          }
+        }
+      }
+      for (size_t r = 0; r < recv_rows && !quant; r++) {
         for (size_t e = 0; e < row; e++) {
           const size_t at = r * row + e;
           long long got = 0, want = 0;
@@ -409,7 +450,7 @@ static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream
         if (h_route[i] != want) bad("route", i, h_route[i], want);
       }
       // the combine of identity experts: every stored slot of token t brings back t's own row
-      for (size_t t = 0; t < tokens; t++) {
+      for (size_t t = 0; t < tokens && !quant; t++) {
         for (size_t e = 0; e < row; e++) {
           float acc = 0.0f;
           for (int j = 0; j < K; j++) {
@@ -423,7 +464,7 @@ static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream
       }
     }
     float ms[2] = {0, 0};
-    for (int phase = 0; phase < 2; phase++) {
+    for (int phase = 0; phase < (quant ? 1 : 2); phase++) {
       for (int i = 0; i < o.warmup; i++) { if (phase == 0) dispatch(); else combine(); }
       RT(cudaStreamSynchronize(st));
       spin_barrier(sh, 2, n, &gen_ctr[2]);
@@ -445,7 +486,10 @@ static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream
     total_errors += es;
     b200collFault f;
     if (b200collCommGetAsyncError(ctx.comm, &f) != b200collSuccess) { fprintf(stderr, "rank %d WATCHDOG code=%u peer=%u block=%u expected=%u observed=%u\n", rank, f.code, f.peer, f.block, f.expected, f.observed); _exit(5); }
-    if (rank == 0) {
+    if (rank == 0 && quant) {
+      printf("%14zu %12zu %6s %8s | %12.2f %12s %6ld\n", tokens * row * is, tokens, dt_name(o.in_dt), n > 1 ? "twoshot" : "copy", worst[0] * 1e3, "-", es);
+      fflush(stdout);
+    } else if (rank == 0) {
       printf("%14zu %12zu %6s %8s | %12.2f %12.2f %6ld\n", tokens * row * is, tokens, dt_name(o.in_dt), n > 1 ? "twoshot" : "copy", worst[0] * 1e3, worst[1] * 1e3, es);
       fflush(stdout);
     }
@@ -507,9 +551,12 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
   }
   if (o.route_e) {
     const auto wide = [](b200collDataType_t t) { return t == b200collBfloat16 || t == b200collFloat16 || t == b200collFloat32; };
-    if (o.op != "alltoall" || o.q_block || o.bs_rows || o.row_len == 0 || o.row_len % 16 || !wide(o.in_dt) || !wide(o.out_dt) || o.route_e % n != 0) {
+    // with --quantize there is no combine, so no out type: the quantising alltoall defaults --out-dtype to the wire type
+    if (o.op != "alltoall" || o.bs_rows || o.row_len == 0 || o.row_len % 16 || !wide(o.in_dt) || (!o.q_block && !wide(o.out_dt)) || o.route_e % n != 0 ||
+        (o.q_block && o.row_len % o.q_block != 0)) {
       fprintf(stderr, "--route E:K takes --op alltoall, -d and --out-dtype bfloat16|half|float, a --row-len that is a multiple of 16, E a multiple of the\n"
-                      "number of ranks, and no --quantize, --block-scale or --combine\n");
+                      "number of ranks, and no --block-scale or --combine; with --quantize WIRE:BLOCK (the FP8 dispatch) a --row-len that is a\n"
+                      "multiple of BLOCK\n");
       return 2;
     }
     return run_route(o, ctx, sh, send, st, e0, e1);
@@ -879,6 +926,10 @@ int main(int argc, char** argv) {
            "                            --out-dtype the combine's out type, recv sized to the mean load (tokens * K rows); size = x bytes per rank;\n"
            "                            reports the dispatch (layout, count exchange and push) and the combine; -c 1 checks every received byte,\n"
            "                            count, route and dropped, and the combine bit for bit, against the host layout\n"
+           "  --route E:K --quantize WIRE:BLOCK   the device-routed FP8 expert dispatch: the same layout, each token's row quantised once to\n"
+           "                            WIRE with one fp32 scale per BLOCK elements (--row-len a multiple of BLOCK); reports the dispatch only (the\n"
+           "                            combine needs a wide expert_out); -c 1 checks every FP8 byte, scale, count, route and dropped against the\n"
+           "                            host layout and the host quantiser\n"
            "  --algo auto|ll|ll2|oneshot|twoshot|nvls   --inplace 0|1|2   --max-ctas N   --sweep kind:ctas:threads,...   --json FILE   --window SIZE\n"
            "  --selfcheck               report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;
@@ -906,7 +957,7 @@ int main(int argc, char** argv) {
     b200collConfig cfg; b200collConfigDefault(&cfg);
     const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
     if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o) +
-                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0);     // --route: recv holds K rows per token
+                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o);     // --route: recv holds K rows per token
     b200collUniqueId id; CC(b200collUniqueIdFromString(("perf/" + lr.job).c_str(), &id));
     RT(cudaSetDevice(dev));
     b200collComm_t comm;
@@ -935,7 +986,7 @@ int main(int argc, char** argv) {
   // arena: two windows (+ max buffers) and slack
   const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
   size_t need = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o) +
-                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0);     // --route: recv holds K rows per token
+                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o);     // --route: recv holds K rows per token
   if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = need;
   if (o.procs) {
     b200collUniqueId id; CC(b200collGetUniqueId(&id));

@@ -141,6 +141,7 @@ def load() -> C.CDLL:
                                            C.POINTER(Epilogue), vp, vp]
     i32p = C.POINTER(C.c_int32)
     L.b200collExpertDispatch.argtypes = [vp, vp, sz, sz, i32p, sz, ci, ci, i32p, i32p, i32p, ci, vp, vp]
+    L.b200collExpertDispatchQuantized.argtypes = [vp, vp, C.POINTER(C.c_float), sz, sz, i32p, sz, ci, ci, i32p, i32p, i32p, ci, ci, ci, vp, vp]
     L.b200collExpertCombine.argtypes = [vp, vp, sz, sz, i32p, C.POINTER(C.c_float), sz, ci, C.POINTER(Epilogue), vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
@@ -439,6 +440,59 @@ def check_expert_dispatch(nranks: int, x, topk_idx, num_experts: int, recv, expe
             if _overlap(t, u):
                 raise ValueError(f"{name} must not overlap {other}")
     return torch_dtype_code(x.dtype)
+
+
+def check_expert_dispatch_quantized(nranks: int, x, topk_idx, num_experts: int, recv, recv_scales, block: int, expert_counts=None, route=None,
+                                    dropped=None) -> tuple[int, int]:
+    """Rules of the device-routed expert dispatch with FP8 on the wire, checked on the tensors' metadata only (no communicator, no
+    library call, no device read): raises ValueError, returns the library codes of (x's type, the wire type). x, topk_idx, num_experts,
+    expert_counts, route and dropped as in check_expert_dispatch; block one of QUANT_BLOCKS and row_elems (x.shape[1]) a positive multiple
+    of it; recv: contiguous float8_e4m3fn or float8_e5m2 (the wire type) of whole rows; recv_scales: contiguous float32 with
+    recv.numel() // block elements. tokens * top_k, nranks * recv rows, tokens * row_elems / 16 (the 16-element vectors of x) and
+    tokens * top_k * row bytes / 16 are at most 2^31 - 1. x, recv and recv_scales must not overlap, and no output may overlap another
+    output, topk_idx, x, recv or recv_scales."""
+    import torch
+    if x.dtype not in (torch.bfloat16, torch.float16, torch.float32) or x.dim() != 2 or not x.is_contiguous():
+        raise ValueError(f"x must be a contiguous bfloat16, float16 or float32 [tokens, row_elems] tensor, got {x.dtype}{list(x.shape)}")
+    tokens, row_elems = x.shape
+    if isinstance(block, bool) or not isinstance(block, int) or block not in QUANT_BLOCKS:
+        raise ValueError(f"block must be one of {QUANT_BLOCKS}, got {block!r}")
+    if row_elems <= 0 or row_elems % block:
+        raise ValueError(f"row_elems (x.shape[1] = {row_elems}) must be a positive multiple of block ({block})")
+    if topk_idx.dtype != torch.int32 or topk_idx.dim() != 2 or not topk_idx.is_contiguous() or topk_idx.shape[1] < 1:
+        raise ValueError(f"topk_idx must be a contiguous int32 [tokens, top_k] tensor with top_k >= 1, got {topk_idx.dtype}{list(topk_idx.shape)}")
+    if topk_idx.shape[0] != tokens:
+        raise ValueError(f"topk_idx has {topk_idx.shape[0]} tokens, x has {tokens}")
+    top_k = topk_idx.shape[1]
+    if isinstance(num_experts, bool) or not isinstance(num_experts, int) or not 1 <= num_experts <= MAX_EXPERTS or num_experts % nranks:
+        raise ValueError(f"num_experts must be an int in [1, {MAX_EXPERTS}] and a multiple of nranks ({nranks}), got {num_experts!r}")
+    if recv.dtype not in (torch.float8_e4m3fn, torch.float8_e5m2) or not recv.is_contiguous() or recv.numel() % row_elems:
+        raise ValueError(f"recv must be a contiguous float8_e4m3fn or float8_e5m2 tensor (the wire type) of whole {row_elems}-element rows, "
+                         f"got {recv.dtype} with {recv.numel()} elements")
+    if recv_scales.dtype != torch.float32 or not recv_scales.is_contiguous() or recv_scales.numel() != recv.numel() // block:
+        raise ValueError(f"recv_scales must be a contiguous float32 tensor of recv.numel() // block = {recv.numel() // block} elements, "
+                         f"got {recv_scales.dtype} with {recv_scales.numel()}")
+    if tokens * top_k > _I31:
+        raise ValueError(f"tokens * top_k ({tokens * top_k}) must be at most 2^31 - 1")
+    if nranks * (recv.numel() // row_elems) > _I31:
+        raise ValueError("nranks * recv rows must be at most 2^31 - 1 (a route is an int32)")
+    if tokens * (row_elems // 16) > _I31:
+        raise ValueError("at most 2^31 - 1 16-element vectors of x (tokens * row_elems / 16)")
+    if tokens * top_k * (row_elems * x.element_size() // 16) > _I31:
+        raise ValueError("at most 2^31 - 1 16-byte vectors may be offered (tokens * top_k * row bytes / 16)")
+    for a, b, an, bn in ((recv, x, "recv", "x"), (recv_scales, x, "recv_scales", "x"), (recv, recv_scales, "recv", "recv_scales")):
+        if _overlap(a, b):
+            raise ValueError(f"{an} must not overlap {bn}")
+    outs = [(n, t, shape) for n, t, shape in (("expert_counts", expert_counts, (num_experts // nranks,)), ("route", route, (tokens, top_k)),
+                                              ("dropped", dropped, (1,))) if t is not None]
+    for name, t, shape in outs:
+        if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != _numel(shape):
+            raise ValueError(f"{name} must be a contiguous int32 tensor of shape {shape}, got {t.dtype}{list(t.shape)}")
+    for k, (name, t, _) in enumerate(outs):
+        for other, u in [(n, o) for n, o, _ in outs[k + 1:]] + [("topk_idx", topk_idx), ("x", x), ("recv", recv), ("recv_scales", recv_scales)]:
+            if _overlap(t, u):
+                raise ValueError(f"{name} must not overlap {other}")
+    return torch_dtype_code(x.dtype), torch_dtype_code(recv.dtype)
 
 
 def check_expert_combine(nranks: int, expert_out, route, weights, out) -> tuple[int, int]:
@@ -823,6 +877,36 @@ class Comm:
                                              tokens, top_k, num_experts, i32(expert_counts), i32(route), i32(dropped), code, self._h,
                                              self._stream(stream)), "ExpertDispatch")
         return recv, expert_counts, route, dropped
+
+    def expert_dispatch_quantized(self, x, topk_idx, num_experts: int, recv, recv_scales, block: int = 128, expert_counts=None, route=None,
+                                  dropped=None, stream=None):
+        """Device-routed expert dispatch with FP8 on the wire (b200collExpertDispatchQuantized): expert_dispatch's layout (the same rows,
+        expert_counts, route and dropped for the same ids), with each token's row quantised once on its own rank in blocks of `block`
+        elements and one fp32 scale per block: recv ([recv_rows * row_elems] FP8, its dtype is the wire type) gets the FP8 rows and
+        recv_scales ([recv_rows * row_elems // block] float32) their scales, row for row; rows not stored keep their bytes in both.
+        Returns (recv, recv_scales, expert_counts, route, dropped). The small outputs are allocated on the call's stream when not given.
+        Nothing is read back to the host. A program that drives several ranks from one thread (virtual ranks sharing a GPU) passes them,
+        allocated before the first rank's call: an allocation between two ranks' calls can wait for the device (a cache flush frees
+        memory, and freeing synchronises), while the earlier rank's layout kernel waits at its barrier for the next rank's call. With more
+        than one rank, recv and recv_scales must be arena tensors (`empty()`) of the same sizes on every rank; every rank calls, a rank
+        with no tokens included."""
+        import torch
+        ic, wc = check_expert_dispatch_quantized(self.nranks, x, topk_idx, num_experts, recv, recv_scales, block, expert_counts, route, dropped)
+        tokens, row_elems = x.shape
+        top_k = topk_idx.shape[1]
+        if expert_counts is None or route is None or dropped is None:
+            with torch.cuda.device(x.device), torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream(x.device)):
+                expert_counts = torch.empty(num_experts // self.nranks, dtype=torch.int32, device=x.device) if expert_counts is None else expert_counts
+                route = torch.empty(tokens, top_k, dtype=torch.int32, device=x.device) if route is None else route
+                dropped = torch.empty(1, dtype=torch.int32, device=x.device) if dropped is None else dropped
+            check_expert_dispatch_quantized(self.nranks, x, topk_idx, num_experts, recv, recv_scales, block, expert_counts, route, dropped)
+        i32 = lambda t: C.cast(C.c_void_p(t.data_ptr()), C.POINTER(C.c_int32))
+        _check(load().b200collExpertDispatchQuantized(C.c_void_p(x.data_ptr()), C.c_void_p(recv.data_ptr()),
+                                                      C.cast(C.c_void_p(recv_scales.data_ptr()), C.POINTER(C.c_float)), row_elems,
+                                                      recv.numel() // row_elems, i32(topk_idx), tokens, top_k, num_experts, i32(expert_counts),
+                                                      i32(route), i32(dropped), ic, wc, block, self._h, self._stream(stream)),
+               "ExpertDispatchQuantized")
+        return recv, recv_scales, expert_counts, route, dropped
 
     def expert_combine(self, expert_out, route, weights, out, scale: float = 1.0, stream=None):
         """Expert combine from the dispatch's device route (b200collExpertCombine): out[t] ([tokens, row_elems]) = round(scale * sum
