@@ -298,6 +298,8 @@ b200collResult_t b200collReduceScatterQuantized(const void* send, void* recv, si
                                                 const b200collEpilogue* ep, b200collRedOp_t op, b200collComm_t comm, b200collStream_t stream);
 b200collResult_t b200collAllReduceQuantized(const void* send, void* recv, size_t count, b200collDataType_t wire_dtype, int block,
                                             const b200collEpilogue* ep, b200collRedOp_t op, b200collComm_t comm, b200collStream_t stream);
+/* --- MoE expert dispatch (src/dispatch.cu) and combine (src/combine.cu). */
+
 /* Quantising all-to-all-v (expert dispatch): bf16, fp16 or fp32 rows in, FP8 rows and their block scales out, one kernel per call. The
  * row geometry is b200collAllToAllv's: send_rows[p] rows of row_elems elements, starting at row send_row_off[p] of send, go to peer p and
  * land at row recv_row_off_at_peer[p] of that peer's recv and recv_scales (host arrays of length nranks). The sender quantises in

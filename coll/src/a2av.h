@@ -1,5 +1,5 @@
-// The per-peer argument blocks of the all-to-all(v) kernels (k_a2av_push in kernels.cuh, k_a2av_quant_push in blockscaled.cu,
-// k_a2av_combine_pull in combine.cu) and the host code that fills and checks them. Plain C++: the kernels take them by value, the host
+// The per-peer argument blocks of the all-to-all(v) kernels (k_a2av_push in kernels.cuh, k_a2av_quant_push in dispatch.cu,
+// k_combine_pull<…, SegmentMap> in combine.cu) and the host code that fills and checks them. Plain C++: the kernels take them by value, the host
 // entry points build them.
 #pragma once
 #include <stddef.h>

@@ -20,16 +20,6 @@
 //   k_quant_pull_reduce<InT, WireT, OutT, true>   two-shot all-reduce: the same over my block slice, the result pushed into every recv
 //   k_quant_copy<InT, WireT, OutT>                one rank: the quantise / dequantise round trip in registers, no scratch, no barrier
 //
-// Quantising all-to-all-v (expert dispatch): bf16, fp16 or fp32 rows in, FP8 rows and their per-row block scales out, one kernel:
-//
-//   k_a2av_quant_push<InT, WireT>   barrier, quantise my rows for every peer and push FP8 and scales into its recv, barrier (releases)
-//   k_a2av_quant_copy<InT, WireT>   one rank: a local quantising copy, no barrier
-//
-// Routed FP8 dispatch (the push half of b200collExpertDispatchQuantized; its layout kernel lives in routed.cu):
-//
-//   k_expert_quant_push<InT, WireT, P>   quantise each token's row once, store FP8 and scales to every routed row of the owners' recv;
-//                                        P: closing barrier (releases), !P (one rank): local, no barrier
-//
 // Scales: a 16-byte FP8 vector lies in exactly one block (row_len and block_cols are multiples of 16; a quantising block is a whole
 // number of vectors), so a vector needs one scale per rank. Lanes of a warp hold consecutive vectors and usually share scales (8 lanes
 // per 1x128 block, whole warps per 128x128 block): __match_any_sync groups the lanes by scale index, the lowest lane of each group loads
@@ -37,9 +27,7 @@
 // vector to its scale: the block-scaled vector -> (row, column) -> block arithmetic is 32-bit multiply-high division by host-computed
 // constants (no integer division in the loops), a quantising block is a shift.
 //
-// Quantising, per block: amax = max |x| (the largest unsigned bit pattern of |x|, so a NaN anywhere makes amax NaN); inv = FMAX / amax
-// and s = amax / FMAX, both IEEE divisions rounded to nearest, inv = s = 1 when amax == 0 or inv overflows; q = fp8_satfinite(x * inv);
-// the dequantised value is float(q) * s. FMAX is 448 (e4m3) or 57344 (e5m2).
+// Quantising, per block: the rule in quant.cuh, which also holds the quantise helpers this file shares with dispatch.cu.
 //
 // Fusing the quantise phase into the pull kernel is sound because of three properties, which the code below keeps:
 //   * Same-index CTAs only. The epoch barrier orders CTA b of this rank against CTA b of every peer, nothing else. Every vector loop in
@@ -63,17 +51,11 @@
 
 #include <type_traits>
 
-#include "a2av.h"
 #include "comm.h"
 #include "launch.cuh"
+#include "quant.cuh"
 
 namespace b200coll {
-
-using bf16 = __nv_bfloat16;
-using f8 = __nv_fp8_e4m3;
-using e5m2 = __nv_fp8_e5m2;
-
-constexpr int kBsqThreads = 512;
 
 // q = floor(n / d) for every 32-bit n as (umulhi(n, m) + n) >> l, l = ceil(log2 d), m = floor(2^32 (2^l - d) / d) + 1 (Granlund and
 // Montgomery, "Division by invariant integers using multiplication", 1994). The sum needs 33 bits, so it is formed in 64.
@@ -98,23 +80,6 @@ struct BsqGeom {
     return br.div(row) * ncb + vpb.div(cv);
   }
 };
-
-struct QuantGeom {
-  size_t data_off, scale_off;     // arena offsets of the scratch FP8 copy and of its scales (the same on every rank)
-  uint32_t nvec;                  // 16-element vectors in one rank's send buffer
-  uint32_t nblk;                  // blocks in one rank's send buffer
-  uint32_t lvpb;                  // log2(vectors per block)
-  __device__ __forceinline__ uint32_t scale_index(uint32_t v) const { return v >> lvpb; }
-};
-
-// The one walk over vectors [v0, v1): a warp takes 32 consecutive vectors starting at v0 plus a multiple of 32, the grid strides
-// over the range, and all 32 lanes run every iteration (f(v, active), active = v < v1), so the full-mask warp intrinsics below always
-// see whole warps. 32-bit indices: the host keeps nvec below 2^31, so b + stride cannot wrap.
-template <typename F>
-__device__ __forceinline__ void warp_walk(uint32_t v0, uint32_t v1, F&& f) {
-  const uint32_t lane = threadIdx.x & 31;
-  for (uint32_t b = v0 + blockIdx.x * blockDim.x + (threadIdx.x & ~31u); b < v1; b += gridDim.x * blockDim.x) f(b + lane, b + lane < v1);
-}
 
 // The scale of every lane's vector, one load per distinct index in the warp. All 32 lanes call it; `active` lanes have a vector.
 struct WarpScale {
@@ -241,74 +206,9 @@ __global__ void __launch_bounds__(kBsqThreads, 1) k_bsq_pull_reduce(COMM_PARAM, 
 }
 
 // Quantising kernels.
-template <typename WireT> constexpr float kWireMax = 448.0f;
-template <> constexpr float kWireMax<__nv_fp8_e5m2> = 57344.0f;
-
 // the first vector of slice s of n: slices are cut at whole blocks
 __device__ __forceinline__ uint32_t quant_slice_start(const QuantGeom& g, uint32_t s, uint32_t n) {
   return (uint32_t)((unsigned long long)g.nblk * s / n) << g.lvpb;
-}
-
-// 16 elements of InT at p, widened (exactly) to fp32
-template <typename InT> __device__ __forceinline__ void quant_load16(const char* p, float* x) {
-  if constexpr (std::is_same<InT, float>::value) {
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-      const uint4 v = ld_vec(p + 16 * k);
-      x[4 * k] = __uint_as_float(v.x); x[4 * k + 1] = __uint_as_float(v.y); x[4 * k + 2] = __uint_as_float(v.z); x[4 * k + 3] = __uint_as_float(v.w);
-    }
-  } else {
-#pragma unroll
-    for (int k = 0; k < 2; k++) {
-      const uint4 v = ld_vec(p + 16 * k);
-      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-      for (int i = 0; i < 4; i++) {
-        if constexpr (std::is_same<InT, __nv_bfloat16>::value) {
-          x[8 * k + 2 * i] = __uint_as_float(w[i] << 16); x[8 * k + 2 * i + 1] = __uint_as_float(w[i] & 0xFFFF0000u);
-        } else {
-          const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
-          x[8 * k + 2 * i] = f.x; x[8 * k + 2 * i + 1] = f.y;
-        }
-      }
-    }
-  }
-}
-
-// Quantise this lane's 16 elements with the amax of its block, whose vectors are held by the aligned group of `gl` lanes (a power of
-// two up to 32) this lane belongs to. All 32 lanes call it; idle lanes pass zeros, and their groups are wholly idle. Returns the FP8
-// vector; *scale receives s.
-template <typename WireT> __device__ __forceinline__ uint4 quant_vec(const float* x, uint32_t gl, float* scale) {
-  uint32_t m = 0;
-#pragma unroll
-  for (int i = 0; i < 16; i++) m = max(m, __float_as_uint(x[i]) & 0x7FFFFFFFu);
-  for (uint32_t o = 1; o < gl; o <<= 1) m = max(m, __shfl_xor_sync(0xFFFFFFFFu, m, o));
-  const float amax = __uint_as_float(m);
-  float inv = __fdiv_rn(kWireMax<WireT>, amax), s = __fdiv_rn(amax, kWireMax<WireT>);
-  if (amax == 0.0f || inv == INFINITY) { inv = 1.0f; s = 1.0f; }
-  float y[16];
-#pragma unroll
-  for (int i = 0; i < 16; i++) y[i] = __fmul_rn(x[i], inv);
-  uint32_t w[4];
-  Pack<WireT, 16>::run(y, w);                                     // cvt.rn.satfinite: F2FP.SATFINITE.E4M3 / .E5M2
-  *scale = s;
-  return make_uint4(w[0], w[1], w[2], w[3]);
-}
-
-// Quantise vectors [v0, v1) of my send buffer into my scratch, walked as the pull loops walk a slice.
-template <typename InT, typename WireT>
-__device__ __forceinline__ void quant_range(const QuantGeom& g, const char* in, char* q, char* scales, uint32_t v0, uint32_t v1) {
-  const uint32_t lane = threadIdx.x & 31, gl = 1u << g.lvpb;
-  warp_walk(v0, v1, [&](uint32_t v, bool act) {
-    float x[16] = {};
-    if (act) quant_load16<InT>(in + (size_t)v * (16 * sizeof(InT)), x);
-    float s;
-    const uint4 w = quant_vec<WireT>(x, gl, &s);
-    if (act) {
-      st_vec(q + (size_t)v * 16, w);
-      if ((lane & (gl - 1)) == 0) *reinterpret_cast<float*>(scales + (size_t)g.scale_index(v) * 4) = s;
-    }
-  });
 }
 
 template <typename InT, typename WireT, typename OutT>
@@ -359,118 +259,7 @@ __global__ void __launch_bounds__(kBsqThreads, 1) k_quant_pull_reduce(COMM_PARAM
   if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
 }
 
-// Quantising all-to-all-v. A2AvArgs counts 16-element vectors here: src_vec[p] of my send, dst_vec[p] of peer p's recv (FP8, 16 bytes
-// per vector), and the prefix over the staggered peer order. The scale of destination vector d is fp32 element d >> lvpb of the peer's
-// recv_scales. Blocks never straddle a warp or a peer's segment: every prefix entry and every destination offset is whole rows, a row is
-// whole blocks, and a block is a power of two of at most 32 vectors. So warp_walk's 32-aligned warps hold whole blocks of one segment
-// (a block's lanes are one aligned lane group, all active or all idle), and quant_vec's butterfly sees exactly the block's lanes.
-template <typename InT, typename WireT>
-__global__ void __launch_bounds__(kBsqThreads) k_a2av_quant_push(COMM_PARAM, const char* __restrict__ in, size_t q_off, size_t s_off,
-                                                                 const __grid_constant__ A2AvArgs a, uint32_t lvpb, uint32_t op) {
-  pdl_prologue();
-  const uint32_t s = load_seq(c, kSeqBarrier);
-  if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;          // every peer has entered the call: its recv is free to overwrite
-  const uint32_t lane = threadIdx.x & 31, gl = 1u << lvpb;
-  warp_walk(0, (uint32_t)a.prefix[c.nranks], [&](uint32_t v, bool act) {
-    int p = 0;
-    uint32_t lv = 0;
-    float x[16] = {};
-    if (act) {
-      int j = 0;
-#pragma unroll
-      for (int q = 1; q < kMaxRanks; q++) if (q < c.nranks && v >= a.prefix[q]) j = q;
-      p = c.rank + 1 + j; if (p >= c.nranks) p -= c.nranks;
-      lv = v - (uint32_t)a.prefix[j];
-      quant_load16<InT>(in + (a.src_vec[p] + lv) * (16 * sizeof(InT)), x);
-    }
-    float sc;
-    const uint4 w = quant_vec<WireT>(x, gl, &sc);
-    if (act) {
-      const unsigned long long d = a.dst_vec[p] + lv;
-      st_vec(c.peer[p] + q_off + d * 16, w);
-      if ((lane & (gl - 1)) == 0) *reinterpret_cast<float*>(c.peer[p] + s_off + (d >> lvpb) * 4) = sc;
-    }
-  });
-  if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // releases my stores to their receivers
-  if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
-}
-
-// One rank: vectors [0, g.nvec) of in quantised into q and scales (all three already offset to the first row), no barrier
-template <typename InT, typename WireT>
-__global__ void __launch_bounds__(kBsqThreads) k_a2av_quant_copy(const __grid_constant__ QuantGeom g, const char* __restrict__ in, char* __restrict__ q,
-                                                                 char* __restrict__ scales) {
-  pdl_prologue();
-  quant_range<InT, WireT>(g, in, q, scales, 0, g.nvec);
-}
-
-// Routed FP8 dispatch (b200collExpertDispatchQuantized; routed.cu launches k_routed_layout before it on the same stream). Vectors
-// [0, nvec) of x are (token, 16-element vector of its row), vpr vectors per row. Each is loaded, widened and quantised once, then stored
-// to every stored slot of its token: the FP8 vector to row `row` of the owner's recv, and the block's scale, by the block's lowest lane,
-// to the same row of the owner's recv_scales. A route outside [0, nranks * recv_rows) stores nothing, so a token's slots all get the
-// same bytes and scales. quant_vec's butterfly sees exactly one block's lanes: a row is whole blocks, a token's first vector t * vpr is a
-// multiple of the vectors per block, and a block is a power of two of at most 32 vectors; so with warp_walk's 32-aligned warps a block's
-// lanes are one aligned lane group of one warp, all active or all idle (and, being one token's, they read the same routes).
-// kPeers: stores into the owners' arenas at q_off / s_off. No entry barrier: layout barrier A, one kernel earlier on this stream, already
-// freed every peer's recv and recv_scales (the ordering argument in routed.cu, as for k_routed_push); one closing releasing barrier.
-// !kPeers (one rank): stores into recv and scales, no barrier.
-template <typename InT, typename WireT, bool kPeers>
-__global__ void __launch_bounds__(kBsqThreads) k_expert_quant_push(COMM_PARAM, const char* __restrict__ x, char* __restrict__ recv, char* __restrict__ scales,
-                                                                   size_t q_off, size_t s_off, const int32_t* __restrict__ route, uint32_t top_k,
-                                                                   uint32_t vpr, uint32_t nvec, uint32_t recv_rows, uint32_t lvpb, uint32_t op) {
-  pdl_prologue();
-  const uint32_t lane = threadIdx.x & 31, gl = 1u << lvpb, limit = (uint32_t)c.nranks * recv_rows;
-  warp_walk(0, nvec, [&](uint32_t v, bool act) {
-    float xv[16] = {};
-    if (act) quant_load16<InT>(x + (size_t)v * (16 * sizeof(InT)), xv);
-    float sc;
-    const uint4 w = quant_vec<WireT>(xv, gl, &sc);
-    if (act) {
-      const uint32_t t = v / vpr, col = v - t * vpr;
-      for (uint32_t j = 0; j < top_k; j++) {
-        const uint32_t r = (uint32_t)route[(size_t)t * top_k + j];
-        if (r >= limit) continue;
-        const uint32_t p = r / recv_rows, row = r - p * recv_rows;
-        const size_t d = (size_t)row * vpr + col;                   // FP8 vector d of the owner's recv; its scale is element d >> lvpb
-        st_vec((kPeers ? c.peer[p] + q_off : recv) + d * 16, w);
-        if ((lane & (gl - 1)) == 0) *reinterpret_cast<float*>((kPeers ? c.peer[p] + s_off : scales) + (d >> lvpb) * 4) = sc;
-      }
-    }
-  });
-  if constexpr (kPeers) {
-    const uint32_t s = load_seq(c, kSeqBarrier);
-    if (!barrier_blocks<true>(c, 2 * s + 1, op)) return;         // my rows and scales are in every owner's buffers before its kernel ends
-    if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
-  }
-}
-
 // ------------------------------------------------------------------------------------------------ host side
-// (wire, out) -> f(Tag<WireT>, Tag<OutT>); the argument checks have refused every other type
-template <typename F>
-static b200collResult_t dispatch_wire_out(b200collDataType_t wire, b200collDataType_t out, F&& f) {
-  auto outs = [&](auto tw) -> b200collResult_t {
-    switch (out) {
-      case b200collBfloat16: return f(tw, Tag<bf16>{});
-      case b200collFloat16: return f(tw, Tag<__half>{});
-      default: return f(tw, Tag<float>{});
-    }
-  };
-  return wire == b200collFloat8e4m3 ? outs(Tag<f8>{}) : outs(Tag<e5m2>{});
-}
-
-// the quantising kernels: one more level for the input type
-template <typename F>
-static b200collResult_t dispatch_quant(b200collDataType_t in, b200collDataType_t wire, b200collDataType_t out, F&& f) {
-  auto wires_outs = [&](auto ti) -> b200collResult_t { return dispatch_wire_out(wire, out, [&](auto tw, auto to) { return f(ti, tw, to); }); };
-  switch (in) {
-    case b200collBfloat16: return wires_outs(Tag<bf16>{});
-    case b200collFloat16: return wires_outs(Tag<__half>{});
-    default: return wires_outs(Tag<float>{});
-  }
-}
-
-static bool is_fp8(b200collDataType_t t) { return t == b200collFloat8e4m3 || t == b200collFloat8e5m2; }
-static bool wide_type(b200collDataType_t t) { return t == b200collBfloat16 || t == b200collFloat16 || t == b200collFloat32; }
-
 template <typename Geom> struct Fp8Call {
   b200collComm* c;
   size_t count;                   // elements of one rank's send buffer
@@ -480,14 +269,14 @@ template <typename Geom> struct Fp8Call {
   Geom g;
 };
 
-// The argument rules both families share; `family_check` returns the message of the first family rule the call breaks, or nullptr.
+// The argument rules both families share; `family_check` returns the message of the first family rule the call breaks, or "".
 // Every refusal comes before the poisoned-communicator check. On success `call` is filled in except for its geometry.
 template <typename Check, typename Geom>
 static b200collResult_t fp8_prepare(b200collComm* c, b200collOp_t which, const void* send, const void* recv, size_t count, const b200collEpilogue* ep,
                                     b200collRedOp_t rop, const char* family, Check&& family_check, Fp8Call<Geom>* call) {
   auto refuse = [](const std::string& msg) { set_last_error(msg); return b200collInvalidArgument; };
   if (!c || !send || !recv || !ep) return refuse("null argument");
-  if (const char* e = family_check()) return refuse(e);
+  if (const std::string e = family_check(); !e.empty()) return refuse(e);
   if (!wide_type(ep->out_dtype)) return refuse(std::string(family) + " collectives: out_dtype must be bf16, fp16 or fp32");
   if (which != b200collOpAllGather && rop != b200collSum && rop != b200collAvg) return refuse(std::string(family) + " reductions take sum or avg only");
   if (count / 16 >= ((size_t)1 << 31)) return refuse(std::string(family) + " collectives: fewer than 2^35 elements per rank");
@@ -510,22 +299,10 @@ static b200collAlgo_t fp8_all_reduce_algo(b200collComm* c, size_t count, const v
   return two ? b200collAlgoTwoShot : b200collAlgoOneShot;
 }
 
-// Whole warps: WarpScale and the amax butterfly are full-mask warp intrinsics, and pick_grid takes a forced thread count as given.
-static Grid warp_grid(const b200collComm* c, size_t vecs) {
-  Grid gr = pick_grid(c, kShapeP2p, vecs, 1);
-  gr.threads = std::max(32, gr.threads & ~31);
-  return gr;
-}
-
 // the pull-reduce grid: sized to my slice (reduce-scatter, two-shot) or to the whole buffer (one-shot)
 static Grid reduce_grid(const b200collComm* c, b200collOp_t which, b200collAlgo_t algo, uint32_t nvec) {
   const uint32_t n = (uint32_t)c->nranks;
   return warp_grid(c, algo == b200collAlgoTwoShot ? nvec / n + 1 : which == b200collOpReduceScatter ? nvec / n : nvec);
-}
-
-// nranks == 1: no peers, no barrier; grid as for the fused copy (streaming, 8 CTAs of 256 threads per SM at most)
-static int copy_blocks(const b200collComm* c, uint32_t nvec) {
-  return (int)std::max<size_t>(1, std::min<size_t>(((size_t)nvec + 255) / 256, (size_t)std::max(1, c->sm_count) * 8));
 }
 
 // ---- block-scaled
@@ -534,7 +311,7 @@ using BsqCall = Fp8Call<BsqGeom>;
 // Everything the three entry points check before they launch. On success `call` is filled in; count == 0 is left to the caller.
 static b200collResult_t bsq_prepare(b200collComm* c, b200collOp_t which, const void* send, void* recv, size_t count, const b200collBlockScale* bs,
                                     const b200collEpilogue* ep, b200collRedOp_t rop, BsqCall* call) {
-  b200collResult_t rc = fp8_prepare(c, which, send, recv, count, ep, rop, "block-scaled", [&]() -> const char* {
+  b200collResult_t rc = fp8_prepare(c, which, send, recv, count, ep, rop, "block-scaled", [&]() -> std::string {
     if (!bs || !bs->scales) return "null argument";
     if (!is_fp8(ep->in_dtype)) return "block-scaled collectives: in_dtype must be e4m3 or e5m2";
     if (bs->row_len == 0 || bs->row_len % 16 != 0) return "block-scaled collectives: row_len must be a positive multiple of 16";
@@ -542,17 +319,14 @@ static b200collResult_t bsq_prepare(b200collComm* c, b200collOp_t which, const v
     if (count % bs->row_len != 0) return "block-scaled collectives: the send count must be a multiple of row_len";
     if (which == b200collOpReduceScatter && (count / bs->row_len) % (size_t)c->nranks != 0) return "block-scaled reduce-scatter: the number of rows must be a multiple of nranks";
     if (!aligned(bs->scales, 4)) return "block-scaled collectives: scales must be 4-byte aligned";
-    return nullptr;
+    return "";
   }, call);
   if (rc != b200collSuccess || count == 0) return rc;
   const size_t rows = count / bs->row_len, vpr = bs->row_len / 16, vpb = (size_t)bs->block_cols / 16;
   const size_t nbr = (rows + bs->block_rows - 1) / bs->block_rows, ncb = (vpr + vpb - 1) / vpb;
   if (overlaps(send, call->in_bytes, recv, call->out_bytes)) { set_last_error("block-scaled collectives: recv must not overlap send"); return b200collInvalidArgument; }
-  // peers read my matrix and scales at MY arena offsets: both must be arena memory (there is no staging path for these ops)
-  if (!b200collIsSymmetric(c, send, count) || !b200collIsSymmetric(c, bs->scales, nbr * ncb * 4)) {
-    set_last_error("block-scaled collectives: send and scales must lie in the symmetric arena (b200collMemAlloc), at the same offsets on every rank");
-    return b200collInvalidUsage;
-  }
+  // peers read my matrix and scales (there is no staging path for these ops)
+  if ((rc = in_arena(c, "block-scaled collectives: ", "send and scales", {{send, count}, {bs->scales, nbr * ncb * 4}})) != b200collSuccess) return rc;
   BsqGeom& g = call->g;
   g.data_off = arena_off(c, send); g.scale_off = arena_off(c, bs->scales);
   g.nvec = (uint32_t)(count / 16); g.ncb = (uint32_t)ncb;
@@ -562,13 +336,13 @@ static b200collResult_t bsq_prepare(b200collComm* c, b200collOp_t which, const v
 
 static b200collResult_t bsq_copy(const BsqCall& k, const void* send, const b200collBlockScale* bs, void* recv, const b200collEpilogue* ep, cudaStream_t st) {
   b200collComm* c = k.c;
-  return dispatch_wire_out(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
+  return with_fp8(ep->in_dtype, [&](auto ti) { return with_wide(ep->out_dtype, [&](auto to) -> b200collResult_t {
     using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
     launch_k(k_bsq_copy<InT, OutT>, copy_blocks(c, k.g.nvec), 256, st, k.g, static_cast<const char*>(send), reinterpret_cast<const char*>(bs->scales),
              static_cast<OutT*>(recv), k.scale);
     LAUNCH_CHECK(c);
     return b200collSuccess;
-  });
+  }); });
 }
 
 static b200collResult_t bsq_reduce(const BsqCall& k, b200collOp_t which, b200collAlgo_t algo, void* recv, const b200collEpilogue* ep, cudaStream_t st) {
@@ -579,7 +353,7 @@ static b200collResult_t bsq_reduce(const BsqCall& k, b200collOp_t which, b200col
     v0 = (uint32_t)((unsigned long long)k.g.nvec * me / n); v1 = (uint32_t)((unsigned long long)k.g.nvec * (me + 1) / n);
   }
   const Grid gr = reduce_grid(c, which, algo, k.g.nvec);
-  return dispatch_wire_out(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
+  return with_fp8(ep->in_dtype, [&](auto ti) { return with_wide(ep->out_dtype, [&](auto to) -> b200collResult_t {
     using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
     if (algo == b200collAlgoTwoShot)
       launch_k(k_bsq_pull_reduce<InT, OutT, true>, gr.blocks, gr.threads, st, c->dev, k.g, static_cast<OutT*>(nullptr), arena_off(c, recv), v0, v1, k.scale, (uint32_t)which);
@@ -587,7 +361,7 @@ static b200collResult_t bsq_reduce(const BsqCall& k, b200collOp_t which, b200col
       launch_k(k_bsq_pull_reduce<InT, OutT, false>, gr.blocks, gr.threads, st, c->dev, k.g, static_cast<OutT*>(recv), (size_t)0, v0, v1, k.scale, (uint32_t)which);
     LAUNCH_CHECK(c);
     return b200collSuccess;
-  });
+  }); });
 }
 
 // ---- quantising
@@ -596,14 +370,14 @@ using QuantCall = Fp8Call<QuantGeom>;
 // Everything the three entry points check before they touch the scratch or launch; count == 0 is left to the caller.
 static b200collResult_t quant_prepare(b200collComm* c, b200collOp_t which, const void* send, void* recv, size_t count, b200collDataType_t wire, int block,
                                       const b200collEpilogue* ep, b200collRedOp_t rop, QuantCall* call) {
-  b200collResult_t rc = fp8_prepare(c, which, send, recv, count, ep, rop, "quantised", [&]() -> const char* {
+  b200collResult_t rc = fp8_prepare(c, which, send, recv, count, ep, rop, "quantised", [&]() -> std::string {
     if (!wide_type(ep->in_dtype)) return "quantised collectives: in_dtype must be bf16, fp16 or fp32";
     if (!is_fp8(wire)) return "quantised collectives: wire_dtype must be e4m3 or e5m2";
-    if (block < 16 || block > 512 || (block & (block - 1)) != 0) return "quantised collectives: block must be 16, 32, 64, 128, 256 or 512";
+    if (quant_lvpb(block) < 0) return std::string("quantised collectives: ") + kBlockRule;
     const bool rs = which == b200collOpReduceScatter;
     if ((rs ? count / (size_t)c->nranks : count) % (size_t)block != 0)
       return rs ? "quantised reduce-scatter: recvcount must be a multiple of block" : "quantised collectives: the count must be a multiple of block";
-    return nullptr;
+    return "";
   }, call);
   if (rc != b200collSuccess || count == 0) return rc;
   // in place (all-reduce only): every vector is read and rewritten at the same position, so the element sizes must agree
@@ -616,8 +390,7 @@ static b200collResult_t quant_prepare(b200collComm* c, b200collOp_t which, const
   QuantGeom& g = call->g;
   g.nvec = (uint32_t)(count / 16);
   g.nblk = (uint32_t)(count / (size_t)block);
-  g.lvpb = 0;
-  while ((16u << g.lvpb) < (uint32_t)block) g.lvpb++;
+  g.lvpb = (uint32_t)quant_lvpb(block);
   return b200collSuccess;
 }
 
@@ -648,12 +421,12 @@ static b200collResult_t quant_scratch(b200collComm* c, QuantCall* k) {
 // nranks == 1: the round trip in registers
 static b200collResult_t quant_copy(const QuantCall& k, const void* send, void* recv, b200collDataType_t wire, const b200collEpilogue* ep, cudaStream_t st) {
   b200collComm* c = k.c;
-  return dispatch_quant(ep->in_dtype, wire, ep->out_dtype, [&](auto ti, auto tw, auto to) -> b200collResult_t {
+  return with_wide(ep->in_dtype, [&](auto ti) { return with_fp8(wire, [&](auto tw) { return with_wide(ep->out_dtype, [&](auto to) -> b200collResult_t {
     using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type; using OutT = typename decltype(to)::type;
     launch_k(k_quant_copy<InT, WireT, OutT>, copy_blocks(c, k.g.nvec), 256, st, static_cast<const char*>(send), static_cast<OutT*>(recv), k.g.nvec, k.g.lvpb, k.scale);
     LAUNCH_CHECK(c);
     return b200collSuccess;
-  });
+  }); }); });
 }
 
 static b200collResult_t quant_reduce(const QuantCall& k, b200collOp_t which, b200collAlgo_t algo, const void* send, void* recv, b200collDataType_t wire,
@@ -661,7 +434,7 @@ static b200collResult_t quant_reduce(const QuantCall& k, b200collOp_t which, b20
   b200collComm* c = k.c;
   const uint32_t nslices = (which == b200collOpReduceScatter || algo == b200collAlgoTwoShot) ? (uint32_t)c->nranks : 1u;
   const Grid gr = reduce_grid(c, which, algo, k.g.nvec);
-  return dispatch_quant(ep->in_dtype, wire, ep->out_dtype, [&](auto ti, auto tw, auto to) -> b200collResult_t {
+  return with_wide(ep->in_dtype, [&](auto ti) { return with_fp8(wire, [&](auto tw) { return with_wide(ep->out_dtype, [&](auto to) -> b200collResult_t {
     using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type; using OutT = typename decltype(to)::type;
     const char* in = static_cast<const char*>(send);
     if (algo == b200collAlgoTwoShot)
@@ -672,94 +445,7 @@ static b200collResult_t quant_reduce(const QuantCall& k, b200collOp_t which, b20
                (uint32_t)which);
     LAUNCH_CHECK(c);
     return b200collSuccess;
-  });
-}
-
-// ---- quantising all-to-all-v
-// (in, wire) -> f(Tag<InT>, Tag<WireT>)
-template <typename F>
-static b200collResult_t dispatch_in_wire(b200collDataType_t in, b200collDataType_t wire, F&& f) {
-  return dispatch_quant(in, wire, b200collFloat32, [&](auto ti, auto tw, auto) { return f(ti, tw); });
-}
-
-// Everything b200collAllToAllvQuantized checks before it launches; on success `a` holds the vector geometry (prefix not yet filled),
-// `nv` the vectors per peer and `in_bytes` the input bytes sent.
-static b200collResult_t a2aq_prepare(b200collComm* c, const void* send, void* recv, float* recv_scales, size_t row_elems, size_t recv_rows,
-                                     const int64_t* send_rows, const int64_t* send_row_off, const int64_t* recv_row_off_at_peer,
-                                     b200collDataType_t in_dtype, b200collDataType_t wire, int block, A2AvArgs* a, unsigned long long* nv,
-                                     size_t* in_bytes) {
-  auto refuse = [](const std::string& msg) { set_last_error("quantised all-to-all-v: " + msg); return b200collInvalidArgument; };
-  if (!c || !send || !recv || !recv_scales || !send_rows || !send_row_off || !recv_row_off_at_peer) return refuse("null argument");
-  if (!wide_type(in_dtype)) return refuse("in_dtype must be bf16, fp16 or fp32");
-  if (!is_fp8(wire)) return refuse("wire_dtype must be e4m3 or e5m2");
-  if (block < 16 || block > 512 || (block & (block - 1)) != 0) return refuse("block must be 16, 32, 64, 128, 256 or 512");
-  if (row_elems == 0 || row_elems % (size_t)block != 0) return refuse("row_elems must be a positive multiple of block");
-  if (!aligned(send, 16) || !aligned(recv, 16) || !aligned(recv_scales, 4)) return refuse("send and recv must be 16-byte aligned, recv_scales 4-byte aligned");
-  const size_t is = b200collTypeSize(in_dtype);
-  const size_t max_rows = (SIZE_MAX >> 4) / (row_elems * is);     // every byte offset below then fits in size_t with room to spare
-  if (recv_rows > max_rows) return refuse("recv_rows * row_elems is too large");
-  const unsigned long long row_vecs = row_elems / 16, max_vecs = (1ull << 31) - 1;
-  unsigned long long total = 0;
-  size_t send_end = 0;                                            // the bytes of send that are read
-  *in_bytes = 0;
-  A2AvRows rg;
-  const std::string bad = a2av_rows(c->nranks, send_rows, send_row_off, recv_row_off_at_peer, recv_rows, max_rows, &rg);
-  if (!bad.empty()) return refuse(bad);
-  for (int p = 0; p < c->nranks; p++) {
-    const size_t rows = rg.rows[p], src = rg.src_row[p], dst = rg.dst_row[p];
-    if (rows > (max_vecs - total) / row_vecs) return refuse("at most 2^31 - 1 16-element vectors may be sent per rank");
-    total += rows * row_vecs;
-    a->src_vec[p] = src * row_vecs;
-    a->dst_vec[p] = dst * row_vecs;
-    nv[p] = rows * row_vecs;
-    *in_bytes += rows * row_elems * is;
-    if (rows) send_end = std::max(send_end, (src + rows) * row_elems * is);
-  }
-  if (comm_poisoned(c)) return b200collRemoteError;
-  const size_t q_bytes = recv_rows * row_elems, s_bytes = recv_rows * (row_elems / (size_t)block) * 4;
-  if (overlaps(send, send_end, recv, q_bytes) || overlaps(send, send_end, recv_scales, s_bytes)) return refuse("send must not overlap recv or recv_scales");
-  if (overlaps(recv, q_bytes, recv_scales, s_bytes)) return refuse("recv and recv_scales must not overlap");
-  // peers store into my recv and recv_scales at MY arena offsets: both must be arena memory
-  if (c->nranks > 1 && (!b200collIsSymmetric(c, recv, std::max<size_t>(q_bytes, 1)) || !b200collIsSymmetric(c, recv_scales, std::max<size_t>(s_bytes, 1)))) {
-    set_last_error("quantised all-to-all-v: recv and recv_scales must lie in the symmetric arena (b200collMemAlloc), at the same offsets on every rank");
-    return b200collInvalidUsage;
-  }
-  return b200collSuccess;
-}
-
-// ---- routed FP8 dispatch: the push after the layout kernel (routed.cu checks the arguments and launches the layout first)
-void load_expert_quant_push() {
-  cudaFuncAttributes fa;
-  for (b200collDataType_t in : {b200collBfloat16, b200collFloat16, b200collFloat32})
-    for (b200collDataType_t wire : {b200collFloat8e4m3, b200collFloat8e5m2})
-      dispatch_in_wire(in, wire, [&](auto ti, auto tw) -> b200collResult_t {
-        using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type;
-        cudaFuncGetAttributes(&fa, k_expert_quant_push<InT, WireT, true>);
-        cudaFuncGetAttributes(&fa, k_expert_quant_push<InT, WireT, false>);
-        return b200collSuccess;
-      });
-}
-
-b200collResult_t launch_expert_quant_push(b200collComm* c, const void* x, void* recv, float* recv_scales, const int32_t* route, size_t tokens, int top_k,
-                                          size_t row_elems, size_t recv_rows, b200collDataType_t in_dtype, b200collDataType_t wire, int block, cudaStream_t st) {
-  uint32_t lvpb = 0;
-  while ((16u << lvpb) < (uint32_t)block) lvpb++;
-  const uint32_t vpr = (uint32_t)(row_elems / 16), nvec = (uint32_t)(tokens * vpr);
-  const char* in = static_cast<const char*>(x);
-  return dispatch_in_wire(in_dtype, wire, [&](auto ti, auto tw) -> b200collResult_t {
-    using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type;
-    if (c->nranks > 1) {
-      // the full P2P grid on every rank, whatever its tokens: CTA b meets CTA b of every peer in the closing barrier
-      const Grid gr = warp_grid(c, ~(size_t)0 >> 8);
-      launch_k(k_expert_quant_push<InT, WireT, true>, gr.blocks, gr.threads, st, c->dev, in, static_cast<char*>(nullptr), static_cast<char*>(nullptr),
-               arena_off(c, recv), arena_off(c, recv_scales), route, (uint32_t)top_k, vpr, nvec, (uint32_t)recv_rows, lvpb, (uint32_t)b200collOpAllToAll);
-    } else {
-      launch_k(k_expert_quant_push<InT, WireT, false>, copy_blocks(c, nvec), 256, st, c->dev, in, static_cast<char*>(recv), reinterpret_cast<char*>(recv_scales),
-               (size_t)0, (size_t)0, route, (uint32_t)top_k, vpr, nvec, (uint32_t)recv_rows, lvpb, (uint32_t)b200collOpAllToAll);
-    }
-    LAUNCH_CHECK(c);
-    return b200collSuccess;
-  });
+  }); }); });
 }
 
 }  // namespace b200coll
@@ -778,13 +464,13 @@ b200collResult_t b200collAllGatherBlockScaled(const void* send, void* recv, size
   rc = cross_check(c, b200collOpAllGather, b200collAlgoOneShot, sendcount, k.g.data_off, k.g.scale_off);
   if (rc != b200collSuccess) return rc;
   account(c, b200collOpAllGather, sendcount, b200collAlgoOneShot);
-  return dispatch_wire_out(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
+  return with_fp8(ep->in_dtype, [&](auto ti) { return with_wide(ep->out_dtype, [&](auto to) -> b200collResult_t {
     using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
     const Grid gr = warp_grid(c, k.g.nvec);
     launch_k(k_bsq_ag_pull<InT, OutT>, gr.blocks, gr.threads, st, c->dev, k.g, static_cast<OutT*>(recv), k.scale, (uint32_t)b200collOpAllGather);
     LAUNCH_CHECK(c);
     return b200collSuccess;
-  });
+  }); });
 }
 
 b200collResult_t b200collReduceScatterBlockScaled(const void* send, void* recv, size_t recvcount, const b200collBlockScale* bs, const b200collEpilogue* ep,
@@ -826,14 +512,14 @@ b200collResult_t b200collAllGatherQuantized(const void* send, void* recv, size_t
   rc = cross_check(c, b200collOpAllGather, b200collAlgoOneShot, sendcount, k.g.data_off, k.g.scale_off);
   if (rc != b200collSuccess) return rc;
   account(c, b200collOpAllGather, k.in_bytes, b200collAlgoOneShot);
-  return dispatch_quant(ep->in_dtype, wire_dtype, ep->out_dtype, [&](auto ti, auto tw, auto to) -> b200collResult_t {
+  return with_wide(ep->in_dtype, [&](auto ti) { return with_fp8(wire_dtype, [&](auto tw) { return with_wide(ep->out_dtype, [&](auto to) -> b200collResult_t {
     using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type; using OutT = typename decltype(to)::type;
     const Grid gr = warp_grid(c, k.g.nvec);
     launch_k(k_quant_ag<InT, WireT, OutT>, gr.blocks, gr.threads, st, c->dev, k.g, static_cast<const char*>(send), static_cast<OutT*>(recv), k.scale,
              (uint32_t)b200collOpAllGather);
     LAUNCH_CHECK(c);
     return b200collSuccess;
-  });
+  }); }); });
 }
 
 b200collResult_t b200collReduceScatterQuantized(const void* send, void* recv, size_t recvcount, b200collDataType_t wire_dtype, int block,
@@ -865,50 +551,6 @@ b200collResult_t b200collAllReduceQuantized(const void* send, void* recv, size_t
   if (rc != b200collSuccess) return rc;
   account(c, b200collOpAllReduce, k.in_bytes, algo);
   return quant_reduce(k, b200collOpAllReduce, algo, send, recv, wire_dtype, ep, st);
-}
-
-b200collResult_t b200collAllToAllvQuantized(const void* send, void* recv, float* recv_scales, size_t row_elems, size_t recv_rows,
-                                            const int64_t* send_rows, const int64_t* send_row_off, const int64_t* recv_row_off_at_peer,
-                                            b200collDataType_t in_dtype, b200collDataType_t wire_dtype, int block,
-                                            b200collComm_t c, b200collStream_t stream) {
-  A2AvArgs a = {};
-  unsigned long long nv[kMaxRanks] = {};
-  size_t in_bytes = 0;
-  b200collResult_t rc = a2aq_prepare(c, send, recv, recv_scales, row_elems, recv_rows, send_rows, send_row_off, recv_row_off_at_peer, in_dtype, wire_dtype,
-                                     block, &a, nv, &in_bytes);
-  if (rc != b200collSuccess) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  uint32_t lvpb = 0;
-  while ((16u << lvpb) < (uint32_t)block) lvpb++;
-  if (c->nranks == 1) {
-    account(c, b200collOpAllToAll, in_bytes, b200collAlgoCopy);
-    if (nv[0] == 0) return b200collSuccess;
-    QuantGeom g = {};
-    g.nvec = (uint32_t)nv[0];
-    g.lvpb = lvpb;
-    const char* in = static_cast<const char*>(send) + a.src_vec[0] * 16 * b200collTypeSize(in_dtype);
-    char* q = static_cast<char*>(recv) + a.dst_vec[0] * 16;
-    char* s = reinterpret_cast<char*>(recv_scales) + (a.dst_vec[0] >> lvpb) * 4;
-    return dispatch_in_wire(in_dtype, wire_dtype, [&](auto ti, auto tw) -> b200collResult_t {
-      using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type;
-      launch_k(k_a2av_quant_copy<InT, WireT>, copy_blocks(c, g.nvec), 256, st, g, in, q, s);
-      LAUNCH_CHECK(c);
-      return b200collSuccess;
-    });
-  }
-  rc = cross_check(c, b200collOpAllToAll, b200collAlgoTwoShot, recv_rows, arena_off(c, recv), arena_off(c, recv_scales));
-  if (rc != b200collSuccess) return rc;
-  a2av_prefix(c->rank, c->nranks, nv, &a);
-  account(c, b200collOpAllToAll, in_bytes, b200collAlgoTwoShot);
-  // the full P2P grid on every rank, whatever it sends: CTA b meets CTA b of every peer in the barriers (see a2av_launch)
-  const Grid gr = warp_grid(c, ~(size_t)0 >> 8);
-  return dispatch_in_wire(in_dtype, wire_dtype, [&](auto ti, auto tw) -> b200collResult_t {
-    using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type;
-    launch_k(k_a2av_quant_push<InT, WireT>, gr.blocks, gr.threads, st, c->dev, static_cast<const char*>(send), arena_off(c, recv), arena_off(c, recv_scales), a,
-             lvpb, (uint32_t)b200collOpAllToAll);
-    LAUNCH_CHECK(c);
-    return b200collSuccess;
-  });
 }
 
 }  // extern "C"

@@ -20,8 +20,6 @@ using bf16 = __nv_bfloat16;
 using f8 = __nv_fp8_e4m3;
 using e5m2 = __nv_fp8_e5m2;
 
-static bool is_fp8(b200collDataType_t t) { return t == b200collFloat8e4m3 || t == b200collFloat8e5m2; }
-
 // Supported (in, out) pairs: same type, widen to f32, narrow f32 to 16-bit, quantise to e4m3 / e5m2; FP8 in, FP8 or 16-bit out
 // (FP8 -> f32 would need a 64-byte store per input vector and is refused).
 template <typename F>

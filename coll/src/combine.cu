@@ -1,22 +1,22 @@
 // libb200coll expert combine: the reverse of the all-to-all-v dispatch with the top-k weighted sum fused, one kernel per call.
 //
-//   k_a2av_combine_pull<InT, OutT>    barrier, pull each token's top_k expert rows from the peers' expert_out, sum in slot order in
+//   k_combine_pull<InT, OutT, Map>    barrier, pull each token's top_k expert rows from the peers' expert_out, sum in slot order in
 //                                     fp32, round once, store locally, barrier
-//   k_a2av_combine_local<InT, OutT>   one rank: the same gather and sum from a local expert_out, no barrier
-//   k_routed_combine_pull / _local    b200collExpertCombine: the same two, each slot's (peer, row) read from the device route that
-//                                     b200collExpertDispatch wrote (RouteMap) instead of the segment table
+//   k_combine_local<InT, OutT, Map>   one rank: the same gather and sum from a local expert_out, no barrier
+//
+// Map names the expert_out row of a slot: SegmentMap for b200collAllToAllvCombine, RouteMap for b200collExpertCombine.
 //
 // Each rank walks (token, 16-element vector) pairs of its own out. For slot j of token t, index[t, j] is a row of the dispatch send
 // buffer; the segment table (A2AvRows, the rows of the dispatch call) maps it to (peer p, row of p's expert_out). A row in no segment
 // is a dropped slot. So every load lies inside a destination range [dst_row[p], + rows[p]) of a peer, which the host has checked against
-// recv_rows: whatever the device-side index holds, the kernel reads nothing else.
+// recv_rows: whatever the device-side index holds, the kernel reads nothing else. b200collExpertCombine reads each slot's (peer, row)
+// from the device route that b200collExpertDispatch wrote instead, and any route outside [0, nranks * recv_rows) is a dropped slot.
 //
 // Per thread, up to kSlots slots are loaded before the first of them is added, so several NVLink (or HBM) reads are in flight; the adds
 // then run in slot order, acc = (acc + w_j * y_j) with both roundings kept, so the batching does not change the result.
 #include <stdint.h>
 
 #include <algorithm>
-#include <type_traits>
 #include <vector>
 
 #include "a2av.h"
@@ -25,46 +25,28 @@
 
 namespace b200coll {
 
-using bf16 = __nv_bfloat16;
-
 constexpr int kCombineThreads = 512;
 
 // The (peer, expert_out row) of dispatch row i, or false when i names no dispatch row. The host refuses overlapping send ranges, so at
-// most one segment matches.
-__device__ __forceinline__ bool combine_row(const A2AvRows& g, int nranks, int32_t i, int* peer, unsigned long long* row) {
-  bool hit = false;
+// most one segment matches. The one-rank kernel passes nranks = 1, so the loop folds to one compare.
+struct SegmentMap {
+  A2AvRows g;
+  __device__ __forceinline__ bool operator()(int32_t i, int nranks, int* peer, unsigned long long* row) const {
+    bool hit = false;
 #pragma unroll
-  for (int q = 0; q < kMaxRanks; q++) {
-    const unsigned long long d = (unsigned long long)((long long)i - (long long)g.src_row[q]);     // negative -> huge -> no match
-    if (q < nranks && d < g.rows[q]) { *peer = q; *row = g.dst_row[q] + d; hit = true; }
-  }
-  return hit;
-}
-
-// 16 elements of InT held as sizeof(InT) 16-byte words, widened (exactly) to fp32
-template <typename InT> __device__ __forceinline__ void combine_widen(const uint4* raw, float* x) {
-#pragma unroll
-  for (int k = 0; k < (int)sizeof(InT); k++) {
-    const uint32_t w[4] = {raw[k].x, raw[k].y, raw[k].z, raw[k].w};
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      if constexpr (std::is_same<InT, float>::value) {
-        x[4 * k + i] = __uint_as_float(w[i]);
-      } else if constexpr (std::is_same<InT, bf16>::value) {
-        x[8 * k + 2 * i] = __uint_as_float(w[i] << 16); x[8 * k + 2 * i + 1] = __uint_as_float(w[i] & 0xFFFF0000u);
-      } else {
-        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
-        x[8 * k + 2 * i] = f.x; x[8 * k + 2 * i + 1] = f.y;
-      }
+    for (int q = 0; q < kMaxRanks; q++) {
+      const unsigned long long d = (unsigned long long)((long long)i - (long long)g.src_row[q]);     // negative -> huge -> no match
+      if (q < nranks && d < g.rows[q]) { *peer = q; *row = g.dst_row[q] + d; hit = true; }
     }
+    return hit;
   }
-}
+};
 
 // The (peer, expert_out row) of a route written by b200collExpertDispatch (peer * recv_rows + row), or false for any value outside
 // [0, limit), limit = nranks * recv_rows <= 2^31 - 1 (the host checks it): negative values are >= 2^31 as unsigned.
 struct RouteMap {
   uint32_t limit, recv_rows;
-  __device__ __forceinline__ bool operator()(int32_t i, int* peer, unsigned long long* row) const {
+  __device__ __forceinline__ bool operator()(int32_t i, int, int* peer, unsigned long long* row) const {
     if ((uint32_t)i >= limit) return false;
     const uint32_t p = (uint32_t)i / recv_rows;
     *peer = (int)p;
@@ -113,7 +95,7 @@ __device__ __forceinline__ void combine_range(Map&& map, Base&& base, const int3
       for (int b = 0; b < kSlots; b++) {
         if (!hit[b]) continue;
         float x[16];
-        combine_widen<InT>(raw[b], x);
+        widen16<InT>(raw[b], x);
 #pragma unroll
         for (int e = 0; e < 16; e++) acc[e] = __fadd_rn(acc[e], __fmul_rn(w[b], x[e]));
       }
@@ -122,23 +104,20 @@ __device__ __forceinline__ void combine_range(Map&& map, Base&& base, const int3
   }
 }
 
-// The grid is the full P2P shape on every rank, whatever its tokens (see b200collAllToAllvCombine). The epoch barrier pairs CTA b of
-// this rank with CTA b of every peer and nothing else; each rank knows only its own tokens, so a grid sized to them would differ from
-// rank to rank, and a CTA missing on one rank would leave CTA b of its peers waiting. With one grid everywhere, the first barrier
-// (relaxed: expert_out was written by earlier kernels on each peer's stream) means every peer's expert_out is complete before any CTA
-// pulls, and the closing barrier means no rank's kernel ends before every CTA of every peer has finished its pulls, so the caller may
-// overwrite expert_out right after the call on its own stream. CTAs with no vectors take only the two barriers.
-template <typename InT, typename OutT>
-__global__ void __launch_bounds__(kCombineThreads, 1) k_a2av_combine_pull(COMM_PARAM, size_t eo_off, const __grid_constant__ A2AvRows g,
-                                                                          const int32_t* __restrict__ index, const float* __restrict__ weights,
-                                                                          OutT* __restrict__ out, uint32_t tokens, uint32_t top_k, uint32_t vpr,
-                                                                          float scale, uint32_t op) {
+// Launched on full_grid. The first barrier (relaxed: expert_out was written by earlier kernels on each peer's stream) means every
+// peer's expert_out is complete before any CTA pulls, and the closing barrier means no rank's kernel ends before every CTA of every
+// peer has finished its pulls, so the caller may overwrite expert_out right after the call on its own stream.
+template <typename InT, typename OutT, typename Map>
+__global__ void __launch_bounds__(kCombineThreads, 1) k_combine_pull(COMM_PARAM, size_t eo_off, const __grid_constant__ Map m,
+                                                                     const int32_t* __restrict__ index, const float* __restrict__ weights,
+                                                                     OutT* __restrict__ out, uint32_t tokens, uint32_t top_k, uint32_t vpr,
+                                                                     float scale, uint32_t op) {
   pdl_prologue();
   {
     const uint32_t s = load_seq(c, kSeqBarrier);
     if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every peer's expert_out is written
   }
-  combine_range<InT, OutT>([&](int32_t i, int* p, unsigned long long* row) { return combine_row(g, c.nranks, i, p, row); },
+  combine_range<InT, OutT>([&](int32_t i, int* p, unsigned long long* row) { return m(i, c.nranks, p, row); },
                            [&](int p) -> const char* { return c.peer[p] + eo_off; }, index, weights, out, tokens, top_k, vpr, scale);
   // the sequence number is read again rather than kept live across the loop: only the last block, after the barrier below, bumps it
   const uint32_t s = load_seq(c, kSeqBarrier);
@@ -146,66 +125,23 @@ __global__ void __launch_bounds__(kCombineThreads, 1) k_a2av_combine_pull(COMM_P
   if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
 }
 
-template <typename InT, typename OutT>
-__global__ void __launch_bounds__(kCombineThreads, 1) k_a2av_combine_local(const __grid_constant__ A2AvRows g, const char* __restrict__ expert_out,
-                                                                           const int32_t* __restrict__ index, const float* __restrict__ weights,
-                                                                           OutT* __restrict__ out, uint32_t tokens, uint32_t top_k, uint32_t vpr,
-                                                                           float scale) {
+// m is a plain parameter here, not __grid_constant__: the compiler then keeps a RouteMap's two fields in registers across the loop.
+template <typename InT, typename OutT, typename Map>
+__global__ void __launch_bounds__(kCombineThreads, 1) k_combine_local(const Map m, const char* __restrict__ expert_out,
+                                                                      const int32_t* __restrict__ index, const float* __restrict__ weights,
+                                                                      OutT* __restrict__ out, uint32_t tokens, uint32_t top_k, uint32_t vpr,
+                                                                      float scale) {
   pdl_prologue();
-  combine_range<InT, OutT>([&](int32_t i, int* p, unsigned long long* row) { return combine_row(g, 1, i, p, row); },
+  combine_range<InT, OutT>([&](int32_t i, int* p, unsigned long long* row) { return m(i, 1, p, row); },
                            [&](int) { return expert_out; }, index, weights, out, tokens, top_k, vpr, scale);
 }
 
-// The combine of b200collExpertCombine: the same kernels with the slot's (peer, row) taken from the dispatch's device route. The
-// barriers and the grid follow k_a2av_combine_pull, for the same reasons.
-template <typename InT, typename OutT>
-__global__ void __launch_bounds__(kCombineThreads, 1) k_routed_combine_pull(COMM_PARAM, size_t eo_off, RouteMap m, const int32_t* __restrict__ route,
-                                                                            const float* __restrict__ weights, OutT* __restrict__ out, uint32_t tokens,
-                                                                            uint32_t top_k, uint32_t vpr, float scale, uint32_t op) {
-  pdl_prologue();
-  {
-    const uint32_t s = load_seq(c, kSeqBarrier);
-    if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every peer's expert_out is written
-  }
-  combine_range<InT, OutT>(m, [&](int p) -> const char* { return c.peer[p] + eo_off; }, route, weights, out, tokens, top_k, vpr, scale);
-  const uint32_t s = load_seq(c, kSeqBarrier);
-  if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // nobody reads my expert_out any more: the caller may overwrite it
-  if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
-}
-
-template <typename InT, typename OutT>
-__global__ void __launch_bounds__(kCombineThreads, 1) k_routed_combine_local(RouteMap m, const char* __restrict__ expert_out, const int32_t* __restrict__ route,
-                                                                             const float* __restrict__ weights, OutT* __restrict__ out, uint32_t tokens,
-                                                                             uint32_t top_k, uint32_t vpr, float scale) {
-  pdl_prologue();
-  combine_range<InT, OutT>(m, [&](int) { return expert_out; }, route, weights, out, tokens, top_k, vpr, scale);
-}
-
 // ------------------------------------------------------------------------------------------------ host side
-static bool combine_type(b200collDataType_t t) { return t == b200collBfloat16 || t == b200collFloat16 || t == b200collFloat32; }
-
-// (in, out) -> f(Tag<InT>, Tag<OutT>); the argument checks have refused every other type
-template <typename F>
-static b200collResult_t dispatch_combine(b200collDataType_t in, b200collDataType_t out, F&& f) {
-  auto outs = [&](auto ti) -> b200collResult_t {
-    switch (out) {
-      case b200collBfloat16: return f(ti, Tag<bf16>{});
-      case b200collFloat16: return f(ti, Tag<__half>{});
-      default: return f(ti, Tag<float>{});
-    }
-  };
-  switch (in) {
-    case b200collBfloat16: return outs(Tag<bf16>{});
-    case b200collFloat16: return outs(Tag<__half>{});
-    default: return outs(Tag<float>{});
-  }
-}
-
 // The argument rules both combines share, after their null checks ("" or why the call is refused); max_rows bounds recv_rows so that
 // every byte offset fits in size_t with room to spare. `index` is the index (b200collAllToAllvCombine) or the route (b200collExpertCombine).
 static std::string combine_shape(const void* expert_out, const void* out, size_t row_elems, size_t recv_rows, const int32_t* index, const float* weights,
                                  size_t tokens, int top_k, const b200collEpilogue* ep, const char* index_name, size_t* max_rows) {
-  if (!combine_type(ep->in_dtype) || !combine_type(ep->out_dtype)) return "in_dtype and out_dtype must be bf16, fp16 or fp32";
+  if (!wide_type(ep->in_dtype) || !wide_type(ep->out_dtype)) return "in_dtype and out_dtype must be bf16, fp16 or fp32";
   if (row_elems == 0 || row_elems % 16 != 0) return "row_elems must be a positive multiple of 16";
   if (top_k < 1) return "top_k must be at least 1";
   if (!aligned(expert_out, 16) || !aligned(out, 16)) return "expert_out and out must be 16-byte aligned";
@@ -230,12 +166,21 @@ static b200collResult_t combine_place(b200collComm* c, const void* expert_out, v
     return b200collInvalidArgument;
   }
   if (comm_poisoned(c)) return b200collRemoteError;
-  // peers pull from my expert_out at MY arena offset: it must be arena memory
-  if (c->nranks > 1 && !b200collIsSymmetric(c, expert_out, std::max<size_t>(eo_bytes, 1))) {
-    set_last_error(std::string(what) + ": expert_out must lie in the symmetric arena (b200collMemAlloc), at the same offset on every rank");
-    return b200collInvalidUsage;
+  // peers pull from my expert_out
+  if (c->nranks == 1) return b200collSuccess;
+  return in_arena(c, std::string(what) + ": ", "expert_out", {{expert_out, eo_bytes}});
+}
+
+// The stats of both combines, as copy with one rank; with more, oneshot after the B200COLL_CHECK=1 cross-check of recv_rows and the
+// expert_out offset.
+static b200collResult_t combine_account(b200collComm* c, size_t recv_rows, const void* expert_out, size_t bytes) {
+  if (c->nranks == 1) {
+    account(c, b200collOpAllToAll, bytes, b200collAlgoCopy);
+    return b200collSuccess;
   }
-  return b200collSuccess;
+  const b200collResult_t rc = cross_check(c, b200collOpAllToAll, b200collAlgoOneShot, recv_rows, arena_off(c, expert_out), 0);
+  if (rc == b200collSuccess) account(c, b200collOpAllToAll, bytes, b200collAlgoOneShot);
+  return rc;
 }
 
 // Everything b200collAllToAllvCombine checks before it launches; on success `g` holds the segment table and `in_bytes` the bytes of
@@ -263,29 +208,26 @@ static b200collResult_t combine_prepare(b200collComm* c, const void* expert_out,
   return combine_place(c, expert_out, out, row_elems, recv_rows, index, weights, tokens, top_k, ep, "all-to-all-v combine", "index");
 }
 
-// (in, out) -> one launch of k_routed_combine_pull (more than one rank) or k_routed_combine_local
-static b200collResult_t routed_combine_launch(b200collComm* c, const void* expert_out, void* out, size_t row_elems, size_t recv_rows, const int32_t* route,
-                                              const float* weights, size_t tokens, int top_k, const b200collEpilogue* ep, cudaStream_t st) {
+// (in, out) -> one launch of k_combine_pull (more than one rank) or k_combine_local
+template <typename Map>
+static b200collResult_t combine_launch(b200collComm* c, const Map& m, const void* expert_out, void* out, size_t row_elems, const int32_t* index,
+                                       const float* weights, size_t tokens, int top_k, const b200collEpilogue* ep, cudaStream_t st) {
   const uint32_t vpr = (uint32_t)(row_elems / 16), nvec = (uint32_t)(tokens * vpr);
-  const RouteMap m{(uint32_t)(c->nranks * recv_rows), (uint32_t)recv_rows};
-  if (c->nranks == 1) {
-    const int blocks = (int)std::max<size_t>(1, std::min<size_t>(((size_t)nvec + kCombineThreads - 1) / kCombineThreads, (size_t)std::max(1, c->sm_count)));
-    return dispatch_combine(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
-      using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
-      launch_k(k_routed_combine_local<InT, OutT>, blocks, kCombineThreads, st, m, static_cast<const char*>(expert_out), route, weights, static_cast<OutT*>(out),
-               (uint32_t)tokens, (uint32_t)top_k, vpr, ep->scale);
-      LAUNCH_CHECK(c);
-      return b200collSuccess;
-    });
-  }
-  const Grid gr = pick_grid(c, kShapeP2p, ~(size_t)0 >> 8, 1);     // the full P2P grid on every rank, as in b200collAllToAllvCombine
-  return dispatch_combine(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
+  const bool peers = c->nranks > 1;
+  const Grid gr = peers ? full_grid(c, 1)
+                        : Grid{(int)std::max<size_t>(1, std::min<size_t>(((size_t)nvec + kCombineThreads - 1) / kCombineThreads, (size_t)std::max(1, c->sm_count))),
+                               kCombineThreads};
+  return with_wide(ep->in_dtype, [&](auto ti) { return with_wide(ep->out_dtype, [&](auto to) -> b200collResult_t {
     using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
-    launch_k(k_routed_combine_pull<InT, OutT>, gr.blocks, gr.threads, st, c->dev, arena_off(c, expert_out), m, route, weights, static_cast<OutT*>(out),
-             (uint32_t)tokens, (uint32_t)top_k, vpr, ep->scale, (uint32_t)b200collOpAllToAll);
+    if (peers)
+      launch_k(k_combine_pull<InT, OutT, Map>, gr.blocks, gr.threads, st, c->dev, arena_off(c, expert_out), m, index, weights, static_cast<OutT*>(out),
+               (uint32_t)tokens, (uint32_t)top_k, vpr, ep->scale, (uint32_t)b200collOpAllToAll);
+    else
+      launch_k(k_combine_local<InT, OutT, Map>, gr.blocks, gr.threads, st, m, static_cast<const char*>(expert_out), index, weights, static_cast<OutT*>(out),
+               (uint32_t)tokens, (uint32_t)top_k, vpr, ep->scale);
     LAUNCH_CHECK(c);
     return b200collSuccess;
-  });
+  }); });
 }
 
 }  // namespace b200coll
@@ -303,31 +245,8 @@ b200collResult_t b200collAllToAllvCombine(const void* expert_out, void* out, siz
   b200collResult_t rc = combine_prepare(c, expert_out, out, row_elems, recv_rows, send_rows, send_row_off, recv_row_off_at_peer, index, weights, tokens,
                                         top_k, ep, &g, &in_bytes);
   if (rc != b200collSuccess) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const uint32_t vpr = (uint32_t)(row_elems / 16), nvec = (uint32_t)(tokens * vpr);
-  if (c->nranks == 1) {
-    account(c, b200collOpAllToAll, in_bytes, b200collAlgoCopy);
-    const int blocks = (int)std::max<size_t>(1, std::min<size_t>(((size_t)nvec + kCombineThreads - 1) / kCombineThreads, (size_t)std::max(1, c->sm_count)));
-    return dispatch_combine(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
-      using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
-      launch_k(k_a2av_combine_local<InT, OutT>, blocks, kCombineThreads, st, g, static_cast<const char*>(expert_out), index, weights, static_cast<OutT*>(out),
-               (uint32_t)tokens, (uint32_t)top_k, vpr, ep->scale);
-      LAUNCH_CHECK(c);
-      return b200collSuccess;
-    });
-  }
-  rc = cross_check(c, b200collOpAllToAll, b200collAlgoOneShot, recv_rows, arena_off(c, expert_out), 0);
-  if (rc != b200collSuccess) return rc;
-  account(c, b200collOpAllToAll, in_bytes, b200collAlgoOneShot);
-  // the full P2P grid on every rank, whatever its tokens: CTA b meets CTA b of every peer in both barriers (see k_a2av_combine_pull)
-  const Grid gr = pick_grid(c, kShapeP2p, ~(size_t)0 >> 8, 1);
-  return dispatch_combine(ep->in_dtype, ep->out_dtype, [&](auto ti, auto to) -> b200collResult_t {
-    using InT = typename decltype(ti)::type; using OutT = typename decltype(to)::type;
-    launch_k(k_a2av_combine_pull<InT, OutT>, gr.blocks, gr.threads, st, c->dev, arena_off(c, expert_out), g, index, weights, static_cast<OutT*>(out),
-             (uint32_t)tokens, (uint32_t)top_k, vpr, ep->scale, (uint32_t)b200collOpAllToAll);
-    LAUNCH_CHECK(c);
-    return b200collSuccess;
-  });
+  if ((rc = combine_account(c, recv_rows, expert_out, in_bytes)) != b200collSuccess) return rc;
+  return combine_launch(c, SegmentMap{g}, expert_out, out, row_elems, index, weights, tokens, top_k, ep, static_cast<cudaStream_t>(stream));
 }
 
 b200collResult_t b200collExpertCombine(const void* expert_out, void* out, size_t row_elems, size_t recv_rows, const int32_t* route,
@@ -341,16 +260,10 @@ b200collResult_t b200collExpertCombine(const void* expert_out, void* out, size_t
   if (recv_rows > (((size_t)1 << 31) - 1) / (size_t)c->nranks) return refuse("nranks * recv_rows must be at most 2^31 - 1 (a route is an int32)");
   b200collResult_t rc = combine_place(c, expert_out, out, row_elems, recv_rows, route, weights, tokens, top_k, ep, "expert combine", "route");
   if (rc != b200collSuccess) return rc;
-  const size_t offered = tokens * (size_t)top_k * row_elems * b200collTypeSize(ep->in_dtype);
-  if (c->nranks == 1) {
-    account(c, b200collOpAllToAll, offered, b200collAlgoCopy);
-  } else {
-    rc = cross_check(c, b200collOpAllToAll, b200collAlgoOneShot, recv_rows, arena_off(c, expert_out), 0);
-    if (rc != b200collSuccess) return rc;
-    account(c, b200collOpAllToAll, offered, b200collAlgoOneShot);
-  }
+  if ((rc = combine_account(c, recv_rows, expert_out, tokens * (size_t)top_k * row_elems * b200collTypeSize(ep->in_dtype))) != b200collSuccess) return rc;
   const DeviceScope on_device(c->device);
-  return routed_combine_launch(c, expert_out, out, row_elems, recv_rows, route, weights, tokens, top_k, ep, static_cast<cudaStream_t>(stream));
+  const RouteMap m{(uint32_t)(c->nranks * recv_rows), (uint32_t)recv_rows};
+  return combine_launch(c, m, expert_out, out, row_elems, route, weights, tokens, top_k, ep, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

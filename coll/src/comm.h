@@ -136,10 +136,4 @@ void hostpath_destroy(b200collComm* c);
 // collectives.cu
 b200collResult_t launch_fill_sentinel(b200collComm* c, cudaStream_t s);
 
-// blockscaled.cu: the push kernel of the routed FP8 dispatch (k_expert_quant_push), launched by routed.cu after the layout kernel on
-// arguments it has checked, and the load of all its instantiations (routed.cu does it once per device, before any layout launch)
-b200collResult_t launch_expert_quant_push(b200collComm* c, const void* x, void* recv, float* recv_scales, const int32_t* route, size_t tokens, int top_k,
-                                          size_t row_elems, size_t recv_rows, b200collDataType_t in_dtype, b200collDataType_t wire, int block, cudaStream_t st);
-void load_expert_quant_push();
-
 }  // namespace b200coll

@@ -12,6 +12,9 @@
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
 #include <stdint.h>
+
+#include <type_traits>
+
 #include "../include/b200coll.h"
 #include "layout.h"
 
@@ -195,6 +198,26 @@ template <__nv_fp8_interpretation_t I> __device__ __forceinline__ void unpack_ad
 }
 template <> __device__ __forceinline__ void unpack_add<__nv_fp8_e4m3>(float* acc, const uint4& v) { unpack_add_fp8<__NV_E4M3>(acc, v); }
 template <> __device__ __forceinline__ void unpack_add<__nv_fp8_e5m2>(float* acc, const uint4& v) { unpack_add_fp8<__NV_E5M2>(acc, v); }
+
+// 16 elements of a bf16, fp16 or fp32 row held as sizeof(InT) 16-byte words, widened to fp32 bit for bit: -0 stays -0 and NaN payloads
+// survive (unpack_add on zeros would turn -0 into +0, which the quantiser would then store as FP8 +0).
+template <typename InT> __device__ __forceinline__ void widen16(const uint4* raw, float* x) {
+#pragma unroll
+  for (int k = 0; k < (int)sizeof(InT); k++) {
+    const uint32_t w[4] = {raw[k].x, raw[k].y, raw[k].z, raw[k].w};
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      if constexpr (std::is_same<InT, float>::value) {
+        x[4 * k + i] = __uint_as_float(w[i]);
+      } else if constexpr (std::is_same<InT, __nv_bfloat16>::value) {
+        x[8 * k + 2 * i] = __uint_as_float(w[i] << 16); x[8 * k + 2 * i + 1] = __uint_as_float(w[i] & 0xFFFF0000u);
+      } else {
+        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
+        x[8 * k + 2 * i] = f.x; x[8 * k + 2 * i + 1] = f.y;
+      }
+    }
+  }
+}
 
 // pack E floats into E*sizeof(OutT)/4 words
 template <typename OutT, int E> struct Pack;

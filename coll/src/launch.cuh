@@ -1,11 +1,13 @@
-// Host-side launch helpers shared by the collective entry points (collectives.cu, generic.cu, and blockscaled.cu for the block-scaled
-// and quantising FP8 collectives): kernel launch through cudaLaunchKernelEx with optional programmatic dependent launch, the
-// launch-shape picker, argument and communicator checks, the type tag, and call accounting.
+// Host-side launch helpers shared by the collective entry points (collectives.cu, generic.cu, blockscaled.cu, combine.cu and
+// dispatch.cu): kernel launch through cudaLaunchKernelEx with optional programmatic dependent launch, the launch-shape pickers,
+// argument, placement and communicator checks, the type dispatch, and call accounting.
 #pragma once
 #include <stdlib.h>
 
 #include <algorithm>
+#include <initializer_list>
 #include <string>
+#include <utility>
 
 #include "comm.h"
 
@@ -89,6 +91,36 @@ inline Grid pick_grid(const b200collComm* c, int kind, size_t vecs, int unroll) 
   return Grid{1, 128};
 }
 
+// Whole warps: WarpScale and the amax butterfly are full-mask warp intrinsics, and pick_grid takes a forced thread count as given.
+inline Grid warp_grid(const b200collComm* c, size_t vecs) {
+  Grid gr = pick_grid(c, kShapeP2p, vecs, 1);
+  gr.threads = std::max(32, gr.threads & ~31);
+  return gr;
+}
+
+// The grid of every all-to-all kernel with a closing barrier: the full P2P shape of the communicator, whatever this rank's work. The
+// epoch barrier pairs CTA b of this rank with CTA b of every peer and nothing else, and each rank knows only its own rows or tokens, so
+// a grid sized to them would differ from rank to rank, and a CTA missing on one rank would leave CTA b of its peers waiting. CTAs
+// without work take only the barriers. `warps`: whole warps, for the kernels that walk with warp_walk.
+inline Grid full_grid(const b200collComm* c, int unroll, bool warps = false) {
+  return warps ? warp_grid(c, ~(size_t)0 >> 8) : pick_grid(c, kShapeP2p, ~(size_t)0 >> 8, unroll);
+}
+
+// nranks == 1: no peers, no barrier; grid as for the fused copy (streaming, 8 CTAs of 256 threads per SM at most)
+inline int copy_blocks(const b200collComm* c, uint32_t nvec) {
+  return (int)std::max<size_t>(1, std::min<size_t>(((size_t)nvec + 255) / 256, (size_t)std::max(1, c->sm_count) * 8));
+}
+
+// The quantising block: a power of two from 16 to 512 elements, so 1 to 32 16-element vectors. Returns log2(vectors per block), or
+// -1 (and the caller refuses with kBlockRule) for any other block.
+constexpr const char* kBlockRule = "block must be 16, 32, 64, 128, 256 or 512";
+inline int quant_lvpb(int block) {
+  if (block < 16 || block > 512 || (block & (block - 1)) != 0) return -1;
+  int l = 0;
+  while ((16 << l) < block) l++;
+  return l;
+}
+
 // Makes the communicator's GPU current while it lives and restores the caller's: a process may drive communicators on several GPUs,
 // and a launch onto a stream of another device than the current one fails (after the peers' kernels are already waiting for it).
 struct DeviceScope {
@@ -112,8 +144,32 @@ inline bool comm_poisoned(const b200collComm* c) {
   return true;
 }
 
-// type dispatch: f(Tag<InT>{}, Tag<OutT>{}) instantiates a launch for the element types
+// Peers read or write these buffers at MY arena offsets, so each must be arena memory: InvalidUsage (with `who`, the entry point's
+// message prefix) when one is not. A zero-length buffer is checked as one byte.
+inline b200collResult_t in_arena(b200collComm* c, const std::string& who, const char* names, std::initializer_list<std::pair<const void*, size_t>> bufs) {
+  for (const auto& b : bufs) {
+    if (b200collIsSymmetric(c, b.first, std::max<size_t>(b.second, 1))) continue;
+    set_last_error(who + names + " must lie in the symmetric arena (b200collMemAlloc), at the same offset" + (bufs.size() > 1 ? "s" : "") + " on every rank");
+    return b200collInvalidUsage;
+  }
+  return b200collSuccess;
+}
+
+// type dispatch: f(Tag<T>{}) instantiates a launch for an element type; nest one per template parameter. The argument checks have
+// refused every other type, so the last case takes what is left.
 template <typename T> struct Tag { using type = T; };
+inline bool wide_type(b200collDataType_t t) { return t == b200collBfloat16 || t == b200collFloat16 || t == b200collFloat32; }
+inline bool is_fp8(b200collDataType_t t) { return t == b200collFloat8e4m3 || t == b200collFloat8e5m2; }
+template <typename F> auto with_wide(b200collDataType_t t, F&& f) {      // bf16, fp16, fp32
+  switch (t) {
+    case b200collBfloat16: return f(Tag<__nv_bfloat16>{});
+    case b200collFloat16: return f(Tag<__half>{});
+    default: return f(Tag<float>{});
+  }
+}
+template <typename F> auto with_fp8(b200collDataType_t t, F&& f) {       // e4m3, e5m2
+  return t == b200collFloat8e4m3 ? f(Tag<__nv_fp8_e4m3>{}) : f(Tag<__nv_fp8_e5m2>{});
+}
 
 // collectives.cu: count a call in the stats (and mark it for NVTX / debug traces); B200COLL_CHECK=1 cross-check of a symmetric launch
 void account(b200collComm* c, b200collOp_t op, size_t bytes, b200collAlgo_t algo);

@@ -36,7 +36,7 @@ constexpr size_t kP2pDoneBytes = (size_t)kMaxRanks * kP2pMaxBlocks * 4;
 static_assert(kOffP2pDone + kP2pDoneBytes <= kOffLL, "p2p mailboxes must fit below the Lamport scratch");
 constexpr int kP2pTagBits = 24, kP2pValueBits = 40;     // each post word = (chunk sequence number mod 2^24) << 40 | value
 
-// Routed expert dispatch (routed.cu): the count mailbox, int32 [source rank][kRouteMaxExperts]. Before the dispatch's exchange barrier
+// Routed expert dispatch (dispatch.cu): the count mailbox, int32 [source rank][kRouteMaxExperts]. Before the dispatch's exchange barrier
 // every rank writes its per-expert slot counts into row [its rank] of every rank's mailbox; after it each rank reads the whole matrix.
 constexpr int kRouteMaxExperts = 1024;
 constexpr size_t kOffRouteCounts = 512 << 10;

@@ -239,6 +239,43 @@ def check_block_scaled(op: str, nranks: int, q, scales, out, block=(1, 128)) -> 
 QUANT_BLOCKS = (16, 32, 64, 128, 256, 512)
 
 
+def _check_wide(name: str, t, rows: bool = False) -> None:
+    """t must be a contiguous bfloat16, float16 or float32 tensor; rows: also 2-D, [tokens, row_elems]."""
+    import torch
+    if t.dtype not in (torch.bfloat16, torch.float16, torch.float32) or not t.is_contiguous() or (rows and t.dim() != 2):
+        raise ValueError(f"{name} must be a contiguous bfloat16, float16 or float32 [tokens, row_elems] tensor, got {t.dtype}{list(t.shape)}" if rows
+                         else f"{name} must be a contiguous bfloat16, float16 or float32 tensor, got {t.dtype}")
+
+
+def _check_block(block) -> None:
+    if isinstance(block, bool) or not isinstance(block, int) or block not in QUANT_BLOCKS:
+        raise ValueError(f"block must be one of {QUANT_BLOCKS}, got {block!r}")
+
+
+def _check_topk(name: str, t) -> None:
+    """t must be a contiguous int32 [tokens, top_k] tensor with top_k >= 1."""
+    import torch
+    if t.dtype != torch.int32 or t.dim() != 2 or not t.is_contiguous() or t.shape[1] < 1:
+        raise ValueError(f"{name} must be a contiguous int32 [tokens, top_k] tensor with top_k >= 1, got {t.dtype}{list(t.shape)}")
+
+
+def _host_rows(nranks: int, send_rows, send_row_off, recv_row_off_at_peer) -> list[tuple[int, int, int]]:
+    """The three host lists of an all-to-all-v call, checked (nranks non-negative integers each): [(rows, send_off, recv_off)] by peer."""
+    import operator
+    vals = []
+    for name, xs in (("send_rows", send_rows), ("send_row_off", send_row_off), ("recv_row_off_at_peer", recv_row_off_at_peer)):
+        try:
+            v = [operator.index(x) for x in xs]
+        except TypeError:
+            raise ValueError(f"{name} must be a sequence of integers") from None
+        if len(v) != nranks:
+            raise ValueError(f"{name} must have nranks = {nranks} entries, got {len(v)}")
+        if any(x < 0 for x in v):
+            raise ValueError(f"{name} must not hold negative entries: {v}")
+        vals.append(v)
+    return list(zip(*vals))
+
+
 def check_quantized(op: str, nranks: int, src, out, block: int = 128, wire=None) -> int:
     """Rules of the quantising collectives ("all_gather", "reduce_scatter", "all_reduce"), checked on the tensors' metadata only (no
     communicator, no library call): raises ValueError, returns the wire type's library code. src and out: contiguous bfloat16, float16
@@ -249,15 +286,11 @@ def check_quantized(op: str, nranks: int, src, out, block: int = 128, wire=None)
     wire = torch.float8_e4m3fn if wire is None else wire
     if op not in ("all_gather", "reduce_scatter", "all_reduce"):
         raise ValueError(f"unknown quantised op {op!r}")
-    wide = (torch.bfloat16, torch.float16, torch.float32)
-    if src.dtype not in wide or not src.is_contiguous():
-        raise ValueError(f"src must be a contiguous bfloat16, float16 or float32 tensor, got {src.dtype}")
-    if out.dtype not in wide or not out.is_contiguous():
-        raise ValueError(f"out must be a contiguous bfloat16, float16 or float32 tensor, got {out.dtype}")
+    _check_wide("src", src)
+    _check_wide("out", out)
     if wire not in (torch.float8_e4m3fn, torch.float8_e5m2):
         raise ValueError(f"wire must be torch.float8_e4m3fn or torch.float8_e5m2, not {wire}")
-    if isinstance(block, bool) or not isinstance(block, int) or block not in QUANT_BLOCKS:
-        raise ValueError(f"block must be one of {QUANT_BLOCKS}, got {block!r}")
+    _check_block(block)
     n = src.numel()
     if op == "reduce_scatter" and n % nranks:
         raise ValueError(f"reduce_scatter: src.numel() ({n}) must be a multiple of nranks ({nranks})")
@@ -283,45 +316,27 @@ def check_all_to_all_v_quantized(nranks: int, src, out, out_scales, row_elems: i
     out.numel() // block elements; block one of QUANT_BLOCKS and row_elems a positive multiple of it. The three lists have nranks
     non-negative entries; every send range [send_row_off[p], + send_rows[p]) lies inside src and every destination range
     [recv_row_off_at_peer[p], + send_rows[p]) inside out, in rows of row_elems elements. src must not overlap out or out_scales."""
-    import operator
-
     import torch
-    if src.dtype not in (torch.bfloat16, torch.float16, torch.float32) or not src.is_contiguous():
-        raise ValueError(f"src must be a contiguous bfloat16, float16 or float32 tensor, got {src.dtype}")
+    _check_wide("src", src)
     if out.dtype not in (torch.float8_e4m3fn, torch.float8_e5m2) or not out.is_contiguous():
         raise ValueError(f"out must be a contiguous float8_e4m3fn or float8_e5m2 tensor (the wire type), got {out.dtype}")
     if out_scales.dtype != torch.float32 or not out_scales.is_contiguous():
         raise ValueError(f"out_scales must be a contiguous float32 tensor, got {out_scales.dtype}")
-    if isinstance(block, bool) or not isinstance(block, int) or block not in QUANT_BLOCKS:
-        raise ValueError(f"block must be one of {QUANT_BLOCKS}, got {block!r}")
+    _check_block(block)
     if isinstance(row_elems, bool) or not isinstance(row_elems, int) or row_elems <= 0 or row_elems % block:
         raise ValueError(f"row_elems must be a positive multiple of block ({block}), got {row_elems!r}")
     if out.numel() % row_elems:
         raise ValueError(f"out.numel() ({out.numel()}) must be a multiple of row_elems ({row_elems})")
     if out_scales.numel() != out.numel() // block:
         raise ValueError(f"out_scales must hold out.numel() // block = {out.numel() // block} floats, got {out_scales.numel()}")
-    lists = {"send_rows": send_rows, "send_row_off": send_row_off, "recv_row_off_at_peer": recv_row_off_at_peer}
-    vals = {}
-    for name, xs in lists.items():
-        try:
-            vals[name] = [operator.index(x) for x in xs]
-        except TypeError:
-            raise ValueError(f"{name} must be a sequence of integers") from None
-        if len(vals[name]) != nranks:
-            raise ValueError(f"{name} must have nranks = {nranks} entries, got {len(vals[name])}")
-        if any(x < 0 for x in vals[name]):
-            raise ValueError(f"{name} must not hold negative entries: {vals[name]}")
     src_rows, out_rows = src.numel() // row_elems, out.numel() // row_elems
-    for p, (rows, so, ro) in enumerate(zip(vals["send_rows"], vals["send_row_off"], vals["recv_row_off_at_peer"])):
+    for p, (rows, so, ro) in enumerate(_host_rows(nranks, send_rows, send_row_off, recv_row_off_at_peer)):
         if so + rows > src_rows:
             raise ValueError(f"peer {p}: send rows [{so}, {so + rows}) lie past the {src_rows} whole rows of src")
         if ro + rows > out_rows:
             raise ValueError(f"peer {p}: destination rows [{ro}, {ro + rows}) lie past the {out_rows} rows of out")
-    a, na = src.data_ptr(), src.numel() * src.element_size()
-    for t in (out, out_scales):
-        b, nb = t.data_ptr(), t.numel() * t.element_size()
-        if na and nb and a < b + nb and b < a + na:
-            raise ValueError("src must not overlap out or out_scales")
+    if _overlap(src, out) or _overlap(src, out_scales):
+        raise ValueError("src must not overlap out or out_scales")
     return torch_dtype_code(src.dtype), torch_dtype_code(out.dtype)
 
 
@@ -333,38 +348,22 @@ def check_all_to_all_v_combine(nranks: int, expert_out, out, row_elems: int, sen
     None or contiguous float32 of index's shape; out.numel() == tokens * row_elems. The three lists have nranks non-negative entries,
     the non-empty send ranges [send_row_off[p], + send_rows[p]) are disjoint, and every destination range [recv_row_off_at_peer[p],
     + send_rows[p]) lies inside expert_out, in rows of row_elems elements. out must not overlap expert_out, index or weights."""
-    import operator
-
     import torch
-    wide = (torch.bfloat16, torch.float16, torch.float32)
-    for name, t in (("expert_out", expert_out), ("out", out)):
-        if t.dtype not in wide or not t.is_contiguous():
-            raise ValueError(f"{name} must be a contiguous bfloat16, float16 or float32 tensor, got {t.dtype}")
+    _check_wide("expert_out", expert_out)
+    _check_wide("out", out)
     if isinstance(row_elems, bool) or not isinstance(row_elems, int) or row_elems <= 0 or row_elems % 16:
         raise ValueError(f"row_elems must be a positive multiple of 16, got {row_elems!r}")
     if expert_out.numel() % row_elems:
         raise ValueError(f"expert_out.numel() ({expert_out.numel()}) must be a multiple of row_elems ({row_elems})")
-    if index.dtype != torch.int32 or index.dim() != 2 or not index.is_contiguous() or index.shape[1] < 1:
-        raise ValueError(f"index must be a contiguous int32 [tokens, top_k] tensor with top_k >= 1, got {index.dtype}{list(index.shape)}")
+    _check_topk("index", index)
     tokens, top_k = index.shape
     if weights is not None and (weights.dtype != torch.float32 or tuple(weights.shape) != (tokens, top_k) or not weights.is_contiguous()):
         raise ValueError(f"weights must be None or a contiguous float32 [{tokens}, {top_k}] tensor, got {weights.dtype}{list(weights.shape)}")
     if out.numel() != tokens * row_elems:
         raise ValueError(f"out must hold tokens * row_elems = {tokens * row_elems} elements, got {out.numel()}")
-    lists = {"send_rows": send_rows, "send_row_off": send_row_off, "recv_row_off_at_peer": recv_row_off_at_peer}
-    vals = {}
-    for name, xs in lists.items():
-        try:
-            vals[name] = [operator.index(x) for x in xs]
-        except TypeError:
-            raise ValueError(f"{name} must be a sequence of integers") from None
-        if len(vals[name]) != nranks:
-            raise ValueError(f"{name} must have nranks = {nranks} entries, got {len(vals[name])}")
-        if any(x < 0 for x in vals[name]):
-            raise ValueError(f"{name} must not hold negative entries: {vals[name]}")
     eo_rows = expert_out.numel() // row_elems
     ranges = []
-    for p, (rows, so, ro) in enumerate(zip(vals["send_rows"], vals["send_row_off"], vals["recv_row_off_at_peer"])):
+    for p, (rows, so, ro) in enumerate(_host_rows(nranks, send_rows, send_row_off, recv_row_off_at_peer)):
         if ro + rows > eo_rows:
             raise ValueError(f"peer {p}: destination rows [{ro}, {ro + rows}) lie past the {eo_rows} rows of expert_out")
         if rows:
@@ -373,12 +372,8 @@ def check_all_to_all_v_combine(nranks: int, expert_out, out, row_elems: int, sen
     for (lo0, hi0, p0), (lo1, hi1, p1) in zip(ranges, ranges[1:]):
         if lo1 < hi0:
             raise ValueError(f"the send ranges of peers {p0} [{lo0}, {hi0}) and {p1} [{lo1}, {hi1}) overlap: a dispatch row must belong to one peer")
-    a, na = out.data_ptr(), out.numel() * out.element_size()
     for name, t in (("expert_out", expert_out), ("index", index), ("weights", weights)):
-        if t is None:
-            continue
-        b, nb = t.data_ptr(), t.numel() * t.element_size()
-        if na and nb and a < b + nb and b < a + na:
+        if t is not None and _overlap(out, t):
             raise ValueError(f"out must not overlap {name}")
     return torch_dtype_code(expert_out.dtype), torch_dtype_code(out.dtype)
 
@@ -400,6 +395,60 @@ def _overlap(t, u) -> bool:
     return bool(na and nb and a < b + nb and b < a + na)
 
 
+def _check_routed(nranks: int, x, topk_idx, num_experts: int, recv, expert_counts, route, dropped, fp8=None) -> None:
+    """The rules of both device-routed dispatches; fp8 is None (check_expert_dispatch) or (recv_scales, block), which adds the FP8
+    call's rules, as routed_prepare in coll/src/dispatch.cu takes a RoutedQuant."""
+    import torch
+    _check_wide("x", x, rows=True)
+    tokens, row_elems = x.shape
+    if fp8 is None:
+        if row_elems <= 0 or row_elems % 16:
+            raise ValueError(f"row_elems (x.shape[1] = {row_elems}) must be a positive multiple of 16")
+    else:
+        recv_scales, block = fp8
+        _check_block(block)
+        if row_elems <= 0 or row_elems % block:
+            raise ValueError(f"row_elems (x.shape[1] = {row_elems}) must be a positive multiple of block ({block})")
+    _check_topk("topk_idx", topk_idx)
+    if topk_idx.shape[0] != tokens:
+        raise ValueError(f"topk_idx has {topk_idx.shape[0]} tokens, x has {tokens}")
+    top_k = topk_idx.shape[1]
+    if isinstance(num_experts, bool) or not isinstance(num_experts, int) or not 1 <= num_experts <= MAX_EXPERTS or num_experts % nranks:
+        raise ValueError(f"num_experts must be an int in [1, {MAX_EXPERTS}] and a multiple of nranks ({nranks}), got {num_experts!r}")
+    inputs = [("topk_idx", topk_idx), ("x", x), ("recv", recv)]
+    if fp8 is None:
+        if recv.dtype != x.dtype or not recv.is_contiguous() or recv.numel() % row_elems:
+            raise ValueError(f"recv must be a contiguous {x.dtype} tensor of whole {row_elems}-element rows, got {recv.dtype} with {recv.numel()} elements")
+    else:
+        if recv.dtype not in (torch.float8_e4m3fn, torch.float8_e5m2) or not recv.is_contiguous() or recv.numel() % row_elems:
+            raise ValueError(f"recv must be a contiguous float8_e4m3fn or float8_e5m2 tensor (the wire type) of whole {row_elems}-element rows, "
+                             f"got {recv.dtype} with {recv.numel()} elements")
+        if recv_scales.dtype != torch.float32 or not recv_scales.is_contiguous() or recv_scales.numel() != recv.numel() // block:
+            raise ValueError(f"recv_scales must be a contiguous float32 tensor of recv.numel() // block = {recv.numel() // block} elements, "
+                             f"got {recv_scales.dtype} with {recv_scales.numel()}")
+        inputs.append(("recv_scales", recv_scales))
+    if tokens * top_k > _I31:
+        raise ValueError(f"tokens * top_k ({tokens * top_k}) must be at most 2^31 - 1")
+    if nranks * (recv.numel() // row_elems) > _I31:
+        raise ValueError("nranks * recv rows must be at most 2^31 - 1 (a route is an int32)")
+    if fp8 is not None and tokens * (row_elems // 16) > _I31:
+        raise ValueError("at most 2^31 - 1 16-element vectors of x (tokens * row_elems / 16)")
+    if tokens * top_k * (row_elems * x.element_size() // 16) > _I31:
+        raise ValueError("at most 2^31 - 1 16-byte vectors may be offered (tokens * top_k * row bytes / 16)")
+    for an, bn in [("recv", "x")] + ([("recv_scales", "x"), ("recv", "recv_scales")] if fp8 is not None else []):
+        if _overlap(dict(inputs)[an], dict(inputs)[bn]):
+            raise ValueError(f"{an} must not overlap {bn}")
+    outs = [(n, t, shape) for n, t, shape in (("expert_counts", expert_counts, (num_experts // nranks,)), ("route", route, (tokens, top_k)),
+                                              ("dropped", dropped, (1,))) if t is not None]
+    for name, t, shape in outs:
+        if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != _numel(shape):
+            raise ValueError(f"{name} must be a contiguous int32 tensor of shape {shape}, got {t.dtype}{list(t.shape)}")
+    for k, (name, t, _) in enumerate(outs):
+        for other, u in [(n, o) for n, o, _ in outs[k + 1:]] + inputs:
+            if _overlap(t, u):
+                raise ValueError(f"{name} must not overlap {other}")
+
+
 def check_expert_dispatch(nranks: int, x, topk_idx, num_experts: int, recv, expert_counts=None, route=None, dropped=None) -> int:
     """Rules of the device-routed expert dispatch, checked on the tensors' metadata only (no communicator, no library call, no device
     read): raises ValueError, returns the library code of x's type. x: contiguous bfloat16, float16 or float32 [tokens, row_elems] with
@@ -407,38 +456,7 @@ def check_expert_dispatch(nranks: int, x, topk_idx, num_experts: int, recv, expe
     multiple of nranks; recv: contiguous, x's dtype, a whole number of rows; expert_counts (num_experts // nranks), route (tokens, top_k)
     and dropped (1 element): contiguous int32 when given. tokens * top_k, nranks * recv rows and tokens * top_k * row bytes / 16 are at
     most 2^31 - 1. recv must not overlap x, and no output may overlap another output, topk_idx, x or recv."""
-    import torch
-    if x.dtype not in (torch.bfloat16, torch.float16, torch.float32) or x.dim() != 2 or not x.is_contiguous():
-        raise ValueError(f"x must be a contiguous bfloat16, float16 or float32 [tokens, row_elems] tensor, got {x.dtype}{list(x.shape)}")
-    tokens, row_elems = x.shape
-    if row_elems <= 0 or row_elems % 16:
-        raise ValueError(f"row_elems (x.shape[1] = {row_elems}) must be a positive multiple of 16")
-    if topk_idx.dtype != torch.int32 or topk_idx.dim() != 2 or not topk_idx.is_contiguous() or topk_idx.shape[1] < 1:
-        raise ValueError(f"topk_idx must be a contiguous int32 [tokens, top_k] tensor with top_k >= 1, got {topk_idx.dtype}{list(topk_idx.shape)}")
-    if topk_idx.shape[0] != tokens:
-        raise ValueError(f"topk_idx has {topk_idx.shape[0]} tokens, x has {tokens}")
-    top_k = topk_idx.shape[1]
-    if isinstance(num_experts, bool) or not isinstance(num_experts, int) or not 1 <= num_experts <= MAX_EXPERTS or num_experts % nranks:
-        raise ValueError(f"num_experts must be an int in [1, {MAX_EXPERTS}] and a multiple of nranks ({nranks}), got {num_experts!r}")
-    if recv.dtype != x.dtype or not recv.is_contiguous() or recv.numel() % row_elems:
-        raise ValueError(f"recv must be a contiguous {x.dtype} tensor of whole {row_elems}-element rows, got {recv.dtype} with {recv.numel()} elements")
-    if tokens * top_k > _I31:
-        raise ValueError(f"tokens * top_k ({tokens * top_k}) must be at most 2^31 - 1")
-    if nranks * (recv.numel() // row_elems) > _I31:
-        raise ValueError("nranks * recv rows must be at most 2^31 - 1 (a route is an int32)")
-    if tokens * top_k * (row_elems * x.element_size() // 16) > _I31:
-        raise ValueError("at most 2^31 - 1 16-byte vectors may be offered (tokens * top_k * row bytes / 16)")
-    if _overlap(recv, x):
-        raise ValueError("recv must not overlap x")
-    outs = [(n, t, shape) for n, t, shape in (("expert_counts", expert_counts, (num_experts // nranks,)), ("route", route, (tokens, top_k)),
-                                              ("dropped", dropped, (1,))) if t is not None]
-    for name, t, shape in outs:
-        if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != _numel(shape):
-            raise ValueError(f"{name} must be a contiguous int32 tensor of shape {shape}, got {t.dtype}{list(t.shape)}")
-    for k, (name, t, _) in enumerate(outs):
-        for other, u in [(n, o) for n, o, _ in outs[k + 1:]] + [("topk_idx", topk_idx), ("x", x), ("recv", recv)]:
-            if _overlap(t, u):
-                raise ValueError(f"{name} must not overlap {other}")
+    _check_routed(nranks, x, topk_idx, num_experts, recv, expert_counts, route, dropped)
     return torch_dtype_code(x.dtype)
 
 
@@ -451,47 +469,7 @@ def check_expert_dispatch_quantized(nranks: int, x, topk_idx, num_experts: int, 
     recv.numel() // block elements. tokens * top_k, nranks * recv rows, tokens * row_elems / 16 (the 16-element vectors of x) and
     tokens * top_k * row bytes / 16 are at most 2^31 - 1. x, recv and recv_scales must not overlap, and no output may overlap another
     output, topk_idx, x, recv or recv_scales."""
-    import torch
-    if x.dtype not in (torch.bfloat16, torch.float16, torch.float32) or x.dim() != 2 or not x.is_contiguous():
-        raise ValueError(f"x must be a contiguous bfloat16, float16 or float32 [tokens, row_elems] tensor, got {x.dtype}{list(x.shape)}")
-    tokens, row_elems = x.shape
-    if isinstance(block, bool) or not isinstance(block, int) or block not in QUANT_BLOCKS:
-        raise ValueError(f"block must be one of {QUANT_BLOCKS}, got {block!r}")
-    if row_elems <= 0 or row_elems % block:
-        raise ValueError(f"row_elems (x.shape[1] = {row_elems}) must be a positive multiple of block ({block})")
-    if topk_idx.dtype != torch.int32 or topk_idx.dim() != 2 or not topk_idx.is_contiguous() or topk_idx.shape[1] < 1:
-        raise ValueError(f"topk_idx must be a contiguous int32 [tokens, top_k] tensor with top_k >= 1, got {topk_idx.dtype}{list(topk_idx.shape)}")
-    if topk_idx.shape[0] != tokens:
-        raise ValueError(f"topk_idx has {topk_idx.shape[0]} tokens, x has {tokens}")
-    top_k = topk_idx.shape[1]
-    if isinstance(num_experts, bool) or not isinstance(num_experts, int) or not 1 <= num_experts <= MAX_EXPERTS or num_experts % nranks:
-        raise ValueError(f"num_experts must be an int in [1, {MAX_EXPERTS}] and a multiple of nranks ({nranks}), got {num_experts!r}")
-    if recv.dtype not in (torch.float8_e4m3fn, torch.float8_e5m2) or not recv.is_contiguous() or recv.numel() % row_elems:
-        raise ValueError(f"recv must be a contiguous float8_e4m3fn or float8_e5m2 tensor (the wire type) of whole {row_elems}-element rows, "
-                         f"got {recv.dtype} with {recv.numel()} elements")
-    if recv_scales.dtype != torch.float32 or not recv_scales.is_contiguous() or recv_scales.numel() != recv.numel() // block:
-        raise ValueError(f"recv_scales must be a contiguous float32 tensor of recv.numel() // block = {recv.numel() // block} elements, "
-                         f"got {recv_scales.dtype} with {recv_scales.numel()}")
-    if tokens * top_k > _I31:
-        raise ValueError(f"tokens * top_k ({tokens * top_k}) must be at most 2^31 - 1")
-    if nranks * (recv.numel() // row_elems) > _I31:
-        raise ValueError("nranks * recv rows must be at most 2^31 - 1 (a route is an int32)")
-    if tokens * (row_elems // 16) > _I31:
-        raise ValueError("at most 2^31 - 1 16-element vectors of x (tokens * row_elems / 16)")
-    if tokens * top_k * (row_elems * x.element_size() // 16) > _I31:
-        raise ValueError("at most 2^31 - 1 16-byte vectors may be offered (tokens * top_k * row bytes / 16)")
-    for a, b, an, bn in ((recv, x, "recv", "x"), (recv_scales, x, "recv_scales", "x"), (recv, recv_scales, "recv", "recv_scales")):
-        if _overlap(a, b):
-            raise ValueError(f"{an} must not overlap {bn}")
-    outs = [(n, t, shape) for n, t, shape in (("expert_counts", expert_counts, (num_experts // nranks,)), ("route", route, (tokens, top_k)),
-                                              ("dropped", dropped, (1,))) if t is not None]
-    for name, t, shape in outs:
-        if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != _numel(shape):
-            raise ValueError(f"{name} must be a contiguous int32 tensor of shape {shape}, got {t.dtype}{list(t.shape)}")
-    for k, (name, t, _) in enumerate(outs):
-        for other, u in [(n, o) for n, o, _ in outs[k + 1:]] + [("topk_idx", topk_idx), ("x", x), ("recv", recv), ("recv_scales", recv_scales)]:
-            if _overlap(t, u):
-                raise ValueError(f"{name} must not overlap {other}")
+    _check_routed(nranks, x, topk_idx, num_experts, recv, expert_counts, route, dropped, fp8=(recv_scales, block))
     return torch_dtype_code(x.dtype), torch_dtype_code(recv.dtype)
 
 
@@ -502,13 +480,11 @@ def check_expert_combine(nranks: int, expert_out, route, weights, out) -> tuple[
     weights: None or contiguous float32 of route's shape. nranks * expert_out rows is at most 2^31 - 1. out must not overlap expert_out,
     route or weights."""
     import torch
-    wide = (torch.bfloat16, torch.float16, torch.float32)
-    if out.dtype not in wide or out.dim() != 2 or not out.is_contiguous():
-        raise ValueError(f"out must be a contiguous bfloat16, float16 or float32 [tokens, row_elems] tensor, got {out.dtype}{list(out.shape)}")
+    _check_wide("out", out, rows=True)
     tokens, row_elems = out.shape
     if row_elems <= 0 or row_elems % 16:
         raise ValueError(f"row_elems (out.shape[1] = {row_elems}) must be a positive multiple of 16")
-    if expert_out.dtype not in wide or not expert_out.is_contiguous() or expert_out.numel() % row_elems:
+    if expert_out.dtype not in (torch.bfloat16, torch.float16, torch.float32) or not expert_out.is_contiguous() or expert_out.numel() % row_elems:
         raise ValueError(f"expert_out must be a contiguous bfloat16, float16 or float32 tensor of whole {row_elems}-element rows, got {expert_out.dtype}")
     if route.dtype != torch.int32 or route.dim() != 2 or not route.is_contiguous() or route.shape[1] < 1 or route.shape[0] != tokens:
         raise ValueError(f"route must be a contiguous int32 [{tokens}, top_k] tensor with top_k >= 1, got {route.dtype}{list(route.shape)}")
@@ -808,10 +784,22 @@ class Comm:
         _check(load().b200collAllToAll(C.c_void_p(src.data_ptr()), C.c_void_p(dst.data_ptr()), src.numel() // self.nranks, C.byref(ep), self._h, self._stream(stream)), "AllToAll")
         return dst
 
+    def _rows(self, xs):
+        """A host list of nranks row counts or offsets, as the library's int64[nranks]."""
+        return (C.c_int64 * self.nranks)(*[int(x) for x in xs])
+
+    def _routed_outputs(self, x, num_experts: int, top_k: int, expert_counts, route, dropped, stream):
+        """The routed dispatch's small int32 outputs, each one not given allocated on x's device and the call's stream."""
+        import torch
+        with torch.cuda.device(x.device), torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream(x.device)):
+            expert_counts = torch.empty(num_experts // self.nranks, dtype=torch.int32, device=x.device) if expert_counts is None else expert_counts
+            route = torch.empty(x.shape[0], top_k, dtype=torch.int32, device=x.device) if route is None else route
+            dropped = torch.empty(1, dtype=torch.int32, device=x.device) if dropped is None else dropped
+        return expert_counts, route, dropped
+
     def all_to_all_v(self, src, dst, row_elems: int, send_rows, send_row_off, recv_row_off_at_peer, scale: float = 1.0, stream=None):
         ep = self._ep(src, dst, scale)
-        n = self.nranks
-        arr = lambda xs: (C.c_int64 * n)(*[int(x) for x in xs])
+        arr = self._rows
         _check(load().b200collAllToAllv(C.c_void_p(src.data_ptr()), C.c_void_p(dst.data_ptr()), row_elems, arr(send_rows), arr(send_row_off), arr(recv_row_off_at_peer),
                                         C.byref(ep), self._h, self._stream(stream)), "AllToAllv")
         return dst
@@ -824,8 +812,7 @@ class Comm:
         ([rows, row_elems // block] fp32). Returns (out, out_scales). With more than one rank, out and out_scales must be arena tensors
         (`empty()`) of the same size on every rank; every rank calls, a rank that sends nothing included."""
         ic, wc = check_all_to_all_v_quantized(self.nranks, src, out, out_scales, row_elems, block, send_rows, send_row_off, recv_row_off_at_peer)
-        n = self.nranks
-        arr = lambda xs: (C.c_int64 * n)(*[int(x) for x in xs])
+        arr = self._rows
         _check(load().b200collAllToAllvQuantized(C.c_void_p(src.data_ptr()), C.c_void_p(out.data_ptr()), C.cast(C.c_void_p(out_scales.data_ptr()), C.POINTER(C.c_float)),
                                                  row_elems, out.numel() // row_elems, arr(send_rows), arr(send_row_off), arr(recv_row_off_at_peer), ic, wc, block,
                                                  self._h, self._stream(stream)), "AllToAllvQuantized")
@@ -840,8 +827,7 @@ class Comm:
         out. With more than one rank, expert_out must be an arena tensor (`empty()`) of the same size on every rank; every rank calls,
         a rank with no tokens included."""
         ic, oc = check_all_to_all_v_combine(self.nranks, expert_out, out, row_elems, send_rows, send_row_off, recv_row_off_at_peer, index, weights)
-        n = self.nranks
-        arr = lambda xs: (C.c_int64 * n)(*[int(x) for x in xs])
+        arr = self._rows
         tokens, top_k = index.shape
         ep = Epilogue(ic, oc, float(scale))
         w = C.cast(C.c_void_p(weights.data_ptr() if weights is not None else None), C.POINTER(C.c_float))
@@ -862,15 +848,11 @@ class Comm:
         ranks' calls can wait for the device (a cache flush frees memory, and freeing synchronises), while the earlier rank's layout
         kernel waits at its barrier for the next rank's call. With more than one rank, recv
         must be an arena tensor (`empty()`) of the same size on every rank; every rank calls, a rank with no tokens included."""
-        import torch
         code = check_expert_dispatch(self.nranks, x, topk_idx, num_experts, recv, expert_counts, route, dropped)
         tokens, row_elems = x.shape
         top_k = topk_idx.shape[1]
         if expert_counts is None or route is None or dropped is None:
-            with torch.cuda.device(x.device), torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream(x.device)):
-                expert_counts = torch.empty(num_experts // self.nranks, dtype=torch.int32, device=x.device) if expert_counts is None else expert_counts
-                route = torch.empty(tokens, top_k, dtype=torch.int32, device=x.device) if route is None else route
-                dropped = torch.empty(1, dtype=torch.int32, device=x.device) if dropped is None else dropped
+            expert_counts, route, dropped = self._routed_outputs(x, num_experts, top_k, expert_counts, route, dropped, stream)
             check_expert_dispatch(self.nranks, x, topk_idx, num_experts, recv, expert_counts, route, dropped)
         i32 = lambda t: C.cast(C.c_void_p(t.data_ptr()), C.POINTER(C.c_int32))
         _check(load().b200collExpertDispatch(C.c_void_p(x.data_ptr()), C.c_void_p(recv.data_ptr()), row_elems, recv.numel() // row_elems, i32(topk_idx),
@@ -890,15 +872,11 @@ class Comm:
         memory, and freeing synchronises), while the earlier rank's layout kernel waits at its barrier for the next rank's call. With more
         than one rank, recv and recv_scales must be arena tensors (`empty()`) of the same sizes on every rank; every rank calls, a rank
         with no tokens included."""
-        import torch
         ic, wc = check_expert_dispatch_quantized(self.nranks, x, topk_idx, num_experts, recv, recv_scales, block, expert_counts, route, dropped)
         tokens, row_elems = x.shape
         top_k = topk_idx.shape[1]
         if expert_counts is None or route is None or dropped is None:
-            with torch.cuda.device(x.device), torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream(x.device)):
-                expert_counts = torch.empty(num_experts // self.nranks, dtype=torch.int32, device=x.device) if expert_counts is None else expert_counts
-                route = torch.empty(tokens, top_k, dtype=torch.int32, device=x.device) if route is None else route
-                dropped = torch.empty(1, dtype=torch.int32, device=x.device) if dropped is None else dropped
+            expert_counts, route, dropped = self._routed_outputs(x, num_experts, top_k, expert_counts, route, dropped, stream)
             check_expert_dispatch_quantized(self.nranks, x, topk_idx, num_experts, recv, recv_scales, block, expert_counts, route, dropped)
         i32 = lambda t: C.cast(C.c_void_p(t.data_ptr()), C.POINTER(C.c_int32))
         _check(load().b200collExpertDispatchQuantized(C.c_void_p(x.data_ptr()), C.c_void_p(recv.data_ptr()),

@@ -12,10 +12,11 @@ import torch
 
 from container_engine_accelerators_b200.ops import coll
 from tests import coll_combine_reference as cr
+from tests.coll_binary_facts import kernels, ptxas, sass, template_args
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 WIDE = ("__nv_bfloat16", "__half", "float")
-FAMILIES = ("k_a2av_combine_pull", "k_a2av_combine_local")
+FAMILIES = ("k_combine_pull", "k_combine_local")
 
 
 def test_header_prototype_matches_the_ctypes_argtypes(tmp_path, coll_lib):
@@ -120,36 +121,20 @@ def test_comm_method_checks_before_calling_the_library():
 
 
 # ------------------------------------------------------------------------------------------------- kernels
-def _kernels(coll_lib):
-    names = subprocess.run(["nm", "-C", coll_lib], capture_output=True, text=True, check=True).stdout
-    return sorted({l.split(" ", 2)[-1] for l in names.splitlines() if "b200coll::k_a2av_combine_" in l})
-
-
-def _targs(k):
-    return tuple(a.strip() for a in k.split("<", 1)[1].split(">", 1)[0].split(","))
 
 
 def test_every_input_and_output_pair_is_instantiated_once(coll_lib):
-    ks = _kernels(coll_lib)
+    ks = [k for k in kernels(coll_lib, "b200coll::k_combine_") if "b200coll::SegmentMap>" in k]
     for fam in FAMILIES:
-        have = [_targs(k) for k in ks if f"::{fam}<" in k]
-        assert sorted(have) == sorted((i, o) for i in WIDE for o in WIDE), (fam, have)
+        have = [template_args(k) for k in ks if f"::{fam}<" in k]
+        assert sorted(have) == sorted((i, o, "b200coll::SegmentMap") for i in WIDE for o in WIDE), (fam, have)
     assert len(ks) == 18, ks
     # outside the name patterns other tests count or filter on
     assert not any("k_a2av_quant_" in k or "k_quant_" in k or "k_bsq_" in k or "k_a2av_push<" in k for k in ks)
 
 
 def test_sass_has_no_ffma_and_no_multimem_loads(coll_lib):
-    out = subprocess.run(["cuobjdump", "-sass", coll_lib], capture_output=True, text=True, check=True).stdout
-    funcs, cur = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            funcs[cur] = []
-        elif cur:
-            funcs[cur].append(line)
-    funcs = {k: "\n".join(v) for k, v in funcs.items() if "k_a2av_combine_" in k}
+    funcs = {k: v for k, v in sass(coll_lib).items() if "k_combine_" in k and "SegmentMap" in k}
     assert len(funcs) == 18, sorted(funcs)
     for name, body in funcs.items():
         assert re.search(r"\bFMUL\b", body) and re.search(r"\bFADD\b", body), name       # the products and sums, each rounded
@@ -157,22 +142,9 @@ def test_sass_has_no_ffma_and_no_multimem_loads(coll_lib):
         assert "LDGMC" not in body, name
 
 
-def test_ptxas_reports_no_stack_and_no_spills(tmp_path):
+def test_ptxas_reports_no_stack_and_no_spills():
     """The compiler's own account, with the library's flags: no stack frame and no spill stores or loads for the combine kernels."""
-    src = os.path.join(ROOT, "coll", "src", "combine.cu")
-    r = subprocess.run([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
-                        "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-c", src, "-o", str(tmp_path / "combine.o")],
-                       capture_output=True, text=True, check=True)
-    report, cur = {}, None
-    for line in r.stderr.splitlines():
-        m = re.search(r"Function properties for (\S+)", line)
-        if m:
-            cur = m.group(1)
-            continue
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and cur and "k_a2av_combine_" in cur:
-            report[cur] = tuple(map(int, m.groups()))
-        cur = None if m else cur
+    report = {k: v for k, v in ptxas("combine.cu")[0].items() if "k_combine_" in k and "SegmentMap" in k}
     assert len(report) == 18, sorted(report)
     assert all(v == (0, 0, 0) for v in report.values()), report
 

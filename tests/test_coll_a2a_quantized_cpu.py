@@ -9,6 +9,7 @@ import pytest
 import torch
 
 from container_engine_accelerators_b200.ops import coll
+from tests.coll_binary_facts import kernels, ptxas, sass, template_args
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E4, E5 = torch.float8_e4m3fn, torch.float8_e5m2
@@ -119,40 +120,20 @@ def test_comm_method_checks_before_calling_the_library():
 
 
 # ------------------------------------------------------------------------------------------------- kernels
-def _kernels(coll_lib):
-    names = subprocess.run(["nm", "-C", coll_lib], capture_output=True, text=True, check=True).stdout
-    return sorted({l.split(" ", 2)[-1] for l in names.splitlines() if "b200coll::k_a2av_quant_" in l})
-
-
-def _targs(k):
-    return tuple(a.strip() for a in k.split("<", 1)[1].split(">", 1)[0].split(","))
 
 
 def test_every_input_and_wire_pair_is_instantiated_once(coll_lib):
-    ks = _kernels(coll_lib)
+    ks = kernels(coll_lib, "b200coll::k_a2av_quant_")
     for fam in FAMILIES:
-        have = [_targs(k) for k in ks if f"::{fam}<" in k]
+        have = [template_args(k) for k in ks if f"::{fam}<" in k]
         assert sorted(have) == sorted((i, w) for i in WIDE for w in WIRES), (fam, have)
     assert len(ks) == 12, ks
     # outside the name patterns other tests count or filter on
     assert not any("k_quant_" in k or "k_bsq_" in k or "k_a2av_push<" in k for k in ks)
 
 
-def _sass(coll_lib):
-    out = subprocess.run(["cuobjdump", "-sass", coll_lib], capture_output=True, text=True, check=True).stdout
-    funcs, cur = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            funcs[cur] = []
-        elif cur:
-            funcs[cur].append(line)
-    return {k: "\n".join(v) for k, v in funcs.items() if "k_a2av_quant_" in k}
-
-
 def test_sass_reduces_amax_across_lanes_and_packs_saturating(coll_lib):
-    funcs = _sass(coll_lib)
+    funcs = {k: v for k, v in sass(coll_lib).items() if "k_a2av_quant_" in k}
     assert len(funcs) == 12, sorted(funcs)
     for name, body in funcs.items():
         wire = "E4M3" if "e4m3" in name else "E5M2"                      # the input type is never FP8, so the name's FP8 type is the wire's
@@ -161,22 +142,9 @@ def test_sass_reduces_amax_across_lanes_and_packs_saturating(coll_lib):
         assert "LDGMC" not in body, name
 
 
-def test_ptxas_reports_no_stack_and_no_spills(tmp_path):
+def test_ptxas_reports_no_stack_and_no_spills():
     """The compiler's own account, with the library's flags: no stack frame and no spill stores or loads for the new kernels."""
-    src = os.path.join(ROOT, "coll", "src", "blockscaled.cu")
-    r = subprocess.run([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
-                        "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-c", src, "-o", str(tmp_path / "blockscaled.o")],
-                       capture_output=True, text=True, check=True)
-    report, cur = {}, None
-    for line in r.stderr.splitlines():
-        m = re.search(r"Function properties for (\S+)", line)
-        if m:
-            cur = m.group(1)
-            continue
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and cur and "k_a2av_quant_" in cur:
-            report[cur] = tuple(map(int, m.groups()))
-        cur = None if m else cur
+    report = {k: v for k, v in ptxas("dispatch.cu")[0].items() if "k_a2av_quant_" in k}
     assert len(report) == 12, sorted(report)
     assert all(v == (0, 0, 0) for v in report.values()), report
 

@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from container_engine_accelerators_b200.ops import coll
+from tests.coll_binary_facts import kernels, ptxas, sass, template_args
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FP8 = ("__nv_fp8_e4m3", "__nv_fp8_e5m2")
@@ -43,40 +44,18 @@ int main(void) {
         assert getattr(L, name).argtypes[3] is C.POINTER(coll.BlockScale)
 
 
-def _kernels(coll_lib):
-    names = subprocess.run(["nm", "-C", coll_lib], capture_output=True, text=True, check=True).stdout
-    return [l.split(" ", 2)[-1] for l in names.splitlines() if "b200coll::k_bsq_" in l]
-
-
-def _args(k):
-    return [a.strip() for a in k.split("<", 1)[1].split(">", 1)[0].split(",")]
-
-
 def test_every_fp8_input_and_output_pair_is_instantiated(coll_lib):
-    ks = _kernels(coll_lib)
+    ks = kernels(coll_lib, "b200coll::k_bsq_")
     for fam, extra in (("k_bsq_ag_pull<", [[]]), ("k_bsq_pull_reduce<", [["false"], ["true"]]), ("k_bsq_copy<", [[]])):
-        have = {tuple(_args(k)) for k in ks if fam in k}
+        have = {template_args(k) for k in ks if fam in k}
         want = {(i, o, *e) for i in FP8 for o in OUTS for e in extra}
         assert want <= have, (fam, sorted(want - have))
     # FP8 -> fp32 exists only in the k_bsq_ family: the existing families' instantiation rules are unchanged
     assert all(re.search(r"k_bsq_[a-z_]+<", k) for k in ks)
 
 
-def _sass(coll_lib):
-    out = subprocess.run(["cuobjdump", "-sass", coll_lib], capture_output=True, text=True, check=True).stdout
-    funcs, cur = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            funcs[cur] = []
-        elif cur:
-            funcs[cur].append(line)
-    return {k: "\n".join(v) for k, v in funcs.items() if "k_bsq_" in k}
-
-
 def test_sass_unpacks_in_hardware_uses_no_multimem_and_no_64bit_division(coll_lib):
-    funcs = _sass(coll_lib)
+    funcs = {k: v for k, v in sass(coll_lib).items() if "k_bsq_" in k}
     assert len(funcs) >= 24, sorted(funcs)
     for name, body in funcs.items():
         unpack = "F2FP.F16.E4M3.UNPACK_B" if "e4m3" in name else "F2FP.F16.E5M2.UNPACK_B"
@@ -91,8 +70,9 @@ def test_sass_unpacks_in_hardware_uses_no_multimem_and_no_64bit_division(coll_li
 
 def test_source_moves_data_without_multimem():
     """The data path is plain loads and stores over NVLink; the only multicast operation is the shared epoch barrier's counter."""
-    src = open(os.path.join(ROOT, "coll", "src", "blockscaled.cu")).read()
-    device = src.split("// ---", 1)[0].split("#include", 1)[1]
+    quant = open(os.path.join(ROOT, "coll", "src", "quant.cuh")).read()            # the quantise helpers blockscaled.cu includes
+    src = open(os.path.join(ROOT, "coll", "src", "blockscaled.cu")).read() + quant
+    device = src.split("// ---", 1)[0].split("#include", 1)[1] + quant
     for loop in ("warp_walk", "dequant_range", "pull_reduce_range", "quant_range", "k_bsq_pull_reduce", "k_quant_pull_reduce"):
         assert f" {loop}(" in device, loop                        # the device section the check covers holds every loop
     assert "multimem" not in device
@@ -113,23 +93,9 @@ def test_no_spills_in_block_scaled_kernels(coll_lib):
     assert seen >= 24
 
 
-def test_ptxas_reports_no_spill_bytes(tmp_path):
+def test_ptxas_reports_no_spill_bytes():
     """The compiler's own account, with the library's flags: 0 bytes spill stores and loads for every k_bsq_ kernel."""
-    src = os.path.join(ROOT, "coll", "src", "blockscaled.cu")
-    r = subprocess.run([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
-                        "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-c", src, "-o", str(tmp_path / "blockscaled.o")],
-                       capture_output=True, text=True, check=True)
-    report = {}
-    cur = None
-    for line in r.stderr.splitlines():
-        m = re.search(r"Function properties for (\S+)", line)
-        if m:
-            cur = m.group(1)
-            continue
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and cur and "k_bsq_" in cur:
-            report[cur] = tuple(map(int, m.groups()))
-        cur = None if m else cur
+    report = {k: v for k, v in ptxas("blockscaled.cu")[0].items() if "k_bsq_" in k}
     assert len(report) == 24, sorted(report)
     spilled = {k: v for k, v in report.items() if v != (0, 0, 0)}
     assert not spilled, spilled

@@ -12,11 +12,10 @@ import torch
 
 from container_engine_accelerators_b200.ops import coll
 from tests import coll_routed_reference as rr
+from tests.coll_binary_facts import kernels, ptxas, sass, template_args
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 WIDE = ("__nv_bfloat16", "__half", "float")
-NVCC = [os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
-        "-Xptxas", "-v", "-c"]
 
 
 def test_header_prototypes_match_the_ctypes_argtypes(tmp_path, coll_lib):
@@ -201,36 +200,21 @@ def test_layout_reference_by_hand():
 
 
 # ------------------------------------------------------------------------------------------------- kernels
-def _kernels(coll_lib, key):
-    names = subprocess.run(["nm", "-C", coll_lib], capture_output=True, text=True, check=True).stdout
-    return sorted({l.split(" ", 2)[-1] for l in names.splitlines() if key in l})
 
 
 def test_kernels_are_instantiated_once(coll_lib):
-    ks = _kernels(coll_lib, "b200coll::k_routed_")
-    for fam in ("k_routed_combine_pull", "k_routed_combine_local"):
-        have = [tuple(a.strip() for a in k.split("<", 1)[1].split(">", 1)[0].split(",")) for k in ks if f"::{fam}<" in k]
-        assert sorted(have) == sorted((i, o) for i in WIDE for o in WIDE), (fam, have)
+    ks = kernels(coll_lib, "b200coll::k_routed_")
+    comb = [k for k in kernels(coll_lib, "b200coll::k_combine_") if "b200coll::RouteMap>" in k]
+    for fam in ("k_combine_pull", "k_combine_local"):
+        have = [template_args(k) for k in comb if f"::{fam}<" in k]
+        assert sorted(have) == sorted((i, o, "b200coll::RouteMap") for i in WIDE for o in WIDE), (fam, have)
     assert sum("::k_routed_push<" in k for k in ks) == 2 and sum("::k_routed_layout(" in k for k in ks) == 1
-    assert len(ks) == 21, ks
-
-
-def _sass(coll_lib):
-    out = subprocess.run(["cuobjdump", "-sass", coll_lib], capture_output=True, text=True, check=True).stdout
-    funcs, cur = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            funcs[cur] = []
-        elif cur:
-            funcs[cur].append(line)
-    return {k: "\n".join(v) for k, v in funcs.items()}
+    assert len(ks) + len(comb) == 21, (ks, comb)
 
 
 def test_sass_of_every_combine_kernel_has_no_ffma(coll_lib):
-    funcs = _sass(coll_lib)
-    combine = {k: v for k, v in funcs.items() if "k_routed_combine_" in k or "k_a2av_combine_" in k}
+    funcs = sass(coll_lib)
+    combine = {k: v for k, v in funcs.items() if "k_combine_" in k}
     assert len(combine) == 36, sorted(combine)
     for name, body in combine.items():
         assert re.search(r"\bFMUL\b", body) and re.search(r"\bFADD\b", body), name
@@ -240,36 +224,15 @@ def test_sass_of_every_combine_kernel_has_no_ffma(coll_lib):
     assert len(layout) == 1 and "MATCH.ANY" in layout[0]                                  # the warp groups lanes by expert id
 
 
-def _ptxas(tmp_path, name):
-    r = subprocess.run(NVCC + [os.path.join(ROOT, "coll", "src", name), "-o", str(tmp_path / (name + ".o"))], capture_output=True, text=True, check=True)
-    report, regs, cur = {}, {}, None
-    for line in r.stderr.splitlines():
-        m = re.search(r"Function properties for (\S+)", line)
-        if m:
-            cur = m.group(1)
-            continue
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and cur:
-            report[cur] = tuple(map(int, m.groups()))
-            continue
-        m = re.search(r"Compiling entry function '(\S+)'", line)
-        if m:
-            cur = m.group(1)
-        m = re.search(r"Used (\d+) registers", line)
-        if m and cur:
-            regs[cur] = int(m.group(1))
-    return report, regs
-
-
-def test_ptxas_reports_no_stack_and_no_spills(tmp_path):
+def test_ptxas_reports_no_stack_and_no_spills():
     """The compiler's own account, with the library's flags: the new kernels and the combine kernels, old and new, have no stack frame
     and no spill stores or loads, and the combine kernels stay within 128 registers."""
-    report, _ = _ptxas(tmp_path, "routed.cu")
+    report, _ = ptxas("dispatch.cu")
     mine = {k: v for k, v in report.items() if "k_routed_" in k}
     assert len(mine) == 3, sorted(mine)
     assert all(v == (0, 0, 0) for v in mine.values()), mine
-    report, regs = _ptxas(tmp_path, "combine.cu")
-    comb = {k: v for k, v in report.items() if "k_routed_combine_" in k or "k_a2av_combine_" in k}
+    report, regs = ptxas("combine.cu")
+    comb = {k: v for k, v in report.items() if "k_combine_" in k}
     assert len(comb) == 36, sorted(comb)
     assert all(v == (0, 0, 0) for v in comb.values()), comb
     assert all(r <= 128 for k, r in regs.items() if "combine_" in k), regs

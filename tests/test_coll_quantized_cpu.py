@@ -12,6 +12,7 @@ import torch
 
 from container_engine_accelerators_b200.ops import coll
 from tests import coll_quant_reference as qr
+from tests.coll_binary_facts import kernels, ptxas, sass, template_args
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E4, E5 = torch.float8_e4m3fn, torch.float8_e5m2
@@ -207,20 +208,11 @@ int main(void) {
     assert L.b200collAllReduceQuantized.argtypes == [vp, vp, sz, ci, ci, ep, ci, vp, vp]
 
 
-def _kernels(coll_lib):
-    names = subprocess.run(["nm", "-C", coll_lib], capture_output=True, text=True, check=True).stdout
-    return sorted({l.split(" ", 2)[-1] for l in names.splitlines() if "b200coll::k_quant_" in l})
-
-
-def _args(k):
-    return tuple(a.strip() for a in k.split("<", 1)[1].split(">", 1)[0].split(","))
-
-
 def test_every_input_wire_and_output_triple_is_instantiated(coll_lib):
-    ks = _kernels(coll_lib)
+    ks = kernels(coll_lib, "b200coll::k_quant_")
     want = set()
     for fam, extra in (("k_quant_ag", [()]), ("k_quant_pull_reduce", [("false",), ("true",)]), ("k_quant_copy", [()])):
-        have = {_args(k) for k in ks if f"::{fam}<" in k}
+        have = {template_args(k) for k in ks if f"::{fam}<" in k}
         fam_want = {(i, w, o, *e) for i in WIDE for w in WIRES for o in WIDE for e in extra}
         assert have == fam_want, (fam, sorted(fam_want ^ have))
         want |= {(fam, t) for t in fam_want}
@@ -228,21 +220,8 @@ def test_every_input_wire_and_output_triple_is_instantiated(coll_lib):
     assert not any("k_bsq_" in k for k in ks)                          # the block-scaled family keeps its own 24 kernels
 
 
-def _sass(coll_lib):
-    out = subprocess.run(["cuobjdump", "-sass", coll_lib], capture_output=True, text=True, check=True).stdout
-    funcs, cur = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            funcs[cur] = []
-        elif cur:
-            funcs[cur].append(line)
-    return {k: "\n".join(v) for k, v in funcs.items() if "k_quant_" in k}
-
-
 def test_sass_reduces_amax_across_lanes_packs_saturating_and_unpacks_in_hardware(coll_lib):
-    funcs = _sass(coll_lib)
+    funcs = {k: v for k, v in sass(coll_lib).items() if "k_quant_" in k}
     assert len(funcs) == 72, sorted(funcs)
     for name, body in funcs.items():
         wire = "E4M3" if "e4m3" in name else "E5M2"                      # the input type is never FP8, so the name's FP8 type is the wire's
@@ -254,23 +233,10 @@ def test_sass_reduces_amax_across_lanes_packs_saturating_and_unpacks_in_hardware
             assert "MATCH.ANY" in body, name                              # pulled scales shared by the lanes that need them
 
 
-def test_ptxas_reports_no_spill_bytes_in_the_shared_fp8_unit(tmp_path):
+def test_ptxas_reports_no_spill_bytes_in_the_shared_fp8_unit():
     """The compiler's own account, with the library's flags: no stack frame and no spill stores or loads for any k_quant_ kernel of
     blockscaled.cu, the translation unit the quantising kernels share with the block-scaled ones."""
-    src = os.path.join(ROOT, "coll", "src", "blockscaled.cu")
-    r = subprocess.run([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
-                        "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-c", src, "-o", str(tmp_path / "blockscaled.o")],
-                       capture_output=True, text=True, check=True)
-    report, cur = {}, None
-    for line in r.stderr.splitlines():
-        m = re.search(r"Function properties for (\S+)", line)
-        if m:
-            cur = m.group(1)
-            continue
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and cur and "k_quant_" in cur:
-            report[cur] = tuple(map(int, m.groups()))
-        cur = None if m else cur
+    report = {k: v for k, v in ptxas("blockscaled.cu")[0].items() if "k_quant_" in k}
     assert len(report) == 72, sorted(report)
     spilled = {k: v for k, v in report.items() if v != (0, 0, 0)}
     assert not spilled, spilled
