@@ -17,6 +17,10 @@ nothing was dropped, the counts add up to the plan's rows, and the routed combin
 Then (j) expert_dispatch_quantized, the same routing with e4m3 rows and 1x128 block scales on the wire, into recv8 / recv_scales;
 routed_fp8_matches says its counts, route and dropped equal the bf16 routed dispatch's and every stored row, dequantised, lies within
 amax * 2^-4 of its source token's row (amax of the element's block: half an e4m3 ulp at the block's largest value).
+Then the quantising combines, e4m3 with 1x128 block scales on the wire: (k) all_to_all_v_combine_quantized over (e)'s expert outputs and
+(l) expert_combine_quantized over (h)'s; q_combine_matches says both equal, bit for bit, the slot-order fp32 sum of the rows quantised
+and dequantised (amax, two fp32 divisions, e4m3 cast, one multiply). At one rank nothing crosses NVLink, so their time over the wide
+combines' is the HBM cost of the quantise pass.
 Bus bandwidth = (bytes a rank sends off-chip, max over ranks) / time. Rank 0 prints one JSON line per shape."""
 from __future__ import annotations
 
@@ -39,7 +43,8 @@ def main() -> int:
     shapes = [(4096, 4096, 0.0), (4096, 7168, 1.0), (16384, 7168, 1.0), (65536, 7168, 1.2)]
     cap_rows = max(expert_dispatch_plan(world, t, h, skew=s).max_rows for t, h, s in shapes)
     cap_hidden = max(h for _, h, _ in shapes)
-    comm = coll.Comm.from_env(arena_mb=int(cap_rows * cap_hidden * 2 * 2.6 / (1 << 20)) + 256, tag="a2av")
+    # send, recv, recv8 and recv_scales, plus the quantising combines' scratch (1.03 bytes per expert_out element, every size's kept)
+    comm = coll.Comm.from_env(arena_mb=int(cap_rows * cap_hidden * 2 * 3.4 / (1 << 20)) + 256, tag="a2av")
     send = comm.empty(cap_rows * cap_hidden, torch.bfloat16)
     recv = comm.empty(cap_rows * cap_hidden, torch.bfloat16)
     recv8 = comm.empty(cap_rows * cap_hidden, torch.float8_e4m3fn)
@@ -60,6 +65,17 @@ def main() -> int:
         t = torch.tensor([e0.elapsed_time(e1) / iters], device="cuda")
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return t.item() * 1e3
+
+    def roundtrip(rows):
+        """bf16 rows quantised to e4m3 in 128-element blocks and dequantised, in fp32: amax, two divisions, the cast, one multiply."""
+        v = rows.float().view(rows.shape[0], -1, 128)
+        amax = v.abs().amax(dim=-1, keepdim=True)
+        fmax = torch.full_like(amax, 448.0)                                  # tensor operands: true divisions, not products with 1 / 448
+        inv, s = fmax / amax, amax / fmax
+        one = (amax == 0) | torch.isinf(inv)
+        inv, s = torch.where(one, torch.ones_like(inv), inv), torch.where(one, torch.ones_like(s), s)
+        q = (v * inv).clamp(-448.0, 448.0).to(torch.float8_e4m3fn)
+        return (q.float() * s).view(rows.shape[0], -1)
     for tokens, hidden, skew in shapes:
         plan = expert_dispatch_plan(world, tokens, hidden, skew=skew, seed=1)
         rows, so, ro = plan.rows[rank].tolist(), plan.send_off[rank].tolist(), [int(plan.recv_off[d, rank]) for d in range(world)]
@@ -90,6 +106,14 @@ def main() -> int:
         for j in range(idx.shape[1]):
             acc = acc + gate[:, j:j + 1] * y[idx[:, j].long()].float()
         comb_ok = bool(torch.equal(out.view(torch.int16), acc.to(torch.bfloat16).view(torch.int16)))
+        qout = torch.empty(tokens, hidden, dtype=torch.bfloat16, device="cuda")
+        us_q_comb = timed(lambda: comm.all_to_all_v_combine_quantized(eo, qout, hidden, rows, so, ro, idx, gate, block=128))
+        comm.check_async_error()
+        yq = roundtrip(y)
+        acc = torch.zeros(tokens, hidden, device="cuda")
+        for j in range(idx.shape[1]):
+            acc = acc + gate[:, j:j + 1] * yq[idx[:, j].long()]
+        q_comb_ok = bool(torch.equal(qout.view(torch.int16), acc.to(torch.bfloat16).view(torch.int16)))
         idx_l = idx.long()
 
         def nccl_combine():
@@ -104,6 +128,13 @@ def main() -> int:
         us_routed = timed(lambda: comm.expert_dispatch(x, topk, n_exp, rrecv, counts, route, dropped))
         us_routed_comb = timed(lambda: comm.expert_combine(rrecv.view(-1, hidden), route, gate, out))
         comm.check_async_error()
+        us_routed_q_comb = timed(lambda: comm.expert_combine_quantized(rrecv.view(-1, hidden), route, gate, qout, block=128))
+        comm.check_async_error()
+        xq = roundtrip(x)
+        acc = torch.zeros(tokens, hidden, device="cuda")
+        for j in range(topk.shape[1]):
+            acc = acc + gate[:, j:j + 1] * xq
+        q_comb_ok = q_comb_ok and bool(torch.equal(qout.view(torch.int16), acc.to(torch.bfloat16).view(torch.int16)))
         # the same routing with FP8 on the wire; x is the same on every rank (send is filled the same way everywhere), so a stored row
         # only needs its source token, which the gathered routes give
         q8, s8 = recv8[:q_rows * hidden], recv_scales[:q_rows * hidden // 128]
@@ -144,7 +175,8 @@ def main() -> int:
             comm.all_to_all_v(permuted, recv, hidden, h_rows, h_so, h_ro)
         us_host_plan = timed(host_plan)
         offchip = max(int(plan.rows[s].sum() - plan.rows[s, s]) for s in range(world)) * hidden * 2
-        oks = torch.tensor([1.0 if ok else 0.0, 1.0 if comb_ok else 0.0, 1.0 if routed_ok else 0.0, 1.0 if fp8_ok else 0.0], device="cuda")
+        oks = torch.tensor([1.0 if ok else 0.0, 1.0 if comb_ok else 0.0, 1.0 if routed_ok else 0.0, 1.0 if fp8_ok else 0.0, 1.0 if q_comb_ok else 0.0],
+                           device="cuda")
         dist.all_reduce(oks, op=dist.ReduceOp.MIN)
         if rank == 0:
             print(json.dumps({"bench": "alltoallv_perf", "n_gpus": world, "tokens_per_rank": tokens, "hidden": hidden, "skew": skew, "top_k": 2,
@@ -156,7 +188,8 @@ def main() -> int:
                               "combine_matches": bool(oks[1].item() == 1.0), "ours_routed_us": round(us_routed, 2),
                               "ours_routed_combine_us": round(us_routed_comb, 2), "host_plan_us": round(us_host_plan, 2),
                               "routed_matches": bool(oks[2].item() == 1.0), "ours_routed_fp8_us": round(us_routed_fp8, 2),
-                              "routed_fp8_matches": bool(oks[3].item() == 1.0)}), flush=True)
+                              "routed_fp8_matches": bool(oks[3].item() == 1.0), "ours_q_combine_us": round(us_q_comb, 2),
+                              "ours_routed_q_combine_us": round(us_routed_q_comb, 2), "q_combine_matches": bool(oks[4].item() == 1.0)}), flush=True)
     comm.destroy()
     dist.destroy_process_group()
     return 0

@@ -430,6 +430,39 @@ b200collResult_t b200collExpertDispatchQuantized(const void* x, void* recv, floa
 b200collResult_t b200collExpertCombine(const void* expert_out, void* out, size_t row_elems, size_t recv_rows, const int32_t* route,
                                        const float* weights, size_t tokens, int top_k, const b200collEpilogue* ep, b200collComm_t comm,
                                        b200collStream_t stream);
+/* Quantising expert combine: b200collAllToAllvCombine (segment table) and b200collExpertCombine (device route) with FP8 on the wire:
+ * row_elems * (1 + 4 / block) bytes per pulled row cross NVLink instead of row_elems * sizeof(in). Two kernels per call: each rank
+ * quantises every row of its expert_out ([recv_rows, row_elems] of ep->in_dtype, bf16, fp16 or fp32) into a library-owned scratch, by
+ * the rule of the quantising collectives: blocks of `block` elements along the row, wire_dtype e4m3 or e5m2, one fp32 scale per block,
+ * the bytes and scales b200collAllToAllvQuantized stores for that row. Then it pulls its slots' FP8 rows and scales from the peers'
+ * scratch and sums them.
+ * Result, per token t and element e, with v = float(q) * s (one fp32 multiply):
+ *   out[t, e] = round_once(scale * ((+0 + w0*v0[e]) + w1*v1[e] + ...)), slots in slot order, every product and every sum rounded to
+ *   fp32 on its own (no fused multiply-add). A slot maps to a row, or is dropped, exactly as in the wide combine of the same map. A block
+ *   holding NaN or +-inf dequantises to NaN throughout (its amax is NaN or inf). The result depends only on the values and the weights:
+ *   the rank count and which rank held a row make no difference, and one rank gives the same bits as eight.
+ *   ep->out_dtype bf16, fp16 or fp32; weights NULL gives all ones; scale = ep->scale.
+ * Refused with InvalidArgument before anything is launched: everything the matching wide combine refuses, except that expert_out need
+ * not be arena memory; and in or out type not bf16, fp16 or fp32, wire_dtype not e4m3 or e5m2, block not 16, 32, 64, 128, 256 or 512,
+ * row_elems % block != 0, more than 2^31 - 1 16-element vectors of expert_out (recv_rows * row_elems / 16).
+ * Placement: expert_out, out, index / route and weights may be any device buffers (peers read only the scratch). recv_rows must be the
+ * same on every rank; with B200COLL_CHECK=1 on multi-process communicators, (recv_rows, scratch offsets) and (row_elems, block,
+ * wire_dtype) are compared across ranks. A poisoned communicator gives RemoteError.
+ * Scratch: recv_rows * row_elems * (1 + 4 / block) bytes, in the scratch of the quantising collectives (a collective contract: the same
+ * calls in the same order on every rank); OutOfMemory, before anything is launched, when the arena cannot hold it. A superseded scratch
+ * is kept until CommDestroy, so a CUDA graph captured earlier stays valid. The quantise pass covers all recv_rows rows, read or not.
+ * Every rank launches on every call. The call returns (on its stream) only after every peer has finished reading this rank's scratch;
+ * expert_out is read only by this rank's quantise pass, so the caller may overwrite it right after the call. One rank: the same two
+ * kernels with no barrier. b200collStats count the call under alltoall, algorithm oneshot (copy with one rank), two kernel launches, and
+ * the bytes the matching wide combine counts. */
+b200collResult_t b200collAllToAllvCombineQuantized(const void* expert_out, void* out, size_t row_elems, size_t recv_rows,
+                                                   const int64_t* send_rows, const int64_t* send_row_off, const int64_t* recv_row_off_at_peer,
+                                                   const int32_t* index, const float* weights, size_t tokens, int top_k,
+                                                   b200collDataType_t wire_dtype, int block, const b200collEpilogue* ep, b200collComm_t comm,
+                                                   b200collStream_t stream);
+b200collResult_t b200collExpertCombineQuantized(const void* expert_out, void* out, size_t row_elems, size_t recv_rows, const int32_t* route,
+                                                const float* weights, size_t tokens, int top_k, b200collDataType_t wire_dtype, int block,
+                                                const b200collEpilogue* ep, b200collComm_t comm, b200collStream_t stream);
 
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.

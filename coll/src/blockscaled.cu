@@ -27,7 +27,8 @@
 // vector to its scale: the block-scaled vector -> (row, column) -> block arithmetic is 32-bit multiply-high division by host-computed
 // constants (no integer division in the loops), a quantising block is a shift.
 //
-// Quantising, per block: the rule in quant.cuh, which also holds the quantise helpers this file shares with dispatch.cu.
+// Quantising, per block: the rule in quant.cuh, which also holds the quantise and dequantise helpers this file shares with dispatch.cu
+// and combine.cu. The quantising combine (combine.cu) shares this file's scratch (quant_scratch_take).
 //
 // Fusing the quantise phase into the pull kernel is sound because of three properties, which the code below keeps:
 //   * Same-index CTAs only. The epoch barrier orders CTA b of this rank against CTA b of every peer, nothing else. Every vector loop in
@@ -96,22 +97,6 @@ struct WarpScale {
     return __shfl_sync(0xFFFFFFFFu, s, leader);
   }
 };
-
-// acc[i] += float(q[i]) * s, both roundings kept (no fused multiply-add): the value of an element is the rounded product.
-template <typename WireT> __device__ __forceinline__ void bsq_dequant_add(float* acc, const uint4& v, float s) {
-  constexpr __nv_fp8_interpretation_t I = std::is_same<WireT, __nv_fp8_e4m3>::value ? __NV_E4M3 : __NV_E5M2;
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int i = 0; i < 4; i++) {
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-      const __half2_raw r = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w[i] >> (16 * h)), I);   // F2FP.F16.E4M3 / E5M2.UNPACK_B
-      const float2 f = __half22float2(__half2(r));
-      acc[4 * i + 2 * h] = __fadd_rn(acc[4 * i + 2 * h], __fmul_rn(f.x, s));
-      acc[4 * i + 2 * h + 1] = __fadd_rn(acc[4 * i + 2 * h + 1], __fmul_rn(f.y, s));
-    }
-  }
-}
 
 // Dequantise vectors [0, nvec) of one rank's FP8 data into dst.
 template <typename WireT, typename OutT, typename Geom>
@@ -394,28 +379,34 @@ static b200collResult_t quant_prepare(b200collComm* c, b200collOp_t which, const
   return b200collSuccess;
 }
 
-// The FP8 copy (count bytes) and its scales (count / block fp32) of one call, in the symmetric heap. Taken with b200collMemAlloc on first
-// use and grown on demand: a collective contract like MemAlloc (every rank makes the same quantised calls in the same order, so every
-// rank gets the same offsets). A superseded scratch is never given back before CommDestroy: a CUDA graph captured earlier still
-// addresses it, and must stay valid when a later, larger call moves the scratch.
-static b200collResult_t quant_scratch(b200collComm* c, QuantCall* k) {
-  const size_t qbytes = k->count, need = qbytes + (size_t)k->g.nblk * 4;
+// The FP8 copy and its scales of one call, in the symmetric heap. Taken with b200collMemAlloc on first use and grown on demand: a
+// collective contract like MemAlloc (every rank makes the same quantised calls in the same order, so every rank gets the same offsets).
+// A superseded scratch is never given back before CommDestroy: a CUDA graph captured earlier still addresses it, and must stay valid
+// when a later, larger call moves the scratch.
+b200collResult_t quant_scratch_take(b200collComm* c, size_t need, const char* who, size_t* off) {
   if (c->quant_scratch_bytes < need) {
     void* p = nullptr;
     size_t bytes = std::max(need, 2 * c->quant_scratch_bytes);
     b200collResult_t rc = b200collMemAlloc(c, &p, bytes);
     if (rc != b200collSuccess && bytes != need) rc = b200collMemAlloc(c, &p, bytes = need);
     if (rc != b200collSuccess) {
-      set_last_error("quantised collectives: the symmetric arena cannot hold the " + std::to_string(need) + "-byte FP8 scratch (raise B200COLL_ARENA_MB)");
+      set_last_error(std::string(who) + ": the symmetric arena cannot hold the " + std::to_string(need) + "-byte FP8 scratch (raise B200COLL_ARENA_MB)");
       return rc;
     }
     if (c->quant_scratch) c->quant_scratch_retired.push_back(c->quant_scratch);
     c->quant_scratch = p;
     c->quant_scratch_bytes = bytes;
   }
-  k->g.data_off = arena_off(c, c->quant_scratch);
-  k->g.scale_off = k->g.data_off + qbytes;                        // count is a multiple of 16: the scales are 16-byte aligned
+  *off = arena_off(c, c->quant_scratch);
   return b200collSuccess;
+}
+
+// The FP8 copy (count bytes) and its scales (count / block fp32) of one call
+static b200collResult_t quant_scratch(b200collComm* c, QuantCall* k) {
+  const size_t qbytes = k->count;
+  const b200collResult_t rc = quant_scratch_take(c, qbytes + (size_t)k->g.nblk * 4, "quantised collectives", &k->g.data_off);
+  k->g.scale_off = k->g.data_off + qbytes;                        // count is a multiple of 16: the scales are 16-byte aligned
+  return rc;
 }
 
 // nranks == 1: the round trip in registers

@@ -136,4 +136,18 @@ void hostpath_destroy(b200collComm* c);
 // collectives.cu
 b200collResult_t launch_fill_sentinel(b200collComm* c, cudaStream_t s);
 
+// blockscaled.cu: `need` bytes of the quantising scratch that the quantising collectives and the quantising combine share, at arena offset
+// *off (the same on every rank); OutOfMemory, the message led by `who`, when the arena cannot hold it
+b200collResult_t quant_scratch_take(b200collComm* c, size_t need, const char* who, size_t* off);
+
+// dispatch.cu: one launch of k_a2av_quant_copy<in, wire> (no barrier): nvec 16-element vectors of `in` quantised into q and scales,
+// 2^lvpb vectors per block
+b200collResult_t launch_quant_copy(b200collComm* c, b200collDataType_t in_dtype, b200collDataType_t wire, const void* in, char* q, char* scales,
+                                   uint32_t nvec, uint32_t lvpb, cudaStream_t st);
+// dispatch.cu: once per device, load every kernel that can run behind a layout kernel or inside a quantising combine (lazy module loading)
+void routed_preload(const b200collComm* c);
+
+// combine.cu: load every combine kernel, wide and quantising (routed_preload calls it)
+void combine_preload();
+
 }  // namespace b200coll

@@ -4,7 +4,7 @@
 // row counts, one kernel:
 //
 //   k_a2av_quant_push<InT, WireT>   barrier, quantise my rows for every peer and push FP8 and scales into its recv, barrier (releases)
-//   k_a2av_quant_copy<InT, WireT>   one rank: a local quantising copy, no barrier
+//   k_a2av_quant_copy<InT, WireT>   one rank: a local quantising copy, no barrier; also the quantising combine's quantise pass
 //
 // Device-routed (b200collExpertDispatch, b200collExpertDispatchQuantized): the router's top-k expert ids in, rows grouped by expert out,
 // no host sync. Two kernels per call:
@@ -44,6 +44,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <mutex>
 #include <string>
 
 #include "a2av.h"
@@ -352,13 +353,20 @@ static b200collResult_t routed_prepare(b200collComm* c, const void* x, const voi
   return cross_check(c, b200collOpAllToAll, b200collAlgoTwoShot, row_elems, (size_t)num_experts, (size_t)q->block * 2 + (q->wire == b200collFloat8e5m2));
 }
 
-// Once per device, before the first layout kernel of either dispatch: its shared-memory limit, and every push kernel that can follow it
-// loaded. With lazy module loading the first launch of a kernel loads it, and the load waits for kernels already running: a push
-// launched for the first time behind a layout kernel that waits at its barrier for a rank driven by the same host thread would wait for
-// a launch that never comes. Whichever dispatch runs first on a device loads the other's push kernels too.
-static void routed_preload(const b200collComm* c) {
+// Once per device, before the first layout kernel of either dispatch and before the first quantising combine launches anything: the
+// layout kernel's shared-memory limit, and every kernel that can follow it loaded: both dispatches' push kernels, the quantise pass
+// k_a2av_quant_copy, and every combine kernel, wide and quantising. With lazy module loading the first launch of a kernel loads it, and
+// the load waits for kernels already running: a kernel launched for the first time behind a layout (or pull) kernel that waits at its
+// barrier for another rank's launch would hold that launch up, whether the other rank is driven by the same host thread or by another
+// thread waiting for the load. Whichever call runs first on a device loads the others' kernels too.
+// One thread loads at a time, and the others wait on the host: a thread that finds the work done makes no CUDA call here, so no load
+// can start after another rank's layout kernel is already running.
+void routed_preload(const b200collComm* c) {
   static std::atomic<unsigned long long> attr_done{0};          // per device, as in launch_bulk
+  static std::mutex mu;
   const unsigned long long bit = 1ull << (c->device & 63);
+  if (attr_done.load(std::memory_order_acquire) & bit) return;
+  const std::lock_guard<std::mutex> lk(mu);
   if (attr_done.load(std::memory_order_acquire) & bit) return;
   cudaFuncSetAttribute(k_routed_layout, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)layout_smem(kRouteMaxExperts));
   cudaFuncAttributes fa;
@@ -370,8 +378,23 @@ static void routed_preload(const b200collComm* c) {
         using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type;
         cudaFuncGetAttributes(&fa, k_expert_quant_push<InT, WireT, true>);
         cudaFuncGetAttributes(&fa, k_expert_quant_push<InT, WireT, false>);
+        cudaFuncGetAttributes(&fa, k_a2av_quant_copy<InT, WireT>);
       }); });
+  combine_preload();
   attr_done.fetch_or(bit, std::memory_order_acq_rel);
+}
+
+b200collResult_t launch_quant_copy(b200collComm* c, b200collDataType_t in_dtype, b200collDataType_t wire, const void* in, char* q, char* scales,
+                                   uint32_t nvec, uint32_t lvpb, cudaStream_t st) {
+  QuantGeom g = {};
+  g.nvec = nvec;
+  g.lvpb = lvpb;
+  return with_wide(in_dtype, [&](auto ti) { return with_fp8(wire, [&](auto tw) -> b200collResult_t {
+    using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type;
+    launch_k(k_a2av_quant_copy<InT, WireT>, copy_blocks(c, g.nvec), 256, st, g, static_cast<const char*>(in), q, scales);
+    LAUNCH_CHECK(c);
+    return b200collSuccess;
+  }); });
 }
 
 static b200collResult_t launch_layout(b200collComm* c, const int32_t* topk_idx, size_t slots, int num_experts, size_t recv_rows, int32_t* route,
@@ -446,18 +469,10 @@ b200collResult_t b200collAllToAllvQuantized(const void* send, void* recv, float*
   if (c->nranks == 1) {
     account(c, b200collOpAllToAll, in_bytes, b200collAlgoCopy);
     if (nv[0] == 0) return b200collSuccess;
-    QuantGeom g = {};
-    g.nvec = (uint32_t)nv[0];
-    g.lvpb = lvpb;
     const char* in = static_cast<const char*>(send) + a.src_vec[0] * 16 * b200collTypeSize(in_dtype);
     char* q = static_cast<char*>(recv) + a.dst_vec[0] * 16;
     char* s = reinterpret_cast<char*>(recv_scales) + (a.dst_vec[0] >> lvpb) * 4;
-    return with_wide(in_dtype, [&](auto ti) { return with_fp8(wire_dtype, [&](auto tw) -> b200collResult_t {
-      using InT = typename decltype(ti)::type; using WireT = typename decltype(tw)::type;
-      launch_k(k_a2av_quant_copy<InT, WireT>, copy_blocks(c, g.nvec), 256, st, g, in, q, s);
-      LAUNCH_CHECK(c);
-      return b200collSuccess;
-    }); });
+    return launch_quant_copy(c, in_dtype, wire_dtype, in, q, s, (uint32_t)nv[0], lvpb, st);
   }
   rc = cross_check(c, b200collOpAllToAll, b200collAlgoTwoShot, recv_rows, arena_off(c, recv), arena_off(c, recv_scales));
   if (rc != b200collSuccess) return rc;

@@ -1,5 +1,6 @@
-// The quantise side of the FP8 kernels, shared by the quantising collectives (blockscaled.cu) and the quantising dispatches
-// (dispatch.cu): the one walk over 16-element vectors, the load-and-widen of a vector, and the per-block quantiser.
+// The quantise side of the FP8 kernels, shared by the quantising collectives (blockscaled.cu), the quantising dispatches (dispatch.cu)
+// and the quantising combine (combine.cu): the one walk over 16-element vectors, the load-and-widen of a vector, the per-block
+// quantiser, and the dequantiser.
 //
 // Quantising, per block: amax = max |x| (the largest unsigned bit pattern of |x|, so a NaN anywhere makes amax NaN); inv = FMAX / amax
 // and s = amax / FMAX, both IEEE divisions rounded to nearest, inv = s = 1 when amax == 0 or inv overflows; q = fp8_satfinite(x * inv);
@@ -11,6 +12,8 @@
 #pragma once
 #include <math.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "device.cuh"
 
@@ -64,6 +67,30 @@ template <typename WireT> __device__ __forceinline__ uint4 quant_vec(const float
   Pack<WireT, 16>::run(y, w);                                     // cvt.rn.satfinite: F2FP.SATFINITE.E4M3 / .E5M2
   *scale = s;
   return make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+// x[i] = float(q[i]) * s for the 16 FP8 elements of v: the dequantised value of an element is the rounded product.
+template <typename WireT> __device__ __forceinline__ void dequant16(const uint4& v, float s, float* x) {
+  constexpr __nv_fp8_interpretation_t I = std::is_same<WireT, __nv_fp8_e4m3>::value ? __NV_E4M3 : __NV_E5M2;
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const __half2_raw r = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w[i] >> (16 * h)), I);   // F2FP.F16.E4M3 / E5M2.UNPACK_B
+      const float2 f = __half22float2(__half2(r));
+      x[4 * i + 2 * h] = __fmul_rn(f.x, s);
+      x[4 * i + 2 * h + 1] = __fmul_rn(f.y, s);
+    }
+  }
+}
+
+// acc[i] += float(q[i]) * s, both roundings kept (no fused multiply-add)
+template <typename WireT> __device__ __forceinline__ void bsq_dequant_add(float* acc, const uint4& v, float s) {
+  float x[16];
+  dequant16<WireT>(v, s, x);
+#pragma unroll
+  for (int i = 0; i < 16; i++) acc[i] = __fadd_rn(acc[i], x[i]);
 }
 
 // Quantise vectors [v0, v1) of in into q and its scales, walked as the pull loops walk a slice.

@@ -57,6 +57,8 @@ struct Opts {
   b200collDataType_t q_wire = b200collFloat8e4m3;
   int combine_k = 0;              // --combine K: the expert combine with top_k = K (0 = off)
   int route_e = 0, route_k = 0;   // --route E:K: the device-routed dispatch and combine, E experts, top-K (0 = off)
+  int cq_block = 0;               // --combine-quantize WIRE:BLOCK: the quantising combine in --combine / --route (0 = off)
+  b200collDataType_t cq_wire = b200collFloat8e4m3;
 };
 
 // Block-scaled mode: each rank's send buffer is a [rows, row_len] FP8 matrix with one fp32 scale per bs_rows x bs_cols block. Scales are
@@ -145,6 +147,32 @@ static float q_val(const Opts& o, int rank, size_t i, QMemo* memo) {
   return __half2float(__half(__nv_cvt_fp8_to_halfraw(q, o.q_wire == b200collFloat8e4m3 ? __NV_E4M3 : __NV_E5M2))) * memo->s;
 }
 
+// The quantising combine's host reference: n values quantised by the per-block rule (amax, two IEEE divisions, RNE saturating pack)
+// and dequantised with one multiply, in place.
+static void q_roundtrip(float* x, size_t n, int block, b200collDataType_t wire) {
+  const float fmax = wire == b200collFloat8e4m3 ? 448.0f : 57344.0f;
+  const __nv_fp8_interpretation_t I = wire == b200collFloat8e4m3 ? __NV_E4M3 : __NV_E5M2;
+  for (size_t b0 = 0; b0 < n; b0 += block) {
+    float amax = 0.0f;
+    for (size_t k = b0; k < b0 + block; k++) amax = std::max(amax, fabsf(x[k]));
+    volatile float a = amax;
+    float inv = fmax / a, s = a / fmax;
+    if (amax == 0.0f || isinf(inv)) inv = s = 1.0f;
+    for (size_t k = b0; k < b0 + block; k++) {
+      const __nv_fp8_storage_t q = __nv_cvt_float_to_fp8(x[k] * inv, __NV_SATFINITE, I);
+      volatile float v = __half2float(__half(__nv_cvt_fp8_to_halfraw(q, I))) * s;
+      x[k] = v;
+    }
+  }
+}
+// The quantising combine's scratch (FP8 copy plus scales of every expert_out row) grows with the sweep and keeps every superseded
+// buffer: reserve twice the largest one.
+static size_t cq_scratch_bytes(const Opts& o) {
+  if (!o.cq_block) return 0;
+  const size_t elems = o.max_bytes / b200collTypeSize(o.in_dt) * (o.route_e ? o.route_k : 1);
+  return 2 * (elems + elems / o.cq_block * 4) + (4u << 20);
+}
+
 template <typename T> __global__ void k_fill(T* p, size_t n, int rank, size_t base) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     size_t g = base + i;
@@ -210,9 +238,14 @@ static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out,
   const b200collEpilogue ep{o.in_dt, o.out_dt, o.scale};
   int gen_ctr[4] = {0, 0, 0, 0};
   long total_errors = 0;
-  if (rank == 0) {
+  if (rank == 0 && o.cq_block) {
+    printf("# b200coll_perf op=alltoall quantising combine top_k=%d nranks=%d in=%s wire=%s block=%d out=%s scale=%g row_len=%zu: size = expert_out bytes per rank\n",
+           K, n, dt_name(o.in_dt), dt_name(o.cq_wire), o.cq_block, dt_name(o.out_dt), o.scale, row);
+  } else if (rank == 0) {
     printf("# b200coll_perf op=alltoall combine top_k=%d nranks=%d in=%s out=%s scale=%g row_len=%zu: size = expert_out bytes read per rank\n", K, n, dt_name(o.in_dt),
            dt_name(o.out_dt), o.scale, row);
+  }
+  if (rank == 0) {
     printf("#%13s %12s %6s %8s | %10s %8s %6s\n", "size(B)", "tokens", "type", "algo", "us", "algbw", "#wrong");
     fflush(stdout);
   }
@@ -243,7 +276,11 @@ static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out,
     RT(cudaGetLastError());
     RT(cudaMemsetAsync(out, 0x5A, out_elems * os, st));
     auto launch = [&] {
-      CC(b200collAllToAllvCombine(expert_out, out, row, recv_rows, rows.data(), soff.data(), roff.data(), d_idx, d_w, tokens, K, &ep, ctx.comm, st));
+      if (o.cq_block)
+        CC(b200collAllToAllvCombineQuantized(expert_out, out, row, recv_rows, rows.data(), soff.data(), roff.data(), d_idx, d_w, tokens, K, o.cq_wire,
+                                             o.cq_block, &ep, ctx.comm, st));
+      else
+        CC(b200collAllToAllvCombine(expert_out, out, row, recv_rows, rows.data(), soff.data(), roff.data(), d_idx, d_w, tokens, K, &ep, ctx.comm, st));
     };
     long errs = 0;
     if (o.check) {
@@ -254,6 +291,10 @@ static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out,
       spin_barrier(sh, 1, n, &gen_ctr[1]);
       std::vector<char> host(out_elems * os);
       RT(cudaMemcpy(host.data(), out, host.size(), cudaMemcpyDeviceToHost));
+      // --combine-quantize: the rows this rank reads (rows [rank * rpp, + rpp) of every peer's expert_out), quantised and dequantised
+      std::vector<float> deq(o.cq_block ? (size_t)n * rpp * row : 0);
+      for (size_t i = 0; i < deq.size(); i++) deq[i] = co_val((int)(i / (rpp * row)), (size_t)rank * rpp * row + i % (rpp * row));
+      for (size_t r = 0; r < deq.size() / row; r++) q_roundtrip(deq.data() + r * row, row, o.cq_block, o.cq_wire);
       for (size_t t = 0; t < tokens; t++) {
         for (size_t e = 0; e < row; e++) {
           float acc = 0.0f;
@@ -262,7 +303,7 @@ static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out,
             if (i < 0) continue;
             const int p = (int)(i / (int64_t)rpp);                      // the range row i lies in, and its row of p's expert_out
             const size_t r = (size_t)rank * rpp + (size_t)(i - soff[p]);
-            volatile float prod = w[t * K + j] * co_val(p, r * row + e);
+            volatile float prod = w[t * K + j] * (o.cq_block ? deq[((size_t)p * rpp + (size_t)(i - soff[p])) * row + e] : co_val(p, r * row + e));
             acc = acc + prod;
           }
           const uint32_t want = out_bits(acc * o.scale, o.out_dt), got = got_bits(host.data(), t * row + e, o.out_dt);
@@ -333,6 +374,9 @@ static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream
   if (rank == 0 && quant) {
     printf("# b200coll_perf op=alltoall routed FP8 dispatch experts=%d top_k=%d nranks=%d in=%s wire=%s block=%d row_len=%zu: size = x bytes per rank; combine not run\n",
            E, K, n, dt_name(o.in_dt), dt_name(o.q_wire), o.q_block, row);
+  } else if (rank == 0 && o.cq_block) {
+    printf("# b200coll_perf op=alltoall routed dispatch + quantising combine experts=%d top_k=%d nranks=%d in=%s wire=%s block=%d out=%s scale=%g row_len=%zu: "
+           "size = x bytes per rank\n", E, K, n, dt_name(o.in_dt), dt_name(o.cq_wire), o.cq_block, dt_name(o.out_dt), o.scale, row);
   } else if (rank == 0) {
     printf("# b200coll_perf op=alltoall routed dispatch + combine experts=%d top_k=%d nranks=%d in=%s out=%s scale=%g row_len=%zu: size = x bytes per rank\n", E, K,
            n, dt_name(o.in_dt), dt_name(o.out_dt), o.scale, row);
@@ -386,7 +430,10 @@ static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream
       else
         CC(b200collExpertDispatch(x, recv, row, recv_rows, d_idx, tokens, K, E, d_counts, d_route, d_dropped, o.in_dt, ctx.comm, st));
     };
-    auto combine = [&] { CC(b200collExpertCombine(recv, out, row, recv_rows, d_route, d_w, tokens, K, &ep, ctx.comm, st)); };
+    auto combine = [&] {
+      if (o.cq_block) CC(b200collExpertCombineQuantized(recv, out, row, recv_rows, d_route, d_w, tokens, K, o.cq_wire, o.cq_block, &ep, ctx.comm, st));
+      else CC(b200collExpertCombine(recv, out, row, recv_rows, d_route, d_w, tokens, K, &ep, ctx.comm, st));
+    };
     long errs = 0;
     auto bad = [&](const char* what, size_t a, long long got, long long want) {
       if (errs < 4) fprintf(stderr, "rank %d route size %zu %s %zu: got %lld want %lld\n", rank, bytes, what, a, got, want);
@@ -449,13 +496,17 @@ static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream
         const long long want = rowof[rank][i] < 0 ? -1 : (long long)(ids[rank][i] / epr) * (long long)recv_rows + rowof[rank][i];
         if (h_route[i] != want) bad("route", i, h_route[i], want);
       }
-      // the combine of identity experts: every stored slot of token t brings back t's own row
+      // the combine of identity experts: every stored slot of token t brings back t's own row (--combine-quantize: quantised and
+      // dequantised, blocks along the row)
+      std::vector<float> xrow(row);
       for (size_t t = 0; t < tokens && !quant; t++) {
+        for (size_t e = 0; e < row; e++) xrow[e] = gen(rank, t * row + e);
+        if (o.cq_block) q_roundtrip(xrow.data(), row, o.cq_block, o.cq_wire);
         for (size_t e = 0; e < row; e++) {
           float acc = 0.0f;
           for (int j = 0; j < K; j++) {
             if (rowof[rank][t * K + j] < 0) continue;
-            volatile float prod = w[t * K + j] * gen(rank, t * row + e);
+            volatile float prod = w[t * K + j] * xrow[e];
             acc = acc + prod;
           }
           const uint32_t want = out_bits(acc * o.scale, o.out_dt), got = got_bits(h_out.data(), t * row + e, o.out_dt);
@@ -875,6 +926,14 @@ int main(int argc, char** argv) {
       }
       o.q_wire = parse_dt(wire);
     }
+    else if (a == "--combine-quantize") {
+      char wire[16] = {};
+      if (sscanf(next(), "%15[a-z0-9]:%d", wire, &o.cq_block) != 2 || (strcmp(wire, "e4m3") && strcmp(wire, "e5m2")) || o.cq_block < 16 || o.cq_block > 512 ||
+          (o.cq_block & (o.cq_block - 1))) {
+        fprintf(stderr, "--combine-quantize WIRE:BLOCK: WIRE e4m3 or e5m2, BLOCK 16, 32, 64, 128, 256 or 512\n"); return 1;
+      }
+      o.cq_wire = parse_dt(wire);
+    }
     else if (a == "--combine") { o.combine_k = atoi(next()); if (o.combine_k < 1) { fprintf(stderr, "--combine K: K >= 1\n"); return 1; } }
     else if (a == "--route") {
       if (sscanf(next(), "%d:%d", &o.route_e, &o.route_k) != 2 || o.route_e < 1 || o.route_e > 1024 || o.route_k < 1) { fprintf(stderr, "--route E:K: 1 <= E <= 1024, K >= 1\n"); return 1; }
@@ -930,6 +989,10 @@ int main(int argc, char** argv) {
            "                            WIRE with one fp32 scale per BLOCK elements (--row-len a multiple of BLOCK); reports the dispatch only (the\n"
            "                            combine needs a wide expert_out); -c 1 checks every FP8 byte, scale, count, route and dropped against the\n"
            "                            host layout and the host quantiser\n"
+           "  --combine-quantize WIRE:BLOCK   with --combine K or --route E:K (no --quantize): the quantising combine in place of the wide one;\n"
+           "                            each rank quantises its whole expert_out to WIRE (e4m3|e5m2) with one fp32 scale per BLOCK elements\n"
+           "                            (--row-len a multiple of BLOCK) and the slots pull FP8 rows and scales; -c 1 checks every output element bit\n"
+           "                            for bit against the host quantiser and the slot-order reference\n"
            "  --algo auto|ll|ll2|oneshot|twoshot|nvls   --inplace 0|1|2   --max-ctas N   --sweep kind:ctas:threads,...   --json FILE   --window SIZE\n"
            "  --selfcheck               report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;
@@ -937,6 +1000,11 @@ int main(int argc, char** argv) {
     else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 1; }
   }
   if (o.factor < 2) o.factor = 2;
+  if (o.cq_block && ((!o.combine_k && !o.route_e) || o.q_block || o.bs_rows || o.row_len % o.cq_block != 0)) {
+    fprintf(stderr, "--combine-quantize WIRE:BLOCK takes --combine K or --route E:K, a --row-len that is a multiple of BLOCK, and no --quantize or\n"
+                    "--block-scale\n");
+    return 1;
+  }
   if (o.q_block && o.op == "alltoall" && !out_given) o.out_dt = o.q_wire;     // the quantising alltoall receives the wire type
   if (o.bs_rows && (o.row_len == 0 || o.row_len % 16)) { fprintf(stderr, "--row-len must be a positive multiple of 16\n"); return 1; }
   const LauncherRank lr = launcher_rank();
@@ -957,7 +1025,7 @@ int main(int argc, char** argv) {
     b200collConfig cfg; b200collConfigDefault(&cfg);
     const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
     if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o) +
-                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o);     // --route: recv holds K rows per token
+                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o);     // --route: recv holds K rows per token
     b200collUniqueId id; CC(b200collUniqueIdFromString(("perf/" + lr.job).c_str(), &id));
     RT(cudaSetDevice(dev));
     b200collComm_t comm;
@@ -986,7 +1054,7 @@ int main(int argc, char** argv) {
   // arena: two windows (+ max buffers) and slack
   const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
   size_t need = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o) +
-                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o);     // --route: recv holds K rows per token
+                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o);     // --route: recv holds K rows per token
   if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = need;
   if (o.procs) {
     b200collUniqueId id; CC(b200collGetUniqueId(&id));

@@ -143,6 +143,9 @@ def load() -> C.CDLL:
     L.b200collExpertDispatch.argtypes = [vp, vp, sz, sz, i32p, sz, ci, ci, i32p, i32p, i32p, ci, vp, vp]
     L.b200collExpertDispatchQuantized.argtypes = [vp, vp, C.POINTER(C.c_float), sz, sz, i32p, sz, ci, ci, i32p, i32p, i32p, ci, ci, ci, vp, vp]
     L.b200collExpertCombine.argtypes = [vp, vp, sz, sz, i32p, C.POINTER(C.c_float), sz, ci, C.POINTER(Epilogue), vp, vp]
+    L.b200collAllToAllvCombineQuantized.argtypes = [vp, vp, sz, sz, i64p, i64p, i64p, i32p, C.POINTER(C.c_float), sz, ci, ci, ci, C.POINTER(Epilogue),
+                                                    vp, vp]
+    L.b200collExpertCombineQuantized.argtypes = [vp, vp, sz, sz, i32p, C.POINTER(C.c_float), sz, ci, ci, ci, C.POINTER(Epilogue), vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -340,18 +343,40 @@ def check_all_to_all_v_quantized(nranks: int, src, out, out_scales, row_elems: i
     return torch_dtype_code(src.dtype), torch_dtype_code(out.dtype)
 
 
-def check_all_to_all_v_combine(nranks: int, expert_out, out, row_elems: int, send_rows, send_row_off, recv_row_off_at_peer, index,
-                               weights) -> tuple[int, int]:
-    """Rules of the expert combine, checked on the tensors' metadata and the host lists only (no communicator, no library call): raises
-    ValueError, returns the library codes of (expert_out's type, out's type). expert_out and out: contiguous bfloat16, float16 or float32;
-    row_elems a positive multiple of 16 dividing expert_out.numel(); index: contiguous int32 [tokens, top_k] with top_k >= 1; weights:
-    None or contiguous float32 of index's shape; out.numel() == tokens * row_elems. The three lists have nranks non-negative entries,
-    the non-empty send ranges [send_row_off[p], + send_rows[p]) are disjoint, and every destination range [recv_row_off_at_peer[p],
-    + send_rows[p]) lies inside expert_out, in rows of row_elems elements. out must not overlap expert_out, index or weights."""
+def _check_combine_quant(fp8, row_elems: int) -> int:
+    """The quantising combine's own rules, fp8 = (block, wire): wire torch.float8_e4m3fn (None) or torch.float8_e5m2, block one of
+    QUANT_BLOCKS and row_elems a positive multiple of it. Returns the wire type's library code."""
+    import torch
+    block, wire = fp8
+    wire = torch.float8_e4m3fn if wire is None else wire
+    if wire not in (torch.float8_e4m3fn, torch.float8_e5m2):
+        raise ValueError(f"wire must be torch.float8_e4m3fn or torch.float8_e5m2, not {wire}")
+    _check_block(block)
+    if isinstance(row_elems, bool) or not isinstance(row_elems, int) or row_elems <= 0 or row_elems % block:
+        raise ValueError(f"row_elems must be a positive multiple of block ({block}), got {row_elems!r}")
+    return torch_dtype_code(wire)
+
+
+def _check_combine_sizes(tokens: int, top_k: int, row_elems: int, eo_rows: int) -> None:
+    """The quantising combine's 32-bit limits: tokens * top_k slots, the 16-element vectors of out and of expert_out."""
+    if tokens * top_k > _I31:
+        raise ValueError("tokens * top_k must be at most 2^31 - 1")
+    if tokens * (row_elems // 16) > _I31:
+        raise ValueError("at most 2^31 - 1 16-element vectors of out (tokens * row_elems / 16)")
+    if eo_rows * (row_elems // 16) > _I31:
+        raise ValueError("at most 2^31 - 1 16-element vectors of expert_out (expert_out.numel() / 16)")
+
+
+def _check_a2av_combine(nranks: int, expert_out, out, row_elems: int, send_rows, send_row_off, recv_row_off_at_peer, index, weights,
+                        fp8=None) -> tuple:
+    """The rules of both all-to-all-v combines; fp8 is None (check_all_to_all_v_combine) or (block, wire), which adds the quantising
+    call's rules, as combine_prepare in coll/src/combine.cu takes a CombineQuant."""
     import torch
     _check_wide("expert_out", expert_out)
     _check_wide("out", out)
-    if isinstance(row_elems, bool) or not isinstance(row_elems, int) or row_elems <= 0 or row_elems % 16:
+    if fp8 is not None:
+        wc = _check_combine_quant(fp8, row_elems)
+    elif isinstance(row_elems, bool) or not isinstance(row_elems, int) or row_elems <= 0 or row_elems % 16:
         raise ValueError(f"row_elems must be a positive multiple of 16, got {row_elems!r}")
     if expert_out.numel() % row_elems:
         raise ValueError(f"expert_out.numel() ({expert_out.numel()}) must be a multiple of row_elems ({row_elems})")
@@ -362,6 +387,8 @@ def check_all_to_all_v_combine(nranks: int, expert_out, out, row_elems: int, sen
     if out.numel() != tokens * row_elems:
         raise ValueError(f"out must hold tokens * row_elems = {tokens * row_elems} elements, got {out.numel()}")
     eo_rows = expert_out.numel() // row_elems
+    if fp8 is not None:
+        _check_combine_sizes(tokens, top_k, row_elems, eo_rows)
     ranges = []
     for p, (rows, so, ro) in enumerate(_host_rows(nranks, send_rows, send_row_off, recv_row_off_at_peer)):
         if ro + rows > eo_rows:
@@ -375,7 +402,28 @@ def check_all_to_all_v_combine(nranks: int, expert_out, out, row_elems: int, sen
     for name, t in (("expert_out", expert_out), ("index", index), ("weights", weights)):
         if t is not None and _overlap(out, t):
             raise ValueError(f"out must not overlap {name}")
-    return torch_dtype_code(expert_out.dtype), torch_dtype_code(out.dtype)
+    codes = (torch_dtype_code(expert_out.dtype), torch_dtype_code(out.dtype))
+    return codes if fp8 is None else codes + (wc,)
+
+
+def check_all_to_all_v_combine(nranks: int, expert_out, out, row_elems: int, send_rows, send_row_off, recv_row_off_at_peer, index,
+                               weights) -> tuple[int, int]:
+    """Rules of the expert combine, checked on the tensors' metadata and the host lists only (no communicator, no library call): raises
+    ValueError, returns the library codes of (expert_out's type, out's type). expert_out and out: contiguous bfloat16, float16 or float32;
+    row_elems a positive multiple of 16 dividing expert_out.numel(); index: contiguous int32 [tokens, top_k] with top_k >= 1; weights:
+    None or contiguous float32 of index's shape; out.numel() == tokens * row_elems. The three lists have nranks non-negative entries,
+    the non-empty send ranges [send_row_off[p], + send_rows[p]) are disjoint, and every destination range [recv_row_off_at_peer[p],
+    + send_rows[p]) lies inside expert_out, in rows of row_elems elements. out must not overlap expert_out, index or weights."""
+    return _check_a2av_combine(nranks, expert_out, out, row_elems, send_rows, send_row_off, recv_row_off_at_peer, index, weights)
+
+
+def check_all_to_all_v_combine_quantized(nranks: int, expert_out, out, row_elems: int, send_rows, send_row_off, recv_row_off_at_peer, index,
+                                         weights, block: int = 128, wire=None) -> tuple[int, int, int]:
+    """Rules of the quantising all-to-all-v combine, checked on the tensors' metadata and the host lists only: raises ValueError, returns
+    the library codes of (expert_out's type, out's type, the wire type). Everything check_all_to_all_v_combine checks, and: wire
+    torch.float8_e4m3fn (None, the default) or torch.float8_e5m2; block one of QUANT_BLOCKS and row_elems a positive multiple of it;
+    tokens * top_k, tokens * row_elems / 16 and expert_out.numel() / 16 at most 2^31 - 1."""
+    return _check_a2av_combine(nranks, expert_out, out, row_elems, send_rows, send_row_off, recv_row_off_at_peer, index, weights, fp8=(block, wire))
 
 
 MAX_EXPERTS = 1024
@@ -473,16 +521,14 @@ def check_expert_dispatch_quantized(nranks: int, x, topk_idx, num_experts: int, 
     return torch_dtype_code(x.dtype), torch_dtype_code(recv.dtype)
 
 
-def check_expert_combine(nranks: int, expert_out, route, weights, out) -> tuple[int, int]:
-    """Rules of the expert combine from a device route, checked on the tensors' metadata only: raises ValueError, returns the library
-    codes of (expert_out's type, out's type). out: contiguous bfloat16, float16 or float32 [tokens, row_elems], row_elems a positive
-    multiple of 16; expert_out: contiguous bfloat16, float16 or float32 of whole rows; route: contiguous int32 [tokens, top_k], top_k >= 1;
-    weights: None or contiguous float32 of route's shape. nranks * expert_out rows is at most 2^31 - 1. out must not overlap expert_out,
-    route or weights."""
+def _check_expert_combine(nranks: int, expert_out, route, weights, out, fp8=None) -> tuple:
+    """The rules of both expert combines; fp8 is None (check_expert_combine) or (block, wire), which adds the quantising call's rules."""
     import torch
     _check_wide("out", out, rows=True)
     tokens, row_elems = out.shape
-    if row_elems <= 0 or row_elems % 16:
+    if fp8 is not None:
+        wc = _check_combine_quant(fp8, row_elems)
+    elif row_elems <= 0 or row_elems % 16:
         raise ValueError(f"row_elems (out.shape[1] = {row_elems}) must be a positive multiple of 16")
     if expert_out.dtype not in (torch.bfloat16, torch.float16, torch.float32) or not expert_out.is_contiguous() or expert_out.numel() % row_elems:
         raise ValueError(f"expert_out must be a contiguous bfloat16, float16 or float32 tensor of whole {row_elems}-element rows, got {expert_out.dtype}")
@@ -494,10 +540,30 @@ def check_expert_combine(nranks: int, expert_out, route, weights, out) -> tuple[
         raise ValueError("tokens * top_k must be at most 2^31 - 1")
     if nranks * (expert_out.numel() // row_elems) > _I31:
         raise ValueError("nranks * expert_out rows must be at most 2^31 - 1 (a route is an int32)")
+    if fp8 is not None:
+        _check_combine_sizes(tokens, route.shape[1], row_elems, expert_out.numel() // row_elems)
     for name, t in (("expert_out", expert_out), ("route", route), ("weights", weights)):
         if t is not None and _overlap(out, t):
             raise ValueError(f"out must not overlap {name}")
-    return torch_dtype_code(expert_out.dtype), torch_dtype_code(out.dtype)
+    codes = (torch_dtype_code(expert_out.dtype), torch_dtype_code(out.dtype))
+    return codes if fp8 is None else codes + (wc,)
+
+
+def check_expert_combine(nranks: int, expert_out, route, weights, out) -> tuple[int, int]:
+    """Rules of the expert combine from a device route, checked on the tensors' metadata only: raises ValueError, returns the library
+    codes of (expert_out's type, out's type). out: contiguous bfloat16, float16 or float32 [tokens, row_elems], row_elems a positive
+    multiple of 16; expert_out: contiguous bfloat16, float16 or float32 of whole rows; route: contiguous int32 [tokens, top_k], top_k >= 1;
+    weights: None or contiguous float32 of route's shape. nranks * expert_out rows is at most 2^31 - 1. out must not overlap expert_out,
+    route or weights."""
+    return _check_expert_combine(nranks, expert_out, route, weights, out)
+
+
+def check_expert_combine_quantized(nranks: int, expert_out, route, weights, out, block: int = 128, wire=None) -> tuple[int, int, int]:
+    """Rules of the quantising expert combine from a device route, checked on the tensors' metadata only: raises ValueError, returns the
+    library codes of (expert_out's type, out's type, the wire type). Everything check_expert_combine checks, and: wire
+    torch.float8_e4m3fn (None, the default) or torch.float8_e5m2; block one of QUANT_BLOCKS and row_elems (out.shape[1]) a positive
+    multiple of it; tokens * row_elems / 16 and expert_out.numel() / 16 at most 2^31 - 1."""
+    return _check_expert_combine(nranks, expert_out, route, weights, out, fp8=(block, wire))
 
 
 class _CudaArray:
@@ -898,6 +964,40 @@ class Comm:
         _check(load().b200collExpertCombine(C.c_void_p(expert_out.data_ptr()), C.c_void_p(out.data_ptr()), row_elems, expert_out.numel() // row_elems,
                                             C.cast(C.c_void_p(route.data_ptr()), C.POINTER(C.c_int32)), w, tokens, route.shape[1], C.byref(ep),
                                             self._h, self._stream(stream)), "ExpertCombine")
+        return out
+
+    def all_to_all_v_combine_quantized(self, expert_out, out, row_elems: int, send_rows, send_row_off, recv_row_off_at_peer, index, weights=None,
+                                       block: int = 128, wire=None, scale: float = 1.0, stream=None):
+        """all_to_all_v_combine with FP8 on the wire (b200collAllToAllvCombineQuantized): every row of this rank's expert_out (bf16, fp16 or
+        fp32, any device tensor) is quantised on this rank to `wire` (torch.float8_e4m3fn, the default, or torch.float8_e5m2) with one
+        fp32 scale per `block` elements, and the slots pull FP8 rows and scales: out[t] = round(scale * sum over slots in slot order of
+        weights[t, j] * float(q) * s). Returns out. The scratch comes from the arena: the same calls in the same order on every rank."""
+        ic, oc, wc = check_all_to_all_v_combine_quantized(self.nranks, expert_out, out, row_elems, send_rows, send_row_off, recv_row_off_at_peer, index,
+                                                          weights, block, wire)
+        arr = self._rows
+        tokens, top_k = index.shape
+        ep = Epilogue(ic, oc, float(scale))
+        w = C.cast(C.c_void_p(weights.data_ptr() if weights is not None else None), C.POINTER(C.c_float))
+        _check(load().b200collAllToAllvCombineQuantized(C.c_void_p(expert_out.data_ptr()), C.c_void_p(out.data_ptr()), row_elems,
+                                                        expert_out.numel() // row_elems, arr(send_rows), arr(send_row_off), arr(recv_row_off_at_peer),
+                                                        C.cast(C.c_void_p(index.data_ptr()), C.POINTER(C.c_int32)), w, tokens, top_k, wc, block,
+                                                        C.byref(ep), self._h, self._stream(stream)), "AllToAllvCombineQuantized")
+        return out
+
+    def expert_combine_quantized(self, expert_out, route, weights, out, block: int = 128, wire=None, scale: float = 1.0, stream=None):
+        """expert_combine with FP8 on the wire (b200collExpertCombineQuantized): every row of this rank's expert_out (bf16, fp16 or fp32,
+        any device tensor, for example a grouped GEMM's output) is quantised on this rank to `wire` (torch.float8_e4m3fn, the default, or
+        torch.float8_e5m2) with one fp32 scale per `block` elements; each slot pulls its FP8 row and scales from the peer the route names,
+        and out[t] = round(scale * sum over slots in slot order of weights[t, j] * float(q) * s). Returns out. The scratch comes from the
+        arena: the same calls in the same order on every rank."""
+        ic, oc, wc = check_expert_combine_quantized(self.nranks, expert_out, route, weights, out, block, wire)
+        tokens, row_elems = out.shape
+        ep = Epilogue(ic, oc, float(scale))
+        w = C.cast(C.c_void_p(weights.data_ptr() if weights is not None else None), C.POINTER(C.c_float))
+        _check(load().b200collExpertCombineQuantized(C.c_void_p(expert_out.data_ptr()), C.c_void_p(out.data_ptr()), row_elems,
+                                                     expert_out.numel() // row_elems, C.cast(C.c_void_p(route.data_ptr()), C.POINTER(C.c_int32)), w,
+                                                     tokens, route.shape[1], wc, block, C.byref(ep), self._h, self._stream(stream)),
+               "ExpertCombineQuantized")
         return out
 
     def broadcast(self, src, dst=None, root: int = 0, scale: float = 1.0, stream=None):
