@@ -464,6 +464,36 @@ b200collResult_t b200collExpertCombineQuantized(const void* expert_out, void* ou
                                                 const float* weights, size_t tokens, int top_k, b200collDataType_t wire_dtype, int block,
                                                 const b200collEpilogue* ep, b200collComm_t comm, b200collStream_t stream);
 
+/* --- fused all-reduce, residual add and RMSNorm (src/rmsnorm.cu): the step after the attention output projection and the MLP down
+ * projection of a pre-norm tensor-parallel block, one kernel per call. x is this rank's [rows, row_len] partial sums, residual
+ * [rows, row_len] (the same on every rank in tensor parallelism), gamma [row_len], all of `dtype` (bf16, fp16 or fp32), as is out. Per row
+ * and element e, in fp32, every product and sum rounded on its own (no fused multiply-add):
+ *   1. h[e] = round_dtype(((+0 + x_0[e]) + x_1[e] + ... + x_{N-1}[e]) + residual[e]): ranks summed in rank order, one rounding at the
+ *      end. h is written back into residual, in place (the new residual stream).
+ *   2. sq[e] = h[e] * h[e], with h as stored (the norm sees exactly the residual the next layer reads).
+ *   3. p[c] = the sum of the 16 sq of chunk c (elements 16c .. 16c+15) in element order from +0; p padded with +0 to the next power of
+ *      two P, then folded p = p[:P/2] + p[P/2:] until one value is left.
+ *   4. ms = fold / row_len, inv = 1 / sqrt(ms + eps): IEEE division and square root, rounded to nearest (no rsqrt approximation).
+ *   5. out[e] = round_dtype((h[e] * inv) * gamma[e]).
+ * Rounding is RNE; NaN and inf propagate as the arithmetic makes them (an all-zero row with eps = 0 gives NaN). The result depends only on
+ * the values and the rank count, not on the algorithm or the launch shape. Every rank holds the same out and new residual provided the
+ * ranks passed the same residual (the caller's condition); on two-shot a row comes from the residual of the rank that owns it.
+ * Algorithms (the tuner's all-reduce pick for rows * row_len * sizeof(dtype) bytes, or the forced algorithm): ll, ll2 and oneshot ->
+ * oneshot (every rank pulls every row of every peer's x and stores residual and out locally); twoshot and nvls -> twoshot (rank r pulls
+ * rows [rows*r/N, rows*(r+1)/N), pushes their residual and out rows into every rank), which needs residual and out in the arena and falls
+ * back to oneshot otherwise. Each rank decides from its own buffers, so residual and out must be placed alike on every rank: in the arena
+ * at the same offsets everywhere, or outside it everywhere (B200COLL_CHECK=1 cross-checks rows, row_len, the offsets and the algorithm
+ * and turns a disagreement into InvalidUsage on multi-process communicators). The kernel ends with a releasing barrier, so the caller
+ * may overwrite x right after the call.
+ * Arguments (InvalidArgument, message in b200collGetLastError, nothing launched): dtype bf16, fp16 or fp32; row_len a multiple of 16 in
+ * [16, 16384]; eps finite and >= 0; rows < 2^31; no null pointer when rows > 0; x, residual, gamma and out 16-byte aligned; out must not
+ * overlap x, residual or gamma, residual must not overlap x or gamma. More than one rank: x in the symmetric arena at the same offset on
+ * every rank, else InvalidUsage. A poisoned communicator gives RemoteError. rows == 0 still launches on every rank (peers' barriers wait
+ * for it), one-shot, and reads and writes nothing, so its pointers may lie anywhere or be null. One rank: a local kernel, no barrier, any device buffers. b200collStats count an allreduce of rows * row_len * sizeof(dtype)
+ * bytes under oneshot, twoshot or copy, one kernel launch. */
+b200collResult_t b200collAllReduceRmsNorm(const void* x, void* residual, const void* gamma, void* out, size_t rows, size_t row_len,
+                                          float eps, b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
+
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.
  * AllReduceHost is the end-to-end step "pinned host -> GPU -> all-reduce -> pinned host" as one asynchronous call on `stream`:

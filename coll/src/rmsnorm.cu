@@ -1,0 +1,298 @@
+// libb200coll fused all-reduce, residual add and RMSNorm (b200collAllReduceRmsNorm): the step that follows the attention output projection
+// and the MLP down projection of every pre-norm tensor-parallel block, one kernel per call:
+//
+//   k_rms_local<T>       one rank: residual = h, out = norm(h) for every row, no barrier
+//   k_rms_oneshot<T>     relaxed barrier, pull every row of every rank's x in rank order, store residual and out locally, releasing barrier
+//   k_rms_twoshot<T>     relaxed barrier, pull my row slice, push its residual and out rows into every rank's residual and out, releasing
+//                        barrier
+//
+// One CTA (kRmsThreads threads) owns one row at a time, walking rows b, b + gridDim.x, ... of its range. Thread t holds the 16-element
+// chunks t and t + kRmsThreads (row_len <= 16384 is at most 1024 chunks), so the new residual h of a whole row stays in registers
+// between the sum and the normalisation.
+//
+// Order, and why the result does not depend on the launch shape. h[e] is (+0 + x_0[e]) + ... + x_{N-1}[e] + residual[e] in fp32, in that
+// order, rounded once. The chunk sums p[c] add their 16 squares of the rounded h in element order from +0. The header's fold pads p with
+// +0 to the next power of two P and halves it, p[i] + p[i + P/2]; this kernel pads to 1024 instead. Every p[c] is +0, positive, +inf or
+// NaN (squares and their sums are never -0), and x + (+0) is exactly x for all of them, so the levels above P only add +0 to the values
+// the header's fold starts from: the same bits. The levels then run in the same index order: chunk t + 512 onto chunk t in registers;
+// bits 8..5 of the chunk index across the CTA's warps through shared memory, every warp folding all 512 values itself (so no second
+// block barrier); bits 4..0 in the lane butterfly xor 16, 8, 4, 2, 1. Lane i of a butterfly step adds its partner's value to its own,
+// so lanes above the partner add in the opposite order. IEEE addition is commutative and a NaN sum is the canonical NaN either way, so
+// every lane ends with lane 0's bits. Every product and sum is __fmul_rn / __fadd_rn (no FFMA contraction), and ms, sqrt and 1 / sqrt
+// are the correctly rounded __fdiv_rn and __fsqrt_rn.
+//
+// Ordering. The entry barrier is relaxed, as in the pull-reduce all-reduce: every x was written by an earlier kernel on its rank's stream,
+// and a peer arrives only once its stream has reached this call. One-shot writes only its own residual and out. Two-shot writes rows of
+// slice r only from rank r, into every rank's residual and out; rank p reads only the rows of slice p from its own residual, and a rank
+// reaches the entry barrier only after everything earlier on its stream (a GEMM reading out) is done, so no store lands on a row that is
+// still read. The closing barrier releases the two-shot stores to every rank and tells each rank that nobody pulls its x any more, so the
+// caller may overwrite x right after the call. Both barriers pair CTA b with CTA b, and every rank launches full_grid's CTAs whatever its
+// row count.
+#include <stdint.h>
+
+#include <atomic>
+#include <mutex>
+#include <string>
+
+#include "comm.h"
+#include "launch.cuh"
+
+namespace b200coll {
+
+constexpr int kRmsThreads = 512, kRmsWarps = kRmsThreads / 32;       // the fold below is written for 16 warps
+constexpr int kRmsMaxChunks = 2 * kRmsThreads;               // 16384 elements
+constexpr size_t kRmsMaxRowLen = 16 * (size_t)kRmsMaxChunks;
+
+// 16 elements of T at p, widened to fp32 bit for bit
+template <typename T> __device__ __forceinline__ void rms_load16(const char* p, float* x) {
+  uint4 raw[sizeof(T)];
+#pragma unroll
+  for (int k = 0; k < (int)sizeof(T); k++) raw[k] = ld_vec(p + 16 * k);
+  widen16<T>(raw, x);
+}
+
+template <typename T> __device__ __forceinline__ float round_to(float v) {
+  if constexpr (std::is_same<T, float>::value) return v;
+  else return to_float<T>(from_float<T>(v));
+}
+
+// Where a kernel finds x, residual and out of row `row`. x_off: arena offset of x (every rank), read from peer 0 .. nranks-1 (one rank:
+// x_local). res / out: local pointers, or (PUSH) arena offsets res_off / out_off stored into every rank.
+struct RmsArgs {
+  const char* x_local;
+  const char* res_in;           // my residual, the rows I read
+  char* res_out;                // my residual (local kernels) or nullptr (PUSH)
+  char* out;                    // my out (local kernels) or nullptr (PUSH)
+  const char* gamma;
+  size_t x_off, res_off, out_off;
+  uint32_t row_len, nchunks;
+  float eps;
+};
+
+// One row: h = round((+0 + x_0 + .. + x_{N-1}) + residual), residual = h, out = round((h * inv) * gamma), inv = 1 / sqrt(fold / row_len + eps).
+// LOCAL: one rank, x is a.x_local; else rank r's x is at a.x_off of its arena. sbuf: this row's 512 floats of shared memory.
+template <typename T, bool LOCAL, bool PUSH>
+__device__ __forceinline__ void rms_row(const CommDev& c, const RmsArgs& a, size_t row, float* sbuf) {
+  const int t = threadIdx.x, lane = t & 31;
+  const size_t row_bytes = (size_t)a.row_len * sizeof(T);
+  float h[2][16];
+  float p[2];
+#pragma unroll
+  for (int k = 0; k < 2; k++) {
+    const uint32_t ch = (uint32_t)t + (uint32_t)k * kRmsThreads;
+    p[k] = 0.f;
+    if (ch < a.nchunks) {
+      const size_t off = row * row_bytes + (size_t)ch * 16 * sizeof(T);
+      float acc[16];
+#pragma unroll
+      for (int i = 0; i < 16; i++) acc[i] = 0.f;
+#pragma unroll
+      for (int r = 0; r < (LOCAL ? 1 : kMaxRanks); r++) {
+        if (LOCAL || r < c.nranks) {
+          float v[16];
+          rms_load16<T>((LOCAL ? a.x_local : c.peer[r] + a.x_off) + off, v);
+#pragma unroll
+          for (int i = 0; i < 16; i++) acc[i] = __fadd_rn(acc[i], v[i]);
+        }
+      }
+      float res[16];
+      rms_load16<T>(a.res_in + off, res);
+#pragma unroll
+      for (int i = 0; i < 16; i++) {
+        h[k][i] = round_to<T>(__fadd_rn(acc[i], res[i]));
+        p[k] = __fadd_rn(p[k], __fmul_rn(h[k][i], h[k][i]));
+      }
+      if (PUSH) {
+#pragma unroll
+        for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
+          int q = c.rank + j; if (q >= c.nranks) q -= c.nranks;
+          store16_scaled<T>(c.peer[q] + a.res_off + off, h[k], 1.0f);
+        }
+      } else {
+        store16_scaled<T>(a.res_out + off, h[k], 1.0f);
+      }
+    }
+  }
+  // the fold: bit 9 in registers, bits 8..5 across warps, bits 4..0 in the butterfly
+  sbuf[t] = __fadd_rn(p[0], p[1]);
+  __syncthreads();
+  float w[kRmsWarps];
+#pragma unroll
+  for (int i = 0; i < kRmsWarps; i++) w[i] = sbuf[32 * i + lane];
+#pragma unroll
+  for (int i = 0; i < 8; i++) w[i] = __fadd_rn(w[i], w[i + 8]);
+#pragma unroll
+  for (int i = 0; i < 4; i++) w[i] = __fadd_rn(w[i], w[i + 4]);
+  w[0] = __fadd_rn(w[0], w[2]); w[1] = __fadd_rn(w[1], w[3]);
+  float f = __fadd_rn(w[0], w[1]);
+#pragma unroll
+  for (int l = 4; l >= 0; l--) f = __fadd_rn(f, __shfl_xor_sync(0xFFFFFFFFu, f, 1 << l));
+  const float inv = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(__fdiv_rn(f, (float)a.row_len), a.eps)));
+#pragma unroll
+  for (int k = 0; k < 2; k++) {
+    const uint32_t ch = (uint32_t)t + (uint32_t)k * kRmsThreads;
+    if (ch < a.nchunks) {
+      const size_t off = row * row_bytes + (size_t)ch * 16 * sizeof(T);
+      float g[16], o[16];
+      rms_load16<T>(a.gamma + (size_t)ch * 16 * sizeof(T), g);
+#pragma unroll
+      for (int i = 0; i < 16; i++) o[i] = __fmul_rn(__fmul_rn(h[k][i], inv), g[i]);
+      if (PUSH) {
+#pragma unroll
+        for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
+          int q = c.rank + j; if (q >= c.nranks) q -= c.nranks;
+          store16_scaled<T>(c.peer[q] + a.out_off + off, o, 1.0f);
+        }
+      } else {
+        store16_scaled<T>(a.out + off, o, 1.0f);
+      }
+    }
+  }
+}
+
+// Rows [r0, r1), CTA b taking r0 + b, r0 + b + gridDim.x, ...; the shared buffer alternates by row so that one block barrier per row
+// suffices (a warp that writes row i + 2's buffer has passed row i + 1's barrier, which every warp reaches only after reading row i's).
+template <typename T, bool LOCAL, bool PUSH>
+__device__ __forceinline__ void rms_rows(const CommDev& c, const RmsArgs& a, uint32_t r0, uint32_t r1) {
+  __shared__ float sbuf[2][kRmsThreads];
+  uint32_t i = 0;
+  for (uint32_t row = r0 + blockIdx.x; row < r1; row += gridDim.x, i ^= 1) rms_row<T, LOCAL, PUSH>(c, a, row, sbuf[i]);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kRmsThreads, 1) k_rms_local(COMM_PARAM, const __grid_constant__ RmsArgs a, uint32_t rows) {
+  pdl_prologue();
+  rms_rows<T, true, false>(c, a, 0, rows);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kRmsThreads, 1) k_rms_oneshot(COMM_PARAM, const __grid_constant__ RmsArgs a, uint32_t rows, uint32_t op) {
+  pdl_prologue();
+  {
+    const uint32_t s = load_seq(c, kSeqBarrier);
+    if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every rank's x is written
+  }
+  rms_rows<T, false, false>(c, a, 0, rows);
+  const uint32_t s = load_seq(c, kSeqBarrier);
+  if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // nobody reads my x any more
+  if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kRmsThreads, 1) k_rms_twoshot(COMM_PARAM, const __grid_constant__ RmsArgs a, uint32_t rows, uint32_t op) {
+  pdl_prologue();
+  {
+    const uint32_t s = load_seq(c, kSeqBarrier);
+    if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every rank's x is written, and its residual and out are free
+  }
+  const uint32_t r0 = (uint32_t)((unsigned long long)rows * c.rank / c.nranks), r1 = (uint32_t)((unsigned long long)rows * (c.rank + 1) / c.nranks);
+  rms_rows<T, false, true>(c, a, r0, r1);
+  const uint32_t s = load_seq(c, kSeqBarrier);
+  if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // my rows are in every rank's residual and out; nobody reads my x
+  if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
+}
+
+// Once per device, before the first kernel of this family launches: load all nine kernels. With lazy module loading a kernel's first
+// launch loads it, and the load waits for kernels already running; a rank whose first launch of one of these kernels came behind its own
+// barrier kernel, which waits for another rank's launch on the same thread, would never get there. One thread loads at a time.
+static void rmsnorm_preload(const b200collComm* c) {
+  static std::atomic<unsigned long long> done{0};
+  static std::mutex mu;
+  const unsigned long long bit = 1ull << (c->device & 63);
+  if (done.load(std::memory_order_acquire) & bit) return;
+  const std::lock_guard<std::mutex> lk(mu);
+  if (done.load(std::memory_order_acquire) & bit) return;
+  cudaFuncAttributes fa;
+  for (b200collDataType_t t : {b200collBfloat16, b200collFloat16, b200collFloat32})
+    with_wide(t, [&](auto tt) {
+      using T = typename decltype(tt)::type;
+      cudaFuncGetAttributes(&fa, k_rms_local<T>);
+      cudaFuncGetAttributes(&fa, k_rms_oneshot<T>);
+      cudaFuncGetAttributes(&fa, k_rms_twoshot<T>);
+    });
+  done.fetch_or(bit, std::memory_order_acq_rel);
+}
+
+// The argument rules, all before the poisoned-communicator check; nothing is launched on a refusal.
+static b200collResult_t rms_prepare(b200collComm* c, const void* x, const void* residual, const void* gamma, const void* out, size_t rows, size_t row_len,
+                                    float eps, b200collDataType_t dtype) {
+  auto refuse = [](const std::string& msg) { set_last_error("all-reduce rms-norm: " + msg); return b200collInvalidArgument; };
+  if (!c) return refuse("null communicator");
+  if (!wide_type(dtype)) return refuse("dtype must be bf16, fp16 or fp32");
+  if (row_len < 16 || row_len > kRmsMaxRowLen || row_len % 16 != 0) return refuse("row_len must be a multiple of 16 in [16, 16384]");
+  if (!(eps >= 0.0f) || !isfinite(eps)) return refuse("eps must be finite and non-negative");
+  if (rows >= ((size_t)1 << 31)) return refuse("rows must be below 2^31");
+  if (rows > 0 && (!x || !residual || !gamma || !out)) return refuse("null argument");
+  if (!aligned(x, 16) || !aligned(residual, 16) || !aligned(gamma, 16) || !aligned(out, 16)) return refuse("x, residual, gamma and out must be 16-byte aligned");
+  const size_t es = b200collTypeSize(dtype), mat = rows * row_len * es, g = row_len * es;
+  if (rows > 0) {
+    if (overlaps(out, mat, x, mat) || overlaps(out, mat, residual, mat) || overlaps(out, mat, gamma, g)) return refuse("out must not overlap x, residual or gamma");
+    if (overlaps(residual, mat, x, mat) || overlaps(residual, mat, gamma, g)) return refuse("residual must not overlap x or gamma");
+  }
+  if (comm_poisoned(c)) return b200collRemoteError;
+  return b200collSuccess;
+}
+
+}  // namespace b200coll
+
+using namespace b200coll;
+
+extern "C" {
+
+b200collResult_t b200collAllReduceRmsNorm(const void* x, void* residual, const void* gamma, void* out, size_t rows, size_t row_len, float eps,
+                                          b200collDataType_t dtype, b200collComm_t c, b200collStream_t stream) {
+  b200collResult_t rc = rms_prepare(c, x, residual, gamma, out, rows, row_len, eps, dtype);
+  if (rc != b200collSuccess) return rc;
+  const size_t mat = rows * row_len * b200collTypeSize(dtype);
+  b200collAlgo_t algo = b200collAlgoCopy;
+  if (c->nranks > 1) {
+    // peers pull my x at my arena offset. rows == 0 reads nothing (any pointer, even null, will do) and runs one-shot: only the barriers
+    if (rows > 0 && (rc = in_arena(c, "all-reduce rms-norm: ", "x", {{x, mat}})) != b200collSuccess) return rc;
+    // the tuner's pick for an all-reduce of these bytes, or the forced algorithm: ll, ll2 and oneshot pull every row; twoshot and nvls
+    // push my rows into the peers' residual and out, so both must be arena memory, else one-shot
+    const b200collAlgo_t want = c->forced_algo != b200collAlgoAuto ? c->forced_algo : b200collTunerPick(b200collOpAllReduce, mat, c->nranks, c->nvls);
+    const bool two = rows > 0 && (want == b200collAlgoTwoShot || want == b200collAlgoNvls) && b200collIsSymmetric(c, residual, mat) &&
+                     b200collIsSymmetric(c, out, mat);
+    algo = two ? b200collAlgoTwoShot : b200collAlgoOneShot;
+    // (rows, row_len) travel as one number (row_len < 2^15); two-shot adds a second exchange for the residual and out offsets
+    const size_t shape = (rows << 15) | row_len;
+    if ((rc = cross_check(c, b200collOpAllReduce, algo, shape, rows > 0 ? arena_off(c, x) : 0, 0)) != b200collSuccess) return rc;
+    if (two && (rc = cross_check(c, b200collOpAllReduce, algo, shape, arena_off(c, residual), arena_off(c, out))) != b200collSuccess) return rc;
+  }
+  const DeviceScope on_device(c->device);
+  rmsnorm_preload(c);
+  account(c, b200collOpAllReduce, mat, algo);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RmsArgs a = {};
+  a.x_local = static_cast<const char*>(x);
+  a.res_in = static_cast<const char*>(residual);
+  a.gamma = static_cast<const char*>(gamma);
+  a.row_len = (uint32_t)row_len;
+  a.nchunks = (uint32_t)(row_len / 16);
+  a.eps = eps;
+  return with_wide(dtype, [&](auto tt) -> b200collResult_t {
+    using T = typename decltype(tt)::type;
+    if (algo == b200collAlgoCopy) {
+      a.res_out = static_cast<char*>(residual);
+      a.out = static_cast<char*>(out);
+      const int blocks = (int)std::max<size_t>(1, std::min<size_t>(rows, (size_t)2 * std::max(1, c->sm_count)));   // 2 per SM where the registers allow
+      launch_k(k_rms_local<T>, blocks, kRmsThreads, st, c->dev, a, (uint32_t)rows);
+    } else {
+      a.x_off = arena_off(c, x);
+      const Grid gr = full_grid(c, 1);
+      if (algo == b200collAlgoTwoShot) {
+        a.res_off = arena_off(c, residual);
+        a.out_off = arena_off(c, out);
+        launch_k(k_rms_twoshot<T>, gr.blocks, kRmsThreads, st, c->dev, a, (uint32_t)rows, (uint32_t)b200collOpAllReduce);
+      } else {
+        a.res_out = static_cast<char*>(residual);
+        a.out = static_cast<char*>(out);
+        launch_k(k_rms_oneshot<T>, gr.blocks, kRmsThreads, st, c->dev, a, (uint32_t)rows, (uint32_t)b200collOpAllReduce);
+      }
+    }
+    LAUNCH_CHECK(c);
+    return b200collSuccess;
+  });
+}
+
+}  // extern "C"

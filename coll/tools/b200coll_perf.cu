@@ -59,6 +59,7 @@ struct Opts {
   int route_e = 0, route_k = 0;   // --route E:K: the device-routed dispatch and combine, E experts, top-K (0 = off)
   int cq_block = 0;               // --combine-quantize WIRE:BLOCK: the quantising combine in --combine / --route (0 = off)
   b200collDataType_t cq_wire = b200collFloat8e4m3;
+  size_t rms_row = 0;             // --rms-norm ROW_LEN: the fused all-reduce, residual add and RMSNorm (0 = off)
 };
 
 // Block-scaled mode: each rank's send buffer is a [rows, row_len] FP8 matrix with one fp32 scale per bs_rows x bs_cols block. Scales are
@@ -342,6 +343,130 @@ static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out,
   return total_errors ? 1 : 0;
 }
 
+// All-reduce + RMSNorm mode (--rms-norm ROW_LEN). Per size, every rank's x holds `bytes` of whole rows (k_fill values of its rank), the
+// residual the same k_fill rows on every rank, gamma one k_fill row; x, residual and out are arena memory. -c 1 runs one call and
+// repeats steps 1-5 of b200collAllReduceRmsNorm on the host (every sum and product rounded on its own, IEEE sqrt and division), then
+// compares every residual and out element bit for bit. The timed calls keep updating the residual in place. "rw GB/s" counts the bytes
+// one rank's HBM moves at one rank: x, residual and gamma read, residual and out written.
+static float round_dt(float v, b200collDataType_t dt) {
+  if (dt == b200collFloat32) return v;
+  if (dt == b200collFloat16) return __half2float(__float2half_rn(v));
+  return __bfloat162float(__float2bfloat16_rn(v));
+}
+static int run_rms(const Opts& o, RankCtx ctx, Shared* sh, void* x, void* out, void* residual, cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1) {
+  const int n = ctx.nranks, rank = ctx.rank;
+  const b200collDataType_t dt = o.in_dt;
+  const size_t es = b200collTypeSize(dt), row = o.rms_row;
+  const float eps = 1e-6f;
+  int gen_ctr[4] = {0, 0, 0, 0};
+  long total_errors = 0;
+  if (rank == 0) {
+    printf("# b200coll_perf op=all_reduce + rms-norm nranks=%d dtype=%s row_len=%zu eps=%g: size = x bytes per rank; rw GB/s = (x + residual + gamma read, "
+           "residual + out written) / time\n", n, dt_name(dt), row, eps);
+    printf("#%13s %10s %6s %8s | %10s %8s %8s %6s\n", "size(B)", "rows", "type", "algo", "us", "algbw", "rw_GB/s", "#wrong");
+    fflush(stdout);
+  }
+  void* gamma = nullptr;
+  RT(cudaMalloc(&gamma, row * es));
+  fill(gamma, row, dt, 7, 0, st);
+  for (size_t bytes = o.min_bytes; bytes <= o.max_bytes; bytes *= o.factor) {
+    const size_t rows = bytes / es / row, elems = rows * row;
+    if (rows == 0) continue;
+    fill(x, elems, dt, rank, 0, st);
+    fill(residual, elems, dt, 99, 0, st);
+    RT(cudaMemsetAsync(out, 0x5A, elems * es, st));
+    RT(cudaGetLastError());
+    auto launch = [&] { CC(b200collAllReduceRmsNorm(x, residual, gamma, out, rows, row, eps, dt, ctx.comm, st)); };
+    long errs = 0;
+    if (o.check) {
+      std::vector<char> hres(elems * es), hg(row * es);
+      RT(cudaStreamSynchronize(st));
+      RT(cudaMemcpy(hres.data(), residual, hres.size(), cudaMemcpyDeviceToHost));
+      RT(cudaMemcpy(hg.data(), gamma, hg.size(), cudaMemcpyDeviceToHost));
+      std::vector<std::vector<char>> hx(n, std::vector<char>(elems * es));
+      for (int r = 0; r < n; r++) {               // every rank's x, from the same generator on the host
+        void* tmp = nullptr;
+        RT(cudaMalloc(&tmp, elems * es));
+        fill(tmp, elems, dt, r, 0, st);
+        RT(cudaStreamSynchronize(st));
+        RT(cudaMemcpy(hx[r].data(), tmp, elems * es, cudaMemcpyDeviceToHost));
+        RT(cudaFree(tmp));
+      }
+      spin_barrier(sh, 0, n, &gen_ctr[0]);
+      launch();
+      RT(cudaStreamSynchronize(st));
+      spin_barrier(sh, 1, n, &gen_ctr[1]);
+      std::vector<char> gres(elems * es), gout(elems * es);
+      RT(cudaMemcpy(gres.data(), residual, gres.size(), cudaMemcpyDeviceToHost));
+      RT(cudaMemcpy(gout.data(), out, gout.size(), cudaMemcpyDeviceToHost));
+      const size_t nch = row / 16;
+      size_t P = 1;
+      while (P < nch) P *= 2;
+      std::vector<float> h(row), p(P);
+      for (size_t i = 0; i < rows; i++) {
+        for (size_t e = 0; e < row; e++) {
+          volatile float acc = 0.0f;
+          for (int r = 0; r < n; r++) acc = acc + to_f(hx[r].data(), i * row + e, dt);
+          h[e] = round_dt(acc + to_f(hres.data(), i * row + e, dt), dt);
+        }
+        for (size_t c = 0; c < P; c++) {
+          volatile float s = 0.0f;
+          for (size_t e = 16 * c; c < nch && e < 16 * c + 16; e++) { volatile float sq = h[e] * h[e]; s = s + sq; }
+          p[c] = s;
+        }
+        for (size_t w = P / 2; w >= 1; w /= 2)
+          for (size_t c = 0; c < w; c++) { volatile float v = p[c] + p[c + w]; p[c] = v; }
+        volatile float ms = p[0] / (float)row;
+        volatile float den = sqrtf(ms + eps);
+        const float inv = 1.0f / den;
+        for (size_t e = 0; e < row; e++) {
+          volatile float hi = h[e] * inv;
+          volatile float y = hi * to_f(hg.data(), e, dt);
+          const uint32_t want_h = out_bits(h[e], dt), got_h = got_bits(gres.data(), i * row + e, dt);
+          const uint32_t want_o = out_bits(y, dt), got_o = got_bits(gout.data(), i * row + e, dt);
+          if (got_h != want_h || got_o != want_o) {
+            if (errs < 4) fprintf(stderr, "rank %d rms-norm size %zu row %zu elem %zu: residual 0x%x want 0x%x, out 0x%x want 0x%x\n", rank, bytes, i, e, got_h,
+                                  want_h, got_o, want_o);
+            errs++;
+          }
+        }
+      }
+    }
+    for (int i = 0; i < o.warmup; i++) launch();
+    RT(cudaStreamSynchronize(st));
+    spin_barrier(sh, 2, n, &gen_ctr[2]);
+    b200collStats s0; CC(b200collCommStatsGet(ctx.comm, &s0));
+    RT(cudaEventRecord(e0, st));
+    for (int i = 0; i < o.iters; i++) launch();
+    RT(cudaEventRecord(e1, st));
+    RT(cudaEventSynchronize(e1));
+    b200collStats s1; CC(b200collCommStatsGet(ctx.comm, &s1));
+    float ms = 0; RT(cudaEventElapsedTime(&ms, e0, e1));
+    sh->ms[rank] = ms / o.iters; sh->errors[rank] = errs;
+    spin_barrier(sh, 3, n, &gen_ctr[3]);
+    float worst = 0; long es_ = 0;
+    for (int r = 0; r < n; r++) { worst = std::max(worst, sh->ms[r]); es_ += sh->errors[r]; }
+    total_errors += es_;
+    spin_barrier(sh, 0, n, &gen_ctr[0]);   // keep ms[] stable until everyone has read it
+    b200collFault f;
+    if (b200collCommGetAsyncError(ctx.comm, &f) != b200collSuccess) { fprintf(stderr, "rank %d WATCHDOG code=%u peer=%u block=%u expected=%u observed=%u\n", rank, f.code, f.peer, f.block, f.expected, f.observed); _exit(5); }
+    if (rank == 0) {
+      const char* algo = "?";
+      for (int a = 0; a < b200collNumAlgos; a++) if (s1.algo_calls[a] != s0.algo_calls[a]) algo = b200collAlgoName((b200collAlgo_t)a);
+      const size_t mat = elems * es, rw = 4 * mat + row * es;
+      printf("%14zu %10zu %6s %8s | %10.2f %8.2f %8.1f %6ld\n", mat, rows, dt_name(dt), algo, worst * 1e3, mat / (worst * 1e3) / 1e3, rw / (worst * 1e3) / 1e3, es_);
+      fflush(stdout);
+    }
+  }
+  RT(cudaFree(gamma));
+  b200collStats s; CC(b200collCommStatsGet(ctx.comm, &s));
+  if (rank == 0) {
+    printf("# launches=%llu errors=%ld\n", (unsigned long long)s.kernel_launches, total_errors);
+    fflush(stdout);
+  }
+  return total_errors ? 1 : 0;
+}
+
 // Routed mode (--route E:K). Per size, every rank holds tokens = size / row bytes tokens of x (k_fill values) and routes slot (t, j) to
 // expert h(rank, t, j) % E, or drops it (id -1) every 61st slot; the hash is seeded, so every rank can draw every rank's ids on the host.
 // recv holds tokens * K rows on every rank, the mean load, so some receivers clip and some do not. -c 1 repeats the layout on the host
@@ -591,6 +716,11 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
   void *send = nullptr, *recv = nullptr;
   CC(b200collMemAlloc(ctx.comm, &send, send_cap + 4096));
   CC(b200collMemAlloc(ctx.comm, &recv, recv_cap + 4096));
+  if (o.rms_row) {
+    void* residual = nullptr;
+    CC(b200collMemAlloc(ctx.comm, &residual, max_in_bytes + 4096));
+    return run_rms(o, ctx, sh, send, recv, residual, st, e0, e1);
+  }
   if (o.combine_k) {
     if (o.op != "alltoall" || o.q_block || o.bs_rows || o.row_len == 0 || o.row_len % 16 ||
         [](b200collDataType_t t) { return t != b200collBfloat16 && t != b200collFloat16 && t != b200collFloat32; }(o.in_dt) ||
@@ -934,6 +1064,11 @@ int main(int argc, char** argv) {
       }
       o.cq_wire = parse_dt(wire);
     }
+    else if (a == "--rms-norm") {
+      const long long v = atoll(next());
+      if (v < 16 || v > 16384 || v % 16) { fprintf(stderr, "--rms-norm ROW_LEN: a multiple of 16 in [16, 16384]\n"); return 1; }
+      o.rms_row = (size_t)v;
+    }
     else if (a == "--combine") { o.combine_k = atoi(next()); if (o.combine_k < 1) { fprintf(stderr, "--combine K: K >= 1\n"); return 1; } }
     else if (a == "--route") {
       if (sscanf(next(), "%d:%d", &o.route_e, &o.route_k) != 2 || o.route_e < 1 || o.route_e > 1024 || o.route_k < 1) { fprintf(stderr, "--route E:K: 1 <= E <= 1024, K >= 1\n"); return 1; }
@@ -994,12 +1129,20 @@ int main(int argc, char** argv) {
            "                            (--row-len a multiple of BLOCK) and the slots pull FP8 rows and scales; -c 1 checks every output element bit\n"
            "                            for bit against the host quantiser and the slot-order reference\n"
            "  --algo auto|ll|ll2|oneshot|twoshot|nvls   --inplace 0|1|2   --max-ctas N   --sweep kind:ctas:threads,...   --json FILE   --window SIZE\n"
+           "  --rms-norm ROW_LEN        --op all_reduce, -d bfloat16|half|float: the fused all-reduce, residual add and RMSNorm over rows of ROW_LEN\n"
+           "                            elements (a multiple of 16 in [16, 16384]); -c 1 checks every residual and out element bit for bit\n"
            "  --selfcheck               report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;
     }
     else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 1; }
   }
   if (o.factor < 2) o.factor = 2;
+  if (o.rms_row && (o.op != "all_reduce" || o.out_dt != o.in_dt || o.scale != 1.0f || o.q_block || o.bs_rows || o.combine_k || o.route_e || o.cq_block ||
+                    (o.in_dt != b200collBfloat16 && o.in_dt != b200collFloat16 && o.in_dt != b200collFloat32))) {
+    fprintf(stderr, "--rms-norm ROW_LEN takes --op all_reduce and -d bfloat16|half|float, and no --out-dtype, --scale, --quantize, --block-scale, --combine\n"
+                    "or --route\n");
+    return 1;
+  }
   if (o.cq_block && ((!o.combine_k && !o.route_e) || o.q_block || o.bs_rows || o.row_len % o.cq_block != 0)) {
     fprintf(stderr, "--combine-quantize WIRE:BLOCK takes --combine K or --route E:K, a --row-len that is a multiple of BLOCK, and no --quantize or\n"
                     "--block-scale\n");
@@ -1025,7 +1168,8 @@ int main(int argc, char** argv) {
     b200collConfig cfg; b200collConfigDefault(&cfg);
     const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
     if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o) +
-                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o);     // --route: recv holds K rows per token
+                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o) +     // --route: recv holds K rows per token
+                     (o.rms_row ? o.max_bytes + 4096 : 0);                                      // --rms-norm: the residual
     b200collUniqueId id; CC(b200collUniqueIdFromString(("perf/" + lr.job).c_str(), &id));
     RT(cudaSetDevice(dev));
     b200collComm_t comm;
@@ -1054,7 +1198,8 @@ int main(int argc, char** argv) {
   // arena: two windows (+ max buffers) and slack
   const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
   size_t need = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o) +
-                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o);     // --route: recv holds K rows per token
+                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o) +     // --route: recv holds K rows per token
+                     (o.rms_row ? o.max_bytes + 4096 : 0);                                      // --rms-norm: the residual
   if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = need;
   if (o.procs) {
     b200collUniqueId id; CC(b200collGetUniqueId(&id));

@@ -146,6 +146,7 @@ def load() -> C.CDLL:
     L.b200collAllToAllvCombineQuantized.argtypes = [vp, vp, sz, sz, i64p, i64p, i64p, i32p, C.POINTER(C.c_float), sz, ci, ci, ci, C.POINTER(Epilogue),
                                                     vp, vp]
     L.b200collExpertCombineQuantized.argtypes = [vp, vp, sz, sz, i32p, C.POINTER(C.c_float), sz, ci, ci, ci, C.POINTER(Epilogue), vp, vp]
+    L.b200collAllReduceRmsNorm.argtypes = [vp, vp, vp, vp, sz, sz, C.c_float, ci, vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -441,6 +442,47 @@ def _overlap(t, u) -> bool:
     a, na = t.data_ptr(), t.numel() * t.element_size()
     b, nb = u.data_ptr(), u.numel() * u.element_size()
     return bool(na and nb and a < b + nb and b < a + na)
+
+
+RMS_NORM_MAX_ROW = 16384
+
+
+def check_all_reduce_rms_norm(x, residual, weight, out, eps: float = 1e-6) -> tuple[int, int]:
+    """The rules of Comm.all_reduce_rms_norm, checked on the tensors' metadata (no device, no communicator): raises ValueError, returns
+    (rows, row_len). x, residual and out are contiguous [..., row_len] tensors of one shape, weight a contiguous [row_len] tensor, all four of
+    one dtype (bfloat16, float16 or float32); row_len a multiple of 16 in [16, 16384]; eps finite and >= 0; fewer than 2^31 rows; every
+    pointer 16-byte aligned; out must not overlap x, residual or weight, residual must not overlap x or weight."""
+    import math
+    import torch
+    for name, t in (("x", x), ("residual", residual), ("weight", weight), ("out", out)):
+        _check_wide(name, t)
+        if t.dtype != x.dtype:
+            raise ValueError(f"{name} must have x's dtype {x.dtype}, got {t.dtype}")
+    if x.dim() < 1:
+        raise ValueError("x must have at least one dimension")
+    shape = tuple(x.shape)
+    for name, t in (("residual", residual), ("out", out)):
+        if tuple(t.shape) != shape:
+            raise ValueError(f"{name} must have x's shape {list(shape)}, got {list(t.shape)}")
+    row_len = shape[-1]
+    if row_len < 16 or row_len > RMS_NORM_MAX_ROW or row_len % 16:
+        raise ValueError(f"row_len (the last dimension) must be a multiple of 16 in [16, {RMS_NORM_MAX_ROW}], got {row_len}")
+    if tuple(weight.shape) != (row_len,):
+        raise ValueError(f"weight must have shape [{row_len}], got {list(weight.shape)}")
+    if isinstance(eps, bool) or not isinstance(eps, (int, float)) or not math.isfinite(eps) or eps < 0:
+        raise ValueError(f"eps must be a finite number >= 0, got {eps!r}")
+    rows = _numel(shape[:-1])
+    if rows > _I31:
+        raise ValueError(f"at most 2^31 - 1 rows, got {rows}")
+    if rows:
+        for name, t in (("x", x), ("residual", residual), ("weight", weight), ("out", out)):
+            if t.data_ptr() % 16:
+                raise ValueError(f"{name} must be 16-byte aligned")
+        if any(_overlap(out, t) for t in (x, residual, weight)):
+            raise ValueError("out must not overlap x, residual or weight")
+        if _overlap(residual, x) or _overlap(residual, weight):
+            raise ValueError("residual must not overlap x or weight")
+    return rows, row_len
 
 
 def _check_routed(nranks: int, x, topk_idx, num_experts: int, recv, expert_counts, route, dropped, fp8=None) -> None:
@@ -843,6 +885,18 @@ class Comm:
         ep = self._ep(src, out, scale)
         _check(load().b200collAllReduceQuantized(C.c_void_p(src.data_ptr()), C.c_void_p(out.data_ptr()), src.numel(), w, block, C.byref(ep), op, self._h,
                                                  self._stream(stream)), "AllReduceQuantized")
+        return out
+
+    def all_reduce_rms_norm(self, x, residual, weight, out=None, eps: float = 1e-6, stream=None):
+        """The pre-norm step of a tensor-parallel block in one kernel: residual += all_reduce(x) in place (ranks summed in rank order,
+        one rounding), then out = rms_norm(residual, weight, eps), bit for bit as coll/include/b200coll.h's b200collAllReduceRmsNorm
+        states. Returns out (a new tensor when None). With more than one rank x must be arena memory (`empty()`); two-shot also needs
+        residual and out there, else the call runs one-shot."""
+        out = x.new_empty(x.shape) if out is None else out
+        rows, row_len = check_all_reduce_rms_norm(x, residual, weight, out, eps)
+        _check(load().b200collAllReduceRmsNorm(C.c_void_p(x.data_ptr()), C.c_void_p(residual.data_ptr()), C.c_void_p(weight.data_ptr()),
+                                               C.c_void_p(out.data_ptr()), rows, row_len, float(eps), torch_dtype_code(x.dtype), self._h,
+                                               self._stream(stream)), "AllReduceRmsNorm")
         return out
 
     def all_to_all(self, src, dst, scale: float = 1.0, stream=None):
