@@ -21,8 +21,9 @@ _LIB_CANDIDATES = [
     "libb200coll.so",
 ]
 
-SUCCESS = 0
-NO_DRIVER = 9
+# b200collResult_t
+(SUCCESS, UNHANDLED_CUDA_ERROR, SYSTEM_ERROR, INTERNAL_ERROR, INVALID_ARGUMENT, INVALID_USAGE, REMOTE_ERROR, IN_PROGRESS, OUT_OF_MEMORY,
+ NO_DRIVER) = range(10)
 MAX_RANKS = 8
 
 F32, F16, BF16, FP8_E4M3, I8, U8, I32, U32, I64, U64, F64, FP8_E5M2 = range(12)

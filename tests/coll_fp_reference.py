@@ -14,7 +14,8 @@ a property of the kernel that ran, so the reference takes it as an argument:
 FP8 inputs are summed in rank order on every P2P kernel (the two-shot all-reduce and the P2P reduce-scatter included), so their
 order model is always [0, 1, ..., N-1].
 
-Not collected by pytest (no test_ prefix); imported by the test_coll_fp_numerics_* and test_coll_fp8_numerics_* files."""
+Not collected by pytest (no test_ prefix); imported by the test_coll_fp_numerics_* and test_coll_fp8_numerics_* files and the other
+GPU tests."""
 import torch
 
 STAGE_HALF_BYTES = 32 << 20          # coll/src/layout.h kStageHalfBytes
@@ -46,6 +47,11 @@ def f32(x):
 def avg_scale(scale, n):
     """What the host multiplies by for avg: fp32(scale) * fp32(1 / N), both rounded in fp32."""
     return float(f32(scale) * (f32(1.0) / f32(float(n))))
+
+
+def scale_of(coll, op, scale, n):
+    """The scale a sum (scale) or an avg (avg_scale) multiplies by."""
+    return scale if op == coll.SUM else avg_scale(scale, n)
 
 
 def cast(x32, dt):
@@ -174,6 +180,18 @@ def ll_move(x):
 
 
 # ------------------------------------------------------------------------------------------------- data
+def random_fp8(torch, n, dt, seed):
+    """Seeded random bytes reinterpreted as FP8, NaN and inf patterns replaced: every exponent occurs, subnormals and values near the
+    maximum included, so sums round and saturate."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    b = torch.randint(0, 256, (n,), generator=g, dtype=torch.int32)
+    if dt == torch.float8_e4m3fn:
+        b = torch.where((b & 0x7F) == 0x7F, b - 1, b)                # S.1111.111 is NaN
+    else:
+        b = torch.where((b & 0x7C) == 0x7C, b & 0x83 | 0x78, b)      # exponent 11111 is inf / NaN
+    return b.to(torch.uint8).view(dt).cuda()
+
+
 def _exp2(e):
     return torch.exp2(e.float())
 

@@ -1,6 +1,35 @@
 """Reference of the device-routed expert dispatch (b200collExpertDispatch), in numpy: from every rank's expert ids, the route of every
-slot, the rows stored per local expert, the dropped rows, and which (source rank, token) every row of every recv holds."""
+slot, the rows stored per local expert, the dropped rows, and which (source rank, token) every row of every recv holds; the seeded
+routings the routed tests draw, and the combine's lookup of a route."""
 import numpy as np
+
+INT32_MIN, INT32_MAX = -2 ** 31, 2 ** 31 - 1
+
+
+def routing(kind, n, E, k, seed, tokens=None):
+    """One [tokens, top_k] int32 array per rank. uniform; zipf (expert_dispatch_plan's skewed draw); one (every slot to one expert);
+    mixed: uniform with every kind of invalid id, a token naming one expert twice, and (n > 1) a last rank with no tokens."""
+    rng = np.random.default_rng(seed)
+    tokens = tokens or [17 + 5 * s for s in range(n)]
+    if kind == "zipf":
+        from container_engine_accelerators_b200.models.workloads import expert_dispatch_plan
+        p = expert_dispatch_plan(n, max(tokens), 16, experts_per_rank=E // n, top_k=k, skew=1.2, seed=seed)
+        return [p.experts[s][:tokens[s]] for s in range(n)]
+    if kind == "one":
+        return [np.full((tokens[s], k), (seed * 7) % E, dtype=np.int32) for s in range(n)]
+    out = [rng.integers(0, E, size=(tokens[s], k)).astype(np.int64) for s in range(n)]
+    if kind == "mixed":
+        bad = [-1, -2, E, E + 3, INT32_MIN, INT32_MAX]
+        for s in range(n):
+            ids = out[s]
+            pos = rng.choice(ids.size, size=min(ids.size, len(bad)), replace=False)
+            for i, p in enumerate(pos):
+                ids.flat[p] = bad[i]
+            if k >= 2:
+                ids[1, 0] = ids[1, 1] = s % E                           # the same expert twice
+        if n > 1:
+            out[-1] = np.zeros((0, k), dtype=np.int64)
+    return [o.astype(np.int32) for o in out]
 
 
 class Layout:
@@ -92,3 +121,18 @@ def recv_rows_of(lay, xs, d, poison):
         if s >= 0:
             want[r] = xs[s][t]
     return want
+
+
+def route_lookup(eo, recv_rows):
+    """coll_combine_reference.combine's lookup for routes: route in [0, nranks * recv_rows) names row route % recv_rows of rank
+    route // recv_rows."""
+    n = len(eo)
+
+    def f(col):
+        col = np.asarray(col, dtype=np.int64)
+        valid = (col >= 0) & (col < n * recv_rows)
+        y = np.zeros((col.size, eo[0].shape[1]), dtype=np.float32)
+        for i in np.nonzero(valid)[0]:
+            y[i] = eo[col[i] // recv_rows][col[i] % recv_rows]
+        return valid, y
+    return f

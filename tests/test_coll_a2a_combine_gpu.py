@@ -3,57 +3,19 @@
 Every out starts poisoned with 0x5A, and every element is compared bit for bit with tests/coll_combine_reference.combine applied to
 the expert_out rows each slot names (NaN matches NaN at the same position)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from container_engine_accelerators_b200.ops.coll import INVALID_ARGUMENT, INVALID_USAGE
 from tests import coll_combine_reference as cr
 from tests import coll_quant_reference as qr
 from tests.coll_fp_reference import assert_same
+from tests.coll_gpu_harness import DTYPES, Group, Plan, assert_nothing_launched, coll_mod, expect_refused, run_perf, torch_cuda  # noqa: F401
+from tests.coll_routed_reference import INT32_MAX, INT32_MIN
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PERF = os.path.join(ROOT, "build", "b200coll_perf")
-INVALID_ARGUMENT, INVALID_USAGE = 4, 5
-INT32_MIN, INT32_MAX = -2 ** 31, 2 ** 31 - 1
 ROW = 48
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch
-
-
-@pytest.fixture(scope="module")
-def coll_mod(coll_lib):
-    from container_engine_accelerators_b200.ops import coll
-    coll.load()
-    return coll
-
-
-def _dt(torch, name):
-    return {"bf16": torch.bfloat16, "f16": torch.float16, "f32": torch.float32}[name]
-
-
-class Plan:
-    """rows[s, d] dispatch rows of rank s (from its row send_off[s, d]) went to rank d (to its expert_out row recv_off[d, s]); index[s] and
-    weights[s] are rank s's [tokens, top_k] combine arguments."""
-
-    def __init__(self, rows, send_off, recv_off, index, weights):
-        self.rows, self.send_off, self.recv_off = (np.asarray(a, dtype=np.int64) for a in (rows, send_off, recv_off))
-        self.index, self.weights = index, weights
-        n = len(self.rows)
-        self.recv_rows = int(max((self.recv_off[d] + self.rows[:, d]).max() for d in range(n)))
-
-    def args(self, r):
-        n = len(self.rows)
-        return self.rows[r].tolist(), self.send_off[r].tolist(), [int(self.recv_off[d, r]) for d in range(n)]
 
 
 def _spoil(index, rng):
@@ -113,68 +75,45 @@ def hand_plan(n, top_k, seed):
     return Plan(rows, send_off, recv_off, index, weights)
 
 
-class Group:
-    def __init__(self, torch, coll, n, arena_mb=64, devices=None):
-        self.torch, self.coll = torch, coll
-        self.comms = coll.Comm.init_all(devices if devices is not None else [0] * n, arena_mb=arena_mb)
-        self.n = n
-        self.streams = []
-        for c in self.comms:
-            with torch.cuda.device(c.device):
-                self.streams.append(torch.cuda.Stream())
+def expert_outs(g, recv_rows, in_dt, seed, specials=True):
+    """(CPU copies, arena tensors) of every rank's [recv_rows, ROW] expert_out."""
+    torch = g.torch
+    xs = [qr.gen(recv_rows * ROW, in_dt, 16, seed + 17 * r, specials=specials) for r in range(g.n)]
+    ds = []
+    for c, x in zip(g.comms, xs):
+        with torch.cuda.device(c.device):
+            d = c.empty(x.numel(), in_dt)
+            d.copy_(x)
+        ds.append(d)
+    g.sync()
+    return xs, ds
 
-    def sync(self):
-        for d in {c.device for c in self.comms}:
-            self.torch.cuda.synchronize(d)
 
-    def destroy(self):
-        self.sync()
-        for c in self.comms:
-            c.destroy()
+def poisoned_outs(g, plan, out_dt):
+    """Every rank's out, all bytes 0x5A."""
+    torch = g.torch
+    res = []
+    for r, c in enumerate(g.comms):
+        t = torch.full((plan.index[r].shape[0] * ROW * torch.empty((), dtype=out_dt).element_size(),), 0x5A, dtype=torch.uint8, device=f"cuda:{c.device}")
+        res.append(t.view(out_dt))
+    return res
 
-    def expert_outs(self, recv_rows, in_dt, seed, specials=True):
-        """(CPU copies, arena tensors) of every rank's [recv_rows, ROW] expert_out."""
-        torch = self.torch
-        xs = [qr.gen(recv_rows * ROW, in_dt, 16, seed + 17 * r, specials=specials) for r in range(self.n)]
-        ds = []
-        for c, x in zip(self.comms, xs):
-            with torch.cuda.device(c.device):
-                d = c.empty(x.numel(), in_dt)
-                d.copy_(x)
-            ds.append(d)
-        self.sync()
-        return xs, ds
 
-    def dev(self, c, a):
-        return None if a is None else self.torch.from_numpy(np.ascontiguousarray(a)).to(f"cuda:{c.device}")
+def call(g, eo, outs, plan, weights, scale, idx_dev=None, w_dev=None):
+    idx_dev = idx_dev or [g.dev(c, plan.index[r]) for r, c in enumerate(g.comms)]
+    w_dev = w_dev or [g.dev(c, plan.weights[r]) if weights else None for r, c in enumerate(g.comms)]
+    g.sync()                                                         # index and weights were copied on the default stream
+    g.run(lambda r, c, st: c.all_to_all_v_combine(eo[r], outs[r], ROW, *plan.args(r), idx_dev[r], w_dev[r], scale=scale, stream=st))
 
-    def outs(self, plan, out_dt):
-        torch = self.torch
-        res = []
-        for r, c in enumerate(self.comms):
-            t = torch.full((plan.index[r].shape[0] * ROW * torch.empty((), dtype=out_dt).element_size(),), 0x5A, dtype=torch.uint8, device=f"cuda:{c.device}")
-            res.append(t.view(out_dt))
-        return res
 
-    def call(self, eo, outs, plan, weights, scale, idx_dev=None, w_dev=None):
-        idx_dev = idx_dev or [self.dev(c, plan.index[r]) for r, c in enumerate(self.comms)]
-        w_dev = w_dev or [self.dev(c, plan.weights[r]) if weights else None for r, c in enumerate(self.comms)]
-        self.sync()                                                  # index and weights were copied on the default stream
-        for r, c in enumerate(self.comms):
-            with self.torch.cuda.device(c.device):
-                c.all_to_all_v_combine(eo[r], outs[r], ROW, *plan.args(r), idx_dev[r], w_dev[r], scale=scale, stream=self.streams[r])
-        self.sync()
-        for c in self.comms:
-            c.check_async_error()
-
-    def check(self, xs, outs, plan, weights, scale, what):
-        got = [o.cpu() for o in outs]
-        eo = [x.float().numpy().reshape(-1, ROW) for x in xs]
-        for r in range(self.n):
-            rows, so, ro = plan.args(r)
-            look = cr.plan_lookup(eo, rows, so, ro)
-            want = cr.combine(look, plan.index[r], plan.weights[r] if weights else None, scale, got[r].dtype)
-            assert_same(got[r], want.reshape(-1), f"{what}: rank {r}")
+def check(g, xs, outs, plan, weights, scale, what):
+    got = [o.cpu() for o in outs]
+    eo = [x.float().numpy().reshape(-1, ROW) for x in xs]
+    for r in range(g.n):
+        rows, so, ro = plan.args(r)
+        look = cr.plan_lookup(eo, rows, so, ro)
+        want = cr.combine(look, plan.index[r], plan.weights[r] if weights else None, scale, got[r].dtype)
+        assert_same(got[r], want.reshape(-1), f"{what}: rank {r}")
 
 
 @pytest.mark.parametrize("out_name", ["bf16", "f16", "f32"])
@@ -184,20 +123,19 @@ def test_grid_bit_exact(torch_cuda, coll_mod, n, in_name, out_name):
     """top_k 1, 2 and 8, with weights and without, scale 1 and not; a skewed dispatch plan and the hand plan; dropped slots of every
     kind; one launch per call and rank, the stats under alltoall."""
     torch, coll = torch_cuda, coll_mod
-    in_dt, out_dt = _dt(torch, in_name), _dt(torch, out_name)
-    g = Group(torch, coll, n)
-    try:
+    in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
+    with Group(torch, coll, n) as g:
         for top_k in (1, 2, 8):
             plans = [dispatch_plan(n, top_k, seed=n * 10 + top_k), hand_plan(n, top_k, seed=n + top_k)]
             recv_rows = max(p.recv_rows for p in plans) + 3
-            xs, eo = g.expert_outs(recv_rows, in_dt, seed=top_k + n)
+            xs, eo = expert_outs(g, recv_rows, in_dt, seed=top_k + n)
             for k, plan in enumerate(plans):
                 for weights, scale in ((True, 1.0), (True, 0.375), (False, 1.0), (False, -3.0)):
-                    outs = g.outs(plan, out_dt)
+                    outs = poisoned_outs(g, plan, out_dt)
                     before = [c.stats() for c in g.comms]
-                    g.call(eo, outs, plan, weights, scale)
+                    call(g, eo, outs, plan, weights, scale)
                     what = f"n={n} {in_name}->{out_name} top_k {top_k} plan {k} weights {weights} scale {scale}"
-                    g.check(xs, outs, plan, weights, scale, what)
+                    check(g, xs, outs, plan, weights, scale, what)
                     for r, c in enumerate(g.comms):
                         st, b = c.stats(), before[r]
                         assert st["kernel_launches"] == b["kernel_launches"] + 1, what
@@ -208,8 +146,6 @@ def test_grid_bit_exact(torch_cuda, coll_mod, n, in_name, out_name):
                         assert st["bytes"][coll.OP_ALLTOALL] == b["bytes"][coll.OP_ALLTOALL] + pulled, what
             for c, d in zip(g.comms, eo):
                 c.release(d)
-    finally:
-        g.destroy()
 
 
 def _dispatch_send(torch, x, index):
@@ -226,8 +162,7 @@ def test_inverse_of_all_to_all_v(torch_cuda, coll_mod, n):
     torch, coll = torch_cuda, coll_mod
     from container_engine_accelerators_b200.models.workloads import expert_dispatch_plan
     p = expert_dispatch_plan(n, 40, ROW, top_k=1, skew=1.3, seed=4)
-    g = Group(torch, coll, n)
-    try:
+    with Group(torch, coll, n) as g:
         gen = torch.Generator().manual_seed(7)
         xs = [(torch.randn(40, ROW, generator=gen) * 3 + 0.5).to(torch.bfloat16) for _ in range(n)]
         sends = [_dispatch_send(torch, xs[r], p.index[r]).cuda() for r in range(n)]
@@ -236,15 +171,13 @@ def test_inverse_of_all_to_all_v(torch_cuda, coll_mod, n):
         g.sync()
         for r, c in enumerate(g.comms):
             c.all_to_all_v(sends[r].view(-1), eo[r], ROW, *plan.args(r), stream=g.streams[r])
-        outs = g.outs(plan, torch.bfloat16)
+        outs = poisoned_outs(g, plan, torch.bfloat16)
         g.sync()
-        g.call(eo, outs, plan, False, 1.0)
+        call(g, eo, outs, plan, False, 1.0)
         for r in range(n):
             assert_same(outs[r].cpu().view(40, ROW), xs[r], f"rank {r}: combine after all_to_all_v", nan_payloads=True)
         for c, d in zip(g.comms, eo):
             c.release(d)
-    finally:
-        g.destroy()
 
 
 def test_moe_round_trip(torch_cuda, coll_mod):
@@ -255,8 +188,7 @@ def test_moe_round_trip(torch_cuda, coll_mod):
     n, tokens, top_k, block, row = 4, 64, 2, 128, 256
     p = expert_dispatch_plan(n, tokens, row, top_k=top_k, skew=1.0, seed=12)
     plan = Plan(p.rows, p.send_off, p.recv_off, p.index, p.weights)
-    g = Group(torch, coll, n)
-    try:
+    with Group(torch, coll, n) as g:
         gen = torch.Generator().manual_seed(3)
         xs = [torch.randn(tokens, row, generator=gen).to(torch.bfloat16) for _ in range(n)]
         sends = [_dispatch_send(torch, xs[r], p.index[r]).cuda().view(-1) for r in range(n)]
@@ -277,8 +209,7 @@ def test_moe_round_trip(torch_cuda, coll_mod):
         for r, c in enumerate(g.comms):
             c.all_to_all_v_combine(eo[r], outs[r], row, *plan.args(r), idx[r], gate[r], stream=g.streams[r])
         g.sync()
-        for c in g.comms:
-            c.check_async_error()
+        g.check_async()
         eo_cpu = [e.float().cpu().numpy().reshape(-1, row) for e in eo]
         for r in range(n):
             rows, so, ro = plan.args(r)
@@ -290,8 +221,6 @@ def test_moe_round_trip(torch_cuda, coll_mod):
             exact = xs[r].float() * wf[:, None]
             tol = 0.08 * exact.abs() + 1e-3 * wf[:, None] * xs[r].float().abs().amax(dim=1, keepdim=True)
             assert ((got - exact).abs() <= tol).all(), f"rank {r}: {float((got - exact).abs().max())}"
-    finally:
-        g.destroy()
 
 
 def test_back_to_back_calls_with_few_ctas(torch_cuda, coll_mod):
@@ -299,17 +228,16 @@ def test_back_to_back_calls_with_few_ctas(torch_cuda, coll_mod):
     barrier must keep every peer's first pull ahead of the rewrite."""
     torch, coll = torch_cuda, coll_mod
     n, top_k = 4, 8
-    g = Group(torch, coll, n)
-    try:
+    with Group(torch, coll, n) as g:
         for c in g.comms:
             c.set_max_ctas(3)
         plan = dispatch_plan(n, top_k, seed=21, tokens=160)
-        xs, eo = g.expert_outs(plan.recv_rows, torch.bfloat16, seed=5)
+        xs, eo = expert_outs(g, plan.recv_rows, torch.bfloat16, seed=5)
         xs2 = [qr.gen(plan.recv_rows * ROW, torch.bfloat16, 16, 900 + r) for r in range(n)]
         new = [x.cuda() for x in xs2]
         idx = [g.dev(c, plan.index[r]) for r, c in enumerate(g.comms)]
         w = [g.dev(c, plan.weights[r]) for r, c in enumerate(g.comms)]
-        o1, o2 = g.outs(plan, torch.float32), g.outs(plan, torch.float32)
+        o1, o2 = poisoned_outs(g, plan, torch.float32), poisoned_outs(g, plan, torch.float32)
         g.sync()
         for r, c in enumerate(g.comms):
             c.all_to_all_v_combine(eo[r], o1[r], ROW, *plan.args(r), idx[r], w[r], stream=g.streams[r])
@@ -317,26 +245,22 @@ def test_back_to_back_calls_with_few_ctas(torch_cuda, coll_mod):
                 eo[r].copy_(new[r])
             c.all_to_all_v_combine(eo[r], o2[r], ROW, *plan.args(r), idx[r], w[r], stream=g.streams[r])
         g.sync()
-        for c in g.comms:
-            c.check_async_error()
-        g.check(xs, o1, plan, True, 1.0, "first of two calls")
-        g.check(xs2, o2, plan, True, 1.0, "second of two calls")
+        g.check_async()
+        check(g, xs, o1, plan, True, 1.0, "first of two calls")
+        check(g, xs2, o2, plan, True, 1.0, "second of two calls")
         for c in g.comms:
             assert c.stats()["kernel_launches"] == 2
-    finally:
-        g.destroy()
 
 
 def test_cuda_graph_replays_the_same_bits(torch_cuda, coll_mod):
     torch, coll = torch_cuda, coll_mod
     n, top_k = 3, 2
-    g = Group(torch, coll, n)
-    try:
+    with Group(torch, coll, n) as g:
         plan = dispatch_plan(n, top_k, seed=9)
-        xs, eo = g.expert_outs(plan.recv_rows, torch.float16, seed=44)
+        xs, eo = expert_outs(g, plan.recv_rows, torch.float16, seed=44)
         idx = [g.dev(c, plan.index[r]) for r, c in enumerate(g.comms)]
         w = [g.dev(c, plan.weights[r]) for r, c in enumerate(g.comms)]
-        outs = g.outs(plan, torch.bfloat16)
+        outs = poisoned_outs(g, plan, torch.bfloat16)
         g.sync()
         graphs = []
         for r, c in enumerate(g.comms):
@@ -352,12 +276,9 @@ def test_cuda_graph_replays_the_same_bits(torch_cuda, coll_mod):
                 with torch.cuda.stream(g.streams[r]):
                     gr.replay()
             g.sync()
-            for c in g.comms:
-                c.check_async_error()
-            g.check(xs, outs, plan, True, 0.5, f"graph replay {rep}")
+            g.check_async()
+            check(g, xs, outs, plan, True, 0.5, f"graph replay {rep}")
         del graphs
-    finally:
-        g.destroy()
 
 
 def _raw(coll, comm, eo, out, row_elems, recv_rows, rows, soff, roff, index, weights, tokens, top_k, in_dt, out_dt):
@@ -371,9 +292,7 @@ def _raw(coll, comm, eo, out, row_elems, recv_rows, rows, soff, roff, index, wei
 
 def test_placement_and_argument_errors(torch_cuda, coll_mod):
     torch, coll = torch_cuda, coll_mod
-    L = coll.load()
-    g = Group(torch, coll, 2)
-    try:
+    with Group(torch, coll, 2) as g:
         c = g.comms[0]
         row, rows_n = 64, 8
         eo = c.empty(rows_n * row, torch.bfloat16)
@@ -414,29 +333,22 @@ def test_placement_and_argument_errors(torch_cuda, coll_mod):
             a = dict(ok, **kw)
             rc = _raw(coll, c, a["eo"], a["out"], a["row_elems"], a["recv_rows"], a["rows"], a["soff"], a["roff"], a["index"], a["weights"],
                       a["tokens"], a["top_k"], a["in_dt"], a["out_dt"])
-            assert rc == want, (what, rc, L.b200collGetLastError().decode())
-            assert L.b200collGetLastError().decode(), what
+            expect_refused(rc, want, what=what)
         with pytest.raises(ValueError):
             c.all_to_all_v_combine(eo, out, row, [2, 3], [0, 1], [0, 4], idx, w)          # Python refuses it before the library call
-        assert c.stats()["kernel_launches"] == 0 and all(x == 0 for x in c.stats()["calls"])   # nothing was launched or counted
-        for comm in g.comms:
-            comm.check_async_error()
+        assert_nothing_launched(c)                                                      # nothing was launched or counted
+        g.check_async()
         del eo
-    finally:
-        g.destroy()
     # one rank: expert_out may be any device buffer
-    g = Group(torch, coll, 1)
-    try:
+    with Group(torch, coll, 1) as g:
         plan = hand_plan(1, 3, seed=2)
         xs = [qr.gen(plan.recv_rows * ROW, torch.float32, 16, 8)]
         eo = [xs[0].cuda()]
         assert not g.comms[0].is_symmetric(eo[0])
-        outs = g.outs(plan, torch.float16)
-        g.call(eo, outs, plan, True, 2.0)
-        g.check(xs, outs, plan, True, 2.0, "one rank outside the arena")
+        outs = poisoned_outs(g, plan, torch.float16)
+        call(g, eo, outs, plan, True, 2.0)
+        check(g, xs, outs, plan, True, 2.0, "one rank outside the arena")
         assert g.comms[0].stats()["algo_calls"]["copy"] == 1 and g.comms[0].stats()["kernel_launches"] == 1
-    finally:
-        g.destroy()
 
 
 def test_multi_gpu(torch_cuda, coll_mod):
@@ -444,25 +356,20 @@ def test_multi_gpu(torch_cuda, coll_mod):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
     n = torch.cuda.device_count()
-    g = Group(torch, coll, n, arena_mb=256, devices=list(range(n)))
-    try:
+    with Group(torch, coll, n, arena_mb=256, devices=list(range(n))) as g:
         for plan in (dispatch_plan(n, 8, seed=1, tokens=512), hand_plan(n, 2, seed=3)):
-            xs, eo = g.expert_outs(plan.recv_rows, torch.bfloat16, seed=90)
-            outs = g.outs(plan, torch.bfloat16)
-            g.call(eo, outs, plan, True, 1.0)
-            g.check(xs, outs, plan, True, 1.0, "multi-GPU")
+            xs, eo = expert_outs(g, plan.recv_rows, torch.bfloat16, seed=90)
+            outs = poisoned_outs(g, plan, torch.bfloat16)
+            call(g, eo, outs, plan, True, 1.0)
+            check(g, xs, outs, plan, True, 1.0, "multi-GPU")
             for c, d in zip(g.comms, eo):
                 c.release(d)
-    finally:
-        g.destroy()
 
 
 def test_perf_tool_combine_bit_exact(torch_cuda, coll_lib):
     for devs, extra in (("0,0", ["-d", "bfloat16", "--out-dtype", "float", "--combine", "4", "-b", "64K", "-e", "4M", "-f", "8"]),
                         ("0,0,0", ["-d", "half", "--out-dtype", "bfloat16", "--combine", "2", "--row-len", "96", "-b", "1M", "-e", "1M"]),
                         ("0", ["-d", "float", "--out-dtype", "half", "--combine", "8", "--row-len", "512", "-b", "1M", "-e", "1M"])):
-        r = subprocess.run([PERF, "--devs", devs, "--op", "alltoall", *extra, "-w", "1", "-n", "2", "-c", "1"], capture_output=True, text=True,
-                           timeout=600)
-        assert r.returncode == 0 and "errors=0" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
-        rows = [l for l in r.stdout.splitlines() if l.strip() and not l.startswith("#")]
-        assert rows, r.stdout
+        out = run_perf(["--op", "alltoall", *extra, "-w", "1", "-n", "2", "-c", "1"], devs)
+        rows = [l for l in out.splitlines() if l.strip() and not l.startswith("#")]
+        assert rows, out

@@ -4,54 +4,17 @@ Every received FP8 byte and scale is checked bit for bit against tests/coll_quan
 (NaN matches NaN at the same position); recv and recv_scales start poisoned with 0x5A, and every byte outside the received ranges must
 still hold it."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from container_engine_accelerators_b200.ops.coll import INVALID_ARGUMENT, INVALID_USAGE
 from tests import coll_quant_reference as qr
 from tests.coll_fp_reference import assert_same
+from tests.coll_gpu_harness import DTYPES, Group, Plan, assert_nothing_launched, coll_mod, expect_refused, run_perf, torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PERF = os.path.join(ROOT, "build", "b200coll_perf")
-INVALID_ARGUMENT, INVALID_USAGE = 4, 5
 ROW = {16: 80, 128: 384, 512: 1024}                                     # row_elems per block: several blocks per row, or one
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch
-
-
-@pytest.fixture(scope="module")
-def coll_mod(coll_lib):
-    from container_engine_accelerators_b200.ops import coll
-    coll.load()
-    return coll
-
-
-def _dt(torch, name):
-    return {"bf16": torch.bfloat16, "f16": torch.float16, "f32": torch.float32, "e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}[name]
-
-
-class Plan:
-    """rows[s, d] rows go from rank s (starting at its row send_off[s, d]) to rank d (landing at its row recv_off[d, s])."""
-
-    def __init__(self, rows, send_off, recv_off):
-        self.rows, self.send_off, self.recv_off = (np.asarray(a, dtype=np.int64) for a in (rows, send_off, recv_off))
-        n = len(self.rows)
-        self.src_rows = int(max((self.send_off[s] + self.rows[s]).max() for s in range(n)))
-        self.recv_rows = int(max((self.recv_off[d] + self.rows[:, d]).max() for d in range(n)))
-
-    def args(self, r):
-        n = len(self.rows)
-        return self.rows[r].tolist(), self.send_off[r].tolist(), [int(self.recv_off[d, r]) for d in range(n)]
 
 
 def dispatch_plan(n, seed, skew=1.2, tokens=48):
@@ -100,69 +63,48 @@ def expected(torch, xs, plan, d, row_elems, block, wire, recv_rows, start=None):
     return q.view(wire), s
 
 
-class Group:
-    def __init__(self, torch, coll, n, arena_mb=64, devices=None):
-        self.torch, self.coll = torch, coll
-        self.comms = coll.Comm.init_all(devices if devices is not None else [0] * n, arena_mb=arena_mb)
-        self.n = n
-        self.streams = []
-        for c in self.comms:
-            with torch.cuda.device(c.device):
-                self.streams.append(torch.cuda.Stream())
+def inputs(g, rows, row_elems, in_dt, block, seed, arena=False):
+    torch = g.torch
+    xs = [qr.gen(rows * row_elems, in_dt, block, seed + 17 * r) for r in range(g.n)]
+    ds = []
+    for c, x in zip(g.comms, xs):
+        with torch.cuda.device(c.device):
+            d = c.empty(x.numel(), in_dt) if arena else torch.empty(x.numel(), dtype=in_dt, device=f"cuda:{c.device}")
+            d.copy_(x)
+        ds.append(d)
+    g.sync()
+    return xs, ds
 
-    def sync(self):
-        for d in {c.device for c in self.comms}:
-            self.torch.cuda.synchronize(d)
 
-    def destroy(self):
-        self.sync()
-        for c in self.comms:
-            c.destroy()
+def outputs(g, recv_rows, row_elems, block, wire):
+    torch = g.torch
+    outs = []
+    for c in g.comms:
+        with torch.cuda.device(c.device):
+            q, s = c.empty(recv_rows * row_elems, wire), c.empty(recv_rows * row_elems // block, torch.float32)
+            q.view(torch.uint8).fill_(0x5A)
+            s.view(torch.uint8).fill_(0x5A)
+        outs.append((q, s))
+    g.sync()
+    return outs
 
-    def inputs(self, rows, row_elems, in_dt, block, seed, arena=False):
-        torch = self.torch
-        xs = [qr.gen(rows * row_elems, in_dt, block, seed + 17 * r) for r in range(self.n)]
-        ds = []
-        for c, x in zip(self.comms, xs):
-            with torch.cuda.device(c.device):
-                d = c.empty(x.numel(), in_dt) if arena else torch.empty(x.numel(), dtype=in_dt, device=f"cuda:{c.device}")
-                d.copy_(x)
-            ds.append(d)
-        self.sync()
-        return xs, ds
 
-    def outputs(self, recv_rows, row_elems, block, wire):
-        torch = self.torch
-        outs = []
-        for c in self.comms:
-            with torch.cuda.device(c.device):
-                q, s = c.empty(recv_rows * row_elems, wire), c.empty(recv_rows * row_elems // block, torch.float32)
-                q.view(torch.uint8).fill_(0x5A)
-                s.view(torch.uint8).fill_(0x5A)
-            outs.append((q, s))
-        self.sync()
-        return outs
+def call(g, ds, outs, plan, row_elems, block):
+    g.run(lambda r, c, st: c.all_to_all_v_quantized(ds[r], outs[r][0], outs[r][1], row_elems, *plan.args(r), block=block, stream=st))
 
-    def call(self, ds, outs, plan, row_elems, block):
-        for r, c in enumerate(self.comms):
-            with self.torch.cuda.device(c.device):
-                c.all_to_all_v_quantized(ds[r], outs[r][0], outs[r][1], row_elems, *plan.args(r), block=block, stream=self.streams[r])
-        self.sync()
-        for c in self.comms:
-            c.check_async_error()
 
-    @staticmethod
-    def fetch(outs):
-        """CPU copies of every rank's (q, s): the checks take these, so a failing assert never holds device tensors whose arena memory the
-        clean-up unmaps before the report is written."""
-        return [(q.cpu(), s.cpu()) for q, s in outs]
+def fetch(outs):
+    """CPU copies of every rank's (q, s): the checks take these, so a failing assert never holds device tensors whose arena memory the
+    clean-up unmaps before the report is written."""
+    return [(q.cpu(), s.cpu()) for q, s in outs]
 
-    def check(self, xs, got, plan, row_elems, block, wire, what, starts=None):
-        for d in range(self.n):
-            q, s = got[d]
-            wq, ws = expected(self.torch, xs, plan, d, row_elems, block, wire, q.numel() // row_elems, None if starts is None else starts[d])
-            assert_same(q, wq, f"{what}: rank {d} FP8 rows")
-            assert_same(s, ws, f"{what}: rank {d} scales")
+
+def check(g, xs, got, plan, row_elems, block, wire, what, starts=None):
+    for d in range(g.n):
+        q, s = got[d]
+        wq, ws = expected(g.torch, xs, plan, d, row_elems, block, wire, q.numel() // row_elems, None if starts is None else starts[d])
+        assert_same(q, wq, f"{what}: rank {d} FP8 rows")
+        assert_same(s, ws, f"{what}: rank {d} scales")
 
 
 @pytest.mark.parametrize("in_name", ["bf16", "f16", "f32"])
@@ -171,23 +113,22 @@ def test_grid_bit_exact(torch_cuda, coll_mod, n, in_name):
     """Every wire type and block size, on a skewed expert-dispatch plan and on the hand plan (a rank that sends nothing, one that
     receives nothing, rows to self); one launch per call and rank, stats under alltoall."""
     torch, coll = torch_cuda, coll_mod
-    in_dt = _dt(torch, in_name)
-    g = Group(torch, coll, n)
-    try:
+    in_dt = DTYPES[in_name]
+    with Group(torch, coll, n) as g:
         for wire_name in ("e4m3", "e5m2"):
-            wire = _dt(torch, wire_name)
+            wire = DTYPES[wire_name]
             for block in (16, 128, 512):
                 row_elems = ROW[block]
                 plans = [dispatch_plan(n, seed=n + block), hand_plan(n)]
                 src_rows = max(p.src_rows for p in plans)
                 recv_rows = max(p.recv_rows for p in plans) + 3
-                xs, ds = g.inputs(src_rows, row_elems, in_dt, block, seed=block + n)
+                xs, ds = inputs(g, src_rows, row_elems, in_dt, block, seed=block + n)
                 for k, plan in enumerate(plans):
-                    outs = g.outputs(recv_rows, row_elems, block, wire)
+                    outs = outputs(g, recv_rows, row_elems, block, wire)
                     before = [c.stats() for c in g.comms]
-                    g.call(ds, outs, plan, row_elems, block)
+                    call(g, ds, outs, plan, row_elems, block)
                     what = f"n={n} {in_name}->{wire_name} block {block} plan {k}"
-                    g.check(xs, g.fetch(outs), plan, row_elems, block, wire, what)
+                    check(g, xs, fetch(outs), plan, row_elems, block, wire, what)
                     for r, c in enumerate(g.comms):
                         st, b = c.stats(), before[r]
                         assert st["kernel_launches"] == b["kernel_launches"] + 1, what
@@ -199,44 +140,37 @@ def test_grid_bit_exact(torch_cuda, coll_mod, n, in_name):
                     for c, (q, s) in zip(g.comms, outs):
                         c.release(q)
                         c.release(s)
-    finally:
-        g.destroy()
 
 
 def test_arena_send_repeated_calls_and_few_ctas(torch_cuda, coll_mod):
     """send in the arena; two back-to-back calls with different plans into the same buffers, with few CTAs so each walks many warps."""
     torch, coll = torch_cuda, coll_mod
     n, block, row_elems, wire = 4, 64, 256, torch.float8_e4m3fn
-    g = Group(torch, coll, n)
-    try:
+    with Group(torch, coll, n) as g:
         for c in g.comms:
             c.set_max_ctas(3)
         a, b = hand_plan(n), dispatch_plan(n, seed=5, tokens=200)
-        xs, ds = g.inputs(max(a.src_rows, b.src_rows), row_elems, torch.bfloat16, block, seed=31, arena=True)
+        xs, ds = inputs(g, max(a.src_rows, b.src_rows), row_elems, torch.bfloat16, block, seed=31, arena=True)
         recv_rows = max(a.recv_rows, b.recv_rows)
-        outs = g.outputs(recv_rows, row_elems, block, wire)
+        outs = outputs(g, recv_rows, row_elems, block, wire)
         for r, c in enumerate(g.comms):
             for plan in (a, b):
                 c.all_to_all_v_quantized(ds[r], outs[r][0], outs[r][1], row_elems, *plan.args(r), block=block, stream=g.streams[r])
         g.sync()
-        for c in g.comms:
-            c.check_async_error()
+        g.check_async()
         starts = [expected(torch, xs, a, d, row_elems, block, wire, recv_rows) for d in range(n)]
-        g.check(xs, g.fetch(outs), b, row_elems, block, wire, "second of two back-to-back calls", starts=starts)
+        check(g, xs, fetch(outs), b, row_elems, block, wire, "second of two back-to-back calls", starts=starts)
         for c in g.comms:
             assert c.stats()["kernel_launches"] == 2
-    finally:
-        g.destroy()
 
 
 def test_cuda_graph_replays_the_same_bits(torch_cuda, coll_mod):
     torch, coll = torch_cuda, coll_mod
     n, block, row_elems, wire = 3, 128, 512, torch.float8_e5m2
-    g = Group(torch, coll, n)
-    try:
+    with Group(torch, coll, n) as g:
         plan = dispatch_plan(n, seed=9)
-        xs, ds = g.inputs(plan.src_rows, row_elems, torch.float32, block, seed=44)
-        outs = g.outputs(plan.recv_rows + 1, row_elems, block, wire)
+        xs, ds = inputs(g, plan.src_rows, row_elems, torch.float32, block, seed=44)
+        outs = outputs(g, plan.recv_rows + 1, row_elems, block, wire)
         graphs = []
         for r, c in enumerate(g.comms):
             gr = torch.cuda.CUDAGraph()
@@ -252,29 +186,23 @@ def test_cuda_graph_replays_the_same_bits(torch_cuda, coll_mod):
                 with torch.cuda.stream(g.streams[r]):
                     gr.replay()
             g.sync()
-            for c in g.comms:
-                c.check_async_error()
-            g.check(xs, g.fetch(outs), plan, row_elems, block, wire, f"graph replay {rep}")
+            g.check_async()
+            check(g, xs, fetch(outs), plan, row_elems, block, wire, f"graph replay {rep}")
         del graphs
-    finally:
-        g.destroy()
 
 
 def test_received_blocks_feed_the_block_scaled_all_gather(torch_cuda, coll_mod):
     """(q, s) as received is a valid block-scaled input with block (1, block): a one-rank all-gather of it gives round(float(q) * s)."""
     torch, coll = torch_cuda, coll_mod
     n, block, row_elems, wire = 2, 32, 128, torch.float8_e4m3fn
-    g = Group(torch, coll, n)
-    try:
+    with Group(torch, coll, n) as g:
         plan = dispatch_plan(n, seed=3)
-        xs, ds = g.inputs(plan.src_rows, row_elems, torch.bfloat16, block, seed=8)
-        outs = g.outputs(plan.recv_rows, row_elems, block, wire)
-        g.call(ds, outs, plan, row_elems, block)
-        got = g.fetch(outs)
-    finally:
-        g.destroy()
-    (c1,) = coll.Comm.init_all([0], arena_mb=16)
-    try:
+        xs, ds = inputs(g, plan.src_rows, row_elems, torch.bfloat16, block, seed=8)
+        outs = outputs(g, plan.recv_rows, row_elems, block, wire)
+        call(g, ds, outs, plan, row_elems, block)
+        got = fetch(outs)
+    with Group(torch, coll, 1, arena_mb=16) as g1:
+        c1 = g1.comms[0]
         for d, (q, s) in enumerate(got):
             rows = q.numel() // row_elems
             bq, bs = c1.empty(q.numel(), wire), c1.empty(s.numel(), torch.float32)        # arena tensors, released below
@@ -292,9 +220,6 @@ def test_received_blocks_feed_the_block_scaled_all_gather(torch_cuda, coll_mod):
             c1.release(bq)
             c1.release(bs)
         c1.check_async_error()
-    finally:
-        torch.cuda.synchronize()
-        c1.destroy()
 
 
 def _raw(coll, comm, send, recv, scales, row_elems, recv_rows, rows, soff, roff, in_dt, wire, block):
@@ -306,9 +231,7 @@ def _raw(coll, comm, send, recv, scales, row_elems, recv_rows, rows, soff, roff,
 
 def test_placement_and_argument_errors(torch_cuda, coll_mod):
     torch, coll = torch_cuda, coll_mod
-    L = coll.load()
-    g = Group(torch, coll, 2)
-    try:
+    with Group(torch, coll, 2) as g:
         c = g.comms[0]
         row, blk, rows = 256, 128, 8
         send = torch.empty(rows * row, dtype=torch.bfloat16, device="cuda")
@@ -342,29 +265,22 @@ def test_placement_and_argument_errors(torch_cuda, coll_mod):
         for what, want, kw in cases:
             a = dict(ok, **kw)
             rc = _raw(coll, c, a["send"], a["recv"], a["scales"], a["row_elems"], a["recv_rows"], a["rows"], a["soff"], a["roff"], a["in_dt"], a["wire"], a["block"])
-            assert rc == want, (what, rc, L.b200collGetLastError().decode())
-            assert L.b200collGetLastError().decode(), what
+            expect_refused(rc, want, what=what)
         with pytest.raises(ValueError):
             c.all_to_all_v_quantized(send, q, s, row, [2, 3], [0, 2], [0, 6])                   # Python refuses it before the library call
-        assert c.stats()["kernel_launches"] == 0 and all(x == 0 for x in c.stats()["calls"])   # nothing was launched or counted
-        for comm in g.comms:
-            comm.check_async_error()
-    finally:
-        g.destroy()
+        assert_nothing_launched(c)                                                              # nothing was launched or counted
+        g.check_async()
     # one rank: recv and recv_scales may be any device buffers
-    g = Group(torch, coll, 1)
-    try:
+    with Group(torch, coll, 1) as g:
         block, row_elems, wire = 16, 64, torch.float8_e5m2
         plan = hand_plan(1)
-        xs, ds = g.inputs(plan.src_rows, row_elems, torch.float16, block, seed=2)
+        xs, ds = inputs(g, plan.src_rows, row_elems, torch.float16, block, seed=2)
         q = torch.full((plan.recv_rows * row_elems,), 0x5A, dtype=torch.uint8, device="cuda").view(wire)
         s = torch.full((plan.recv_rows * row_elems // block * 4,), 0x5A, dtype=torch.uint8, device="cuda").view(torch.float32)
         assert not g.comms[0].is_symmetric(q) and not g.comms[0].is_symmetric(s)
-        g.call(ds, [(q, s)], plan, row_elems, block)
-        g.check(xs, g.fetch([(q, s)]), plan, row_elems, block, wire, "one rank outside the arena")
+        call(g, ds, [(q, s)], plan, row_elems, block)
+        check(g, xs, fetch([(q, s)]), plan, row_elems, block, wire, "one rank outside the arena")
         assert g.comms[0].stats()["algo_calls"]["copy"] == 1 and g.comms[0].stats()["kernel_launches"] == 1
-    finally:
-        g.destroy()
 
 
 def test_multi_gpu(torch_cuda, coll_mod):
@@ -372,25 +288,19 @@ def test_multi_gpu(torch_cuda, coll_mod):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
     n, block, row_elems, wire = torch.cuda.device_count(), 128, 1024, torch.float8_e4m3fn
-    g = Group(torch, coll, n, arena_mb=256, devices=list(range(n)))
-    try:
+    with Group(torch, coll, n, arena_mb=256, devices=list(range(n))) as g:
         for plan in (dispatch_plan(n, seed=1, tokens=512), hand_plan(n)):
-            xs, ds = g.inputs(plan.src_rows, row_elems, torch.bfloat16, block, seed=90)
-            outs = g.outputs(plan.recv_rows, row_elems, block, wire)
-            g.call(ds, outs, plan, row_elems, block)
-            g.check(xs, g.fetch(outs), plan, row_elems, block, wire, "multi-GPU")
-    finally:
-        g.destroy()
+            xs, ds = inputs(g, plan.src_rows, row_elems, torch.bfloat16, block, seed=90)
+            outs = outputs(g, plan.recv_rows, row_elems, block, wire)
+            call(g, ds, outs, plan, row_elems, block)
+            check(g, xs, fetch(outs), plan, row_elems, block, wire, "multi-GPU")
 
 
 def test_perf_tool_alltoall_quantize_bit_exact(torch_cuda, coll_lib):
-    r = subprocess.run([PERF, "--devs", "0,0", "--op", "alltoall", "-d", "bfloat16", "--out-dtype", "e4m3", "--quantize", "e4m3:128",
-                        "-b", "64K", "-e", "4M", "-f", "8", "-w", "1", "-n", "2", "-c", "1"], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-    assert "errors=0" in r.stdout and "quantised: wire=e4m3 block=128" in r.stdout, r.stdout[-2000:]
-    rows = [l for l in r.stdout.splitlines() if l.strip() and not l.startswith("#")]
-    assert len(rows) == 3, r.stdout                                      # 64 KiB, 512 KiB and 4 MiB
+    out = run_perf(["--op", "alltoall", "-d", "bfloat16", "--out-dtype", "e4m3", "--quantize", "e4m3:128", "-b", "64K", "-e", "4M", "-f", "8",
+                    "-w", "1", "-n", "2", "-c", "1"], "0,0")
+    assert "quantised: wire=e4m3 block=128" in out, out[-2000:]
+    rows = [l for l in out.splitlines() if l.strip() and not l.startswith("#")]
+    assert len(rows) == 3, out                                           # 64 KiB, 512 KiB and 4 MiB
     for devs, extra in (("0,0,0", ["-d", "half", "--quantize", "e5m2:32", "--row-len", "96"]), ("0", ["-d", "float", "--quantize", "e4m3:512"])):
-        r = subprocess.run([PERF, "--devs", devs, "--op", "alltoall", *extra, "-b", "1M", "-e", "1M", "-w", "1", "-n", "2", "-c", "1"],
-                           capture_output=True, text=True, timeout=600)
-        assert r.returncode == 0 and "errors=0" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
+        run_perf(["--op", "alltoall", *extra, "-b", "1M", "-e", "1M", "-w", "1", "-n", "2", "-c", "1"], devs)

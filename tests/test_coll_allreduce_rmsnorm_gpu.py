@@ -2,52 +2,16 @@
 
 Bit-exact means equal (NaN matching NaN at the same position) to tests/coll_rmsnorm_reference.rms_norm, for both the new residual and
 out, on every rank."""
-import os
-import subprocess
-import sys
-
 import pytest
 
+from container_engine_accelerators_b200.ops.coll import INVALID_ARGUMENT, INVALID_USAGE
 from tests import coll_rmsnorm_reference as ref
 from tests.coll_fp_reference import assert_same
+from tests.coll_gpu_harness import DTYPES, Group, coll_mod, expect_refused, run_perf, run_python, torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PERF = os.path.join(ROOT, "build", "b200coll_perf")
-INVALID_ARGUMENT, INVALID_USAGE = 4, 5
-DTYPES = ("bf16", "f16", "f32")
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch
-
-
-@pytest.fixture(scope="module")
-def coll_mod(coll_lib):
-    from container_engine_accelerators_b200.ops import coll
-    coll.load()
-    return coll
-
-
-def _dt(torch, name):
-    return {"bf16": torch.bfloat16, "f16": torch.float16, "f32": torch.float32}[name]
-
-
-class Group:
-    def __init__(self, torch, coll, n, arena_mb=64):
-        self.torch, self.n = torch, n
-        self.comms = coll.Comm.init_all([0] * n, arena_mb=arena_mb)
-        self.streams = [torch.cuda.Stream() for _ in self.comms]
-
-    def destroy(self):
-        self.torch.cuda.synchronize()
-        for c in self.comms:
-            c.destroy()
+DT_NAMES = ("bf16", "f16", "f32")
 
 
 _groups = {}
@@ -55,7 +19,11 @@ _groups = {}
 
 @pytest.fixture(scope="module")
 def groups(torch_cuda, coll_mod):
-    yield lambda n: _groups.setdefault(n, Group(torch_cuda, coll_mod, n))
+    def get(n):
+        if n not in _groups:
+            _groups[n] = Group(torch_cuda, coll_mod, n)
+        return _groups[n]
+    yield get
     for g in _groups.values():
         g.destroy()
     _groups.clear()
@@ -123,11 +91,11 @@ def check(outs, xs, res, gamma, eps, what):
 SWEEP = [(1, [0, 1, 5]), (2, [0, 1, 7]), (3, [0, 1, 8]), (4, [0, 1, 10]), (8, [0, 1, 13])]
 
 
-@pytest.mark.parametrize("dtn", DTYPES)
+@pytest.mark.parametrize("dtn", DT_NAMES)
 @pytest.mark.parametrize("n,rows_list", SWEEP, ids=[f"n{n}" for n, _ in SWEEP])
 def test_bit_exact_sweep(torch_cuda, groups, n, rows_list, dtn):
     torch = torch_cuda
-    dt = _dt(torch, dtn)
+    dt = DTYPES[dtn]
     g = groups(n)
     algos = ("oneshot", "twoshot") if n > 1 else ("auto",)
     for row_len in (16, 4096, 7168, 16384):
@@ -150,8 +118,8 @@ def test_bit_exact_sweep(torch_cuda, groups, n, rows_list, dtn):
 def test_algorithm_independence(torch_cuda, groups, n):
     torch = torch_cuda
     g = groups(n)
-    for dtn in DTYPES:
-        xs, res, gamma = data(torch, n, 37, 7168, _dt(torch, dtn), seed=n)
+    for dtn in DT_NAMES:
+        xs, res, gamma = data(torch, n, 37, 7168, DTYPES[dtn], seed=n)
         one, _, _ = run(g, xs, res, gamma, 1e-5, "oneshot", True)
         two, _, _ = run(g, xs, res, gamma, 1e-5, "twoshot", True)
         for r in range(n):
@@ -167,8 +135,8 @@ def test_agrees_with_pytorch(torch_cuda, groups, n):
     import torch.nn.functional as F
     torch = torch_cuda
     g = groups(n)
-    for dtn in DTYPES:
-        dt = _dt(torch, dtn)
+    for dtn in DT_NAMES:
+        dt = DTYPES[dtn]
         for row_len in (4096, 7168):
             xs, res, gamma = data(torch, n, 64, row_len, dt, seed=7 + n)
             outs, _, _ = run(g, xs, res, gamma, 1e-6, "auto", True)
@@ -186,8 +154,8 @@ def test_agrees_with_pytorch(torch_cuda, groups, n):
 def test_special_values(torch_cuda, groups, n):
     torch = torch_cuda
     g = groups(n)
-    for dtn in DTYPES:
-        dt = _dt(torch, dtn)
+    for dtn in DT_NAMES:
+        dt = DTYPES[dtn]
         xs, res, gamma = data(torch, n, 6, 64, dt, seed=3)
         xs[0][0, 3] = float("nan")
         xs[-1][1, 17] = float("inf")
@@ -297,17 +265,13 @@ def test_refusals_launch_nothing(torch_cuda, coll_mod, groups):
     torch.cuda.synchronize()
     for args, code in cases:
         before = c.stats()
-        rc = L.b200collAllReduceRmsNorm(*args, c._h, C.c_void_p(0))
-        assert rc == code, (args, rc, L.b200collGetLastError().decode())
-        assert L.b200collGetLastError().decode(), args
+        expect_refused(L.b200collAllReduceRmsNorm(*args, c._h, C.c_void_p(0)), code, what=args)
         after = c.stats()
         assert after["kernel_launches"] == before["kernel_launches"] and after["calls"] == before["calls"], args
     c.release(xb)
 
 
 _LAZY = r'''
-import sys
-sys.path.insert(0, sys.argv[1])
 import torch
 from container_engine_accelerators_b200.ops import coll
 from tests import coll_rmsnorm_reference as ref
@@ -352,14 +316,11 @@ def test_lazy_module_loading_rms_norm(torch_cuda, coll_lib):
     """A fresh process with lazy module loading and a short watchdog drives two virtual ranks from one thread, each rank enqueueing three
     fused calls that run three different kernels: the first launch of the second and third must not wait behind the rank's own first
     kernel, which waits at its barrier for the other rank's call. The results must be exact."""
-    env = {**os.environ, "CUDA_MODULE_LOADING": "LAZY", "B200COLL_TIMEOUT_MS": "10000"}
-    r = subprocess.run([sys.executable, "-c", _LAZY, ROOT], cwd=ROOT, env=env, capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0 and "lazy ok" in r.stdout, r.stdout[-2000:] + r.stderr[-3000:]
+    run_python(_LAZY, {"CUDA_MODULE_LOADING": "LAZY", "B200COLL_TIMEOUT_MS": "10000"}, "lazy ok")
 
 
 @pytest.mark.parametrize("devs,dtype,row_len", [("0", "bfloat16", 8192), ("0,0", "half", 7168), ("0,0,0", "float", 4096)])
 def test_perf_tool_checks_every_value(torch_cuda, coll_lib, devs, dtype, row_len):
-    r = subprocess.run([PERF, "--devs", devs, "--op", "all_reduce", "-d", dtype, "--rms-norm", str(row_len), "-b", "64K", "-e", "4M", "-f", "4",
-                        "-w", "1", "-n", "2", "-c", "1"], capture_output=True, text=True, timeout=600, env={**os.environ, "B200COLL_TIMEOUT_MS": "20000"})
-    assert r.returncode == 0 and "errors=0" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
-    assert "op=all_reduce + rms-norm" in r.stdout, r.stdout
+    out = run_perf(["--op", "all_reduce", "-d", dtype, "--rms-norm", str(row_len), "-b", "64K", "-e", "4M", "-f", "4", "-w", "1", "-n", "2", "-c", "1"],
+                   devs, env={"B200COLL_TIMEOUT_MS": "20000"})
+    assert "op=all_reduce + rms-norm" in out, out

@@ -4,49 +4,22 @@ Every numeric check is bit for bit against a torch fp32 reference that applies t
 one per element, v = float(q) * s (one fp32 multiply), a rank-order sum starting from zeros, times the fp32 scale (avg: times the fp32
 value 1/N), one cast to the output type. NaN is compared as NaN (the NaN bit pattern a cast produces is not part of the semantics)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from tests.test_coll_fp8_gpu import random_fp8
+from container_engine_accelerators_b200.ops.coll import INVALID_ARGUMENT, INVALID_USAGE
+from tests.coll_fp_reference import random_fp8
+from tests.coll_gpu_harness import Group, assert_nothing_launched, coll_mod, expect_refused, group_fixture, run_perf, torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PERF = os.path.join(ROOT, "build", "b200coll_perf")
-INVALID_ARGUMENT, INVALID_USAGE = 4, 5
 
 # (rows, row_len, block): rows are multiples of 24 so that every N in {2, 3, 4, 8} can reduce-scatter them; the last three leave a
 # partial last block column, the last two a partial last block row as well
 CASES = [(48, 64, (1, 16)), (48, 400, (1, 128)), (264, 320, (128, 128)), (120, 208, (32, 64))]
 
 
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch
-
-
-@pytest.fixture(scope="module")
-def coll_mod(coll_lib):
-    from container_engine_accelerators_b200.ops import coll
-    coll.load()
-    return coll
-
-
-@pytest.fixture
-def group(torch_cuda, coll_mod, request):
-    n = getattr(request, "param", 2)
-    comms = coll_mod.Comm.init_all([0] * n, arena_mb=192)          # the heap starts 77 MiB into the arena; the grid test keeps its outputs
-    streams = [torch_cuda.cuda.Stream() for _ in comms]
-    yield comms, streams
-    torch_cuda.cuda.synchronize()
-    for c in comms:
-        c.destroy()
+group = group_fixture(2, arena_mb=192)          # the heap starts 77 MiB into the arena; the grid test keeps its outputs
 
 
 def f32(x):
@@ -128,14 +101,6 @@ def assert_same(torch, got, want, what):
         raise AssertionError(f"{what}: first difference at non-NaN element {i}: got {got[~gn][i].item()} want {want[~wn][i].item()}")
 
 
-def run_all(torch, comms, streams, fn):
-    for r, c in enumerate(comms):
-        fn(r, c, streams[r])
-    torch.cuda.synchronize()
-    for c in comms:
-        c.check_async_error()
-
-
 def out_dtypes(torch):
     return (torch.bfloat16, torch.float16, torch.float32)
 
@@ -147,8 +112,7 @@ def fp8_dtypes(torch):
 @pytest.mark.parametrize("group", [2, 3, 4, 8], indirect=True)
 def test_grid_bit_exact(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for ci, (rows, row_len, block) in enumerate(CASES):
         for di, dt in enumerate(fp8_dtypes(torch)):
             qs, ss = make_inputs(torch, comms, rows, row_len, block, dt, seed=1000 * n + 10 * ci + di)
@@ -156,20 +120,20 @@ def test_grid_bit_exact(torch_cuda, coll_mod, group):
                 what = f"n={n} {rows}x{row_len} block={block} {dt}->{out_dt}"
                 scale = (1.0, 0.375, 3.0)[oi]
                 ag = [c.empty(n * rows * row_len, out_dt).view(n * rows, row_len) for c in comms]
-                run_all(torch, comms, streams, lambda r, c, st: c.all_gather_block_scaled(qs[r], ss[r], ag[r], block=block, scale=scale, stream=st))
+                group.run(lambda r, c, st: c.all_gather_block_scaled(qs[r], ss[r], ag[r], block=block, scale=scale, stream=st))
                 want = ref_gather(torch, qs, ss, block, f32(scale), out_dt)
                 for r in range(n):
                     assert_same(torch, ag[r], want, f"all_gather {what} rank {r}")
                 for op, s_eff in ((coll.SUM, f32(scale)), (coll.AVG, avg_scale(scale, n))):
                     rs = [c.empty(rows // n * row_len, out_dt).view(rows // n, row_len) for c in comms]
-                    run_all(torch, comms, streams, lambda r, c, st: c.reduce_scatter_block_scaled(qs[r], ss[r], rs[r], block=block, scale=scale, op=op, stream=st))
+                    group.run(lambda r, c, st: c.reduce_scatter_block_scaled(qs[r], ss[r], rs[r], block=block, scale=scale, op=op, stream=st))
                     want = ref_reduce(torch, qs, ss, block, s_eff, out_dt)
                     for r in range(n):
                         assert_same(torch, rs[r], want[r * rows // n:(r + 1) * rows // n], f"reduce_scatter op={op} {what} rank {r}")
                     for algo in ("oneshot", "twoshot"):
                         ar = [c.empty(rows * row_len, out_dt).view(rows, row_len) for c in comms]
                         before = [c.stats()["algo_calls"][algo] for c in comms]
-                        run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.all_reduce_block_scaled(qs[r], ss[r], ar[r], block=block, scale=scale, op=op, stream=st)))
+                        group.run(lambda r, c, st: (c.set_algo(algo), c.all_reduce_block_scaled(qs[r], ss[r], ar[r], block=block, scale=scale, op=op, stream=st)))
                         for r in range(n):
                             assert_same(torch, ar[r], want, f"all_reduce {algo} op={op} {what} rank {r}")
                         assert [c.stats()["algo_calls"][algo] for c in comms] == [b + 1 for b in before]
@@ -181,14 +145,13 @@ def test_grid_bit_exact(torch_cuda, coll_mod, group):
 @pytest.mark.parametrize("group", [2, 4], indirect=True)
 def test_special_scales_and_values_propagate(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     rows, row_len, block = 96, 256, (16, 32)
     for dt in fp8_dtypes(torch):
         qs, ss = make_inputs(torch, comms, rows, row_len, block, dt, seed=77, specials=True)
         for out_dt in out_dtypes(torch):
             ag = [c.empty(n * rows * row_len, out_dt).view(n * rows, row_len) for c in comms]
-            run_all(torch, comms, streams, lambda r, c, st: c.all_gather_block_scaled(qs[r], ss[r], ag[r], block=block, scale=0.5, stream=st))
+            group.run(lambda r, c, st: c.all_gather_block_scaled(qs[r], ss[r], ag[r], block=block, scale=0.5, stream=st))
             want = ref_gather(torch, qs, ss, block, 0.5, out_dt)
             assert bool(torch.isnan(want.float()).any()) and bool(torch.isinf(want.float()).any())
             for r in range(n):
@@ -196,11 +159,11 @@ def test_special_scales_and_values_propagate(torch_cuda, coll_mod, group):
             want = ref_reduce(torch, qs, ss, block, 2.0, out_dt)
             for algo in ("oneshot", "twoshot"):
                 ar = [c.empty(rows * row_len, out_dt).view(rows, row_len) for c in comms]
-                run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.all_reduce_block_scaled(qs[r], ss[r], ar[r], block=block, scale=2.0, stream=st)))
+                group.run(lambda r, c, st: (c.set_algo(algo), c.all_reduce_block_scaled(qs[r], ss[r], ar[r], block=block, scale=2.0, stream=st)))
                 for r in range(n):
                     assert_same(torch, ar[r], want, f"all_reduce {algo} specials {dt}->{out_dt} rank {r}")
             rs = [c.empty(rows // n * row_len, out_dt).view(rows // n, row_len) for c in comms]
-            run_all(torch, comms, streams, lambda r, c, st: c.reduce_scatter_block_scaled(qs[r], ss[r], rs[r], block=block, scale=2.0, stream=st))
+            group.run(lambda r, c, st: c.reduce_scatter_block_scaled(qs[r], ss[r], rs[r], block=block, scale=2.0, stream=st))
             for r in range(n):
                 assert_same(torch, rs[r], want[r * rows // n:(r + 1) * rows // n], f"reduce_scatter specials {dt}->{out_dt} rank {r}")
     for c in comms:
@@ -210,7 +173,7 @@ def test_special_scales_and_values_propagate(torch_cuda, coll_mod, group):
 @pytest.mark.parametrize("group", [2], indirect=True)
 def test_negative_zero_becomes_positive_zero(torch_cuda, group):
     torch = torch_cuda
-    comms, streams = group
+    comms = group.comms
     rows, row_len, block = 4, 64, (1, 64)
     qs, ss = [], []
     for c in comms:
@@ -220,7 +183,7 @@ def test_negative_zero_becomes_positive_zero(torch_cuda, group):
         qs.append(q); ss.append(s)
     torch.cuda.synchronize()
     out = [c.empty(2 * rows * row_len, torch.bfloat16).view(2 * rows, row_len) for c in comms]
-    run_all(torch, comms, streams, lambda r, c, st: c.all_gather_block_scaled(qs[r], ss[r], out[r], block=block, stream=st))
+    group.run(lambda r, c, st: c.all_gather_block_scaled(qs[r], ss[r], out[r], block=block, stream=st))
     for o in out:
         assert int(o.view(torch.int16).abs().max()) == 0        # +0 only: 0 + (-0) is +0
 
@@ -228,8 +191,7 @@ def test_negative_zero_becomes_positive_zero(torch_cuda, group):
 @pytest.mark.parametrize("group", [2, 3], indirect=True)
 def test_algorithm_mapping_and_fallback(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     rows, row_len, block = 48, 256, (1, 128)
     qs, ss = make_inputs(torch, comms, rows, row_len, block, torch.float8_e4m3fn, seed=5)
     want = ref_reduce(torch, qs, ss, block, 1.0, torch.bfloat16)
@@ -237,7 +199,7 @@ def test_algorithm_mapping_and_fallback(torch_cuda, coll_mod, group):
     for forced, ran in (("ll", "oneshot"), ("ll2", "oneshot"), ("oneshot", "oneshot"), ("twoshot", "twoshot"), ("nvls", "twoshot")):
         ar = [c.empty(rows * row_len, torch.bfloat16).view(rows, row_len) for c in comms]
         before = [c.stats() for c in comms]
-        run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(forced), c.all_reduce_block_scaled(qs[r], ss[r], ar[r], block=block, stream=st)))
+        group.run(lambda r, c, st: (c.set_algo(forced), c.all_reduce_block_scaled(qs[r], ss[r], ar[r], block=block, stream=st)))
         for r, c in enumerate(comms):
             assert_same(torch, ar[r], want, f"forced {forced} rank {r}")
             s = c.stats()
@@ -248,7 +210,7 @@ def test_algorithm_mapping_and_fallback(torch_cuda, coll_mod, group):
     # two-shot writes into every rank's recv: with recv outside the arena it runs as one-shot
     outside = [torch.empty(rows, row_len, dtype=torch.bfloat16, device="cuda") for _ in comms]
     before = [c.stats()["algo_calls"] for c in comms]
-    run_all(torch, comms, streams, lambda r, c, st: (c.set_algo("twoshot"), c.all_reduce_block_scaled(qs[r], ss[r], outside[r], block=block, stream=st)))
+    group.run(lambda r, c, st: (c.set_algo("twoshot"), c.all_reduce_block_scaled(qs[r], ss[r], outside[r], block=block, stream=st)))
     for r, c in enumerate(comms):
         assert_same(torch, outside[r], want, f"two-shot outside the arena rank {r}")
         a = c.stats()["algo_calls"]
@@ -257,8 +219,8 @@ def test_algorithm_mapping_and_fallback(torch_cuda, coll_mod, group):
     before = [c.stats() for c in comms]
     ag = [c.empty(n * rows * row_len, torch.float32).view(n * rows, row_len) for c in comms]
     rs = [torch.empty(rows // n, row_len, dtype=torch.float16, device="cuda") for _ in comms]      # recv of a reduce-scatter may be anywhere
-    run_all(torch, comms, streams, lambda r, c, st: (c.set_algo("auto"), c.all_gather_block_scaled(qs[r], ss[r], ag[r], block=block, stream=st)))
-    run_all(torch, comms, streams, lambda r, c, st: c.reduce_scatter_block_scaled(qs[r], ss[r], rs[r], block=block, op=coll.AVG, stream=st))
+    group.run(lambda r, c, st: (c.set_algo("auto"), c.all_gather_block_scaled(qs[r], ss[r], ag[r], block=block, stream=st)))
+    group.run(lambda r, c, st: c.reduce_scatter_block_scaled(qs[r], ss[r], rs[r], block=block, op=coll.AVG, stream=st))
     want_rs = ref_reduce(torch, qs, ss, block, avg_scale(1.0, n), torch.float16)
     for r, c in enumerate(comms):
         assert_same(torch, ag[r], ref_gather(torch, qs, ss, block, 1.0, torch.float32), f"all_gather fp32 rank {r}")
@@ -274,7 +236,7 @@ def test_algorithm_mapping_and_fallback(torch_cuda, coll_mod, group):
         q2, s2 = make_inputs(torch, comms, nbytes_rows, 256, block, torch.float8_e5m2, seed=9)
         ar = [c.empty(nbytes_rows * 256, torch.bfloat16).view(nbytes_rows, 256) for c in comms]
         before = [c.stats()["algo_calls"] for c in comms]
-        run_all(torch, comms, streams, lambda r, c, st: c.all_reduce_block_scaled(q2[r], s2[r], ar[r], block=block, stream=st))
+        group.run(lambda r, c, st: c.all_reduce_block_scaled(q2[r], s2[r], ar[r], block=block, stream=st))
         w2 = ref_reduce(torch, q2, s2, block, 1.0, torch.bfloat16)
         for r, c in enumerate(comms):
             assert_same(torch, ar[r], w2, f"auto rows={nbytes_rows} rank {r}")
@@ -285,8 +247,8 @@ def test_algorithm_mapping_and_fallback(torch_cuda, coll_mod, group):
 
 def test_one_rank_is_a_dequantising_copy(torch_cuda, coll_mod):
     torch, coll = torch_cuda, coll_mod
-    (c,) = coll.Comm.init_all([0], arena_mb=96)
-    try:
+    with Group(torch, coll, 1, arena_mb=96) as g:
+        c = g.comms[0]
         for rows, row_len, block in CASES:
             for dt in fp8_dtypes(torch):
                 qs, ss = make_inputs(torch, [c], rows, row_len, block, dt, seed=rows + row_len)
@@ -310,16 +272,12 @@ def test_one_rank_is_a_dequantising_copy(torch_cuda, coll_mod):
                     for op in (coll.OP_ALLREDUCE, coll.OP_ALLGATHER, coll.OP_REDUCESCATTER):
                         assert s["calls"][op] == before["calls"][op] + 1
         c.check_async_error()
-    finally:
-        torch.cuda.synchronize()
-        c.destroy()
 
 
 @pytest.mark.parametrize("group", [2, 3], indirect=True)
 def test_cuda_graph_capture_and_replay(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     rows, row_len, block = 72, 384, (128, 128)
     qs, ss = make_inputs(torch, comms, rows, row_len, block, torch.float8_e4m3fn, seed=3)
     ag = [c.empty(n * rows * row_len, torch.bfloat16).view(n * rows, row_len) for c in comms]
@@ -329,13 +287,13 @@ def test_cuda_graph_capture_and_replay(torch_cuda, coll_mod, group):
     graphs = []
     for r, c in enumerate(comms):
         g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g, stream=streams[r]):
-            c.all_gather_block_scaled(qs[r], ss[r], ag[r], block=block, scale=0.5, stream=streams[r])
-            c.reduce_scatter_block_scaled(qs[r], ss[r], rs[r], block=block, op=coll.AVG, stream=streams[r])
+        with torch.cuda.graph(g, stream=group.streams[r]):
+            c.all_gather_block_scaled(qs[r], ss[r], ag[r], block=block, scale=0.5, stream=group.streams[r])
+            c.reduce_scatter_block_scaled(qs[r], ss[r], rs[r], block=block, op=coll.AVG, stream=group.streams[r])
             c.set_algo("oneshot")
-            c.all_reduce_block_scaled(qs[r], ss[r], ar1[r], block=block, stream=streams[r])
+            c.all_reduce_block_scaled(qs[r], ss[r], ar1[r], block=block, stream=group.streams[r])
             c.set_algo("twoshot")
-            c.all_reduce_block_scaled(qs[r], ss[r], ar2[r], block=block, scale=4.0, stream=streams[r])
+            c.all_reduce_block_scaled(qs[r], ss[r], ar2[r], block=block, scale=4.0, stream=group.streams[r])
             c.set_algo("auto")
         graphs.append(g)
     for it in range(3):
@@ -344,7 +302,7 @@ def test_cuda_graph_capture_and_replay(torch_cuda, coll_mod, group):
             ss[r].mul_(2.0 if it % 2 else 0.5)
         torch.cuda.synchronize()
         for r, g in enumerate(graphs):
-            with torch.cuda.stream(streams[r]):
+            with torch.cuda.stream(group.streams[r]):
                 g.replay()
         torch.cuda.synchronize()
         for c in comms:
@@ -370,8 +328,7 @@ def _raw(coll, c, fn, q, s, out, count, row_len, br, bc, in_dt, out_dt, *extra):
 @pytest.mark.parametrize("group", [2], indirect=True)
 def test_error_codes(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, _ = group
-    c = comms[0]
+    c = group.comms[0]
     L = coll.load()
     rows, row_len = 32, 128
     q = c.empty(rows * row_len, torch.float8_e4m3fn)
@@ -401,12 +358,9 @@ def test_error_codes(torch_cuda, coll_mod, group):
         ("FP8 output", AG, q, s, n_, row_len, 1, 128, E4, E5, (), INVALID_ARGUMENT),
     ]
     for what, fn, qq, ss, count, rl, br, bc, i, o, extra, code in cases:
-        rc = _raw(coll, c, fn, qq, ss, out, count, rl, br, bc, i, o, *extra)
-        assert rc == code, (what, rc, L.b200collGetLastError().decode())
-        assert L.b200collGetLastError().decode(), what
+        expect_refused(_raw(coll, c, fn, qq, ss, out, count, rl, br, bc, i, o, *extra), code, what=what)
     # recv overlapping send
-    rc = _raw(coll, c, AR, q, s, q, n_ // 2, row_len, 1, 128, E4, BF, coll.SUM)
-    assert rc == INVALID_ARGUMENT and "overlap" in L.b200collGetLastError().decode()
+    expect_refused(_raw(coll, c, AR, q, s, q, n_ // 2, row_len, 1, 128, E4, BF, coll.SUM), INVALID_ARGUMENT, "overlap")
     # Python-level mistakes raise ValueError before the library is called; library refusals raise B200CollError
     with pytest.raises(ValueError):
         c.all_gather_block_scaled(q.view(rows, row_len), s.view(rows // 2, 2), out.view(2 * rows, row_len))     # scales of the wrong shape
@@ -417,21 +371,19 @@ def test_error_codes(torch_cuda, coll_mod, group):
         c.all_reduce_block_scaled(q.view(rows, row_len), s.view(rows, 1), out[:n_].view(rows, row_len), block=(1, 128), op=coll.MAX)
     assert e.value.code == INVALID_ARGUMENT
     # nothing was launched, nothing was counted, and the communicator still works
-    assert all(x == 0 for x in c.stats()["calls"])
-    for comm in comms:
-        comm.check_async_error()
+    assert_nothing_launched(c)
+    group.check_async()
 
 
 @pytest.mark.parametrize("op", ["all_gather", "reduce_scatter", "all_reduce"])
 @pytest.mark.parametrize("dtypes", [("e4m3", "bfloat16", "1x128"), ("e5m2", "float", "128x128"), ("e4m3", "half", "32x64")])
 def test_perf_tool_block_scaled_bit_exact(torch_cuda, coll_lib, op, dtypes):
     dt, out, block = dtypes
-    r = subprocess.run([PERF, "--devs", "0,0", "--op", op, "-d", dt, "--out-dtype", out, "--block-scale", block, "--row-len", "1024",
-                        "-b", "64K", "-e", "1M", "-f", "16", "-w", "1", "-n", "2", "-c", "1"], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-    assert "errors=0" in r.stdout and "block-scaled: row_len=1024" in r.stdout, r.stdout[-2000:]
-    rows = [l for l in r.stdout.splitlines() if l.strip() and not l.startswith("#")]
-    assert len(rows) == 2, r.stdout                                     # 64 KiB and 1 MiB
+    stdout = run_perf(["--op", op, "-d", dt, "--out-dtype", out, "--block-scale", block, "--row-len", "1024", "-b", "64K", "-e", "1M", "-f", "16",
+                       "-w", "1", "-n", "2", "-c", "1"], "0,0")
+    assert "block-scaled: row_len=1024" in stdout, stdout[-2000:]
+    rows = [l for l in stdout.splitlines() if l.strip() and not l.startswith("#")]
+    assert len(rows) == 2, stdout                                         # 64 KiB and 1 MiB
 
 
 def test_multi_gpu_block_scaled(torch_cuda, coll_mod):
@@ -439,8 +391,8 @@ def test_multi_gpu_block_scaled(torch_cuda, coll_mod):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
     n = torch.cuda.device_count()
-    comms = coll.Comm.init_all(list(range(n)), arena_mb=256)
-    try:
+    with Group(torch, coll, n, devices=list(range(n)), arena_mb=256) as g:
+        comms = g.comms
         rows, row_len, block = 24 * 64, 2048, (1, 128)
         qs, ss, ag, ar = [], [], [], []
         for r, c in enumerate(comms):
@@ -469,8 +421,3 @@ def test_multi_gpu_block_scaled(torch_cuda, coll_mod):
                 c.check_async_error()
                 assert_same(torch, ag[r].to("cuda:0"), w_ag, f"multi-GPU all_gather rank {r}")
                 assert_same(torch, ar[r].to("cuda:0"), w_ar, f"multi-GPU all_reduce {algo} rank {r}")
-    finally:
-        for r in range(n):
-            torch.cuda.synchronize(r)
-        for c in comms:
-            c.destroy()

@@ -3,73 +3,23 @@
 Bit-exact means equal (NaN matching NaN at the same position) to tests/coll_combine_reference.combine over the dequantised rows
 tests/coll_quant_reference.quantize(row)[2] of every rank's expert_out: each rank quantises its whole expert_out by the per-block rule, and
 each slot's row is summed in slot order exactly as the wide combine of the same map sums it."""
-import os
-import subprocess
-import sys
-
 import ctypes as C
 import numpy as np
 import pytest
 
+from container_engine_accelerators_b200.ops.coll import INVALID_ARGUMENT, OUT_OF_MEMORY
 from tests import coll_combine_reference as cr
 from tests import coll_quant_reference as qr
 from tests import coll_routed_reference as rr
 from tests.coll_fp_reference import assert_same
-from tests.test_coll_a2a_combine_gpu import Plan
-from tests.test_coll_expert_routed_gpu import route_lookup, routing
+from tests.coll_gpu_harness import (DTYPES, Group, Plan, assert_nothing_launched, coll_mod, expect_refused, run_perf, run_python,  # noqa: F401
+                                    torch_cuda)
+from tests.coll_routed_reference import route_lookup, routing
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PERF = os.path.join(ROOT, "build", "b200coll_perf")
-INVALID_ARGUMENT, OUT_OF_MEMORY = 4, 8
 ROW = 512                                                               # whole blocks of every size tested
 PAIRS = [(i, o) for i in ("bf16", "f16", "f32") for o in ("bf16", "f16", "f32")]
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch
-
-
-@pytest.fixture(scope="module")
-def coll_mod(coll_lib):
-    from container_engine_accelerators_b200.ops import coll
-    coll.load()
-    return coll
-
-
-def _dt(torch, name):
-    return {"bf16": torch.bfloat16, "f16": torch.float16, "f32": torch.float32, "e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}[name]
-
-
-class Group:
-    def __init__(self, torch, coll, n, devices=None, arena_mb=64):
-        self.torch, self.coll, self.n = torch, coll, n
-        self.comms = coll.Comm.init_all(devices if devices is not None else [0] * n, arena_mb=arena_mb)
-        self.streams = []
-        for c in self.comms:
-            with torch.cuda.device(c.device):
-                self.streams.append(torch.cuda.Stream())
-
-    def sync(self):
-        for d in {c.device for c in self.comms}:
-            self.torch.cuda.synchronize(d)
-
-    def destroy(self):
-        self.sync()
-        for c in self.comms:
-            c.destroy()
-
-    def dev(self, c, a):
-        return self.torch.from_numpy(np.ascontiguousarray(a)).to(f"cuda:{c.device}")
-
-    def check_async(self):
-        for c in self.comms:
-            c.check_async_error()
 
 
 def segment_plan(topk, E, tight, seed):
@@ -155,9 +105,8 @@ def test_combine_bit_exact(torch_cuda, coll_mod, n, kind):
     expert twice, an empty rank) x ample and tight capacity, weights given and None, scale != 1, the 9 (in, out) pairs in turn; inputs
     with specials; rows no slot reads hold NaN and inf; two launches, the algorithm and the bytes of the wide combine."""
     torch, coll = torch_cuda, coll_mod
-    g = Group(torch, coll, n)
-    case = 0
-    try:
+    with Group(torch, coll, n) as g:
+        case = 0
         for block, (epr, k) in CONFIGS.items():
             E = epr * n
             for rkind in ("uniform", "zipf", "one", "mixed"):
@@ -182,7 +131,7 @@ def test_combine_bit_exact(torch_cuda, coll_mod, n, kind):
                         with_w = case % 2 == 0
                         scale = 1.0 if with_w else 0.75
                         case += 1
-                        in_dt, out_dt, wire = _dt(torch, in_name), _dt(torch, out_name), _dt(torch, wire_name)
+                        in_dt, out_dt, wire = DTYPES[in_name], DTYPES[out_name], DTYPES[wire_name]
                         eo = expert_outs(torch, n, recv_rows, in_dt, block, seed=case, used=used)
                         deq = dequantised(torch, eo, block, wire)
                         w = wts if with_w else None
@@ -203,8 +152,6 @@ def test_combine_bit_exact(torch_cuda, coll_mod, n, kind):
                             assert st["calls"][coll.OP_ALLTOALL] == b["calls"][coll.OP_ALLTOALL] + 1, what
                             nbytes = (int(maps.rows[r].sum()) if kind == "segment" else ix.size) * ROW * in_dt.itemsize
                             assert st["bytes"][coll.OP_ALLTOALL] == b["bytes"][coll.OP_ALLTOALL] + nbytes, what
-    finally:
-        g.destroy()
 
 
 def test_rank_count_makes_no_difference(torch_cuda, coll_mod):
@@ -219,8 +166,7 @@ def test_rank_count_makes_no_difference(torch_cuda, coll_mod):
     w = rng.uniform(-2, 2, size=(tokens, k)).astype(np.float32)
     results = {}
     for n in (1, 4):
-        g = Group(torch, coll, n)
-        try:
+        with Group(torch, coll, n) as g:
             recv_rows = 4 * R // n
             eo = [rows_g[r * recv_rows:(r + 1) * recv_rows].cuda() for r in range(n)]
             route = np.where(gidx >= 0, (gidx // recv_rows) * recv_rows + gidx % recv_rows, -1).astype(np.int32)
@@ -233,8 +179,6 @@ def test_rank_count_makes_no_difference(torch_cuda, coll_mod):
             g.sync()
             g.check_async()
             results[n] = outs[0].cpu()
-        finally:
-            g.destroy()
     assert torch.equal(results[1].view(torch.int32), results[4].view(torch.int32))
     deq = dequantised(torch, [rows_g], block, wire)
     assert_same(results[1], cr.combine(route_lookup(deq, 4 * R), gidx, w, 0.5, torch.float32), "one rank vs the reference")
@@ -246,11 +190,10 @@ def test_cuda_graph_dispatch_expert_combine(torch_cuda, coll_mod, n):
     expert_combine_quantized over the dispatch's route in one CUDA graph, at a size the scratch already holds; topk_idx is rewritten in
     place between replays and every replay is checked."""
     torch, coll = torch_cuda, coll_mod
-    g = Group(torch, coll, n)
-    rng = np.random.default_rng(60 + n)
-    block, wire = 128, torch.float8_e4m3fn
-    nb = ROW // block
-    try:
+    with Group(torch, coll, n) as g:
+        rng = np.random.default_rng(60 + n)
+        block, wire = 128, torch.float8_e4m3fn
+        nb = ROW // block
         E, k, tokens = 4 * n, 2, 24
         recv_rows = tokens * k * 3 // 4
         xs = [qr.gen(tokens * ROW, torch.bfloat16, block, 9 + s, specials=False).view(tokens, ROW) for s in range(n)]
@@ -300,8 +243,6 @@ def test_cuda_graph_dispatch_expert_combine(torch_cuda, coll_mod, n):
                 want = cr.combine(route_lookup(deq, recv_rows), lay.route[r], w[r], 1.0, torch.float32)
                 assert_same(outs[r].cpu(), want, f"replay {rep} ({rkind}): combine rank {r}")
         del graphs
-    finally:
-        g.destroy()
 
 
 def test_shared_scratch_with_quantised_all_reduce(torch_cuda, coll_mod):
@@ -309,9 +250,8 @@ def test_shared_scratch_with_quantised_all_reduce(torch_cuda, coll_mod):
     scratch grow between calls; every result is exact. A graph of a combine captured before the growth still replays exactly."""
     torch, coll = torch_cuda, coll_mod
     n, block, wire = 2, 32, torch.float8_e5m2
-    g = Group(torch, coll, n)
-    rng = np.random.default_rng(3)
-    try:
+    with Group(torch, coll, n) as g:
+        rng = np.random.default_rng(3)
         def combine_case(recv_rows, tokens, k, seed):
             eo = [qr.gen(recv_rows * ROW, torch.float16, block, seed + r).view(recv_rows, ROW) for r in range(n)]
             routes = [rng.integers(-2, n * recv_rows + 2, size=(tokens, k)).astype(np.int32) for _ in range(n)]
@@ -375,8 +315,6 @@ def test_shared_scratch_with_quantised_all_reduce(torch_cuda, coll_mod):
         for r in range(n):
             assert_same(small[3][r].cpu(), small_want[r], f"graph captured before the growth, rank {r}")
         del graphs
-    finally:
-        g.destroy()
 
 
 def _raw_a2av(coll, comm, a):
@@ -399,9 +337,7 @@ def test_refusals_launch_nothing(torch_cuda, coll_mod):
     """Every refusal of both calls, each breaking one rule, returns its code and message and launches nothing: the stats stay at zero.
     OutOfMemory comes from a scratch the arena cannot hold."""
     torch, coll = torch_cuda, coll_mod
-    L = coll.load()
-    g = Group(torch, coll, 2, arena_mb=8)
-    try:
+    with Group(torch, coll, 2, arena_mb=8) as g:
         c = g.comms[0]
         row, block, rows_n, tokens, k = 128, 32, 16, 4, 2
         eo = torch.empty(rows_n * row, dtype=torch.bfloat16, device="cuda")
@@ -438,24 +374,15 @@ def test_refusals_launch_nothing(torch_cuda, coll_mod):
             ("expert scratch larger than the arena", _raw_expert, dict(base, eo=big.data_ptr(), row_elems=512, recv_rows=65536), OUT_OF_MEMORY, "cannot hold"),
         ]
         for what, fn, args, want, msg in cases:
-            rc = fn(coll, c, args)
-            err = L.b200collGetLastError().decode()
-            assert rc == want, (what, rc, err)
-            assert msg in err, (what, err)
-            assert err.startswith("quantised expert combine: " if fn is _raw_expert else "quantised all-to-all-v combine: "), (what, err)
+            expect_refused(fn(coll, c, args), want, msg, "quantised expert combine: " if fn is _raw_expert else "quantised all-to-all-v combine: ", what)
         with pytest.raises(ValueError):
             c.expert_combine_quantized(eo.view(-1, row), torch.zeros(tokens, k, dtype=torch.int32, device="cuda"), None,
                                        out[:tokens * row].view(tokens, row), block=256)
-        st = c.stats()
-        assert st["kernel_launches"] == 0 and all(v == 0 for v in st["calls"]) and all(v == 0 for v in st["bytes"])
+        assert_nothing_launched(c)
         g.check_async()
-    finally:
-        g.destroy()
 
 
 _LAZY = r'''
-import sys
-sys.path.insert(0, sys.argv[1])
 import numpy as np
 import torch
 from container_engine_accelerators_b200.ops import coll
@@ -514,17 +441,13 @@ def test_lazy_module_loading_dispatch_then_combine(torch_cuda, coll_lib):
     """A fresh process with lazy module loading and a short watchdog drives two virtual ranks from one thread, enqueueing per rank the
     FP8 routed dispatch and the quantising combine back to back: the first launch of the combine's kernels must not wait behind the
     rank's own layout kernel, which waits for the other rank's call. Both results must be exact."""
-    env = {**os.environ, "CUDA_MODULE_LOADING": "LAZY", "B200COLL_TIMEOUT_MS": "10000"}
-    r = subprocess.run([sys.executable, "-c", _LAZY, ROOT], cwd=ROOT, env=env, capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0 and "lazy ok" in r.stdout, r.stdout[-2000:] + r.stderr[-3000:]
+    run_python(_LAZY, {"CUDA_MODULE_LOADING": "LAZY", "B200COLL_TIMEOUT_MS": "10000"}, "lazy ok")
 
 
 def _perf(devs, procs, extra, header):
-    r = subprocess.run([PERF, "--devs", devs, *(["--procs"] if procs else []), "--op", "alltoall", *extra, "-w", "1", "-n", "2", "-c", "1"],
-                       capture_output=True, text=True, timeout=600, env={**os.environ, "B200COLL_TIMEOUT_MS": "20000"})
-    assert r.returncode == 0 and "errors=0" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
-    assert header in r.stdout, r.stdout
-    assert [l for l in r.stdout.splitlines() if l.strip() and not l.startswith("#")], r.stdout
+    out = run_perf(["--op", "alltoall", *extra, "-w", "1", "-n", "2", "-c", "1"], devs, procs, env={"B200COLL_TIMEOUT_MS": "20000"})
+    assert header in out, out
+    assert [l for l in out.splitlines() if l.strip() and not l.startswith("#")], out
 
 
 def test_perf_tool_quantising_combine_modes(torch_cuda, coll_lib):
@@ -553,8 +476,7 @@ def test_one_process_on_two_gpus(torch_cuda, coll_mod):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
     n, E, k, block = 2, 8, 4, 128
-    g = Group(torch, coll, n, devices=[0, 1])
-    try:
+    with Group(torch, coll, n, devices=[0, 1]) as g:
         topk = routing("zipf", n, E, k, seed=3, tokens=[300, 200])
         recv_rows = max(int(c.sum()) for c in rr.layout(topk, E, 1 << 20).counts) * 4 // 5
         lay = rr.layout(topk, E, recv_rows)
@@ -565,5 +487,3 @@ def test_one_process_on_two_gpus(torch_cuda, coll_mod):
         deq = dequantised(torch, eo, block, torch.float8_e4m3fn)
         for r in range(n):
             assert_same(outs[r], cr.combine(route_lookup(deq, recv_rows), lay.route[r], w[r], 1.0, torch.bfloat16), f"two GPUs rank {r}")
-    finally:
-        g.destroy()

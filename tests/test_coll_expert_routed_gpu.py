@@ -4,70 +4,21 @@ Every recv starts poisoned with 0x5A; stored rows are compared byte for byte wit
 -0 included), every other row must keep the poison, and expert_counts, route and dropped must match exactly. Combine outputs are
 compared bit for bit with tests/coll_combine_reference.combine through a route lookup."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from container_engine_accelerators_b200.ops.coll import INVALID_ARGUMENT, INVALID_USAGE
 from tests import coll_combine_reference as cr
 from tests import coll_quant_reference as qr
 from tests import coll_routed_reference as rr
 from tests.coll_fp_reference import assert_same
+from tests.coll_gpu_harness import DTYPES, Group, assert_nothing_launched, coll_mod, expect_refused, run_perf, torch_cuda  # noqa: F401
+from tests.coll_routed_reference import INT32_MAX, INT32_MIN, route_lookup, routing
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PERF = os.path.join(ROOT, "build", "b200coll_perf")
-INVALID_ARGUMENT, INVALID_USAGE = 4, 5
-INT32_MIN, INT32_MAX = -2 ** 31, 2 ** 31 - 1
 ROW = 48
 POISON = 0x5A
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch
-
-
-@pytest.fixture(scope="module")
-def coll_mod(coll_lib):
-    from container_engine_accelerators_b200.ops import coll
-    coll.load()
-    return coll
-
-
-def _dt(torch, name):
-    return {"bf16": torch.bfloat16, "f16": torch.float16, "f32": torch.float32}[name]
-
-
-def routing(kind, n, E, k, seed, tokens=None):
-    """One [tokens, top_k] int32 array per rank. uniform; zipf (expert_dispatch_plan's skewed draw); one (every slot to one expert);
-    mixed: uniform with every kind of invalid id, a token naming one expert twice, and (n > 1) a last rank with no tokens."""
-    rng = np.random.default_rng(seed)
-    tokens = tokens or [17 + 5 * s for s in range(n)]
-    if kind == "zipf":
-        from container_engine_accelerators_b200.models.workloads import expert_dispatch_plan
-        p = expert_dispatch_plan(n, max(tokens), 16, experts_per_rank=E // n, top_k=k, skew=1.2, seed=seed)
-        return [p.experts[s][:tokens[s]] for s in range(n)]
-    if kind == "one":
-        return [np.full((tokens[s], k), (seed * 7) % E, dtype=np.int32) for s in range(n)]
-    out = [rng.integers(0, E, size=(tokens[s], k)).astype(np.int64) for s in range(n)]
-    if kind == "mixed":
-        bad = [-1, -2, E, E + 3, INT32_MIN, INT32_MAX]
-        for s in range(n):
-            ids = out[s]
-            pos = rng.choice(ids.size, size=min(ids.size, len(bad)), replace=False)
-            for i, p in enumerate(pos):
-                ids.flat[p] = bad[i]
-            if k >= 2:
-                ids[1, 0] = ids[1, 1] = s % E                           # the same expert twice
-        if n > 1:
-            out[-1] = np.zeros((0, k), dtype=np.int64)
-    return [o.astype(np.int32) for o in out]
 
 
 def _x_bytes(rng, tokens, row_bytes, esize):
@@ -81,44 +32,19 @@ def _x_bytes(rng, tokens, row_bytes, esize):
     return x
 
 
-class Group:
-    def __init__(self, torch, coll, n, arena_mb=64, devices=None):
-        self.torch, self.coll, self.n = torch, coll, n
-        self.comms = coll.Comm.init_all(devices if devices is not None else [0] * n, arena_mb=arena_mb)
-        self.streams = []
-        for c in self.comms:
-            with torch.cuda.device(c.device):
-                self.streams.append(torch.cuda.Stream())
+def dev_rows(g, c, a, dt):
+    """[tokens, row bytes] uint8 rows on c's device, viewed as dt (also for tokens == 0)."""
+    t = g.torch.empty(a.shape, dtype=g.torch.uint8, device=f"cuda:{c.device}")
+    if a.size:
+        t.copy_(g.torch.from_numpy(np.ascontiguousarray(a)))
+    return t.view(dt)
 
-    def sync(self):
-        for d in {c.device for c in self.comms}:
-            self.torch.cuda.synchronize(d)
 
-    def destroy(self):
-        self.sync()
-        for c in self.comms:
-            c.destroy()
-
-    def dev(self, c, a):
-        return self.torch.from_numpy(np.ascontiguousarray(a)).to(f"cuda:{c.device}")
-
-    def dev_rows(self, c, a, dt):
-        """[tokens, row bytes] uint8 rows on c's device, viewed as dt (also for tokens == 0)."""
-        t = self.torch.empty(a.shape, dtype=self.torch.uint8, device=f"cuda:{c.device}")
-        if a.size:
-            t.copy_(self.torch.from_numpy(np.ascontiguousarray(a)))
-        return t.view(dt)
-
-    def recv_bufs(self, recv_rows, dt):
-        torch = self.torch
-        bufs = [c.empty(recv_rows * ROW, dt) for c in self.comms]
-        for b in bufs:
-            b.view(torch.uint8).fill_(POISON)
-        return bufs
-
-    def check_async(self):
-        for c in self.comms:
-            c.check_async_error()
+def recv_bufs(g, recv_rows, dt):
+    bufs = [c.empty(recv_rows * ROW, dt) for c in g.comms]
+    for b in bufs:
+        b.view(g.torch.uint8).fill_(POISON)
+    return bufs
 
 
 def small_outputs(g, topk, E):
@@ -132,7 +58,7 @@ def small_outputs(g, topk, E):
 def run_dispatch(g, xs_np, topk, E, recv, dt):
     """Dispatch on every rank's stream; returns the CPU copies of (recv bytes, counts, route, dropped) per rank."""
     torch = g.torch
-    xd = [g.dev_rows(c, xs_np[r], dt) for r, c in enumerate(g.comms)]
+    xd = [dev_rows(g, c, xs_np[r], dt) for r, c in enumerate(g.comms)]
     idx = [g.dev(c, topk[r]) for r, c in enumerate(g.comms)]
     small = small_outputs(g, topk, E)
     g.sync()
@@ -169,12 +95,11 @@ def test_dispatch_bit_exact(torch_cuda, coll_mod, n, dt_name):
     """(E, top_k) in (N, 1), (4N, 2), (8N, 8) (and 256 experts top-8 at 8 ranks) x uniform, Zipf, one-expert and mixed routings x ample
     and tight capacity; two launches per call and the stats under alltoall."""
     torch, coll = torch_cuda, coll_mod
-    dt = _dt(torch, dt_name)
+    dt = DTYPES[dt_name]
     es = dt.itemsize
-    g = Group(torch, coll, n)
-    rng = np.random.default_rng(n * 100 + es)
-    clipped_inside = 0
-    try:
+    with Group(torch, coll, n) as g:
+        rng = np.random.default_rng(n * 100 + es)
+        clipped_inside = 0
         for E, k in _configs(n):
             for kind in ("uniform", "zipf", "one", "mixed"):
                 topk = routing(kind, n, E, k, seed=E + k + n)
@@ -185,7 +110,7 @@ def test_dispatch_bit_exact(torch_cuda, coll_mod, n, dt_name):
                     totals = rr.layout(topk, E, 1 << 20).counts
                     clipped_inside += sum(int(((lay.counts[d] > 0) & (lay.counts[d] < totals[d])).sum()) for d in range(n))
                     xs = [_x_bytes(rng, t.shape[0], ROW * es, es) for t in topk]
-                    recv = g.recv_bufs(recv_rows, dt)
+                    recv = recv_bufs(g, recv_rows, dt)
                     before = [c.stats() for c in g.comms]
                     got = run_dispatch(g, xs, topk, E, recv, dt)
                     what = f"n={n} {dt_name} E={E} top_k={k} {kind} {cap_name}"
@@ -200,22 +125,6 @@ def test_dispatch_bit_exact(torch_cuda, coll_mod, n, dt_name):
                     for c, b in zip(g.comms, recv):
                         c.release(b)
         assert clipped_inside > 0                                      # some receiver stored part of an expert
-    finally:
-        g.destroy()
-
-
-def route_lookup(eo, recv_rows):
-    """cr.combine's lookup for routes: route in [0, nranks * recv_rows) names row route % recv_rows of rank route // recv_rows."""
-    n = len(eo)
-
-    def f(col):
-        col = np.asarray(col, dtype=np.int64)
-        valid = (col >= 0) & (col < n * recv_rows)
-        y = np.zeros((col.size, eo[0].shape[1]), dtype=np.float32)
-        for i in np.nonzero(valid)[0]:
-            y[i] = eo[col[i] // recv_rows][col[i] % recv_rows]
-        return valid, y
-    return f
 
 
 def _spoil(route, n, recv_rows, rng):
@@ -232,13 +141,12 @@ def test_combine_bit_exact(torch_cuda, coll_mod, n):
     """Every type pair, with weights and without, on routes from a dispatch and on spoiled routes (-1, INT32_MIN, INT32_MAX,
     nranks * recv_rows); one launch per call, the stats under alltoall."""
     torch, coll = torch_cuda, coll_mod
-    g = Group(torch, coll, n)
-    rng = np.random.default_rng(n)
-    try:
+    with Group(torch, coll, n) as g:
+        rng = np.random.default_rng(n)
         E, k = 4 * n, 3
         topk = routing("mixed", n, E, k, seed=5)
         recv_rows = max(1, max(int(c.sum()) for c in rr.layout(topk, E, 1 << 20).counts) * 4 // 5)
-        recv = g.recv_bufs(recv_rows, torch.bfloat16)
+        recv = recv_bufs(g, recv_rows, torch.bfloat16)
         xs = [_x_bytes(rng, t.shape[0], ROW * 2, 2) for t in topk]
         got = run_dispatch(g, xs, topk, E, recv, torch.bfloat16)
         routes = [o[2] for o in got]
@@ -247,7 +155,7 @@ def test_combine_bit_exact(torch_cuda, coll_mod, n):
         for c, b in zip(g.comms, recv):
             c.release(b)
         for in_name in ("bf16", "f16", "f32"):
-            in_dt = _dt(torch, in_name)
+            in_dt = DTYPES[in_name]
             xs_eo = [qr.gen(recv_rows * ROW, in_dt, 16, 31 * r + 7) for r in range(n)]
             eo = []
             for c, x in zip(g.comms, xs_eo):
@@ -256,7 +164,7 @@ def test_combine_bit_exact(torch_cuda, coll_mod, n):
                 eo.append(d)
             eo_np = [x.float().numpy().reshape(-1, ROW) for x in xs_eo]
             for out_name in ("bf16", "f16", "f32"):
-                out_dt = _dt(torch, out_name)
+                out_dt = DTYPES[out_name]
                 for spoiled in (False, True):
                     rts = [_spoil(rt, n, recv_rows, rng) if spoiled else rt for rt in routes]
                     for weights, scale in ((True, 1.0), (False, 0.75)):
@@ -281,8 +189,6 @@ def test_combine_bit_exact(torch_cuda, coll_mod, n):
                             assert st["bytes"][coll.OP_ALLTOALL] == b["bytes"][coll.OP_ALLTOALL] + rts[r].size * ROW * in_dt.itemsize, what
             for c, d in zip(g.comms, eo):
                 c.release(d)
-    finally:
-        g.destroy()
 
 
 @pytest.mark.parametrize("n", [2, 3])
@@ -290,15 +196,14 @@ def test_cuda_graph_without_host_sync(torch_cuda, coll_mod, n):
     """Each rank captures dispatch then combine (recv as the expert output) in one CUDA graph; topk_idx is rewritten in place between
     replays so counts, clipping and routes change, and every replay is checked."""
     torch, coll = torch_cuda, coll_mod
-    g = Group(torch, coll, n)
-    rng = np.random.default_rng(40 + n)
-    try:
+    with Group(torch, coll, n) as g:
+        rng = np.random.default_rng(40 + n)
         E, k, tokens = 4 * n, 2, 24
         recv_rows = tokens * k * 3 // 4
-        recv = g.recv_bufs(recv_rows, torch.bfloat16)
+        recv = recv_bufs(g, recv_rows, torch.bfloat16)
         xs = [_x_bytes(rng, tokens, ROW * 2, 2) for _ in range(n)]
         xs[0][:, :] = (np.arange(ROW * 2) % 7).astype(np.uint8)          # finite values too, so the sums are not all NaN
-        xd = [g.dev_rows(c, xs[r], torch.bfloat16) for r, c in enumerate(g.comms)]
+        xd = [dev_rows(g, c, xs[r], torch.bfloat16) for r, c in enumerate(g.comms)]
         idx = [torch.zeros(tokens, k, dtype=torch.int32, device="cuda") for _ in range(n)]
         w = [rng.uniform(0.1, 1.0, size=(tokens, k)).astype(np.float32) for _ in range(n)]
         wd = [g.dev(c, w[r]) for r, c in enumerate(g.comms)]
@@ -336,8 +241,6 @@ def test_cuda_graph_without_host_sync(torch_cuda, coll_mod, n):
                 want = cr.combine(route_lookup(eo, recv_rows), lay.route[r], w[r], 1.0, torch.float32)
                 assert_same(outs[r].cpu(), want, f"replay {rep} ({kind}): combine rank {r}")
         del graphs
-    finally:
-        g.destroy()
 
 
 def test_interleaved_with_other_collectives(torch_cuda, coll_mod):
@@ -345,15 +248,14 @@ def test_interleaved_with_other_collectives(torch_cuda, coll_mod):
     count mailbox stay in step with the other collectives."""
     torch, coll = torch_cuda, coll_mod
     n, E, k, tokens = 4, 16, 2, 40
-    g = Group(torch, coll, n)
-    rng = np.random.default_rng(3)
-    try:
+    with Group(torch, coll, n) as g:
+        rng = np.random.default_rng(3)
         t1, t2 = routing("zipf", n, E, k, seed=1, tokens=[tokens] * n), routing("uniform", n, E, k, seed=2, tokens=[tokens] * n)
         recv_rows = tokens * k
-        r1, r2 = g.recv_bufs(recv_rows, torch.float32), g.recv_bufs(recv_rows, torch.float32)
+        r1, r2 = recv_bufs(g, recv_rows, torch.float32), recv_bufs(g, recv_rows, torch.float32)
         xs = [_x_bytes(rng, tokens, ROW * 4, 4) for _ in range(n)]
         xs[0][:, 8:] = 0
-        xd = [g.dev_rows(c, xs[r], torch.float32) for r, c in enumerate(g.comms)]
+        xd = [dev_rows(g, c, xs[r], torch.float32) for r, c in enumerate(g.comms)]
         i1 = [g.dev(c, t1[r]) for r, c in enumerate(g.comms)]
         i2 = [g.dev(c, t2[r]) for r, c in enumerate(g.comms)]
         ar = [c.empty(4096, torch.float32) for c in g.comms]
@@ -390,8 +292,6 @@ def test_interleaved_with_other_collectives(torch_cuda, coll_mod):
                 lo, cnt = int(p.recv_off[r, s]), int(p.rows[s, r])
                 want = sends[s][int(p.send_off[s, r]) * ROW:(int(p.send_off[s, r]) + cnt) * ROW]
                 assert torch.equal(a2a[r][lo * ROW:(lo + cnt) * ROW], want)
-    finally:
-        g.destroy()
 
 
 def _raw_dispatch(coll, comm, **a):
@@ -409,9 +309,7 @@ def _raw_combine(coll, comm, **a):
 
 def test_refusals_launch_nothing(torch_cuda, coll_mod):
     torch, coll = torch_cuda, coll_mod
-    L = coll.load()
-    g = Group(torch, coll, 2)
-    try:
+    with Group(torch, coll, 2) as g:
         c = g.comms[0]
         row, rows_n, tokens, k = 64, 16, 4, 2
         recv = c.empty(rows_n * row, torch.bfloat16)
@@ -440,10 +338,7 @@ def test_refusals_launch_nothing(torch_cuda, coll_mod):
             ("more than 2^31 - 1 vectors", dict(tokens=1 << 24, top_k=8, row_elems=512), "16-byte vectors"),  # 2^27 slots x 64 vectors
         ]]
         for what, want, kw, msg in cases:
-            rc = _raw_dispatch(coll, c, **dict(ok, **kw))
-            err = L.b200collGetLastError().decode()
-            assert rc == want, (what, rc, err)
-            assert msg in err, (what, err)
+            expect_refused(_raw_dispatch(coll, c, **dict(ok, **kw)), want, msg, what=what)
         eo = c.empty(rows_n * row, torch.bfloat16)
         out = torch.empty(tokens, row, dtype=torch.bfloat16, device="cuda")
         wts = torch.ones(tokens, k, device="cuda")
@@ -461,26 +356,18 @@ def test_refusals_launch_nothing(torch_cuda, coll_mod):
             ("tokens * top_k > 2^31 - 1", dict(tokens=1 << 30, top_k=4, row_elems=16), "tokens * top_k"),
         ]]
         for what, want, kw, msg in ccases:
-            rc = _raw_combine(coll, c, **dict(okc, **kw))
-            err = L.b200collGetLastError().decode()
-            assert rc == want, (what, rc, err)
-            assert msg in err, (what, err)
+            expect_refused(_raw_combine(coll, c, **dict(okc, **kw)), want, msg, what=what)
         with pytest.raises(ValueError):
             c.expert_dispatch(x, torch.zeros(tokens, k, dtype=torch.int32, device="cuda"), 3, recv)       # 3 experts for 2 ranks
         with pytest.raises(ValueError):
             c.expert_combine(eo, torch.zeros(tokens, k, dtype=torch.int64, device="cuda"), None, out)
-        st = c.stats()
-        assert st["kernel_launches"] == 0 and all(v == 0 for v in st["calls"]) and all(v == 0 for v in st["bytes"])
+        assert_nothing_launched(c)
         g.check_async()
-    finally:
-        g.destroy()
 
 
 def _perf_route(devs, procs, extra):
-    r = subprocess.run([PERF, "--devs", devs, *(["--procs"] if procs else []), "--op", "alltoall", *extra, "-w", "1", "-n", "2", "-c", "1"],
-                       capture_output=True, text=True, timeout=600, env={**os.environ, "B200COLL_TIMEOUT_MS": "20000"})
-    assert r.returncode == 0 and "errors=0" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
-    assert [l for l in r.stdout.splitlines() if l.strip() and not l.startswith("#")], r.stdout
+    out = run_perf(["--op", "alltoall", *extra, "-w", "1", "-n", "2", "-c", "1"], devs, procs, env={"B200COLL_TIMEOUT_MS": "20000"})
+    assert [l for l in out.splitlines() if l.strip() and not l.startswith("#")], out
 
 
 def test_two_processes_on_two_gpus(torch_cuda, coll_lib):
@@ -503,15 +390,14 @@ def test_multi_gpu(torch_cuda, coll_mod):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
     n = 2
-    g = Group(torch, coll, n, devices=[0, 1])
-    rng = np.random.default_rng(11)
-    try:
+    with Group(torch, coll, n, devices=[0, 1]) as g:
+        rng = np.random.default_rng(11)
         E, k = 8, 4
         topk = routing("zipf", n, E, k, seed=3, tokens=[300, 200])
         recv_rows = max(int(c.sum()) for c in rr.layout(topk, E, 1 << 20).counts) * 4 // 5
         lay = rr.layout(topk, E, recv_rows)
         xs = [_x_bytes(rng, t.shape[0], ROW * 2, 2) for t in topk]
-        recv = g.recv_bufs(recv_rows, torch.bfloat16)
+        recv = recv_bufs(g, recv_rows, torch.bfloat16)
         got = run_dispatch(g, xs, topk, E, recv, torch.bfloat16)
         check_dispatch(lay, xs, got, "two GPUs")
         outs = [torch.empty(t.shape[0], ROW, dtype=torch.float32, device=f"cuda:{c.device}") for t, c in zip(topk, g.comms)]
@@ -524,16 +410,12 @@ def test_multi_gpu(torch_cuda, coll_mod):
         eo = [recv[r].float().cpu().numpy().reshape(-1, ROW) for r in range(n)]
         for r in range(n):
             assert_same(outs[r].cpu(), cr.combine(route_lookup(eo, recv_rows), lay.route[r], None, 1.0, torch.float32), f"two GPUs combine rank {r}")
-    finally:
-        g.destroy()
 
 
 def test_perf_tool_route_mode(torch_cuda, coll_lib):
     for devs, extra in (("0", ["-d", "bfloat16", "--route", "16:4", "-b", "64K", "-e", "1M", "-f", "4"]),
                         ("0,0", ["-d", "float", "--route", "8:2", "--row-len", "96", "-b", "256K", "-e", "256K"]),
                         ("0,0", ["-d", "half", "--route", "256:8", "-b", "1M", "-e", "1M"])):
-        r = subprocess.run([PERF, "--devs", devs, "--op", "alltoall", *extra, "-w", "1", "-n", "2", "-c", "1"], capture_output=True, text=True,
-                           timeout=600)
-        assert r.returncode == 0 and "errors=0" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
-        rows = [l for l in r.stdout.splitlines() if l.strip() and not l.startswith("#")]
-        assert rows, r.stdout
+        out = run_perf(["--op", "alltoall", *extra, "-w", "1", "-n", "2", "-c", "1"], devs)
+        rows = [l for l in out.splitlines() if l.strip() and not l.startswith("#")]
+        assert rows, out

@@ -4,92 +4,40 @@ Every recv and recv_scales starts poisoned with 0x5A bytes. Every stored row mus
 as in the other quantised tests), tests/coll_quant_reference.quantize of its source token's row (the source from
 tests/coll_routed_reference.layout), and its scales that block's scales; every other row must keep the poison in both buffers.
 expert_counts, route and dropped must equal the layout reference and the bf16 routed dispatch's."""
-import os
-import subprocess
-import sys
-
 import ctypes as C
 import numpy as np
 import pytest
 
+from container_engine_accelerators_b200.ops.coll import INVALID_ARGUMENT, INVALID_USAGE
 from tests import coll_combine_reference as cr
 from tests import coll_quant_reference as qr
 from tests import coll_routed_reference as rr
 from tests.coll_fp_reference import assert_same
-from tests.test_coll_expert_routed_gpu import route_lookup, routing
+from tests.coll_gpu_harness import (DTYPES, Group, assert_nothing_launched, coll_mod, expect_refused, release, run_perf, run_python,  # noqa: F401
+                                    torch_cuda)
+from tests.coll_routed_reference import route_lookup, routing
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PERF = os.path.join(ROOT, "build", "b200coll_perf")
-INVALID_ARGUMENT, INVALID_USAGE = 4, 5
 ROW = 512                                                               # whole blocks of every size tested, 32 vectors per row
 POISON = 0x5A
 
 
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch
+def small_outputs(g, topk, E):
+    """Every rank's (expert_counts, route, dropped), allocated before any rank enqueues."""
+    torch = g.torch
+    return [(torch.empty(E // g.n, dtype=torch.int32, device=f"cuda:{c.device}"), torch.empty(topk[r].shape, dtype=torch.int32, device=f"cuda:{c.device}"),
+             torch.empty(1, dtype=torch.int32, device=f"cuda:{c.device}")) for r, c in enumerate(g.comms)]
 
 
-@pytest.fixture(scope="module")
-def coll_mod(coll_lib):
-    from container_engine_accelerators_b200.ops import coll
-    coll.load()
-    return coll
-
-
-def _dt(torch, name):
-    return {"bf16": torch.bfloat16, "f16": torch.float16, "f32": torch.float32, "e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}[name]
-
-
-class Group:
-    def __init__(self, torch, coll, n, devices=None):
-        self.torch, self.coll, self.n = torch, coll, n
-        self.comms = coll.Comm.init_all(devices if devices is not None else [0] * n, arena_mb=64)
-        self.streams = []
-        for c in self.comms:
-            with torch.cuda.device(c.device):
-                self.streams.append(torch.cuda.Stream())
-
-    def sync(self):
-        for d in {c.device for c in self.comms}:
-            self.torch.cuda.synchronize(d)
-
-    def destroy(self):
-        self.sync()
-        for c in self.comms:
-            c.destroy()
-
-    def dev(self, c, a):
-        return self.torch.from_numpy(np.ascontiguousarray(a)).to(f"cuda:{c.device}")
-
-    def check_async(self):
-        for c in self.comms:
-            c.check_async_error()
-
-    def small(self, topk, E):
-        """Every rank's (expert_counts, route, dropped), allocated before any rank enqueues."""
-        torch = self.torch
-        return [(torch.empty(E // self.n, dtype=torch.int32, device=f"cuda:{c.device}"), torch.empty(topk[r].shape, dtype=torch.int32, device=f"cuda:{c.device}"),
-                 torch.empty(1, dtype=torch.int32, device=f"cuda:{c.device}")) for r, c in enumerate(self.comms)]
-
-    def q_bufs(self, recv_rows, wire, block):
-        """Poisoned arena recv ([recv_rows * ROW] of wire) and recv_scales ([recv_rows * ROW / block] float32) on every rank."""
-        torch = self.torch
-        recv = [c.empty(recv_rows * ROW, wire) for c in self.comms]
-        sc = [c.empty(recv_rows * ROW // block, torch.float32) for c in self.comms]
-        for t in recv + sc:
-            t.view(torch.uint8).fill_(POISON)
-        return recv, sc
-
-    def release(self, *lists):
-        for ts in lists:
-            for c, t in zip(self.comms, ts):
-                c.release(t)
+def q_bufs(g, recv_rows, wire, block):
+    """Poisoned arena recv ([recv_rows * ROW] of wire) and recv_scales ([recv_rows * ROW / block] float32) on every rank."""
+    torch = g.torch
+    recv = [c.empty(recv_rows * ROW, wire) for c in g.comms]
+    sc = [c.empty(recv_rows * ROW // block, torch.float32) for c in g.comms]
+    for t in recv + sc:
+        t.view(torch.uint8).fill_(POISON)
+    return recv, sc
 
 
 def inputs(torch, topk, in_dt, block, seed, specials=True):
@@ -130,8 +78,8 @@ def run_q(g, xd, idx, E, recv_rows, wire, block):
     """The FP8 dispatch on every rank's stream into fresh poisoned buffers; returns (CPU results, buffers)."""
     torch = g.torch
     topk_shapes = [i.shape for i in idx]
-    small = g.small([np.empty(s) for s in topk_shapes], E)
-    recv, sc = g.q_bufs(recv_rows, wire, block)
+    small = small_outputs(g, [np.empty(s) for s in topk_shapes], E)
+    recv, sc = q_bufs(g, recv_rows, wire, block)
     g.sync()
     for r, c in enumerate(g.comms):
         c.expert_dispatch_quantized(xd[r], idx[r], E, recv[r], sc[r], block, *small[r], stream=g.streams[r])
@@ -143,14 +91,14 @@ def run_q(g, xd, idx, E, recv_rows, wire, block):
 def run_bf16_small(g, xd, idx, E, recv_rows):
     """The bf16 (raw rows) routed dispatch of the same ids: its (counts, route, dropped) per rank."""
     torch = g.torch
-    small = g.small([np.empty(i.shape) for i in idx], E)
+    small = small_outputs(g, [np.empty(i.shape) for i in idx], E)
     recv = [c.empty(max(1, recv_rows) * ROW, xd[0].dtype) for c in g.comms]
     g.sync()
     for r, c in enumerate(g.comms):
         c.expert_dispatch(xd[r], idx[r], E, recv[r][:recv_rows * ROW], *small[r], stream=g.streams[r])
     g.sync()
     g.check_async()
-    g.release(recv)
+    release(g.comms, recv)
     return [(s[0].cpu().numpy(), s[1].cpu().numpy(), int(s[2].item())) for s in small]
 
 
@@ -164,10 +112,9 @@ def test_dispatch_bit_exact(torch_cuda, coll_mod, n, in_name):
     """Both wire types x blocks 16, 128, 512 x uniform, Zipf, one-expert and mixed routings (invalid ids, a token naming one expert twice,
     an empty rank) x ample and tight capacity; small outputs equal to the layout and to the bf16 dispatch's; two launches and the stats."""
     torch, coll = torch_cuda, coll_mod
-    in_dt = _dt(torch, in_name)
-    g = Group(torch, coll, n)
-    clipped_inside = twice = 0
-    try:
+    in_dt = DTYPES[in_name]
+    with Group(torch, coll, n) as g:
+        clipped_inside = twice = 0
         for block, (epr, k) in CONFIGS.items():
             E = epr * n
             for kind in ("uniform", "zipf", "one", "mixed"):
@@ -182,7 +129,7 @@ def test_dispatch_bit_exact(torch_cuda, coll_mod, n, in_name):
                     clipped_inside += sum(int(((lay.counts[d] > 0) & (lay.counts[d] < totals[d])).sum()) for d in range(n))
                     wide = run_bf16_small(g, xd, idx, E, recv_rows)
                     for wire_name in ("e4m3", "e5m2"):
-                        wire = _dt(torch, wire_name)
+                        wire = DTYPES[wire_name]
                         ref = quant_ref(torch, xs, block, wire)
                         before = [c.stats() for c in g.comms]
                         got, bufs = run_q(g, xd, idx, E, recv_rows, wire, block)
@@ -203,11 +150,9 @@ def test_dispatch_bit_exact(torch_cuda, coll_mod, n, in_name):
                             assert st["algo_calls"][algo] == b["algo_calls"][algo] + 1, what
                             assert st["calls"][coll.OP_ALLTOALL] == b["calls"][coll.OP_ALLTOALL] + 1, what
                             assert st["bytes"][coll.OP_ALLTOALL] == b["bytes"][coll.OP_ALLTOALL] + topk[r].size * ROW * in_dt.itemsize, what
-                        g.release(*bufs)
+                        release(g.comms, *bufs)
         assert clipped_inside > 0                                      # some receiver stored part of an expert
         assert twice > 0
-    finally:
-        g.destroy()
 
 
 @pytest.mark.parametrize("n", [2, 3])
@@ -216,11 +161,10 @@ def test_cuda_graph_dispatch_dequantise_combine(torch_cuda, coll_mod, n):
     expert_combine over the dispatch's route in one CUDA graph; topk_idx is rewritten in place between replays, and every replay's
     dispatch and combine are checked."""
     torch, coll = torch_cuda, coll_mod
-    g = Group(torch, coll, n)
-    rng = np.random.default_rng(40 + n)
-    block, wire = 128, torch.float8_e4m3fn
-    nb = ROW // block
-    try:
+    with Group(torch, coll, n) as g:
+        rng = np.random.default_rng(40 + n)
+        block, wire = 128, torch.float8_e4m3fn
+        nb = ROW // block
         E, k, tokens = 4 * n, 2, 24
         recv_rows = tokens * k * 3 // 4
         xs = [qr.gen(tokens * ROW, torch.bfloat16, block, 7 + s, specials=False).view(tokens, ROW) for s in range(n)]
@@ -229,8 +173,8 @@ def test_cuda_graph_dispatch_dequantise_combine(torch_cuda, coll_mod, n):
         idx = [torch.zeros(tokens, k, dtype=torch.int32, device="cuda") for _ in range(n)]
         w = [rng.uniform(0.1, 1.0, size=(tokens, k)).astype(np.float32) for _ in range(n)]
         wd = [g.dev(c, w[r]) for r, c in enumerate(g.comms)]
-        small = g.small([np.empty((tokens, k))] * n, E)
-        recv, sc = g.q_bufs(recv_rows, wire, block)
+        small = small_outputs(g, [np.empty((tokens, k))] * n, E)
+        recv, sc = q_bufs(g, recv_rows, wire, block)
         eo = [c.empty(recv_rows * ROW, torch.float32) for c in g.comms]
         outs = [torch.empty(tokens, ROW, dtype=torch.float32, device="cuda") for _ in range(n)]
         g.sync()
@@ -267,8 +211,6 @@ def test_cuda_graph_dispatch_dequantise_combine(torch_cuda, coll_mod, n):
                 want = cr.combine(route_lookup(deq, recv_rows), lay.route[r], w[r], 1.0, torch.float32)
                 assert_same(outs[r].cpu(), want, f"replay {rep} ({kind}): combine rank {r}")
         del graphs
-    finally:
-        g.destroy()
 
 
 def test_interleaved_with_other_collectives(torch_cuda, coll_mod):
@@ -276,16 +218,15 @@ def test_interleaved_with_other_collectives(torch_cuda, coll_mod):
     with no host sync in between, then every result checked: the epochs and the count mailbox stay in step."""
     torch, coll = torch_cuda, coll_mod
     n, E, k, tokens = 4, 16, 2, 40
-    g = Group(torch, coll, n)
-    try:
+    with Group(torch, coll, n) as g:
         t1, t2 = routing("zipf", n, E, k, seed=1, tokens=[tokens] * n), routing("uniform", n, E, k, seed=2, tokens=[tokens] * n)
         recv_rows = tokens * k * 3 // 4
         xs = [qr.gen(tokens * ROW, torch.float32, 16, 3 + s).view(tokens, ROW) for s in range(n)]
         xd = [x.cuda() for x in xs]
         i1 = [g.dev(c, t1[r]) for r, c in enumerate(g.comms)]
         i2 = [g.dev(c, t2[r]) for r, c in enumerate(g.comms)]
-        q1, s1 = g.q_bufs(recv_rows, torch.float8_e4m3fn, 128)
-        q2, s2 = g.q_bufs(recv_rows, torch.float8_e5m2, 16)
+        q1, s1 = q_bufs(g, recv_rows, torch.float8_e4m3fn, 128)
+        q2, s2 = q_bufs(g, recv_rows, torch.float8_e5m2, 16)
         wide = [c.empty(recv_rows * ROW, torch.float32) for c in g.comms]
         ar = [c.empty(4096, torch.float32) for c in g.comms]
         for r, a in enumerate(ar):
@@ -294,7 +235,7 @@ def test_interleaved_with_other_collectives(torch_cuda, coll_mod):
         p = expert_dispatch_plan(n, 20, 64, top_k=1, seed=9)
         sends = [torch.randn(20 * 64, device="cuda").to(torch.bfloat16) for _ in range(n)]
         a2a = [c.empty(p.max_rows * 64, torch.bfloat16) for c in g.comms]
-        sm1, smw, sm2 = g.small(t1, E), g.small(t2, E), g.small(t2, E)
+        sm1, smw, sm2 = small_outputs(g, t1, E), small_outputs(g, t2, E), small_outputs(g, t2, E)
         g.sync()
         for r, c in enumerate(g.comms):
             c.expert_dispatch_quantized(xd[r], i1[r], E, q1[r], s1[r], 128, *sm1[r], stream=g.streams[r])
@@ -323,8 +264,6 @@ def test_interleaved_with_other_collectives(torch_cuda, coll_mod):
                 lo, cnt = int(p.recv_off[r, s]), int(p.rows[s, r])
                 want = sends[s][int(p.send_off[s, r]) * 64:(int(p.send_off[s, r]) + cnt) * 64]
                 assert torch.equal(a2a[r][lo * 64:(lo + cnt) * 64], want)
-    finally:
-        g.destroy()
 
 
 def _raw(coll, comm, **a):
@@ -336,9 +275,7 @@ def _raw(coll, comm, **a):
 
 def test_refusals_launch_nothing(torch_cuda, coll_mod):
     torch, coll = torch_cuda, coll_mod
-    L = coll.load()
-    g = Group(torch, coll, 2)
-    try:
+    with Group(torch, coll, 2) as g:
         c = g.comms[0]
         row, block, rows_n, tokens, k = 128, 32, 16, 4, 2
         recv = c.empty(rows_n * row, torch.float8_e4m3fn)
@@ -376,24 +313,16 @@ def test_refusals_launch_nothing(torch_cuda, coll_mod):
                 ("more than 2^31 - 1 vectors offered", dict(tokens=1 << 22, top_k=32, row_elems=512), "16-byte vectors offered"),
             ]]
         for what, want, kw, msg in cases:
-            rc = _raw(coll, c, **dict(ok, **kw))
-            err = L.b200collGetLastError().decode()
-            assert rc == want, (what, rc, err)
-            assert msg in err, (what, err)
+            expect_refused(_raw(coll, c, **dict(ok, **kw)), want, msg, what=what)
         with pytest.raises(ValueError):
             c.expert_dispatch_quantized(x, torch.zeros(tokens, k, dtype=torch.int32, device="cuda"), 3, recv, scales, block)    # 3 experts, 2 ranks
         with pytest.raises(ValueError):
             c.expert_dispatch_quantized(x, torch.zeros(tokens, k, dtype=torch.int32, device="cuda"), 4, recv, scales, 64)       # scales hold block 32
-        st = c.stats()
-        assert st["kernel_launches"] == 0 and all(v == 0 for v in st["calls"]) and all(v == 0 for v in st["bytes"])
+        assert_nothing_launched(c)
         g.check_async()
-    finally:
-        g.destroy()
 
 
 _LAZY = r'''
-import sys
-sys.path.insert(0, sys.argv[1])
 import numpy as np
 import torch
 from container_engine_accelerators_b200.ops import coll
@@ -445,17 +374,13 @@ def test_lazy_module_loading_bf16_dispatch_first(torch_cuda, coll_lib):
     """A fresh process with lazy module loading and a short watchdog runs the bf16 routed dispatch, then the FP8 one, on two virtual ranks
     driven by one thread: the first dispatch on the device loads every push kernel that can follow a layout kernel, so the FP8 push's
     first launch does not wait behind a layout kernel that waits for the next rank's launch. Both results must be exact."""
-    env = {**os.environ, "CUDA_MODULE_LOADING": "LAZY", "B200COLL_TIMEOUT_MS": "10000"}
-    r = subprocess.run([sys.executable, "-c", _LAZY, ROOT], cwd=ROOT, env=env, capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0 and "lazy ok" in r.stdout, r.stdout[-2000:] + r.stderr[-3000:]
+    run_python(_LAZY, {"CUDA_MODULE_LOADING": "LAZY", "B200COLL_TIMEOUT_MS": "10000"}, "lazy ok")
 
 
 def _perf(devs, procs, extra):
-    r = subprocess.run([PERF, "--devs", devs, *(["--procs"] if procs else []), "--op", "alltoall", *extra, "-w", "1", "-n", "2", "-c", "1"],
-                       capture_output=True, text=True, timeout=600, env={**os.environ, "B200COLL_TIMEOUT_MS": "20000"})
-    assert r.returncode == 0 and "errors=0" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
-    assert "routed FP8 dispatch" in r.stdout, r.stdout
-    assert [l for l in r.stdout.splitlines() if l.strip() and not l.startswith("#")], r.stdout
+    out = run_perf(["--op", "alltoall", *extra, "-w", "1", "-n", "2", "-c", "1"], devs, procs, env={"B200COLL_TIMEOUT_MS": "20000"})
+    assert "routed FP8 dispatch" in out, out
+    assert [l for l in out.splitlines() if l.strip() and not l.startswith("#")], out
 
 
 def test_perf_tool_routed_fp8_mode(torch_cuda, coll_lib):
@@ -476,8 +401,7 @@ def test_one_process_on_two_gpus(torch_cuda, coll_mod):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
     n, E, k, block = 2, 8, 4, 128
-    g = Group(torch, coll, n, devices=[0, 1])
-    try:
+    with Group(torch, coll, n, devices=[0, 1]) as g:
         topk = routing("zipf", n, E, k, seed=3, tokens=[300, 200])
         recv_rows = max(int(c.sum()) for c in rr.layout(topk, E, 1 << 20).counts) * 4 // 5
         xs = inputs(torch, topk, torch.bfloat16, block, seed=21)
@@ -485,6 +409,4 @@ def test_one_process_on_two_gpus(torch_cuda, coll_mod):
         idx = [g.dev(c, topk[r]) for r, c in enumerate(g.comms)]
         got, bufs = run_q(g, xd, idx, E, recv_rows, torch.float8_e4m3fn, block)
         check_q(torch, rr.layout(topk, E, recv_rows), quant_ref(torch, xs, block, torch.float8_e4m3fn), got, torch.float8_e4m3fn, "two GPUs")
-        g.release(*bufs)
-    finally:
-        g.destroy()
+        release(g.comms, *bufs)

@@ -8,36 +8,12 @@ import os
 
 import pytest
 
+from tests.coll_fp_reference import random_fp8
+from tests.coll_gpu_harness import ROOT, Group, coll_mod, group_fixture, run_perf, torch_cuda  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PERF = os.path.join(ROOT, "build", "b200coll_perf")
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch
-
-
-@pytest.fixture(scope="module")
-def coll_mod(coll_lib):
-    from container_engine_accelerators_b200.ops import coll
-    coll.load()
-    return coll
-
-
-@pytest.fixture
-def group(torch_cuda, coll_mod, request):
-    n = getattr(request, "param", 2)
-    comms = coll_mod.Comm.init_all([0] * n, arena_mb=96)
-    streams = [torch_cuda.cuda.Stream() for _ in comms]
-    yield comms, streams
-    torch_cuda.cuda.synchronize()
-    for c in comms:
-        c.destroy()
+group = group_fixture(2, arena_mb=96)
 
 
 def fp8_types(torch):
@@ -46,18 +22,6 @@ def fp8_types(torch):
 
 def finite_max(torch, dt):
     return {torch.float8_e4m3fn: 448.0, torch.float8_e5m2: 57344.0}.get(dt)
-
-
-def random_fp8(torch, n, dt, seed):
-    """Seeded random bytes reinterpreted as FP8, NaN and inf patterns replaced: every exponent occurs, subnormals and values near the
-    maximum included, so sums round and saturate."""
-    g = torch.Generator(device="cpu").manual_seed(seed)
-    b = torch.randint(0, 256, (n,), generator=g, dtype=torch.int32)
-    if dt == torch.float8_e4m3fn:
-        b = torch.where((b & 0x7F) == 0x7F, b - 1, b)                # S.1111.111 is NaN
-    else:
-        b = torch.where((b & 0x7C) == 0x7C, b & 0x83 | 0x78, b)      # exponent 11111 is inf / NaN
-    return b.to(torch.uint8).view(dt).cuda()
 
 
 def cast_ref(torch, f32, dt):
@@ -87,22 +51,13 @@ def assert_bits(torch, got, want, what):
         raise AssertionError(f"{what}: first difference at element {i // e}: got {got.view(-1)[i // e].item()} want {want.view(-1)[i // e].item()}")
 
 
-def run_all(torch, comms, streams, fn):
-    for r, c in enumerate(comms):
-        fn(r, c, streams[r])
-    torch.cuda.synchronize()
-    for c in comms:
-        c.check_async_error()
-
-
 STAGED = 600 << 10          # FP8 elements: 600 KiB per rank, beyond the one-shot Lamport path, buffers outside the arena
 
 
 @pytest.mark.parametrize("group", [2, 4], indirect=True)
 def test_all_reduce_grid_bit_exact(torch_cuda, group):
     torch = torch_cuda
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     outs = lambda dt: [dt, *[o for o in fp8_types(torch) if o != dt], torch.bfloat16, torch.float16]
     for count in (16, 1003, 1 << 15, STAGED):
         staged = count == STAGED
@@ -123,7 +78,7 @@ def test_all_reduce_grid_bit_exact(torch_cuda, group):
                         def body(r, c, st):
                             c.set_algo(algo)
                             c.all_reduce(xs[r], ys[r], scale=scale, op=op, stream=st)
-                        run_all(torch, comms, streams, body)
+                        group.run(body)
                         s = scale if op == 0 else scale * (1.0 / n)
                         want = reduce_ref(torch, xs, s, out_dt)
                         for r in range(n):
@@ -137,8 +92,7 @@ def test_all_reduce_grid_bit_exact(torch_cuda, group):
 @pytest.mark.parametrize("group", [2, 4], indirect=True)
 def test_in_place_fp8_all_reduce(torch_cuda, group):
     torch = torch_cuda
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for dt in fp8_types(torch):
         for algo in ("ll", "ll2", "twoshot"):
             bufs = [c.empty(4099, dt) for c in comms]
@@ -147,7 +101,7 @@ def test_in_place_fp8_all_reduce(torch_cuda, group):
                 b.copy_(random_fp8(torch, 4099, dt, seed=7 * r + 1))
                 xs.append(b.clone())
             torch.cuda.synchronize()
-            run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.all_reduce(bufs[r], op=1, stream=st)))
+            group.run(lambda r, c, st: (c.set_algo(algo), c.all_reduce(bufs[r], op=1, stream=st)))
             want = reduce_ref(torch, xs, 1.0 / n, dt)
             for r in range(n):
                 assert_bits(torch, bufs[r], want, f"in-place {algo} {dt} rank {r}")
@@ -158,7 +112,7 @@ def test_in_place_fp8_all_reduce(torch_cuda, group):
 @pytest.mark.parametrize("group", [2], indirect=True)
 def test_edge_values_saturate_and_nan_propagates(torch_cuda, coll_mod, group):
     torch = torch_cuda
-    comms, streams = group
+    comms = group.comms
     count = 64
     for algo in ("ll", "twoshot"):
         # 448 on every rank: 896 saturates to 448, not NaN
@@ -168,7 +122,7 @@ def test_edge_values_saturate_and_nan_propagates(torch_cuda, coll_mod, group):
         for x in xs:
             x.copy_(v.to(torch.float8_e4m3fn))
         torch.cuda.synchronize()
-        run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.all_reduce(xs[r], ys[r], stream=st)))
+        group.run(lambda r, c, st: (c.set_algo(algo), c.all_reduce(xs[r], ys[r], stream=st)))
         for y in ys:
             assert y[0].float().item() == 448.0 and y[1].float().item() == -448.0 and not torch.isnan(y.float()).any()
         # e5m2 +-inf saturates to +-57344; a NaN on one rank is NaN on every rank
@@ -178,7 +132,7 @@ def test_edge_values_saturate_and_nan_propagates(torch_cuda, coll_mod, group):
         v1 = torch.ones(count); v1[0] = float("inf"); v1[1] = 2.0; v1[2] = float("nan")
         a[0].copy_(v0.to(torch.float8_e5m2)); a[1].copy_(v1.to(torch.float8_e5m2))
         torch.cuda.synchronize()
-        run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.all_reduce(a[r], b[r], stream=st)))
+        group.run(lambda r, c, st: (c.set_algo(algo), c.all_reduce(a[r], b[r], stream=st)))
         for y in b:
             f = y.float()
             assert f[0].item() == 57344.0 and f[1].item() == -57344.0 and torch.isnan(f[2]).item() and f[3].item() == 2.0
@@ -189,8 +143,7 @@ def test_edge_values_saturate_and_nan_propagates(torch_cuda, coll_mod, group):
 @pytest.mark.parametrize("group", [2, 4], indirect=True)
 def test_reduce_scatter_and_rooted_reduce(torch_cuda, group):
     torch = torch_cuda
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     per = 1 << 12
     for in_dt in fp8_types(torch):
         xs = [c.empty(per * n, in_dt) for c in comms]
@@ -200,7 +153,7 @@ def test_reduce_scatter_and_rooted_reduce(torch_cuda, group):
         for out_dt in (torch.bfloat16, in_dt):
             for algo in ("ll", "twoshot", "nvls"):
                 ys = [c.empty(per, out_dt) for c in comms]
-                run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.reduce_scatter(xs[r], ys[r], op=1, stream=st)))
+                group.run(lambda r, c, st: (c.set_algo(algo), c.reduce_scatter(xs[r], ys[r], op=1, stream=st)))
                 for r in range(n):
                     want = reduce_ref(torch, [x[r * per:(r + 1) * per] for x in xs], 1.0 / n, out_dt)
                     assert_bits(torch, ys[r], want, f"reduce_scatter {algo} {in_dt}->{out_dt} rank {r}")
@@ -208,7 +161,7 @@ def test_reduce_scatter_and_rooted_reduce(torch_cuda, group):
                     c.release(y)
             for root in range(n):
                 ys = [c.empty(per * n, out_dt) for c in comms]
-                run_all(torch, comms, streams, lambda r, c, st: (c.set_algo("nvls"), c.reduce(xs[r], ys[r], root=root, scale=0.5, stream=st)))
+                group.run(lambda r, c, st: (c.set_algo("nvls"), c.reduce(xs[r], ys[r], root=root, scale=0.5, stream=st)))
                 assert_bits(torch, ys[root], reduce_ref(torch, xs, 0.5, out_dt), f"reduce root {root} {in_dt}->{out_dt}")
                 for c, y in zip(comms, ys):
                     c.release(y)
@@ -220,8 +173,7 @@ def test_reduce_scatter_and_rooted_reduce(torch_cuda, group):
 @pytest.mark.parametrize("group", [2], indirect=True)
 def test_dequantising_all_gather_broadcast_all_to_all(torch_cuda, group):
     torch = torch_cuda
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     inv = 0.0078125
     for count, arena in ((1 << 20, True), (1 << 20, False), (4096, True)):
         mk = (lambda c, k, dt: c.empty(k, dt)) if arena else (lambda c, k, dt: torch.empty(k, dtype=dt, device="cuda"))
@@ -232,16 +184,16 @@ def test_dequantising_all_gather_broadcast_all_to_all(torch_cuda, group):
         bulk0 = [c.stats()["bulk_launches"] for c in comms]
         deq = lambda x: reduce_ref(torch, [x], inv, torch.bfloat16)     # widened into a zeroed fp32 accumulator (-0 becomes +0), scaled, rounded
         ag = [mk(c, count * n, torch.bfloat16) for c in comms]
-        run_all(torch, comms, streams, lambda r, c, st: c.all_gather(xs[r][:count], ag[r], scale=inv, stream=st))
+        group.run(lambda r, c, st: c.all_gather(xs[r][:count], ag[r], scale=inv, stream=st))
         want = torch.cat([deq(x[:count]) for x in xs])
         for r in range(n):
             assert_bits(torch, ag[r], want, f"all_gather arena={arena} rank {r}")
         bc = [mk(c, count, torch.bfloat16) for c in comms]
-        run_all(torch, comms, streams, lambda r, c, st: c.broadcast(xs[r][:count], bc[r], root=1, scale=inv, stream=st))
+        group.run(lambda r, c, st: c.broadcast(xs[r][:count], bc[r], root=1, scale=inv, stream=st))
         for r in range(n):
             assert_bits(torch, bc[r], deq(xs[1][:count]), f"broadcast arena={arena} rank {r}")
         a2a = [mk(c, count * n, torch.bfloat16) for c in comms]
-        run_all(torch, comms, streams, lambda r, c, st: c.all_to_all(xs[r], a2a[r], scale=inv, stream=st))
+        group.run(lambda r, c, st: c.all_to_all(xs[r], a2a[r], scale=inv, stream=st))
         for r in range(n):
             want = torch.cat([deq(xs[q][r * count:(r + 1) * count]) for q in range(n)])
             assert_bits(torch, a2a[r], want, f"all_to_all arena={arena} rank {r}")
@@ -252,8 +204,7 @@ def test_dequantising_all_gather_broadcast_all_to_all(torch_cuda, group):
 def test_generic_min_max_prod(torch_cuda, coll_mod, group):
     torch = torch_cuda
     coll = coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     count = 5003
     for dt in fp8_types(torch):
         for arena in (True, False):
@@ -265,7 +216,7 @@ def test_generic_min_max_prod(torch_cuda, coll_mod, group):
             for op in (coll.MIN, coll.MAX, coll.PROD):
                 ys = [mk(c, count) for c in comms]
                 gen0 = [c.stats()["generic_launches"] for c in comms]
-                run_all(torch, comms, streams, lambda r, c, st: c.all_reduce(xs[r], ys[r], op=op, stream=st))
+                group.run(lambda r, c, st: c.all_reduce(xs[r], ys[r], op=op, stream=st))
                 acc = xs[0].float()
                 for x in xs[1:]:
                     b = x.float()
@@ -285,21 +236,20 @@ def test_generic_min_max_prod(torch_cuda, coll_mod, group):
     for call in refused:
         with pytest.raises(coll.B200CollError) as e:
             call()
-        assert e.value.code == 4
+        assert e.value.code == coll.INVALID_ARGUMENT
 
 
 @pytest.mark.parametrize("group", [2], indirect=True)
 def test_all_reduce_host_fp8(torch_cuda, group):
     torch = torch_cuda
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for count, key in ((4096, "host_zero_copy"), (9 << 20, "host_pipelined")):
         ins = [c.host_empty(count, torch.float8_e5m2) for c in comms]
         outs = [c.host_empty(count, torch.float8_e4m3fn) for c in comms]
         for r, h in enumerate(ins):
             h.copy_(random_fp8(torch, count, torch.float8_e5m2, seed=77 + r).cpu())
         before = [c.stats()[key] for c in comms]
-        run_all(torch, comms, streams, lambda r, c, st: c.all_reduce_host(ins[r], outs[r], scale=0.25, stream=st))
+        group.run(lambda r, c, st: c.all_reduce_host(ins[r], outs[r], scale=0.25, stream=st))
         want = reduce_ref(torch, [h.cuda() for h in ins], 0.25, torch.float8_e4m3fn).cpu()
         for r in range(n):
             assert_bits(torch, outs[r], want, f"all_reduce_host {count} rank {r}")
@@ -410,10 +360,7 @@ def test_nccl_shim_fp8(torch_cuda, coll_lib):
 @pytest.mark.parametrize("args", [["--op", "all_reduce", "-d", "e4m3", "--out-dtype", "bf16"], ["--op", "all_reduce", "-d", "e5m2", "--out-dtype", "bf16"],
                                   ["--op", "reduce_scatter", "-d", "e4m3"]])
 def test_perf_tool_fp8_zero_errors(torch_cuda, coll_lib, args):
-    import subprocess
-    r = subprocess.run([PERF, "--devs", "0,0,0,0", *args, "-b", "1K", "-e", "64M", "-w", "1", "-n", "2"], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-    assert "errors=0" in r.stdout, r.stdout[-2000:]
+    run_perf([*args, "-b", "1K", "-e", "64M", "-w", "1", "-n", "2"], "0,0,0,0")
 
 
 def test_multi_gpu_fp8_all_reduce_never_records_nvls(torch_cuda, coll_mod):
@@ -421,8 +368,8 @@ def test_multi_gpu_fp8_all_reduce_never_records_nvls(torch_cuda, coll_mod):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
     n = torch.cuda.device_count()
-    comms = coll_mod.Comm.init_all(list(range(n)), arena_mb=256)
-    try:
+    with Group(torch, coll_mod, n, devices=list(range(n)), arena_mb=256) as g:
+        comms = g.comms
         count = 32 << 20
         xs, ys = [], []
         for r, c in enumerate(comms):
@@ -442,11 +389,6 @@ def test_multi_gpu_fp8_all_reduce_never_records_nvls(torch_cuda, coll_mod):
             c.check_async_error()
             assert c.stats()["algo_calls"]["nvls"] == 0
             assert_bits(torch, ys[r].to("cuda:0"), want, f"multi-GPU rank {r}")
-    finally:
-        for r in range(n):
-            torch.cuda.synchronize(r)
-        for c in comms:
-            c.destroy()
 
 
 # ------------------------------------------------------------------------------------------------- process group, two processes

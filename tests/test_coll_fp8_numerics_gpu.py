@@ -11,7 +11,7 @@ import pytest
 import torch
 
 from tests import coll_fp_reference as R
-from tests.test_coll_fp_numerics_gpu import algo_snapshot, coll_mod, dt, group, inputs, poison, ran, release, run_all, scale_of, torch_cuda  # noqa: F401
+from tests.coll_gpu_harness import DTYPES, Group, algo_snapshot, arena_inputs, coll_mod, group_fixture, poison, ran, release, torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -20,6 +20,8 @@ PAIRS = [(E4, E4), (E4, E5), (E4, "bfloat16"), (E4, "float16"), (E5, E5), (E5, E
 SUBSET = [(E5, "bfloat16"), (E5, E5), (E4, E5), (E5, E4)]
 E = 16                                                          # FP8 elements per 16-byte vector
 RANK_ORDER_ALGOS = ("ll", "ll2", "oneshot")
+
+group = group_fixture(3, arena_mb=160, timeout_ms=60000)
 
 
 def is_fp8(name):
@@ -46,10 +48,10 @@ def order_for(algo, n, in_dt, count):
     return ("owner", n, R.vec_elems(in_dt), count)
 
 
-def check_ar(torch, coll, comms, streams, ins, count, in_name, out_name, algo, op, scale, what, outs=None, xs=None):
+def check_ar(torch, coll, g, ins, count, in_name, out_name, algo, op, scale, what, outs=None, xs=None):
     """One all-reduce on arena buffers, checked against the rank-order reference; returns the algorithm that ran."""
-    n = len(comms)
-    in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+    comms, n = g.comms, g.n
+    in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
     is_, os_ = R.esize(in_dt), R.esize(out_dt)
     xs = ins if xs is None else xs
     own_outs = outs is None
@@ -58,14 +60,14 @@ def check_ar(torch, coll, comms, streams, ins, count, in_name, out_name, algo, o
     if not inplace:
         poison(outs)
     before = algo_snapshot(comms)
-    run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.all_reduce(ins[r], outs[r], scale=scale, op=op, stream=st)))
+    g.run(lambda r, c, st: (c.set_algo(algo), c.all_reduce(ins[r], outs[r], scale=scale, op=op, stream=st)))
     got = ran(comms, before)
     assert len(got) == 1 and sum(got.values()) == 1, f"{what}: {got}"
     a = next(iter(got))
     want_algo = ar_pick(coll, n, comms[0].nvls, algo, count * is_, is_, os_, True, inplace=inplace)
     assert a == want_algo, f"{what}: asked for {algo}, expected {want_algo}, ran {a}"
     assert a != "nvls" and (a != "ll2" or is_ == os_), f"{what}: ran {a}"
-    want = R.ref_reduce(xs, list(range(n)), scale_of(coll, op, scale, n), out_dt)
+    want = R.ref_reduce(xs, list(range(n)), R.scale_of(coll, op, scale, n), out_dt)
     for r in range(n):
         R.assert_same(outs[r], want, f"{what} rank {r} ran {a}")
     if own_outs:
@@ -82,8 +84,7 @@ def bound_counts(n):
 @pytest.mark.parametrize("group", [2, 3, 5, 6, 7, 8], indirect=True)
 def test_all_reduce_grid(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     pairs = PAIRS if n <= 3 else SUBSET
     reds = [(coll.SUM, 1.0), (coll.SUM, 0.1), (coll.AVG, 1.0)]
     algos = ("ll", "ll2", "oneshot", "twoshot", "nvls", "auto")
@@ -92,14 +93,14 @@ def test_all_reduce_grid(torch_cuda, coll_mod, group):
         outs_for = [o for i, o in pairs if i == in_name]
         if not outs_for:
             continue
-        in_dt = dt(torch, in_name)
+        in_dt = DTYPES[in_name]
         counts = [1, 15, 17, 1003, E * (37 * n + 1) + 3] + (bound_counts(n) if n <= 3 or in_name == E5 else [])
         for count in counts:
-            ins = inputs(torch, comms, count, in_dt, seed=100 * n + count % 97 + (in_name == E5))
+            ins = arena_inputs(comms, count, in_dt, seed=100 * n + count % 97 + (in_name == E5))
             for out_name in outs_for:
                 for algo in algos:
                     for op, scale in (reds if count < 100000 else reds[:2]):
-                        a = check_ar(torch, coll, comms, streams, ins, count, in_name, out_name, algo, op, scale,
+                        a = check_ar(torch, coll, group, ins, count, in_name, out_name, algo, op, scale,
                                      f"all_reduce n={n} count={count} {in_name}->{out_name} {algo} op={op} scale={scale}")
                         seen.add(a)
                         if algo == "auto":
@@ -118,14 +119,13 @@ def test_all_reduce_grid(torch_cuda, coll_mod, group):
 def test_all_reduce_in_place_mixed_sizes(torch_cuda, coll_mod, group):
     """In place, one-shot and two-shot Lamport and two-shot alternating with growing and shrinking ragged counts."""
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     seq = [("ll", 4099, E5), ("ll2", 1003, E4), ("twoshot", E * (37 * n + 1) + 3, E5), ("ll", 9, E4), ("ll2", 70001, E5),
            ("twoshot", 1003, E4), ("ll2", 17, E5), ("ll", 1003, E5), ("ll2", 4099, E4), ("twoshot", 70001, E5)]
     for it, (algo, count, name) in enumerate(seq):
-        bufs = inputs(torch, comms, count, dt(torch, name), seed=it)
+        bufs = arena_inputs(comms, count, DTYPES[name], seed=it)
         xs = [b.clone() for b in bufs]
-        check_ar(torch, coll, comms, streams, bufs, count, name, name, algo, coll.AVG, 1.0, f"in place #{it} n={n} {algo} {name} count={count}",
+        check_ar(torch, coll, group, bufs, count, name, name, algo, coll.AVG, 1.0, f"in place #{it} n={n} {algo} {name} count={count}",
                  outs=bufs, xs=xs)
         release(comms, bufs)
 
@@ -134,10 +134,9 @@ def test_all_reduce_in_place_mixed_sizes(torch_cuda, coll_mod, group):
 def test_all_reduce_staged_chunks(torch_cuda, coll_mod, group):
     """Buffers outside the arena: one two-shot per staging chunk (16 Mi elements for e5m2 -> bf16, 32 Mi for e4m3 -> e4m3)."""
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for in_name, out_name, nchunks in ((E5, "bfloat16", 2), (E4, E4, 1)):
-        in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+        in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
         chunk = R.staged_chunk(1, R.esize(out_dt), n, "all_reduce")
         assert chunk == (16 << 20 if out_name == "bfloat16" else 32 << 20)
         count = nchunks * chunk + 1003
@@ -146,9 +145,9 @@ def test_all_reduce_staged_chunks(torch_cuda, coll_mod, group):
         for op, scale in ((coll.SUM, 0.1), (coll.AVG, 1.0)):
             poison(outs)
             before = algo_snapshot(comms)
-            run_all(torch, comms, streams, lambda r, c, st: (c.set_algo("auto"), c.all_reduce(xs[r], outs[r], scale=scale, op=op, stream=st)))
+            group.run(lambda r, c, st: (c.set_algo("auto"), c.all_reduce(xs[r], outs[r], scale=scale, op=op, stream=st)))
             assert ran(comms, before) == {"twoshot": nchunks + 1}
-            want = R.ref_reduce(xs, list(range(n)), scale_of(coll, op, scale, n), out_dt)
+            want = R.ref_reduce(xs, list(range(n)), R.scale_of(coll, op, scale, n), out_dt)
             for r in range(n):
                 R.assert_same(outs[r], want, f"staged all_reduce {in_name}->{out_name} count={count} op={op} rank {r}")
         del outs, xs
@@ -158,29 +157,28 @@ def test_all_reduce_staged_chunks(torch_cuda, coll_mod, group):
 @pytest.mark.parametrize("group", [2, 3, 5, 7], indirect=True)
 def test_reduce_scatter_grid(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     pairs = PAIRS if n <= 3 else SUBSET
     ll = R.LL_ONESHOT_MAX_BYTES
     for in_name in (E4, E5):
-        in_dt = dt(torch, in_name)
+        in_dt = DTYPES[in_name]
         for count in (E, 37 * E, ll, ll + E):
-            ins = inputs(torch, comms, count * n, in_dt, seed=count + n + (in_name == E5))
+            ins = arena_inputs(comms, count * n, in_dt, seed=count + n + (in_name == E5))
             for i_, out_name in pairs:
                 if i_ != in_name:
                     continue
-                out_dt = dt(torch, out_name)
+                out_dt = DTYPES[out_name]
                 outs = [c.empty(count, out_dt) for c in comms]
                 for algo in ("ll", "twoshot", "nvls"):
                     for op, scale in ((coll.SUM, 1.0), (coll.SUM, 0.1), (coll.AVG, 1.0)):
                         poison(outs)
                         before = algo_snapshot(comms)
-                        run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.reduce_scatter(ins[r], outs[r], scale=scale, op=op, stream=st)))
+                        group.run(lambda r, c, st: (c.set_algo(algo), c.reduce_scatter(ins[r], outs[r], scale=scale, op=op, stream=st)))
                         a = next(iter(ran(comms, before)))
                         assert a == ("ll" if algo == "ll" and count <= ll else "twoshot"), (algo, count, a)
                         for r in range(n):
                             xs = [x[r * count:(r + 1) * count] for x in ins]
-                            R.assert_same(outs[r], R.ref_reduce(xs, list(range(n)), scale_of(coll, op, scale, n), out_dt),
+                            R.assert_same(outs[r], R.ref_reduce(xs, list(range(n)), R.scale_of(coll, op, scale, n), out_dt),
                                           f"reduce_scatter n={n} count={count} {in_name}->{out_name} {algo} ran {a} op={op} scale={scale} rank {r}")
                 release(comms, outs)
             release(comms, ins)
@@ -191,16 +189,15 @@ def test_reduce_scatter_grid(torch_cuda, coll_mod, group):
 @pytest.mark.parametrize("group", [3], indirect=True)
 def test_reduce_scatter_staged_two_chunks(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
-    in_dt, out_dt = dt(torch, E5), torch.bfloat16
+    comms, n = group.comms, group.n
+    in_dt, out_dt = DTYPES[E5], torch.bfloat16
     chunk = R.staged_chunk(1, 2, n, "reduce_scatter")
     count = chunk + 37 * E
     xs = R.gen_inputs(n, count * n, in_dt, seed=9)
     outs = [torch.empty(count, dtype=out_dt, device="cuda") for _ in comms]
     poison(outs)
     before = algo_snapshot(comms)
-    run_all(torch, comms, streams, lambda r, c, st: (c.set_algo("auto"), c.reduce_scatter(xs[r], outs[r], scale=0.1, op=coll.AVG, stream=st)))
+    group.run(lambda r, c, st: (c.set_algo("auto"), c.reduce_scatter(xs[r], outs[r], scale=0.1, op=coll.AVG, stream=st)))
     assert ran(comms, before) == {"twoshot": 2}
     for r in range(n):
         R.assert_same(outs[r], R.ref_reduce([x[r * count:(r + 1) * count] for x in xs], list(range(n)), R.avg_scale(0.1, n), out_dt),
@@ -211,21 +208,20 @@ def test_reduce_scatter_staged_two_chunks(torch_cuda, coll_mod, group):
 @pytest.mark.parametrize("group", [3, 5], indirect=True)
 def test_reduce_every_root(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     pairs = PAIRS if n <= 3 else SUBSET
     for in_name, out_name in pairs:
-        in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+        in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
         for count in (1003, E * (37 * n + 1) + 3):
-            ins = inputs(torch, comms, count, in_dt, seed=count * 3 + n)
+            ins = arena_inputs(comms, count, in_dt, seed=count * 3 + n)
             outs = [c.empty(count, out_dt) for c in comms]
             for root in range(n):
                 for op, scale in ((coll.SUM, 0.1), (coll.AVG, 1.0)):
                     poison(outs)
                     untouched = outs[0].view(torch.uint8).clone()
-                    run_all(torch, comms, streams, lambda r, c, st: c.reduce(ins[r], outs[r], root=root, scale=scale, op=op, stream=st))
+                    group.run(lambda r, c, st: c.reduce(ins[r], outs[r], root=root, scale=scale, op=op, stream=st))
                     what = f"reduce n={n} root={root} count={count} {in_name}->{out_name} op={op}"
-                    R.assert_same(outs[root], R.ref_reduce(ins, list(range(n)), scale_of(coll, op, scale, n), out_dt), what)
+                    R.assert_same(outs[root], R.ref_reduce(ins, list(range(n)), R.scale_of(coll, op, scale, n), out_dt), what)
                     for r in range(n):
                         if r != root:
                             assert torch.equal(outs[r].view(torch.uint8), untouched), f"{what}: rank {r}'s recv was written"
@@ -241,27 +237,26 @@ def test_data_movement(torch_cuda, coll_mod, group):
     """All-gather, broadcast, all-to-all and all-to-all-v: round((0 + x) * scale) with a cast or a scale; with the identity epilogue a
     bit copy (NaN payloads, -0 and the sentinel words kept) on the barrier kernels, and from 1 MiB on the copy engine."""
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for in_name, out_name, scale in MOVES:
-        in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+        in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
         ident = in_name == out_name and scale == 1.0
         mv = lambda x: R.ref_move(x, scale, out_dt, ident)
         tag = f"n={n} {in_name}->{out_name} scale={scale}"
         big = (1 << 20) + 5 * E                                          # >= 1 MiB per rank: the copy-engine ring for the identity
         for count in (37 * E, big):
-            src = inputs(torch, comms, count * n, in_dt, seed=count + 31 * n)
+            src = arena_inputs(comms, count * n, in_dt, seed=count + 31 * n)
             for algo in (("twoshot",) if ident else ("auto", "ll", "twoshot")):
                 bulk0 = [c.stats()["bulk_launches"] for c in comms]
                 ag = [c.empty(count * n, out_dt) for c in comms]
                 poison(ag)
-                run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.all_gather(src[r][:count], ag[r], scale=scale, stream=st)))
+                group.run(lambda r, c, st: (c.set_algo(algo), c.all_gather(src[r][:count], ag[r], scale=scale, stream=st)))
                 want = torch.cat([mv(x[:count]) for x in src])
                 for r in range(n):
                     R.assert_same(ag[r], want, f"all_gather {tag} count={count} {algo} rank {r}", nan_payloads=ident)
                 a2a = [c.empty(count * n, out_dt) for c in comms]
                 poison(a2a)
-                run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.all_to_all(src[r], a2a[r], scale=scale, stream=st)))
+                group.run(lambda r, c, st: (c.set_algo(algo), c.all_to_all(src[r], a2a[r], scale=scale, stream=st)))
                 for r in range(n):
                     want = torch.cat([mv(src[q][r * count:(r + 1) * count]) for q in range(n)])
                     R.assert_same(a2a[r], want, f"all_to_all {tag} count={count} {algo} rank {r}", nan_payloads=ident)
@@ -275,7 +270,7 @@ def test_data_movement(torch_cuda, coll_mod, group):
                     bc = [c.empty(bcount, out_dt) for c in comms]
                     poison(bc)
                     bulk0 = [c.stats()["bulk_launches"] for c in comms]
-                    run_all(torch, comms, streams, lambda r, c, st: c.broadcast(src[r][:bcount], bc[r], root=root, scale=scale, stream=st))
+                    group.run(lambda r, c, st: c.broadcast(src[r][:bcount], bc[r], root=root, scale=scale, stream=st))
                     for r in range(n):
                         R.assert_same(bc[r], mv(src[root][:bcount]), f"broadcast {tag} count={bcount} root={root} rank {r}", nan_payloads=ident)
                     if ident and bcount == big:
@@ -285,12 +280,12 @@ def test_data_movement(torch_cuda, coll_mod, group):
         hidden = 8 * E
         rows = [[(3 * s + 5 * d) % 7 for d in range(n)] for s in range(n)]
         cap = max(max(sum(rows[s]) for s in range(n)), max(sum(rows[s][d] for s in range(n)) for d in range(n))) + 1
-        send = inputs(torch, comms, cap * hidden, in_dt, seed=77 + n)
+        send = arena_inputs(comms, cap * hidden, in_dt, seed=77 + n)
         recv = [c.empty(cap * hidden, out_dt) for c in comms]
         poison(recv)
         send_off = [[sum(rows[s][:d]) for d in range(n)] for s in range(n)]
         recv_off = [[sum(rows[x][d] for x in range(s)) for s in range(n)] for d in range(n)]
-        run_all(torch, comms, streams, lambda r, c, st: c.all_to_all_v(send[r], recv[r], hidden, rows[r], send_off[r], [recv_off[d][r] for d in range(n)],
+        group.run(lambda r, c, st: c.all_to_all_v(send[r], recv[r], hidden, rows[r], send_off[r], [recv_off[d][r] for d in range(n)],
                                                                        scale=scale, stream=st))
         for d in range(n):
             for s in range(n):
@@ -306,21 +301,20 @@ def test_lamport_identity_movement(torch_cuda, coll_mod, group):
     arrives unchanged (e5m2 +-inf, -0 and NaN payloads included) except a 4-byte word equal to the empty-slot sentinel FF FF FF FF,
     which arrives as FF 7F FF 7F. The same holds for 16- and 32-bit payloads."""
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for name in (E5, E4, "bfloat16", "float16", "float32"):
-        t = dt(torch, name)
+        t = DTYPES[name]
         e = R.vec_elems(t)
         for count in (37 * e, 4096 * e):
-            src = inputs(torch, comms, count * n, t, seed=count + 3 * n)
+            src = arena_inputs(comms, count * n, t, seed=count + 3 * n)
             ag = [c.empty(count * n, t) for c in comms]
             a2a = [c.empty(count * n, t) for c in comms]
             poison(ag + a2a)
             before = algo_snapshot(comms)
-            # one collective per run_all: with virtual ranks, a second kernel queued behind a spinning one on a rank's stream can hold
+            # one collective per group.run: with virtual ranks, a second kernel queued behind a spinning one on a rank's stream can hold
             # up another rank's first kernel in the device's shared work queues
-            run_all(torch, comms, streams, lambda r, c, st: (c.set_algo("ll"), c.all_gather(src[r][:count], ag[r], stream=st)))
-            run_all(torch, comms, streams, lambda r, c, st: c.all_to_all(src[r], a2a[r], stream=st))
+            group.run(lambda r, c, st: (c.set_algo("ll"), c.all_gather(src[r][:count], ag[r], stream=st)))
+            group.run(lambda r, c, st: c.all_to_all(src[r], a2a[r], stream=st))
             assert ran(comms, before) == {"ll": 2}
             if t == torch.float8_e5m2:                                      # +inf from rank 0 and -inf from rank N-1 stay infinite
                 got = [ag[0][p].float().item() for p in (11, count * (n - 1) + 19)]
@@ -356,10 +350,9 @@ def _generic_ref(torch, coll, xs, op):
 @pytest.mark.parametrize("group", [3, 5], indirect=True)
 def test_generic_kernel(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for name in (E4, E5):
-        t = dt(torch, name)
+        t = DTYPES[name]
         for op in (coll.MIN, coll.MAX, coll.PROD):
             for count in (1003, E * (37 * n + 1) + 3):
                 xs = R.gen_inputs(n, count, t, seed=count + op + n)
@@ -377,20 +370,20 @@ def test_generic_kernel(torch_cuda, coll_mod, group):
                 outs = [c.empty(count, t) for c in comms]
                 poison(outs)
                 gen0 = [c.stats()["generic_launches"] for c in comms]
-                run_all(torch, comms, streams, lambda r, c, st: c.all_reduce(ins[r], outs[r], op=op, stream=st))
+                group.run(lambda r, c, st: c.all_reduce(ins[r], outs[r], op=op, stream=st))
                 for r in range(n):
                     R.assert_same(outs[r], want, f"{what} all_reduce rank {r}")
                 assert all(c.stats()["generic_launches"] == g0 + 1 for c, g0 in zip(comms, gen0))
                 for root in (0, n - 1):
                     poison(outs)
                     untouched = outs[0].view(torch.uint8).clone()
-                    run_all(torch, comms, streams, lambda r, c, st: c.reduce(ins[r], outs[r], root=root, op=op, stream=st))
+                    group.run(lambda r, c, st: c.reduce(ins[r], outs[r], root=root, op=op, stream=st))
                     R.assert_same(outs[root], want, f"{what} reduce root {root}")
                     assert all(torch.equal(outs[r].view(torch.uint8), untouched) for r in range(n) if r != root)
                 release(comms, outs)
                 rc = (count // n) // E * E
                 rs = [c.empty(rc, t) for c in comms]
-                run_all(torch, comms, streams, lambda r, c, st: c.reduce_scatter(ins[r][:rc * n], rs[r], op=op, stream=st))
+                group.run(lambda r, c, st: c.reduce_scatter(ins[r][:rc * n], rs[r], op=op, stream=st))
                 for r in range(n):
                     R.assert_same(rs[r], _generic_ref(torch, coll, [x[r * rc:(r + 1) * rc] for x in xs], op), f"{what} reduce_scatter rank {r}")
                 release(comms, rs, ins)
@@ -400,7 +393,7 @@ def test_generic_kernel(torch_cuda, coll_mod, group):
                 outs = [torch.empty(count, dtype=t, device="cuda") for _ in comms]
                 poison(outs)
                 st0 = [c.stats()["staged_calls"] for c in comms]
-                run_all(torch, comms, streams, lambda r, c, st: c.all_reduce(xs[r], outs[r], op=op, stream=st))
+                group.run(lambda r, c, st: c.all_reduce(xs[r], outs[r], op=op, stream=st))
                 assert [c.stats()["staged_calls"] - s for c, s in zip(comms, st0)] == [1] * n
                 for r in range(n):
                     R.assert_same(outs[r], _generic_ref(torch, coll, xs, op), f"generic staged {name} op={op} rank {r}")
@@ -411,10 +404,10 @@ def test_one_rank(torch_cuda, coll_mod):
     """nranks == 1: the FP8 identity is a bit copy at every size (the copy engine from 1 MiB when the size is whole 16-byte vectors;
     in place nothing is launched), and e4m3 -> bf16 at scale 0.1 is round((0 + x) * 0.1) in the vector body and the tail alike."""
     torch, coll = torch_cuda, coll_mod
-    (c,) = coll.Comm.init_all([0], arena_mb=96, timeout_ms=60000)
-    try:
+    with Group(torch, coll, 1, arena_mb=96, timeout_ms=60000) as g:
+        c = g.comms[0]
         for in_name, out_name, scale in ((E4, E4, 1.0), (E5, E5, 1.0), (E4, "bfloat16", 0.1)):
-            in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+            in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
             ident = in_name == out_name
             for count in (1, 17, (1 << 20) + 3, (1 << 20) + 16):
                 (x,) = R.gen_inputs(1, count, in_dt, seed=count)
@@ -440,9 +433,6 @@ def test_one_rank(torch_cuda, coll_mod):
                     assert c.stats()["kernel_launches"] == k0
                 c.release(src)
         c.check_async_error()
-    finally:
-        torch.cuda.synchronize()
-        c.destroy()
 
 
 # ------------------------------------------------------------------------------------------------- grid-stride loops
@@ -450,25 +440,24 @@ def test_one_rank(torch_cuda, coll_mod):
 def test_one_cta_launch_shape(torch_cuda, coll_mod, group):
     """One CTA of 128 threads: every grid-stride loop runs many passes. The communicators are destroyed afterwards."""
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for c in comms:
         c.set_launch_shape("p2p", max_ctas=1, threads=128)
         c.set_launch_shape("ll", 1, 128)
     for out_name in ("bfloat16", E5):
-        out_dt = dt(torch, out_name)
+        out_dt = DTYPES[out_name]
         for count in (1003, E * (37 * n + 1) + 3, 100003):
-            ins = inputs(torch, comms, count, dt(torch, E5), seed=count)
+            ins = arena_inputs(comms, count, DTYPES[E5], seed=count)
             for algo in ("ll", "ll2", "oneshot", "twoshot"):
-                check_ar(torch, coll, comms, streams, ins, count, E5, out_name, algo, coll.SUM, 0.1, f"one CTA all_reduce e5m2->{out_name} {count} {algo}")
+                check_ar(torch, coll, group, ins, count, E5, out_name, algo, coll.SUM, 0.1, f"one CTA all_reduce e5m2->{out_name} {count} {algo}")
             release(comms, ins)
         rcount = 3001 * E
-        ins = inputs(torch, comms, rcount * n, dt(torch, E5), seed=3)
+        ins = arena_inputs(comms, rcount * n, DTYPES[E5], seed=3)
         outs = [c.empty(rcount, out_dt) for c in comms]
         for algo in ("ll", "twoshot"):
             poison(outs)
             before = algo_snapshot(comms)
-            run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.reduce_scatter(ins[r], outs[r], scale=0.1, stream=st)))
+            group.run(lambda r, c, st: (c.set_algo(algo), c.reduce_scatter(ins[r], outs[r], scale=0.1, stream=st)))
             assert ran(comms, before) == {algo: 1}
             for r in range(n):
                 R.assert_same(outs[r], R.ref_reduce([x[r * rcount:(r + 1) * rcount] for x in ins], list(range(n)), 0.1, out_dt),
@@ -489,11 +478,11 @@ def test_all_reduce_host_per_chunk(torch_cuda, coll_mod, group):
     is an all-reduce of its own on arena staging buffers, so each has its own algorithm (predicted here with the tuner and the feasibility
     rules) and, on two-shot with 16- or 32-bit inputs, its own slices: the reference is built chunk by chunk."""
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
+    comms = group.comms
     n, nvls = len(comms), comms[0].nvls
     regimes = set()
     for in_name, out_name, counts in HOST_CASES:
-        in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+        in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
         is_, os_ = R.esize(in_dt), R.esize(out_dt)
         for count in counts:
             inplace = in_name == out_name == "bfloat16" and count == counts[-1]
@@ -516,7 +505,7 @@ def test_all_reduce_host_per_chunk(torch_cuda, coll_mod, group):
             st0 = [(c.stats()["host_zero_copy"], c.stats()["host_pipelined"]) for c in comms]
             for c in comms:
                 c.set_algo("auto")
-            run_all(torch, comms, streams, lambda r, c, st: c.all_reduce_host(h_in[r], h_out[r], scale=0.1, stream=st))
+            group.run(lambda r, c, st: c.all_reduce_host(h_in[r], h_out[r], scale=0.1, stream=st))
             what = f"all_reduce_host n={n} {in_name}->{out_name} count={count} {regime} in_place={inplace}"
             assert ran(comms, before) == want_calls, (what, algos)
             assert [(c.stats()["host_zero_copy"] - z, c.stats()["host_pipelined"] - p) for c, (z, p) in zip(comms, st0)] == \
@@ -543,9 +532,9 @@ def test_multi_gpu_e5m2(torch_cuda, coll_mod):
     n = torch.cuda.device_count()
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
-    comms = coll.Comm.init_all(list(range(n)), arena_mb=256, timeout_ms=60000)
-    try:
-        t = dt(torch, E5)
+    with Group(torch, coll, n, devices=list(range(n)), arena_mb=256, timeout_ms=60000) as g:
+        comms = g.comms
+        t = DTYPES[E5]
         for algo, count in (("twoshot", E * (4099 * n + 1) + 3), ("ll", 100003)):
             xs = R.gen_inputs(n, count, t, seed=n + count % 7)
             ins, outs = [], []
@@ -571,8 +560,3 @@ def test_multi_gpu_e5m2(torch_cuda, coll_mod):
                 R.assert_same(outs[r].to("cuda:0"), want, f"multi-GPU e5m2->bf16 {algo} rank {r}")
             for r, c in enumerate(comms):
                 c.release(outs[r]); c.release(ins[r])
-    finally:
-        for r in range(n):
-            torch.cuda.synchronize(r)
-        for c in comms:
-            c.destroy()

@@ -10,6 +10,7 @@ import warnings
 import pytest
 
 from tests import coll_fp_reference as R
+from tests.coll_gpu_harness import DTYPES, Group, algo_snapshot, arena_inputs, coll_mod, group_fixture, poison, ran, release, torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -21,57 +22,7 @@ SUBSET = [("bfloat16", "bfloat16"), ("float32", "bfloat16"), ("float16", "float1
 RANK_ORDER_ALGOS = ("ll", "ll2", "oneshot")
 
 
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch
-
-
-@pytest.fixture(scope="module")
-def coll_mod(coll_lib):
-    from container_engine_accelerators_b200.ops import coll
-    coll.load()
-    return coll
-
-
-@pytest.fixture
-def group(torch_cuda, coll_mod, request):
-    n = getattr(request, "param", 3)
-    comms = coll_mod.Comm.init_all([0] * n, arena_mb=160, timeout_ms=60000)
-    streams = [torch_cuda.cuda.Stream() for _ in comms]
-    yield comms, streams
-    torch_cuda.cuda.synchronize()
-    for c in comms:
-        c.destroy()
-
-
-def dt(torch, name):
-    return getattr(torch, name)
-
-
-def run_all(torch, comms, streams, fn):
-    """Launch one call per rank on the rank's own stream. The rank streams are not ordered after the default stream, where the inputs
-    are filled and the receive buffers poisoned, so each one waits for it first."""
-    for r, c in enumerate(comms):
-        streams[r].wait_stream(torch.cuda.current_stream())
-        fn(r, c, streams[r])
-    torch.cuda.synchronize()
-    for c in comms:
-        c.check_async_error()
-
-
-def algo_snapshot(comms):
-    return [c.stats()["algo_calls"] for c in comms]
-
-
-def ran(comms, before):
-    """The algorithms the last call(s) recorded: {name: calls}, the same on every rank."""
-    after = algo_snapshot(comms)
-    deltas = [{k: a[k] - b[k] for k in a if a[k] != b[k]} for a, b in zip(after, before)]
-    assert all(d == deltas[0] for d in deltas), deltas
-    return deltas[0]
+group = group_fixture(3, arena_mb=160, timeout_ms=60000)
 
 
 def order_for(algo, n, e, count):
@@ -79,32 +30,6 @@ def order_for(algo, n, e, count):
         return list(range(n))
     assert algo == "twoshot", f"no bit-exact order model for {algo}"
     return ("owner", n, e, count)
-
-
-def scale_of(coll, op, scale, n):
-    return scale if op == coll.SUM else R.avg_scale(scale, n)
-
-
-def poison(ts):
-    """Fill receive buffers with a byte pattern first, so that an element a kernel never wrote cannot pass as a stale right answer."""
-    for t in ts:
-        t.view(-1).view(R.INT_VIEW[1]).fill_(0x7B)
-
-
-def inputs(torch, comms, count, in_dt, seed):
-    """Seeded inputs in arena buffers (one per rank)."""
-    xs = R.gen_inputs(len(comms), count, in_dt, seed)
-    bufs = [c.empty(count, in_dt) for c in comms]
-    for b, x in zip(bufs, xs):
-        b.copy_(x)
-    torch.cuda.synchronize()
-    return bufs
-
-
-def release(comms, *per_rank_lists):
-    for lst in per_rank_lists:
-        for c, t in zip(comms, lst):
-            c.release(t)
 
 
 def ar_expected(coll, comms, algo, count, is_, os_):
@@ -118,10 +43,10 @@ def ar_expected(coll, comms, algo, count, is_, os_):
     return algo if feasible else ("nvls" if nvls and n > 2 else "twoshot")
 
 
-def check_all_reduce(torch, coll, comms, streams, ins, count, in_name, out_name, algo, op, scale, what, outs=None, xs=None):
+def check_all_reduce(torch, coll, g, ins, count, in_name, out_name, algo, op, scale, what, outs=None, xs=None):
     """One all-reduce; returns the algorithm that ran. ins are the send buffers, xs their contents (default: ins)."""
-    n = len(comms)
-    in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+    comms, n = g.comms, g.n
+    in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
     is_, os_ = R.esize(in_dt), R.esize(out_dt)
     xs = ins if xs is None else xs
     own_outs = outs is None
@@ -129,13 +54,13 @@ def check_all_reduce(torch, coll, comms, streams, ins, count, in_name, out_name,
     if outs[0].data_ptr() != ins[0].data_ptr():
         poison(outs)
     before = algo_snapshot(comms)
-    run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.all_reduce(ins[r], outs[r], scale=scale, op=op, stream=st)))
+    g.run(lambda r, c, st: (c.set_algo(algo), c.all_reduce(ins[r], outs[r], scale=scale, op=op, stream=st)))
     got = ran(comms, before)
     assert len(got) == 1 and sum(got.values()) == 1, f"{what}: {got}"
     a = next(iter(got))
     want_algo = ar_expected(coll, comms, algo, count, is_, os_)
     assert a == want_algo, f"{what}: asked for {algo}, expected {want_algo}, ran {a}"
-    want = R.ref_reduce(xs, order_for(a, n, R.vec_elems(in_dt), count), scale_of(coll, op, scale, n), out_dt)
+    want = R.ref_reduce(xs, order_for(a, n, R.vec_elems(in_dt), count), R.scale_of(coll, op, scale, n), out_dt)
     for r in range(n):
         R.assert_same(outs[r], want, f"{what} rank {r} ran {a}")
     if own_outs:
@@ -157,8 +82,7 @@ def bound_counts(in_dt, n):
 @pytest.mark.parametrize("group", [2, 3, 5, 8], indirect=True)
 def test_all_reduce_grid(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     pairs = PAIRS if n <= 3 else SUBSET
     reds = [(coll.SUM, 1.0), (coll.SUM, 0.1), (coll.AVG, 1.0)]
     seen = set()
@@ -167,15 +91,15 @@ def test_all_reduce_grid(torch_cuda, coll_mod, group):
         outs_for = [o for i, o in pairs if i == in_name]
         if not outs_for:
             continue
-        in_dt = dt(torch, in_name)
+        in_dt = DTYPES[in_name]
         e = R.vec_elems(in_dt)
         counts = ar_counts(e, n) + (bound_counts(in_dt, n) if n <= 3 or in_name == "bfloat16" else [])
         for count in counts:
-            ins = inputs(torch, comms, count, in_dt, seed=100 * n + count % 97)
+            ins = arena_inputs(comms, count, in_dt, seed=100 * n + count % 97)
             for out_name in outs_for:
                 for algo in ("ll", "ll2", "oneshot", "twoshot", "auto"):
                     for op, scale in (reds if count < 100000 else reds[:2]):
-                        a = check_all_reduce(torch, coll, comms, streams, ins, count, in_name, out_name, algo, op, scale,
+                        a = check_all_reduce(torch, coll, group, ins, count, in_name, out_name, algo, op, scale,
                                              f"all_reduce n={n} count={count} {in_name}->{out_name} {algo} op={op} scale={scale}")
                         seen.add(a)
                         if algo == "auto":
@@ -185,9 +109,9 @@ def test_all_reduce_grid(torch_cuda, coll_mod, group):
     if n <= 3:
         # the auto choice changes at the size bounds: LL up to 512 KiB per rank, then LL2 up to 512 KiB * N (same types), then two-shot
         for in_name, out_name in pairs:
-            ll = R.LL_ONESHOT_MAX_BYTES // R.esize(dt(torch, in_name))
-            e = R.vec_elems(dt(torch, in_name))
-            got = [auto[(in_name, out_name, k)] for k in bound_counts(dt(torch, in_name), n)]
+            ll = R.LL_ONESHOT_MAX_BYTES // R.esize(DTYPES[in_name])
+            e = R.vec_elems(DTYPES[in_name])
+            got = [auto[(in_name, out_name, k)] for k in bound_counts(DTYPES[in_name], n)]
             want = ["ll", "ll2", "ll2", "twoshot"] if in_name == out_name else ["ll", "twoshot", "twoshot", "twoshot"]
             assert got == want, (n, in_name, out_name, ll, e, got)
 
@@ -195,16 +119,15 @@ def test_all_reduce_grid(torch_cuda, coll_mod, group):
 @pytest.mark.parametrize("group", [6, 7], indirect=True)
 def test_all_reduce_odd_rank_counts(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for in_name, out_name in SUBSET[:3]:
-        in_dt = dt(torch, in_name)
+        in_dt = DTYPES[in_name]
         e = R.vec_elems(in_dt)
         for count in (e + 1, 1003, e * (37 * n + 1) + 3):
-            ins = inputs(torch, comms, count, in_dt, seed=7 * n + count)
+            ins = arena_inputs(comms, count, in_dt, seed=7 * n + count)
             for algo in ("ll", "ll2", "twoshot"):
                 for op, scale in ((coll.SUM, 0.1), (coll.AVG, 1.0)):
-                    check_all_reduce(torch, coll, comms, streams, ins, count, in_name, out_name, algo, op, scale,
+                    check_all_reduce(torch, coll, group, ins, count, in_name, out_name, algo, op, scale,
                                      f"all_reduce n={n} count={count} {in_name}->{out_name} {algo} op={op}")
             release(comms, ins)
 
@@ -214,14 +137,13 @@ def test_all_reduce_in_place_mixed_sizes(torch_cuda, coll_mod, group):
     """In place, one-shot and two-shot Lamport and two-shot alternating with growing and shrinking ragged counts: the stale-slot
     clearing must follow, and every result is still bit-exact."""
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     seq = [("ll", 4099, "bfloat16"), ("ll2", 1003, "bfloat16"), ("twoshot", 8 * (37 * n + 1) + 3, "bfloat16"), ("ll", 9, "float32"),
            ("ll2", 70001, "float16"), ("twoshot", 1003, "float32"), ("ll2", 17, "bfloat16"), ("ll", 1003, "float16"), ("ll2", 4099, "float32")]
     for it, (algo, count, name) in enumerate(seq):
-        bufs = inputs(torch, comms, count, dt(torch, name), seed=it)
+        bufs = arena_inputs(comms, count, DTYPES[name], seed=it)
         xs = [b.clone() for b in bufs]
-        check_all_reduce(torch, coll, comms, streams, bufs, count, name, name, algo, coll.AVG, 1.0, f"in place #{it} n={n} {algo} {name} count={count}",
+        check_all_reduce(torch, coll, group, bufs, count, name, name, algo, coll.AVG, 1.0, f"in place #{it} n={n} {algo} {name} count={count}",
                          outs=bufs, xs=xs)
         release(comms, bufs)
 
@@ -230,10 +152,9 @@ def test_all_reduce_in_place_mixed_sizes(torch_cuda, coll_mod, group):
 def test_all_reduce_staged_chunks(torch_cuda, coll_mod, group):
     """Buffers outside the arena: the two-shot runs once per staging chunk, the last one ragged, and slices come from each chunk."""
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for in_name, out_name, nchunks in (("bfloat16", "bfloat16", 1), ("float32", "bfloat16", 2)):
-        in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+        in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
         chunk = R.staged_chunk(R.esize(in_dt), R.esize(out_dt), n, "all_reduce")
         assert chunk == (16 << 20 if in_name == "bfloat16" else 8 << 20)
         count = nchunks * chunk + 1003
@@ -243,10 +164,10 @@ def test_all_reduce_staged_chunks(torch_cuda, coll_mod, group):
             poison(outs)
             before = algo_snapshot(comms)
             st0 = [c.stats()["staged_calls"] for c in comms]
-            run_all(torch, comms, streams, lambda r, c, st: (c.set_algo("auto"), c.all_reduce(xs[r], outs[r], scale=scale, op=op, stream=st)))
+            group.run(lambda r, c, st: (c.set_algo("auto"), c.all_reduce(xs[r], outs[r], scale=scale, op=op, stream=st)))
             assert ran(comms, before) == {"twoshot": nchunks + 1}
             assert [c.stats()["staged_calls"] - s for c, s in zip(comms, st0)] == [1] * n
-            want = R.ref_reduce(xs, ("staged", n, R.vec_elems(in_dt), count, chunk), scale_of(coll, op, scale, n), out_dt)
+            want = R.ref_reduce(xs, ("staged", n, R.vec_elems(in_dt), count, chunk), R.scale_of(coll, op, scale, n), out_dt)
             for r in range(n):
                 R.assert_same(outs[r], want, f"staged all_reduce {in_name}->{out_name} count={count} op={op} rank {r}")
 
@@ -255,31 +176,30 @@ def test_all_reduce_staged_chunks(torch_cuda, coll_mod, group):
 @pytest.mark.parametrize("group", [2, 3, 5], indirect=True)
 def test_reduce_scatter_grid(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     pairs = PAIRS if n <= 3 else SUBSET
     for in_name in ("float32", "bfloat16", "float16"):
-        in_dt = dt(torch, in_name)
+        in_dt = DTYPES[in_name]
         e = R.vec_elems(in_dt)
         ll = R.LL_ONESHOT_MAX_BYTES // R.esize(in_dt)
         for count in (e, 37 * e, ll, ll + e):
-            ins = inputs(torch, comms, count * n, in_dt, seed=count + n)
+            ins = arena_inputs(comms, count * n, in_dt, seed=count + n)
             for i_, out_name in pairs:
                 if i_ != in_name:
                     continue
-                out_dt = dt(torch, out_name)
+                out_dt = DTYPES[out_name]
                 outs = [c.empty(count, out_dt) for c in comms]
                 for algo in ("ll", "twoshot"):
                     for op, scale in ((coll.SUM, 1.0), (coll.SUM, 0.1), (coll.AVG, 1.0)):
                         poison(outs)
                         before = algo_snapshot(comms)
-                        run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.reduce_scatter(ins[r], outs[r], scale=scale, op=op, stream=st)))
+                        group.run(lambda r, c, st: (c.set_algo(algo), c.reduce_scatter(ins[r], outs[r], scale=scale, op=op, stream=st)))
                         a = next(iter(ran(comms, before)))
                         assert a == ("ll" if algo == "ll" and count * R.esize(in_dt) <= R.LL_ONESHOT_MAX_BYTES else "twoshot"), (algo, count, a)
                         for r in range(n):
                             xs = [x[r * count:(r + 1) * count] for x in ins]
                             order = list(range(n)) if a == "ll" else ("rotate", r)
-                            R.assert_same(outs[r], R.ref_reduce(xs, order, scale_of(coll, op, scale, n), out_dt),
+                            R.assert_same(outs[r], R.ref_reduce(xs, order, R.scale_of(coll, op, scale, n), out_dt),
                                           f"reduce_scatter n={n} count={count} {in_name}->{out_name} {algo} ran {a} op={op} scale={scale} rank {r}")
                 release(comms, outs)
             release(comms, ins)
@@ -288,17 +208,16 @@ def test_reduce_scatter_grid(torch_cuda, coll_mod, group):
 @pytest.mark.parametrize("group", [3], indirect=True)
 def test_reduce_scatter_staged_two_chunks(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for in_name, out_name in (("bfloat16", "bfloat16"), ("float32", "float16")):
-        in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+        in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
         chunk = R.staged_chunk(R.esize(in_dt), R.esize(out_dt), n, "reduce_scatter")
         count = chunk + 37 * R.vec_elems(in_dt)
         xs = R.gen_inputs(n, count * n, in_dt, seed=9)
         outs = [torch.empty(count, dtype=out_dt, device="cuda") for _ in comms]
         poison(outs)
         before = algo_snapshot(comms)
-        run_all(torch, comms, streams, lambda r, c, st: (c.set_algo("auto"), c.reduce_scatter(xs[r], outs[r], scale=0.1, op=coll.AVG, stream=st)))
+        group.run(lambda r, c, st: (c.set_algo("auto"), c.reduce_scatter(xs[r], outs[r], scale=0.1, op=coll.AVG, stream=st)))
         assert ran(comms, before) == {"twoshot": 2}
         for r in range(n):
             R.assert_same(outs[r], R.ref_reduce([x[r * count:(r + 1) * count] for x in xs], ("rotate", r), R.avg_scale(0.1, n), out_dt),
@@ -309,22 +228,21 @@ def test_reduce_scatter_staged_two_chunks(torch_cuda, coll_mod, group):
 @pytest.mark.parametrize("group", [3, 5], indirect=True)
 def test_reduce_every_root(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     pairs = PAIRS if n <= 3 else SUBSET
     for in_name, out_name in pairs:
-        in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+        in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
         e = R.vec_elems(in_dt)
         for count in (1003, e * (37 * n + 1) + 3):
-            ins = inputs(torch, comms, count, in_dt, seed=count * 3 + n)
+            ins = arena_inputs(comms, count, in_dt, seed=count * 3 + n)
             outs = [c.empty(count, out_dt) for c in comms]
             for root in range(n):
                 for op, scale in ((coll.SUM, 0.1), (coll.AVG, 1.0)):
                     poison(outs)
                     untouched = outs[0].view(torch.uint8).clone()
-                    run_all(torch, comms, streams, lambda r, c, st: c.reduce(ins[r], outs[r], root=root, scale=scale, op=op, stream=st))
+                    group.run(lambda r, c, st: c.reduce(ins[r], outs[r], root=root, scale=scale, op=op, stream=st))
                     what = f"reduce n={n} root={root} count={count} {in_name}->{out_name} op={op}"
-                    R.assert_same(outs[root], R.ref_reduce(ins, list(range(n)), scale_of(coll, op, scale, n), out_dt), what)
+                    R.assert_same(outs[root], R.ref_reduce(ins, list(range(n)), R.scale_of(coll, op, scale, n), out_dt), what)
                     for r in range(n):
                         if r != root:
                             assert torch.equal(outs[r].view(torch.uint8), untouched), f"{what}: rank {r}'s recv was written"
@@ -335,7 +253,7 @@ def test_reduce_every_root(torch_cuda, coll_mod, group):
         outs = [torch.empty(count, dtype=torch.bfloat16, device="cuda") for _ in comms]
         poison(outs)
         untouched = outs[0].view(torch.uint8).clone()
-        run_all(torch, comms, streams, lambda r, c, st: c.reduce(xs[r], outs[r], root=2, scale=0.1, stream=st))
+        group.run(lambda r, c, st: c.reduce(xs[r], outs[r], root=2, scale=0.1, stream=st))
         R.assert_same(outs[2], R.ref_reduce(xs, [0, 1, 2], 0.1, torch.bfloat16), "staged reduce root 2")
         assert torch.equal(outs[0].view(torch.uint8), untouched) and torch.equal(outs[1].view(torch.uint8), untouched)
 
@@ -351,28 +269,27 @@ def test_data_movement(torch_cuda, coll_mod, group):
     payloads included) with the identity epilogue. The Lamport path rewrites a word equal to its empty-slot marker, so identity copies
     force the barrier-based kernels, as Comm.bit_exact does (test_coll_fp8_numerics_gpu.py checks the Lamport identity model)."""
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for in_name, out_name, scale in MOVES:
-        in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+        in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
         ident = in_name == out_name and scale == 1.0
         e = R.vec_elems(in_dt)
         mv = lambda x: R.ref_move(x, scale, out_dt, ident)
         tag = f"n={n} {in_name}->{out_name} scale={scale}"
         big = ((1 << 20) // R.esize(in_dt)) + 5 * e                       # >= 1 MiB per rank: the copy-engine ring for the identity
         for count in (37 * e, big):
-            src = inputs(torch, comms, count * n, in_dt, seed=count + 31 * n)
+            src = arena_inputs(comms, count * n, in_dt, seed=count + 31 * n)
             for algo in (("twoshot",) if ident else ("auto", "ll", "twoshot")):
                 bulk0 = [c.stats()["bulk_launches"] for c in comms]
                 ag = [c.empty(count * n, out_dt) for c in comms]
                 poison(ag)
-                run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.all_gather(src[r][:count], ag[r], scale=scale, stream=st)))
+                group.run(lambda r, c, st: (c.set_algo(algo), c.all_gather(src[r][:count], ag[r], scale=scale, stream=st)))
                 want = torch.cat([mv(x[:count]) for x in src])
                 for r in range(n):
                     R.assert_same(ag[r], want, f"all_gather {tag} count={count} {algo} rank {r}", nan_payloads=ident)
                 a2a = [c.empty(count * n, out_dt) for c in comms]
                 poison(a2a)
-                run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.all_to_all(src[r], a2a[r], scale=scale, stream=st)))
+                group.run(lambda r, c, st: (c.set_algo(algo), c.all_to_all(src[r], a2a[r], scale=scale, stream=st)))
                 for r in range(n):
                     want = torch.cat([mv(src[q][r * count:(r + 1) * count]) for q in range(n)])
                     R.assert_same(a2a[r], want, f"all_to_all {tag} count={count} {algo} rank {r}", nan_payloads=ident)
@@ -386,7 +303,7 @@ def test_data_movement(torch_cuda, coll_mod, group):
                     bc = [c.empty(bcount, out_dt) for c in comms]
                     poison(bc)
                     bulk0 = [c.stats()["bulk_launches"] for c in comms]
-                    run_all(torch, comms, streams, lambda r, c, st: c.broadcast(src[r][:bcount], bc[r], root=root, scale=scale, stream=st))
+                    group.run(lambda r, c, st: c.broadcast(src[r][:bcount], bc[r], root=root, scale=scale, stream=st))
                     for r in range(n):
                         R.assert_same(bc[r], mv(src[root][:bcount]), f"broadcast {tag} count={bcount} root={root} rank {r}", nan_payloads=ident)
                     if ident and bcount == big:
@@ -397,12 +314,12 @@ def test_data_movement(torch_cuda, coll_mod, group):
         hidden = 8 * e
         rows = [[(3 * s + 5 * d) % 7 for d in range(n)] for s in range(n)]
         cap = max(max(sum(rows[s]) for s in range(n)), max(sum(rows[s][d] for s in range(n)) for d in range(n))) + 1
-        send = inputs(torch, comms, cap * hidden, in_dt, seed=77 + n)
+        send = arena_inputs(comms, cap * hidden, in_dt, seed=77 + n)
         recv = [c.empty(cap * hidden, out_dt) for c in comms]
         poison(recv)
         send_off = [[sum(rows[s][:d]) for d in range(n)] for s in range(n)]
         recv_off = [[sum(rows[x][d] for x in range(s)) for s in range(n)] for d in range(n)]
-        run_all(torch, comms, streams, lambda r, c, st: c.all_to_all_v(send[r], recv[r], hidden, rows[r], send_off[r], [recv_off[d][r] for d in range(n)],
+        group.run(lambda r, c, st: c.all_to_all_v(send[r], recv[r], hidden, rows[r], send_off[r], [recv_off[d][r] for d in range(n)],
                                                                        scale=scale, stream=st))
         for d in range(n):
             for s in range(n):
@@ -415,10 +332,9 @@ def test_data_movement(torch_cuda, coll_mod, group):
 @pytest.mark.parametrize("group", [3], indirect=True)
 def test_data_movement_staged(torch_cuda, coll_mod, group):
     torch = torch_cuda
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for in_name, out_name, scale in (MOVES[0], MOVES[3]):
-        in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+        in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
         ident = scale == 1.0
         mv = lambda x: R.ref_move(x, scale, out_dt, ident)
         e = R.vec_elems(in_dt)
@@ -426,12 +342,12 @@ def test_data_movement_staged(torch_cuda, coll_mod, group):
         xs = R.gen_inputs(n, count * n, in_dt, seed=21)
         st0 = [c.stats()["staged_calls"] for c in comms]
         ag = [torch.empty(count * n, dtype=out_dt, device="cuda") for _ in comms]
-        run_all(torch, comms, streams, lambda r, c, st: (c.set_algo("twoshot"), c.all_gather(xs[r][:count], ag[r], scale=scale, stream=st)))
+        group.run(lambda r, c, st: (c.set_algo("twoshot"), c.all_gather(xs[r][:count], ag[r], scale=scale, stream=st)))
         for r in range(n):
             R.assert_same(ag[r], torch.cat([mv(x[:count]) for x in xs]), f"staged all_gather {in_name}->{out_name} rank {r}", nan_payloads=ident)
         del ag
         a2a = [torch.empty(count * n, dtype=out_dt, device="cuda") for _ in comms]
-        run_all(torch, comms, streams, lambda r, c, st: c.all_to_all(xs[r], a2a[r], scale=scale, stream=st))
+        group.run(lambda r, c, st: c.all_to_all(xs[r], a2a[r], scale=scale, stream=st))
         for r in range(n):
             R.assert_same(a2a[r], torch.cat([mv(xs[q][r * count:(r + 1) * count]) for q in range(n)]), f"staged all_to_all {in_name}->{out_name} rank {r}",
                           nan_payloads=ident)
@@ -439,7 +355,7 @@ def test_data_movement_staged(torch_cuda, coll_mod, group):
         bcount = R.staged_chunk(R.esize(in_dt), R.esize(out_dt), n, "broadcast") + 1003
         bc = [torch.empty(bcount, dtype=out_dt, device="cuda") for _ in comms]
         src = [x.repeat(2)[:bcount] if x.numel() < bcount else x[:bcount] for x in xs]
-        run_all(torch, comms, streams, lambda r, c, st: c.broadcast(src[r], bc[r], root=1, scale=scale, stream=st))
+        group.run(lambda r, c, st: c.broadcast(src[r], bc[r], root=1, scale=scale, stream=st))
         for r in range(n):
             R.assert_same(bc[r], mv(src[1]), f"staged broadcast {in_name}->{out_name} rank {r}", nan_payloads=ident)
         del bc
@@ -455,8 +371,7 @@ def test_grid_stride_many_passes(torch_cuda, coll_mod, group, shape):
     """One CTA of 128 threads (or a cap of two CTAs): every grid-stride loop runs many passes and ends on a partial unroll. The
     communicators are destroyed afterwards, so the launch shapes do not leak into other tests."""
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for c in comms:
         if shape == "one_cta":
             c.set_launch_shape("p2p", max_ctas=1, threads=128)
@@ -464,32 +379,32 @@ def test_grid_stride_many_passes(torch_cuda, coll_mod, group, shape):
         else:
             c.set_max_ctas(2)
     for in_name, out_name in (("bfloat16", "bfloat16"), ("float32", "bfloat16"), ("float16", "float32")):
-        in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+        in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
         e = R.vec_elems(in_dt)
         for count in (1003, e * (37 * n + 1) + 3, 100003):
-            ins = inputs(torch, comms, count, in_dt, seed=count)
+            ins = arena_inputs(comms, count, in_dt, seed=count)
             for algo in ("ll", "ll2", "oneshot", "twoshot"):
-                check_all_reduce(torch, coll, comms, streams, ins, count, in_name, out_name, algo, coll.SUM, 0.1, f"{shape} all_reduce {in_name}->{out_name} {count} {algo}")
+                check_all_reduce(torch, coll, group, ins, count, in_name, out_name, algo, coll.SUM, 0.1, f"{shape} all_reduce {in_name}->{out_name} {count} {algo}")
             red = [c.empty(count, out_dt) for c in comms]
-            run_all(torch, comms, streams, lambda r, c, st: c.reduce(ins[r], red[r], root=1, scale=0.1, stream=st))
+            group.run(lambda r, c, st: c.reduce(ins[r], red[r], root=1, scale=0.1, stream=st))
             R.assert_same(red[1], R.ref_reduce(ins, list(range(n)), 0.1, out_dt), f"{shape} reduce {in_name}->{out_name} {count}")
             bc = [c.empty(count, out_dt) for c in comms]
-            run_all(torch, comms, streams, lambda r, c, st: c.broadcast(ins[r], bc[r], root=2, scale=0.1, stream=st))
+            group.run(lambda r, c, st: c.broadcast(ins[r], bc[r], root=2, scale=0.1, stream=st))
             for r in range(n):
                 R.assert_same(bc[r], R.ref_move(ins[2], 0.1, out_dt, False), f"{shape} broadcast {in_name}->{out_name} {count} rank {r}")
             release(comms, bc, red, ins)
         rcount = 3001 * e
-        ins = inputs(torch, comms, rcount * n, in_dt, seed=3)
+        ins = arena_inputs(comms, rcount * n, in_dt, seed=3)
         outs = [c.empty(rcount, out_dt) for c in comms]
         for algo in ("ll", "twoshot"):
             before = algo_snapshot(comms)
-            run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.reduce_scatter(ins[r], outs[r], scale=0.1, stream=st)))
+            group.run(lambda r, c, st: (c.set_algo(algo), c.reduce_scatter(ins[r], outs[r], scale=0.1, stream=st)))
             a = next(iter(ran(comms, before)))
             for r in range(n):
                 xs = [x[r * rcount:(r + 1) * rcount] for x in ins]
                 R.assert_same(outs[r], R.ref_reduce(xs, list(range(n)) if a == "ll" else ("rotate", r), 0.1, out_dt), f"{shape} reduce_scatter {algo} rank {r}")
             ag = [c.empty(rcount * n, out_dt) for c in comms]
-            run_all(torch, comms, streams, lambda r, c, st: (c.set_algo(algo), c.all_gather(ins[r][:rcount], ag[r], scale=0.1, stream=st)))
+            group.run(lambda r, c, st: (c.set_algo(algo), c.all_gather(ins[r][:rcount], ag[r], scale=0.1, stream=st)))
             for r in range(n):
                 R.assert_same(ag[r], torch.cat([R.ref_move(x[:rcount], 0.1, out_dt, False) for x in ins]), f"{shape} all_gather {algo} rank {r}")
             release(comms, ag)
@@ -501,12 +416,12 @@ def test_one_rank_all_ops(torch_cuda, coll_mod):
     """nranks == 1: every op is the copy epilogue. The identity is a bit copy at every size (-0 and NaN payloads kept; in place it is
     a no-op; from 1 MiB the copy engine moves it); a cast or a scale is round((0 + x) * scale) in the vector body and the tail alike."""
     torch, coll = torch_cuda, coll_mod
-    (c,) = coll.Comm.init_all([0], arena_mb=96, timeout_ms=60000)
-    try:
+    with Group(torch, coll, 1, arena_mb=96, timeout_ms=60000) as g:
+        c = g.comms[0]
         cases = [("bfloat16", "bfloat16", 1.0), ("float32", "float32", 1.0), ("float16", "float16", 1.0), ("bfloat16", "float32", 1.0),
                  ("float32", "bfloat16", 1.0), ("float16", "float16", 0.1), ("float32", "float8_e4m3fn", 0.1)]
         for in_name, out_name, scale in cases:
-            in_dt, out_dt = dt(torch, in_name), dt(torch, out_name)
+            in_dt, out_dt = DTYPES[in_name], DTYPES[out_name]
             ident = in_name == out_name and scale == 1.0
             e = R.vec_elems(in_dt)
             for count in (1, e + 3, (1 << 20) + 3, (1 << 20) + e):
@@ -543,9 +458,6 @@ def test_one_rank_all_ops(torch_cuda, coll_mod):
                     if where == "arena":
                         c.release(src)
         c.check_async_error()
-    finally:
-        torch.cuda.synchronize()
-        c.destroy()
 
 
 # ------------------------------------------------------------------------------------------------- generic kernel
@@ -570,13 +482,12 @@ def _generic_ref(torch, coll, xs, op):
 @pytest.mark.parametrize("group", [3, 5], indirect=True)
 def test_generic_kernel(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     g = torch.Generator(device="cuda").manual_seed(n)
     cases = [(name, op) for name in ("float32", "float16", "bfloat16") for op in (coll.MIN, coll.MAX, coll.PROD)]
     cases += [("int8", coll.SUM), ("uint8", coll.SUM), ("int32", coll.SUM), ("float64", coll.SUM), ("int32", coll.MIN)]
     for name, op in cases:
-        t = dt(torch, name)
+        t = DTYPES[name]
         e = 16 // R.esize(t)
         for count in (1003, e * (37 * n + 1) + 3):
             if t.is_floating_point and t != torch.float64:
@@ -598,20 +509,20 @@ def test_generic_kernel(torch_cuda, coll_mod, group):
             what = f"generic n={n} {name} op={op} count={count}"
             outs = [c.empty(count, t) for c in comms]
             gen0 = [c.stats()["generic_launches"] for c in comms]
-            run_all(torch, comms, streams, lambda r, c, st: c.all_reduce(ins[r], outs[r], op=op, stream=st))
+            group.run(lambda r, c, st: c.all_reduce(ins[r], outs[r], op=op, stream=st))
             for r in range(n):
                 R.assert_same(outs[r], want, f"{what} all_reduce rank {r}")
             assert all(c.stats()["generic_launches"] == g0 + 1 for c, g0 in zip(comms, gen0))
             for root in (0, n - 1):
                 poison(outs)
                 untouched = outs[0].view(torch.uint8).clone()
-                run_all(torch, comms, streams, lambda r, c, st: c.reduce(ins[r], outs[r], root=root, op=op, stream=st))
+                group.run(lambda r, c, st: c.reduce(ins[r], outs[r], root=root, op=op, stream=st))
                 R.assert_same(outs[root], want, f"{what} reduce root {root}")
                 assert all(torch.equal(outs[r].view(torch.uint8), untouched) for r in range(n) if r != root)
             release(comms, outs)
             rc = (count // n) // e * e
             rs = [c.empty(rc, t) for c in comms]
-            run_all(torch, comms, streams, lambda r, c, st: c.reduce_scatter(ins[r][:rc * n], rs[r], op=op, stream=st))
+            group.run(lambda r, c, st: c.reduce_scatter(ins[r][:rc * n], rs[r], op=op, stream=st))
             for r in range(n):
                 R.assert_same(rs[r], want[r * rc:(r + 1) * rc], f"{what} reduce_scatter rank {r}")
             # a reduce-scatter block must be whole 16-byte vectors (the generic kernel has no per-block tail): refused before anything
@@ -619,7 +530,7 @@ def test_generic_kernel(torch_cuda, coll_mod, group):
             st0 = comms[0].stats()
             with pytest.raises(coll.B200CollError) as err:
                 comms[0].reduce_scatter(ins[0], ins[0][:rc + 1], op=op)
-            assert err.value.code == 4 and comms[0].stats() == st0
+            assert err.value.code == coll.INVALID_ARGUMENT and comms[0].stats() == st0
             release(comms, rs, ins)
 
 
@@ -631,10 +542,10 @@ def test_multi_gpu_two_shot_and_nvls(torch_cuda, coll_mod):
     n = torch.cuda.device_count()
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
-    comms = coll.Comm.init_all(list(range(n)), arena_mb=256, timeout_ms=60000)
-    try:
+    with Group(torch, coll, n, devices=list(range(n)), arena_mb=256, timeout_ms=60000) as g:
+        comms = g.comms
         for name in ("bfloat16", "float32"):
-            t = dt(torch, name)
+            t = DTYPES[name]
             e = R.vec_elems(t)
             count = e * (4099 * n + 1) + 3
             xs = R.gen_inputs(n, count, t, seed=n)
@@ -679,8 +590,3 @@ def test_multi_gpu_two_shot_and_nvls(torch_cuda, coll_mod):
                     tol = ulp + n * x64.abs().max(0).values * 2.0 ** -22
                     err = (got[:tail].double() - ref).abs()
                     assert bool((err[fin] <= tol[fin]).all()), f"{what}: max error {float((err[fin] - tol[fin]).max())} over tolerance"
-    finally:
-        for r in range(n):
-            torch.cuda.synchronize(r)
-        for c in comms:
-            c.destroy()

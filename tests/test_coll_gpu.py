@@ -7,36 +7,11 @@ import sys
 
 import pytest
 
+from tests.coll_gpu_harness import PERF, ROOT, coll_mod, group_fixture, run_perf, torch_cuda  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PERF = os.path.join(ROOT, "build", "b200coll_perf")
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch
-
-
-@pytest.fixture(scope="module")
-def coll_mod(coll_lib):
-    from container_engine_accelerators_b200.ops import coll
-    coll.load()          # raises if the .so is missing: GPU tests must never pass on a fallback
-    return coll
-
-
-@pytest.fixture
-def group(torch_cuda, coll_mod, request):
-    n = getattr(request, "param", 2)
-    comms = coll_mod.Comm.init_all([0] * n, arena_mb=96)
-    streams = [torch_cuda.cuda.Stream() for _ in comms]
-    yield comms, streams
-    torch_cuda.cuda.synchronize()
-    for c in comms:
-        c.destroy()
+group = group_fixture(2, arena_mb=96)
 
 
 def fill(torch, comms, count, dtype):
@@ -47,14 +22,6 @@ def fill(torch, comms, count, dtype):
         srcs.append(t)
     torch.cuda.synchronize()
     return srcs
-
-
-def run_all(torch, comms, streams, fn):
-    for r, c in enumerate(comms):
-        fn(r, c, streams[r])
-    torch.cuda.synchronize()
-    for c in comms:
-        c.check_async_error()
 
 
 def test_self_check_and_arena_tensor_aliasing(torch_cuda, coll_mod):
@@ -82,13 +49,13 @@ def test_self_check_and_arena_tensor_aliasing(torch_cuda, coll_mod):
 @pytest.mark.parametrize("count", [8, 1000, 1 << 15])
 def test_all_reduce_matches_fp32_reference(torch_cuda, group, algo, count):
     torch = torch_cuda
-    comms, streams = group
+    comms = group.comms
     srcs = fill(torch, comms, count, torch.bfloat16)
     dsts = [c.empty(count, torch.bfloat16) for c in comms]
     want = sum(s.float() for s in srcs)
     for c in comms:
         c.set_algo(algo)
-    run_all(torch, comms, streams, lambda r, c, st: c.all_reduce(srcs[r], dsts[r], stream=st))
+    group.run(lambda r, c, st: c.all_reduce(srcs[r], dsts[r], stream=st))
     for d in dsts:
         assert torch.equal(d.float(), want)
     for a, b in zip(dsts, dsts[1:]):
@@ -98,14 +65,14 @@ def test_all_reduce_matches_fp32_reference(torch_cuda, group, algo, count):
 @pytest.mark.parametrize("group", [4], indirect=True)
 def test_in_place_and_repeated_launches_rotate_lamport_buffers(torch_cuda, group):
     torch = torch_cuda
-    comms, streams = group
+    comms = group.comms
     for it, (algo, count) in enumerate([("ll", 4096), ("ll2", 64), ("ll", 9000), ("ll2", 70001), ("ll2", 16), ("ll", 4096), ("ll2", 4096), ("ll", 128), ("ll", 128)]):
         # shrinking/growing sizes and alternating one-/two-shot Lamport kernels: stale-slot clearing (lo and hi halves) must follow
         for c in comms:
             c.set_algo(algo)
         srcs = fill(torch, comms, count, torch.bfloat16)
         want = sum(s.float() for s in srcs)
-        run_all(torch, comms, streams, lambda r, c, st: c.all_reduce(srcs[r], stream=st))
+        group.run(lambda r, c, st: c.all_reduce(srcs[r], stream=st))
         for s in srcs:
             assert torch.equal(s.float(), want), f"iteration {it} count {count}"
 
@@ -114,7 +81,7 @@ def test_in_place_and_repeated_launches_rotate_lamport_buffers(torch_cuda, group
 @pytest.mark.parametrize("in_dt,out_dt,scale", [("bfloat16", "float32", 0.5), ("float32", "bfloat16", 0.25), ("float16", "float16", 2.0), ("bfloat16", "float8_e4m3fn", 0.125)])
 def test_fused_scale_cast_epilogue(torch_cuda, group, in_dt, out_dt, scale):
     torch = torch_cuda
-    comms, streams = group
+    comms = group.comms
     count = 4096
     srcs = fill(torch, comms, count, getattr(torch, in_dt))
     dsts = [c.empty(count, getattr(torch, out_dt)) for c in comms]
@@ -122,7 +89,7 @@ def test_fused_scale_cast_epilogue(torch_cuda, group, in_dt, out_dt, scale):
     for algo in ("ll", "twoshot"):
         for c in comms:
             c.set_algo(algo)
-        run_all(torch, comms, streams, lambda r, c, st: c.all_reduce(srcs[r], dsts[r], scale=scale, stream=st))
+        group.run(lambda r, c, st: c.all_reduce(srcs[r], dsts[r], scale=scale, stream=st))
         for d in dsts:
             if out_dt == "float8_e4m3fn":
                 assert torch.allclose(d.float(), want.to(torch.float8_e4m3fn).float())
@@ -134,23 +101,23 @@ def test_fused_scale_cast_epilogue(torch_cuda, group, in_dt, out_dt, scale):
 @pytest.mark.parametrize("algo", ["ll", "twoshot"])
 def test_all_gather_reduce_scatter_all_to_all(torch_cuda, group, algo):
     torch = torch_cuda
-    comms, streams = group
+    comms = group.comms
     n, count = len(comms), 2048
     for c in comms:
         c.set_algo(algo)
     srcs = fill(torch, comms, count, torch.bfloat16)
     gat = [c.empty(count * n, torch.bfloat16) for c in comms]
-    run_all(torch, comms, streams, lambda r, c, st: c.all_gather(srcs[r], gat[r], stream=st))
+    group.run(lambda r, c, st: c.all_gather(srcs[r], gat[r], stream=st))
     for g in gat:
         assert torch.equal(g, torch.cat(srcs))
     big = fill(torch, comms, count * n, torch.bfloat16)
     rs = [c.empty(count, torch.bfloat16) for c in comms]
-    run_all(torch, comms, streams, lambda r, c, st: c.reduce_scatter(big[r], rs[r], stream=st))
+    group.run(lambda r, c, st: c.reduce_scatter(big[r], rs[r], stream=st))
     total = sum(b.float() for b in big)
     for r in range(n):
         assert torch.equal(rs[r].float(), total[r * count:(r + 1) * count])
     a2a = [c.empty(count * n, torch.bfloat16) for c in comms]
-    run_all(torch, comms, streams, lambda r, c, st: c.all_to_all(big[r], a2a[r], stream=st))
+    group.run(lambda r, c, st: c.all_to_all(big[r], a2a[r], stream=st))
     for r in range(n):
         want = torch.cat([big[s][r * count:(r + 1) * count] for s in range(n)])
         assert torch.equal(a2a[r], want)
@@ -161,8 +128,7 @@ def test_copy_engine_path_all_gather_all_to_all_broadcast(torch_cuda, group):
     """Identity epilogue and >= 1 MiB: the payload moves through the cp.async.bulk ring (k_bulk) instead of LDG/STG — all-gather, all-to-all
     and the P2P broadcast, odd chunk counts so the last chunk of a segment is short; bit-exact against plain tensor ops."""
     torch = torch_cuda
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     count = (1 << 20) + 40 * 8                                      # 2 MiB + 640 B per rank: 129 chunks of 16 KiB, the last one short
     srcs = []
     for r, c in enumerate(comms):
@@ -172,17 +138,17 @@ def test_copy_engine_path_all_gather_all_to_all_broadcast(torch_cuda, group):
     torch.cuda.synchronize()
     before = comms[0].stats()["bulk_launches"]
     gat = [c.empty(count * n, torch.bfloat16) for c in comms]
-    run_all(torch, comms, streams, lambda r, c, st: c.all_gather(srcs[r][:count], gat[r], stream=st))
+    group.run(lambda r, c, st: c.all_gather(srcs[r][:count], gat[r], stream=st))
     for g in gat:
         assert torch.equal(g, torch.cat([s[:count] for s in srcs]))
     a2a = [c.empty(count * n, torch.bfloat16) for c in comms]
     for rep in range(2):                                            # twice: the ring's mbarrier phases and the barrier epochs carry over
-        run_all(torch, comms, streams, lambda r, c, st: c.all_to_all(srcs[r], a2a[r], stream=st))
+        group.run(lambda r, c, st: c.all_to_all(srcs[r], a2a[r], stream=st))
         for r in range(n):
             assert torch.equal(a2a[r], torch.cat([srcs[s][r * count:(r + 1) * count] for s in range(n)]))
     for root in range(n):
         outs = [c.empty(count, torch.bfloat16) for c in comms]
-        run_all(torch, comms, streams, lambda r, c, st: c.broadcast(srcs[r][:count], outs[r], root=root, stream=st))
+        group.run(lambda r, c, st: c.broadcast(srcs[r][:count], outs[r], root=root, stream=st))
         for o in outs:
             assert torch.equal(o, srcs[root][:count])
         for c, o in zip(comms, outs):
@@ -214,22 +180,21 @@ def test_broadcast_and_reduce_rooted(torch_cuda, group, count):
     """ncclBroadcast / ncclReduce semantics incl. a count that is not a whole number of 16-byte vectors, every root,
     in-place, and the fused cast/scale epilogue (fp32 reference)."""
     torch = torch_cuda
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     srcs = fill(torch, comms, count, torch.bfloat16)
     for root in range(n):
         outs = [c.empty(count, torch.bfloat16) for c in comms]
         for o in outs:
             o.fill_(55.0)
         torch.cuda.synchronize()
-        run_all(torch, comms, streams, lambda r, c, st: c.broadcast(srcs[r], outs[r], root=root, stream=st))
+        group.run(lambda r, c, st: c.broadcast(srcs[r], outs[r], root=root, stream=st))
         for o in outs:
             assert torch.equal(o, srcs[root]), root
         red = [c.empty(count, torch.float32) for c in comms]
         for o in red:
             o.fill_(55.0)
         torch.cuda.synchronize()
-        run_all(torch, comms, streams, lambda r, c, st: c.reduce(srcs[r], red[r], root=root, scale=0.5, stream=st))   # bf16 in, fp32 out, x0.5 fused
+        group.run(lambda r, c, st: c.reduce(srcs[r], red[r], root=root, scale=0.5, stream=st))   # bf16 in, fp32 out, x0.5 fused
         want = sum(t.float() for t in srcs) * 0.5
         for r in range(n):
             assert torch.equal(red[r], want if r == root else torch.full_like(want, 55.0)), (root, r)
@@ -239,7 +204,7 @@ def test_broadcast_and_reduce_rooted(torch_cuda, group, count):
         b.copy_(torch.arange(count, device="cuda").float() * 0.5 + r)
     torch.cuda.synchronize()
     want = bufs[1].clone() * 2.0
-    run_all(torch, comms, streams, lambda r, c, st: c.broadcast(bufs[r], root=1, scale=2.0, stream=st))
+    group.run(lambda r, c, st: c.broadcast(bufs[r], root=1, scale=2.0, stream=st))
     for b in bufs:
         assert torch.equal(b, want)
     for c in comms:
@@ -250,15 +215,15 @@ def test_broadcast_and_reduce_rooted(torch_cuda, group, count):
 @pytest.mark.parametrize("group", [2], indirect=True)
 def test_rooted_ops_outside_the_arena_are_staged(torch_cuda, group):
     torch = torch_cuda
-    comms, streams = group
+    comms = group.comms
     count = (1 << 20) + 24
     srcs = [(((torch.arange(count, device="cuda") * (r + 2)) % 9) - 4).to(torch.bfloat16) for r in range(len(comms))]
     dsts = [torch.full((count,), 9.0, dtype=torch.bfloat16, device="cuda") for _ in comms]
-    run_all(torch, comms, streams, lambda r, c, st: c.broadcast(srcs[r], dsts[r], root=1, stream=st))
+    group.run(lambda r, c, st: c.broadcast(srcs[r], dsts[r], root=1, stream=st))
     for d in dsts:
         assert torch.equal(d, srcs[1])
     red = [torch.full((count,), 9.0, dtype=torch.bfloat16, device="cuda") for _ in comms]
-    run_all(torch, comms, streams, lambda r, c, st: c.reduce(srcs[r], red[r], root=0, stream=st))
+    group.run(lambda r, c, st: c.reduce(srcs[r], red[r], root=0, stream=st))
     assert torch.equal(red[0].float(), sum(s.float() for s in srcs)) and torch.equal(red[1], torch.full_like(red[1], 9.0))
     assert all(c.stats()["staged_calls"] == 2 for c in comms)
 
@@ -267,7 +232,7 @@ def test_rooted_ops_outside_the_arena_are_staged(torch_cuda, group):
 def test_all_to_all_v_expert_dispatch(torch_cuda, group):
     """Skewed per-peer row counts (MoE dispatch shape): rows land at the offsets the receiver advertised."""
     torch = torch_cuda
-    comms, streams = group
+    comms = group.comms
     n, hidden = len(comms), 256
     rows = [[(3 * s + 5 * d) % 7 for d in range(n)] for s in range(n)]                 # rows[s][d]: s -> d
     send = []
@@ -282,7 +247,7 @@ def test_all_to_all_v_expert_dispatch(torch_cuda, group):
     torch.cuda.synchronize()
     send_off = [[sum(rows[s][:d]) for d in range(n)] for s in range(n)]
     recv_off = [[sum(rows[x][d] for x in range(s)) for s in range(n)] for d in range(n)]  # recv_off[d][s]: where s's rows start at d
-    run_all(torch, comms, streams, lambda r, c, st: c.all_to_all_v(send[r], recv[r], hidden, rows[r], send_off[r], [recv_off[d][r] for d in range(n)], stream=st))
+    group.run(lambda r, c, st: c.all_to_all_v(send[r], recv[r], hidden, rows[r], send_off[r], [recv_off[d][r] for d in range(n)], stream=st))
     for d in range(n):
         for s in range(n):
             got = recv[d][recv_off[d][s] * hidden:(recv_off[d][s] + rows[s][d]) * hidden]
@@ -293,11 +258,11 @@ def test_all_to_all_v_expert_dispatch(torch_cuda, group):
 @pytest.mark.parametrize("group", [2], indirect=True)
 def test_buffers_outside_the_arena_are_staged(torch_cuda, group):
     torch = torch_cuda
-    comms, streams = group
+    comms = group.comms
     count = 1 << 20                                             # 2 MiB > LL limit: must take the staging path
     srcs = [(((torch.arange(count, device="cuda") * (r + 2)) % 9) - 4).to(torch.bfloat16) for r in range(len(comms))]
     dsts = [torch.empty(count, dtype=torch.bfloat16, device="cuda") for _ in comms]
-    run_all(torch, comms, streams, lambda r, c, st: c.all_reduce(srcs[r], dsts[r], stream=st))
+    group.run(lambda r, c, st: c.all_reduce(srcs[r], dsts[r], stream=st))
     want = sum(s.float() for s in srcs)
     for d in dsts:
         assert torch.equal(d.float(), want)
@@ -308,7 +273,7 @@ def test_buffers_outside_the_arena_are_staged(torch_cuda, group):
 def test_cuda_graph_replay(torch_cuda, group):
     """Epochs and Lamport phases live in device memory, so a captured collective replays correctly."""
     torch = torch_cuda
-    comms, streams = group
+    comms = group.comms
     count = 2048
     srcs = fill(torch, comms, count, torch.bfloat16)
     dsts = [c.empty(count, torch.bfloat16) for c in comms]
@@ -319,8 +284,8 @@ def test_cuda_graph_replay(torch_cuda, group):
         graphs = []
         for r, c in enumerate(comms):
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=streams[r]):
-                c.all_reduce(srcs[r], dsts[r], stream=streams[r])
+            with torch.cuda.graph(g, stream=group.streams[r]):
+                c.all_reduce(srcs[r], dsts[r], stream=group.streams[r])
             graphs.append(g)
         for it in range(5):
             for r in range(len(comms)):
@@ -328,7 +293,7 @@ def test_cuda_graph_replay(torch_cuda, group):
             torch.cuda.synchronize()
             want = sum(s.float() for s in srcs)
             for r, g in enumerate(graphs):
-                with torch.cuda.stream(streams[r]):
+                with torch.cuda.stream(group.streams[r]):
                     g.replay()
             torch.cuda.synchronize()
             for d in dsts:
@@ -354,10 +319,7 @@ def test_watchdog_reports_instead_of_hanging(torch_cuda, coll_mod):
 def test_perf_tool_virtual_ranks_zero_errors(torch_cuda, coll_lib):
     assert os.path.exists(PERF), "build/b200coll_perf missing (python -c 'import __graft_entry__ as g; g.build()')"
     for op in ("all_reduce", "all_gather", "reduce_scatter", "alltoall", "broadcast", "reduce"):
-        r = subprocess.run([PERF, "--devs", "0,0,0,0", "--op", op, "-b", "1K", "-e", "1M", "-f", "4", "--iters", "3", "--warmup", "1"], capture_output=True, text=True, timeout=120,
-                           env={**os.environ, "B200COLL_TIMEOUT_MS": "5000"})
-        assert r.returncode == 0, r.stdout + r.stderr
-        assert "errors=0" in r.stdout
+        run_perf(["--op", op, "-b", "1K", "-e", "1M", "-f", "4", "--iters", "3", "--warmup", "1"], "0,0,0,0", env={"B200COLL_TIMEOUT_MS": "5000"}, timeout=120)
 
 
 def test_nccl_tests_names_and_launcher_rank_mode(torch_cuda, coll_lib):
@@ -385,17 +347,13 @@ def test_multi_gpu_procs_nvls(torch_cuda, coll_lib):
         pytest.skip("needs >= 2 GPUs")
     devs = ",".join(str(i) for i in range(n))
     for algo in ("auto", "nvls", "twoshot"):
-        r = subprocess.run([PERF, "--devs", devs, "--procs", "--op", "all_reduce", "--algo", algo, "-b", "1K", "-e", "64M", "-f", "16", "--iters", "3", "--warmup", "1"],
-                           capture_output=True, text=True, timeout=180, env={**os.environ, "B200COLL_TIMEOUT_MS": "5000"})
-        assert r.returncode == 0 and "errors=0" in r.stdout, r.stdout + r.stderr
+        run_perf(["--op", "all_reduce", "--algo", algo, "-b", "1K", "-e", "64M", "-f", "16", "--iters", "3", "--warmup", "1"], devs, procs=True,
+                 env={"B200COLL_TIMEOUT_MS": "5000"}, timeout=180)
     for op in ("all_gather", "alltoall", "broadcast"):     # one process driving every GPU (threads): the copy-engine kernel's shared-memory opt-in is per device
-        r = subprocess.run([PERF, "--devs", devs, "--op", op, "-b", "4M", "-e", "64M", "-f", "16", "--iters", "2", "--warmup", "1"],
-                           capture_output=True, text=True, timeout=180, env={**os.environ, "B200COLL_TIMEOUT_MS": "5000"})
-        assert r.returncode == 0 and "errors=0" in r.stdout, r.stdout + r.stderr
+        run_perf(["--op", op, "-b", "4M", "-e", "64M", "-f", "16", "--iters", "2", "--warmup", "1"], devs, env={"B200COLL_TIMEOUT_MS": "5000"}, timeout=180)
     for op in ("broadcast", "reduce"):                     # multimem.st fan-out / multimem.ld_reduce by the root (N >= 3) or P2P (N == 2)
-        r = subprocess.run([PERF, "--devs", devs, "--procs", "--op", op, "-b", "1K", "-e", "64M", "-f", "16", "--iters", "3", "--warmup", "1"],
-                           capture_output=True, text=True, timeout=180, env={**os.environ, "B200COLL_TIMEOUT_MS": "5000"})
-        assert r.returncode == 0 and "errors=0" in r.stdout, r.stdout + r.stderr
+        run_perf(["--op", op, "-b", "1K", "-e", "64M", "-f", "16", "--iters", "3", "--warmup", "1"], devs, procs=True, env={"B200COLL_TIMEOUT_MS": "5000"},
+                 timeout=180)
 
 
 def test_bench_contract_one_gpu(torch_cuda):
@@ -436,13 +394,13 @@ def test_bench_dumps_the_same_outputs_from_run_to_run(torch_cuda, tmp_path):
 @pytest.mark.parametrize("group", [2], indirect=True)
 def test_all_reduce_from_host_pipelines_copy_and_collective(torch_cuda, group):
     torch = torch_cuda
-    comms, streams = group
+    comms = group.comms
     count = (5 << 20) + 1024                                     # several 4 MiB chunks and a ragged tail
     hosts = [(((torch.arange(count) * (r + 2)) % 11) - 5).to(torch.bfloat16).pin_memory() for r in range(len(comms))]
     outs = [c.empty(count, torch.bfloat16) for c in comms]
     for rep in range(3):                                         # staging buffers are reused across calls
         for r, c in enumerate(comms):
-            with torch.cuda.stream(streams[r]):
+            with torch.cuda.stream(group.streams[r]):
                 c.all_reduce_from_host(hosts[r], outs[r], chunk_bytes=4 << 20)
         torch.cuda.synchronize()
         want = sum(h.float() for h in hosts).cuda()
@@ -459,8 +417,7 @@ def test_all_reduce_host_zero_copy_single_chunk_and_pipeline(torch_cuda, group, 
     chunk, staging rings reused and regrown across calls) — against an fp32 reference on data whose sums are not exact in bf16."""
     torch = torch_cuda
     from container_engine_accelerators_b200.parallel import harness
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     gen = harness._gen_expected(torch, "all_reduce", 0, n, 0, "cpu")
     for count in (1 << 12, (1 << 18) + 8, (1 << 19) + 24, (5 << 20) + 13, (9 << 20) + 5):      # one-shot / two-shot Lamport zero-copy, one chunk, 3 and 5 chunks with a ragged tail
         idx = torch.arange(count)
@@ -471,7 +428,7 @@ def test_all_reduce_host_zero_copy_single_chunk_and_pipeline(torch_cuda, group, 
             h_in[r].copy_(ins[r]); h_out[r].fill_(77.0)
         for rep in range(2):
             for r, c in enumerate(comms):
-                c.all_reduce_host(h_in[r], h_out[r], stream=streams[r])
+                c.all_reduce_host(h_in[r], h_out[r], stream=group.streams[r])
             torch.cuda.synchronize()
             want = sum(x.float() for x in ins)
             for r in range(n):
@@ -674,8 +631,7 @@ def test_send_recv_ring_step(torch_cuda, coll_mod, group, nbytes, arena_recv):
     """Grouped send to the right / recv from the left (nccl-tests sendrecv): bytes arrive untouched, for sizes that are not a multiple
     of a vector, in place in the arena or through staging windows smaller than the message; repeated so sequence numbers advance."""
     torch = torch_cuda
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     for c in comms:
         c.set_p2p_window(1 << 20)                   # 3 MiB + 5 B through 1 MiB windows: four chunks, both windows reused
     srcs = [c.empty(nbytes, torch.uint8) for c in comms]
@@ -687,8 +643,8 @@ def test_send_recv_ring_step(torch_cuda, coll_mod, group, nbytes, arena_recv):
         torch.cuda.synchronize()
         with coll_mod.group():
             for r, c in enumerate(comms):
-                c.send(srcs[r], (r + 1) % n, stream=streams[r])
-                c.recv(dsts[r], (r - 1) % n, stream=streams[r])
+                c.send(srcs[r], (r + 1) % n, stream=group.streams[r])
+                c.recv(dsts[r], (r - 1) % n, stream=group.streams[r])
         torch.cuda.synchronize()
         for r, c in enumerate(comms):
             c.check_async_error()
@@ -703,22 +659,22 @@ def test_send_recv_pipeline_handover_and_self(torch_cuda, coll_mod, group):
     """Ungrouped calls: rank 0 sends, rank 1 receives (each blocks its own stream until the other arrives); then the reverse direction
     with another size; send/recv to self inside a group is a local copy."""
     torch = torch_cuda
-    comms, streams = group
+    comms = group.comms
     a = comms[0].empty(1 << 16, torch.float32); a.copy_(torch.arange(1 << 16, device="cuda", dtype=torch.float32))
     b = comms[1].empty(1 << 16, torch.float32); b.zero_()
-    comms[0].send(a, 1, stream=streams[0])
-    comms[1].recv(b, 0, stream=streams[1])
+    comms[0].send(a, 1, stream=group.streams[0])
+    comms[1].recv(b, 0, stream=group.streams[1])
     torch.cuda.synchronize()
     assert torch.equal(a, b)
     back = torch.empty(100, dtype=torch.bfloat16, device="cuda")            # 200 bytes, not in the arena
-    comms[1].send(b[:50].view(torch.bfloat16), 0, stream=streams[1])
-    comms[0].recv(back, 1, stream=streams[0])
+    comms[1].send(b[:50].view(torch.bfloat16), 0, stream=group.streams[1])
+    comms[0].recv(back, 1, stream=group.streams[0])
     torch.cuda.synchronize()
     assert torch.equal(back.view(torch.float32), a[:50])
     mine = torch.empty(1 << 10, dtype=torch.float32, device="cuda")
     with coll_mod.group():
-        comms[0].send(a[:1 << 10], 0, stream=streams[0])
-        comms[0].recv(mine, 0, stream=streams[0])
+        comms[0].send(a[:1 << 10], 0, stream=group.streams[0])
+        comms[0].recv(mine, 0, stream=group.streams[0])
     torch.cuda.synchronize()
     assert torch.equal(mine, a[:1 << 10])
     for c in comms:
@@ -730,8 +686,7 @@ def test_send_recv_irregular_group_and_graph_replay(torch_cuda, coll_mod, group)
     """One group with different sizes per pair and two messages for one pair (second one runs in a follow-up kernel); then a captured
     ring step replayed five times."""
     torch = torch_cuda
-    comms, streams = group
-    n = len(comms)
+    comms, n = group.comms, group.n
     size = lambda s, d: 4096 * (1 + s) + 16 * d
     out = {(s, d): comms[s].empty(size(s, d), torch.uint8) for s in range(n) for d in range(n) if s != d}
     inn = {(s, d): comms[d].empty(size(s, d), torch.uint8) for s in range(n) for d in range(n) if s != d}
@@ -744,10 +699,10 @@ def test_send_recv_irregular_group_and_graph_replay(torch_cuda, coll_mod, group)
         for r, c in enumerate(comms):
             for p in range(n):
                 if p != r:
-                    c.send(out[(r, p)], p, stream=streams[r])
-                    c.recv(inn[(p, r)], p, stream=streams[r])
-        comms[0].send(extra_out, 1, stream=streams[0])                      # a second message 0 -> 1 in the same group
-        comms[1].recv(extra_in, 0, stream=streams[1])
+                    c.send(out[(r, p)], p, stream=group.streams[r])
+                    c.recv(inn[(p, r)], p, stream=group.streams[r])
+        comms[0].send(extra_out, 1, stream=group.streams[0])                      # a second message 0 -> 1 in the same group
+        comms[1].recv(extra_in, 0, stream=group.streams[1])
     torch.cuda.synchronize()
     for k in out:
         assert torch.equal(out[k], inn[k]), k
@@ -759,17 +714,17 @@ def test_send_recv_irregular_group_and_graph_replay(torch_cuda, coll_mod, group)
     graphs = []
     for r, c in enumerate(comms):
         g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g, stream=streams[r]):
+        with torch.cuda.graph(g, stream=group.streams[r]):
             with coll_mod.group():
-                c.send(srcs[r], (r + 1) % n, stream=streams[r])
-                c.recv(dsts[r], (r - 1) % n, stream=streams[r])
+                c.send(srcs[r], (r + 1) % n, stream=group.streams[r])
+                c.recv(dsts[r], (r - 1) % n, stream=group.streams[r])
         graphs.append(g)
     for it in range(5):
         for r in range(n):
             srcs[r].fill_(float(10 * it + r))
         torch.cuda.synchronize()
         for r, g in enumerate(graphs):
-            with torch.cuda.stream(streams[r]):
+            with torch.cuda.stream(group.streams[r]):
                 g.replay()
         torch.cuda.synchronize()
         for r in range(n):

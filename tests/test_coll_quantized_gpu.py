@@ -3,52 +3,15 @@
 Every numeric check is bit for bit against tests/coll_quant_reference.py (per-block amax, IEEE divisions, RNE saturating FP8 pack, one
 multiply to dequantise, rank-order fp32 sum, one rounding); NaN matches NaN at the same position."""
 import ctypes as C
-import os
-import subprocess
 
 import pytest
 
+from container_engine_accelerators_b200.ops.coll import INVALID_ARGUMENT, OUT_OF_MEMORY
 from tests import coll_quant_reference as qr
 from tests.coll_fp_reference import assert_same, avg_scale
+from tests.coll_gpu_harness import DTYPES, Group, assert_nothing_launched, coll_mod, expect_refused, run_perf, torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PERF = os.path.join(ROOT, "build", "b200coll_perf")
-INVALID_ARGUMENT, OUT_OF_MEMORY = 4, 8
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch
-
-
-@pytest.fixture(scope="module")
-def coll_mod(coll_lib):
-    from container_engine_accelerators_b200.ops import coll
-    coll.load()
-    return coll
-
-
-def make_group(torch, coll, n, arena_mb=192):
-    return coll.Comm.init_all([0] * n, arena_mb=arena_mb), [torch.cuda.Stream() for _ in range(n)]
-
-
-def destroy(torch, comms):
-    torch.cuda.synchronize()
-    for c in comms:
-        c.destroy()
-
-
-def run_all(torch, comms, streams, fn):
-    for r, c in enumerate(comms):
-        fn(r, c, streams[r])
-    torch.cuda.synchronize()
-    for c in comms:
-        c.check_async_error()
 
 
 def inputs(torch, comms, count, in_dt, block, seed, arena=True):
@@ -71,8 +34,8 @@ def outputs(torch, comms, numel, dt, arena=True):
     return outs
 
 
-def call(torch, coll, comms, streams, op, ds, outs, block, wire, scale=1.0, red=None, algo=None):
-    red = coll.SUM if red is None else red
+def call(g, op, ds, outs, block, wire, scale=1.0, red=None, algo=None):
+    red = g.coll.SUM if red is None else red
 
     def fn(r, c, st):
         if algo:
@@ -83,7 +46,7 @@ def call(torch, coll, comms, streams, op, ds, outs, block, wire, scale=1.0, red=
             c.reduce_scatter_quantized(ds[r], outs[r], block=block, wire=wire, scale=scale, op=red, stream=st)
         else:
             c.all_reduce_quantized(ds[r], outs[r], block=block, wire=wire, scale=scale, op=red, stream=st)
-    run_all(torch, comms, streams, fn)
+    g.run(fn)
 
 
 def reference(coll, op, xs, block, wire, scale, red, out_dt, rank):
@@ -120,90 +83,74 @@ GRID = [
 ]
 
 
-def _dt(torch, name):
-    return {"bf16": torch.bfloat16, "f16": torch.float16, "f32": torch.float32, "e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}[name]
-
-
 @pytest.mark.parametrize("case", GRID, ids=lambda c: "-".join(str(x) for x in c if x is not None))
 def test_grid_bit_exact(torch_cuda, coll_mod, case):
     torch, coll = torch_cuda, coll_mod
     n, op, algo, in_name, wire_name, out_name, block, nblk = case
-    in_dt, wire, out_dt = _dt(torch, in_name), _dt(torch, wire_name), _dt(torch, out_name)
+    in_dt, wire, out_dt = DTYPES[in_name], DTYPES[wire_name], DTYPES[out_name]
     count = nblk * block * (n if op == "reduce_scatter" else 1)
-    comms, streams = make_group(torch, coll, n)
-    try:
-        xs, ds = inputs(torch, comms, count, in_dt, block, seed=nblk + block)
+    with Group(torch, coll, n, arena_mb=192) as g:
+        xs, ds = inputs(torch, g.comms, count, in_dt, block, seed=nblk + block)
         numel = {"all_gather": count * n, "reduce_scatter": count // n, "all_reduce": count}[op]
         for red, scale in ((coll.SUM, 1.0), (coll.AVG, 0.7)):
             if op == "all_gather" and red == coll.AVG:
                 red = coll.SUM
-            outs = outputs(torch, comms, numel, out_dt)
-            before = [c.stats() for c in comms]
-            call(torch, coll, comms, streams, op, ds, outs, block, wire, scale, red, algo)
-            for r, c in enumerate(comms):
+            outs = outputs(torch, g.comms, numel, out_dt)
+            before = [c.stats() for c in g.comms]
+            call(g, op, ds, outs, block, wire, scale, red, algo)
+            for r, c in enumerate(g.comms):
                 want = reference(coll, op, xs, block, wire, scale, red, out_dt, r)
                 assert_same(outs[r].cpu(), want, f"{case} rank {r} op {red} scale {scale}")
                 st = c.stats()
                 assert st["kernel_launches"] == before[r]["kernel_launches"] + 1
                 used = "copy" if n == 1 else (algo or "oneshot")
                 assert st["algo_calls"][used] == before[r]["algo_calls"][used] + 1, (used, st["algo_calls"])
-    finally:
-        destroy(torch, comms)
 
 
 def test_algorithms_and_reduce_scatter_agree_and_one_rank_is_the_round_trip(torch_cuda, coll_mod):
     torch, coll = torch_cuda, coll_mod
     n, block, count = 3, 64, 64 * 31 * 3
-    comms, streams = make_group(torch, coll, n)
-    try:
-        xs, ds = inputs(torch, comms, count, torch.bfloat16, block, seed=3)
-        one, two = outputs(torch, comms, count, torch.float32), outputs(torch, comms, count, torch.float32)
-        rs = outputs(torch, comms, count // n, torch.float32)
-        call(torch, coll, comms, streams, "all_reduce", ds, one, block, torch.float8_e4m3fn, algo="oneshot")
-        call(torch, coll, comms, streams, "all_reduce", ds, two, block, torch.float8_e4m3fn, algo="twoshot")
-        call(torch, coll, comms, streams, "reduce_scatter", ds, rs, block, torch.float8_e4m3fn)
+    with Group(torch, coll, n, arena_mb=192) as g:
+        xs, ds = inputs(torch, g.comms, count, torch.bfloat16, block, seed=3)
+        one, two = outputs(torch, g.comms, count, torch.float32), outputs(torch, g.comms, count, torch.float32)
+        rs = outputs(torch, g.comms, count // n, torch.float32)
+        call(g, "all_reduce", ds, one, block, torch.float8_e4m3fn, algo="oneshot")
+        call(g, "all_reduce", ds, two, block, torch.float8_e4m3fn, algo="twoshot")
+        call(g, "reduce_scatter", ds, rs, block, torch.float8_e4m3fn)
         m = count // n
         for r in range(n):
             assert_same(one[r].cpu(), one[0].cpu(), f"one-shot rank {r} vs rank 0", nan_payloads=True)
             assert_same(two[r].cpu(), one[0].cpu(), f"two-shot rank {r} vs one-shot", nan_payloads=True)
             assert_same(rs[r].cpu(), one[0][r * m:(r + 1) * m].cpu(), f"reduce-scatter rank {r} vs all-reduce slice", nan_payloads=True)
-    finally:
-        destroy(torch, comms)
-    comms, streams = make_group(torch, coll, 1)
-    try:
-        xs, ds = inputs(torch, comms, 128 * 8, torch.float32, 128, seed=9, arena=False)
-        out = outputs(torch, comms, 128 * 8, torch.float32, arena=False)
-        call(torch, coll, comms, streams, "all_reduce", ds, out, 128, torch.float8_e4m3fn)
+    with Group(torch, coll, 1, arena_mb=192) as g:
+        xs, ds = inputs(torch, g.comms, 128 * 8, torch.float32, 128, seed=9, arena=False)
+        out = outputs(torch, g.comms, 128 * 8, torch.float32, arena=False)
+        call(g, "all_reduce", ds, out, 128, torch.float8_e4m3fn)
         want = qr.quantize(xs[0], 128, torch.float8_e4m3fn)[2]
         assert_same(out[0].cpu(), qr.reduce([want], 1.0, torch.float32), "one rank")
         fin = torch.isfinite(xs[0])
         assert not torch.equal(out[0].cpu()[fin], xs[0][fin]), "one rank must be the round trip, not a copy"
-    finally:
-        destroy(torch, comms)
 
 
 def test_send_outside_the_arena_and_two_shot_fallback(torch_cuda, coll_mod):
     torch, coll = torch_cuda, coll_mod
     n, block, count, wire = 2, 128, 128 * 20 * 2, torch.float8_e5m2
-    comms, streams = make_group(torch, coll, n)
-    try:
-        xs, ds = inputs(torch, comms, count, torch.float16, block, seed=11, arena=False)
-        assert not any(c.is_symmetric(d) for c, d in zip(comms, ds))
+    with Group(torch, coll, n, arena_mb=192) as g:
+        xs, ds = inputs(torch, g.comms, count, torch.float16, block, seed=11, arena=False)
+        assert not any(c.is_symmetric(d) for c, d in zip(g.comms, ds))
         for op, numel in (("all_gather", count * n), ("reduce_scatter", count // n), ("all_reduce", count)):
-            outs = outputs(torch, comms, numel, torch.bfloat16)
-            call(torch, coll, comms, streams, op, ds, outs, block, wire, algo="twoshot")
+            outs = outputs(torch, g.comms, numel, torch.bfloat16)
+            call(g, op, ds, outs, block, wire, algo="twoshot")
             for r in range(n):
                 assert_same(outs[r].cpu(), reference(coll, op, xs, block, wire, 1.0, coll.SUM, torch.bfloat16, r), f"{op} send outside the arena")
         # two-shot pushes into every recv: with recv outside the arena the call runs one-shot
-        outs = outputs(torch, comms, count, torch.bfloat16, arena=False)
-        before = [c.stats()["algo_calls"] for c in comms]
-        call(torch, coll, comms, streams, "all_reduce", ds, outs, block, wire, algo="twoshot")
-        for r, c in enumerate(comms):
+        outs = outputs(torch, g.comms, count, torch.bfloat16, arena=False)
+        before = [c.stats()["algo_calls"] for c in g.comms]
+        call(g, "all_reduce", ds, outs, block, wire, algo="twoshot")
+        for r, c in enumerate(g.comms):
             after = c.stats()["algo_calls"]
             assert after["oneshot"] == before[r]["oneshot"] + 1 and after["twoshot"] == before[r]["twoshot"], after
             assert_same(outs[r].cpu(), reference(coll, "all_reduce", xs, block, wire, 1.0, coll.SUM, torch.bfloat16, r), "fallback")
-    finally:
-        destroy(torch, comms)
 
 
 @pytest.mark.parametrize("algo", ["oneshot", "twoshot"])
@@ -211,13 +158,12 @@ def test_send_outside_the_arena_and_two_shot_fallback(torch_cuda, coll_mod):
 def test_in_place_all_reduce(torch_cuda, coll_mod, algo, dts):
     torch, coll = torch_cuda, coll_mod
     n, block = 4, 32
-    in_dt, out_dt = _dt(torch, dts[0]), _dt(torch, dts[1])
+    in_dt, out_dt = DTYPES[dts[0]], DTYPES[dts[1]]
     count = block * 157
-    comms, streams = make_group(torch, coll, n)
-    try:
-        for c in comms:
+    with Group(torch, coll, n, arena_mb=192) as g:
+        for c in g.comms:
             c.set_max_ctas(3)                                            # few CTAs: many grid-stride iterations per CTA
-        xs, ds = inputs(torch, comms, count, in_dt, block, seed=21)
+        xs, ds = inputs(torch, g.comms, count, in_dt, block, seed=21)
         want = qr.all_reduce(xs, block, torch.float8_e4m3fn, 1.0, out_dt)
 
         def fn(r, c, st):
@@ -227,13 +173,11 @@ def test_in_place_all_reduce(torch_cuda, coll_mod, algo, dts):
                 c.all_reduce_quantized(ds[r], block=block, stream=st)
             else:
                 c.all_reduce_quantized(ds[r], buf, block=block, stream=st)
-        run_all(torch, comms, streams, fn)
-        for r, c in enumerate(comms):
+        g.run(fn)
+        for r, c in enumerate(g.comms):
             got = ds[r] if in_dt == out_dt else ds[r].view(out_dt)
             assert_same(got.cpu(), want, f"in-place {algo} {dts} rank {r}")
             assert c.stats()["algo_calls"][algo] == 1
-    finally:
-        destroy(torch, comms)
 
 
 def _raw(coll, comm, fn, send, recv, count, wire, block, in_dt, out_dt, *extra):
@@ -244,9 +188,8 @@ def _raw(coll, comm, fn, send, recv, count, wire, block, in_dt, out_dt, *extra):
 def test_argument_errors(torch_cuda, coll_mod):
     torch, coll = torch_cuda, coll_mod
     L = coll.load()
-    comms, streams = make_group(torch, coll, 2)
-    try:
-        c = comms[0]
+    with Group(torch, coll, 2, arena_mb=192) as g:
+        c = g.comms[0]
         send = c.empty(4096, torch.bfloat16)
         recv = c.empty(8192, torch.float32)
         s, r = send.data_ptr(), recv.data_ptr()
@@ -280,97 +223,83 @@ def test_argument_errors(torch_cuda, coll_mod):
             ("all-reduce in place, other size", AR, s, s, 2048, E4, 128, BF, F32, (coll.SUM,)),
         ]
         for what, fn, snd, rcv, count, wire, block, i, o, extra in cases:
-            rc = _raw(coll, c, fn, snd, rcv, count, wire, block, i, o, *extra)
-            assert rc == INVALID_ARGUMENT, (what, rc, L.b200collGetLastError().decode())
-            assert L.b200collGetLastError().decode(), what
+            expect_refused(_raw(coll, c, fn, snd, rcv, count, wire, block, i, o, *extra), INVALID_ARGUMENT, what=what)
         with pytest.raises(ValueError):
             c.all_gather_quantized(send, send[:2048])                    # Python refuses overlap before the library call
         with pytest.raises(ValueError):
             c.reduce_scatter_quantized(send, send[:2048])
-        assert all(x == 0 for x in c.stats()["calls"])                   # nothing was counted
-        assert c.stats()["kernel_launches"] == 0
-        for comm in comms:
-            comm.check_async_error()
-    finally:
-        destroy(torch, comms)
+        assert_nothing_launched(c)                                       # nothing was counted
+        g.check_async()
     # the arena cannot hold the scratch: OutOfMemory with a message, nothing counted
-    comms, streams = make_group(torch, coll, 2, arena_mb=4)                # a 4 MiB heap; the scratch needs 8.25 MiB
-    try:
+    with Group(torch, coll, 2, arena_mb=4) as g:                # a 4 MiB heap; the scratch needs 8.25 MiB
         big = torch.zeros(8 << 20, dtype=torch.bfloat16, device="cuda")
         out = torch.empty(8 << 20, dtype=torch.bfloat16, device="cuda")
-        rc = _raw(coll, comms[0], L.b200collAllReduceQuantized, big.data_ptr(), out.data_ptr(), big.numel(), coll.FP8_E4M3, 128, coll.BF16, coll.BF16, coll.SUM)
-        assert rc == OUT_OF_MEMORY and "scratch" in L.b200collGetLastError().decode()
+        rc = _raw(coll, g.comms[0], L.b200collAllReduceQuantized, big.data_ptr(), out.data_ptr(), big.numel(), coll.FP8_E4M3, 128, coll.BF16, coll.BF16, coll.SUM)
+        expect_refused(rc, OUT_OF_MEMORY, "scratch")
         with pytest.raises(coll.B200CollError) as e:
-            comms[1].all_gather_quantized(big, torch.empty(2 * big.numel(), dtype=torch.bfloat16, device="cuda"))
+            g.comms[1].all_gather_quantized(big, torch.empty(2 * big.numel(), dtype=torch.bfloat16, device="cuda"))
         assert e.value.code == OUT_OF_MEMORY
-        assert all(x == 0 for x in comms[0].stats()["calls"]) and comms[0].stats()["kernel_launches"] == 0
-    finally:
-        destroy(torch, comms)
+        assert_nothing_launched(g.comms[0])
 
 
 def test_scratch_growth_keeps_a_captured_graph_valid(torch_cuda, coll_mod):
     torch, coll = torch_cuda, coll_mod
     n, block, wire = 2, 128, torch.float8_e4m3fn
-    comms, streams = make_group(torch, coll, n)
-    try:
+    with Group(torch, coll, n, arena_mb=192) as g:
         # eager calls that grow and shrink the scratch
         for k, count in enumerate((128 * 64, 128 * 256, 128 * 32, 128 * 512, 128 * 16)):
-            xs, ds = inputs(torch, comms, count, torch.float32, block, seed=40 + k)
-            outs = outputs(torch, comms, count, torch.bfloat16)
-            call(torch, coll, comms, streams, "all_reduce", ds, outs, block, wire, algo="twoshot" if k % 2 else "oneshot")
+            xs, ds = inputs(torch, g.comms, count, torch.float32, block, seed=40 + k)
+            outs = outputs(torch, g.comms, count, torch.bfloat16)
+            call(g, "all_reduce", ds, outs, block, wire, algo="twoshot" if k % 2 else "oneshot")
             want = qr.all_reduce(xs, block, wire, 1.0, torch.bfloat16)
             for r in range(n):
                 assert_same(outs[r].cpu(), want, f"eager size {count} rank {r}")
         # a graph per rank, captured at a size the current scratch holds
         count = 128 * 600
-        xs, ds = inputs(torch, comms, count, torch.bfloat16, block, seed=77)
-        outs = outputs(torch, comms, count, torch.float32)
+        xs, ds = inputs(torch, g.comms, count, torch.bfloat16, block, seed=77)
+        outs = outputs(torch, g.comms, count, torch.float32)
         graphs = []
-        for r, c in enumerate(comms):
+        for r, c in enumerate(g.comms):
             c.set_algo("twoshot")
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=streams[r]):
+            gr = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(gr, stream=g.streams[r]):
                 c.all_reduce_quantized(ds[r], outs[r], block=block, wire=wire)
-            graphs.append(g)
+            graphs.append(gr)
         # an eager call four times larger moves the scratch; an arena tensor allocated afterwards must never be written by the replay
-        xs4, ds4 = inputs(torch, comms, 4 * count, torch.bfloat16, block, seed=78)
-        outs4 = outputs(torch, comms, 4 * count, torch.bfloat16)
-        call(torch, coll, comms, streams, "all_reduce", ds4, outs4, block, wire, algo="oneshot")
+        xs4, ds4 = inputs(torch, g.comms, 4 * count, torch.bfloat16, block, seed=78)
+        outs4 = outputs(torch, g.comms, 4 * count, torch.bfloat16)
+        call(g, "all_reduce", ds4, outs4, block, wire, algo="oneshot")
         want4 = qr.all_reduce(xs4, block, wire, 1.0, torch.bfloat16)
         for r in range(n):
             assert_same(outs4[r].cpu(), want4, f"grown rank {r}")
-        guards = [c.empty(count * 2, torch.float32) for c in comms]
+        guards = [c.empty(count * 2, torch.float32) for c in g.comms]
         for gd in guards:
             gd.fill_(3.25)
         for o in outs:
             o.view(torch.uint8).fill_(0x5A)
         torch.cuda.synchronize()
-        for r, g in enumerate(graphs):
-            with torch.cuda.stream(streams[r]):
-                g.replay()
+        for r, gr in enumerate(graphs):
+            with torch.cuda.stream(g.streams[r]):
+                gr.replay()
         torch.cuda.synchronize()
-        for c in comms:
+        for c in g.comms:
             c.check_async_error()
         want = qr.all_reduce(xs, block, wire, 1.0, torch.float32)
         for r in range(n):
             assert_same(outs[r].cpu(), want, f"graph replay rank {r}")
             assert bool((guards[r] == 3.25).all()), f"rank {r}: the replay wrote into memory allocated after the scratch grew"
         del graphs
-    finally:
-        destroy(torch, comms)
 
 
 @pytest.mark.parametrize("op", ["all_gather", "reduce_scatter", "all_reduce"])
 def test_perf_tool_quantize_bit_exact(torch_cuda, coll_lib, op):
-    r = subprocess.run([PERF, "--devs", "0,0", "--op", op, "-d", "bfloat16", "--out-dtype", "float", "--quantize", "e4m3:128",
-                        "-b", "64K", "-e", "4M", "-f", "8", "-w", "1", "-n", "2", "-c", "1"], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-    assert "errors=0" in r.stdout and "quantised: wire=e4m3 block=128" in r.stdout, r.stdout[-2000:]
-    rows = [l for l in r.stdout.splitlines() if l.strip() and not l.startswith("#")]
-    assert len(rows) == 3, r.stdout                                      # 64 KiB, 512 KiB and 4 MiB
-    r = subprocess.run([PERF, "--devs", "0,0,0", "--op", op, "-d", "half", "--out-dtype", "bfloat16", "--quantize", "e5m2:32", "--algo", "twoshot",
-                        "-b", "1M", "-e", "1M", "-w", "1", "-n", "2", "-c", "1"], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "errors=0" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
+    out = run_perf(["--op", op, "-d", "bfloat16", "--out-dtype", "float", "--quantize", "e4m3:128", "-b", "64K", "-e", "4M", "-f", "8", "-w", "1",
+                    "-n", "2", "-c", "1"], "0,0")
+    assert "quantised: wire=e4m3 block=128" in out, out[-2000:]
+    rows = [l for l in out.splitlines() if l.strip() and not l.startswith("#")]
+    assert len(rows) == 3, out                                           # 64 KiB, 512 KiB and 4 MiB
+    run_perf(["--op", op, "-d", "half", "--out-dtype", "bfloat16", "--quantize", "e5m2:32", "--algo", "twoshot", "-b", "1M", "-e", "1M", "-w", "1",
+              "-n", "2", "-c", "1"], "0,0,0")
 
 
 def test_multi_gpu_quantized(torch_cuda, coll_mod):
@@ -379,8 +308,8 @@ def test_multi_gpu_quantized(torch_cuda, coll_mod):
         pytest.skip("needs >= 2 GPUs")
     n, block, wire = torch.cuda.device_count(), 128, torch.float8_e4m3fn
     count = block * 96 * n
-    comms = coll.Comm.init_all(list(range(n)), arena_mb=256)
-    try:
+    with Group(torch, coll, n, devices=list(range(n)), arena_mb=256) as g:
+        comms = g.comms
         xs = [qr.gen(count, torch.bfloat16, block, 90 + r) for r in range(n)]
         ds, ag, rs, ar = [], [], [], []
         for r, c in enumerate(comms):
@@ -405,8 +334,3 @@ def test_multi_gpu_quantized(torch_cuda, coll_mod):
                 assert_same(ag[r].cpu(), qr.all_gather(xs, block, wire, 1.0, torch.bfloat16), f"multi-GPU all_gather rank {r}")
                 assert_same(rs[r].cpu(), qr.reduce_scatter(xs, block, wire, avg_scale(1.0, n), torch.float32, r), f"multi-GPU reduce_scatter rank {r}")
                 assert_same(ar[r].cpu(), qr.all_reduce(xs, block, wire, 1.0, torch.bfloat16), f"multi-GPU all_reduce {algo} rank {r}")
-    finally:
-        for r in range(n):
-            torch.cuda.synchronize(r)
-        for c in comms:
-            c.destroy()
