@@ -9,6 +9,8 @@
 //         --procs      fork one process per rank and rendezvous over the Unix-socket bootstrap
 // Timing: CUDA events on each rank's stream around `iters` back-to-back launches, max over ranks.
 // Buffers rotate through a >L2 window so every timed launch sees cold lines.
+// Exit status: 0 every check passed; 1 a bad argument; 2 a CUDA error; 3 a library error; 4 a -c 1 check found a wrong value (in every
+// mode); 5 the library's watchdog recorded a fault; 6 a host barrier timed out.
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -111,59 +113,77 @@ static b200collDataType_t parse_dt(const char* s) {
   if (!strcmp(s, "e5m2")) return b200collFloat8e5m2;
   fprintf(stderr, "bad dtype %s\n", s); exit(1);
 }
-static const char* dt_name(b200collDataType_t t) { return t == b200collFloat32 ? "f32" : t == b200collFloat16 ? "f16" : t == b200collBfloat16 ? "bf16" : t == b200collFloat8e5m2 ? "e5m2" : "e4m3"; }
-
-// deterministic input: multiples of 0.25 in [-2, 2] (exact in e4m3 and e5m2 too) so sums over <= 8 ranks are exact in bf16/f16/f32
-static inline float gen(int rank, size_t i) { return (float)((int)((i * 7 + (size_t)rank * 13 + (i >> 9)) % 17) - 8) * 0.25f; }
-
-// Quantising mode: rank r's input element i is gen(r, i) times a power of two that changes from block to block (2^-6 .. 2^6, exact in
-// bf16, fp16 and fp32), so blocks have different amax values. The check repeats the library's per-block rule on the host (amax, two
-// IEEE divisions, RNE saturating pack, one multiply) and the rank-order fp32 sum, bit for bit.
-static float q_in(const Opts& o, int rank, size_t i) { return gen(rank, i) * ldexpf(1.0f, (int)(((i / o.q_block) * 5 + (size_t)rank * 3) % 13) - 6); }
-template <typename T> __global__ void k_fill_q(T* p, size_t n, int rank, int block) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float v = (float)((int)((i * 7 + (size_t)rank * 13 + (i >> 9)) % 17) - 8) * 0.25f;
-    p[i] = T(v * ldexpf(1.0f, (int)(((i / block) * 5 + (size_t)rank * 3) % 13) - 6));
+// --quantize and --combine-quantize WIRE:BLOCK
+static void parse_wire_block(const std::string& flag, const char* s, b200collDataType_t* wire, int* block) {
+  char w[16] = {};
+  if (sscanf(s, "%15[a-z0-9]:%d", w, block) != 2 || (strcmp(w, "e4m3") && strcmp(w, "e5m2")) || *block < 16 || *block > 512 || (*block & (*block - 1))) {
+    fprintf(stderr, "%s WIRE:BLOCK: WIRE e4m3 or e5m2, BLOCK 16, 32, 64, 128, 256 or 512\n", flag.c_str()); exit(1);
   }
+  *wire = parse_dt(w);
 }
-// The FP8 code of rank r's element i; `memo` keeps the last block's (index, inv, s), as the check walks elements in order.
-struct QMemo { size_t blk = SIZE_MAX; float inv = 1.0f, s = 1.0f; };
+static const char* dt_name(b200collDataType_t t) { return t == b200collFloat32 ? "f32" : t == b200collFloat16 ? "f16" : t == b200collBfloat16 ? "bf16" : t == b200collFloat8e5m2 ? "e5m2" : "e4m3"; }
+static bool wide(b200collDataType_t t) { return t == b200collBfloat16 || t == b200collFloat16 || t == b200collFloat32; }
+
+// Deterministic input: multiples of 0.25 in [-2, 2] (exact in e4m3 and e5m2 too) so sums over <= 8 ranks are exact in bf16/f16/f32.
+// With block > 0 (the quantising modes) each value is also multiplied by a power of two that changes from block to block (2^-6 .. 2^6,
+// exact in bf16, fp16 and fp32), so blocks have different amax values.
+__host__ __device__ inline float gen(int rank, size_t i, int block = 0) {
+  const float v = (float)((int)((i * 7 + (size_t)rank * 13 + (i >> 9)) % 17) - 8) * 0.25f;
+  return block ? v * ldexpf(1.0f, (int)(((i / block) * 5 + (size_t)rank * 3) % 13) - 6) : v;
+}
+template <typename T> __global__ void k_fill(T* p, size_t n, int rank, int block) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = T(gen(rank, i, block));
+}
+static void fill(void* p, size_t n, b200collDataType_t dt, int rank, cudaStream_t st, int block = 0) {
+  if (dt == b200collFloat32) k_fill<float><<<256, 256, 0, st>>>((float*)p, n, rank, block);
+  else if (dt == b200collFloat16) k_fill<__half><<<256, 256, 0, st>>>((__half*)p, n, rank, block);
+  else if (dt == b200collFloat8e4m3) k_fill<__nv_fp8_e4m3><<<256, 256, 0, st>>>((__nv_fp8_e4m3*)p, n, rank, block);
+  else if (dt == b200collFloat8e5m2) k_fill<__nv_fp8_e5m2><<<256, 256, 0, st>>>((__nv_fp8_e5m2*)p, n, rank, block);
+  else k_fill<__nv_bfloat16><<<256, 256, 0, st>>>((__nv_bfloat16*)p, n, rank, block);
+  RT(cudaGetLastError());
+}
+
+// The library's per-block quantisation rule on the host: amax, two IEEE divisions, the RNE saturating pack of each value times inv into
+// q. Returns the block's scale; dequant() turns a code back into a value with one multiply. The checks repeat it bit for bit.
+static __nv_fp8_interpretation_t fp8_kind(b200collDataType_t wire) { return wire == b200collFloat8e4m3 ? __NV_E4M3 : __NV_E5M2; }
+static float quantise_block(const float* x, int n, b200collDataType_t wire, __nv_fp8_storage_t* q) {
+  const float fmax = wire == b200collFloat8e4m3 ? 448.0f : 57344.0f;
+  float amax = 0.0f;
+  for (int k = 0; k < n; k++) amax = std::max(amax, fabsf(x[k]));
+  volatile float a = amax;                                     // keep both divisions as written: IEEE, rounded to nearest
+  float inv = fmax / a, s = a / fmax;
+  if (amax == 0.0f || isinf(inv)) inv = s = 1.0f;
+  for (int k = 0; k < n; k++) q[k] = __nv_cvt_float_to_fp8(x[k] * inv, __NV_SATFINITE, fp8_kind(wire));
+  return s;
+}
+static float dequant(__nv_fp8_storage_t q, float s, b200collDataType_t wire) {
+  volatile float v = __half2float(__half(__nv_cvt_fp8_to_halfraw(q, fp8_kind(wire)))) * s;
+  return v;
+}
+// Quantising mode: the FP8 code of rank r's element gen(r, i, q_block); `memo` keeps the last block's codes and scale, as the checks
+// walk elements in order.
+struct QMemo { size_t blk = SIZE_MAX; float s = 1.0f; __nv_fp8_storage_t q[512]; };
 static __nv_fp8_storage_t q_code(const Opts& o, int rank, size_t i, QMemo* memo) {
   const size_t blk = i / o.q_block;
-  const float fmax = o.q_wire == b200collFloat8e4m3 ? 448.0f : 57344.0f;
   if (memo->blk != blk) {
-    float amax = 0.0f;
-    for (size_t k = blk * o.q_block; k < (blk + 1) * o.q_block; k++) amax = std::max(amax, fabsf(q_in(o, rank, k)));
-    volatile float a = amax;                                     // keep both divisions as written: IEEE, rounded to nearest
-    float inv = fmax / a, s = a / fmax;
-    if (amax == 0.0f || isinf(inv)) inv = s = 1.0f;
-    *memo = QMemo{blk, inv, s};
+    float x[512];
+    for (int k = 0; k < o.q_block; k++) x[k] = gen(rank, blk * o.q_block + k, o.q_block);
+    memo->s = quantise_block(x, o.q_block, o.q_wire, memo->q);
+    memo->blk = blk;
   }
-  const float y = q_in(o, rank, i) * memo->inv;
-  return __nv_cvt_float_to_fp8(y, __NV_SATFINITE, o.q_wire == b200collFloat8e4m3 ? __NV_E4M3 : __NV_E5M2);
+  return memo->q[i % o.q_block];
 }
 // ... and its dequantised value
 static float q_val(const Opts& o, int rank, size_t i, QMemo* memo) {
   const __nv_fp8_storage_t q = q_code(o, rank, i, memo);
-  return __half2float(__half(__nv_cvt_fp8_to_halfraw(q, o.q_wire == b200collFloat8e4m3 ? __NV_E4M3 : __NV_E5M2))) * memo->s;
+  return dequant(q, memo->s, o.q_wire);
 }
-
-// The quantising combine's host reference: n values quantised by the per-block rule (amax, two IEEE divisions, RNE saturating pack)
-// and dequantised with one multiply, in place.
+// The quantising combine's host reference: n values quantised block by block and dequantised, in place.
 static void q_roundtrip(float* x, size_t n, int block, b200collDataType_t wire) {
-  const float fmax = wire == b200collFloat8e4m3 ? 448.0f : 57344.0f;
-  const __nv_fp8_interpretation_t I = wire == b200collFloat8e4m3 ? __NV_E4M3 : __NV_E5M2;
+  __nv_fp8_storage_t q[512];
   for (size_t b0 = 0; b0 < n; b0 += block) {
-    float amax = 0.0f;
-    for (size_t k = b0; k < b0 + block; k++) amax = std::max(amax, fabsf(x[k]));
-    volatile float a = amax;
-    float inv = fmax / a, s = a / fmax;
-    if (amax == 0.0f || isinf(inv)) inv = s = 1.0f;
-    for (size_t k = b0; k < b0 + block; k++) {
-      const __nv_fp8_storage_t q = __nv_cvt_float_to_fp8(x[k] * inv, __NV_SATFINITE, I);
-      volatile float v = __half2float(__half(__nv_cvt_fp8_to_halfraw(q, I))) * s;
-      x[k] = v;
-    }
+    const float s = quantise_block(x + b0, block, wire, q);
+    for (int k = 0; k < block; k++) x[b0 + k] = dequant(q[k], s, wire);
   }
 }
 // The quantising combine's scratch (FP8 copy plus scales of every expert_out row) grows with the sweep and keeps every superseded
@@ -172,21 +192,6 @@ static size_t cq_scratch_bytes(const Opts& o) {
   if (!o.cq_block) return 0;
   const size_t elems = o.max_bytes / b200collTypeSize(o.in_dt) * (o.route_e ? o.route_k : 1);
   return 2 * (elems + elems / o.cq_block * 4) + (4u << 20);
-}
-
-template <typename T> __global__ void k_fill(T* p, size_t n, int rank, size_t base) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    size_t g = base + i;
-    float v = (float)((int)((g * 7 + (size_t)rank * 13 + (g >> 9)) % 17) - 8) * 0.25f;
-    p[i] = T(v);
-  }
-}
-static void fill(void* p, size_t n, b200collDataType_t dt, int rank, size_t base, cudaStream_t st) {
-  if (dt == b200collFloat32) k_fill<float><<<256, 256, 0, st>>>((float*)p, n, rank, base);
-  else if (dt == b200collFloat16) k_fill<__half><<<256, 256, 0, st>>>((__half*)p, n, rank, base);
-  else if (dt == b200collFloat8e4m3) k_fill<__nv_fp8_e4m3><<<256, 256, 0, st>>>((__nv_fp8_e4m3*)p, n, rank, base);
-  else if (dt == b200collFloat8e5m2) k_fill<__nv_fp8_e5m2><<<256, 256, 0, st>>>((__nv_fp8_e5m2*)p, n, rank, base);
-  else k_fill<__nv_bfloat16><<<256, 256, 0, st>>>((__nv_bfloat16*)p, n, rank, base);
 }
 
 static float to_f(const void* p, size_t i, b200collDataType_t dt) {
@@ -217,7 +222,64 @@ static void spin_barrier(Shared* sh, int which, int n, int* gen) {
 
 constexpr int kRoot = 0;   // rooted ops (broadcast, reduce) are driven from rank 0, like nccl-tests' default
 
-struct RankCtx { int rank, nranks; b200collComm_t comm; int dev; };
+struct RankCtx {
+  int rank, nranks; b200collComm_t comm; int dev;
+  Shared* sh;
+  cudaStream_t st = nullptr; cudaEvent_t e0 = nullptr, e1 = nullptr;   // made by run_rank
+  int barrier_gen[4] = {0, 0, 0, 0};
+  void barrier(int which) { spin_barrier(sh, which, nranks, &barrier_gen[which]); }
+};
+
+// A fault the library's watchdog recorded ends the rank.
+static void watchdog(const RankCtx& c, const char* when) {
+  b200collFault f;
+  if (b200collCommGetAsyncError(c.comm, &f) != b200collSuccess) {
+    fprintf(stderr, "rank %d WATCHDOG (%s) code=%u peer=%u block=%u expected=%u observed=%u op=%u\n", c.rank, when, f.code, f.peer, f.block, f.expected,
+            f.observed, f.op);
+    _exit(5);
+  }
+}
+// The -c 1 launch: inputs ready on every rank (barrier 0), rank 0 late by --skew-us, launch(0), every rank done (barrier 1).
+template <typename F> static void check_launch(const Opts& o, RankCtx& c, F&& launch) {
+  RT(cudaStreamSynchronize(c.st));
+  c.barrier(0);
+  if (o.skew_us && c.rank == 0) usleep(o.skew_us);
+  launch(0);
+  RT(cudaStreamSynchronize(c.st));
+  c.barrier(1);
+  watchdog(c, "check");
+}
+// The timing protocol: launch(i) for `warmup` untimed iterations, all ranks lined up (barrier 2), then CUDA events on this rank's stream
+// around `iters` back-to-back launches. Every rank posts its per-launch ms and error count `errs` (barrier 3) and reads all of them;
+// barrier 0 keeps the page stable until everyone has. Returns the worst ms over ranks and the sum of their errors.
+struct Timing { float ms; long errors; };
+template <typename F> static Timing timed(const Opts& o, RankCtx& c, long errs, F&& launch) {
+  for (int i = 0; i < o.warmup; i++) launch(i);
+  RT(cudaStreamSynchronize(c.st));
+  c.barrier(2);
+  RT(cudaEventRecord(c.e0, c.st));
+  for (int i = 0; i < o.iters; i++) launch(i);
+  RT(cudaEventRecord(c.e1, c.st));
+  RT(cudaEventSynchronize(c.e1));
+  float ms = 0; RT(cudaEventElapsedTime(&ms, c.e0, c.e1));
+  c.sh->ms[c.rank] = ms / o.iters; c.sh->errors[c.rank] = errs;
+  c.barrier(3);
+  Timing t{0, 0};
+  for (int r = 0; r < c.nranks; r++) { t.ms = std::max(t.ms, c.sh->ms[r]); t.errors += c.sh->errors[r]; }
+  c.barrier(0);
+  watchdog(c, "timing");
+  return t;
+}
+
+// The end of a mode runner (--combine, --rms-norm, --route): rank 0 reports the launches and the errors of every size.
+static int mode_result(const RankCtx& c, long total_errors) {
+  b200collStats s; CC(b200collCommStatsGet(c.comm, &s));
+  if (c.rank == 0) {
+    printf("# launches=%llu errors=%ld\n", (unsigned long long)s.kernel_launches, total_errors);
+    fflush(stdout);
+  }
+  return total_errors ? 4 : 0;
+}
 
 // Expert-combine mode (--combine K). Per size, every rank's expert_out holds `bytes` of whole --row-len rows, an even split: rpp rows
 // came from every rank. So rank r's dispatch rows for peer p are rows [p * rpp, + rpp) of its (notional) send buffer and their expert
@@ -226,18 +288,11 @@ struct RankCtx { int rank, nranks; b200collComm_t comm; int dev; };
 // seeded in [0.25, 1.25). Expert-out values are exact in every input type and the weights have full mantissas, so products and sums
 // round; -c 1 repeats the slot-order fp32 arithmetic on the host and compares every output element bit for bit.
 static uint32_t co_hash(uint32_t x) { x ^= x >> 16; x *= 0x7FEB352Du; x ^= x >> 15; x *= 0x846CA68Bu; x ^= x >> 16; return x; }
-static float co_val(int rank, size_t i) { return gen(rank, i) * ldexpf(1.0f, (int)((i / 16 * 5 + (size_t)rank * 3) % 13) - 6); }
-template <typename T> __global__ void k_fill_co(T* p, size_t n, int rank) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float v = (float)((int)((i * 7 + (size_t)rank * 13 + (i >> 9)) % 17) - 8) * 0.25f;
-    p[i] = T(v * ldexpf(1.0f, (int)((i / 16 * 5 + (size_t)rank * 3) % 13) - 6));
-  }
-}
-static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out, void* out, cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1) {
+static int run_combine(const Opts& o, RankCtx& ctx, void* expert_out, void* out) {
   const int n = ctx.nranks, rank = ctx.rank, K = o.combine_k;
   const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt), row = o.row_len;
   const b200collEpilogue ep{o.in_dt, o.out_dt, o.scale};
-  int gen_ctr[4] = {0, 0, 0, 0};
+  const cudaStream_t st = ctx.st;
   long total_errors = 0;
   if (rank == 0 && o.cq_block) {
     printf("# b200coll_perf op=alltoall quantising combine top_k=%d nranks=%d in=%s wire=%s block=%d out=%s scale=%g row_len=%zu: size = expert_out bytes per rank\n",
@@ -271,12 +326,9 @@ static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out,
     RT(cudaMemcpy(d_idx, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice));
     RT(cudaMemcpy(d_w, w.data(), w.size() * 4, cudaMemcpyHostToDevice));
     const size_t eo_elems = recv_rows * row, out_elems = tokens * row;
-    if (o.in_dt == b200collFloat32) k_fill_co<float><<<256, 256, 0, st>>>((float*)expert_out, eo_elems, rank);
-    else if (o.in_dt == b200collFloat16) k_fill_co<__half><<<256, 256, 0, st>>>((__half*)expert_out, eo_elems, rank);
-    else k_fill_co<__nv_bfloat16><<<256, 256, 0, st>>>((__nv_bfloat16*)expert_out, eo_elems, rank);
-    RT(cudaGetLastError());
+    fill(expert_out, eo_elems, o.in_dt, rank, st, 16);
     RT(cudaMemsetAsync(out, 0x5A, out_elems * os, st));
-    auto launch = [&] {
+    auto launch = [&](int) {
       if (o.cq_block)
         CC(b200collAllToAllvCombineQuantized(expert_out, out, row, recv_rows, rows.data(), soff.data(), roff.data(), d_idx, d_w, tokens, K, o.cq_wire,
                                              o.cq_block, &ep, ctx.comm, st));
@@ -285,16 +337,12 @@ static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out,
     };
     long errs = 0;
     if (o.check) {
-      RT(cudaStreamSynchronize(st));
-      spin_barrier(sh, 0, n, &gen_ctr[0]);
-      launch();
-      RT(cudaStreamSynchronize(st));
-      spin_barrier(sh, 1, n, &gen_ctr[1]);
+      check_launch(o, ctx, launch);
       std::vector<char> host(out_elems * os);
       RT(cudaMemcpy(host.data(), out, host.size(), cudaMemcpyDeviceToHost));
       // --combine-quantize: the rows this rank reads (rows [rank * rpp, + rpp) of every peer's expert_out), quantised and dequantised
       std::vector<float> deq(o.cq_block ? (size_t)n * rpp * row : 0);
-      for (size_t i = 0; i < deq.size(); i++) deq[i] = co_val((int)(i / (rpp * row)), (size_t)rank * rpp * row + i % (rpp * row));
+      for (size_t i = 0; i < deq.size(); i++) deq[i] = gen((int)(i / (rpp * row)), (size_t)rank * rpp * row + i % (rpp * row), 16);
       for (size_t r = 0; r < deq.size() / row; r++) q_roundtrip(deq.data() + r * row, row, o.cq_block, o.cq_wire);
       for (size_t t = 0; t < tokens; t++) {
         for (size_t e = 0; e < row; e++) {
@@ -304,7 +352,7 @@ static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out,
             if (i < 0) continue;
             const int p = (int)(i / (int64_t)rpp);                      // the range row i lies in, and its row of p's expert_out
             const size_t r = (size_t)rank * rpp + (size_t)(i - soff[p]);
-            volatile float prod = w[t * K + j] * (o.cq_block ? deq[((size_t)p * rpp + (size_t)(i - soff[p])) * row + e] : co_val(p, r * row + e));
+            volatile float prod = w[t * K + j] * (o.cq_block ? deq[((size_t)p * rpp + (size_t)(i - soff[p])) * row + e] : gen(p, r * row + e, 16));
             acc = acc + prod;
           }
           const uint32_t want = out_bits(acc * o.scale, o.out_dt), got = got_bits(host.data(), t * row + e, o.out_dt);
@@ -312,35 +360,17 @@ static int run_combine(const Opts& o, RankCtx ctx, Shared* sh, void* expert_out,
         }
       }
     }
-    for (int i = 0; i < o.warmup; i++) launch();
-    RT(cudaStreamSynchronize(st));
-    spin_barrier(sh, 2, n, &gen_ctr[2]);
-    RT(cudaEventRecord(e0, st));
-    for (int i = 0; i < o.iters; i++) launch();
-    RT(cudaEventRecord(e1, st));
-    RT(cudaEventSynchronize(e1));
-    float ms = 0; RT(cudaEventElapsedTime(&ms, e0, e1));
-    sh->ms[rank] = ms / o.iters; sh->errors[rank] = errs;
-    spin_barrier(sh, 3, n, &gen_ctr[3]);
-    float worst = 0; long es = 0;
-    for (int r = 0; r < n; r++) { worst = std::max(worst, sh->ms[r]); es += sh->errors[r]; }
-    total_errors += es;
-    spin_barrier(sh, 0, n, &gen_ctr[0]);   // keep ms[] stable until everyone has read it
-    b200collFault f;
-    if (b200collCommGetAsyncError(ctx.comm, &f) != b200collSuccess) { fprintf(stderr, "rank %d WATCHDOG code=%u peer=%u block=%u expected=%u observed=%u\n", rank, f.code, f.peer, f.block, f.expected, f.observed); _exit(5); }
+    const Timing tm = timed(o, ctx, errs, launch);
+    total_errors += tm.errors;
     if (rank == 0) {
       const size_t eo_bytes = recv_rows * row * is;
-      printf("%14zu %12zu %6s %8s | %10.2f %8.2f %6ld\n", eo_bytes, tokens, dt_name(o.in_dt), n > 1 ? "oneshot" : "copy", worst * 1e3, eo_bytes / (worst * 1e3) / 1e3, es);
+      printf("%14zu %12zu %6s %8s | %10.2f %8.2f %6ld\n", eo_bytes, tokens, dt_name(o.in_dt), n > 1 ? "oneshot" : "copy", tm.ms * 1e3, eo_bytes / (tm.ms * 1e3) / 1e3,
+             tm.errors);
       fflush(stdout);
     }
     RT(cudaFree(d_idx)); RT(cudaFree(d_w));
   }
-  b200collStats s; CC(b200collCommStatsGet(ctx.comm, &s));
-  if (rank == 0) {
-    printf("# launches=%llu errors=%ld\n", (unsigned long long)s.kernel_launches, total_errors);
-    fflush(stdout);
-  }
-  return total_errors ? 1 : 0;
+  return mode_result(ctx, total_errors);
 }
 
 // All-reduce + RMSNorm mode (--rms-norm ROW_LEN). Per size, every rank's x holds `bytes` of whole rows (k_fill values of its rank), the
@@ -353,12 +383,12 @@ static float round_dt(float v, b200collDataType_t dt) {
   if (dt == b200collFloat16) return __half2float(__float2half_rn(v));
   return __bfloat162float(__float2bfloat16_rn(v));
 }
-static int run_rms(const Opts& o, RankCtx ctx, Shared* sh, void* x, void* out, void* residual, cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1) {
+static int run_rms(const Opts& o, RankCtx& ctx, void* x, void* out, void* residual) {
   const int n = ctx.nranks, rank = ctx.rank;
   const b200collDataType_t dt = o.in_dt;
   const size_t es = b200collTypeSize(dt), row = o.rms_row;
   const float eps = 1e-6f;
-  int gen_ctr[4] = {0, 0, 0, 0};
+  const cudaStream_t st = ctx.st;
   long total_errors = 0;
   if (rank == 0) {
     printf("# b200coll_perf op=all_reduce + rms-norm nranks=%d dtype=%s row_len=%zu eps=%g: size = x bytes per rank; rw GB/s = (x + residual + gamma read, "
@@ -368,34 +398,17 @@ static int run_rms(const Opts& o, RankCtx ctx, Shared* sh, void* x, void* out, v
   }
   void* gamma = nullptr;
   RT(cudaMalloc(&gamma, row * es));
-  fill(gamma, row, dt, 7, 0, st);
+  fill(gamma, row, dt, 7, st);
   for (size_t bytes = o.min_bytes; bytes <= o.max_bytes; bytes *= o.factor) {
     const size_t rows = bytes / es / row, elems = rows * row;
     if (rows == 0) continue;
-    fill(x, elems, dt, rank, 0, st);
-    fill(residual, elems, dt, 99, 0, st);
+    fill(x, elems, dt, rank, st);
+    fill(residual, elems, dt, 99, st);
     RT(cudaMemsetAsync(out, 0x5A, elems * es, st));
-    RT(cudaGetLastError());
-    auto launch = [&] { CC(b200collAllReduceRmsNorm(x, residual, gamma, out, rows, row, eps, dt, ctx.comm, st)); };
+    auto launch = [&](int) { CC(b200collAllReduceRmsNorm(x, residual, gamma, out, rows, row, eps, dt, ctx.comm, st)); };
     long errs = 0;
     if (o.check) {
-      std::vector<char> hres(elems * es), hg(row * es);
-      RT(cudaStreamSynchronize(st));
-      RT(cudaMemcpy(hres.data(), residual, hres.size(), cudaMemcpyDeviceToHost));
-      RT(cudaMemcpy(hg.data(), gamma, hg.size(), cudaMemcpyDeviceToHost));
-      std::vector<std::vector<char>> hx(n, std::vector<char>(elems * es));
-      for (int r = 0; r < n; r++) {               // every rank's x, from the same generator on the host
-        void* tmp = nullptr;
-        RT(cudaMalloc(&tmp, elems * es));
-        fill(tmp, elems, dt, r, 0, st);
-        RT(cudaStreamSynchronize(st));
-        RT(cudaMemcpy(hx[r].data(), tmp, elems * es, cudaMemcpyDeviceToHost));
-        RT(cudaFree(tmp));
-      }
-      spin_barrier(sh, 0, n, &gen_ctr[0]);
-      launch();
-      RT(cudaStreamSynchronize(st));
-      spin_barrier(sh, 1, n, &gen_ctr[1]);
+      check_launch(o, ctx, launch);
       std::vector<char> gres(elems * es), gout(elems * es);
       RT(cudaMemcpy(gres.data(), residual, gres.size(), cudaMemcpyDeviceToHost));
       RT(cudaMemcpy(gout.data(), out, gout.size(), cudaMemcpyDeviceToHost));
@@ -406,8 +419,8 @@ static int run_rms(const Opts& o, RankCtx ctx, Shared* sh, void* x, void* out, v
       for (size_t i = 0; i < rows; i++) {
         for (size_t e = 0; e < row; e++) {
           volatile float acc = 0.0f;
-          for (int r = 0; r < n; r++) acc = acc + to_f(hx[r].data(), i * row + e, dt);
-          h[e] = round_dt(acc + to_f(hres.data(), i * row + e, dt), dt);
+          for (int r = 0; r < n; r++) acc = acc + gen(r, i * row + e);     // the fill values, exact in every dtype
+          h[e] = round_dt(acc + gen(99, i * row + e), dt);
         }
         for (size_t c = 0; c < P; c++) {
           volatile float s = 0.0f;
@@ -421,7 +434,7 @@ static int run_rms(const Opts& o, RankCtx ctx, Shared* sh, void* x, void* out, v
         const float inv = 1.0f / den;
         for (size_t e = 0; e < row; e++) {
           volatile float hi = h[e] * inv;
-          volatile float y = hi * to_f(hg.data(), e, dt);
+          volatile float y = hi * gen(7, e);
           const uint32_t want_h = out_bits(h[e], dt), got_h = got_bits(gres.data(), i * row + e, dt);
           const uint32_t want_o = out_bits(y, dt), got_o = got_bits(gout.data(), i * row + e, dt);
           if (got_h != want_h || got_o != want_o) {
@@ -432,39 +445,21 @@ static int run_rms(const Opts& o, RankCtx ctx, Shared* sh, void* x, void* out, v
         }
       }
     }
-    for (int i = 0; i < o.warmup; i++) launch();
-    RT(cudaStreamSynchronize(st));
-    spin_barrier(sh, 2, n, &gen_ctr[2]);
     b200collStats s0; CC(b200collCommStatsGet(ctx.comm, &s0));
-    RT(cudaEventRecord(e0, st));
-    for (int i = 0; i < o.iters; i++) launch();
-    RT(cudaEventRecord(e1, st));
-    RT(cudaEventSynchronize(e1));
+    const Timing tm = timed(o, ctx, errs, launch);
     b200collStats s1; CC(b200collCommStatsGet(ctx.comm, &s1));
-    float ms = 0; RT(cudaEventElapsedTime(&ms, e0, e1));
-    sh->ms[rank] = ms / o.iters; sh->errors[rank] = errs;
-    spin_barrier(sh, 3, n, &gen_ctr[3]);
-    float worst = 0; long es_ = 0;
-    for (int r = 0; r < n; r++) { worst = std::max(worst, sh->ms[r]); es_ += sh->errors[r]; }
-    total_errors += es_;
-    spin_barrier(sh, 0, n, &gen_ctr[0]);   // keep ms[] stable until everyone has read it
-    b200collFault f;
-    if (b200collCommGetAsyncError(ctx.comm, &f) != b200collSuccess) { fprintf(stderr, "rank %d WATCHDOG code=%u peer=%u block=%u expected=%u observed=%u\n", rank, f.code, f.peer, f.block, f.expected, f.observed); _exit(5); }
+    total_errors += tm.errors;
     if (rank == 0) {
       const char* algo = "?";
       for (int a = 0; a < b200collNumAlgos; a++) if (s1.algo_calls[a] != s0.algo_calls[a]) algo = b200collAlgoName((b200collAlgo_t)a);
       const size_t mat = elems * es, rw = 4 * mat + row * es;
-      printf("%14zu %10zu %6s %8s | %10.2f %8.2f %8.1f %6ld\n", mat, rows, dt_name(dt), algo, worst * 1e3, mat / (worst * 1e3) / 1e3, rw / (worst * 1e3) / 1e3, es_);
+      printf("%14zu %10zu %6s %8s | %10.2f %8.2f %8.1f %6ld\n", mat, rows, dt_name(dt), algo, tm.ms * 1e3, mat / (tm.ms * 1e3) / 1e3, rw / (tm.ms * 1e3) / 1e3,
+             tm.errors);
       fflush(stdout);
     }
   }
   RT(cudaFree(gamma));
-  b200collStats s; CC(b200collCommStatsGet(ctx.comm, &s));
-  if (rank == 0) {
-    printf("# launches=%llu errors=%ld\n", (unsigned long long)s.kernel_launches, total_errors);
-    fflush(stdout);
-  }
-  return total_errors ? 1 : 0;
+  return mode_result(ctx, total_errors);
 }
 
 // Routed mode (--route E:K). Per size, every rank holds tokens = size / row bytes tokens of x (k_fill values) and routes slot (t, j) to
@@ -472,7 +467,7 @@ static int run_rms(const Opts& o, RankCtx ctx, Shared* sh, void* x, void* out, v
 // recv holds tokens * K rows on every rank, the mean load, so some receivers clip and some do not. -c 1 repeats the layout on the host
 // (per-expert counts, then each slot's row) and checks every byte of recv (stored rows, and the 0x5A poison elsewhere), every count,
 // every route and dropped; then the combine (recv as the expert output, seeded weights) bit for bit against the slot-order reference.
-// With --quantize WIRE:BLOCK it runs the FP8 routed dispatch instead: x holds the quantising mode's values (k_fill_q), recv FP8 rows
+// With --quantize WIRE:BLOCK it runs the FP8 routed dispatch instead: x holds the quantising mode's values (gen with BLOCK), recv FP8 rows
 // and recv_scales one fp32 scale per block; -c 1 checks every FP8 byte and scale against the host quantiser (q_code) and the 0x5A
 // poison of rows not stored in both, besides counts, routes and dropped. The combine needs a wide expert_out, so only the dispatch is timed.
 static size_t route_scale_bytes(const Opts& o) {
@@ -482,11 +477,12 @@ static int32_t ro_id(int rank, size_t t, int j, int E) {
   const uint32_t h = co_hash((uint32_t)(t * 0x9E3779B1u) ^ (uint32_t)(rank * 0x85EBCA77u) ^ (uint32_t)(j * 0xC2B2AE3Du));
   return h % 61 == 7 ? -1 : (int32_t)(h % (uint32_t)E);
 }
-static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1) {
+static int run_route(const Opts& o, RankCtx& ctx, void* x) {
   const int n = ctx.nranks, rank = ctx.rank, E = o.route_e, K = o.route_k, epr = E / n;
   const bool quant = o.q_block > 0;
   const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt), row = o.row_len, rs = quant ? 1 : is;   // rs: bytes of a recv element
   const b200collEpilogue ep{o.in_dt, o.out_dt, o.scale};
+  const cudaStream_t st = ctx.st;
   void* recv = nullptr;
   CC(b200collMemAlloc(ctx.comm, &recv, o.max_bytes * K + 4096));     // tokens * K rows at the largest size, the same on every rank
   float* recv_scales = nullptr;
@@ -494,7 +490,6 @@ static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream
   int32_t* small = nullptr;
   RT(cudaMalloc(&small, (size_t)(epr + 1) * 4));
   int32_t *d_counts = small, *d_dropped = small + epr;
-  int gen_ctr[4] = {0, 0, 0, 0};
   long total_errors = 0;
   if (rank == 0 && quant) {
     printf("# b200coll_perf op=alltoall routed FP8 dispatch experts=%d top_k=%d nranks=%d in=%s wire=%s block=%d row_len=%zu: size = x bytes per rank; combine not run\n",
@@ -541,21 +536,17 @@ static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream
     RT(cudaMemcpy(d_idx, ids[rank].data(), slots * 4, cudaMemcpyHostToDevice));
     RT(cudaMemcpy(d_w, w.data(), slots * 4, cudaMemcpyHostToDevice));
     const size_t nsc = quant ? recv_rows * row / o.q_block : 0;     // scales in recv_scales
-    if (!quant) fill(x, tokens * row, o.in_dt, rank, 0, st);
-    else if (o.in_dt == b200collFloat32) k_fill_q<float><<<256, 256, 0, st>>>((float*)x, tokens * row, rank, o.q_block);
-    else if (o.in_dt == b200collFloat16) k_fill_q<__half><<<256, 256, 0, st>>>((__half*)x, tokens * row, rank, o.q_block);
-    else k_fill_q<__nv_bfloat16><<<256, 256, 0, st>>>((__nv_bfloat16*)x, tokens * row, rank, o.q_block);
-    RT(cudaGetLastError());
+    fill(x, tokens * row, o.in_dt, rank, st, o.q_block);
     RT(cudaMemsetAsync(recv, 0x5A, recv_rows * row * rs, st));
     if (quant) RT(cudaMemsetAsync(recv_scales, 0x5A, nsc * 4, st));
-    auto dispatch = [&] {
+    auto dispatch = [&](int) {
       if (quant)
         CC(b200collExpertDispatchQuantized(x, recv, recv_scales, row, recv_rows, d_idx, tokens, K, E, d_counts, d_route, d_dropped, o.in_dt, o.q_wire, o.q_block,
                                            ctx.comm, st));
       else
         CC(b200collExpertDispatch(x, recv, row, recv_rows, d_idx, tokens, K, E, d_counts, d_route, d_dropped, o.in_dt, ctx.comm, st));
     };
-    auto combine = [&] {
+    auto combine = [&](int) {
       if (o.cq_block) CC(b200collExpertCombineQuantized(recv, out, row, recv_rows, d_route, d_w, tokens, K, o.cq_wire, o.cq_block, &ep, ctx.comm, st));
       else CC(b200collExpertCombine(recv, out, row, recv_rows, d_route, d_w, tokens, K, &ep, ctx.comm, st));
     };
@@ -565,12 +556,7 @@ static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream
       errs++;
     };
     if (o.check) {
-      RT(cudaStreamSynchronize(st));
-      spin_barrier(sh, 0, n, &gen_ctr[0]);
-      dispatch();
-      if (!quant) combine();
-      RT(cudaStreamSynchronize(st));
-      spin_barrier(sh, 1, n, &gen_ctr[1]);
+      check_launch(o, ctx, [&](int) { dispatch(0); if (!quant) combine(0); });
       std::vector<unsigned char> h_recv(recv_rows * row * rs);
       std::vector<int32_t> h_route(slots), h_small(epr + 1);
       std::vector<char> h_out(tokens * row * os);
@@ -639,45 +625,21 @@ static int run_route(const Opts& o, RankCtx ctx, Shared* sh, void* x, cudaStream
         }
       }
     }
-    float ms[2] = {0, 0};
-    for (int phase = 0; phase < (quant ? 1 : 2); phase++) {
-      for (int i = 0; i < o.warmup; i++) { if (phase == 0) dispatch(); else combine(); }
-      RT(cudaStreamSynchronize(st));
-      spin_barrier(sh, 2, n, &gen_ctr[2]);
-      RT(cudaEventRecord(e0, st));
-      for (int i = 0; i < o.iters; i++) { if (phase == 0) dispatch(); else combine(); }
-      RT(cudaEventRecord(e1, st));
-      RT(cudaEventSynchronize(e1));
-      RT(cudaEventElapsedTime(&ms[phase], e0, e1));
-      ms[phase] /= o.iters;
-    }
-    float worst[2] = {0, 0};
-    long es = 0;
-    for (int phase = 0; phase < 2; phase++) {
-      sh->ms[rank] = ms[phase]; sh->errors[rank] = errs;
-      spin_barrier(sh, 3, n, &gen_ctr[3]);
-      for (int r = 0; r < n; r++) { worst[phase] = std::max(worst[phase], sh->ms[r]); if (phase == 0) es += sh->errors[r]; }
-      spin_barrier(sh, 0, n, &gen_ctr[0]);   // keep ms[] stable until everyone has read it
-    }
-    total_errors += es;
-    b200collFault f;
-    if (b200collCommGetAsyncError(ctx.comm, &f) != b200collSuccess) { fprintf(stderr, "rank %d WATCHDOG code=%u peer=%u block=%u expected=%u observed=%u\n", rank, f.code, f.peer, f.block, f.expected, f.observed); _exit(5); }
+    const Timing td = timed(o, ctx, errs, dispatch);                          // errors are counted with the dispatch only
+    const Timing tc = quant ? Timing{0, 0} : timed(o, ctx, 0, combine);
+    total_errors += td.errors;
     if (rank == 0 && quant) {
-      printf("%14zu %12zu %6s %8s | %12.2f %12s %6ld\n", tokens * row * is, tokens, dt_name(o.in_dt), n > 1 ? "twoshot" : "copy", worst[0] * 1e3, "-", es);
+      printf("%14zu %12zu %6s %8s | %12.2f %12s %6ld\n", tokens * row * is, tokens, dt_name(o.in_dt), n > 1 ? "twoshot" : "copy", td.ms * 1e3, "-", td.errors);
       fflush(stdout);
     } else if (rank == 0) {
-      printf("%14zu %12zu %6s %8s | %12.2f %12.2f %6ld\n", tokens * row * is, tokens, dt_name(o.in_dt), n > 1 ? "twoshot" : "copy", worst[0] * 1e3, worst[1] * 1e3, es);
+      printf("%14zu %12zu %6s %8s | %12.2f %12.2f %6ld\n", tokens * row * is, tokens, dt_name(o.in_dt), n > 1 ? "twoshot" : "copy", td.ms * 1e3, tc.ms * 1e3,
+             td.errors);
       fflush(stdout);
     }
     RT(cudaFree(d_idx)); RT(cudaFree(d_route)); RT(cudaFree(d_w)); RT(cudaFree(out));
   }
   RT(cudaFree(small));
-  b200collStats s; CC(b200collCommStatsGet(ctx.comm, &s));
-  if (rank == 0) {
-    printf("# launches=%llu errors=%ld\n", (unsigned long long)s.kernel_launches, total_errors);
-    fflush(stdout);
-  }
-  return total_errors ? 1 : 0;
+  return mode_result(ctx, total_errors);
 }
 
 // expected value of output element e (element index in the op's output) for this rank
@@ -691,25 +653,22 @@ static float expected(const Opts& o, int rank, int n, size_t e, size_t count) {
   /* alltoall */ { int src = (int)(e / count); return gen(src, (size_t)rank * count + e % count) * o.scale; }
 }
 
-static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
+static int run_rank(const Opts& o, RankCtx ctx) {
   const int n = ctx.nranks, rank = ctx.rank;
   RT(cudaSetDevice(ctx.dev));
-  cudaStream_t st; RT(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-  cudaEvent_t e0, e1; RT(cudaEventCreate(&e0)); RT(cudaEventCreate(&e1));
+  RT(cudaStreamCreateWithFlags(&ctx.st, cudaStreamNonBlocking));
+  RT(cudaEventCreate(&ctx.e0)); RT(cudaEventCreate(&ctx.e1));
+  const cudaStream_t st = ctx.st;
   if (o.algo != "auto") {
     for (int a = 0; a < b200collNumAlgos; a++) if (o.algo == b200collAlgoName((b200collAlgo_t)a)) CC(b200collCommSetAlgo(ctx.comm, (b200collAlgo_t)a));
   }
   if (o.max_ctas > 0) CC(b200collCommSetMaxCtas(ctx.comm, o.max_ctas));
   const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt);
   const bool is_bc = o.op == "broadcast", is_rd = o.op == "reduce", is_sr = o.op == "sendrecv";
-  if (is_sr && (o.in_dt != o.out_dt || o.scale != 1.0f)) { fprintf(stderr, "sendrecv moves opaque bytes: --in and --out must match and --scale must be 1\n"); return 2; }
   const bool is_ar = o.op == "all_reduce" || is_bc || is_rd || is_sr;      // "whole message" geometry: count elements in, count out
   const bool is_hc = o.op == "hypercube";          // nccl-tests hypercube_perf: an all-gather made of log2(n) pairwise exchanges of doubling size
-  if (is_hc && (n & (n - 1))) { fprintf(stderr, "hypercube needs a power-of-two number of ranks\n"); return 2; }
   const bool is_ga = o.op == "gather" || is_hc, is_sc = o.op == "scatter";                 // nccl-tests gather_perf / scatter_perf: one send/recv group around the root
-  if ((is_ga || is_sc) && (o.in_dt != o.out_dt || o.scale != 1.0f)) { fprintf(stderr, "%s moves opaque bytes: --in and --out must match and --scale must be 1\n", o.op.c_str()); return 2; }
   const bool is_ag = o.op == "all_gather" || is_ga, is_rs = o.op == "reduce_scatter" || is_sc;      // same buffer geometry
-  if (!is_ar && !is_ag && !is_rs && o.op != "alltoall") { fprintf(stderr, "unknown --op %s\n", o.op.c_str()); return 2; }
   // nccl-tests convention: "size" is the larger of the two buffers in bytes of the input type
   const size_t max_in_bytes = o.max_bytes, max_out_bytes = o.max_bytes / is * os;
   const size_t send_cap = std::max(o.window, max_in_bytes), recv_cap = std::max(o.window / is * os, max_out_bytes);
@@ -719,48 +678,17 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
   if (o.rms_row) {
     void* residual = nullptr;
     CC(b200collMemAlloc(ctx.comm, &residual, max_in_bytes + 4096));
-    return run_rms(o, ctx, sh, send, recv, residual, st, e0, e1);
+    return run_rms(o, ctx, send, recv, residual);
   }
-  if (o.combine_k) {
-    if (o.op != "alltoall" || o.q_block || o.bs_rows || o.row_len == 0 || o.row_len % 16 ||
-        [](b200collDataType_t t) { return t != b200collBfloat16 && t != b200collFloat16 && t != b200collFloat32; }(o.in_dt) ||
-        [](b200collDataType_t t) { return t != b200collBfloat16 && t != b200collFloat16 && t != b200collFloat32; }(o.out_dt)) {
-      fprintf(stderr, "--combine K takes --op alltoall, -d and --out-dtype bfloat16|half|float, a --row-len that is a multiple of 16, and no --quantize or --block-scale\n");
-      return 2;
-    }
-    return run_combine(o, ctx, sh, send, recv, st, e0, e1);
-  }
-  if (o.route_e) {
-    const auto wide = [](b200collDataType_t t) { return t == b200collBfloat16 || t == b200collFloat16 || t == b200collFloat32; };
-    // with --quantize there is no combine, so no out type: the quantising alltoall defaults --out-dtype to the wire type
-    if (o.op != "alltoall" || o.bs_rows || o.row_len == 0 || o.row_len % 16 || !wide(o.in_dt) || (!o.q_block && !wide(o.out_dt)) || o.route_e % n != 0 ||
-        (o.q_block && o.row_len % o.q_block != 0)) {
-      fprintf(stderr, "--route E:K takes --op alltoall, -d and --out-dtype bfloat16|half|float, a --row-len that is a multiple of 16, E a multiple of the\n"
-                      "number of ranks, and no --block-scale or --combine; with --quantize WIRE:BLOCK (the FP8 dispatch) a --row-len that is a\n"
-                      "multiple of BLOCK\n");
-      return 2;
-    }
-    return run_route(o, ctx, sh, send, st, e0, e1);
-  }
+  if (o.combine_k) return run_combine(o, ctx, send, recv);
+  if (o.route_e) return run_route(o, ctx, send);
   const bool bs_mode = o.bs_rows > 0, q_mode = o.q_block > 0, is_a2a = o.op == "alltoall";
-  const bool wide_in = o.in_dt == b200collBfloat16 || o.in_dt == b200collFloat16 || o.in_dt == b200collFloat32;
-  const bool wide_out = o.out_dt == b200collBfloat16 || o.out_dt == b200collFloat16 || o.out_dt == b200collFloat32;
-  if (q_mode && ((o.op != "all_gather" && o.op != "reduce_scatter" && o.op != "all_reduce" && !is_a2a) || bs_mode || !wide_in ||
-                 (is_a2a ? o.out_dt != o.q_wire || o.row_len % o.q_block != 0 : !wide_out))) {
-    fprintf(stderr, "--quantize takes --op all_gather, reduce_scatter or all_reduce with -d and --out-dtype bfloat16|half|float, or --op alltoall with\n"
-                    "-d bfloat16|half|float, --out-dtype WIRE (or none) and a --row-len that is a multiple of BLOCK; and no --block-scale\n");
-    return 2;
-  }
   float* q_scales = nullptr;                                     // quantising alltoall: the received scales, one window of them
   if (q_mode && is_a2a) CC(b200collMemAlloc(ctx.comm, (void**)&q_scales, q_a2a_scale_bytes(o)));
   float* scales = nullptr;
   std::vector<float> host_scales;
-  if (bs_mode) {
-    if (o.op != "all_gather" && o.op != "reduce_scatter" && o.op != "all_reduce") { fprintf(stderr, "--block-scale takes --op all_gather, reduce_scatter or all_reduce\n"); return 2; }
-    CC(b200collMemAlloc(ctx.comm, (void**)&scales, bs_max_scales(o) * 4));
-  }
+  if (bs_mode) CC(b200collMemAlloc(ctx.comm, (void**)&scales, bs_max_scales(o) * 4));
   b200collEpilogue ep{o.in_dt, o.out_dt, o.scale};
-  int gen_ctr[4] = {0, 0, 0, 0};
   std::vector<char> host;
   b200collCommInfo info; CC(b200collCommInfoGet(ctx.comm, &info));
   if (rank == 0) {
@@ -877,24 +805,8 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
       if (o.check) {
         if (!ip) RT(cudaMemsetAsync(rbuf(0), 0x5A, out_b, st));
         if (q_mode && is_a2a) RT(cudaMemsetAsync(qsbuf(0), 0x5A, out_elems / o.q_block * 4, st));
-        if (q_mode) {
-          void* p = sbuf(0);
-          if (o.in_dt == b200collFloat32) k_fill_q<float><<<256, 256, 0, st>>>((float*)p, in_elems, rank, o.q_block);
-          else if (o.in_dt == b200collFloat16) k_fill_q<__half><<<256, 256, 0, st>>>((__half*)p, in_elems, rank, o.q_block);
-          else k_fill_q<__nv_bfloat16><<<256, 256, 0, st>>>((__nv_bfloat16*)p, in_elems, rank, o.q_block);
-          RT(cudaGetLastError());
-        }
-        else if (ip && is_ag) fill(sbuf(0), in_elems, o.in_dt, rank, 0, st);
-        else if (ip && is_rs) fill((char*)recv, in_elems, o.in_dt, rank, 0, st);
-        else fill(sbuf(0), in_elems, o.in_dt, rank, 0, st);
-        RT(cudaStreamSynchronize(st));
-        spin_barrier(sh, 0, n, &gen_ctr[0]);
-        if (o.skew_us && rank == 0) usleep(o.skew_us);
-        launch(0);
-        RT(cudaStreamSynchronize(st));
-        spin_barrier(sh, 1, n, &gen_ctr[1]);
-        b200collFault f;
-        if (b200collCommGetAsyncError(ctx.comm, &f) != b200collSuccess) { fprintf(stderr, "rank %d WATCHDOG code=%u peer=%u block=%u expected=%u observed=%u op=%u\n", rank, f.code, f.peer, f.block, f.expected, f.observed, f.op); _exit(5); }
+        fill(sbuf(0), in_elems, o.in_dt, rank, st, o.q_block);       // in-place reduce-scatter: sbuf(0) is recv
+        check_launch(o, ctx, launch);
         const char* outp = (ip && is_rs) ? rbuf(0) : (ip ? (char*)recv : rbuf(0));
         const size_t check_elems = ((is_rd || (is_ga && !is_hc)) && rank != kRoot) ? 0 : out_elems;   // a rooted reduce defines the root's output only
         host.resize(check_elems * os);
@@ -940,23 +852,8 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
           if (!(fabsf(got - want) <= tol)) { if (errs < 4) fprintf(stderr, "rank %d %s size %zu %s elem %zu: got %g want %g\n", rank, o.op.c_str(), bytes, ip ? "ip" : "oop", e, got, want); errs++; }
         }
       }
-      // ---- timing
-      for (int i = 0; i < o.warmup; i++) launch(i % slots);
-      RT(cudaStreamSynchronize(st));
-      spin_barrier(sh, 2, n, &gen_ctr[2]);
-      RT(cudaEventRecord(e0, st));
-      for (int i = 0; i < o.iters; i++) launch(i % slots);
-      RT(cudaEventRecord(e1, st));
-      RT(cudaEventSynchronize(e1));
-      float ms = 0; RT(cudaEventElapsedTime(&ms, e0, e1));
-      sh->ms[rank] = ms / o.iters; sh->errors[rank] = errs;
-      spin_barrier(sh, 3, n, &gen_ctr[3]);
-      float worst = 0; long es = 0;
-      for (int r = 0; r < n; r++) { worst = std::max(worst, sh->ms[r]); es += sh->errors[r]; }
-      res_us[ip] = worst * 1e3; res_err[ip] = es; total_errors += es;
-      spin_barrier(sh, 0, n, &gen_ctr[0]);   // keep ms[] stable until everyone has read it
-      b200collFault f;
-      if (b200collCommGetAsyncError(ctx.comm, &f) != b200collSuccess) { fprintf(stderr, "rank %d WATCHDOG (timing) code=%u peer=%u block=%u expected=%u observed=%u\n", rank, f.code, f.peer, f.block, f.expected, f.observed); _exit(5); }
+      const Timing tm = timed(o, ctx, errs, [&](int i) { launch(i % slots); });
+      res_us[ip] = tm.ms * 1e3; res_err[ip] = tm.errors; total_errors += tm.errors;
     }
     if (rank == 0) {
       size_t tb = is_ar ? count * is : count * is * n;   // nccl-tests "size"
@@ -998,11 +895,11 @@ static int run_rank(const Opts& o, RankCtx ctx, Shared* sh) {
 // gpudirect-tcpx/nccl-config.yaml:61-62, gpudirect-rdma/nccl-test-a4x-max-jobset.yaml:153): the binary answers to those
 // names through symlinks, takes the same flags, and when a launcher exported a rank (OpenMPI, PMI, torchrun) it is ONE rank
 // of the job instead of forking its own.
+static const struct { const char* name; const char* op; } kOps[] = {{"all_reduce_perf", "all_reduce"}, {"all_gather_perf", "all_gather"}, {"reduce_scatter_perf", "reduce_scatter"},
+                                                                    {"alltoall_perf", "alltoall"}, {"broadcast_perf", "broadcast"}, {"reduce_perf", "reduce"}, {"sendrecv_perf", "sendrecv"}, {"gather_perf", "gather"}, {"scatter_perf", "scatter"}, {"hypercube_perf", "hypercube"}};
 static const char* op_from_argv0(const char* argv0) {
   const char* base = strrchr(argv0, '/'); base = base ? base + 1 : argv0;
-  static const struct { const char* name; const char* op; } kNames[] = {{"all_reduce_perf", "all_reduce"}, {"all_gather_perf", "all_gather"}, {"reduce_scatter_perf", "reduce_scatter"},
-                                                                        {"alltoall_perf", "alltoall"}, {"broadcast_perf", "broadcast"}, {"reduce_perf", "reduce"}, {"sendrecv_perf", "sendrecv"}, {"gather_perf", "gather"}, {"scatter_perf", "scatter"}, {"hypercube_perf", "hypercube"}};
-  for (auto& k : kNames) if (!strcmp(base, k.name)) return k.op;
+  for (auto& k : kOps) if (!strcmp(base, k.name)) return k.op;
   return nullptr;
 }
 struct LauncherRank { int rank = -1, size = 0, local_rank = 0; std::string job; };
@@ -1023,6 +920,63 @@ static LauncherRank launcher_rank() {
   for (const char* k : {"B200COLL_JOB_ID", "OMPI_MCA_ess_base_jobid", "PMIX_NAMESPACE", "PMI_JOBID", "TORCHELASTIC_RUN_ID"}) if (const char* v = getenv(k)) { l.job = std::string(k) + "=" + v; break; }
   if (l.job.empty()) { const char* a = getenv("MASTER_ADDR"); const char* p = getenv("MASTER_PORT"); l.job = std::string(a ? a : "local") + ":" + (p ? p : "0"); }
   return l;
+}
+
+// Every conflict between flags and with the number of ranks (o.nranks), refused before any communicator or buffer exists.
+static bool flags_ok(const Opts& o) {
+  const int n = o.nranks;
+  if (o.rms_row && (o.op != "all_reduce" || o.out_dt != o.in_dt || o.scale != 1.0f || o.q_block || o.bs_rows || o.combine_k || o.route_e || o.cq_block ||
+                    !wide(o.in_dt))) {
+    fprintf(stderr, "--rms-norm ROW_LEN takes --op all_reduce and -d bfloat16|half|float, and no --out-dtype, --scale, --quantize, --block-scale, --combine\n"
+                    "or --route\n");
+    return false;
+  }
+  if (o.cq_block && ((!o.combine_k && !o.route_e) || o.q_block || o.bs_rows || o.row_len % o.cq_block != 0)) {
+    fprintf(stderr, "--combine-quantize WIRE:BLOCK takes --combine K or --route E:K, a --row-len that is a multiple of BLOCK, and no --quantize or\n"
+                    "--block-scale\n");
+    return false;
+  }
+  if (o.bs_rows && (o.row_len == 0 || o.row_len % 16)) { fprintf(stderr, "--row-len must be a positive multiple of 16\n"); return false; }
+  if (o.op == "hypercube" && (n & (n - 1))) { fprintf(stderr, "hypercube needs a power-of-two number of ranks\n"); return false; }
+  if ((o.op == "sendrecv" || o.op == "gather" || o.op == "hypercube" || o.op == "scatter") && (o.in_dt != o.out_dt || o.scale != 1.0f)) {
+    fprintf(stderr, "%s moves opaque bytes: --in and --out must match and --scale must be 1\n", o.op.c_str());
+    return false;
+  }
+  if (std::none_of(std::begin(kOps), std::end(kOps), [&](const auto& k) { return o.op == k.op; })) { fprintf(stderr, "unknown --op %s\n", o.op.c_str()); return false; }
+  if (o.combine_k && (o.op != "alltoall" || o.q_block || o.bs_rows || o.row_len == 0 || o.row_len % 16 || !wide(o.in_dt) || !wide(o.out_dt))) {
+    fprintf(stderr, "--combine K takes --op alltoall, -d and --out-dtype bfloat16|half|float, a --row-len that is a multiple of 16, and no --quantize or --block-scale\n");
+    return false;
+  }
+  if (o.combine_k) return true;           // --combine runs the combine mode, whatever --route says
+  // with --quantize there is no combine, so no out type: the quantising alltoall defaults --out-dtype to the wire type
+  if (o.route_e && (o.op != "alltoall" || o.bs_rows || o.row_len == 0 || o.row_len % 16 || !wide(o.in_dt) || (!o.q_block && !wide(o.out_dt)) ||
+                    o.route_e % n != 0 || (o.q_block && o.row_len % o.q_block != 0))) {
+    fprintf(stderr, "--route E:K takes --op alltoall, -d and --out-dtype bfloat16|half|float, a --row-len that is a multiple of 16, E a multiple of the\n"
+                    "number of ranks, and no --block-scale or --combine; with --quantize WIRE:BLOCK (the FP8 dispatch) a --row-len that is a\n"
+                    "multiple of BLOCK\n");
+    return false;
+  }
+  if (o.route_e) return true;             // --quantize with --route is the FP8 dispatch, checked above
+  const bool is_a2a = o.op == "alltoall";
+  if (o.q_block && ((o.op != "all_gather" && o.op != "reduce_scatter" && o.op != "all_reduce" && !is_a2a) || o.bs_rows || !wide(o.in_dt) ||
+                    (is_a2a ? o.out_dt != o.q_wire || o.row_len % o.q_block != 0 : !wide(o.out_dt)))) {
+    fprintf(stderr, "--quantize takes --op all_gather, reduce_scatter or all_reduce with -d and --out-dtype bfloat16|half|float, or --op alltoall with\n"
+                    "-d bfloat16|half|float, --out-dtype WIRE (or none) and a --row-len that is a multiple of BLOCK; and no --block-scale\n");
+    return false;
+  }
+  if (o.bs_rows && o.op != "all_gather" && o.op != "reduce_scatter" && o.op != "all_reduce") {
+    fprintf(stderr, "--block-scale takes --op all_gather, reduce_scatter or all_reduce\n");
+    return false;
+  }
+  return true;
+}
+
+// The arena every rank needs: the send and receive windows (or the largest buffers), 64 MiB of slack, and what each mode adds.
+static size_t arena_bytes(const Opts& o) {
+  const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt);
+  return std::max(o.window, o.max_bytes) + std::max(o.window / is * os, o.max_bytes / is * os) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) +
+         q_scratch_bytes(o) + (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o) +     // --route: recv holds K rows per token
+         (o.rms_row ? o.max_bytes + 4096 : 0);                                                                                  // --rms-norm: the residual
 }
 
 int main(int argc, char** argv) {
@@ -1048,22 +1002,8 @@ int main(int argc, char** argv) {
     else if (a == "--out-dtype") { o.out_dt = parse_dt(next()); out_given = true; }
     else if (a == "--block-scale") { if (sscanf(next(), "%dx%d", &o.bs_rows, &o.bs_cols) != 2 || o.bs_rows < 1 || o.bs_cols < 16 || o.bs_cols % 16) { fprintf(stderr, "--block-scale RxC: R >= 1, C a multiple of 16\n"); return 1; } }
     else if (a == "--row-len") o.row_len = (size_t)atoll(next());
-    else if (a == "--quantize") {
-      char wire[16] = {};
-      if (sscanf(next(), "%15[a-z0-9]:%d", wire, &o.q_block) != 2 || (strcmp(wire, "e4m3") && strcmp(wire, "e5m2")) || o.q_block < 16 || o.q_block > 512 ||
-          (o.q_block & (o.q_block - 1))) {
-        fprintf(stderr, "--quantize WIRE:BLOCK: WIRE e4m3 or e5m2, BLOCK 16, 32, 64, 128, 256 or 512\n"); return 1;
-      }
-      o.q_wire = parse_dt(wire);
-    }
-    else if (a == "--combine-quantize") {
-      char wire[16] = {};
-      if (sscanf(next(), "%15[a-z0-9]:%d", wire, &o.cq_block) != 2 || (strcmp(wire, "e4m3") && strcmp(wire, "e5m2")) || o.cq_block < 16 || o.cq_block > 512 ||
-          (o.cq_block & (o.cq_block - 1))) {
-        fprintf(stderr, "--combine-quantize WIRE:BLOCK: WIRE e4m3 or e5m2, BLOCK 16, 32, 64, 128, 256 or 512\n"); return 1;
-      }
-      o.cq_wire = parse_dt(wire);
-    }
+    else if (a == "--quantize") parse_wire_block(a, next(), &o.q_wire, &o.q_block);
+    else if (a == "--combine-quantize") parse_wire_block(a, next(), &o.cq_wire, &o.cq_block);
     else if (a == "--rms-norm") {
       const long long v = atoll(next());
       if (v < 16 || v > 16384 || v % 16) { fprintf(stderr, "--rms-norm ROW_LEN: a multiple of 16 in [16, 16384]\n"); return 1; }
@@ -1137,24 +1077,23 @@ int main(int argc, char** argv) {
     else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 1; }
   }
   if (o.factor < 2) o.factor = 2;
-  if (o.rms_row && (o.op != "all_reduce" || o.out_dt != o.in_dt || o.scale != 1.0f || o.q_block || o.bs_rows || o.combine_k || o.route_e || o.cq_block ||
-                    (o.in_dt != b200collBfloat16 && o.in_dt != b200collFloat16 && o.in_dt != b200collFloat32))) {
-    fprintf(stderr, "--rms-norm ROW_LEN takes --op all_reduce and -d bfloat16|half|float, and no --out-dtype, --scale, --quantize, --block-scale, --combine\n"
-                    "or --route\n");
-    return 1;
-  }
-  if (o.cq_block && ((!o.combine_k && !o.route_e) || o.q_block || o.bs_rows || o.row_len % o.cq_block != 0)) {
-    fprintf(stderr, "--combine-quantize WIRE:BLOCK takes --combine K or --route E:K, a --row-len that is a multiple of BLOCK, and no --quantize or\n"
-                    "--block-scale\n");
-    return 1;
-  }
   if (o.q_block && o.op == "alltoall" && !out_given) o.out_dt = o.q_wire;     // the quantising alltoall receives the wire type
-  if (o.bs_rows && (o.row_len == 0 || o.row_len % 16)) { fprintf(stderr, "--row-len must be a positive multiple of 16\n"); return 1; }
   const LauncherRank lr = launcher_rank();
-  if (lr.size > 1 && o.devs.empty() && !o.procs) {
-    // one rank of an mpirun / torchrun job (nccl-tests' -g 1 layout): rendezvous on the job id, timing page in /dev/shm
+  const bool launched = lr.size > 1 && o.devs.empty() && !o.procs;         // one rank of an mpirun / torchrun job (nccl-tests' -g 1 layout)
+  if (launched) {
     if (gpus_per_proc > 1) { fprintf(stderr, "-g %d under a launcher is not supported: run one rank per GPU (-g 1)\n", gpus_per_proc); return 1; }
     if (lr.size > B200COLL_MAX_RANKS) { fprintf(stderr, "libb200coll is an intra-node transport: %d ranks > %d GPUs of one NVSwitch domain\n", lr.size, B200COLL_MAX_RANKS); return 1; }
+    o.nranks = lr.size; o.procs = true;
+  } else {
+    if (gpus_per_proc > 0 && o.nranks == 0) o.nranks = gpus_per_proc;     // nccl-tests -g N without a launcher: N ranks in this process
+    if (!o.devs.empty()) o.nranks = (int)o.devs.size();
+    if (o.nranks == 0) { int nd = 0; cudaGetDeviceCount(&nd); o.nranks = nd > 0 ? nd : 1; }     // no rank count given: one rank per GPU
+  }
+  if (!flags_ok(o)) return 1;
+  b200collConfig cfg; b200collConfigDefault(&cfg);
+  if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = arena_bytes(o);
+  if (launched) {
+    // rendezvous on the job id, timing page in /dev/shm
     int nd = 0; RT(cudaGetDeviceCount(&nd));
     const int dev = nd > 0 ? lr.local_rank % nd : 0;
     unsigned h = 2166136261u; for (char ch : lr.job) h = (h ^ (unsigned char)ch) * 16777619u;
@@ -1164,12 +1103,6 @@ int main(int argc, char** argv) {
     Shared* sh = (Shared*)mmap(nullptr, sizeof(Shared), PROT_READ | PROT_WRITE, MAP_SHARED, fd, 0);
     close(fd);
     if (sh == MAP_FAILED) { perror("mmap"); return 1; }
-    o.nranks = lr.size; o.procs = true;
-    b200collConfig cfg; b200collConfigDefault(&cfg);
-    const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
-    if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o) +
-                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o) +     // --route: recv holds K rows per token
-                     (o.rms_row ? o.max_bytes + 4096 : 0);                                      // --rms-norm: the residual
     b200collUniqueId id; CC(b200collUniqueIdFromString(("perf/" + lr.job).c_str(), &id));
     RT(cudaSetDevice(dev));
     b200collComm_t comm;
@@ -1179,28 +1112,18 @@ int main(int argc, char** argv) {
     CC(b200collHostBarrier(comm));
     if (lr.rank == 0) memset((void*)sh, 0, sizeof(Shared));
     CC(b200collHostBarrier(comm));
-    int rc = run_rank(o, RankCtx{lr.rank, lr.size, comm, dev}, sh);
+    int rc = run_rank(o, RankCtx{lr.rank, lr.size, comm, dev, sh});
     CC(b200collCommDestroy(comm));          // ends with a host barrier: every rank is past its last use of the page
     if (lr.rank == 0) shm_unlink(shm_name);
     return rc;
   }
-  if (gpus_per_proc > 0 && o.devs.empty() && o.nranks == 0) o.nranks = gpus_per_proc;     // nccl-tests -g N without a launcher: N ranks in this process
-  if (o.devs.empty()) {
+  if (o.devs.empty()) {                     // the ranks take the visible GPUs in turn
     int nd = 0; cudaGetDeviceCount(&nd);
-    if (o.nranks == 0) o.nranks = nd > 0 ? nd : 1;
     for (int i = 0; i < o.nranks; i++) o.devs.push_back(nd > 0 ? i % nd : 0);
   }
-  o.nranks = (int)o.devs.size();
   const int n = o.nranks;
   Shared* sh = (Shared*)mmap(nullptr, sizeof(Shared), PROT_READ | PROT_WRITE, MAP_SHARED | MAP_ANONYMOUS, -1, 0);
   memset(sh, 0, sizeof(Shared));
-  b200collConfig cfg; b200collConfigDefault(&cfg);
-  // arena: two windows (+ max buffers) and slack
-  const size_t is_ = b200collTypeSize(o.in_dt), os_ = b200collTypeSize(o.out_dt);
-  size_t need = std::max(o.window, o.max_bytes) + std::max(o.window / is_ * os_, o.max_bytes / is_ * os_) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) + q_scratch_bytes(o) +
-                     (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o) +     // --route: recv holds K rows per token
-                     (o.rms_row ? o.max_bytes + 4096 : 0);                                      // --rms-norm: the residual
-  if (!getenv("B200COLL_ARENA_MB")) cfg.arena_bytes = need;
   if (o.procs) {
     b200collUniqueId id; CC(b200collGetUniqueId(&id));
     std::vector<pid_t> kids;
@@ -1210,7 +1133,7 @@ int main(int argc, char** argv) {
         RT(cudaSetDevice(o.devs[r]));
         b200collComm_t comm;
         CC(b200collCommInitRank(&comm, n, &id, r, &cfg));
-        int rc = run_rank(o, RankCtx{r, n, comm, o.devs[r]}, sh);
+        int rc = run_rank(o, RankCtx{r, n, comm, o.devs[r], sh});
         CC(b200collCommDestroy(comm));
         _exit(rc);
       }
@@ -1224,7 +1147,7 @@ int main(int argc, char** argv) {
   CC(b200collCommInitAll(comms.data(), n, o.devs.data(), &cfg));
   std::vector<std::thread> th;
   std::vector<int> rcs(n, 0);
-  for (int r = 0; r < n; r++) th.emplace_back([&, r] { rcs[r] = run_rank(o, RankCtx{r, n, comms[r], o.devs[r]}, sh); });
+  for (int r = 0; r < n; r++) th.emplace_back([&, r] { rcs[r] = run_rank(o, RankCtx{r, n, comms[r], o.devs[r], sh}); });
   for (auto& t : th) t.join();
   for (int r = 0; r < n; r++) CC(b200collCommDestroy(comms[r]));
   int worst = 0; for (int rc : rcs) worst = std::max(worst, rc);
