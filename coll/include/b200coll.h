@@ -493,6 +493,35 @@ b200collResult_t b200collExpertCombineQuantized(const void* expert_out, void* ou
  * bytes under oneshot, twoshot or copy, one kernel launch. */
 b200collResult_t b200collAllReduceRmsNorm(const void* x, void* residual, const void* gamma, void* out, size_t rows, size_t row_len,
                                           float eps, b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
+/* Fused all-reduce, residual add, RMSNorm and FP8 block quantisation: the normed rows go straight to an FP8 GEMM (the QKV projection after
+ * the attention norm, the gate/up projection after the MLP norm) as e4m3 or e5m2 rows with one fp32 scale per 1 x block group, in one
+ * kernel per call. Steps 1-4 are b200collAllReduceRmsNorm's, unchanged, and residual receives the same bits in place. Then, per row:
+ *   5. o[e] = round_dtype((h[e] * inv) * gamma[e]): the value b200collAllReduceRmsNorm stores in out.
+ *   6. The row is cut into blocks of `block` consecutive elements, and each block of o, widened exactly to fp32, is quantised by the rule
+ *      of the quantising collectives: amax the largest bit pattern of |o| (a NaN anywhere makes amax NaN); inv = FMAX / amax and
+ *      s = amax / FMAX, IEEE divisions rounded to nearest, inv = s = 1 when amax == 0 or inv is +inf; q = satfinite RNE(o * inv). FMAX is
+ *      448 (e4m3) or 57344 (e5m2).
+ * q: [rows, row_len] of wire_dtype. scales: [rows, row_len / block] fp32, row-major: the block_rows = 1, block_cols = block layout of
+ * b200collBlockScale, so q and scales are also an input of b200collAllGatherBlockScaled.
+ * Equivalence: the result is b200collAllReduceRmsNorm's out quantised by b200collAllToAllvQuantized's rule, bit for bit. Step 6 quantises
+ * the rounded o, not the fp32 product, which is what makes this hold (for fp32 the two are the same). A block whose o holds a NaN comes
+ * out as NaN codes throughout with a NaN scale: a NaN in h makes the whole row's o NaN, as does an all-zero row with eps = 0, and an inf
+ * in h makes that element's o NaN and the rest of the row +-0 (inv = 0), so its block is NaN and the others are zeros with s = 1. An
+ * all-zero row with eps > 0 gives q = 0 and s = 1.
+ * Arguments: everything b200collAllReduceRmsNorm refuses is refused the same way (with q in place of out). Also InvalidArgument, before
+ * anything is launched: wire_dtype not e4m3 or e5m2; block not 16, 32, 64, 128, 256 or 512; row_len % block != 0; q not 16-byte aligned
+ * or scales not 4-byte aligned; q or scales null when rows > 0; any overlap among x, residual, gamma, q and scales. rows == 0 behaves as
+ * in b200collAllReduceRmsNorm.
+ * Algorithms and placement as in b200collAllReduceRmsNorm, with q and scales in place of out: the tuner's all-reduce pick for
+ * rows * row_len * sizeof(dtype) bytes, or the forced algorithm; ll, ll2 and oneshot -> oneshot; twoshot and nvls -> twoshot, which
+ * needs residual, q and scales in the arena and falls back to oneshot otherwise. Two-shot pushes FP8 rows and scales to the peers,
+ * row_len * (1 + 4 / block) bytes per row instead of row_len * sizeof(dtype). B200COLL_CHECK=1 cross-checks rows, row_len, the x offset,
+ * the algorithm, the two-shot offsets of residual, q and scales, and (block, wire_dtype). The kernel ends with a releasing barrier, so the
+ * caller may overwrite x right after the call. b200collStats count an allreduce of rows * row_len * sizeof(dtype) bytes under oneshot,
+ * twoshot or copy, one kernel launch. */
+b200collResult_t b200collAllReduceRmsNormQuantized(const void* x, void* residual, const void* gamma, void* q, float* scales, size_t rows,
+                                                   size_t row_len, float eps, b200collDataType_t dtype, b200collDataType_t wire_dtype,
+                                                   int block, b200collComm_t comm, b200collStream_t stream);
 
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.

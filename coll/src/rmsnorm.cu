@@ -6,6 +6,12 @@
 //   k_rms_twoshot<T>     relaxed barrier, pull my row slice, push its residual and out rows into every rank's residual and out, releasing
 //                        barrier
 //
+// and the quantising call (b200collAllReduceRmsNormQuantized), the same three kernels with step 6 in place of the out store:
+//
+//   k_rmsq_local<T, WireT>, k_rmsq_oneshot<T, WireT>, k_rmsq_twoshot<T, WireT>
+//                        o = round_T((h * inv) * gamma) quantised per block of the row with quant.cuh's quant_vec: q and the block scales
+//                        stored locally, or (two-shot) pushed into every rank's q and scales
+//
 // One CTA (kRmsThreads threads) owns one row at a time, walking rows b, b + gridDim.x, ... of its range. Thread t holds the 16-element
 // chunks t and t + kRmsThreads (row_len <= 16384 is at most 1024 chunks), so the new residual h of a whole row stays in registers
 // between the sum and the normalisation.
@@ -28,6 +34,11 @@
 // still read. The closing barrier releases the two-shot stores to every rank and tells each rank that nobody pulls its x any more, so the
 // caller may overwrite x right after the call. Both barriers pair CTA b with CTA b, and every rank launches full_grid's CTAs whatever its
 // row count.
+//
+// Step 6. A quantising block is 1 to 32 chunks (16 to 512 elements, a power of two) and row_len is a multiple of it, so the chunks of
+// one block are consecutive lanes of one warp (chunk t or t + 512 of thread t), starting on an aligned group of lanes: the contract of
+// quant_vec. Lanes past the row pass zeros, and they make up whole groups; a warp wholly past the row skips the step. The lowest lane of
+// each group stores the block's scale.
 #include <stdint.h>
 
 #include <atomic>
@@ -36,6 +47,7 @@
 
 #include "comm.h"
 #include "launch.cuh"
+#include "quant.cuh"
 
 namespace b200coll {
 
@@ -69,10 +81,20 @@ struct RmsArgs {
   float eps;
 };
 
+// What the quantising kernels add: where q and the scales of row `row` go, and the block. q: [rows, row_len] FP8, scales:
+// [rows, row_len / block] fp32. Local pointers, or (PUSH) arena offsets q_off / s_off stored into every rank.
+struct RmsQuant {
+  char* q;
+  char* scales;
+  size_t q_off, s_off;
+  uint32_t lvpb;                // log2(chunks per block)
+};
+
 // One row: h = round((+0 + x_0 + .. + x_{N-1}) + residual), residual = h, out = round((h * inv) * gamma), inv = 1 / sqrt(fold / row_len + eps).
 // LOCAL: one rank, x is a.x_local; else rank r's x is at a.x_off of its arena. sbuf: this row's 512 floats of shared memory.
-template <typename T, bool LOCAL, bool PUSH>
-__device__ __forceinline__ void rms_row(const CommDev& c, const RmsArgs& a, size_t row, float* sbuf) {
+// WireT void: out is stored (qa unused); else out is quantised to WireT per block into qa's q and scales.
+template <typename T, typename WireT, bool LOCAL, bool PUSH>
+__device__ __forceinline__ void rms_row(const CommDev& c, const RmsArgs& a, const RmsQuant& qa, size_t row, float* sbuf) {
   const int t = threadIdx.x, lane = t & 31;
   const size_t row_bytes = (size_t)a.row_len * sizeof(T);
   float h[2][16];
@@ -128,23 +150,62 @@ __device__ __forceinline__ void rms_row(const CommDev& c, const RmsArgs& a, size
 #pragma unroll
   for (int l = 4; l >= 0; l--) f = __fadd_rn(f, __shfl_xor_sync(0xFFFFFFFFu, f, 1 << l));
   const float inv = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(__fdiv_rn(f, (float)a.row_len), a.eps)));
+  if constexpr (std::is_void<WireT>::value) {
 #pragma unroll
-  for (int k = 0; k < 2; k++) {
-    const uint32_t ch = (uint32_t)t + (uint32_t)k * kRmsThreads;
-    if (ch < a.nchunks) {
-      const size_t off = row * row_bytes + (size_t)ch * 16 * sizeof(T);
-      float g[16], o[16];
-      rms_load16<T>(a.gamma + (size_t)ch * 16 * sizeof(T), g);
+    for (int k = 0; k < 2; k++) {
+      const uint32_t ch = (uint32_t)t + (uint32_t)k * kRmsThreads;
+      if (ch < a.nchunks) {
+        const size_t off = row * row_bytes + (size_t)ch * 16 * sizeof(T);
+        float g[16], o[16];
+        rms_load16<T>(a.gamma + (size_t)ch * 16 * sizeof(T), g);
 #pragma unroll
-      for (int i = 0; i < 16; i++) o[i] = __fmul_rn(__fmul_rn(h[k][i], inv), g[i]);
-      if (PUSH) {
+        for (int i = 0; i < 16; i++) o[i] = __fmul_rn(__fmul_rn(h[k][i], inv), g[i]);
+        if (PUSH) {
 #pragma unroll
-        for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
-          int q = c.rank + j; if (q >= c.nranks) q -= c.nranks;
-          store16_scaled<T>(c.peer[q] + a.out_off + off, o, 1.0f);
+          for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
+            int q = c.rank + j; if (q >= c.nranks) q -= c.nranks;
+            store16_scaled<T>(c.peer[q] + a.out_off + off, o, 1.0f);
+          }
+        } else {
+          store16_scaled<T>(a.out + off, o, 1.0f);
         }
+      }
+    }
+  } else {
+    // step 6, one chunk at a time: o as the wide call would store it, widened back, then quantised with its block's amax
+    const uint32_t gl = 1u << qa.lvpb;
+    const size_t q_row = row * a.row_len, s_row = row * (a.nchunks >> qa.lvpb);
+#pragma unroll
+    for (int k = 0; k < 2; k++) {
+      const uint32_t ch = (uint32_t)t + (uint32_t)k * kRmsThreads;
+      if ((ch & ~31u) >= a.nchunks) continue;                        // the whole warp is past the row
+      const bool act = ch < a.nchunks;
+      float o[16];
+      if (act) {
+        float g[16];
+        rms_load16<T>(a.gamma + (size_t)ch * 16 * sizeof(T), g);
+#pragma unroll
+        for (int i = 0; i < 16; i++) o[i] = round_to<T>(__fmul_rn(__fmul_rn(h[k][i], inv), g[i]));
       } else {
-        store16_scaled<T>(a.out + off, o, 1.0f);
+#pragma unroll
+        for (int i = 0; i < 16; i++) o[i] = 0.f;
+      }
+      float s;
+      const uint4 w = quant_vec<WireT>(o, gl, &s);
+      if (act) {
+        const size_t q_off = q_row + (size_t)ch * 16, s_off = (s_row + (ch >> qa.lvpb)) * 4;
+        const bool lead = (lane & (gl - 1)) == 0;
+        if (PUSH) {
+#pragma unroll
+          for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
+            int q = c.rank + j; if (q >= c.nranks) q -= c.nranks;
+            st_vec(c.peer[q] + qa.q_off + q_off, w);
+            if (lead) *reinterpret_cast<float*>(c.peer[q] + qa.s_off + s_off) = s;
+          }
+        } else {
+          st_vec(qa.q + q_off, w);
+          if (lead) *reinterpret_cast<float*>(qa.scales + s_off) = s;
+        }
       }
     }
   }
@@ -152,49 +213,85 @@ __device__ __forceinline__ void rms_row(const CommDev& c, const RmsArgs& a, size
 
 // Rows [r0, r1), CTA b taking r0 + b, r0 + b + gridDim.x, ...; the shared buffer alternates by row so that one block barrier per row
 // suffices (a warp that writes row i + 2's buffer has passed row i + 1's barrier, which every warp reaches only after reading row i's).
-template <typename T, bool LOCAL, bool PUSH>
-__device__ __forceinline__ void rms_rows(const CommDev& c, const RmsArgs& a, uint32_t r0, uint32_t r1) {
+template <typename T, typename WireT, bool LOCAL, bool PUSH>
+__device__ __forceinline__ void rms_rows(const CommDev& c, const RmsArgs& a, const RmsQuant& qa, uint32_t r0, uint32_t r1) {
   __shared__ float sbuf[2][kRmsThreads];
   uint32_t i = 0;
-  for (uint32_t row = r0 + blockIdx.x; row < r1; row += gridDim.x, i ^= 1) rms_row<T, LOCAL, PUSH>(c, a, row, sbuf[i]);
+  for (uint32_t row = r0 + blockIdx.x; row < r1; row += gridDim.x, i ^= 1) rms_row<T, WireT, LOCAL, PUSH>(c, a, qa, row, sbuf[i]);
 }
 
-template <typename T>
-__global__ void __launch_bounds__(kRmsThreads, 1) k_rms_local(COMM_PARAM, const __grid_constant__ RmsArgs a, uint32_t rows) {
+// The kernel bodies, shared by the wide kernels (WireT void) and the quantising ones.
+template <typename T, typename WireT>
+__device__ __forceinline__ void rms_local(const CommDev& c, const RmsArgs& a, const RmsQuant& qa, uint32_t rows) {
   pdl_prologue();
-  rms_rows<T, true, false>(c, a, 0, rows);
+  rms_rows<T, WireT, true, false>(c, a, qa, 0, rows);
 }
 
-template <typename T>
-__global__ void __launch_bounds__(kRmsThreads, 1) k_rms_oneshot(COMM_PARAM, const __grid_constant__ RmsArgs a, uint32_t rows, uint32_t op) {
+template <typename T, typename WireT>
+__device__ __forceinline__ void rms_oneshot(const CommDev& c, const RmsArgs& a, const RmsQuant& qa, uint32_t rows, uint32_t op) {
   pdl_prologue();
   {
     const uint32_t s = load_seq(c, kSeqBarrier);
     if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every rank's x is written
   }
-  rms_rows<T, false, false>(c, a, 0, rows);
+  rms_rows<T, WireT, false, false>(c, a, qa, 0, rows);
   const uint32_t s = load_seq(c, kSeqBarrier);
   if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // nobody reads my x any more
   if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
 }
 
-template <typename T>
-__global__ void __launch_bounds__(kRmsThreads, 1) k_rms_twoshot(COMM_PARAM, const __grid_constant__ RmsArgs a, uint32_t rows, uint32_t op) {
+template <typename T, typename WireT>
+__device__ __forceinline__ void rms_twoshot(const CommDev& c, const RmsArgs& a, const RmsQuant& qa, uint32_t rows, uint32_t op) {
   pdl_prologue();
   {
     const uint32_t s = load_seq(c, kSeqBarrier);
-    if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every rank's x is written, and its residual and out are free
+    if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every rank's x is written, and its residual and out (q, scales) are free
   }
   const uint32_t r0 = (uint32_t)((unsigned long long)rows * c.rank / c.nranks), r1 = (uint32_t)((unsigned long long)rows * (c.rank + 1) / c.nranks);
-  rms_rows<T, false, true>(c, a, r0, r1);
+  rms_rows<T, WireT, false, true>(c, a, qa, r0, r1);
   const uint32_t s = load_seq(c, kSeqBarrier);
   if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // my rows are in every rank's residual and out; nobody reads my x
   if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
 }
 
-// Once per device, before the first kernel of this family launches: load all nine kernels. With lazy module loading a kernel's first
-// launch loads it, and the load waits for kernels already running; a rank whose first launch of one of these kernels came behind its own
-// barrier kernel, which waits for another rank's launch on the same thread, would never get there. One thread loads at a time.
+template <typename T>
+__global__ void __launch_bounds__(kRmsThreads, 1) k_rms_local(COMM_PARAM, const __grid_constant__ RmsArgs a, uint32_t rows) {
+  rms_local<T, void>(c, a, RmsQuant{}, rows);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kRmsThreads, 1) k_rms_oneshot(COMM_PARAM, const __grid_constant__ RmsArgs a, uint32_t rows, uint32_t op) {
+  rms_oneshot<T, void>(c, a, RmsQuant{}, rows, op);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kRmsThreads, 1) k_rms_twoshot(COMM_PARAM, const __grid_constant__ RmsArgs a, uint32_t rows, uint32_t op) {
+  rms_twoshot<T, void>(c, a, RmsQuant{}, rows, op);
+}
+
+// 16-bit T: 2 CTAs per SM (at most 64 registers), as the 16-bit wide local kernels fit; fp32 would spill there
+template <typename T, typename WireT>
+__global__ void __launch_bounds__(kRmsThreads, sizeof(T) == 2 ? 2 : 1) k_rmsq_local(COMM_PARAM, const __grid_constant__ RmsArgs a, const __grid_constant__ RmsQuant qa,
+                                                                uint32_t rows) {
+  rms_local<T, WireT>(c, a, qa, rows);
+}
+
+template <typename T, typename WireT>
+__global__ void __launch_bounds__(kRmsThreads, 1) k_rmsq_oneshot(COMM_PARAM, const __grid_constant__ RmsArgs a, const __grid_constant__ RmsQuant qa,
+                                                                  uint32_t rows, uint32_t op) {
+  rms_oneshot<T, WireT>(c, a, qa, rows, op);
+}
+
+template <typename T, typename WireT>
+__global__ void __launch_bounds__(kRmsThreads, 1) k_rmsq_twoshot(COMM_PARAM, const __grid_constant__ RmsArgs a, const __grid_constant__ RmsQuant qa,
+                                                                  uint32_t rows, uint32_t op) {
+  rms_twoshot<T, WireT>(c, a, qa, rows, op);
+}
+
+// Once per device, before the first kernel of this family launches: load all 27 kernels, wide and quantising. With lazy module loading a
+// kernel's first launch loads it, and the load waits for kernels already running; a rank whose first launch of one of these kernels came
+// behind its own barrier kernel, which waits for another rank's launch on the same thread, would never get there. One thread loads at a
+// time.
 static void rmsnorm_preload(const b200collComm* c) {
   static std::atomic<unsigned long long> done{0};
   static std::mutex mu;
@@ -209,55 +306,83 @@ static void rmsnorm_preload(const b200collComm* c) {
       cudaFuncGetAttributes(&fa, k_rms_local<T>);
       cudaFuncGetAttributes(&fa, k_rms_oneshot<T>);
       cudaFuncGetAttributes(&fa, k_rms_twoshot<T>);
+      for (b200collDataType_t w : {b200collFloat8e4m3, b200collFloat8e5m2})
+        with_fp8(w, [&](auto tw) {
+          using WireT = typename decltype(tw)::type;
+          cudaFuncGetAttributes(&fa, k_rmsq_local<T, WireT>);
+          cudaFuncGetAttributes(&fa, k_rmsq_oneshot<T, WireT>);
+          cudaFuncGetAttributes(&fa, k_rmsq_twoshot<T, WireT>);
+        });
     });
   done.fetch_or(bit, std::memory_order_acq_rel);
 }
 
-// The argument rules, all before the poisoned-communicator check; nothing is launched on a refusal.
+// What the quantising call passes instead of out.
+struct RmsQuantCall {
+  void* q;
+  float* scales;
+  b200collDataType_t wire;
+  int block;
+};
+
+// The argument rules of both calls (qz == nullptr: b200collAllReduceRmsNorm, whose messages these are), all before the
+// poisoned-communicator check; nothing is launched on a refusal.
 static b200collResult_t rms_prepare(b200collComm* c, const void* x, const void* residual, const void* gamma, const void* out, size_t rows, size_t row_len,
-                                    float eps, b200collDataType_t dtype) {
-  auto refuse = [](const std::string& msg) { set_last_error("all-reduce rms-norm: " + msg); return b200collInvalidArgument; };
+                                    float eps, b200collDataType_t dtype, const RmsQuantCall* qz) {
+  const std::string who = qz ? "quantised all-reduce rms-norm: " : "all-reduce rms-norm: ";
+  auto refuse = [&](const std::string& msg) { set_last_error(who + msg); return b200collInvalidArgument; };
   if (!c) return refuse("null communicator");
   if (!wide_type(dtype)) return refuse("dtype must be bf16, fp16 or fp32");
+  if (qz && !is_fp8(qz->wire)) return refuse("wire_dtype must be e4m3 or e5m2");
+  if (qz && quant_lvpb(qz->block) < 0) return refuse(kBlockRule);
   if (row_len < 16 || row_len > kRmsMaxRowLen || row_len % 16 != 0) return refuse("row_len must be a multiple of 16 in [16, 16384]");
+  if (qz && row_len % (size_t)qz->block != 0) return refuse("row_len must be a multiple of block");
   if (!(eps >= 0.0f) || !isfinite(eps)) return refuse("eps must be finite and non-negative");
   if (rows >= ((size_t)1 << 31)) return refuse("rows must be below 2^31");
-  if (rows > 0 && (!x || !residual || !gamma || !out)) return refuse("null argument");
-  if (!aligned(x, 16) || !aligned(residual, 16) || !aligned(gamma, 16) || !aligned(out, 16)) return refuse("x, residual, gamma and out must be 16-byte aligned");
   const size_t es = b200collTypeSize(dtype), mat = rows * row_len * es, g = row_len * es;
-  if (rows > 0) {
-    if (overlaps(out, mat, x, mat) || overlaps(out, mat, residual, mat) || overlaps(out, mat, gamma, g)) return refuse("out must not overlap x, residual or gamma");
-    if (overlaps(residual, mat, x, mat) || overlaps(residual, mat, gamma, g)) return refuse("residual must not overlap x or gamma");
+  if (!qz) {
+    if (rows > 0 && (!x || !residual || !gamma || !out)) return refuse("null argument");
+    if (!aligned(x, 16) || !aligned(residual, 16) || !aligned(gamma, 16) || !aligned(out, 16)) return refuse("x, residual, gamma and out must be 16-byte aligned");
+    if (rows > 0 && (overlaps(out, mat, x, mat) || overlaps(out, mat, residual, mat) || overlaps(out, mat, gamma, g)))
+      return refuse("out must not overlap x, residual or gamma");
+  } else {
+    if (rows > 0 && (!x || !residual || !gamma || !qz->q || !qz->scales)) return refuse("null argument");
+    if (!aligned(x, 16) || !aligned(residual, 16) || !aligned(gamma, 16) || !aligned(qz->q, 16)) return refuse("x, residual, gamma and q must be 16-byte aligned");
+    if (!aligned(qz->scales, 4)) return refuse("scales must be 4-byte aligned");
+    const size_t qb = rows * row_len, sb = rows * (row_len / (size_t)qz->block) * 4;
+    if (rows > 0 && (overlaps(qz->q, qb, x, mat) || overlaps(qz->q, qb, residual, mat) || overlaps(qz->q, qb, gamma, g) || overlaps(qz->q, qb, qz->scales, sb)))
+      return refuse("q must not overlap x, residual, gamma or scales");
+    if (rows > 0 && (overlaps(qz->scales, sb, x, mat) || overlaps(qz->scales, sb, residual, mat) || overlaps(qz->scales, sb, gamma, g)))
+      return refuse("scales must not overlap x, residual or gamma");
   }
+  if (rows > 0 && (overlaps(residual, mat, x, mat) || overlaps(residual, mat, gamma, g))) return refuse("residual must not overlap x or gamma");
   if (comm_poisoned(c)) return b200collRemoteError;
   return b200collSuccess;
 }
 
-}  // namespace b200coll
-
-using namespace b200coll;
-
-extern "C" {
-
-b200collResult_t b200collAllReduceRmsNorm(const void* x, void* residual, const void* gamma, void* out, size_t rows, size_t row_len, float eps,
-                                          b200collDataType_t dtype, b200collComm_t c, b200collStream_t stream) {
-  b200collResult_t rc = rms_prepare(c, x, residual, gamma, out, rows, row_len, eps, dtype);
-  if (rc != b200collSuccess) return rc;
+// Both calls after their arguments passed: the algorithm, the B200COLL_CHECK=1 cross-check, one launch. qz == nullptr: the wide call.
+static b200collResult_t rms_run(b200collComm* c, const void* x, void* residual, const void* gamma, void* out, size_t rows, size_t row_len, float eps,
+                                b200collDataType_t dtype, const RmsQuantCall* qz, b200collStream_t stream) {
+  const char* who = qz ? "quantised all-reduce rms-norm: " : "all-reduce rms-norm: ";
+  b200collResult_t rc = b200collSuccess;
   const size_t mat = rows * row_len * b200collTypeSize(dtype);
+  const size_t qb = qz ? rows * row_len : 0, sb = qz ? rows * (row_len / (size_t)qz->block) * 4 : 0;
   b200collAlgo_t algo = b200collAlgoCopy;
   if (c->nranks > 1) {
     // peers pull my x at my arena offset. rows == 0 reads nothing (any pointer, even null, will do) and runs one-shot: only the barriers
-    if (rows > 0 && (rc = in_arena(c, "all-reduce rms-norm: ", "x", {{x, mat}})) != b200collSuccess) return rc;
+    if (rows > 0 && (rc = in_arena(c, who, "x", {{x, mat}})) != b200collSuccess) return rc;
     // the tuner's pick for an all-reduce of these bytes, or the forced algorithm: ll, ll2 and oneshot pull every row; twoshot and nvls
-    // push my rows into the peers' residual and out, so both must be arena memory, else one-shot
+    // push my rows into the peers' residual and out (or q and scales), so these must be arena memory, else one-shot
     const b200collAlgo_t want = c->forced_algo != b200collAlgoAuto ? c->forced_algo : b200collTunerPick(b200collOpAllReduce, mat, c->nranks, c->nvls);
     const bool two = rows > 0 && (want == b200collAlgoTwoShot || want == b200collAlgoNvls) && b200collIsSymmetric(c, residual, mat) &&
-                     b200collIsSymmetric(c, out, mat);
+                     (qz ? b200collIsSymmetric(c, qz->q, qb) && b200collIsSymmetric(c, qz->scales, sb) : b200collIsSymmetric(c, out, mat));
     algo = two ? b200collAlgoTwoShot : b200collAlgoOneShot;
-    // (rows, row_len) travel as one number (row_len < 2^15); two-shot adds a second exchange for the residual and out offsets
-    const size_t shape = (rows << 15) | row_len;
-    if ((rc = cross_check(c, b200collOpAllReduce, algo, shape, rows > 0 ? arena_off(c, x) : 0, 0)) != b200collSuccess) return rc;
-    if (two && (rc = cross_check(c, b200collOpAllReduce, algo, shape, arena_off(c, residual), arena_off(c, out))) != b200collSuccess) return rc;
+    // (rows, row_len) travel as one number (row_len < 2^15), and with them the x offset and, quantising, (block, wire); two-shot adds a
+    // second exchange for the residual and out (q) offsets, and quantising a third for the scales offset
+    const size_t shape = (rows << 15) | row_len, fmt = qz ? (size_t)qz->block * 2 + (qz->wire == b200collFloat8e5m2) : 0;
+    if ((rc = cross_check(c, b200collOpAllReduce, algo, shape, rows > 0 ? arena_off(c, x) : 0, fmt)) != b200collSuccess) return rc;
+    if (two && (rc = cross_check(c, b200collOpAllReduce, algo, shape, arena_off(c, residual), arena_off(c, qz ? qz->q : out))) != b200collSuccess) return rc;
+    if (two && qz && (rc = cross_check(c, b200collOpAllReduce, algo, shape, arena_off(c, qz->scales), 0)) != b200collSuccess) return rc;
   }
   const DeviceScope on_device(c->device);
   rmsnorm_preload(c);
@@ -270,29 +395,65 @@ b200collResult_t b200collAllReduceRmsNorm(const void* x, void* residual, const v
   a.row_len = (uint32_t)row_len;
   a.nchunks = (uint32_t)(row_len / 16);
   a.eps = eps;
-  return with_wide(dtype, [&](auto tt) -> b200collResult_t {
-    using T = typename decltype(tt)::type;
-    if (algo == b200collAlgoCopy) {
+  RmsQuant qa = {};
+  if (qz) qa.lvpb = (uint32_t)quant_lvpb(qz->block);
+  // one launch of the local, one-shot or two-shot kernel: the wide one (WireT void) or the quantising one
+  auto launch = [&](auto tt, auto tw) -> b200collResult_t {
+    using T = typename decltype(tt)::type; using WireT = typename decltype(tw)::type;
+    constexpr bool kQuant = !std::is_void<WireT>::value;
+    const uint32_t op = (uint32_t)b200collOpAllReduce;
+    if (algo == b200collAlgoTwoShot) {
+      a.x_off = arena_off(c, x);
+      a.res_off = arena_off(c, residual);
+      if (qz) { qa.q_off = arena_off(c, qz->q); qa.s_off = arena_off(c, qz->scales); }
+      else a.out_off = arena_off(c, out);
+      const Grid gr = full_grid(c, 1);
+      if constexpr (kQuant) launch_k(k_rmsq_twoshot<T, WireT>, gr.blocks, kRmsThreads, st, c->dev, a, qa, (uint32_t)rows, op);
+      else launch_k(k_rms_twoshot<T>, gr.blocks, kRmsThreads, st, c->dev, a, (uint32_t)rows, op);
+    } else {
       a.res_out = static_cast<char*>(residual);
       a.out = static_cast<char*>(out);
-      const int blocks = (int)std::max<size_t>(1, std::min<size_t>(rows, (size_t)2 * std::max(1, c->sm_count)));   // 2 per SM where the registers allow
-      launch_k(k_rms_local<T>, blocks, kRmsThreads, st, c->dev, a, (uint32_t)rows);
-    } else {
-      a.x_off = arena_off(c, x);
-      const Grid gr = full_grid(c, 1);
-      if (algo == b200collAlgoTwoShot) {
-        a.res_off = arena_off(c, residual);
-        a.out_off = arena_off(c, out);
-        launch_k(k_rms_twoshot<T>, gr.blocks, kRmsThreads, st, c->dev, a, (uint32_t)rows, (uint32_t)b200collOpAllReduce);
+      if (qz) { qa.q = static_cast<char*>(qz->q); qa.scales = reinterpret_cast<char*>(qz->scales); }
+      if (algo == b200collAlgoCopy) {
+        const int blocks = (int)std::max<size_t>(1, std::min<size_t>(rows, (size_t)2 * std::max(1, c->sm_count)));   // 2 per SM where the registers allow
+        if constexpr (kQuant) launch_k(k_rmsq_local<T, WireT>, blocks, kRmsThreads, st, c->dev, a, qa, (uint32_t)rows);
+        else launch_k(k_rms_local<T>, blocks, kRmsThreads, st, c->dev, a, (uint32_t)rows);
       } else {
-        a.res_out = static_cast<char*>(residual);
-        a.out = static_cast<char*>(out);
-        launch_k(k_rms_oneshot<T>, gr.blocks, kRmsThreads, st, c->dev, a, (uint32_t)rows, (uint32_t)b200collOpAllReduce);
+        a.x_off = arena_off(c, x);
+        const Grid gr = full_grid(c, 1);
+        if constexpr (kQuant) launch_k(k_rmsq_oneshot<T, WireT>, gr.blocks, kRmsThreads, st, c->dev, a, qa, (uint32_t)rows, op);
+        else launch_k(k_rms_oneshot<T>, gr.blocks, kRmsThreads, st, c->dev, a, (uint32_t)rows, op);
       }
     }
     LAUNCH_CHECK(c);
     return b200collSuccess;
+  };
+  return with_wide(dtype, [&](auto tt) -> b200collResult_t {
+    if (!qz) return launch(tt, Tag<void>{});
+    return with_fp8(qz->wire, [&](auto tw) { return launch(tt, tw); });
   });
+}
+
+}  // namespace b200coll
+
+using namespace b200coll;
+
+extern "C" {
+
+b200collResult_t b200collAllReduceRmsNorm(const void* x, void* residual, const void* gamma, void* out, size_t rows, size_t row_len, float eps,
+                                          b200collDataType_t dtype, b200collComm_t c, b200collStream_t stream) {
+  const b200collResult_t rc = rms_prepare(c, x, residual, gamma, out, rows, row_len, eps, dtype, nullptr);
+  if (rc != b200collSuccess) return rc;
+  return rms_run(c, x, residual, gamma, out, rows, row_len, eps, dtype, nullptr, stream);
+}
+
+b200collResult_t b200collAllReduceRmsNormQuantized(const void* x, void* residual, const void* gamma, void* q, float* scales, size_t rows, size_t row_len,
+                                                   float eps, b200collDataType_t dtype, b200collDataType_t wire_dtype, int block, b200collComm_t c,
+                                                   b200collStream_t stream) {
+  const RmsQuantCall qz = {q, scales, wire_dtype, block};
+  const b200collResult_t rc = rms_prepare(c, x, residual, gamma, nullptr, rows, row_len, eps, dtype, &qz);
+  if (rc != b200collSuccess) return rc;
+  return rms_run(c, x, residual, gamma, nullptr, rows, row_len, eps, dtype, &qz, stream);
 }
 
 }  // extern "C"

@@ -62,6 +62,8 @@ struct Opts {
   int cq_block = 0;               // --combine-quantize WIRE:BLOCK: the quantising combine in --combine / --route (0 = off)
   b200collDataType_t cq_wire = b200collFloat8e4m3;
   size_t rms_row = 0;             // --rms-norm ROW_LEN: the fused all-reduce, residual add and RMSNorm (0 = off)
+  int rq_block = 0;               // --rms-norm-quantize WIRE:BLOCK: its FP8 out, one fp32 scale per 1 x BLOCK (0 = off)
+  b200collDataType_t rq_wire = b200collFloat8e4m3;
 };
 
 // Block-scaled mode: each rank's send buffer is a [rows, row_len] FP8 matrix with one fp32 scale per bs_rows x bs_cols block. Scales are
@@ -113,7 +115,7 @@ static b200collDataType_t parse_dt(const char* s) {
   if (!strcmp(s, "e5m2")) return b200collFloat8e5m2;
   fprintf(stderr, "bad dtype %s\n", s); exit(1);
 }
-// --quantize and --combine-quantize WIRE:BLOCK
+// --quantize, --combine-quantize and --rms-norm-quantize WIRE:BLOCK
 static void parse_wire_block(const std::string& flag, const char* s, b200collDataType_t* wire, int* block) {
   char w[16] = {};
   if (sscanf(s, "%15[a-z0-9]:%d", w, block) != 2 || (strcmp(w, "e4m3") && strcmp(w, "e5m2")) || *block < 16 || *block > 512 || (*block & (*block - 1))) {
@@ -378,6 +380,12 @@ static int run_combine(const Opts& o, RankCtx& ctx, void* expert_out, void* out)
 // repeats steps 1-5 of b200collAllReduceRmsNorm on the host (every sum and product rounded on its own, IEEE sqrt and division), then
 // compares every residual and out element bit for bit. The timed calls keep updating the residual in place. "rw GB/s" counts the bytes
 // one rank's HBM moves at one rank: x, residual and gamma read, residual and out written.
+// With --rms-norm-quantize WIRE:BLOCK it runs b200collAllReduceRmsNormQuantized: out holds the FP8 rows q and an arena buffer their
+// scales; -c 1 adds step 6 on the host (each row's out values, rounded to the dtype, quantised per BLOCK by quantise_block) and compares
+// every residual element, FP8 byte and scale bit for bit. "rw GB/s" then counts q and the scales written instead of out.
+static size_t rms_scale_bytes(const Opts& o) {
+  return o.rq_block ? o.max_bytes / b200collTypeSize(o.in_dt) / o.rq_block * 4 + 4096 : 0;
+}
 static float round_dt(float v, b200collDataType_t dt) {
   if (dt == b200collFloat32) return v;
   if (dt == b200collFloat16) return __half2float(__float2half_rn(v));
@@ -389,33 +397,49 @@ static int run_rms(const Opts& o, RankCtx& ctx, void* x, void* out, void* residu
   const size_t es = b200collTypeSize(dt), row = o.rms_row;
   const float eps = 1e-6f;
   const cudaStream_t st = ctx.st;
+  const int blk = o.rq_block;
   long total_errors = 0;
-  if (rank == 0) {
+  if (rank == 0 && blk) {
+    printf("# b200coll_perf op=all_reduce + rms-norm + quantize nranks=%d dtype=%s wire=%s block=%d row_len=%zu eps=%g: size = x bytes per rank; rw GB/s = "
+           "(x + residual + gamma read, residual + q + scales written) / time\n", n, dt_name(dt), dt_name(o.rq_wire), blk, row, eps);
+  } else if (rank == 0) {
     printf("# b200coll_perf op=all_reduce + rms-norm nranks=%d dtype=%s row_len=%zu eps=%g: size = x bytes per rank; rw GB/s = (x + residual + gamma read, "
            "residual + out written) / time\n", n, dt_name(dt), row, eps);
+  }
+  if (rank == 0) {
     printf("#%13s %10s %6s %8s | %10s %8s %8s %6s\n", "size(B)", "rows", "type", "algo", "us", "algbw", "rw_GB/s", "#wrong");
     fflush(stdout);
   }
   void* gamma = nullptr;
   RT(cudaMalloc(&gamma, row * es));
   fill(gamma, row, dt, 7, st);
+  float* scales = nullptr;                                         // --rms-norm-quantize: the scales of q, in the arena like q
+  if (blk) CC(b200collMemAlloc(ctx.comm, (void**)&scales, rms_scale_bytes(o)));
   for (size_t bytes = o.min_bytes; bytes <= o.max_bytes; bytes *= o.factor) {
     const size_t rows = bytes / es / row, elems = rows * row;
     if (rows == 0) continue;
     fill(x, elems, dt, rank, st);
     fill(residual, elems, dt, 99, st);
-    RT(cudaMemsetAsync(out, 0x5A, elems * es, st));
-    auto launch = [&](int) { CC(b200collAllReduceRmsNorm(x, residual, gamma, out, rows, row, eps, dt, ctx.comm, st)); };
+    const size_t nblk = blk ? elems / blk : 0, out_bytes = blk ? elems + nblk * 4 : elems * es;    // q and scales, or out
+    RT(cudaMemsetAsync(out, 0x5A, blk ? elems : elems * es, st));
+    if (blk) RT(cudaMemsetAsync(scales, 0x5A, nblk * 4, st));
+    auto launch = [&](int) {
+      if (blk) CC(b200collAllReduceRmsNormQuantized(x, residual, gamma, out, scales, rows, row, eps, dt, o.rq_wire, blk, ctx.comm, st));
+      else CC(b200collAllReduceRmsNorm(x, residual, gamma, out, rows, row, eps, dt, ctx.comm, st));
+    };
     long errs = 0;
     if (o.check) {
       check_launch(o, ctx, launch);
-      std::vector<char> gres(elems * es), gout(elems * es);
+      std::vector<char> gres(elems * es), gout(blk ? elems : elems * es);
+      std::vector<float> gsc(nblk);
       RT(cudaMemcpy(gres.data(), residual, gres.size(), cudaMemcpyDeviceToHost));
       RT(cudaMemcpy(gout.data(), out, gout.size(), cudaMemcpyDeviceToHost));
+      if (blk) RT(cudaMemcpy(gsc.data(), scales, nblk * 4, cudaMemcpyDeviceToHost));
       const size_t nch = row / 16;
       size_t P = 1;
       while (P < nch) P *= 2;
-      std::vector<float> h(row), p(P);
+      std::vector<float> h(row), p(P), y(row);
+      std::vector<__nv_fp8_storage_t> qw(row);
       for (size_t i = 0; i < rows; i++) {
         for (size_t e = 0; e < row; e++) {
           volatile float acc = 0.0f;
@@ -434,12 +458,23 @@ static int run_rms(const Opts& o, RankCtx& ctx, void* x, void* out, void* residu
         const float inv = 1.0f / den;
         for (size_t e = 0; e < row; e++) {
           volatile float hi = h[e] * inv;
-          volatile float y = hi * gen(7, e);
+          volatile float ye = hi * gen(7, e);
+          y[e] = blk ? round_dt(ye, dt) : ye;                            // step 6 quantises out as stored
+        }
+        for (size_t b = 0; blk && b < row / blk; b++) {
+          const float sw = quantise_block(y.data() + b * blk, blk, o.rq_wire, qw.data() + b * blk), sg = gsc[i * (row / blk) + b];
+          uint32_t want_s, got_s; memcpy(&want_s, &sw, 4); memcpy(&got_s, &sg, 4);
+          if (got_s != want_s) {
+            if (errs < 4) fprintf(stderr, "rank %d rms-norm size %zu row %zu block %zu: scale 0x%x want 0x%x\n", rank, bytes, i, b, got_s, want_s);
+            errs++;
+          }
+        }
+        for (size_t e = 0; e < row; e++) {
           const uint32_t want_h = out_bits(h[e], dt), got_h = got_bits(gres.data(), i * row + e, dt);
-          const uint32_t want_o = out_bits(y, dt), got_o = got_bits(gout.data(), i * row + e, dt);
+          const uint32_t want_o = blk ? qw[e] : out_bits(y[e], dt), got_o = blk ? (uint8_t)gout[i * row + e] : got_bits(gout.data(), i * row + e, dt);
           if (got_h != want_h || got_o != want_o) {
-            if (errs < 4) fprintf(stderr, "rank %d rms-norm size %zu row %zu elem %zu: residual 0x%x want 0x%x, out 0x%x want 0x%x\n", rank, bytes, i, e, got_h,
-                                  want_h, got_o, want_o);
+            if (errs < 4) fprintf(stderr, "rank %d rms-norm size %zu row %zu elem %zu: residual 0x%x want 0x%x, %s 0x%x want 0x%x\n", rank, bytes, i, e, got_h,
+                                  want_h, blk ? "q" : "out", got_o, want_o);
             errs++;
           }
         }
@@ -452,13 +487,14 @@ static int run_rms(const Opts& o, RankCtx& ctx, void* x, void* out, void* residu
     if (rank == 0) {
       const char* algo = "?";
       for (int a = 0; a < b200collNumAlgos; a++) if (s1.algo_calls[a] != s0.algo_calls[a]) algo = b200collAlgoName((b200collAlgo_t)a);
-      const size_t mat = elems * es, rw = 4 * mat + row * es;
+      const size_t mat = elems * es, rw = 3 * mat + row * es + out_bytes;
       printf("%14zu %10zu %6s %8s | %10.2f %8.2f %8.1f %6ld\n", mat, rows, dt_name(dt), algo, tm.ms * 1e3, mat / (tm.ms * 1e3) / 1e3, rw / (tm.ms * 1e3) / 1e3,
              tm.errors);
       fflush(stdout);
     }
   }
   RT(cudaFree(gamma));
+  if (scales) CC(b200collMemFree(ctx.comm, scales));
   return mode_result(ctx, total_errors);
 }
 
@@ -931,6 +967,10 @@ static bool flags_ok(const Opts& o) {
                     "or --route\n");
     return false;
   }
+  if (o.rq_block && (!o.rms_row || o.rms_row % o.rq_block != 0)) {
+    fprintf(stderr, "--rms-norm-quantize WIRE:BLOCK takes --rms-norm ROW_LEN, with ROW_LEN a multiple of BLOCK\n");
+    return false;
+  }
   if (o.cq_block && ((!o.combine_k && !o.route_e) || o.q_block || o.bs_rows || o.row_len % o.cq_block != 0)) {
     fprintf(stderr, "--combine-quantize WIRE:BLOCK takes --combine K or --route E:K, a --row-len that is a multiple of BLOCK, and no --quantize or\n"
                     "--block-scale\n");
@@ -976,7 +1016,7 @@ static size_t arena_bytes(const Opts& o) {
   const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt);
   return std::max(o.window, o.max_bytes) + std::max(o.window / is * os, o.max_bytes / is * os) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) +
          q_scratch_bytes(o) + (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o) +     // --route: recv holds K rows per token
-         (o.rms_row ? o.max_bytes + 4096 : 0);                                                                                  // --rms-norm: the residual
+         (o.rms_row ? o.max_bytes + 4096 : 0) + rms_scale_bytes(o);                                   // --rms-norm: the residual (and the scales of q)
 }
 
 int main(int argc, char** argv) {
@@ -1004,6 +1044,7 @@ int main(int argc, char** argv) {
     else if (a == "--row-len") o.row_len = (size_t)atoll(next());
     else if (a == "--quantize") parse_wire_block(a, next(), &o.q_wire, &o.q_block);
     else if (a == "--combine-quantize") parse_wire_block(a, next(), &o.cq_wire, &o.cq_block);
+    else if (a == "--rms-norm-quantize") parse_wire_block(a, next(), &o.rq_wire, &o.rq_block);
     else if (a == "--rms-norm") {
       const long long v = atoll(next());
       if (v < 16 || v > 16384 || v % 16) { fprintf(stderr, "--rms-norm ROW_LEN: a multiple of 16 in [16, 16384]\n"); return 1; }
@@ -1071,6 +1112,9 @@ int main(int argc, char** argv) {
            "  --algo auto|ll|ll2|oneshot|twoshot|nvls   --inplace 0|1|2   --max-ctas N   --sweep kind:ctas:threads,...   --json FILE   --window SIZE\n"
            "  --rms-norm ROW_LEN        --op all_reduce, -d bfloat16|half|float: the fused all-reduce, residual add and RMSNorm over rows of ROW_LEN\n"
            "                            elements (a multiple of 16 in [16, 16384]); -c 1 checks every residual and out element bit for bit\n"
+           "  --rms-norm-quantize WIRE:BLOCK   with --rms-norm ROW_LEN (a multiple of BLOCK): out quantised in the same kernel to WIRE (e4m3|e5m2)\n"
+           "                            rows with one fp32 scale per 1 x BLOCK (16..512) group; rw GB/s counts q and scales written instead of out;\n"
+           "                            -c 1 checks every residual element, FP8 byte and scale bit for bit against the host quantiser\n"
            "  --selfcheck               report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;
     }

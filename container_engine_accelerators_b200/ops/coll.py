@@ -148,6 +148,7 @@ def load() -> C.CDLL:
                                                     vp, vp]
     L.b200collExpertCombineQuantized.argtypes = [vp, vp, sz, sz, i32p, C.POINTER(C.c_float), sz, ci, ci, ci, C.POINTER(Epilogue), vp, vp]
     L.b200collAllReduceRmsNorm.argtypes = [vp, vp, vp, vp, sz, sz, C.c_float, ci, vp, vp]
+    L.b200collAllReduceRmsNormQuantized.argtypes = [vp, vp, vp, vp, C.POINTER(C.c_float), sz, sz, C.c_float, ci, ci, ci, vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -448,22 +449,19 @@ def _overlap(t, u) -> bool:
 RMS_NORM_MAX_ROW = 16384
 
 
-def check_all_reduce_rms_norm(x, residual, weight, out, eps: float = 1e-6) -> tuple[int, int]:
-    """The rules of Comm.all_reduce_rms_norm, checked on the tensors' metadata (no device, no communicator): raises ValueError, returns
-    (rows, row_len). x, residual and out are contiguous [..., row_len] tensors of one shape, weight a contiguous [row_len] tensor, all four of
-    one dtype (bfloat16, float16 or float32); row_len a multiple of 16 in [16, 16384]; eps finite and >= 0; fewer than 2^31 rows; every
-    pointer 16-byte aligned; out must not overlap x, residual or weight, residual must not overlap x or weight."""
+def _check_rms_norm(x, residual, weight, eps, out=None) -> tuple[int, int]:
+    """The rules both all-reduce + RMSNorm calls share, and out's when it is given (the wide call): returns (rows, row_len)."""
     import math
-    import torch
-    for name, t in (("x", x), ("residual", residual), ("weight", weight), ("out", out)):
+    wides = (("x", x), ("residual", residual), ("weight", weight)) + ((("out", out),) if out is not None else ())
+    for name, t in wides:
         _check_wide(name, t)
         if t.dtype != x.dtype:
             raise ValueError(f"{name} must have x's dtype {x.dtype}, got {t.dtype}")
     if x.dim() < 1:
         raise ValueError("x must have at least one dimension")
     shape = tuple(x.shape)
-    for name, t in (("residual", residual), ("out", out)):
-        if tuple(t.shape) != shape:
+    for name, t in wides[1:]:
+        if name != "weight" and tuple(t.shape) != shape:
             raise ValueError(f"{name} must have x's shape {list(shape)}, got {list(t.shape)}")
     row_len = shape[-1]
     if row_len < 16 or row_len > RMS_NORM_MAX_ROW or row_len % 16:
@@ -476,14 +474,51 @@ def check_all_reduce_rms_norm(x, residual, weight, out, eps: float = 1e-6) -> tu
     if rows > _I31:
         raise ValueError(f"at most 2^31 - 1 rows, got {rows}")
     if rows:
-        for name, t in (("x", x), ("residual", residual), ("weight", weight), ("out", out)):
+        for name, t in wides:
             if t.data_ptr() % 16:
                 raise ValueError(f"{name} must be 16-byte aligned")
-        if any(_overlap(out, t) for t in (x, residual, weight)):
+        if out is not None and any(_overlap(out, t) for t in (x, residual, weight)):
             raise ValueError("out must not overlap x, residual or weight")
         if _overlap(residual, x) or _overlap(residual, weight):
             raise ValueError("residual must not overlap x or weight")
     return rows, row_len
+
+
+def check_all_reduce_rms_norm(x, residual, weight, out, eps: float = 1e-6) -> tuple[int, int]:
+    """The rules of Comm.all_reduce_rms_norm, checked on the tensors' metadata (no device, no communicator): raises ValueError, returns
+    (rows, row_len). x, residual and out are contiguous [..., row_len] tensors of one shape, weight a contiguous [row_len] tensor, all four of
+    one dtype (bfloat16, float16 or float32); row_len a multiple of 16 in [16, 16384]; eps finite and >= 0; fewer than 2^31 rows; every
+    pointer 16-byte aligned; out must not overlap x, residual or weight, residual must not overlap x or weight."""
+    return _check_rms_norm(x, residual, weight, eps, out)
+
+
+def check_all_reduce_rms_norm_quantized(x, residual, weight, q, scales, block: int = 128, wire=None, eps: float = 1e-6) -> tuple[int, int, int]:
+    """The rules of Comm.all_reduce_rms_norm_quantized, checked on the tensors' metadata (no device, no communicator): raises ValueError,
+    returns (rows, row_len, the wire type's library code). x, residual and weight as in check_all_reduce_rms_norm; wire
+    torch.float8_e4m3fn (None, the default) or torch.float8_e5m2; block one of QUANT_BLOCKS and row_len a multiple of it; q a contiguous
+    tensor of x's shape and the wire dtype, 16-byte aligned; scales a contiguous float32 [..., row_len // block] tensor (x's leading
+    dimensions); x, residual, weight, q and scales must not overlap."""
+    import torch
+    rows, row_len = _check_rms_norm(x, residual, weight, eps)
+    wire = torch.float8_e4m3fn if wire is None else wire
+    if wire not in (torch.float8_e4m3fn, torch.float8_e5m2):
+        raise ValueError(f"wire must be torch.float8_e4m3fn or torch.float8_e5m2, not {wire}")
+    _check_block(block)
+    if row_len % block:
+        raise ValueError(f"row_len ({row_len}) must be a multiple of block ({block})")
+    if q.dtype != wire or tuple(q.shape) != tuple(x.shape) or not q.is_contiguous():
+        raise ValueError(f"q must be a contiguous {wire} tensor of x's shape {list(x.shape)}, got {q.dtype}{list(q.shape)}")
+    want = tuple(x.shape[:-1]) + (row_len // block,)
+    if scales.dtype != torch.float32 or tuple(scales.shape) != want or not scales.is_contiguous():
+        raise ValueError(f"scales must be a contiguous float32 tensor of shape {list(want)}, got {scales.dtype}{list(scales.shape)}")
+    if rows:
+        if q.data_ptr() % 16:
+            raise ValueError("q must be 16-byte aligned")
+        if any(_overlap(q, t) for t in (x, residual, weight, scales)):
+            raise ValueError("q must not overlap x, residual, weight or scales")
+        if any(_overlap(scales, t) for t in (x, residual, weight)):
+            raise ValueError("scales must not overlap x, residual or weight")
+    return rows, row_len, torch_dtype_code(wire)
 
 
 def _check_routed(nranks: int, x, topk_idx, num_experts: int, recv, expert_counts, route, dropped, fp8=None) -> None:
@@ -899,6 +934,27 @@ class Comm:
                                                C.c_void_p(out.data_ptr()), rows, row_len, float(eps), torch_dtype_code(x.dtype), self._h,
                                                self._stream(stream)), "AllReduceRmsNorm")
         return out
+
+    def all_reduce_rms_norm_quantized(self, x, residual, weight, q=None, scales=None, block: int = 128, wire=None, eps: float = 1e-6,
+                                      stream=None):
+        """all_reduce_rms_norm with its out quantised for an FP8 GEMM, in one kernel: residual += all_reduce(x) in place, then
+        o = rms_norm(residual, weight, eps) as all_reduce_rms_norm would store it, quantised per 1 x `block` group of each row to `wire`
+        (torch.float8_e4m3fn by default, or torch.float8_e5m2) with one fp32 scale per group, bit for bit as coll/include/b200coll.h's
+        b200collAllReduceRmsNormQuantized states. Returns (q, scales): q of x's shape and the wire dtype, scales float32
+        [..., row_len // block] (new tensors when None). With more than one rank x must be arena memory (`empty()`); two-shot also needs
+        residual, q and scales there, else the call runs one-shot."""
+        import torch
+        w = torch.float8_e4m3fn if wire is None else wire
+        q = x.new_empty(x.shape, dtype=w) if q is None else q
+        if scales is None:
+            _check_block(block)
+            scales = x.new_empty(tuple(x.shape[:-1]) + ((x.shape[-1] if x.dim() else 0) // block,), dtype=torch.float32)
+        rows, row_len, wc = check_all_reduce_rms_norm_quantized(x, residual, weight, q, scales, block, wire, eps)
+        _check(load().b200collAllReduceRmsNormQuantized(C.c_void_p(x.data_ptr()), C.c_void_p(residual.data_ptr()), C.c_void_p(weight.data_ptr()),
+                                                        C.c_void_p(q.data_ptr()), C.cast(C.c_void_p(scales.data_ptr()), C.POINTER(C.c_float)), rows,
+                                                        row_len, float(eps), torch_dtype_code(x.dtype), wc, block, self._h, self._stream(stream)),
+               "AllReduceRmsNormQuantized")
+        return q, scales
 
     def all_to_all(self, src, dst, scale: float = 1.0, stream=None):
         ep = self._ep(src, dst, scale)
