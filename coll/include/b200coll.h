@@ -522,6 +522,36 @@ b200collResult_t b200collAllReduceRmsNorm(const void* x, void* residual, const v
 b200collResult_t b200collAllReduceRmsNormQuantized(const void* x, void* residual, const void* gamma, void* q, float* scales, size_t rows,
                                                    size_t row_len, float eps, b200collDataType_t dtype, b200collDataType_t wire_dtype,
                                                    int block, b200collComm_t comm, b200collStream_t stream);
+/* Fused reduce-scatter, residual add and RMSNorm for sequence-parallel layers (Megatron-style sequence parallelism: the residual stream
+ * and the norms are sharded along the sequence), one kernel per call, with the all-gather for the next column-parallel GEMM fused in
+ * when `gather` is 1.
+ * Shapes: x is this rank's [rows, row_len] partial sums; rows % nranks == 0 and S = rows / nranks. residual is this rank's shard
+ * [S, row_len], rows [rank * S, (rank + 1) * S) of the residual stream, updated in place. gamma is [row_len]. All of `dtype`.
+ * Result: steps 1-5 are exactly b200collAllReduceRmsNorm's, applied to the rows of slice `rank` (6 for the quantised call, exactly
+ * b200collAllReduceRmsNormQuantized's). Equivalence, bit for bit: stack the N ranks' shards into a full residual R; then the new shards
+ * are b200collAllReduceRmsNorm(x, R, ...)'s new residual slice by slice, out (q, scales) is that call's output rows of slice `rank`, and
+ * with gather every rank's full out (q, scales) is that call's out.
+ * gather == 0: out [S, row_len] (q [S, row_len], scales [S, row_len / block]), any device buffer, written by the local rank only.
+ * gather == 1: out [rows, row_len] (q [rows, row_len], scales [rows, row_len / block]); rank r pushes slice r into every rank, so every
+ * rank ends with all rows. These must be arena memory at the same offsets on every rank, else InvalidUsage: there is no fallback, as no
+ * rank holds another rank's residual.
+ * Placement: with more than one rank, x in the arena at the same offset on every rank, else InvalidUsage. residual and gamma may be any
+ * device buffers; only the local rank reads or writes residual. gather must be the same on every rank. B200COLL_CHECK=1 cross-checks
+ * (rows, row_len, gather), the x offset, the out (q, scales) offsets when gathering, and (block, wire_dtype) on multi-process
+ * communicators.
+ * Algorithm: one with more than one rank (rank r pulls rows [r*S, (r+1)*S) of every rank's x, as two-shot does); the tuner and
+ * b200collCommSetAlgo do not apply, and forcing oneshot or ll changes nothing. One rank: S == rows, gather is irrelevant, and the call
+ * runs b200collAllReduceRmsNorm's (...Quantized's) local kernel. b200collStats count a reducescatter of S * row_len * sizeof(dtype) bytes
+ * under twoshot (copy with one rank), one kernel launch.
+ * Arguments (InvalidArgument, nothing launched): everything the all-reduce form refuses, with residual sized [S, row_len] and out (q,
+ * scales) sized by S or, gathering, by rows in the alignment and overlap checks; rows % nranks != 0; gather not 0 or 1. rows == 0 still
+ * launches on every rank and touches nothing. The kernel ends with a releasing barrier, so the caller may overwrite x right after the
+ * call. */
+b200collResult_t b200collReduceScatterRmsNorm(const void* x, void* residual, const void* gamma, void* out, size_t rows, size_t row_len,
+                                              float eps, int gather, b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
+b200collResult_t b200collReduceScatterRmsNormQuantized(const void* x, void* residual, const void* gamma, void* q, float* scales, size_t rows,
+                                                       size_t row_len, float eps, int gather, b200collDataType_t dtype,
+                                                       b200collDataType_t wire_dtype, int block, b200collComm_t comm, b200collStream_t stream);
 
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.

@@ -12,6 +12,13 @@
 //                        o = round_T((h * inv) * gamma) quantised per block of the row with quant.cuh's quant_vec: q and the block scales
 //                        stored locally, or (two-shot) pushed into every rank's q and scales
 //
+// and the reduce-scatter form for sequence parallelism (b200collReduceScatterRmsNorm, ...Quantized), where each rank holds only its
+// shard of the residual stream, rows [rows*r/N, rows*(r+1)/N) (one rank: the local kernels above):
+//
+//   k_rs_norm<T, GATHER>, k_rs_normq<T, WireT, GATHER>
+//                        two-shot's body: relaxed barrier, pull my row slice, read and write my residual shard locally at row - r0, store
+//                        out (q, scales) locally at row - r0, or (GATHER) push it into every rank's out at row, releasing barrier
+//
 // One CTA (kRmsThreads threads) owns one row at a time, walking rows b, b + gridDim.x, ... of its range. Thread t holds the 16-element
 // chunks t and t + kRmsThreads (row_len <= 16384 is at most 1024 chunks), so the new residual h of a whole row stays in registers
 // between the sum and the normalisation.
@@ -34,6 +41,10 @@
 // still read. The closing barrier releases the two-shot stores to every rank and tells each rank that nobody pulls its x any more, so the
 // caller may overwrite x right after the call. Both barriers pair CTA b with CTA b, and every rank launches full_grid's CTAs whatever its
 // row count.
+// The reduce-scatter kernels: rank r reads and writes only its own residual rows, so no other rank's store can meet them. With GATHER,
+// rank r stores rows of slice r into every rank's out, and rank p reaches the entry barrier only after everything earlier on its stream
+// (a GEMM reading out) is done: the same argument as two-shot's, so a peer's out rows are free. Without GATHER nothing is stored outside
+// the rank. The closing barrier both publishes the pushed out rows and tells each rank that nobody pulls its x any more.
 //
 // Step 6. A quantising block is 1 to 32 chunks (16 to 512 elements, a power of two) and row_len is a multiple of it, so the chunks of
 // one block are consecutive lanes of one warp (chunk t or t + 512 of thread t), starting on an aligned group of lanes: the contract of
@@ -93,10 +104,14 @@ struct RmsQuant {
 // One row: h = round((+0 + x_0 + .. + x_{N-1}) + residual), residual = h, out = round((h * inv) * gamma), inv = 1 / sqrt(fold / row_len + eps).
 // LOCAL: one rank, x is a.x_local; else rank r's x is at a.x_off of its arena. sbuf: this row's 512 floats of shared memory.
 // WireT void: out is stored (qa unused); else out is quantised to WireT per block into qa's q and scales.
-template <typename T, typename WireT, bool LOCAL, bool PUSH>
-__device__ __forceinline__ void rms_row(const CommDev& c, const RmsArgs& a, const RmsQuant& qa, size_t row, float* sbuf) {
+// x is read at row `row`. RES_PUSH: the residual is read locally and pushed into every rank at `row`; else read and written locally at
+// `lrow`. OUT_PUSH: out (q, scales) pushed into every rank at `row`; else stored locally at `lrow`. The all-reduce kernels pass
+// lrow == row; the reduce-scatter kernels pass the row's index in this rank's shard.
+template <typename T, typename WireT, bool LOCAL, bool RES_PUSH, bool OUT_PUSH>
+__device__ __forceinline__ void rms_row(const CommDev& c, const RmsArgs& a, const RmsQuant& qa, size_t row, size_t lrow, float* sbuf) {
   const int t = threadIdx.x, lane = t & 31;
   const size_t row_bytes = (size_t)a.row_len * sizeof(T);
+  const size_t res_row = RES_PUSH ? row : lrow, out_row = OUT_PUSH ? row : lrow;
   float h[2][16];
   float p[2];
 #pragma unroll
@@ -117,21 +132,22 @@ __device__ __forceinline__ void rms_row(const CommDev& c, const RmsArgs& a, cons
           for (int i = 0; i < 16; i++) acc[i] = __fadd_rn(acc[i], v[i]);
         }
       }
+      const size_t roff = res_row * row_bytes + (size_t)ch * 16 * sizeof(T);
       float res[16];
-      rms_load16<T>(a.res_in + off, res);
+      rms_load16<T>(a.res_in + roff, res);
 #pragma unroll
       for (int i = 0; i < 16; i++) {
         h[k][i] = round_to<T>(__fadd_rn(acc[i], res[i]));
         p[k] = __fadd_rn(p[k], __fmul_rn(h[k][i], h[k][i]));
       }
-      if (PUSH) {
+      if (RES_PUSH) {
 #pragma unroll
         for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
           int q = c.rank + j; if (q >= c.nranks) q -= c.nranks;
-          store16_scaled<T>(c.peer[q] + a.res_off + off, h[k], 1.0f);
+          store16_scaled<T>(c.peer[q] + a.res_off + roff, h[k], 1.0f);
         }
       } else {
-        store16_scaled<T>(a.res_out + off, h[k], 1.0f);
+        store16_scaled<T>(a.res_out + roff, h[k], 1.0f);
       }
     }
   }
@@ -155,12 +171,12 @@ __device__ __forceinline__ void rms_row(const CommDev& c, const RmsArgs& a, cons
     for (int k = 0; k < 2; k++) {
       const uint32_t ch = (uint32_t)t + (uint32_t)k * kRmsThreads;
       if (ch < a.nchunks) {
-        const size_t off = row * row_bytes + (size_t)ch * 16 * sizeof(T);
+        const size_t off = out_row * row_bytes + (size_t)ch * 16 * sizeof(T);
         float g[16], o[16];
         rms_load16<T>(a.gamma + (size_t)ch * 16 * sizeof(T), g);
 #pragma unroll
         for (int i = 0; i < 16; i++) o[i] = __fmul_rn(__fmul_rn(h[k][i], inv), g[i]);
-        if (PUSH) {
+        if (OUT_PUSH) {
 #pragma unroll
           for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
             int q = c.rank + j; if (q >= c.nranks) q -= c.nranks;
@@ -174,7 +190,7 @@ __device__ __forceinline__ void rms_row(const CommDev& c, const RmsArgs& a, cons
   } else {
     // step 6, one chunk at a time: o as the wide call would store it, widened back, then quantised with its block's amax
     const uint32_t gl = 1u << qa.lvpb;
-    const size_t q_row = row * a.row_len, s_row = row * (a.nchunks >> qa.lvpb);
+    const size_t q_row = out_row * a.row_len, s_row = out_row * (a.nchunks >> qa.lvpb);
 #pragma unroll
     for (int k = 0; k < 2; k++) {
       const uint32_t ch = (uint32_t)t + (uint32_t)k * kRmsThreads;
@@ -195,7 +211,7 @@ __device__ __forceinline__ void rms_row(const CommDev& c, const RmsArgs& a, cons
       if (act) {
         const size_t q_off = q_row + (size_t)ch * 16, s_off = (s_row + (ch >> qa.lvpb)) * 4;
         const bool lead = (lane & (gl - 1)) == 0;
-        if (PUSH) {
+        if (OUT_PUSH) {
 #pragma unroll
           for (int j = 0; j < kMaxRanks; j++) if (j < c.nranks) {
             int q = c.rank + j; if (q >= c.nranks) q -= c.nranks;
@@ -213,18 +229,20 @@ __device__ __forceinline__ void rms_row(const CommDev& c, const RmsArgs& a, cons
 
 // Rows [r0, r1), CTA b taking r0 + b, r0 + b + gridDim.x, ...; the shared buffer alternates by row so that one block barrier per row
 // suffices (a warp that writes row i + 2's buffer has passed row i + 1's barrier, which every warp reaches only after reading row i's).
-template <typename T, typename WireT, bool LOCAL, bool PUSH>
-__device__ __forceinline__ void rms_rows(const CommDev& c, const RmsArgs& a, const RmsQuant& qa, uint32_t r0, uint32_t r1) {
+// Local buffers are indexed from `base`: row - base is the row's index in them.
+template <typename T, typename WireT, bool LOCAL, bool RES_PUSH, bool OUT_PUSH>
+__device__ __forceinline__ void rms_rows(const CommDev& c, const RmsArgs& a, const RmsQuant& qa, uint32_t r0, uint32_t r1, uint32_t base) {
   __shared__ float sbuf[2][kRmsThreads];
   uint32_t i = 0;
-  for (uint32_t row = r0 + blockIdx.x; row < r1; row += gridDim.x, i ^= 1) rms_row<T, WireT, LOCAL, PUSH>(c, a, qa, row, sbuf[i]);
+  for (uint32_t row = r0 + blockIdx.x; row < r1; row += gridDim.x, i ^= 1)
+    rms_row<T, WireT, LOCAL, RES_PUSH, OUT_PUSH>(c, a, qa, row, row - base, sbuf[i]);
 }
 
 // The kernel bodies, shared by the wide kernels (WireT void) and the quantising ones.
 template <typename T, typename WireT>
 __device__ __forceinline__ void rms_local(const CommDev& c, const RmsArgs& a, const RmsQuant& qa, uint32_t rows) {
   pdl_prologue();
-  rms_rows<T, WireT, true, false>(c, a, qa, 0, rows);
+  rms_rows<T, WireT, true, false, false>(c, a, qa, 0, rows, 0);
 }
 
 template <typename T, typename WireT>
@@ -234,7 +252,7 @@ __device__ __forceinline__ void rms_oneshot(const CommDev& c, const RmsArgs& a, 
     const uint32_t s = load_seq(c, kSeqBarrier);
     if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every rank's x is written
   }
-  rms_rows<T, WireT, false, false>(c, a, qa, 0, rows);
+  rms_rows<T, WireT, false, false, false>(c, a, qa, 0, rows, 0);
   const uint32_t s = load_seq(c, kSeqBarrier);
   if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // nobody reads my x any more
   if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
@@ -248,9 +266,25 @@ __device__ __forceinline__ void rms_twoshot(const CommDev& c, const RmsArgs& a, 
     if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every rank's x is written, and its residual and out (q, scales) are free
   }
   const uint32_t r0 = (uint32_t)((unsigned long long)rows * c.rank / c.nranks), r1 = (uint32_t)((unsigned long long)rows * (c.rank + 1) / c.nranks);
-  rms_rows<T, WireT, false, true>(c, a, qa, r0, r1);
+  rms_rows<T, WireT, false, true, true>(c, a, qa, r0, r1, 0);
   const uint32_t s = load_seq(c, kSeqBarrier);
   if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // my rows are in every rank's residual and out; nobody reads my x
+  if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
+}
+
+// The reduce-scatter form: two-shot's slice, with my residual shard read and written locally at row - r0, and out (q, scales) stored
+// locally at row - r0 or (GATHER) pushed into every rank at row.
+template <typename T, typename WireT, bool GATHER>
+__device__ __forceinline__ void rs_norm(const CommDev& c, const RmsArgs& a, const RmsQuant& qa, uint32_t rows, uint32_t op) {
+  pdl_prologue();
+  {
+    const uint32_t s = load_seq(c, kSeqBarrier);
+    if (!barrier_blocks<false>(c, 2 * s + 1, op)) return;        // every rank's x is written, and (GATHER) its out (q, scales) is free
+  }
+  const uint32_t r0 = (uint32_t)((unsigned long long)rows * c.rank / c.nranks), r1 = (uint32_t)((unsigned long long)rows * (c.rank + 1) / c.nranks);
+  rms_rows<T, WireT, false, false, GATHER>(c, a, qa, r0, r1, r0);
+  const uint32_t s = load_seq(c, kSeqBarrier);
+  if (!barrier_blocks<true>(c, 2 * s + 2, op)) return;           // (GATHER) my rows are in every rank's out; nobody reads my x
   if (threadIdx.x == 0 && last_block_ticket(c)) c.state[kSeqBarrier] = s + 1;
 }
 
@@ -288,10 +322,21 @@ __global__ void __launch_bounds__(kRmsThreads, 1) k_rmsq_twoshot(COMM_PARAM, con
   rms_twoshot<T, WireT>(c, a, qa, rows, op);
 }
 
-// Once per device, before the first kernel of this family launches: load all 27 kernels, wide and quantising. With lazy module loading a
-// kernel's first launch loads it, and the load waits for kernels already running; a rank whose first launch of one of these kernels came
-// behind its own barrier kernel, which waits for another rank's launch on the same thread, would never get there. One thread loads at a
-// time.
+template <typename T, bool GATHER>
+__global__ void __launch_bounds__(kRmsThreads, 1) k_rs_norm(COMM_PARAM, const __grid_constant__ RmsArgs a, uint32_t rows, uint32_t op) {
+  rs_norm<T, void, GATHER>(c, a, RmsQuant{}, rows, op);
+}
+
+template <typename T, typename WireT, bool GATHER>
+__global__ void __launch_bounds__(kRmsThreads, 1) k_rs_normq(COMM_PARAM, const __grid_constant__ RmsArgs a, const __grid_constant__ RmsQuant qa,
+                                                              uint32_t rows, uint32_t op) {
+  rs_norm<T, WireT, GATHER>(c, a, qa, rows, op);
+}
+
+// Once per device, before the first kernel of this family launches: load all 45 kernels, all-reduce and reduce-scatter, wide and
+// quantising. With lazy module loading a kernel's first launch loads it, and the load waits for kernels already running; a rank whose
+// first launch of one of these kernels came behind its own barrier kernel, which waits for another rank's launch on the same thread,
+// would never get there. One thread loads at a time.
 static void rmsnorm_preload(const b200collComm* c) {
   static std::atomic<unsigned long long> done{0};
   static std::mutex mu;
@@ -306,12 +351,16 @@ static void rmsnorm_preload(const b200collComm* c) {
       cudaFuncGetAttributes(&fa, k_rms_local<T>);
       cudaFuncGetAttributes(&fa, k_rms_oneshot<T>);
       cudaFuncGetAttributes(&fa, k_rms_twoshot<T>);
+      cudaFuncGetAttributes(&fa, k_rs_norm<T, false>);
+      cudaFuncGetAttributes(&fa, k_rs_norm<T, true>);
       for (b200collDataType_t w : {b200collFloat8e4m3, b200collFloat8e5m2})
         with_fp8(w, [&](auto tw) {
           using WireT = typename decltype(tw)::type;
           cudaFuncGetAttributes(&fa, k_rmsq_local<T, WireT>);
           cudaFuncGetAttributes(&fa, k_rmsq_oneshot<T, WireT>);
           cudaFuncGetAttributes(&fa, k_rmsq_twoshot<T, WireT>);
+          cudaFuncGetAttributes(&fa, k_rs_normq<T, WireT, false>);
+          cudaFuncGetAttributes(&fa, k_rs_normq<T, WireT, true>);
         });
     });
   done.fetch_or(bit, std::memory_order_acq_rel);
@@ -325,11 +374,22 @@ struct RmsQuantCall {
   int block;
 };
 
-// The argument rules of both calls (qz == nullptr: b200collAllReduceRmsNorm, whose messages these are), all before the
-// poisoned-communicator check; nothing is launched on a refusal.
+// The reduce-scatter form's extra argument (nullptr: the all-reduce form).
+struct RsCall {
+  int gather;
+};
+
+static const char* rms_who(const RmsQuantCall* qz, const RsCall* rs) {
+  if (rs) return qz ? "quantised reduce-scatter rms-norm: " : "reduce-scatter rms-norm: ";
+  return qz ? "quantised all-reduce rms-norm: " : "all-reduce rms-norm: ";
+}
+
+// The argument rules of all four calls (qz == nullptr: the wide call; rs == nullptr: the all-reduce form, whose messages these are), all
+// before the poisoned-communicator check; nothing is launched on a refusal. The reduce-scatter form's residual is [rows / nranks, row_len],
+// and its out (q, scales) has rows / nranks rows, or rows when gathering.
 static b200collResult_t rms_prepare(b200collComm* c, const void* x, const void* residual, const void* gamma, const void* out, size_t rows, size_t row_len,
-                                    float eps, b200collDataType_t dtype, const RmsQuantCall* qz) {
-  const std::string who = qz ? "quantised all-reduce rms-norm: " : "all-reduce rms-norm: ";
+                                    float eps, b200collDataType_t dtype, const RmsQuantCall* qz, const RsCall* rs = nullptr) {
+  const std::string who = rms_who(qz, rs);
   auto refuse = [&](const std::string& msg) { set_last_error(who + msg); return b200collInvalidArgument; };
   if (!c) return refuse("null communicator");
   if (!wide_type(dtype)) return refuse("dtype must be bf16, fp16 or fp32");
@@ -339,31 +399,36 @@ static b200collResult_t rms_prepare(b200collComm* c, const void* x, const void* 
   if (qz && row_len % (size_t)qz->block != 0) return refuse("row_len must be a multiple of block");
   if (!(eps >= 0.0f) || !isfinite(eps)) return refuse("eps must be finite and non-negative");
   if (rows >= ((size_t)1 << 31)) return refuse("rows must be below 2^31");
-  const size_t es = b200collTypeSize(dtype), mat = rows * row_len * es, g = row_len * es;
+  if (rs && rs->gather != 0 && rs->gather != 1) return refuse("gather must be 0 or 1");
+  if (rs && rows % (size_t)c->nranks != 0) return refuse("rows must be a multiple of nranks");
+  const size_t shard = rs ? rows / (size_t)c->nranks : rows, out_rows = rs && !rs->gather ? shard : rows;
+  const size_t es = b200collTypeSize(dtype), mat = rows * row_len * es, g = row_len * es, res = shard * row_len * es, om = out_rows * row_len * es;
   if (!qz) {
     if (rows > 0 && (!x || !residual || !gamma || !out)) return refuse("null argument");
     if (!aligned(x, 16) || !aligned(residual, 16) || !aligned(gamma, 16) || !aligned(out, 16)) return refuse("x, residual, gamma and out must be 16-byte aligned");
-    if (rows > 0 && (overlaps(out, mat, x, mat) || overlaps(out, mat, residual, mat) || overlaps(out, mat, gamma, g)))
+    if (rows > 0 && (overlaps(out, om, x, mat) || overlaps(out, om, residual, res) || overlaps(out, om, gamma, g)))
       return refuse("out must not overlap x, residual or gamma");
   } else {
     if (rows > 0 && (!x || !residual || !gamma || !qz->q || !qz->scales)) return refuse("null argument");
     if (!aligned(x, 16) || !aligned(residual, 16) || !aligned(gamma, 16) || !aligned(qz->q, 16)) return refuse("x, residual, gamma and q must be 16-byte aligned");
     if (!aligned(qz->scales, 4)) return refuse("scales must be 4-byte aligned");
-    const size_t qb = rows * row_len, sb = rows * (row_len / (size_t)qz->block) * 4;
-    if (rows > 0 && (overlaps(qz->q, qb, x, mat) || overlaps(qz->q, qb, residual, mat) || overlaps(qz->q, qb, gamma, g) || overlaps(qz->q, qb, qz->scales, sb)))
+    const size_t qb = out_rows * row_len, sb = out_rows * (row_len / (size_t)qz->block) * 4;
+    if (rows > 0 && (overlaps(qz->q, qb, x, mat) || overlaps(qz->q, qb, residual, res) || overlaps(qz->q, qb, gamma, g) || overlaps(qz->q, qb, qz->scales, sb)))
       return refuse("q must not overlap x, residual, gamma or scales");
-    if (rows > 0 && (overlaps(qz->scales, sb, x, mat) || overlaps(qz->scales, sb, residual, mat) || overlaps(qz->scales, sb, gamma, g)))
+    if (rows > 0 && (overlaps(qz->scales, sb, x, mat) || overlaps(qz->scales, sb, residual, res) || overlaps(qz->scales, sb, gamma, g)))
       return refuse("scales must not overlap x, residual or gamma");
   }
-  if (rows > 0 && (overlaps(residual, mat, x, mat) || overlaps(residual, mat, gamma, g))) return refuse("residual must not overlap x or gamma");
+  if (rows > 0 && (overlaps(residual, res, x, mat) || overlaps(residual, res, gamma, g))) return refuse("residual must not overlap x or gamma");
   if (comm_poisoned(c)) return b200collRemoteError;
   return b200collSuccess;
 }
 
-// Both calls after their arguments passed: the algorithm, the B200COLL_CHECK=1 cross-check, one launch. qz == nullptr: the wide call.
+// Both all-reduce calls after their arguments passed: the algorithm, the B200COLL_CHECK=1 cross-check, one launch. qz == nullptr: the
+// wide call. The reduce-scatter form with one rank is this call's local kernel, counted under `stats_op`.
 static b200collResult_t rms_run(b200collComm* c, const void* x, void* residual, const void* gamma, void* out, size_t rows, size_t row_len, float eps,
-                                b200collDataType_t dtype, const RmsQuantCall* qz, b200collStream_t stream) {
-  const char* who = qz ? "quantised all-reduce rms-norm: " : "all-reduce rms-norm: ";
+                                b200collDataType_t dtype, const RmsQuantCall* qz, b200collStream_t stream,
+                                b200collOp_t stats_op = b200collOpAllReduce) {
+  const char* who = rms_who(qz, nullptr);
   b200collResult_t rc = b200collSuccess;
   const size_t mat = rows * row_len * b200collTypeSize(dtype);
   const size_t qb = qz ? rows * row_len : 0, sb = qz ? rows * (row_len / (size_t)qz->block) * 4 : 0;
@@ -386,7 +451,7 @@ static b200collResult_t rms_run(b200collComm* c, const void* x, void* residual, 
   }
   const DeviceScope on_device(c->device);
   rmsnorm_preload(c);
-  account(c, b200collOpAllReduce, mat, algo);
+  account(c, stats_op, mat, algo);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   RmsArgs a = {};
   a.x_local = static_cast<const char*>(x);
@@ -434,6 +499,71 @@ static b200collResult_t rms_run(b200collComm* c, const void* x, void* residual, 
   });
 }
 
+// Both reduce-scatter calls after their arguments passed. One rank: the all-reduce form's local kernel (the shard is every row). More:
+// one algorithm, k_rs_norm / k_rs_normq, whatever the tuner or b200collCommSetAlgo says.
+static b200collResult_t rs_run(b200collComm* c, const void* x, void* residual, const void* gamma, void* out, size_t rows, size_t row_len, float eps,
+                               b200collDataType_t dtype, const RmsQuantCall* qz, const RsCall& rs, b200collStream_t stream) {
+  if (c->nranks == 1) return rms_run(c, x, residual, gamma, out, rows, row_len, eps, dtype, qz, stream, b200collOpReduceScatter);
+  const char* who = rms_who(qz, &rs);
+  b200collResult_t rc = b200collSuccess;
+  const size_t es = b200collTypeSize(dtype), mat = rows * row_len * es, shard = rows / (size_t)c->nranks;
+  const size_t qb = rows * row_len, sb = qz ? rows * (row_len / (size_t)qz->block) * 4 : 0;
+  // peers pull my x at my arena offset, and with gather push their rows into my out (q, scales) at my offsets. rows == 0 touches
+  // nothing, so any pointer will do.
+  if (rows > 0 && (rc = in_arena(c, who, "x", {{x, mat}})) != b200collSuccess) return rc;
+  if (rows > 0 && rs.gather) {
+    if (qz) rc = in_arena(c, who, "q and scales (gather)", {{qz->q, qb}, {qz->scales, sb}});
+    else rc = in_arena(c, who, "out (gather)", {{out, mat}});
+    if (rc != b200collSuccess) return rc;
+  }
+  // (rows, row_len, gather) travel as one number (row_len < 2^15), with the x offset and, quantising, (block, wire); gathering adds a
+  // second exchange for the out (q) and scales offsets
+  const size_t shape = (rows << 16) | (row_len << 1) | (size_t)rs.gather, fmt = qz ? (size_t)qz->block * 2 + (qz->wire == b200collFloat8e5m2) : 0;
+  const b200collAlgo_t algo = b200collAlgoTwoShot;
+  if ((rc = cross_check(c, b200collOpReduceScatter, algo, shape, rows > 0 ? arena_off(c, x) : 0, fmt)) != b200collSuccess) return rc;
+  if (rs.gather && (rc = cross_check(c, b200collOpReduceScatter, algo, shape, rows > 0 ? arena_off(c, qz ? qz->q : out) : 0,
+                                     rows > 0 && qz ? arena_off(c, qz->scales) : 0)) != b200collSuccess)
+    return rc;
+  const DeviceScope on_device(c->device);
+  rmsnorm_preload(c);
+  account(c, b200collOpReduceScatter, shard * row_len * es, algo);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RmsArgs a = {};
+  a.res_in = static_cast<const char*>(residual);
+  a.res_out = static_cast<char*>(residual);
+  a.gamma = static_cast<const char*>(gamma);
+  a.row_len = (uint32_t)row_len;
+  a.nchunks = (uint32_t)(row_len / 16);
+  a.eps = eps;
+  if (rows > 0) a.x_off = arena_off(c, x);
+  RmsQuant qa = {};
+  if (qz) qa.lvpb = (uint32_t)quant_lvpb(qz->block);
+  if (rs.gather && rows > 0) {
+    if (qz) { qa.q_off = arena_off(c, qz->q); qa.s_off = arena_off(c, qz->scales); }
+    else a.out_off = arena_off(c, out);
+  } else {
+    a.out = static_cast<char*>(out);
+    if (qz) { qa.q = static_cast<char*>(qz->q); qa.scales = reinterpret_cast<char*>(qz->scales); }
+  }
+  const Grid gr = full_grid(c, 1);
+  const uint32_t op = (uint32_t)b200collOpReduceScatter;
+  auto launch = [&](auto tt, auto tw, auto tg) -> b200collResult_t {
+    using T = typename decltype(tt)::type; using WireT = typename decltype(tw)::type;
+    constexpr bool kGather = decltype(tg)::value;
+    if constexpr (std::is_void<WireT>::value) launch_k(k_rs_norm<T, kGather>, gr.blocks, kRmsThreads, st, c->dev, a, (uint32_t)rows, op);
+    else launch_k(k_rs_normq<T, WireT, kGather>, gr.blocks, kRmsThreads, st, c->dev, a, qa, (uint32_t)rows, op);
+    LAUNCH_CHECK(c);
+    return b200collSuccess;
+  };
+  return with_wide(dtype, [&](auto tt) -> b200collResult_t {
+    auto with_gather = [&](auto tw) {
+      return rs.gather ? launch(tt, tw, std::true_type{}) : launch(tt, tw, std::false_type{});
+    };
+    if (!qz) return with_gather(Tag<void>{});
+    return with_fp8(qz->wire, [&](auto tw) { return with_gather(tw); });
+  });
+}
+
 }  // namespace b200coll
 
 using namespace b200coll;
@@ -454,6 +584,24 @@ b200collResult_t b200collAllReduceRmsNormQuantized(const void* x, void* residual
   const b200collResult_t rc = rms_prepare(c, x, residual, gamma, nullptr, rows, row_len, eps, dtype, &qz);
   if (rc != b200collSuccess) return rc;
   return rms_run(c, x, residual, gamma, nullptr, rows, row_len, eps, dtype, &qz, stream);
+}
+
+b200collResult_t b200collReduceScatterRmsNorm(const void* x, void* residual, const void* gamma, void* out, size_t rows, size_t row_len, float eps,
+                                              int gather, b200collDataType_t dtype, b200collComm_t c, b200collStream_t stream) {
+  const RsCall rs = {gather};
+  const b200collResult_t rc = rms_prepare(c, x, residual, gamma, out, rows, row_len, eps, dtype, nullptr, &rs);
+  if (rc != b200collSuccess) return rc;
+  return rs_run(c, x, residual, gamma, out, rows, row_len, eps, dtype, nullptr, rs, stream);
+}
+
+b200collResult_t b200collReduceScatterRmsNormQuantized(const void* x, void* residual, const void* gamma, void* q, float* scales, size_t rows,
+                                                       size_t row_len, float eps, int gather, b200collDataType_t dtype, b200collDataType_t wire_dtype,
+                                                       int block, b200collComm_t c, b200collStream_t stream) {
+  const RmsQuantCall qz = {q, scales, wire_dtype, block};
+  const RsCall rs = {gather};
+  const b200collResult_t rc = rms_prepare(c, x, residual, gamma, nullptr, rows, row_len, eps, dtype, &qz, &rs);
+  if (rc != b200collSuccess) return rc;
+  return rs_run(c, x, residual, gamma, nullptr, rows, row_len, eps, dtype, &qz, rs, stream);
 }
 
 }  // extern "C"

@@ -63,6 +63,7 @@ struct Opts {
   b200collDataType_t cq_wire = b200collFloat8e4m3;
   size_t rms_row = 0;             // --rms-norm ROW_LEN: the fused all-reduce, residual add and RMSNorm (0 = off)
   int rq_block = 0;               // --rms-norm-quantize WIRE:BLOCK: its FP8 out, one fp32 scale per 1 x BLOCK (0 = off)
+  bool rms_gather = false;        // --rms-norm-gather: with --op reduce_scatter, the normed rows all-gathered in the same kernel
   b200collDataType_t rq_wire = b200collFloat8e4m3;
 };
 
@@ -383,6 +384,10 @@ static int run_combine(const Opts& o, RankCtx& ctx, void* expert_out, void* out)
 // With --rms-norm-quantize WIRE:BLOCK it runs b200collAllReduceRmsNormQuantized: out holds the FP8 rows q and an arena buffer their
 // scales; -c 1 adds step 6 on the host (each row's out values, rounded to the dtype, quantised per BLOCK by quantise_block) and compares
 // every residual element, FP8 byte and scale bit for bit. "rw GB/s" then counts q and the scales written instead of out.
+// With --op reduce_scatter it runs b200collReduceScatterRmsNorm (...Quantized): rows are rounded down to a multiple of nranks, and rank r
+// passes rows [r*S, (r+1)*S) of the residual buffer as its shard. -c 1 checks the shard's rows and that no other residual row changed,
+// and out (q, scales) for the slice, stored from row 0, or with --rms-norm-gather for every row. "rw GB/s" counts x, the shard read and
+// written, gamma, and the out rows this rank stores.
 static size_t rms_scale_bytes(const Opts& o) {
   return o.rq_block ? o.max_bytes / b200collTypeSize(o.in_dt) / o.rq_block * 4 + 4096 : 0;
 }
@@ -398,8 +403,13 @@ static int run_rms(const Opts& o, RankCtx& ctx, void* x, void* out, void* residu
   const float eps = 1e-6f;
   const cudaStream_t st = ctx.st;
   const int blk = o.rq_block;
+  const bool sp = o.op == "reduce_scatter", gather = sp && o.rms_gather;
   long total_errors = 0;
-  if (rank == 0 && blk) {
+  if (rank == 0 && sp) {
+    printf("# b200coll_perf op=reduce_scatter + rms-norm%s%s nranks=%d dtype=%s wire=%s block=%d row_len=%zu eps=%g: size = x bytes per rank; rw GB/s = "
+           "(x + residual shard + gamma read, residual shard + %s written) / time\n", gather ? " + gather" : "", blk ? " + quantize" : "", n, dt_name(dt),
+           blk ? dt_name(o.rq_wire) : "-", blk, row, eps, blk ? "q + scales" : "out");
+  } else if (rank == 0 && blk) {
     printf("# b200coll_perf op=all_reduce + rms-norm + quantize nranks=%d dtype=%s wire=%s block=%d row_len=%zu eps=%g: size = x bytes per rank; rw GB/s = "
            "(x + residual + gamma read, residual + q + scales written) / time\n", n, dt_name(dt), dt_name(o.rq_wire), blk, row, eps);
   } else if (rank == 0) {
@@ -416,15 +426,20 @@ static int run_rms(const Opts& o, RankCtx& ctx, void* x, void* out, void* residu
   float* scales = nullptr;                                         // --rms-norm-quantize: the scales of q, in the arena like q
   if (blk) CC(b200collMemAlloc(ctx.comm, (void**)&scales, rms_scale_bytes(o)));
   for (size_t bytes = o.min_bytes; bytes <= o.max_bytes; bytes *= o.factor) {
-    const size_t rows = bytes / es / row, elems = rows * row;
+    const size_t rows = sp ? bytes / es / row / n * n : bytes / es / row, elems = rows * row;
     if (rows == 0) continue;
+    // the reduce-scatter form: my shard of the residual, and the rows of out (q, scales) I store, from row o_row0 of mine
+    const size_t shard = sp ? rows / n : rows, r0 = sp ? shard * rank : 0, o_rows = sp && !gather ? shard : rows, o_row0 = gather || !sp ? 0 : r0;
+    char* res = static_cast<char*>(residual) + r0 * row * es;
     fill(x, elems, dt, rank, st);
     fill(residual, elems, dt, 99, st);
-    const size_t nblk = blk ? elems / blk : 0, out_bytes = blk ? elems + nblk * 4 : elems * es;    // q and scales, or out
+    const size_t nblk = blk ? elems / blk : 0, out_bytes = (blk ? elems + nblk * 4 : elems * es) / rows * o_rows;    // q and scales, or out
     RT(cudaMemsetAsync(out, 0x5A, blk ? elems : elems * es, st));
     if (blk) RT(cudaMemsetAsync(scales, 0x5A, nblk * 4, st));
     auto launch = [&](int) {
-      if (blk) CC(b200collAllReduceRmsNormQuantized(x, residual, gamma, out, scales, rows, row, eps, dt, o.rq_wire, blk, ctx.comm, st));
+      if (sp && blk) CC(b200collReduceScatterRmsNormQuantized(x, res, gamma, out, scales, rows, row, eps, gather, dt, o.rq_wire, blk, ctx.comm, st));
+      else if (sp) CC(b200collReduceScatterRmsNorm(x, res, gamma, out, rows, row, eps, gather, dt, ctx.comm, st));
+      else if (blk) CC(b200collAllReduceRmsNormQuantized(x, residual, gamma, out, scales, rows, row, eps, dt, o.rq_wire, blk, ctx.comm, st));
       else CC(b200collAllReduceRmsNorm(x, residual, gamma, out, rows, row, eps, dt, ctx.comm, st));
     };
     long errs = 0;
@@ -461,8 +476,10 @@ static int run_rms(const Opts& o, RankCtx& ctx, void* x, void* out, void* residu
           volatile float ye = hi * gen(7, e);
           y[e] = blk ? round_dt(ye, dt) : ye;                            // step 6 quantises out as stored
         }
-        for (size_t b = 0; blk && b < row / blk; b++) {
-          const float sw = quantise_block(y.data() + b * blk, blk, o.rq_wire, qw.data() + b * blk), sg = gsc[i * (row / blk) + b];
+        const bool mine = i >= r0 && i < r0 + shard, stored = mine || gather;    // residual row i changes, out row i is stored here
+        const size_t oi = i - o_row0;                                    // (stored) out row i's index in out
+        for (size_t b = 0; blk && stored && b < row / blk; b++) {
+          const float sw = quantise_block(y.data() + b * blk, blk, o.rq_wire, qw.data() + b * blk), sg = gsc[oi * (row / blk) + b];
           uint32_t want_s, got_s; memcpy(&want_s, &sw, 4); memcpy(&got_s, &sg, 4);
           if (got_s != want_s) {
             if (errs < 4) fprintf(stderr, "rank %d rms-norm size %zu row %zu block %zu: scale 0x%x want 0x%x\n", rank, bytes, i, b, got_s, want_s);
@@ -470,8 +487,12 @@ static int run_rms(const Opts& o, RankCtx& ctx, void* x, void* out, void* residu
           }
         }
         for (size_t e = 0; e < row; e++) {
-          const uint32_t want_h = out_bits(h[e], dt), got_h = got_bits(gres.data(), i * row + e, dt);
-          const uint32_t want_o = blk ? qw[e] : out_bits(y[e], dt), got_o = blk ? (uint8_t)gout[i * row + e] : got_bits(gout.data(), i * row + e, dt);
+          const uint32_t want_h = out_bits(mine ? h[e] : gen(99, i * row + e), dt), got_h = got_bits(gres.data(), i * row + e, dt);
+          uint32_t want_o = 0, got_o = 0;
+          if (stored) {
+            want_o = blk ? qw[e] : out_bits(y[e], dt);
+            got_o = blk ? (uint8_t)gout[oi * row + e] : got_bits(gout.data(), oi * row + e, dt);
+          }
           if (got_h != want_h || got_o != want_o) {
             if (errs < 4) fprintf(stderr, "rank %d rms-norm size %zu row %zu elem %zu: residual 0x%x want 0x%x, %s 0x%x want 0x%x\n", rank, bytes, i, e, got_h,
                                   want_h, blk ? "q" : "out", got_o, want_o);
@@ -487,7 +508,7 @@ static int run_rms(const Opts& o, RankCtx& ctx, void* x, void* out, void* residu
     if (rank == 0) {
       const char* algo = "?";
       for (int a = 0; a < b200collNumAlgos; a++) if (s1.algo_calls[a] != s0.algo_calls[a]) algo = b200collAlgoName((b200collAlgo_t)a);
-      const size_t mat = elems * es, rw = 3 * mat + row * es + out_bytes;
+      const size_t mat = elems * es, rw = mat + 2 * shard * row * es + row * es + out_bytes;
       printf("%14zu %10zu %6s %8s | %10.2f %8.2f %8.1f %6ld\n", mat, rows, dt_name(dt), algo, tm.ms * 1e3, mat / (tm.ms * 1e3) / 1e3, rw / (tm.ms * 1e3) / 1e3,
              tm.errors);
       fflush(stdout);
@@ -961,10 +982,14 @@ static LauncherRank launcher_rank() {
 // Every conflict between flags and with the number of ranks (o.nranks), refused before any communicator or buffer exists.
 static bool flags_ok(const Opts& o) {
   const int n = o.nranks;
-  if (o.rms_row && (o.op != "all_reduce" || o.out_dt != o.in_dt || o.scale != 1.0f || o.q_block || o.bs_rows || o.combine_k || o.route_e || o.cq_block ||
+  if (o.rms_row && ((o.op != "all_reduce" && o.op != "reduce_scatter") || o.out_dt != o.in_dt || o.scale != 1.0f || o.q_block || o.bs_rows || o.combine_k || o.route_e || o.cq_block ||
                     !wide(o.in_dt))) {
-    fprintf(stderr, "--rms-norm ROW_LEN takes --op all_reduce and -d bfloat16|half|float, and no --out-dtype, --scale, --quantize, --block-scale, --combine\n"
-                    "or --route\n");
+    fprintf(stderr, "--rms-norm ROW_LEN takes --op all_reduce or reduce_scatter and -d bfloat16|half|float, and no --out-dtype, --scale, --quantize,\n"
+                    "--block-scale, --combine or --route\n");
+    return false;
+  }
+  if (o.rms_gather && (!o.rms_row || o.op != "reduce_scatter")) {
+    fprintf(stderr, "--rms-norm-gather takes --rms-norm ROW_LEN and --op reduce_scatter\n");
     return false;
   }
   if (o.rq_block && (!o.rms_row || o.rms_row % o.rq_block != 0)) {
@@ -1045,6 +1070,7 @@ int main(int argc, char** argv) {
     else if (a == "--quantize") parse_wire_block(a, next(), &o.q_wire, &o.q_block);
     else if (a == "--combine-quantize") parse_wire_block(a, next(), &o.cq_wire, &o.cq_block);
     else if (a == "--rms-norm-quantize") parse_wire_block(a, next(), &o.rq_wire, &o.rq_block);
+    else if (a == "--rms-norm-gather") o.rms_gather = true;
     else if (a == "--rms-norm") {
       const long long v = atoll(next());
       if (v < 16 || v > 16384 || v % 16) { fprintf(stderr, "--rms-norm ROW_LEN: a multiple of 16 in [16, 16384]\n"); return 1; }
@@ -1115,7 +1141,11 @@ int main(int argc, char** argv) {
            "  --rms-norm-quantize WIRE:BLOCK   with --rms-norm ROW_LEN (a multiple of BLOCK): out quantised in the same kernel to WIRE (e4m3|e5m2)\n"
            "                            rows with one fp32 scale per 1 x BLOCK (16..512) group; rw GB/s counts q and scales written instead of out;\n"
            "                            -c 1 checks every residual element, FP8 byte and scale bit for bit against the host quantiser\n"
-           "  --selfcheck               report whether this node can run the NVLink fast paths (exit 1 if not)");
+           "  --op reduce_scatter --rms-norm ROW_LEN   the sequence-parallel form: the fused reduce-scatter, residual add and RMSNorm; rows\n"
+           "                            are rounded down to a multiple of the ranks, each rank keeps a residual shard of rows / nranks rows and\n"
+           "                            stores the out rows of its slice; -c 1 checks the shard, every other residual row unchanged, and out\n"
+           "  --rms-norm-gather         with --op reduce_scatter --rms-norm ROW_LEN: the normed rows all-gathered in the same kernel\n"
+           "  --selfcheck              report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;
     }
     else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 1; }

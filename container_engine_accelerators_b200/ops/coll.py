@@ -149,6 +149,8 @@ def load() -> C.CDLL:
     L.b200collExpertCombineQuantized.argtypes = [vp, vp, sz, sz, i32p, C.POINTER(C.c_float), sz, ci, ci, ci, C.POINTER(Epilogue), vp, vp]
     L.b200collAllReduceRmsNorm.argtypes = [vp, vp, vp, vp, sz, sz, C.c_float, ci, vp, vp]
     L.b200collAllReduceRmsNormQuantized.argtypes = [vp, vp, vp, vp, C.POINTER(C.c_float), sz, sz, C.c_float, ci, ci, ci, vp, vp]
+    L.b200collReduceScatterRmsNorm.argtypes = [vp, vp, vp, vp, sz, sz, C.c_float, ci, ci, vp, vp]
+    L.b200collReduceScatterRmsNormQuantized.argtypes = [vp, vp, vp, vp, C.POINTER(C.c_float), sz, sz, C.c_float, ci, ci, ci, ci, vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -449,8 +451,21 @@ def _overlap(t, u) -> bool:
 RMS_NORM_MAX_ROW = 16384
 
 
-def _check_rms_norm(x, residual, weight, eps, out=None) -> tuple[int, int]:
-    """The rules both all-reduce + RMSNorm calls share, and out's when it is given (the wide call): returns (rows, row_len)."""
+def _rs_shapes(x, nranks: int, gather: bool) -> tuple[tuple, tuple]:
+    """The reduce-scatter form's (residual shape, out shape): x's shape with dim 0 divided by nranks, and x's own when gathering."""
+    if x.dim() < 2:
+        raise ValueError("x must have at least two dimensions (the sequence, sharded along dim 0, then the rows' elements)")
+    shape = tuple(x.shape)
+    if shape[0] % nranks:
+        raise ValueError(f"x.shape[0] ({shape[0]}) must be a multiple of nranks ({nranks})")
+    shard = (shape[0] // nranks,) + shape[1:]
+    return shard, (shape if gather else shard)
+
+
+def _check_rms_norm(x, residual, weight, eps, out=None, sp=None) -> tuple[int, int]:
+    """The rules the all-reduce and reduce-scatter + RMSNorm calls share, and out's when it is given (the wide calls): returns (rows,
+    row_len), rows counting every row of x. sp: None (the all-reduce form: residual and out of x's shape) or (nranks, gather), the
+    reduce-scatter form's shapes."""
     import math
     wides = (("x", x), ("residual", residual), ("weight", weight)) + ((("out", out),) if out is not None else ())
     for name, t in wides:
@@ -460,9 +475,13 @@ def _check_rms_norm(x, residual, weight, eps, out=None) -> tuple[int, int]:
     if x.dim() < 1:
         raise ValueError("x must have at least one dimension")
     shape = tuple(x.shape)
+    want = {"residual": shape, "out": shape}
+    if sp is not None:
+        want["residual"], want["out"] = _rs_shapes(x, *sp)
     for name, t in wides[1:]:
-        if name != "weight" and tuple(t.shape) != shape:
-            raise ValueError(f"{name} must have x's shape {list(shape)}, got {list(t.shape)}")
+        if name != "weight" and tuple(t.shape) != want[name]:
+            whose = "x's shape" if want[name] == shape else "the shard's shape"
+            raise ValueError(f"{name} must have {whose} {list(want[name])}, got {list(t.shape)}")
     row_len = shape[-1]
     if row_len < 16 or row_len > RMS_NORM_MAX_ROW or row_len % 16:
         raise ValueError(f"row_len (the last dimension) must be a multiple of 16 in [16, {RMS_NORM_MAX_ROW}], got {row_len}")
@@ -498,17 +517,24 @@ def check_all_reduce_rms_norm_quantized(x, residual, weight, q, scales, block: i
     torch.float8_e4m3fn (None, the default) or torch.float8_e5m2; block one of QUANT_BLOCKS and row_len a multiple of it; q a contiguous
     tensor of x's shape and the wire dtype, 16-byte aligned; scales a contiguous float32 [..., row_len // block] tensor (x's leading
     dimensions); x, residual, weight, q and scales must not overlap."""
+    return _check_rms_norm_quantized(x, residual, weight, q, scales, block, wire, eps)
+
+
+def _check_rms_norm_quantized(x, residual, weight, q, scales, block, wire, eps, sp=None) -> tuple[int, int, int]:
+    """The rules of both quantising + RMSNorm calls; sp as in _check_rms_norm (q and scales take out's rows)."""
     import torch
-    rows, row_len = _check_rms_norm(x, residual, weight, eps)
+    rows, row_len = _check_rms_norm(x, residual, weight, eps, sp=sp)
+    oshape = tuple(x.shape) if sp is None else _rs_shapes(x, *sp)[1]
     wire = torch.float8_e4m3fn if wire is None else wire
     if wire not in (torch.float8_e4m3fn, torch.float8_e5m2):
         raise ValueError(f"wire must be torch.float8_e4m3fn or torch.float8_e5m2, not {wire}")
     _check_block(block)
     if row_len % block:
         raise ValueError(f"row_len ({row_len}) must be a multiple of block ({block})")
-    if q.dtype != wire or tuple(q.shape) != tuple(x.shape) or not q.is_contiguous():
-        raise ValueError(f"q must be a contiguous {wire} tensor of x's shape {list(x.shape)}, got {q.dtype}{list(q.shape)}")
-    want = tuple(x.shape[:-1]) + (row_len // block,)
+    if q.dtype != wire or tuple(q.shape) != oshape or not q.is_contiguous():
+        whose = "x's shape" if oshape == tuple(x.shape) else "the shard's shape"
+        raise ValueError(f"q must be a contiguous {wire} tensor of {whose} {list(oshape)}, got {q.dtype}{list(q.shape)}")
+    want = oshape[:-1] + (row_len // block,)
     if scales.dtype != torch.float32 or tuple(scales.shape) != want or not scales.is_contiguous():
         raise ValueError(f"scales must be a contiguous float32 tensor of shape {list(want)}, got {scales.dtype}{list(scales.shape)}")
     if rows:
@@ -519,6 +545,22 @@ def check_all_reduce_rms_norm_quantized(x, residual, weight, q, scales, block: i
         if any(_overlap(scales, t) for t in (x, residual, weight)):
             raise ValueError("scales must not overlap x, residual or weight")
     return rows, row_len, torch_dtype_code(wire)
+
+
+def check_reduce_scatter_rms_norm(nranks: int, x, residual, weight, out, eps: float = 1e-6, gather: bool = False) -> tuple[int, int]:
+    """The rules of Comm.reduce_scatter_rms_norm, checked on the tensors' metadata (no device, no communicator): raises ValueError, returns
+    (rows, row_len), rows counting every row of x. As check_all_reduce_rms_norm, except for the shapes: x has at least two dimensions
+    and x.shape[0] is a multiple of nranks (the sequence is sharded along dim 0); residual has x's shape with dim 0 divided by nranks;
+    out has residual's shape, or x's when gathering."""
+    return _check_rms_norm(x, residual, weight, eps, out, sp=(nranks, bool(gather)))
+
+
+def check_reduce_scatter_rms_norm_quantized(nranks: int, x, residual, weight, q, scales, block: int = 128, wire=None, eps: float = 1e-6,
+                                            gather: bool = False) -> tuple[int, int, int]:
+    """The rules of Comm.reduce_scatter_rms_norm_quantized, checked on the tensors' metadata: raises ValueError, returns (rows, row_len,
+    the wire type's library code). Shapes as in check_reduce_scatter_rms_norm, with q of out's shape and scales [..., row_len // block]
+    of out's leading dimensions; everything else as in check_all_reduce_rms_norm_quantized."""
+    return _check_rms_norm_quantized(x, residual, weight, q, scales, block, wire, eps, sp=(nranks, bool(gather)))
 
 
 def _check_routed(nranks: int, x, topk_idx, num_experts: int, recv, expert_counts, route, dropped, fp8=None) -> None:
@@ -954,6 +996,48 @@ class Comm:
                                                         C.c_void_p(q.data_ptr()), C.cast(C.c_void_p(scales.data_ptr()), C.POINTER(C.c_float)), rows,
                                                         row_len, float(eps), torch_dtype_code(x.dtype), wc, block, self._h, self._stream(stream)),
                "AllReduceRmsNormQuantized")
+        return q, scales
+
+    def reduce_scatter_rms_norm(self, x, residual, weight, out=None, eps: float = 1e-6, gather: bool = False, stream=None):
+        """The sequence-parallel pre-norm step in one kernel: x's rows are summed over the ranks, and this rank keeps its slice of dim 0
+        (rows [rank * S, (rank + 1) * S), S = x.shape[0] // nranks). residual, this rank's [S, ...] shard of the residual stream, gets
+        that slice added in place, then out = rms_norm(residual, weight, eps), bit for bit as coll/include/b200coll.h's
+        b200collReduceScatterRmsNorm states. gather=True also all-gathers out: every rank receives every slice, out of x's shape.
+        Returns out (a new tensor when None and not gathering). With more than one rank x must be arena memory (`empty()`), and when
+        gathering so must out: it has to be passed then."""
+        sp = _rs_shapes(x, self.nranks, bool(gather))
+        if out is None:
+            if gather and self.nranks > 1:
+                raise ValueError("gather=True needs out: an arena tensor (Comm.empty) of x's shape, the same on every rank")
+            out = x.new_empty(sp[1])
+        rows, row_len = check_reduce_scatter_rms_norm(self.nranks, x, residual, weight, out, eps, gather)
+        _check(load().b200collReduceScatterRmsNorm(C.c_void_p(x.data_ptr()), C.c_void_p(residual.data_ptr()), C.c_void_p(weight.data_ptr()),
+                                                   C.c_void_p(out.data_ptr()), rows, row_len, float(eps), int(bool(gather)),
+                                                   torch_dtype_code(x.dtype), self._h, self._stream(stream)), "ReduceScatterRmsNorm")
+        return out
+
+    def reduce_scatter_rms_norm_quantized(self, x, residual, weight, q=None, scales=None, block: int = 128, wire=None, eps: float = 1e-6,
+                                          gather: bool = False, stream=None):
+        """reduce_scatter_rms_norm with its out quantised for an FP8 GEMM, in one kernel, as all_reduce_rms_norm_quantized quantises:
+        `wire` torch.float8_e4m3fn (the default) or torch.float8_e5m2, one fp32 scale per 1 x `block` group, bit for bit as
+        b200collReduceScatterRmsNormQuantized states. Returns (q, scales): q of residual's shape (x's when gathering) and the wire dtype,
+        scales float32 [..., row_len // block] (new tensors when None and not gathering). gather=True with more than one rank needs q
+        and scales passed, as arena tensors."""
+        import torch
+        sp = _rs_shapes(x, self.nranks, bool(gather))
+        if (q is None or scales is None) and gather and self.nranks > 1:
+            raise ValueError("gather=True needs q and scales: arena tensors (Comm.empty) of the gathered shapes, the same on every rank")
+        w = torch.float8_e4m3fn if wire is None else wire
+        q = x.new_empty(sp[1], dtype=w) if q is None else q
+        if scales is None:
+            _check_block(block)
+            scales = x.new_empty(sp[1][:-1] + (sp[1][-1] // block,), dtype=torch.float32)
+        rows, row_len, wc = check_reduce_scatter_rms_norm_quantized(self.nranks, x, residual, weight, q, scales, block, wire, eps, gather)
+        _check(load().b200collReduceScatterRmsNormQuantized(C.c_void_p(x.data_ptr()), C.c_void_p(residual.data_ptr()),
+                                                            C.c_void_p(weight.data_ptr()), C.c_void_p(q.data_ptr()),
+                                                            C.cast(C.c_void_p(scales.data_ptr()), C.POINTER(C.c_float)), rows, row_len, float(eps),
+                                                            int(bool(gather)), torch_dtype_code(x.dtype), wc, block, self._h, self._stream(stream)),
+               "ReduceScatterRmsNormQuantized")
         return q, scales
 
     def all_to_all(self, src, dst, scale: float = 1.0, stream=None):
