@@ -6,14 +6,15 @@ import numpy as np
 INT32_MIN, INT32_MAX = -2 ** 31, 2 ** 31 - 1
 
 
-def routing(kind, n, E, k, seed, tokens=None):
-    """One [tokens, top_k] int32 array per rank. uniform; zipf (expert_dispatch_plan's skewed draw); one (every slot to one expert);
-    mixed: uniform with every kind of invalid id, a token naming one expert twice, and (n > 1) a last rank with no tokens."""
+def routing(kind, n, E, k, seed, tokens=None, skew=1.2):
+    """One [tokens, top_k] int32 array per rank. uniform; zipf (expert_dispatch_plan's skewed draw, popularity 1 / rank^skew); one
+    (every slot to one expert); mixed: uniform with every kind of invalid id, a token naming one expert twice, and (n > 1) a last rank
+    with no tokens."""
     rng = np.random.default_rng(seed)
     tokens = tokens or [17 + 5 * s for s in range(n)]
     if kind == "zipf":
         from container_engine_accelerators_b200.models.workloads import expert_dispatch_plan
-        p = expert_dispatch_plan(n, max(tokens), 16, experts_per_rank=E // n, top_k=k, skew=1.2, seed=seed)
+        p = expert_dispatch_plan(n, max(tokens), 16, experts_per_rank=E // n, top_k=k, skew=skew, seed=seed)
         return [p.experts[s][:tokens[s]] for s in range(n)]
     if kind == "one":
         return [np.full((tokens[s], k), (seed * 7) % E, dtype=np.int32) for s in range(n)]
@@ -25,7 +26,7 @@ def routing(kind, n, E, k, seed, tokens=None):
             pos = rng.choice(ids.size, size=min(ids.size, len(bad)), replace=False)
             for i, p in enumerate(pos):
                 ids.flat[p] = bad[i]
-            if k >= 2:
+            if k >= 2 and ids.shape[0] >= 2:
                 ids[1, 0] = ids[1, 1] = s % E                           # the same expert twice
         if n > 1:
             out[-1] = np.zeros((0, k), dtype=np.int64)
@@ -71,9 +72,11 @@ def layout(topk, num_experts, recv_rows):
         keep = row < recv_rows
         route[slots[keep]] = owner[e[keep]] * recv_rows + row[keep]
         routes.append(route.reshape(np.shape(topk[s])).astype(np.int32))
-        tok = slots[keep] // np.shape(topk[s])[1]
-        for d, r, t in zip(owner[e[keep]], row[keep], tok):
-            source[d][r] = (s, t)
+        tok, dest, rows = slots[keep] // np.shape(topk[s])[1], owner[e[keep]], row[keep]
+        for d in range(n):
+            at = dest == d
+            source[d][rows[at], 0] = s
+            source[d][rows[at], 1] = tok[at]
     counts, dropped = [], []
     for d in range(n):
         mine = slice(d * epr, (d + 1) * epr)
@@ -117,9 +120,10 @@ def recv_rows_of(lay, xs, d, poison):
     """Rank d's expected recv as bytes: row r holds x[s][t] for source[d][r] = (s, t), the poison row elsewhere. xs: one [tokens, row_bytes]
     uint8 array per rank; poison: [recv_rows, row_bytes] uint8."""
     want = poison.copy()
-    for r, (s, t) in enumerate(lay.source[d]):
-        if s >= 0:
-            want[r] = xs[s][t]
+    src = lay.source[d]
+    for s in range(len(xs)):
+        at = src[:, 0] == s
+        want[at] = xs[s][src[at, 1]]
     return want
 
 
@@ -132,7 +136,9 @@ def route_lookup(eo, recv_rows):
         col = np.asarray(col, dtype=np.int64)
         valid = (col >= 0) & (col < n * recv_rows)
         y = np.zeros((col.size, eo[0].shape[1]), dtype=np.float32)
-        for i in np.nonzero(valid)[0]:
-            y[i] = eo[col[i] // recv_rows][col[i] % recv_rows]
+        i = np.nonzero(valid)[0]
+        for p in range(n):
+            at = i[col[i] // recv_rows == p]
+            y[at] = eo[p][col[at] % recv_rows]
         return valid, y
     return f

@@ -187,6 +187,84 @@ def test_layout_reference_matches_slot_by_slot_placement(seed):
         assert sum(a.dropped) + sum(int(c.sum()) for c in a.counts) == valid
 
 
+@pytest.mark.parametrize("n, E", [(1, 1024), (2, 1024), (3, 1023), (8, 1024)])
+def test_layout_reference_matches_slot_by_slot_placement_at_1024_experts_top_10(n, E):
+    """The most experts the dispatch takes and a top_k past the combine's slot batch, at small token counts: a hot expert, the last
+    expert, invalid ids, and capacities from nothing to everything."""
+    rng = np.random.default_rng(n)
+    k = 10
+    topk = [rng.integers(-2, E + 2, size=(int(rng.integers(0, 6)), k)) for _ in range(n)]
+    topk[0] = np.vstack([topk[0], np.full((2, k), E - 1), rng.integers(0, 3, size=(2, k))])
+    valid = sum(int(((t >= 0) & (t < E)).sum()) for t in topk)
+    for recv_rows in (0, 1, valid // 2, valid - 1, valid, valid + 3):
+        a, b = rr.layout(topk, E, recv_rows), rr.brute_force(topk, E, recv_rows)
+        for s in range(n):
+            assert (a.route[s] == b.route[s]).all() and (a.counts[s] == b.counts[s]).all() and a.dropped[s] == b.dropped[s]
+            assert (a.source[s] == b.source[s]).all()
+        assert sum(a.dropped) + sum(int(c.sum()) for c in a.counts) == valid
+
+
+def _recv_rows_by_row(lay, xs, d, poison):
+    want = poison.copy()
+    for r, (s, t) in enumerate(lay.source[d]):
+        if s >= 0:
+            want[r] = xs[s][t]
+    return want
+
+
+def _route_lookup_by_slot(eo, recv_rows):
+    n = len(eo)
+
+    def f(col):
+        col = np.asarray(col, dtype=np.int64)
+        valid = (col >= 0) & (col < n * recv_rows)
+        y = np.zeros((col.size, eo[0].shape[1]), dtype=np.float32)
+        for i in np.nonzero(valid)[0]:
+            y[i] = eo[col[i] // recv_rows][col[i] % recv_rows]
+        return valid, y
+    return f
+
+
+@pytest.mark.parametrize("seed", range(6))
+def test_recv_rows_and_route_lookup_match_row_by_row(seed):
+    """recv_rows_of and route_lookup (numpy fancy indexing) against a row-by-row and a slot-by-slot rendering, on brute-force layouts;
+    the lookup also sees every kind of value outside the routes."""
+    rng = np.random.default_rng(50 + seed)
+    for _ in range(10):
+        n = int(rng.choice([1, 2, 3, 4, 8]))
+        E, k = n * int(rng.integers(1, 6)), int(rng.integers(1, 11))
+        topk = [rng.integers(-2, E + 2, size=(int(rng.integers(0, 12)), k)) for _ in range(n)]
+        valid = sum(int(((t >= 0) & (t < E)).sum()) for t in topk)
+        recv_rows = int(rng.integers(0, valid + 3))
+        lay = rr.brute_force(topk, E, recv_rows)
+        xs = [rng.integers(0, 256, size=(t.shape[0], 32), dtype=np.uint8) for t in topk]
+        poison = np.full((recv_rows, 32), 0x5A, dtype=np.uint8)
+        for d in range(n):
+            assert (rr.recv_rows_of(lay, xs, d, poison) == _recv_rows_by_row(lay, xs, d, poison)).all()
+        eo = [rng.standard_normal((recv_rows, 16)).astype(np.float32) for _ in range(n)]
+        for s in range(n):
+            cols = np.concatenate([lay.route[s].reshape(-1), [-1, rr.INT32_MIN, rr.INT32_MAX, n * recv_rows, n * recv_rows - 1, 0]])
+            (va, ya), (vb, yb) = rr.route_lookup(eo, recv_rows)(cols), _route_lookup_by_slot(eo, recv_rows)(cols)
+            assert (va == vb).all() and (ya.view(np.int32) == yb.view(np.int32)).all()
+
+
+def test_reference_keeps_up_with_model_shapes():
+    """8 ranks x 4096 tokens x top-8 (262,144 slots): the layout, one rank's expected recv and one slot column's lookup each take well
+    under a second, so the GPU tests at model shapes spend their time on the GPU."""
+    import time
+    n, E, k, T = 8, 256, 8, 4096
+    topk = rr.routing("zipf", n, E, k, seed=1, tokens=[T] * n, skew=2.0)
+    t0 = time.perf_counter()
+    lay = rr.layout(topk, E, 40000)
+    assert time.perf_counter() - t0 < 1.0
+    xs = [np.zeros((T, 64), dtype=np.uint8) for _ in range(n)]
+    eo = [np.zeros((40000, 32), dtype=np.float32) for _ in range(n)]
+    t0 = time.perf_counter()
+    rr.recv_rows_of(lay, xs, 0, np.zeros((40000, 64), dtype=np.uint8))
+    rr.route_lookup(eo, 40000)(lay.route[0][:, 0])
+    assert time.perf_counter() - t0 < 1.0
+
+
 def test_layout_reference_by_hand():
     """2 ranks, 4 experts (rank 0 owns 0 and 1): rank 1's rows for expert 1 follow rank 0's; expert 0's rows come first."""
     topk = [np.array([[1, 0], [1, 9]]), np.array([[1, 1], [-1, 2]])]
