@@ -206,7 +206,7 @@ def self_check() -> tuple[bool, str]:
 def torch_dtype_code(dtype) -> int:
     import torch
     return {torch.float32: F32, torch.float16: F16, torch.bfloat16: BF16, torch.float8_e4m3fn: FP8_E4M3, torch.float8_e5m2: FP8_E5M2, torch.int8: I8, torch.uint8: U8, torch.int32: I32,
-            torch.int64: I64, torch.float64: F64, torch.bool: U8}[dtype]
+            torch.uint32: U32, torch.int64: I64, torch.uint64: U64, torch.float64: F64, torch.bool: U8}[dtype]
 
 
 def check_block_scaled(op: str, nranks: int, q, scales, out, block=(1, 128)) -> tuple[int, int]:

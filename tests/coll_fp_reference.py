@@ -16,12 +16,16 @@ order model is always [0, 1, ..., N-1].
 
 Not collected by pytest (no test_ prefix); imported by the test_coll_fp_numerics_* and test_coll_fp8_numerics_* files and the other
 GPU tests."""
+import numpy as np
 import torch
+
+from container_engine_accelerators_b200.ops.coll import MAX, MIN, PROD, SUM
 
 STAGE_HALF_BYTES = 32 << 20          # coll/src/layout.h kStageHalfBytes
 LL_ONESHOT_MAX_BYTES = 512 << 10     # kLLOneShotMaxBytes: per source
 HOST_ZEROCOPY_BYTES = 4096 << 10     # hostpath.cu defaults: B200COLL_HOST_ZEROCOPY_KB
 HOST_PIPELINE_BYTES = 8192 << 10     # B200COLL_HOST_PIPELINE_KB
+BULK_MIN_BYTES = 1 << 20             # collectives.cu bulk_min_bytes default (B200COLL_BULK_MIN_KB): identity moves from here on the copy engine
 LL_SENTINEL, LL_SANITIZED = 0xFFFFFFFF, 0x7FFF7FFF    # layout.h kLLSentinel / kLLSanitized
 
 FP8_MAX = {torch.float8_e4m3fn: 448.0, torch.float8_e5m2: 57344.0}
@@ -131,6 +135,18 @@ def rotation(r, n):
     return [(r + j) % n for j in range(n)]
 
 
+RANK_ORDER_ALGOS = ("ll", "ll2", "oneshot")
+
+
+def order_for(algo, n, in_dt, count):
+    """The order model of an all-reduce that recorded `algo`: FP8 inputs are summed in rank order on every kernel; 16- and 32-bit inputs
+    in rank order except on two-shot (slice owner first)."""
+    if in_dt in FP8_MAX or algo in RANK_ORDER_ALGOS:
+        return list(range(n))
+    assert algo == "twoshot", f"no bit-exact order model for {algo}"
+    return ("owner", n, vec_elems(in_dt), count)
+
+
 # ------------------------------------------------------------------------------------------------- reference ops
 def _sum(xs, order):
     acc = torch.zeros(xs[0].numel(), dtype=torch.float32, device=xs[0].device)
@@ -177,6 +193,72 @@ def ll_move(x):
     w = u[:u.numel() // 4 * 4].view(torch.int32)                              # a partial last word is padded with zeros: never the sentinel
     w[w == -1] = LL_SANITIZED
     return u.view(x.dtype)
+
+
+# the generic kernel (coll/src/generic.cu): every type, sum / prod / min / max
+NP_INT = {torch.int8: np.int8, torch.uint8: np.uint8, torch.int32: np.int32, torch.uint32: np.uint32, torch.int64: np.int64,
+          torch.uint64: np.uint64}
+
+
+def int_numpy(t):
+    """An integer tensor's values as a numpy array of its own type (through its bytes: torch has few kernels for uint32 / uint64)."""
+    return t.contiguous().view(torch.uint8).cpu().numpy().view(NP_INT[t.dtype])
+
+
+def int_tensor(a, dtype, device="cuda"):
+    """A numpy integer array as a tensor of dtype (same width) on `device`, bit for bit."""
+    return torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).copy()).to(device).view(dtype)
+
+
+def generic_ref(xs, op):
+    """The generic kernel's result: rank 0's value, then ranks 1 .. N-1 in order. Integers wrap (numpy arithmetic in the type's own
+    width; min and max compare as the type is signed or not). Floating point accumulates in fp32 for fp16, bf16 and FP8 and in its own
+    type otherwise, and is rounded once at the end (FP8 saturates); min / max propagate a NaN from any rank and keep the lower rank's
+    value on a tie."""
+    dt = xs[0].dtype
+    if dt in NP_INT:
+        a = [int_numpy(x) for x in xs]
+        acc = a[0].copy()
+        with np.errstate(over="ignore"):
+            for b in a[1:]:
+                acc = {SUM: np.add, PROD: np.multiply, MIN: np.minimum, MAX: np.maximum}[op](acc, b).astype(a[0].dtype)
+        return int_tensor(acc, dt, xs[0].device)
+    wide = dt in (torch.float16, torch.bfloat16) or dt in FP8_MAX
+    acc = xs[0].float() if wide else xs[0].clone()
+    for x in xs[1:]:
+        b = x.float() if wide else x
+        if op == SUM:
+            acc = acc + b
+        elif op == PROD:
+            acc = acc * b
+        elif op == MIN:
+            acc = torch.where((b < acc) | (b != b), b, acc)
+        else:
+            assert op == MAX, op
+            acc = torch.where((b > acc) | (b != b), b, acc)
+    return cast(acc, dt)
+
+
+def int_inputs(n, count, dtype, seed):
+    """Seeded per-rank integers over the type's whole range (so half are >= 2^31 or 2^63 as unsigned, negative as signed, and sums and
+    products wrap), with the type's extremes at fixed positions: at element 5 + k, rank k % N holds the k-th of min, max, 0, all ones,
+    the top bit alone and the top bit's complement, and element 17 holds max on rank 0 and min on the other ranks (13: the reverse)."""
+    nt = NP_INT[dtype]
+    info = np.iinfo(nt)
+    rng = np.random.default_rng(seed)
+    bits = 8 * np.dtype(nt).itemsize
+    u = np.dtype(f"u{bits // 8}")
+    xs = [rng.integers(0, 1 << bits, size=count, dtype=np.uint64).astype(u).view(nt) for _ in range(n)]
+    as_t = lambda v: np.array([v], dtype=u).view(nt)[0]
+    extremes = [info.min, info.max, 0, as_t((1 << bits) - 1), as_t(1 << (bits - 1)), as_t((1 << (bits - 1)) - 1)]
+    for k, v in enumerate(extremes):
+        if 5 + k < count:
+            xs[k % n][5 + k] = v
+    for pos, first, rest in ((17, info.max, info.min), (13, info.min, info.max)):
+        if pos < count:
+            for r in range(n):
+                xs[r][pos] = first if r == 0 else rest
+    return xs
 
 
 # ------------------------------------------------------------------------------------------------- data

@@ -17,7 +17,7 @@ PERF = os.path.join(ROOT, "build", "b200coll_perf")
 
 DTYPES = {"bf16": torch.bfloat16, "f16": torch.float16, "f32": torch.float32, "e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2,
           **{name: getattr(torch, name) for name in ("bfloat16", "float16", "float32", "float64", "float8_e4m3fn", "float8_e5m2", "int8",
-                                                      "uint8", "int32")}}
+                                                      "uint8", "int32", "uint32", "int64", "uint64")}}
 
 
 @pytest.fixture(scope="module")

@@ -19,7 +19,6 @@ E4, E5 = "float8_e4m3fn", "float8_e5m2"
 PAIRS = [(E4, E4), (E4, E5), (E4, "bfloat16"), (E4, "float16"), (E5, E5), (E5, E4), (E5, "bfloat16"), (E5, "float16")]
 SUBSET = [(E5, "bfloat16"), (E5, E5), (E4, E5), (E5, E4)]
 E = 16                                                          # FP8 elements per 16-byte vector
-RANK_ORDER_ALGOS = ("ll", "ll2", "oneshot")
 
 group = group_fixture(3, arena_mb=160, timeout_ms=60000)
 
@@ -38,14 +37,6 @@ def ar_pick(coll, n, nvls, algo, nbytes, is_, os_, fp8_in, sym=True, inplace=Fal
     if feasible(algo):
         return algo
     return next((a for a in ("nvls", "twoshot", "oneshot", "ll", "ll2") if feasible(a) and not (a == "nvls" and n == 2)), None)
-
-
-def order_for(algo, n, in_dt, count):
-    """FP8 inputs: rank order on every kernel; 16- and 32-bit inputs: rank order except on two-shot (slice owner first)."""
-    if in_dt in R.FP8_MAX or algo in RANK_ORDER_ALGOS:
-        return list(range(n))
-    assert algo == "twoshot", f"no bit-exact order model for {algo}"
-    return ("owner", n, R.vec_elems(in_dt), count)
 
 
 def check_ar(torch, coll, g, ins, count, in_name, out_name, algo, op, scale, what, outs=None, xs=None):
@@ -332,21 +323,6 @@ def test_lamport_identity_movement(torch_cuda, coll_mod, group):
 
 
 # ------------------------------------------------------------------------------------------------- generic kernel
-def _generic_ref(torch, coll, xs, op):
-    """Rank order from rank 0's value in fp32 (exact for FP8 products of up to 5 ranks); min / max propagate a NaN from any rank and
-    keep the lower rank's value on a tie; the result is rounded once with saturation (R.cast, not .to)."""
-    acc = xs[0].float()
-    for x in xs[1:]:
-        b = x.float()
-        if op == coll.PROD:
-            acc = acc * b
-        elif op == coll.MIN:
-            acc = torch.where((b < acc) | (b != b), b, acc)
-        else:
-            acc = torch.where((b > acc) | (b != b), b, acc)
-    return R.cast(acc, xs[0].dtype)
-
-
 @pytest.mark.parametrize("group", [3, 5], indirect=True)
 def test_generic_kernel(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
@@ -363,7 +339,7 @@ def test_generic_kernel(torch_cuda, coll_mod, group):
                 ins = [c.empty(count, t) for c in comms]
                 for b, x in zip(ins, xs):
                     b.copy_(x)
-                want = _generic_ref(torch, coll, xs, op)
+                want = R.generic_ref(xs, op)
                 if op != coll.PROD:
                     assert int(want.view(torch.uint8)[60]) == 0x00 and int(want.view(torch.uint8)[62]) == 0x80
                 what = f"generic n={n} {name} op={op} count={count}"
@@ -385,7 +361,7 @@ def test_generic_kernel(torch_cuda, coll_mod, group):
                 rs = [c.empty(rc, t) for c in comms]
                 group.run(lambda r, c, st: c.reduce_scatter(ins[r][:rc * n], rs[r], op=op, stream=st))
                 for r in range(n):
-                    R.assert_same(rs[r], _generic_ref(torch, coll, [x[r * rc:(r + 1) * rc] for x in xs], op), f"{what} reduce_scatter rank {r}")
+                    R.assert_same(rs[r], R.generic_ref([x[r * rc:(r + 1) * rc] for x in xs], op), f"{what} reduce_scatter rank {r}")
                 release(comms, rs, ins)
             if n == 3:                                                       # staged: buffers outside the arena
                 count = 4099
@@ -396,7 +372,7 @@ def test_generic_kernel(torch_cuda, coll_mod, group):
                 group.run(lambda r, c, st: c.all_reduce(xs[r], outs[r], op=op, stream=st))
                 assert [c.stats()["staged_calls"] - s for c, s in zip(comms, st0)] == [1] * n
                 for r in range(n):
-                    R.assert_same(outs[r], _generic_ref(torch, coll, xs, op), f"generic staged {name} op={op} rank {r}")
+                    R.assert_same(outs[r], R.generic_ref(xs, op), f"generic staged {name} op={op} rank {r}")
 
 
 # ------------------------------------------------------------------------------------------------- one rank
@@ -512,7 +488,7 @@ def test_all_reduce_host_per_chunk(torch_cuda, coll_mod, group):
                 [(int(regime == "zero_copy"), int(regime == "pipelined"))] * n, what
             parts, d = [], 0
             for m, a in zip(chunks, algos):
-                parts.append(R.ref_reduce([x[d:d + m] for x in xs], order_for(a, n, in_dt, m), 0.1, out_dt))
+                parts.append(R.ref_reduce([x[d:d + m] for x in xs], R.order_for(a, n, in_dt, m), 0.1, out_dt))
                 d += m
             want = torch.cat(parts)
             for r in range(n):

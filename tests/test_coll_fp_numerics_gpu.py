@@ -19,17 +19,9 @@ PAIRS = [("float32", "float32"), ("float32", "bfloat16"), ("float32", "float16")
          ("float16", "float16"), ("float16", "float32"), ("float16", "float8_e4m3fn"), ("float16", "float8_e5m2")]
 SUBSET = [("bfloat16", "bfloat16"), ("float32", "bfloat16"), ("float16", "float16"), ("bfloat16", "float32"), ("float32", "float32"),
           ("float16", "float8_e4m3fn")]
-RANK_ORDER_ALGOS = ("ll", "ll2", "oneshot")
 
 
 group = group_fixture(3, arena_mb=160, timeout_ms=60000)
-
-
-def order_for(algo, n, e, count):
-    if algo in RANK_ORDER_ALGOS:
-        return list(range(n))
-    assert algo == "twoshot", f"no bit-exact order model for {algo}"
-    return ("owner", n, e, count)
 
 
 def ar_expected(coll, comms, algo, count, is_, os_):
@@ -60,7 +52,7 @@ def check_all_reduce(torch, coll, g, ins, count, in_name, out_name, algo, op, sc
     a = next(iter(got))
     want_algo = ar_expected(coll, comms, algo, count, is_, os_)
     assert a == want_algo, f"{what}: asked for {algo}, expected {want_algo}, ran {a}"
-    want = R.ref_reduce(xs, order_for(a, n, R.vec_elems(in_dt), count), R.scale_of(coll, op, scale, n), out_dt)
+    want = R.ref_reduce(xs, R.order_for(a, n, in_dt, count), R.scale_of(coll, op, scale, n), out_dt)
     for r in range(n):
         R.assert_same(outs[r], want, f"{what} rank {r} ran {a}")
     if own_outs:
@@ -461,24 +453,6 @@ def test_one_rank_all_ops(torch_cuda, coll_mod):
 
 
 # ------------------------------------------------------------------------------------------------- generic kernel
-def _generic_ref(torch, coll, xs, op):
-    """Rank order from rank 0's value, in the accumulator type (fp32 for fp16 / bf16); min / max propagate NaN from any rank and keep
-    the lower rank's value on a tie."""
-    wide = xs[0].dtype in (torch.float16, torch.bfloat16)
-    acc = xs[0].float() if wide else xs[0].clone()
-    for x in xs[1:]:
-        b = x.float() if wide else x
-        if op == coll.SUM:
-            acc = acc + b
-        elif op == coll.PROD:
-            acc = acc * b
-        elif op == coll.MIN:
-            acc = torch.where((b < acc) | (b != b), b, acc)
-        else:
-            acc = torch.where((b > acc) | (b != b), b, acc)
-    return acc.to(xs[0].dtype)
-
-
 @pytest.mark.parametrize("group", [3, 5], indirect=True)
 def test_generic_kernel(torch_cuda, coll_mod, group):
     torch, coll = torch_cuda, coll_mod
@@ -486,6 +460,9 @@ def test_generic_kernel(torch_cuda, coll_mod, group):
     g = torch.Generator(device="cuda").manual_seed(n)
     cases = [(name, op) for name in ("float32", "float16", "bfloat16") for op in (coll.MIN, coll.MAX, coll.PROD)]
     cases += [("int8", coll.SUM), ("uint8", coll.SUM), ("int32", coll.SUM), ("float64", coll.SUM), ("int32", coll.MIN)]
+    # unsigned against signed compares (values >= 2^31 and >= 2^63, INT64_MIN and INT64_MAX) and wrapping sums and products
+    cases += [(name, op) for name in ("uint32", "int64", "uint64") for op in (coll.SUM, coll.PROD, coll.MIN, coll.MAX)]
+    cases += [("int8", coll.PROD), ("int32", coll.PROD)]
     for name, op in cases:
         t = DTYPES[name]
         e = 16 // R.esize(t)
@@ -500,12 +477,11 @@ def test_generic_kernel(torch_cuda, coll_mod, group):
                 xs = [torch.randn(count, generator=g, device="cuda", dtype=torch.float64) * 2.0 ** torch.randint(-30, 30, (count,), generator=g, device="cuda")
                       for _ in range(n)]
             else:
-                lo, hi = (torch.iinfo(t).min, torch.iinfo(t).max)
-                xs = [torch.randint(lo, hi, (count,), generator=g, device="cuda", dtype=torch.int64).to(t) for _ in range(n)]
+                xs = [R.int_tensor(x, t) for x in R.int_inputs(n, count, t, seed=count + 10 * op + n)]
             ins = [c.empty(count, t) for c in comms]
             for b, x in zip(ins, xs):
                 b.copy_(x)
-            want = _generic_ref(torch, coll, ins, op)
+            want = R.generic_ref(ins, op)
             what = f"generic n={n} {name} op={op} count={count}"
             outs = [c.empty(count, t) for c in comms]
             gen0 = [c.stats()["generic_launches"] for c in comms]
