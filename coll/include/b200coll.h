@@ -553,6 +553,47 @@ b200collResult_t b200collReduceScatterRmsNormQuantized(const void* x, void* resi
                                                        size_t row_len, float eps, int gather, b200collDataType_t dtype,
                                                        b200collDataType_t wire_dtype, int block, b200collComm_t comm, b200collStream_t stream);
 
+/* Ulysses all-to-all for sequence-parallel attention (DeepSpeed-Ulysses), one kernel per call for 1 to 3 tensors (q, k and v, or one
+ * attention output) of one element type and one batch, seq_local and head_dim. N ranks, B = batch, S_l = seq_local, S = N * S_l,
+ * D = head_dim. Tensor i has heads H_i, counted in the full (unsharded) layout, and two sides:
+ *   seq:  the sequence-sharded side [B, S_l, H_i, D], row-strided: token row (b, t) starts row_stride elements after row (b, t - 1) (and
+ *         row (b, 0) after (b - 1, S_l - 1)), and holds H_i * D contiguous elements. A column slice of a packed [B * S_l, (Hq + 2 Hkv) * D]
+ *         QKV projection output has this shape.
+ *   head: the head-sharded side, dense [B, S, Hl_i, D].
+ * SeqToHeads (before attention): on rank r, head[b, s * S_l + t, j, :] = seq of rank s [b, t, head_i(r, j), :], where
+ *   H_i % N == 0:  Hl_i = H_i / N and head_i(r, j) = r * H_i / N + j;
+ *   else N % H_i == 0 (fewer KV heads than ranks, MQA included):  Hl_i = 1 and head_i(r, 0) = floor(r * H_i / N), the KV head of rank r's
+ *   query heads whenever Hq % N == 0; each source head goes to N / H_i ranks;
+ *   anything else is InvalidArgument.
+ * HeadsToSeq (after attention), the inverse layout move: on rank r, seq[b, t, h, :] = head of rank h / (H_i / N) [b, r * S_l + t,
+ * h % (H_i / N), :]. It needs H_i % N == 0 (the replicated layout is refused: its inverse is a sum over the replicas). HeadsToSeq of
+ * SeqToHeads is the identity for every tensor that is not replicated.
+ * Values: a bit copy (NaN payloads, -0 and inf survive), no cast and no scale. dtype bf16, fp16, fp32, e4m3 or e5m2.
+ * Arguments (InvalidArgument, message in b200collGetLastError, nothing launched): ntensors not in [1, 3]; head_dim * sizeof(dtype) not a
+ * positive multiple of 16; heads <= 0; a pointer not 16-byte aligned, or null when B * S_l > 0; row_stride < heads * head_dim, or
+ * row_stride * sizeof(dtype) not a multiple of 16; B * S_l >= 2^31; more than 2^31 - 1 16-byte vectors per rank in one side of a tensor or
+ * moved by the call; an output (head for SeqToHeads, seq for HeadsToSeq) overlapping any source or another output (column slices of one
+ * buffer with one row stride overlap only where their columns meet).
+ * Placement, as b200collAllToAllv (the kernel pushes): with more than one rank every output must be arena memory at the same offset on
+ * every rank, else InvalidUsage (there is no staging path); sources may be any device buffer, as only their own rank reads them. Shapes
+ * must be equal on every rank; B200COLL_CHECK=1 cross-checks the direction, ntensors, B, S_l, D, dtype, every heads, row_stride and output
+ * offset on multi-process communicators and turns a disagreement into InvalidUsage. B * S_l == 0 (then the same on every rank) returns
+ * without a launch. A poisoned communicator gives RemoteError. The kernel ends with a releasing barrier, so the outputs may be read and the
+ * sources overwritten by the next operation on the stream. The host reads no device data, so the call can be captured in a CUDA graph.
+ * One rank: a local strided copy, no barrier, any device buffers (splitting a packed QKV into dense q, k and v).
+ * b200collStats count an alltoall of the source bytes (B * S_l * H_i * D * sizeof(dtype) summed over the tensors) under twoshot (copy with
+ * one rank), one kernel launch. The tuner and b200collCommSetAlgo do not apply. */
+typedef struct {
+  void* seq;            /* the sequence-sharded side: source of SeqToHeads, destination of HeadsToSeq */
+  size_t row_stride;    /* elements between consecutive token rows of seq (>= heads * head_dim) */
+  void* head;           /* the head-sharded side, dense: destination of SeqToHeads, source of HeadsToSeq */
+  int heads;            /* H_i, in the full layout */
+} b200collUlyssesTensor;
+b200collResult_t b200collAllToAllSeqToHeads(const b200collUlyssesTensor* tensors, int ntensors, size_t batch, size_t seq_local,
+                                            size_t head_dim, b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
+b200collResult_t b200collAllToAllHeadsToSeq(const b200collUlyssesTensor* tensors, int ntensors, size_t batch, size_t seq_local,
+                                            size_t head_dim, b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
+
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.
  * AllReduceHost is the end-to-end step "pinned host -> GPU -> all-reduce -> pinned host" as one asynchronous call on `stream`:

@@ -65,6 +65,8 @@ struct Opts {
   int rq_block = 0;               // --rms-norm-quantize WIRE:BLOCK: its FP8 out, one fp32 scale per 1 x BLOCK (0 = off)
   bool rms_gather = false;        // --rms-norm-gather: with --op reduce_scatter, the normed rows all-gathered in the same kernel
   b200collDataType_t rq_wire = b200collFloat8e4m3;
+  int uly_hq = 0, uly_hkv = 0, uly_d = 0;   // --ulysses HQ:HKV:D: the Ulysses all-to-all of a packed QKV (0 = off)
+  bool uly_back = false;                    // --ulysses-back: heads -> sequence, the attention output
 };
 
 // Block-scaled mode: each rank's send buffer is a [rows, row_len] FP8 matrix with one fp32 scale per bs_rows x bs_cols block. Scales are
@@ -710,6 +712,107 @@ static float expected(const Opts& o, int rank, int n, size_t e, size_t count) {
   /* alltoall */ { int src = (int)(e / count); return gen(src, (size_t)rank * count + e % count) * o.scale; }
 }
 
+// Ulysses mode (--ulysses HQ:HKV:D). B = 1. Sequence -> heads: every rank's source is a packed QKV projection output [S_l, (HQ + 2 HKV) * D]
+// whose q, k and v are column slices (row stride (HQ + 2 HKV) * D), moved by one b200collAllToAllSeqToHeads into three dense head shards
+// [S, Hl, D]. --ulysses-back: the attention output, a dense [S, HQ / N, D] head shard, back to a dense [S_l, HQ, D] sequence shard. S_l is
+// the largest token count whose source fits in `bytes`. Sources hold a hash of (rank, 32-bit word), so every misplaced byte shows; -c 1
+// computes every output byte's source on the host. "rw GB/s" counts the source bytes read and the output bytes written.
+static uint32_t uly_word(int rank, size_t w) { return co_hash((uint32_t)w * 2654435761u ^ (uint32_t)(w >> 32) ^ (uint32_t)rank * 0x9E3779B9u); }
+static uint8_t uly_byte(int rank, size_t b) { return (uint8_t)(uly_word(rank, b / 4) >> (8 * (b % 4))); }
+__global__ void k_uly_fill(uint32_t* p, size_t n, int rank) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    uint32_t x = (uint32_t)i * 2654435761u ^ (uint32_t)(i >> 32) ^ (uint32_t)rank * 0x9E3779B9u;
+    x ^= x >> 16; x *= 0x7FEB352Du; x ^= x >> 15; x *= 0x846CA68Bu; x ^= x >> 16;     // co_hash
+    p[i] = x;
+  }
+}
+static size_t uly_local_heads(int n, int h) { return h % n == 0 ? (size_t)(h / n) : 1; }
+// Output bytes per source byte, at most: the replicated heads are stored N / H times.
+static size_t uly_out_bytes(const Opts& o, int n, size_t src_bytes) {
+  if (o.uly_back) return src_bytes;
+  const size_t in = (size_t)o.uly_hq + 2 * (size_t)o.uly_hkv, out = (size_t)n * (uly_local_heads(n, o.uly_hq) + 2 * uly_local_heads(n, o.uly_hkv));
+  return src_bytes / in * out + 4096;
+}
+static int run_ulysses(const Opts& o, RankCtx& ctx) {
+  const int n = ctx.nranks, rank = ctx.rank;
+  const size_t es = b200collTypeSize(o.in_dt), D = (size_t)o.uly_d, hb = D * es;   // head bytes
+  const int nt = o.uly_back ? 1 : 3;
+  const int H[3] = {o.uly_hq, o.uly_hkv, o.uly_hkv};
+  const size_t col[3] = {0, (size_t)o.uly_hq, (size_t)o.uly_hq + o.uly_hkv};     // the first head of q, k and v in the packed row
+  const size_t src_row = o.uly_back ? (size_t)o.uly_hq / n * hb : ((size_t)o.uly_hq + 2 * (size_t)o.uly_hkv) * hb;   // source bytes per token row
+  void *src = nullptr, *dst = nullptr;
+  CC(b200collMemAlloc(ctx.comm, &src, o.max_bytes + 4096));
+  CC(b200collMemAlloc(ctx.comm, &dst, uly_out_bytes(o, n, o.max_bytes + 4096)));
+  const cudaStream_t st = ctx.st;
+  long total_errors = 0;
+  if (rank == 0) {
+    printf("# b200coll_perf op=alltoall ulysses %s nranks=%d dtype=%s HQ=%d HKV=%d D=%zu B=1: size = source bytes per rank (%s); rw GB/s = "
+           "(source read + output written) / time\n", o.uly_back ? "heads->seq" : "seq->heads", n, dt_name(o.in_dt), o.uly_hq, o.uly_hkv, D,
+           o.uly_back ? "the attention output" : "q + k + v, packed");
+    printf("#%13s %10s %6s %8s | %10s %8s %6s\n", "size(B)", "seq_local", "type", "algo", "us", "rwGB/s", "#wrong");
+    fflush(stdout);
+  }
+  for (size_t bytes = o.min_bytes; bytes <= o.max_bytes; bytes *= o.factor) {
+    const size_t sl = o.uly_back ? bytes / (src_row * n) : bytes / src_row;           // back: the source is [S = N * S_l, HQ / N, D]
+    if (sl == 0) continue;
+    const size_t S = sl * n, src_bytes = o.uly_back ? S * src_row : sl * src_row;
+    b200collUlyssesTensor t[3];
+    size_t out_off[3], out_bytes = 0;
+    for (int i = 0; i < nt; i++) {
+      out_off[i] = out_bytes;
+      const size_t hl = uly_local_heads(n, H[i]);
+      if (o.uly_back) t[i] = {dst, (size_t)o.uly_hq * D, src, o.uly_hq};
+      else t[i] = {static_cast<char*>(src) + col[i] * hb, ((size_t)o.uly_hq + 2 * (size_t)o.uly_hkv) * D, static_cast<char*>(dst) + out_bytes, H[i]};
+      out_bytes += o.uly_back ? sl * o.uly_hq * hb : S * hl * hb;
+    }
+    k_uly_fill<<<256, 256, 0, st>>>(static_cast<uint32_t*>(src), src_bytes / 4, rank);
+    RT(cudaGetLastError());
+    RT(cudaMemsetAsync(dst, 0x7B, out_bytes, st));
+    auto launch = [&](int) {
+      if (o.uly_back) CC(b200collAllToAllHeadsToSeq(t, nt, 1, sl, D, o.in_dt, ctx.comm, st));
+      else CC(b200collAllToAllSeqToHeads(t, nt, 1, sl, D, o.in_dt, ctx.comm, st));
+    };
+    long errs = 0;
+    if (o.check) {
+      check_launch(o, ctx, launch);
+      std::vector<uint8_t> host(out_bytes);
+      RT(cudaMemcpy(host.data(), dst, out_bytes, cudaMemcpyDeviceToHost));
+      for (int i = 0; i < nt; i++) {
+        const size_t hl = uly_local_heads(n, H[i]);
+        const uint8_t* got = host.data() + out_off[i];
+        if (o.uly_back) {                     // x_r[t, h] = y_{h / Hl}[r * S_l + t, h % Hl]
+          const size_t hlq = (size_t)o.uly_hq / n;
+          for (size_t tk = 0; tk < sl; tk++)
+            for (size_t h = 0; h < (size_t)o.uly_hq; h++)
+              for (size_t e = 0; e < hb; e++) {
+                const uint8_t want = uly_byte((int)(h / hlq), (((size_t)rank * sl + tk) * hlq + h % hlq) * hb + e), g = got[(tk * o.uly_hq + h) * hb + e];
+                if (g != want) { if (errs < 4) fprintf(stderr, "rank %d ulysses back size %zu token %zu head %zu byte %zu: got 0x%02x want 0x%02x\n", rank, bytes, tk, h, e, g, want); errs++; }
+              }
+        } else {                              // y_r[s * S_l + t, j] = x_s[t, head(r, j)], x_s a column slice of the packed row
+          for (size_t T = 0; T < S; T++)
+            for (size_t j = 0; j < hl; j++) {
+              const size_t s = T / sl, tk = T % sl, h = H[i] % n == 0 ? (size_t)rank * hl + j : (size_t)rank * H[i] / n;
+              for (size_t e = 0; e < hb; e++) {
+                const uint8_t want = uly_byte((int)s, tk * src_row + (col[i] + h) * hb + e), g = got[(T * hl + j) * hb + e];
+                if (g != want) { if (errs < 4) fprintf(stderr, "rank %d ulysses tensor %d size %zu token %zu head %zu byte %zu: got 0x%02x want 0x%02x\n", rank, i, bytes, T, j, e, g, want); errs++; }
+              }
+            }
+        }
+      }
+    }
+    const Timing tm = timed(o, ctx, errs, launch);
+    total_errors += tm.errors;
+    if (rank == 0) {
+      printf("%14zu %10zu %6s %8s | %10.2f %8.2f %6ld\n", src_bytes, sl, dt_name(o.in_dt), n > 1 ? "twoshot" : "copy", tm.ms * 1e3,
+             (src_bytes + out_bytes) / (tm.ms * 1e3) / 1e3, tm.errors);
+      fflush(stdout);
+    }
+  }
+  CC(b200collMemFree(ctx.comm, dst));
+  CC(b200collMemFree(ctx.comm, src));
+  return mode_result(ctx, total_errors);
+}
+
 static int run_rank(const Opts& o, RankCtx ctx) {
   const int n = ctx.nranks, rank = ctx.rank;
   RT(cudaSetDevice(ctx.dev));
@@ -720,6 +823,7 @@ static int run_rank(const Opts& o, RankCtx ctx) {
     for (int a = 0; a < b200collNumAlgos; a++) if (o.algo == b200collAlgoName((b200collAlgo_t)a)) CC(b200collCommSetAlgo(ctx.comm, (b200collAlgo_t)a));
   }
   if (o.max_ctas > 0) CC(b200collCommSetMaxCtas(ctx.comm, o.max_ctas));
+  if (o.uly_d) return run_ulysses(o, ctx);
   const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt);
   const bool is_bc = o.op == "broadcast", is_rd = o.op == "reduce", is_sr = o.op == "sendrecv";
   const bool is_ar = o.op == "all_reduce" || is_bc || is_rd || is_sr;      // "whole message" geometry: count elements in, count out
@@ -982,6 +1086,18 @@ static LauncherRank launcher_rank() {
 // Every conflict between flags and with the number of ranks (o.nranks), refused before any communicator or buffer exists.
 static bool flags_ok(const Opts& o) {
   const int n = o.nranks;
+  if (o.uly_back && !o.uly_d) { fprintf(stderr, "--ulysses-back takes --ulysses HQ:HKV:D\n"); return false; }
+  if (o.uly_d) {
+    if (o.op != "alltoall" || o.out_dt != o.in_dt || o.scale != 1.0f || o.q_block || o.bs_rows || o.combine_k || o.route_e || o.cq_block || o.rms_row) {
+      fprintf(stderr, "--ulysses HQ:HKV:D takes --op alltoall, and no --out-dtype, --scale, --quantize, --block-scale, --combine, --route or --rms-norm\n");
+      return false;
+    }
+    if (((size_t)o.uly_d * b200collTypeSize(o.in_dt)) % 16) { fprintf(stderr, "--ulysses HQ:HKV:D: D * sizeof(dtype) must be a multiple of 16 bytes\n"); return false; }
+    for (int h : {o.uly_hq, o.uly_hkv})
+      if (h % n && n % h) { fprintf(stderr, "--ulysses HQ:HKV:D: HQ and HKV must each be a multiple or a divisor of the %d ranks\n", n); return false; }
+    if (o.uly_back && o.uly_hq % n) { fprintf(stderr, "--ulysses-back: HQ must be a multiple of the %d ranks\n", n); return false; }
+    return true;
+  }
   if (o.rms_row && ((o.op != "all_reduce" && o.op != "reduce_scatter") || o.out_dt != o.in_dt || o.scale != 1.0f || o.q_block || o.bs_rows || o.combine_k || o.route_e || o.cq_block ||
                     !wide(o.in_dt))) {
     fprintf(stderr, "--rms-norm ROW_LEN takes --op all_reduce or reduce_scatter and -d bfloat16|half|float, and no --out-dtype, --scale, --quantize,\n"
@@ -1041,7 +1157,8 @@ static size_t arena_bytes(const Opts& o) {
   const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt);
   return std::max(o.window, o.max_bytes) + std::max(o.window / is * os, o.max_bytes / is * os) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) +
          q_scratch_bytes(o) + (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o) +     // --route: recv holds K rows per token
-         (o.rms_row ? o.max_bytes + 4096 : 0) + rms_scale_bytes(o);                                   // --rms-norm: the residual (and the scales of q)
+         (o.rms_row ? o.max_bytes + 4096 : 0) + rms_scale_bytes(o) +                                  // --rms-norm: the residual (and the scales of q)
+         (o.uly_d ? uly_out_bytes(o, o.nranks, o.max_bytes + 4096) : 0);                             // --ulysses: the head shards
 }
 
 int main(int argc, char** argv) {
@@ -1076,6 +1193,12 @@ int main(int argc, char** argv) {
       if (v < 16 || v > 16384 || v % 16) { fprintf(stderr, "--rms-norm ROW_LEN: a multiple of 16 in [16, 16384]\n"); return 1; }
       o.rms_row = (size_t)v;
     }
+    else if (a == "--ulysses") {
+      if (sscanf(next(), "%d:%d:%d", &o.uly_hq, &o.uly_hkv, &o.uly_d) != 3 || o.uly_hq < 1 || o.uly_hkv < 1 || o.uly_d < 1) {
+        fprintf(stderr, "--ulysses HQ:HKV:D: three positive integers\n"); return 1;
+      }
+    }
+    else if (a == "--ulysses-back") o.uly_back = true;
     else if (a == "--combine") { o.combine_k = atoi(next()); if (o.combine_k < 1) { fprintf(stderr, "--combine K: K >= 1\n"); return 1; } }
     else if (a == "--route") {
       if (sscanf(next(), "%d:%d", &o.route_e, &o.route_k) != 2 || o.route_e < 1 || o.route_e > 1024 || o.route_k < 1) { fprintf(stderr, "--route E:K: 1 <= E <= 1024, K >= 1\n"); return 1; }
@@ -1145,6 +1268,10 @@ int main(int argc, char** argv) {
            "                            are rounded down to a multiple of the ranks, each rank keeps a residual shard of rows / nranks rows and\n"
            "                            stores the out rows of its slice; -c 1 checks the shard, every other residual row unchanged, and out\n"
            "  --rms-norm-gather         with --op reduce_scatter --rms-norm ROW_LEN: the normed rows all-gathered in the same kernel\n"
+           "  --ulysses HQ:HKV:D        --op alltoall, -d bfloat16|half|float|e4m3|e5m2: the Ulysses all-to-all of sequence-parallel attention, B = 1;\n"
+           "                            every rank's packed QKV [S_l, (HQ + 2 HKV) * D] (q, k and v column slices) to dense head shards in one\n"
+           "                            call; size = source bytes per rank, rounded down to whole tokens; -c 1 checks every output byte\n"
+           "  --ulysses-back            with --ulysses HQ:HKV:D: heads -> sequence, the [S, HQ / N, D] attention output back to [S_l, HQ, D]\n"
            "  --selfcheck              report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;
     }

@@ -46,6 +46,10 @@ class BlockScale(C.Structure):
     _fields_ = [("scales", C.c_void_p), ("row_len", C.c_size_t), ("block_rows", C.c_int), ("block_cols", C.c_int)]
 
 
+class UlyssesTensor(C.Structure):
+    _fields_ = [("seq", C.c_void_p), ("row_stride", C.c_size_t), ("head", C.c_void_p), ("heads", C.c_int)]
+
+
 class Config(C.Structure):
     _fields_ = [("arena_bytes", C.c_size_t), ("enable_nvls", C.c_int), ("max_ctas", C.c_int), ("timeout_ms", C.c_int), ("debug", C.c_int)]
 
@@ -151,6 +155,8 @@ def load() -> C.CDLL:
     L.b200collAllReduceRmsNormQuantized.argtypes = [vp, vp, vp, vp, C.POINTER(C.c_float), sz, sz, C.c_float, ci, ci, ci, vp, vp]
     L.b200collReduceScatterRmsNorm.argtypes = [vp, vp, vp, vp, sz, sz, C.c_float, ci, ci, vp, vp]
     L.b200collReduceScatterRmsNormQuantized.argtypes = [vp, vp, vp, vp, C.POINTER(C.c_float), sz, sz, C.c_float, ci, ci, ci, ci, vp, vp]
+    L.b200collAllToAllSeqToHeads.argtypes = [C.POINTER(UlyssesTensor), ci, sz, sz, sz, ci, vp, vp]
+    L.b200collAllToAllHeadsToSeq.argtypes = [C.POINTER(UlyssesTensor), ci, sz, sz, sz, ci, vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -561,6 +567,116 @@ def check_reduce_scatter_rms_norm_quantized(nranks: int, x, residual, weight, q,
     the wire type's library code). Shapes as in check_reduce_scatter_rms_norm, with q of out's shape and scales [..., row_len // block]
     of out's leading dimensions; everything else as in check_all_reduce_rms_norm_quantized."""
     return _check_rms_norm_quantized(x, residual, weight, q, scales, block, wire, eps, sp=(nranks, bool(gather)))
+
+
+def ulysses_local_heads(nranks: int, heads: int, replicate: bool = True) -> int:
+    """Heads per rank on the head-sharded side of the Ulysses all-to-all: heads // nranks when nranks divides heads, else 1 when heads
+    divides nranks (each head replicated to nranks // heads ranks; replicate=False, heads -> sequence, refuses it); ValueError otherwise."""
+    if heads % nranks == 0:
+        return heads // nranks
+    if not replicate:
+        raise ValueError(f"heads ({heads}) must be a multiple of nranks ({nranks}): the replicated layout has no inverse move")
+    if nranks % heads:
+        raise ValueError(f"heads ({heads}) must be a multiple or a divisor of nranks ({nranks})")
+    return 1
+
+
+def _seq_row_stride(name: str, t) -> int:
+    """The row stride (elements) of a sequence-side [B, S_l, H, D] view whose token rows are uniformly strided."""
+    B, S_l, H, D = t.shape
+    if (D > 1 and t.stride(3) != 1) or (H > 1 and t.stride(2) != D):
+        raise ValueError(f"{name}: each token row must hold its heads * head_dim elements contiguously (stride(3) == 1, stride(2) == head_dim), "
+                         f"got strides {t.stride()}")
+    rs = t.stride(1) if S_l > 1 or B == 1 else t.stride(0)
+    if S_l > 1 and B > 1 and t.stride(0) != S_l * rs:
+        raise ValueError(f"{name}: token rows must be uniformly strided (stride(0) == seq_local * stride(1)), got strides {t.stride()}")
+    return rs if B * S_l > 1 else H * D          # one token row: its stride is never used
+
+
+def _spans_overlap(a, b) -> bool:
+    """Whether two row-strided byte regions (ptr, rows, stride, width) share a byte; as the library decides it."""
+    ext = [0 if r == 0 else (r - 1) * s + w for _, r, s, w in (a, b)]
+    if not ext[0] or not ext[1] or not (a[0] < b[0] + ext[1] and b[0] < a[0] + ext[0]):
+        return False
+    if a[1] < 2 or b[1] < 2 or a[2] != b[2] or a[3] > a[2] or b[3] > b[2]:
+        return True
+    dd = (b[0] - a[0]) % a[2]
+    return dd < a[3] or dd + b[3] > a[2]
+
+
+def _check_ulysses(nranks: int, seqs, heads, s2h: bool) -> tuple[int, int, int, list[tuple[int, int]]]:
+    import torch
+    what = "seq_to_heads" if s2h else "heads_to_seq"
+    seqs, heads = list(seqs), list(heads)
+    if not 1 <= len(seqs) <= 3 or len(heads) != len(seqs):
+        raise ValueError(f"{what}: 1 to 3 tensors and one output per tensor, got {len(seqs)} and {len(heads)}")
+    sname, hname = ("xs", "outs") if s2h else ("outs", "ys")
+    dt = seqs[0].dtype
+    if dt not in (torch.bfloat16, torch.float16, torch.float32, torch.float8_e4m3fn, torch.float8_e5m2):
+        raise ValueError(f"{what}: dtype must be bfloat16, float16, float32, float8_e4m3fn or float8_e5m2, got {dt}")
+    if any(t.dim() != 4 for t in seqs + heads):
+        raise ValueError(f"{what}: every tensor must be 4-D: [B, S_l, H, D] on the sequence side, [B, S, H / N, D] on the head side")
+    B, S_l, _, D = seqs[0].shape
+    es = seqs[0].element_size()
+    if (D * es) % 16 or D == 0:
+        raise ValueError(f"{what}: head_dim * sizeof(dtype) must be a positive multiple of 16 bytes, got {D} x {es}")
+    rows = B * S_l
+    if rows > _I31:
+        raise ValueError(f"{what}: batch * seq_local must be below 2^31, got {rows}")
+    per, srcs, dsts, moved = [], [], [], 0
+    for i, (x, y) in enumerate(zip(seqs, heads)):
+        if x.dtype != dt or y.dtype != dt:
+            raise ValueError(f"{what}: tensor {i}: every tensor must have dtype {dt}, got {x.dtype} and {y.dtype}")
+        if (x.shape[0], x.shape[1], x.shape[3]) != (B, S_l, D):
+            raise ValueError(f"{what}: {sname}[{i}] must be [{B}, {S_l}, H, {D}] like the first, got {list(x.shape)}")
+        H = x.shape[2]
+        if H < 1:
+            raise ValueError(f"{what}: {sname}[{i}] has no heads")
+        hl = ulysses_local_heads(nranks, H, s2h)
+        want = (B, nranks * S_l, hl, D)
+        if tuple(y.shape) != want or not y.is_contiguous():
+            raise ValueError(f"{what}: {hname}[{i}] must be a contiguous {list(want)} tensor, got {list(y.shape)}")
+        rs = _seq_row_stride(f"{sname}[{i}]", x)
+        if rs < H * D or (rs * es) % 16:
+            raise ValueError(f"{what}: {sname}[{i}]: the row stride ({rs}) must be at least heads * head_dim ({H * D}) and a multiple of 16 bytes")
+        if rows and (x.data_ptr() % 16 or y.data_ptr() % 16):
+            raise ValueError(f"{what}: tensor {i}: every pointer must be 16-byte aligned")
+        dv = D * es // 16
+        if (rows - 1) * rs * es // 16 + H * dv > _I31 or y.numel() * es // 16 > _I31:
+            raise ValueError(f"{what}: tensor {i}: more than 2^31 - 1 16-byte vectors per rank")
+        moved += rows * H * dv
+        seq_span = (x.data_ptr(), rows, rs * es, H * D * es)          # (address, rows, stride, width) in bytes
+        head_span = (y.data_ptr(), 1, y.numel() * es, y.numel() * es)
+        srcs.append(seq_span if s2h else head_span)
+        dsts.append(head_span if s2h else seq_span)
+        per.append((rs, H))
+    if moved > _I31:
+        raise ValueError(f"{what}: more than 2^31 - 1 16-byte vectors moved per rank")
+    for i, d in enumerate(dsts):
+        for j, s in enumerate(srcs):
+            if _spans_overlap(d, s):
+                raise ValueError(f"{what}: output {i} overlaps source {j}")
+        for j in range(i + 1, len(dsts)):
+            if _spans_overlap(d, dsts[j]):
+                raise ValueError(f"{what}: outputs {i} and {j} overlap")
+    return B, S_l, D, per
+
+
+def check_all_to_all_seq_to_heads(nranks: int, xs, outs) -> tuple[int, int, int, list[tuple[int, int]]]:
+    """The rules of Comm.all_to_all_seq_to_heads, checked on the tensors' metadata (no device, no communicator): raises ValueError, returns
+    (batch, seq_local, head_dim, [(row_stride, heads)] per tensor). xs: 1 to 3 [B, S_l, H_i, D] views of one dtype (bfloat16, float16,
+    float32, float8_e4m3fn or float8_e5m2) whose token rows are uniformly strided (stride(3) == 1, stride(2) == D, stride(0) == S_l *
+    stride(1)), such as column slices of a packed QKV tensor; outs: contiguous [B, N * S_l, Hl_i, D], Hl_i = H_i / N, or 1 when H_i divides
+    N (ulysses_local_heads). D * sizeof(dtype) and every row stride a multiple of 16 bytes, every pointer 16-byte aligned, B * S_l below
+    2^31, at most 2^31 - 1 16-byte vectors per rank; no output may overlap a source or another output."""
+    return _check_ulysses(nranks, xs, outs, True)
+
+
+def check_all_to_all_heads_to_seq(nranks: int, ys, outs) -> tuple[int, int, int, list[tuple[int, int]]]:
+    """The rules of Comm.all_to_all_heads_to_seq, checked on the tensors' metadata: raises ValueError, returns as
+    check_all_to_all_seq_to_heads. ys: 1 to 3 contiguous [B, N * S_l, H_i / N, D] tensors; outs: the [B, S_l, H_i, D] sequence-side views
+    (row-strided as xs there). H_i must be a multiple of N: the replicated layout has no inverse. Everything else as seq-to-heads."""
+    return _check_ulysses(nranks, outs, ys, False)
 
 
 def _check_routed(nranks: int, x, topk_idx, num_experts: int, recv, expert_counts, route, dropped, fp8=None) -> None:
@@ -1044,6 +1160,41 @@ class Comm:
         ep = self._ep(src, dst, scale)
         _check(load().b200collAllToAll(C.c_void_p(src.data_ptr()), C.c_void_p(dst.data_ptr()), src.numel() // self.nranks, C.byref(ep), self._h, self._stream(stream)), "AllToAll")
         return dst
+
+    def _ulysses(self, fn, name, seqs, heads, per, B, S_l, D, stream):
+        arr = (UlyssesTensor * len(seqs))(*[UlyssesTensor(x.data_ptr(), rs, y.data_ptr(), h) for x, y, (rs, h) in zip(seqs, heads, per)])
+        _check(fn(arr, len(seqs), B, S_l, D, torch_dtype_code(seqs[0].dtype), self._h, self._stream(stream)), name)
+
+    def all_to_all_seq_to_heads(self, xs, outs=None, stream=None):
+        """Ulysses all-to-all before attention, one kernel for up to three tensors (q, k, v): each [B, S_l, H_i, D] sequence shard in xs
+        (views with uniformly strided token rows, e.g. column slices of a packed QKV projection output) becomes a dense [B, N * S_l, Hl_i, D]
+        head shard, Hl_i = H_i / N; with fewer heads than ranks (GQA or MQA K and V, H_i dividing N) Hl_i = 1 and rank r gets head
+        r * H_i // N. Bit for bit as coll/include/b200coll.h's b200collAllToAllSeqToHeads states. Returns outs. With more than one rank outs
+        must be given, as arena tensors (`empty()`) at the same offsets on every rank; with one rank None allocates them."""
+        xs = list(xs)
+        if outs is None:
+            if self.nranks > 1:
+                raise ValueError("seq_to_heads with more than one rank needs outs: arena tensors (Comm.empty) of [B, S, H / N, D], the same on every rank")
+            outs = [x.new_empty(x.shape) for x in xs]
+        outs = list(outs)
+        B, S_l, D, per = check_all_to_all_seq_to_heads(self.nranks, xs, outs)
+        self._ulysses(load().b200collAllToAllSeqToHeads, "AllToAllSeqToHeads", xs, outs, per, B, S_l, D, stream)
+        return outs
+
+    def all_to_all_heads_to_seq(self, ys, outs=None, stream=None):
+        """The inverse of all_to_all_seq_to_heads, after attention: each dense [B, N * S_l, H_i / N, D] head shard in ys becomes the
+        [B, S_l, H_i, D] sequence shard in outs, which may be row-strided views; H_i must be a multiple of N. Bit for bit as
+        b200collAllToAllHeadsToSeq states. Returns outs. With more than one rank outs must be given, as arena tensors; with one rank None
+        allocates them."""
+        ys = list(ys)
+        if outs is None:
+            if self.nranks > 1:
+                raise ValueError("heads_to_seq with more than one rank needs outs: arena tensors (Comm.empty) of [B, S_l, H, D], the same on every rank")
+            outs = [y.new_empty(y.shape) for y in ys]
+        outs = list(outs)
+        B, S_l, D, per = check_all_to_all_heads_to_seq(self.nranks, ys, outs)
+        self._ulysses(load().b200collAllToAllHeadsToSeq, "AllToAllHeadsToSeq", outs, ys, per, B, S_l, D, stream)
+        return outs
 
     def _rows(self, xs):
         """A host list of nranks row counts or offsets, as the library's int64[nranks]."""
