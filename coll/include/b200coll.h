@@ -77,6 +77,7 @@ typedef enum {
  *                                                           the last whole vector are summed in rank order. A staged all-reduce (buffers
  *                                                           outside the arena) runs this per staging chunk, slices taken from the chunk.
  *   P2P reduce-scatter (16- and 32-bit inputs)              receiving rank r sums r, r+1, .., N-1, 0, .., r-1
+ *   context-parallel reduce-scatter                         ranks 0 .. N-1
  *   NVLS (multimem.ld_reduce)                               the switch's order: within an ulp of the exact sum, not bit-reproducible
  * Rounding to FP8 saturates to the finite range (+-inf becomes +-max, NaN stays NaN); fp16 overflows to inf.
  * All-gather, broadcast and all-to-all(v) apply the same epilogue per element: round((0 + x) * scale) (e4m3 in, bf16 out, scale =
@@ -593,6 +594,51 @@ b200collResult_t b200collAllToAllSeqToHeads(const b200collUlyssesTensor* tensors
                                             size_t head_dim, b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
 b200collResult_t b200collAllToAllHeadsToSeq(const b200collUlyssesTensor* tensors, int ntensors, size_t batch, size_t seq_local,
                                             size_t head_dim, b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
+
+/* Context parallelism, all-gather form (Llama 3's long-context training, cp_comm_type "all_gather" in Megatron / TransformerEngine):
+ * each rank keeps its query shard and gathers K and V over the whole sequence before attention (AllGatherContext); after it, the
+ * full-sequence dK and dV, partial sums over the rank's own queries, are reduce-scattered back to the sequence shards
+ * (ReduceScatterContext). One kernel per call for 1 to 3 tensors (K and V, or MLA's c_kv and k_pe) of one element type and one batch,
+ * seq_local and chunks. N ranks, B = batch, S_l = seq_local, S = N * S_l, C = chunks. Tensor i has width W_i elements per token and
+ * two sides:
+ *   shard: this rank's [B, S_l, W_i], row-strided: token row (b, t) starts row_stride elements after row (b, t - 1) (and row (b, 0)
+ *          after (b - 1, S_l - 1)), and holds W_i contiguous elements. A column slice of a packed QKV (or dQKV) tensor has this shape.
+ *   full:  dense [B, S, W_i], tokens in sequence order.
+ * Layout. C is 1 or 2; c = S_l / C. Local token t of rank r has k = t / c, u = t % c and global token gtok(r, t) = G(r, k) * c + u with
+ *   G(r, 0) = r,  G(r, 1) = 2N - 1 - r.
+ * C = 1 is contiguous sharding; C = 2 is the load-balanced causal layout (the sequence cut into 2N chunks, rank r holding chunks r
+ * and 2N - 1 - r), and needs S_l even.
+ * AllGatherContext: on every rank, full[b, gtok(s, t), :] = shard of rank s [b, t, :] for every rank s. A bit copy (NaN payloads, -0 and
+ * inf survive); dtype bf16, fp16, fp32, e4m3 or e5m2.
+ * ReduceScatterContext: on rank r, shard[b, t, :] = round_once(((+0 + full_0[b, g, :]) + full_1[b, g, :]) + .. + full_{N-1}[b, g, :])
+ * with g = gtok(r, t) and full_s rank s's full: summed in fp32 in rank order (the order table above) and rounded once to nearest even;
+ * dtype bf16, fp16 or fp32. With one rank it is a bit copy, as b200collReduceScatter is.
+ * Arguments (InvalidArgument, message in b200collGetLastError, nothing launched): ntensors not in [1, 3]; chunks not 1 or 2, or 2 with
+ * S_l odd; W_i * sizeof(dtype) not a positive multiple of 16; row_stride < W_i, or row_stride * sizeof(dtype) not a multiple of 16; a
+ * pointer not 16-byte aligned, or null when B * S_l > 0; B * S_l >= 2^31; more than 2^31 - 1 16-byte vectors in one side of a tensor
+ * or moved by the call; a dtype outside the lists above; an output (full for the gather, shard for the reduce-scatter) overlapping any
+ * source or another output (column slices of one buffer with one row stride overlap only where their columns meet).
+ * Placement: with more than one rank every full must be arena memory at the same offset on every rank, else InvalidUsage (the gather
+ * pushes into it, the reduce-scatter pulls from it; there is no staging path); shard may be any device buffer, as only its own rank
+ * touches it. With one rank any device buffers. Shapes must be equal on every rank; B200COLL_CHECK=1 cross-checks the direction,
+ * ntensors, dtype, B, S_l, C, and every W_i, row_stride and full offset on multi-process communicators and turns a disagreement into
+ * InvalidUsage. B * S_l == 0 (then the same on every rank) returns without a launch. A poisoned communicator gives RemoteError. The
+ * kernel starts with a barrier (no rank stores into or reads a full that an earlier operation on a peer's stream still uses) and ends
+ * with a releasing one, so the outputs may be read and the sources overwritten by the next operation on the stream. The host reads no
+ * device data, so both calls can be captured in a CUDA graph. One rank: a local strided copy, no barrier.
+ * b200collStats count an allgather (AllGatherContext) or a reducescatter (ReduceScatterContext) of the shard bytes (B * S_l * W_i *
+ * sizeof(dtype) summed over the tensors) under twoshot (copy with one rank), one kernel launch. The tuner and b200collCommSetAlgo do
+ * not apply. */
+typedef struct {
+  void* shard;          /* this rank's [B, S_l, W] rows, row-strided: source of the gather, destination of the reduce-scatter */
+  size_t row_stride;    /* elements between consecutive token rows of shard (>= width) */
+  void* full;           /* dense [B, S, W] in token order: destination of the gather, source of the reduce-scatter */
+  size_t width;         /* W, elements per token row (Hkv * D for K or V) */
+} b200collContextTensor;
+b200collResult_t b200collAllGatherContext(const b200collContextTensor* tensors, int ntensors, size_t batch, size_t seq_local, int chunks,
+                                          b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
+b200collResult_t b200collReduceScatterContext(const b200collContextTensor* tensors, int ntensors, size_t batch, size_t seq_local, int chunks,
+                                              b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
 
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.

@@ -67,6 +67,9 @@ struct Opts {
   b200collDataType_t rq_wire = b200collFloat8e4m3;
   int uly_hq = 0, uly_hkv = 0, uly_d = 0;   // --ulysses HQ:HKV:D: the Ulysses all-to-all of a packed QKV (0 = off)
   bool uly_back = false;                    // --ulysses-back: heads -> sequence, the attention output
+  int cp_c = 0;                             // --context W:C or HQ:HKV:D:C: the context-parallel gather / reduce-scatter, C chunks per rank (0 = off)
+  int cp_hq = 0, cp_hkv = 0, cp_d = 0;      // packed QKV (K and V column slices), or 0 with cp_w
+  size_t cp_w = 0;                          // one dense tensor of cp_w elements per token
 };
 
 // Block-scaled mode: each rank's send buffer is a [rows, row_len] FP8 matrix with one fp32 scale per bs_rows x bs_cols block. Scales are
@@ -813,6 +816,129 @@ static int run_ulysses(const Opts& o, RankCtx& ctx) {
   return mode_result(ctx, total_errors);
 }
 
+// Context-parallel mode (--context W:C or HQ:HKV:D:C). B = 1. --op all_gather: b200collAllGatherContext from each rank's shard, either K
+// and V as column slices of a packed QKV projection output [S_l, (HQ + 2 HKV) * D] or one dense [S_l, W] tensor, into dense [S, W]
+// full tensors (W = HKV * D) in token order. --op reduce_scatter: b200collReduceScatterContext from the full tensors back into the K and
+// V column slices of a packed dQKV [S_l, (HQ + 2 HKV) * D] (its Q columns poisoned, and checked untouched) or into a dense [S_l, W].
+// C = 1 contiguous sharding, 2 the load-balanced causal layout. The size is the shard bytes per rank (K + V, or the one tensor), rounded
+// down to whole tokens (an even count with C = 2). Gather sources hold a hash of (rank, 32-bit word); reduce-scatter fulls hold seeded
+// values with full mantissas, so the sums round. -c 1 checks every output byte on the host: the gather against the source byte the
+// header's gtok places there, the reduce-scatter against the fp32 sum in rank order rounded once. "rw GB/s" counts the shard bytes and
+// the full bytes this rank reads or writes.
+__host__ __device__ inline float cp_val(int rank, size_t i) {
+  uint32_t h = (uint32_t)(i * 2654435761u) ^ (uint32_t)(rank * 40503u + 0x9E3779B9u) ^ (uint32_t)(i >> 32);
+  h ^= h >> 15; h *= 0x2C1B3C6Du; h ^= h >> 12;
+  return ((h >> 31) ? -1.0f : 1.0f) * ldexpf(1.0f + (float)(h & 0x7FFFFF) * 0x1p-23f, (int)((h >> 23) % 17) - 8);
+}
+template <typename T> __global__ void k_cp_fill(T* p, size_t n, int rank) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = T(cp_val(rank, i));
+}
+static bool cp_packed(const Opts& o) { return o.cp_d > 0; }
+static size_t cp_width(const Opts& o) { return cp_packed(o) ? (size_t)o.cp_hkv * o.cp_d : o.cp_w; }          // elements per token of one tensor
+static size_t cp_row(const Opts& o) { return cp_packed(o) ? ((size_t)o.cp_hq + 2 * (size_t)o.cp_hkv) * o.cp_d : o.cp_w; }   // shard row stride
+static int cp_tensors(const Opts& o) { return cp_packed(o) ? 2 : 1; }
+// The shard buffer (packed QKV / dQKV, or the dense tensor) and the full tensors, in bytes, for shards of at most max_bytes.
+static size_t cp_shard_bytes(const Opts& o) { return o.max_bytes / (cp_tensors(o) * cp_width(o)) * cp_row(o) + 4096; }
+static size_t cp_full_bytes(const Opts& o, int n) { return (size_t)n * o.max_bytes + 4096; }
+static int run_context(const Opts& o, RankCtx& ctx) {
+  const int n = ctx.nranks, rank = ctx.rank, C = o.cp_c, nt = cp_tensors(o);
+  const bool gather = o.op == "all_gather";
+  const b200collDataType_t dt = o.in_dt;
+  const size_t es = b200collTypeSize(dt), W = cp_width(o), rowe = cp_row(o);
+  const size_t col[2] = {cp_packed(o) ? (size_t)o.cp_hq * o.cp_d : 0, cp_packed(o) ? ((size_t)o.cp_hq + o.cp_hkv) * o.cp_d : 0};   // K and V columns
+  void *shard = nullptr, *full = nullptr;
+  CC(b200collMemAlloc(ctx.comm, &shard, cp_shard_bytes(o)));
+  CC(b200collMemAlloc(ctx.comm, &full, cp_full_bytes(o, n)));
+  const cudaStream_t st = ctx.st;
+  long total_errors = 0;
+  if (rank == 0) {
+    printf("# b200coll_perf op=%s context nranks=%d dtype=%s chunks=%d B=1 %s: size = shard bytes per rank; rw GB/s = (shard + full bytes "
+           "this rank reads or writes) / time\n", o.op.c_str(), n, dt_name(dt), C, cp_packed(o) ? "K and V column slices of a packed QKV" : "one dense tensor");
+    if (cp_packed(o)) printf("# HQ=%d HKV=%d D=%d W=%zu\n", o.cp_hq, o.cp_hkv, o.cp_d, W);
+    else printf("# W=%zu\n", W);
+    printf("#%13s %10s %6s %8s | %10s %8s %6s\n", "size(B)", "seq_local", "type", "algo", "us", "rwGB/s", "#wrong");
+    fflush(stdout);
+  }
+  for (size_t bytes = o.min_bytes; bytes <= o.max_bytes; bytes *= o.factor) {
+    const size_t sl = bytes / (nt * W * es) / C * C;
+    if (sl == 0) continue;
+    const size_t S = sl * n, c = sl / C, shard_bytes = sl * nt * W * es, full_one = S * W * es;
+    b200collContextTensor t[2];
+    for (int i = 0; i < nt; i++) t[i] = {static_cast<char*>(shard) + col[i] * es, rowe, static_cast<char*>(full) + i * full_one, W};
+    auto gtok = [&](int r, size_t tk) { const size_t k = tk / c; return (k == 0 ? (size_t)r : (size_t)(2 * n - 1 - r)) * c + tk % c; };
+    if (gather) {
+      k_uly_fill<<<256, 256, 0, st>>>(static_cast<uint32_t*>(shard), sl * rowe * es / 4, rank);
+      RT(cudaGetLastError());
+      RT(cudaMemsetAsync(full, 0x7B, nt * full_one, st));
+    } else {
+      if (dt == b200collFloat32) k_cp_fill<float><<<256, 256, 0, st>>>(static_cast<float*>(full), nt * S * W, rank);
+      else if (dt == b200collFloat16) k_cp_fill<__half><<<256, 256, 0, st>>>(static_cast<__half*>(full), nt * S * W, rank);
+      else k_cp_fill<__nv_bfloat16><<<256, 256, 0, st>>>(static_cast<__nv_bfloat16*>(full), nt * S * W, rank);
+      RT(cudaGetLastError());
+      RT(cudaMemsetAsync(shard, 0x7B, sl * rowe * es, st));
+    }
+    auto launch = [&](int) {
+      if (gather) CC(b200collAllGatherContext(t, nt, 1, sl, C, dt, ctx.comm, st));
+      else CC(b200collReduceScatterContext(t, nt, 1, sl, C, dt, ctx.comm, st));
+    };
+    long errs = 0;
+    if (o.check) {
+      check_launch(o, ctx, launch);
+      if (gather) {                       // full[gtok(s, t)] = shard_s[t], a column slice of rank s's packed row
+        std::vector<uint8_t> host(nt * full_one);
+        RT(cudaMemcpy(host.data(), full, host.size(), cudaMemcpyDeviceToHost));
+        for (int i = 0; i < nt; i++)
+          for (int s = 0; s < n; s++)
+            for (size_t tk = 0; tk < sl; tk++) {
+              const uint8_t* got = host.data() + i * full_one + gtok(s, tk) * W * es;
+              for (size_t e = 0; e < W * es; e++) {
+                const uint8_t want = uly_byte(s, tk * rowe * es + col[i] * es + e);
+                if (got[e] != want) {
+                  if (errs < 4) fprintf(stderr, "rank %d context gather size %zu tensor %d from rank %d token %zu byte %zu: got 0x%02x want 0x%02x\n", rank, bytes, i, s, tk, e, got[e], want);
+                  errs++;
+                }
+              }
+            }
+      } else {                            // shard[t] = round_once(sum over s in rank order of full_s[gtok(rank, t)]); other columns untouched
+        std::vector<uint8_t> host(sl * rowe * es);
+        RT(cudaMemcpy(host.data(), shard, host.size(), cudaMemcpyDeviceToHost));
+        std::vector<bool> mine(rowe, false);
+        for (int i = 0; i < nt; i++) for (size_t e = 0; e < W; e++) mine[col[i] + e] = true;
+        for (size_t tk = 0; tk < sl; tk++) {
+          const size_t g = gtok(rank, tk);
+          for (size_t e = 0; e < rowe; e++) {
+            const void* row = host.data() + tk * rowe * es;
+            if (!mine[e]) {
+              bool ok = true;
+              for (size_t b = 0; b < es; b++) ok = ok && ((const uint8_t*)row)[e * es + b] == 0x7B;
+              if (!ok) { if (errs < 4) fprintf(stderr, "rank %d context reduce-scatter size %zu token %zu column %zu: written, not one of ours\n", rank, bytes, tk, e); errs++; }
+              continue;
+            }
+            const int i = (nt == 2 && e >= col[1]) ? 1 : 0;
+            float acc = 0.0f;
+            for (int s = 0; s < n; s++) acc += round_dt(cp_val(s, i * S * W + g * W + (e - col[i])), dt);
+            const uint32_t want = out_bits(acc, dt), got = got_bits(row, e, dt);
+            if (got != want) {
+              if (errs < 4) fprintf(stderr, "rank %d context reduce-scatter size %zu token %zu column %zu: got 0x%x want 0x%x\n", rank, bytes, tk, e, got, want);
+              errs++;
+            }
+          }
+        }
+      }
+    }
+    const Timing tm = timed(o, ctx, errs, launch);
+    total_errors += tm.errors;
+    if (rank == 0) {
+      printf("%14zu %10zu %6s %8s | %10.2f %8.2f %6ld\n", shard_bytes, sl, dt_name(dt), n > 1 ? "twoshot" : "copy", tm.ms * 1e3,
+             (shard_bytes + nt * full_one) / (tm.ms * 1e3) / 1e3, tm.errors);
+      fflush(stdout);
+    }
+  }
+  CC(b200collMemFree(ctx.comm, full));
+  CC(b200collMemFree(ctx.comm, shard));
+  return mode_result(ctx, total_errors);
+}
+
 static int run_rank(const Opts& o, RankCtx ctx) {
   const int n = ctx.nranks, rank = ctx.rank;
   RT(cudaSetDevice(ctx.dev));
@@ -824,6 +950,7 @@ static int run_rank(const Opts& o, RankCtx ctx) {
   }
   if (o.max_ctas > 0) CC(b200collCommSetMaxCtas(ctx.comm, o.max_ctas));
   if (o.uly_d) return run_ulysses(o, ctx);
+  if (o.cp_c) return run_context(o, ctx);
   const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt);
   const bool is_bc = o.op == "broadcast", is_rd = o.op == "reduce", is_sr = o.op == "sendrecv";
   const bool is_ar = o.op == "all_reduce" || is_bc || is_rd || is_sr;      // "whole message" geometry: count elements in, count out
@@ -1087,6 +1214,18 @@ static LauncherRank launcher_rank() {
 static bool flags_ok(const Opts& o) {
   const int n = o.nranks;
   if (o.uly_back && !o.uly_d) { fprintf(stderr, "--ulysses-back takes --ulysses HQ:HKV:D\n"); return false; }
+  if (o.cp_c) {
+    if ((o.op != "all_gather" && o.op != "reduce_scatter") || o.out_dt != o.in_dt || o.scale != 1.0f || o.q_block || o.bs_rows || o.combine_k ||
+        o.route_e || o.cq_block || o.rms_row || o.uly_d) {
+      fprintf(stderr, "--context W:C takes --op all_gather or reduce_scatter, and no --out-dtype, --scale, --quantize, --block-scale, --combine, --route,\n"
+                      "--rms-norm or --ulysses\n");
+      return false;
+    }
+    if (o.op == "reduce_scatter" && !wide(o.in_dt)) { fprintf(stderr, "--context W:C with --op reduce_scatter takes -d bfloat16|half|float\n"); return false; }
+    const size_t es = b200collTypeSize(o.in_dt);
+    if ((cp_width(o) * es) % 16 || (cp_row(o) * es) % 16) { fprintf(stderr, "--context W:C: W * sizeof(dtype) (HKV * D * sizeof(dtype)) must be a multiple of 16 bytes\n"); return false; }
+    return true;
+  }
   if (o.uly_d) {
     if (o.op != "alltoall" || o.out_dt != o.in_dt || o.scale != 1.0f || o.q_block || o.bs_rows || o.combine_k || o.route_e || o.cq_block || o.rms_row) {
       fprintf(stderr, "--ulysses HQ:HKV:D takes --op alltoall, and no --out-dtype, --scale, --quantize, --block-scale, --combine, --route or --rms-norm\n");
@@ -1158,7 +1297,8 @@ static size_t arena_bytes(const Opts& o) {
   return std::max(o.window, o.max_bytes) + std::max(o.window / is * os, o.max_bytes / is * os) + (64u << 20) + (o.bs_rows ? bs_max_scales(o) * 4 : 0) +
          q_scratch_bytes(o) + (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o) +     // --route: recv holds K rows per token
          (o.rms_row ? o.max_bytes + 4096 : 0) + rms_scale_bytes(o) +                                  // --rms-norm: the residual (and the scales of q)
-         (o.uly_d ? uly_out_bytes(o, o.nranks, o.max_bytes + 4096) : 0);                             // --ulysses: the head shards
+         (o.uly_d ? uly_out_bytes(o, o.nranks, o.max_bytes + 4096) : 0) +                            // --ulysses: the head shards
+         (o.cp_c ? cp_shard_bytes(o) + cp_full_bytes(o, o.nranks) : 0);                                // --context: the shards and full tensors
 }
 
 int main(int argc, char** argv) {
@@ -1199,6 +1339,18 @@ int main(int argc, char** argv) {
       }
     }
     else if (a == "--ulysses-back") o.uly_back = true;
+    else if (a == "--context") {
+      const char* v = next();
+      long long w = 0;
+      int c = 0, hq = 0, hkv = 0, d = 0, used = 0;
+      if (sscanf(v, "%d:%d:%d:%d%n", &hq, &hkv, &d, &c, &used) == 4 && !v[used] && hq > 0 && hkv > 0 && d > 0 && (c == 1 || c == 2)) {
+        o.cp_hq = hq; o.cp_hkv = hkv; o.cp_d = d; o.cp_c = c;
+      } else if (sscanf(v, "%lld:%d%n", &w, &c, &used) == 2 && !v[used] && w > 0 && (c == 1 || c == 2)) {
+        o.cp_w = (size_t)w; o.cp_c = c;
+      } else {
+        fprintf(stderr, "--context W:C or HQ:HKV:D:C: positive integers, C 1 or 2\n"); return 1;
+      }
+    }
     else if (a == "--combine") { o.combine_k = atoi(next()); if (o.combine_k < 1) { fprintf(stderr, "--combine K: K >= 1\n"); return 1; } }
     else if (a == "--route") {
       if (sscanf(next(), "%d:%d", &o.route_e, &o.route_k) != 2 || o.route_e < 1 || o.route_e > 1024 || o.route_k < 1) { fprintf(stderr, "--route E:K: 1 <= E <= 1024, K >= 1\n"); return 1; }
@@ -1272,6 +1424,12 @@ int main(int argc, char** argv) {
            "                            every rank's packed QKV [S_l, (HQ + 2 HKV) * D] (q, k and v column slices) to dense head shards in one\n"
            "                            call; size = source bytes per rank, rounded down to whole tokens; -c 1 checks every output byte\n"
            "  --ulysses-back            with --ulysses HQ:HKV:D: heads -> sequence, the [S, HQ / N, D] attention output back to [S_l, HQ, D]\n"
+           "  --context W:C | HQ:HKV:D:C   --op all_gather or reduce_scatter (bfloat16|half|float; the gather also e4m3|e5m2): context parallelism,\n"
+           "                            B = 1, C = 1 contiguous or 2 load-balanced (causal) sharding. all_gather: K and V, the column slices of a\n"
+           "                            packed QKV [S_l, (HQ + 2 HKV) * D] (or one dense [S_l, W]), gathered into dense [S, HKV * D] in token\n"
+           "                            order in one call; reduce_scatter: the gradient, [S, HKV * D] summed over the ranks into the K and V\n"
+           "                            slices of a packed dQKV; size = shard bytes per rank, rounded down to whole tokens; -c 1 checks every\n"
+           "                            output byte (the reduce-scatter against the fp32 sum in rank order)\n"
            "  --selfcheck              report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;
     }

@@ -50,6 +50,10 @@ class UlyssesTensor(C.Structure):
     _fields_ = [("seq", C.c_void_p), ("row_stride", C.c_size_t), ("head", C.c_void_p), ("heads", C.c_int)]
 
 
+class ContextTensor(C.Structure):
+    _fields_ = [("shard", C.c_void_p), ("row_stride", C.c_size_t), ("full", C.c_void_p), ("width", C.c_size_t)]
+
+
 class Config(C.Structure):
     _fields_ = [("arena_bytes", C.c_size_t), ("enable_nvls", C.c_int), ("max_ctas", C.c_int), ("timeout_ms", C.c_int), ("debug", C.c_int)]
 
@@ -157,6 +161,8 @@ def load() -> C.CDLL:
     L.b200collReduceScatterRmsNormQuantized.argtypes = [vp, vp, vp, vp, C.POINTER(C.c_float), sz, sz, C.c_float, ci, ci, ci, ci, vp, vp]
     L.b200collAllToAllSeqToHeads.argtypes = [C.POINTER(UlyssesTensor), ci, sz, sz, sz, ci, vp, vp]
     L.b200collAllToAllHeadsToSeq.argtypes = [C.POINTER(UlyssesTensor), ci, sz, sz, sz, ci, vp, vp]
+    L.b200collAllGatherContext.argtypes = [C.POINTER(ContextTensor), ci, sz, sz, ci, ci, vp, vp]
+    L.b200collReduceScatterContext.argtypes = [C.POINTER(ContextTensor), ci, sz, sz, ci, ci, vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -679,6 +685,103 @@ def check_all_to_all_heads_to_seq(nranks: int, ys, outs) -> tuple[int, int, int,
     return _check_ulysses(nranks, outs, ys, False)
 
 
+def _shard_row_stride(name: str, t) -> int:
+    """The row stride (elements) of a [B, S_l, ...] view whose token rows are uniformly strided and hold their elements contiguously."""
+    B, S_l = t.shape[:2]
+    want = 1
+    for size, st in reversed(list(zip(t.shape[2:], t.stride()[2:]))):
+        if size > 1 and st != want:
+            raise ValueError(f"{name}: each token row must hold its elements contiguously, got shape {list(t.shape)} and strides {t.stride()}")
+        want *= size
+    rs = t.stride(1) if S_l > 1 or B == 1 else t.stride(0)
+    if S_l > 1 and B > 1 and t.stride(0) != S_l * rs:
+        raise ValueError(f"{name}: token rows must be uniformly strided (stride(0) == seq_local * stride(1)), got strides {t.stride()}")
+    return rs if B * S_l > 1 else want          # one token row: its stride is never used
+
+
+def _check_context(nranks: int, shards, fulls, chunks: int, gather: bool) -> tuple[int, int, list[tuple[int, int]]]:
+    import torch
+    what = "all_gather_context" if gather else "reduce_scatter_context"
+    shards, fulls = list(shards), list(fulls)
+    if not 1 <= len(shards) <= 3 or len(fulls) != len(shards):
+        raise ValueError(f"{what}: 1 to 3 tensors and one full tensor per shard, got {len(shards)} shards and {len(fulls)} fulls")
+    dt = shards[0].dtype
+    allowed = (torch.bfloat16, torch.float16, torch.float32) + ((torch.float8_e4m3fn, torch.float8_e5m2) if gather else ())
+    if dt not in allowed:
+        raise ValueError(f"{what}: dtype must be one of {', '.join(str(d).split('.')[-1] for d in allowed)}, got {dt}")
+    if chunks not in (1, 2):
+        raise ValueError(f"{what}: chunks must be 1 or 2, got {chunks}")
+    if any(t.dim() < 3 for t in shards + fulls):
+        raise ValueError(f"{what}: every tensor must be [B, S_l, ...] (shards) or [B, N * S_l, ...] (fulls), at least 3-D")
+    B, S_l = shards[0].shape[:2]
+    if chunks == 2 and S_l % 2:
+        raise ValueError(f"{what}: chunks = 2 needs an even seq_local, got {S_l}")
+    rows = B * S_l
+    if rows > _I31:
+        raise ValueError(f"{what}: batch * seq_local must be below 2^31, got {rows}")
+    es = shards[0].element_size()
+    per, srcs, dsts, moved = [], [], [], 0
+    for i, (x, f) in enumerate(zip(shards, fulls)):
+        if x.dtype != dt or f.dtype != dt:
+            raise ValueError(f"{what}: tensor {i}: every tensor must have dtype {dt}, got {x.dtype} and {f.dtype}")
+        if tuple(x.shape[:2]) != (B, S_l):
+            raise ValueError(f"{what}: shards[{i}] must be [{B}, {S_l}, ...] like the first, got {list(x.shape)}")
+        want = (B, nranks * S_l, *x.shape[2:])
+        if tuple(f.shape) != want or not f.is_contiguous():
+            raise ValueError(f"{what}: fulls[{i}] must be a contiguous {list(want)} tensor, got {list(f.shape)}")
+        W = _prod(x.shape[2:])
+        if W == 0 or (W * es) % 16:
+            raise ValueError(f"{what}: tensor {i}: width * sizeof(dtype) must be a positive multiple of 16 bytes, got {W} x {es}")
+        rs = _shard_row_stride(f"shards[{i}]", x)
+        if rs < W or (rs * es) % 16:
+            raise ValueError(f"{what}: shards[{i}]: the row stride ({rs}) must be at least the width ({W}) and a multiple of 16 bytes")
+        if rows and (x.data_ptr() % 16 or f.data_ptr() % 16):
+            raise ValueError(f"{what}: tensor {i}: every pointer must be 16-byte aligned")
+        wv = W * es // 16
+        if rows and ((rows - 1) * rs * es // 16 + wv > _I31 or nranks * rows * wv > _I31):
+            raise ValueError(f"{what}: tensor {i}: more than 2^31 - 1 16-byte vectors per rank")
+        moved += rows * wv
+        shard_span = (x.data_ptr(), rows, rs * es, W * es)           # (address, rows, stride, width) in bytes
+        full_span = (f.data_ptr(), 1, f.numel() * es, f.numel() * es)
+        srcs.append(shard_span if gather else full_span)
+        dsts.append(full_span if gather else shard_span)
+        per.append((rs, W))
+    if moved > _I31:
+        raise ValueError(f"{what}: more than 2^31 - 1 16-byte vectors moved per rank")
+    for i, d in enumerate(dsts):
+        for j, s in enumerate(srcs):
+            if _spans_overlap(d, s):
+                raise ValueError(f"{what}: output {i} overlaps source {j}")
+        for j in range(i + 1, len(dsts)):
+            if _spans_overlap(d, dsts[j]):
+                raise ValueError(f"{what}: outputs {i} and {j} overlap")
+    return B, S_l, per
+
+
+def _prod(shape) -> int:
+    n = 1
+    for d in shape:
+        n *= d
+    return n
+
+
+def check_all_gather_context(nranks: int, shards, fulls, chunks: int) -> tuple[int, int, list[tuple[int, int]]]:
+    """The rules of Comm.all_gather_context, checked on the tensors' metadata (no device, no communicator): raises ValueError, returns
+    (batch, seq_local, [(row_stride, width)] per tensor). shards: 1 to 3 [B, S_l, ...] views of one dtype (bfloat16, float16, float32,
+    float8_e4m3fn or float8_e5m2) whose token rows are uniformly strided and hold their W elements contiguously, such as the K and V
+    column slices of a packed QKV tensor; fulls: contiguous [B, N * S_l, ...] with the shards' trailing shape. chunks 1 or 2 (2 needs an
+    even S_l); W * sizeof(dtype) and every row stride a multiple of 16 bytes, every pointer 16-byte aligned, B * S_l below 2^31, at most
+    2^31 - 1 16-byte vectors per rank; no output may overlap a source or another output."""
+    return _check_context(nranks, shards, fulls, chunks, True)
+
+
+def check_reduce_scatter_context(nranks: int, fulls, shards, chunks: int) -> tuple[int, int, list[tuple[int, int]]]:
+    """The rules of Comm.reduce_scatter_context, checked on the tensors' metadata: raises ValueError, returns as
+    check_all_gather_context. fulls: 1 to 3 contiguous [B, N * S_l, ...] tensors of bfloat16, float16 or float32; shards: the [B, S_l,
+    ...] outputs, row-strided views allowed (the K and V column slices of a packed dQKV tensor). Everything else as the gather."""
+    return _check_context(nranks, shards, fulls, chunks, False)
+
+
 def _check_routed(nranks: int, x, topk_idx, num_experts: int, recv, expert_counts, route, dropped, fp8=None) -> None:
     """The rules of both device-routed dispatches; fp8 is None (check_expert_dispatch) or (recv_scales, block), which adds the FP8
     call's rules, as routed_prepare in coll/src/dispatch.cu takes a RoutedQuant."""
@@ -1195,6 +1298,43 @@ class Comm:
         B, S_l, D, per = check_all_to_all_heads_to_seq(self.nranks, ys, outs)
         self._ulysses(load().b200collAllToAllHeadsToSeq, "AllToAllHeadsToSeq", outs, ys, per, B, S_l, D, stream)
         return outs
+
+    def _context(self, fn, name, shards, fulls, per, B, S_l, chunks, stream):
+        arr = (ContextTensor * len(shards))(*[ContextTensor(x.data_ptr(), rs, f.data_ptr(), w) for x, f, (rs, w) in zip(shards, fulls, per)])
+        _check(fn(arr, len(shards), B, S_l, chunks, torch_dtype_code(shards[0].dtype), self._h, self._stream(stream)), name)
+
+    def all_gather_context(self, shards, fulls=None, *, chunks: int, stream=None):
+        """Context-parallel all-gather before attention, one kernel for up to three tensors (K and V): each [B, S_l, ...] sequence shard
+        in shards (views with uniformly strided token rows, e.g. the K and V column slices of a packed QKV projection output) is gathered
+        from every rank into the dense [B, N * S_l, ...] full tensor in fulls, in token order. chunks is the sharding: 1 contiguous (rank
+        r holds tokens [r * S_l, (r + 1) * S_l)), 2 load-balanced for causal attention (the sequence cut into 2N chunks, rank r holding
+        chunks r and 2N - 1 - r). A bit copy, as coll/include/b200coll.h's b200collAllGatherContext states. Returns fulls. With more than
+        one rank fulls must be given, as arena tensors (`empty()`) at the same offsets on every rank; with one rank None allocates them."""
+        shards = list(shards)
+        if fulls is None:
+            if self.nranks > 1:
+                raise ValueError("all_gather_context with more than one rank needs fulls: arena tensors (Comm.empty) of [B, N * S_l, ...], "
+                                 "the same on every rank")
+            fulls = [x.new_empty(x.shape) for x in shards]
+        fulls = list(fulls)
+        B, S_l, per = check_all_gather_context(self.nranks, shards, fulls, chunks)
+        self._context(load().b200collAllGatherContext, "AllGatherContext", shards, fulls, per, B, S_l, chunks, stream)
+        return fulls
+
+    def reduce_scatter_context(self, fulls, shards=None, *, chunks: int, stream=None):
+        """The gradient of all_gather_context, after attention's backward: every rank's [B, N * S_l, ...] full tensors in fulls (dK and
+        dV over the whole sequence, partial sums over the rank's own queries) are summed in fp32 in rank order, rounded once, and this
+        rank's tokens (the layout chunks names) stored into the [B, S_l, ...] shards, which may be row-strided views such as the K and V
+        column slices of a packed dQKV tensor. bfloat16, float16 or float32; bit for bit as b200collReduceScatterContext states. Returns
+        shards. With more than one rank fulls must be arena tensors at the same offsets on every rank; shards may be any device tensors,
+        and None allocates them."""
+        fulls = list(fulls)
+        if shards is None:
+            shards = [f.new_empty((f.shape[0], f.shape[1] // self.nranks, *f.shape[2:])) for f in fulls]
+        shards = list(shards)
+        B, S_l, per = check_reduce_scatter_context(self.nranks, fulls, shards, chunks)
+        self._context(load().b200collReduceScatterContext, "ReduceScatterContext", shards, fulls, per, B, S_l, chunks, stream)
+        return shards
 
     def _rows(self, xs):
         """A host list of nranks row counts or offsets, as the library's int64[nranks]."""
