@@ -1,7 +1,7 @@
 """Reference for the context-parallel all-gather and reduce-scatter (b200collAllGatherContext / ReduceScatterContext): the gather built
 from stacking and index_select on byte views, so every dtype (FP8 included) moves bit for bit; the reduce-scatter from
 coll_fp_reference.ref_sum in rank order plus cast. One tensor at a time; a rank's shard is [B, S_l, ...] and a full tensor
-[B, N * S_l, ...]."""
+[B, N * S_l, ...]. all_gather and reduce_scatter run on the device their inputs are on."""
 import numpy as np
 import torch
 
@@ -16,15 +16,22 @@ def gtok(n, chunks, S_l, r, t):
     return (r if k == 0 else 2 * n - 1 - r) * c + u
 
 
-def token_index(n, chunks, S_l):
+def token_index(n, chunks, S_l, device="cpu"):
     """idx[g] = s * S_l + t for the (rank s, local token t) that holds global token g: the gather's index over the stacked shards."""
     c = S_l // chunks
-    idx = torch.empty(n * S_l, dtype=torch.int64)
+    idx = torch.empty(n * S_l, dtype=torch.int64, device=device)
     for s in range(n):
         for k in range(chunks):
             g0 = (s if k == 0 else 2 * n - 1 - s) * c
-            idx[g0:g0 + c] = s * S_l + k * c + torch.arange(c)
+            idx[g0:g0 + c] = s * S_l + k * c + torch.arange(c, device=device)
     return idx
+
+
+def local_index(n, chunks, S_l, r, device="cpu"):
+    """g[t] = gtok(r, t) for every local token t of rank r: the reduce-scatter's index into the full tensors."""
+    c = S_l // chunks
+    t = torch.arange(S_l, device=device)
+    return torch.where(t < c, r * c + t, (2 * n - 1 - r) * c + t - c)
 
 
 def _bytes(t):
@@ -38,7 +45,7 @@ def all_gather(shards, chunks):
     n = len(shards)
     x = torch.stack([_bytes(t) for t in shards], dim=1)                     # [B, N(s), S_l, Wb]
     B, _, S_l, Wb = x.shape
-    return x.reshape(B, n * S_l, Wb).index_select(1, token_index(n, chunks, S_l))
+    return x.reshape(B, n * S_l, Wb).index_select(1, token_index(n, chunks, S_l, x.device))
 
 
 def reduce_scatter(fulls, chunks):
@@ -51,7 +58,7 @@ def reduce_scatter(fulls, chunks):
         return [fulls[0].clone()]
     out = []
     for r in range(n):
-        g = torch.tensor([gtok(n, chunks, S_l, r, t) for t in range(S_l)], dtype=torch.int64)
+        g = local_index(n, chunks, S_l, r, fulls[0].device)
         xs = [f.index_select(1, g).reshape(-1) for f in fulls]
         out.append(R.cast(R.ref_sum(xs, list(range(n))), fulls[0].dtype).view(B, S_l, *fulls[0].shape[2:]))
     return out

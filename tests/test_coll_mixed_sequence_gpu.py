@@ -7,7 +7,9 @@ Every family keeps state on the communicator that the next call of any family in
 by family and size, so rows one call leaves unused keep older epochs), the Lamport sequence and the spans the next Lamport call clears,
 the two staging halves, the FP8 quantisation scratch (grown mid-stream), and the route-count and send/recv mailboxes. Each call here is
 a *kind*: one public `Comm` call with its inputs, its own output buffers and its check against the order-exact reference of its family.
-The three schedules:
+The sequence-parallel kinds (the Ulysses all-to-all both ways, the context-parallel gather and reduce-scatter) share the barrier epoch
+with every two-shot, block-scaled, RMSNorm, dispatch and combine kernel; each draws its head config (replicated K and V included),
+packed or dense layout, chunks, B and S_l from the schedule's rng. The three schedules:
 
   a. every ordered pair of kinds adjacent once (an Eulerian circuit of the complete directed graph with loops), at n = 3 and 4;
   b. seeded random schedules at n = 2, 3, 4 and 8 with launch-shape changes, one rank held back by a delay kernel, and inputs rewritten
@@ -28,12 +30,14 @@ import torch
 
 from container_engine_accelerators_b200.ops.coll import AVG, MAX, MIN, PROD, QUANT_BLOCKS, SUM, B200CollError
 from tests import coll_combine_reference as CR
+from tests import coll_context_reference as cref
 from tests import coll_fp_reference as R
 from tests import coll_quant_reference as QR
 from tests import coll_rmsnorm_quant_reference as RNQ
 from tests import coll_rmsnorm_reference as RN
 from tests import coll_routed_reference as RR
 from tests import coll_rs_rmsnorm_reference as RS
+from tests import coll_ulysses_reference as uref
 from tests.coll_gpu_harness import DTYPES, Group, Plan, coll_mod, poison, torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
@@ -888,6 +892,173 @@ class SendRecv(Call):
             same(self.outs[r], self.xs[(r - 1) % self.n], f"rank {r}", nan_payloads=True)
 
 
+def random_bytes(shape, dt, seed):
+    """Host random bytes (NaN payloads, -0 and inf in every float type) viewed as a dt tensor of `shape`."""
+    nb = int(np.prod(shape)) * R.esize(dt)
+    return torch.randint(0, 256, (nb,), dtype=torch.uint8, generator=torch.Generator().manual_seed(seed)).view(dt).view(shape)
+
+
+def load_views(bufs, xs):
+    """Host tensors into device views of the same shape (column slices of a packed buffer included)."""
+    for b, x in zip(bufs, xs):
+        b.copy_(x.to(b.device))
+
+
+def same_bytes(got, want, what):
+    g, w = got.contiguous().view(torch.uint8).reshape(-1).cpu(), want.contiguous().view(torch.uint8).reshape(-1).cpu()
+    assert g.numel() == w.numel(), f"{what}: {g.numel()} bytes vs {w.numel()}"
+    bad = (g != w).nonzero()
+    assert bad.numel() == 0, f"{what}: {bad.numel()} bytes differ, first at byte {int(bad[0])}"
+
+
+def head_choices(n):
+    """(name, Hq, Hkv) that n ranks allow: MHA, GQA, GQA with K and V replicated (Hkv a divisor of n below it) and MQA."""
+    cfgs = [("mha", 2 * n, 2 * n), ("gqa", 4 * n, n)]
+    small = [h for h in range(2, n) if n % h == 0]
+    if small:
+        cfgs.append(("gqa-replicated", 4 * n, small[-1]))
+    cfgs.append(("mqa", 2 * n, 1))
+    return cfgs
+
+
+class Ulysses(Call):
+    """all_to_all_seq_to_heads of q, k and v (column slices of one packed QKV or dense tensors; K and V replicated where the head config
+    has fewer KV heads than ranks), or all_to_all_heads_to_seq of q alone or of q, k and v (dense head shards into column slices of a
+    packed buffer or dense tensors). Head-side outputs and sequence-side outputs live in the arena."""
+
+    def __init__(self, g, rng, s2h):
+        super().__init__(g, rng)
+        n, self.s2h = self.n, s2h
+        self.kind = "all_to_all_seq_to_heads" if s2h else "all_to_all_heads_to_seq"
+        name, hq, hkv = pick(rng, head_choices(n) if s2h else [h for h in head_choices(n) if h[2] % n == 0])
+        heads = (hq, hkv, hkv) if s2h or rng.random() < 0.5 else (hq,)
+        self.p = dict(dt=pick(rng, WIDE + ("float8_e4m3fn",)), heads=f"{name}{heads}", D=pick(rng, [16, 64, 80]), B=pick(rng, [1, 2, 3]),
+                      S_l=pick(rng, [1, 5, 8, 33]), layout=pick(rng, ["packed", "dense"]))
+        self.heads, self.dt = heads, DTYPES[self.p["dt"]]
+        B, S_l, D, dt = self.p["B"], self.p["S_l"], self.p["D"], self.dt
+        self.cols = np.cumsum([0] + [h * D for h in heads]).tolist()
+        seq_bufs = self.bufs("plain" if s2h else "arena", B * S_l * self.cols[-1], dt) if self.p["layout"] == "packed" else None
+        self.seq_whole = [] if seq_bufs is None else [b.view(B * S_l, self.cols[-1]) for b in seq_bufs]
+        self.seq = []
+        for r in range(n):
+            if seq_bufs is not None:
+                self.seq.append([self.seq_whole[r][:, self.cols[i]:self.cols[i + 1]].view(B, S_l, h, D) for i, h in enumerate(heads)])
+            else:
+                self.seq.append([])
+        if seq_bufs is None:
+            for h in heads:
+                for r, t in enumerate(self.bufs("plain" if s2h else "arena", B * S_l * h * D, dt)):
+                    self.seq[r].append(t.view(B, S_l, h, D))
+        self.head = [[] for _ in range(n)]
+        for h in heads:
+            hl = h // n if h % n == 0 else 1
+            for r, t in enumerate(self.bufs("arena" if s2h else "plain", B * n * S_l * hl * D, dt)):
+                self.head[r].append(t.view(B, n * S_l, hl, D))
+        src = self.seq if s2h else self.head
+        self.inputs = [self.seq_whole[r:r + 1] if s2h and self.seq_whole else list(src[r]) for r in range(n)]
+
+    def fill(self, seed):
+        n, B, S_l, D = self.n, self.p["B"], self.p["S_l"], self.p["D"]
+        if self.s2h:
+            self.hx = [[random_bytes((B, S_l, h, D), self.dt, seed + 31 * r + i) for i, h in enumerate(self.heads)] for r in range(n)]
+            load_views([t for row in self.seq for t in row], [t for row in self.hx for t in row])
+            poison([t for row in self.head for t in row])
+        else:
+            self.hy = [[random_bytes(tuple(t.shape), self.dt, seed + 31 * r + i) for i, t in enumerate(self.head[r])] for r in range(n)]
+            load_views([t for row in self.head for t in row], [t for row in self.hy for t in row])
+            poison(self.seq_whole if self.seq_whole else [t for row in self.seq for t in row])
+
+    def enqueue(self, r, c, st):
+        if self.s2h:
+            c.all_to_all_seq_to_heads(self.seq[r], self.head[r], stream=st)
+        else:
+            c.all_to_all_heads_to_seq(self.head[r], self.seq[r], stream=st)
+
+    def check(self):
+        n = self.n
+        for i in range(len(self.heads)):
+            if self.s2h:
+                want = uref.seq_to_heads([self.hx[s][i] for s in range(n)])
+                for r in range(n):
+                    same_bytes(self.head[r][i], want[r], f"tensor {i} rank {r}")
+            else:
+                want = uref.heads_to_seq([self.hy[s][i] for s in range(n)])
+                for r in range(n):
+                    same_bytes(self.seq[r][i], want[r], f"tensor {i} rank {r}")
+
+
+class Context(Call):
+    """all_gather_context (bf16, fp16, fp32, e4m3 or e5m2) or reduce_scatter_context (bf16, fp16 or fp32) of one tensor, K and V as column
+    slices of a packed QKV (dQKV, whose Q columns must stay poisoned), or an MLA-like pair of dense tensors; contiguous or load-balanced
+    chunks. Full tensors live in the arena, and so do the reduce-scatter's shards."""
+
+    def __init__(self, g, rng, gather):
+        super().__init__(g, rng)
+        n, self.gather = self.n, gather
+        self.kind = "all_gather_context" if gather else "reduce_scatter_context"
+        dt = pick(rng, WIDE + FP8 if gather else WIDE)
+        e = 16 // esize(dt)
+        chunks = pick(rng, [1, 2])
+        layout = pick(rng, ["kv-packed", "mla-dense", "one"])
+        widths = {"kv-packed": (pick(rng, [2, 4]) * e,) * 2, "mla-dense": (8 * e, e), "one": (pick(rng, [1, 3, 5]) * e,)}[layout]
+        self.p = dict(dt=dt, layout=layout, widths=widths, chunks=chunks, B=pick(rng, [1, 2, 3]), S_l=pick(rng, [2, 6, 12] if chunks == 2 else [1, 5, 7, 12]))
+        self.dt, self.widths = DTYPES[dt], widths
+        B, S_l, S = self.p["B"], self.p["S_l"], n * self.p["S_l"]
+        self.q_cols = 2 * widths[0] if layout == "kv-packed" else None
+        self.full = [[] for _ in range(n)]
+        for w in widths:
+            for r, t in enumerate(self.arena(B * S * w, self.dt)):
+                self.full[r].append(t.view(B, S, w))
+        where = "plain" if gather else "arena"
+        self.whole, self.shard = [], [[] for _ in range(n)]
+        if self.q_cols is not None:
+            row = self.q_cols + sum(widths)
+            self.whole = [b.view(B * S_l, row) for b in self.bufs(where, B * S_l * row, self.dt)]
+            for r, b in enumerate(self.whole):
+                c0 = self.q_cols
+                for w in widths:
+                    self.shard[r].append(b[:, c0:c0 + w].view(B, S_l, w))
+                    c0 += w
+        else:
+            for w in widths:
+                for r, t in enumerate(self.bufs(where, B * S_l * w, self.dt)):
+                    self.shard[r].append(t.view(B, S_l, w))
+        self.inputs = [(self.whole[r:r + 1] if self.whole else list(self.shard[r])) if gather else list(self.full[r]) for r in range(n)]
+
+    def fill(self, seed):
+        n, B, S_l = self.n, self.p["B"], self.p["S_l"]
+        if self.gather:
+            self.hx = [[random_bytes((B, S_l, w), self.dt, seed + 31 * r + i) for i, w in enumerate(self.widths)] for r in range(n)]
+            load_views([t for row in self.shard for t in row], [t for row in self.hx for t in row])
+            poison([t for row in self.full for t in row])
+        else:
+            per = [R.gen_inputs(n, B * n * S_l * w, self.dt, seed + i, device="cpu") for i, w in enumerate(self.widths)]
+            self.hf = [[per[i][r].view(B, n * S_l, w) for i, w in enumerate(self.widths)] for r in range(n)]
+            load_views([t for row in self.full for t in row], [t for row in self.hf for t in row])
+            poison(self.whole if self.whole else [t for row in self.shard for t in row])
+
+    def enqueue(self, r, c, st):
+        if self.gather:
+            c.all_gather_context(self.shard[r], self.full[r], chunks=self.p["chunks"], stream=st)
+        else:
+            c.reduce_scatter_context(self.full[r], self.shard[r], chunks=self.p["chunks"], stream=st)
+
+    def check(self):
+        n, chunks = self.n, self.p["chunks"]
+        for i in range(len(self.widths)):
+            if self.gather:
+                want = cref.all_gather([self.hx[s][i] for s in range(n)], chunks)
+                for r in range(n):
+                    same_bytes(self.full[r][i], want, f"tensor {i} rank {r}")
+            else:
+                want = cref.reduce_scatter([self.hf[s][i] for s in range(n)], chunks)
+                for r in range(n):
+                    same(self.shard[r][i].contiguous(), want[r], f"tensor {i} rank {r}")
+        if not self.gather and self.whole:
+            for r in range(n):
+                assert bool((self.whole[r][:, :self.q_cols].view(torch.uint8) == 0x7B).all()), f"rank {r}'s Q columns of dQKV were written"
+
+
 class Barrier(Call):
     kind = "barrier"
 
@@ -932,6 +1103,10 @@ KINDS = {
     "expert_combine_quantized": lambda g, rng: Expert(g, rng, True, True),
     "send_recv_ring": SendRecv,
     "barrier": Barrier,
+    "all_to_all_seq_to_heads": lambda g, rng: Ulysses(g, rng, True),
+    "all_to_all_heads_to_seq": lambda g, rng: Ulysses(g, rng, False),
+    "all_gather_context": lambda g, rng: Context(g, rng, True),
+    "reduce_scatter_context": lambda g, rng: Context(g, rng, False),
 }
 KIND_NAMES = list(KINDS)
 MULTI_OP = ("all_reduce_host", "all_reduce_staged_big")           # several dependent operations per rank in one call
