@@ -78,6 +78,7 @@ typedef enum {
  *                                                           outside the arena) runs this per staging chunk, slices taken from the chunk.
  *   P2P reduce-scatter (16- and 32-bit inputs)              receiving rank r sums r, r+1, .., N-1, 0, .., r-1
  *   context-parallel reduce-scatter                         ranks 0 .. N-1
+ *   FSDP shard reduce-scatter (ReduceScatterShards)         ranks 0 .. N-1, then * scale, then + the old shard
  *   NVLS (multimem.ld_reduce)                               the switch's order: within an ulp of the exact sum, not bit-reproducible
  * Rounding to FP8 saturates to the finite range (+-inf becomes +-max, NaN stays NaN); fp16 overflows to inf.
  * All-gather, broadcast and all-to-all(v) apply the same epilogue per element: round((0 + x) * scale) (e4m3 in, bf16 out, scale =
@@ -639,6 +640,56 @@ b200collResult_t b200collAllGatherContext(const b200collContextTensor* tensors, 
                                           b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
 b200collResult_t b200collReduceScatterContext(const b200collContextTensor* tensors, int ntensors, size_t batch, size_t seq_local, int chunks,
                                               b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
+
+/* FSDP / ZeRO-3, dim-0 sharding (torch.distributed.fsdp.fully_shard's Shard(0)): before forward each rank gathers a unit's parameters
+ * from their shards, casting them on the owning rank (AllGatherShards); after backward the unit's gradients are reduce-scattered back
+ * to the shards, summed in fp32, scaled and optionally added to the gradient already there (ReduceScatterShards). One kernel per call
+ * for 1 to 64 tensors (one unit: a Llama block has 9) sharing one pair of dtypes. N ranks, this rank r. Tensor i has rows d_i (its
+ * unsharded dim 0), width W_i (the product of its other dims) and shard_rows p_i, the rows per rank, with N * p_i >= d_i (FSDP2 uses
+ * p_i = ceil(d_i / N); a caller may round it up to meet the alignment rule below). Rank s owns rows [s * p_i, s * p_i + n_s) with
+ *   n_s = clamp(d_i - s * p_i, 0, p_i)
+ * (a 3-row tensor on 8 ranks leaves ranks 3 .. 7 with none). Two sides:
+ *   shard: this rank's rows, dense [>= n_r, W_i]; rows n_r .. p_i - 1 (padding) are never read or written.
+ *   full:  the unsharded tensor, dense [d_i, W_i], no padding.
+ * AllGatherShards: on every rank, full[s * p_i + j, :] = cast(shard of rank s [j, :]) for every rank s and j < n_s. Pairs (shard ->
+ * full): one dtype in and out (bf16, fp16, fp32, e4m3 or e5m2), a bit copy (NaN payloads, -0 and inf survive); or fp32 -> bf16 or
+ * fp16, IEEE round to nearest even with overflow to inf, as Tensor.to (NaN stays NaN, its payload not kept). The cast runs on the
+ * owning rank, before the push, so the narrow type is what crosses NVLink.
+ * ReduceScatterShards: on rank r, for j < n_r and e = (r * p_i + j, :), every step in fp32 with no FMA contraction:
+ *   t = ((+0 + full_0[e]) + full_1[e]) + .. + full_{N-1}[e]     (full_s rank s's full; rank order, the order table above)
+ *   t = t * scale
+ *   t = (float)shard[j, :] + t                                 if accumulate
+ *   shard[j, :] = round_once(t)                                 to nearest even; fp16 overflows to inf
+ * Pairs (full -> shard): bf16 -> bf16, fp16 -> fp16, fp32 -> fp32, bf16 -> fp32, fp16 -> fp32. With one rank, one dtype, scale == 1
+ * and accumulate == 0 it is a bit copy, as b200collReduceScatter is; in every other case the formula holds with N = 1.
+ * Arguments (InvalidArgument, message in b200collGetLastError, nothing launched): ntensors not in [1, 64]; a dtype pair outside the
+ * lists above; d_i, W_i or p_i zero; N * p_i < d_i; p_i * W_i or d_i * W_i not a multiple of 16 bytes in either dtype; a pointer not
+ * 16-byte aligned, full null, or shard null when n_r > 0; more than 2^31 - 1 16-byte vectors in a side of a tensor or in sum p_i * W_i;
+ * an output (full for the gather, this rank's n_r rows of shard for the reduce-scatter) overlapping any source or another output.
+ * Placement: with more than one rank every full must be arena memory at the same offset on every rank, else InvalidUsage (the gather
+ * pushes into it, the reduce-scatter pulls from it; there is no staging path: gradients reach the arena through the communicator's
+ * memory pool); shard may be any device buffer, as only its own rank touches it. With one rank any device buffers. Shapes, dtypes,
+ * scale and accumulate must be equal on every rank; B200COLL_CHECK=1 cross-checks the direction, ntensors, both dtypes, the bits of
+ * scale, accumulate, and every d_i, W_i, p_i and full offset on multi-process communicators and turns a disagreement into InvalidUsage.
+ * A poisoned communicator gives RemoteError. The kernel starts with a barrier (no rank stores into or reads a full that an earlier
+ * operation on a peer's stream still uses) and ends with a releasing one, so the outputs may be read and the sources overwritten by the
+ * next operation on the stream. Every rank launches the same grid, sized from sum p_i * W_i, so a rank with no rows still takes part.
+ * The host reads no device data, so both calls can be captured in a CUDA graph. One rank: a local copy or reduction, no barrier.
+ * b200collStats count an allgather (AllGatherShards) or a reducescatter (ReduceScatterShards) of this rank's rows in the full dtype
+ * (n_r * W_i * sizeof(full dtype) summed over the tensors) under twoshot (copy with one rank), one kernel launch. The tuner and
+ * b200collCommSetAlgo do not apply. */
+typedef struct {
+  void* shard;          /* this rank's rows, dense [>= n_r, W]: source of the gather, destination of the reduce-scatter */
+  void* full;           /* dense [rows, W]: destination of the gather, source of the reduce-scatter */
+  size_t rows;          /* d, the unsharded dim 0 */
+  size_t width;         /* W, the product of the other dims */
+  size_t shard_rows;    /* p, rows per rank (N * p >= d) */
+} b200collShardTensor;
+b200collResult_t b200collAllGatherShards(const b200collShardTensor* tensors, int ntensors, b200collDataType_t shard_dtype,
+                                         b200collDataType_t full_dtype, b200collComm_t comm, b200collStream_t stream);
+b200collResult_t b200collReduceScatterShards(const b200collShardTensor* tensors, int ntensors, b200collDataType_t full_dtype,
+                                             b200collDataType_t shard_dtype, float scale, int accumulate, b200collComm_t comm,
+                                             b200collStream_t stream);
 
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.

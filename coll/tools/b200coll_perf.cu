@@ -70,6 +70,8 @@ struct Opts {
   int cp_c = 0;                             // --context W:C or HQ:HKV:D:C: the context-parallel gather / reduce-scatter, C chunks per rank (0 = off)
   int cp_hq = 0, cp_hkv = 0, cp_d = 0;      // packed QKV (K and V column slices), or 0 with cp_w
   size_t cp_w = 0;                          // one dense tensor of cp_w elements per token
+  int fs_h = 0, fs_f = 0, fs_kv = 0;        // --fsdp H:F[:KV]: the FSDP shard gather / reduce-scatter of one Llama block (0 = off)
+  bool accumulate = false;                  // --accumulate: the reduce-scatter adds into the old shard
 };
 
 // Block-scaled mode: each rank's send buffer is a [rows, row_len] FP8 matrix with one fp32 scale per bs_rows x bs_cols block. Scales are
@@ -939,6 +941,144 @@ static int run_context(const Opts& o, RankCtx& ctx) {
   return mode_result(ctx, total_errors);
 }
 
+// FSDP mode (--fsdp H:F[:KV]). One Llama block's nine tensors, in this order: q [H, H], k [KV, H], v [KV, H], o [H, H], gate [F, H],
+// up [F, H], down [H, F], and the attention and MLP norm weights [H] (KV = H by default). Tensor i is sharded along dim 0 with p_i =
+// ceil(d_i / N) rows per rank, rounded up until p_i * W_i is a whole number of 16-byte vectors. --op all_gather: b200collAllGatherShards
+// from -d shards (float with --out-dtype bfloat16|half: the cast) into --out-dtype fulls. --op reduce_scatter: b200collReduceScatterShards
+// from -d gradients into --out-dtype shards (bfloat16|half -> float), times --scale, added to the old shard with --accumulate. Every
+// tensor lives in the arena, the fulls back to back at 256-byte offsets in one buffer and the shards in another. Bit-copy gather sources
+// hold a hash of (rank, 32-bit word); cast sources, gradients and old shards hold seeded values with full mantissas (cp_val), so casts
+// and sums round. -c 1 checks every output element on the host: the gather against the source bits or their cast, the reduce-scatter
+// against t = sum over ranks in rank order from +0, t * scale, old + t, rounded once. The size is the block's bytes in the full dtype;
+// "rw GB/s" counts the shard and full bytes this rank reads or writes.
+struct FsTensor { size_t d, W, p, foff, soff; };      // rows, width, rows per rank, byte offsets in the full and shard buffers
+static std::vector<FsTensor> fs_tensors(const Opts& o, int n, size_t* full_bytes, size_t* shard_bytes) {
+  const size_t H = o.fs_h, F = o.fs_f, KV = o.fs_kv ? o.fs_kv : o.fs_h;
+  const size_t ess = b200collTypeSize(o.op == "all_gather" ? o.in_dt : o.out_dt), esf = b200collTypeSize(o.op == "all_gather" ? o.out_dt : o.in_dt);
+  const size_t es = std::min(ess, esf);
+  const size_t shapes[9][2] = {{H, H}, {KV, H}, {KV, H}, {H, H}, {F, H}, {F, H}, {H, F}, {H, 1}, {H, 1}};
+  std::vector<FsTensor> ts;
+  size_t fo = 0, so = 0;
+  for (const auto& sh : shapes) {
+    FsTensor t{sh[0], sh[1], (sh[0] + n - 1) / n, fo, so};
+    while ((t.p * t.W * es) % 16) t.p++;
+    fo += (t.d * t.W * esf + 255) / 256 * 256;
+    so += (t.p * t.W * ess + 255) / 256 * 256;
+    ts.push_back(t);
+  }
+  *full_bytes = fo; *shard_bytes = so;
+  return ts;
+}
+static size_t fs_arena_bytes(const Opts& o) {
+  size_t fb = 0, sb = 0;
+  fs_tensors(o, o.nranks, &fb, &sb);
+  return fb + sb + 8192;
+}
+static int run_fsdp(const Opts& o, RankCtx& ctx) {
+  const int n = ctx.nranks, rank = ctx.rank;
+  const bool gather = o.op == "all_gather";
+  const b200collDataType_t sdt = gather ? o.in_dt : o.out_dt, fdt = gather ? o.out_dt : o.in_dt;
+  const size_t ess = b200collTypeSize(sdt), esf = b200collTypeSize(fdt);
+  size_t full_bytes = 0, shard_bytes = 0;
+  const std::vector<FsTensor> ts = fs_tensors(o, n, &full_bytes, &shard_bytes);
+  void *full = nullptr, *shard = nullptr;
+  CC(b200collMemAlloc(ctx.comm, &full, full_bytes));
+  CC(b200collMemAlloc(ctx.comm, &shard, shard_bytes));
+  std::vector<b200collShardTensor> desc;
+  size_t unit = 0, mine = 0;                         // the block's bytes in the full dtype; this rank's rows of it
+  auto own = [&](const FsTensor& t, int r) { const size_t f = std::min(t.d, (size_t)r * t.p); return std::min(t.d - f, t.p); };
+  for (const FsTensor& t : ts) {
+    desc.push_back({static_cast<char*>(shard) + t.soff, static_cast<char*>(full) + t.foff, t.d, t.W, t.p});
+    unit += t.d * t.W * esf;
+    mine += own(t, rank) * t.W * esf;
+  }
+  const bool cast_in = gather && sdt != fdt;
+  const cudaStream_t st = ctx.st;
+  if (gather) {
+    if (cast_in) k_cp_fill<float><<<256, 256, 0, st>>>(static_cast<float*>(shard), shard_bytes / 4, rank);
+    else k_uly_fill<<<256, 256, 0, st>>>(static_cast<uint32_t*>(shard), shard_bytes / 4, rank);
+    RT(cudaGetLastError());
+    RT(cudaMemsetAsync(full, 0x7B, full_bytes, st));
+  } else {
+    if (fdt == b200collFloat32) k_cp_fill<float><<<256, 256, 0, st>>>(static_cast<float*>(full), full_bytes / 4, rank);
+    else if (fdt == b200collFloat16) k_cp_fill<__half><<<256, 256, 0, st>>>(static_cast<__half*>(full), full_bytes / 2, rank);
+    else k_cp_fill<__nv_bfloat16><<<256, 256, 0, st>>>(static_cast<__nv_bfloat16*>(full), full_bytes / 2, rank);
+    if (sdt == b200collFloat32) k_cp_fill<float><<<256, 256, 0, st>>>(static_cast<float*>(shard), shard_bytes / 4, 1000 + rank);
+    else if (sdt == b200collFloat16) k_cp_fill<__half><<<256, 256, 0, st>>>(static_cast<__half*>(shard), shard_bytes / 2, 1000 + rank);
+    else k_cp_fill<__nv_bfloat16><<<256, 256, 0, st>>>(static_cast<__nv_bfloat16*>(shard), shard_bytes / 2, 1000 + rank);
+    RT(cudaGetLastError());
+  }
+  if (rank == 0) {
+    printf("# b200coll_perf op=%s fsdp nranks=%d %s -> %s H=%d F=%d KV=%d tensors=9%s%s: size = the block's bytes in the full dtype; rw GB/s = "
+           "(shard + full bytes this rank reads or writes) / time\n", o.op.c_str(), n, dt_name(gather ? sdt : fdt), dt_name(gather ? fdt : sdt),
+           o.fs_h, o.fs_f, o.fs_kv ? o.fs_kv : o.fs_h, gather ? "" : (o.accumulate ? " accumulate" : " overwrite"), gather ? "" : (" scale=" + std::to_string(o.scale)).c_str());
+    printf("#%13s %6s %8s | %10s %8s %6s\n", "size(B)", "type", "algo", "us", "rwGB/s", "#wrong");
+    fflush(stdout);
+  }
+  auto launch = [&](int) {
+    if (gather) CC(b200collAllGatherShards(desc.data(), (int)desc.size(), sdt, fdt, ctx.comm, st));
+    else CC(b200collReduceScatterShards(desc.data(), (int)desc.size(), fdt, sdt, o.scale, o.accumulate ? 1 : 0, ctx.comm, st));
+  };
+  long errs = 0;
+  if (o.check) {
+    check_launch(o, ctx, launch);
+    if (gather) {                        // full[s * p + j] = cast(shard_s[j]) for every rank s
+      std::vector<uint8_t> host(full_bytes);
+      RT(cudaMemcpy(host.data(), full, full_bytes, cudaMemcpyDeviceToHost));
+      for (size_t i = 0; i < ts.size(); i++) {
+        const FsTensor& t = ts[i];
+        for (int s = 0; s < n; s++)
+          for (size_t e = 0; e < own(t, s) * t.W; e++) {
+            const size_t fe = s * t.p * t.W + e;                                 // element of the full tensor
+            uint32_t want = 0, got = 0;
+            if (cast_in) {
+              want = out_bits(cp_val(s, t.soff / 4 + e), fdt);
+              got = got_bits(host.data() + t.foff, fe, fdt);
+            } else {
+              for (size_t b = 0; b < esf; b++) {
+                want |= (uint32_t)uly_byte(s, t.soff + e * esf + b) << (8 * b);
+                got |= (uint32_t)host[t.foff + fe * esf + b] << (8 * b);
+              }
+            }
+            if (got != want) {
+              if (errs < 4) fprintf(stderr, "rank %d fsdp gather tensor %zu from rank %d element %zu: got 0x%x want 0x%x\n", rank, i, s, e, got, want);
+              errs++;
+            }
+          }
+      }
+    } else {                             // shard[j] = round_once(old + (sum over s in rank order of full_s[r p + j]) * scale)
+      std::vector<uint8_t> host(shard_bytes);
+      RT(cudaMemcpy(host.data(), shard, shard_bytes, cudaMemcpyDeviceToHost));
+      const bool bit_copy = n == 1 && sdt == fdt && o.scale == 1.0f && !o.accumulate;
+      for (size_t i = 0; i < ts.size(); i++) {
+        const FsTensor& t = ts[i];
+        for (size_t e = 0; e < own(t, rank) * t.W; e++) {
+          const size_t fe = t.foff / esf + rank * t.p * t.W + e;              // element of the full buffer
+          float acc = 0.0f;
+          for (int s = 0; s < n; s++) acc = acc + round_dt(cp_val(s, fe), fdt);
+          acc = acc * o.scale;
+          if (o.accumulate) acc = round_dt(cp_val(1000 + rank, t.soff / ess + e), sdt) + acc;
+          const uint32_t want = bit_copy ? out_bits(round_dt(cp_val(0, fe), fdt), fdt) : out_bits(acc, sdt);
+          const uint32_t got = got_bits(host.data() + t.soff, e, sdt);
+          if (got != want) {
+            if (errs < 4) fprintf(stderr, "rank %d fsdp reduce-scatter tensor %zu element %zu: got 0x%x want 0x%x\n", rank, i, e, got, want);
+            errs++;
+          }
+        }
+      }
+    }
+  }
+  const Timing tm = timed(o, ctx, errs, launch);
+  if (rank == 0) {
+    const size_t rw = gather ? mine / esf * ess + (size_t)n * mine : mine * n + mine / esf * ess * (o.accumulate ? 2 : 1);
+    printf("%14zu %6s %8s | %10.2f %8.2f %6ld\n", unit, dt_name(fdt), n > 1 ? "twoshot" : "copy", tm.ms * 1e3, rw / (tm.ms * 1e3) / 1e3, tm.errors);
+    fflush(stdout);
+  }
+  CC(b200collMemFree(ctx.comm, shard));
+  CC(b200collMemFree(ctx.comm, full));
+  return mode_result(ctx, tm.errors);
+}
+
 static int run_rank(const Opts& o, RankCtx ctx) {
   const int n = ctx.nranks, rank = ctx.rank;
   RT(cudaSetDevice(ctx.dev));
@@ -951,6 +1091,7 @@ static int run_rank(const Opts& o, RankCtx ctx) {
   if (o.max_ctas > 0) CC(b200collCommSetMaxCtas(ctx.comm, o.max_ctas));
   if (o.uly_d) return run_ulysses(o, ctx);
   if (o.cp_c) return run_context(o, ctx);
+  if (o.fs_h) return run_fsdp(o, ctx);
   const size_t is = b200collTypeSize(o.in_dt), os = b200collTypeSize(o.out_dt);
   const bool is_bc = o.op == "broadcast", is_rd = o.op == "reduce", is_sr = o.op == "sendrecv";
   const bool is_ar = o.op == "all_reduce" || is_bc || is_rd || is_sr;      // "whole message" geometry: count elements in, count out
@@ -1214,6 +1355,25 @@ static LauncherRank launcher_rank() {
 static bool flags_ok(const Opts& o) {
   const int n = o.nranks;
   if (o.uly_back && !o.uly_d) { fprintf(stderr, "--ulysses-back takes --ulysses HQ:HKV:D\n"); return false; }
+  if (o.accumulate && !o.fs_h) { fprintf(stderr, "--accumulate takes --fsdp H:F[:KV]\n"); return false; }
+  if (o.fs_h) {
+    const bool gather = o.op == "all_gather";
+    if ((!gather && o.op != "reduce_scatter") || o.q_block || o.bs_rows || o.combine_k || o.route_e || o.cq_block || o.rms_row || o.uly_d || o.cp_c) {
+      fprintf(stderr, "--fsdp H:F[:KV] takes --op all_gather or reduce_scatter, and no --quantize, --block-scale, --combine, --route, --rms-norm,\n"
+                      "--ulysses or --context\n");
+      return false;
+    }
+    if (gather && (o.accumulate || o.scale != 1.0f)) { fprintf(stderr, "--fsdp: --accumulate and --scale take --op reduce_scatter\n"); return false; }
+    const b200collDataType_t a = o.in_dt, b = o.out_dt;
+    const bool ok = gather ? ((a == b) || (a == b200collFloat32 && (b == b200collBfloat16 || b == b200collFloat16)))
+                           : ((a == b && wide(a)) || (b == b200collFloat32 && (a == b200collBfloat16 || a == b200collFloat16)));
+    if (!ok) {
+      fprintf(stderr, "--fsdp: dtype pair (-d -> --out-dtype) must be, for all_gather, one dtype or float -> bfloat16|half; for reduce_scatter,\n"
+                      "bfloat16|half|float -> the same or bfloat16|half -> float\n");
+      return false;
+    }
+    return true;
+  }
   if (o.cp_c) {
     if ((o.op != "all_gather" && o.op != "reduce_scatter") || o.out_dt != o.in_dt || o.scale != 1.0f || o.q_block || o.bs_rows || o.combine_k ||
         o.route_e || o.cq_block || o.rms_row || o.uly_d) {
@@ -1298,7 +1458,8 @@ static size_t arena_bytes(const Opts& o) {
          q_scratch_bytes(o) + (o.route_e ? o.max_bytes * o.route_k + 4096 : 0) + route_scale_bytes(o) + cq_scratch_bytes(o) +     // --route: recv holds K rows per token
          (o.rms_row ? o.max_bytes + 4096 : 0) + rms_scale_bytes(o) +                                  // --rms-norm: the residual (and the scales of q)
          (o.uly_d ? uly_out_bytes(o, o.nranks, o.max_bytes + 4096) : 0) +                            // --ulysses: the head shards
-         (o.cp_c ? cp_shard_bytes(o) + cp_full_bytes(o, o.nranks) : 0);                                // --context: the shards and full tensors
+         (o.cp_c ? cp_shard_bytes(o) + cp_full_bytes(o, o.nranks) : 0) +                              // --context: the shards and full tensors
+         (o.fs_h ? fs_arena_bytes(o) : 0);                                                          // --fsdp: the block's fulls and shards
 }
 
 int main(int argc, char** argv) {
@@ -1339,6 +1500,16 @@ int main(int argc, char** argv) {
       }
     }
     else if (a == "--ulysses-back") o.uly_back = true;
+    else if (a == "--fsdp") {
+      const char* v = next();
+      int h = 0, f = 0, kv = 0, used = 0;
+      const int got = sscanf(v, "%d:%d%n:%d%n", &h, &f, &used, &kv, &used);
+      if (!((got == 2 || got == 3) && !v[used] && h > 0 && f > 0 && (got == 2 || kv > 0) && h % 16 == 0 && f % 16 == 0 && kv % 16 == 0)) {
+        fprintf(stderr, "--fsdp H:F[:KV]: positive integers, each a multiple of 16\n"); return 1;
+      }
+      o.fs_h = h; o.fs_f = f; o.fs_kv = got == 3 ? kv : 0;
+    }
+    else if (a == "--accumulate") o.accumulate = true;
     else if (a == "--context") {
       const char* v = next();
       long long w = 0;
@@ -1430,6 +1601,12 @@ int main(int argc, char** argv) {
            "                            order in one call; reduce_scatter: the gradient, [S, HKV * D] summed over the ranks into the K and V\n"
            "                            slices of a packed dQKV; size = shard bytes per rank, rounded down to whole tokens; -c 1 checks every\n"
            "                            output byte (the reduce-scatter against the fp32 sum in rank order)\n"
+           "  --fsdp H:F[:KV]           --op all_gather or reduce_scatter: FSDP's dim-0 shards of one Llama block (q, k, v, o, gate, up, down and two\n"
+           "                            norm weights; hidden H, MLP F, K/V width KV, default H), one call for the nine tensors, p = ceil(d / N)\n"
+           "                            rows per rank. all_gather: -d shards -> --out-dtype fulls (float -> bfloat16|half casts, else one dtype);\n"
+           "                            reduce_scatter: -d gradients -> --out-dtype shards (bfloat16|half -> float widens), times --scale X,\n"
+           "                            --accumulate adds into the old shard; -c 1 checks every output element against the header's formulas\n"
+           "  --accumulate              with --fsdp and --op reduce_scatter: shard = round_once(old + sum * scale)\n"
            "  --selfcheck              report whether this node can run the NVLink fast paths (exit 1 if not)");
       return 0;
     }

@@ -54,6 +54,10 @@ class ContextTensor(C.Structure):
     _fields_ = [("shard", C.c_void_p), ("row_stride", C.c_size_t), ("full", C.c_void_p), ("width", C.c_size_t)]
 
 
+class ShardTensor(C.Structure):
+    _fields_ = [("shard", C.c_void_p), ("full", C.c_void_p), ("rows", C.c_size_t), ("width", C.c_size_t), ("shard_rows", C.c_size_t)]
+
+
 class Config(C.Structure):
     _fields_ = [("arena_bytes", C.c_size_t), ("enable_nvls", C.c_int), ("max_ctas", C.c_int), ("timeout_ms", C.c_int), ("debug", C.c_int)]
 
@@ -163,6 +167,8 @@ def load() -> C.CDLL:
     L.b200collAllToAllHeadsToSeq.argtypes = [C.POINTER(UlyssesTensor), ci, sz, sz, sz, ci, vp, vp]
     L.b200collAllGatherContext.argtypes = [C.POINTER(ContextTensor), ci, sz, sz, ci, ci, vp, vp]
     L.b200collReduceScatterContext.argtypes = [C.POINTER(ContextTensor), ci, sz, sz, ci, ci, vp, vp]
+    L.b200collAllGatherShards.argtypes = [C.POINTER(ShardTensor), ci, ci, ci, vp, vp]
+    L.b200collReduceScatterShards.argtypes = [C.POINTER(ShardTensor), ci, ci, ci, C.c_float, ci, vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -782,6 +788,102 @@ def check_reduce_scatter_context(nranks: int, fulls, shards, chunks: int) -> tup
     return _check_context(nranks, shards, fulls, chunks, False)
 
 
+MAX_SHARD_TENSORS = 64
+
+
+def shard_range(rows: int, shard_rows: int, rank: int) -> tuple[int, int]:
+    """The rows [first, first + n) that rank owns of a tensor of `rows` rows sharded `shard_rows` per rank along dim 0, as the header
+    states it: first = rank * shard_rows, n = clamp(rows - first, 0, shard_rows) (first clamped to rows when n is 0)."""
+    first = min(rows, rank * shard_rows)
+    return first, max(0, min(rows - first, shard_rows))
+
+
+def _check_shards(nranks: int, rank: int, shards, fulls, shard_rows, gather: bool) -> list[tuple[int, int, int]]:
+    import torch
+    what = "all_gather_shards" if gather else "reduce_scatter_shards"
+    shards, fulls = list(shards), list(fulls)
+    if not 1 <= len(fulls) <= MAX_SHARD_TENSORS or len(shards) != len(fulls):
+        raise ValueError(f"{what}: 1 to {MAX_SHARD_TENSORS} tensors and one shard per full, got {len(shards)} shards and {len(fulls)} fulls")
+    sdt, fdt = shards[0].dtype, fulls[0].dtype
+    if gather:
+        ok = (sdt == fdt and sdt in (torch.bfloat16, torch.float16, torch.float32, torch.float8_e4m3fn, torch.float8_e5m2)) or \
+             (sdt == torch.float32 and fdt in (torch.bfloat16, torch.float16))
+        pairs = "one dtype in and out (bfloat16, float16, float32, float8_e4m3fn or float8_e5m2), or float32 -> bfloat16 or float16"
+    else:
+        ok = (sdt == fdt and sdt in (torch.bfloat16, torch.float16, torch.float32)) or \
+             (sdt == torch.float32 and fdt in (torch.bfloat16, torch.float16))
+        pairs = "bfloat16, float16 or float32 -> the same, or bfloat16 or float16 -> float32"
+    if not ok:
+        src, dst = (sdt, fdt) if gather else (fdt, sdt)
+        raise ValueError(f"{what}: the dtype pair must be {pairs}, got {src} -> {dst}")
+    if shard_rows is None or isinstance(shard_rows, int):
+        rows_per = [shard_rows] * len(fulls)
+    else:
+        rows_per = list(shard_rows)
+        if len(rows_per) != len(fulls):
+            raise ValueError(f"{what}: shard_rows must be one int or one per tensor, got {len(rows_per)} for {len(fulls)} tensors")
+    ess, esf = shards[0].element_size(), fulls[0].element_size()
+    per, srcs, dsts, total = [], [], [], 0
+    for i, (x, f, p) in enumerate(zip(shards, fulls, rows_per)):
+        if x.dtype != sdt or f.dtype != fdt:
+            raise ValueError(f"{what}: tensor {i}: every shard must be {sdt} and every full {fdt}, got {x.dtype} and {f.dtype}")
+        if f.dim() < 1 or not f.is_contiguous():
+            raise ValueError(f"{what}: fulls[{i}] must be a contiguous tensor of at least one dim, got shape {list(f.shape)}")
+        d, W = f.shape[0], _prod(f.shape[1:])
+        if d == 0 or W == 0:
+            raise ValueError(f"{what}: tensor {i}: rows and width must be positive, got shape {list(f.shape)}")
+        p = -(-d // nranks) if p is None else p
+        if p < 1:
+            raise ValueError(f"{what}: tensor {i}: shard_rows must be positive, got {p}")
+        if nranks * p < d:
+            raise ValueError(f"{what}: tensor {i}: nranks * shard_rows must be at least rows, got {nranks} x {p} < {d}")
+        _, n_r = shard_range(d, p, rank)
+        if x.dim() != f.dim() or tuple(x.shape[1:]) != tuple(f.shape[1:]) or x.shape[0] < n_r or not x.is_contiguous():
+            raise ValueError(f"{what}: shards[{i}] must be a contiguous [>= {n_r}, {', '.join(str(e) for e in f.shape[1:])}] tensor "
+                             f"(rank {rank}'s rows of fulls[{i}]), got {list(x.shape)}")
+        if any((p * W * es) % 16 or (d * W * es) % 16 for es in (ess, esf)):
+            raise ValueError(f"{what}: tensor {i}: shard_rows * width and rows * width must be multiples of 16 bytes in both dtypes, "
+                             f"got {p} x {W} and {d} x {W}")
+        if max(d, p) * W * max(ess, esf) // 16 > _I31:
+            raise ValueError(f"{what}: tensor {i}: more than 2^31 - 1 16-byte vectors in one side")
+        if f.data_ptr() % 16 or (n_r and x.data_ptr() % 16):
+            raise ValueError(f"{what}: tensor {i}: every pointer must be 16-byte aligned")
+        total += p * W * esf // 16
+        shard_span = (x.data_ptr(), 1, n_r * W * ess, n_r * W * ess)
+        full_span = (f.data_ptr(), 1, d * W * esf, d * W * esf)
+        srcs.append(shard_span if gather else full_span)
+        dsts.append(full_span if gather else shard_span)
+        per.append((d, W, p))
+    if total > _I31:
+        raise ValueError(f"{what}: more than 2^31 - 1 16-byte vectors in the call")
+    for i, dd in enumerate(dsts):
+        for j, sp in enumerate(srcs):
+            if _spans_overlap(dd, sp):
+                raise ValueError(f"{what}: output {i} overlaps source {j}")
+        for j in range(i + 1, len(dsts)):
+            if _spans_overlap(dd, dsts[j]):
+                raise ValueError(f"{what}: outputs {i} and {j} overlap")
+    return per
+
+
+def check_all_gather_shards(nranks: int, rank: int, shards, fulls, shard_rows=None) -> list[tuple[int, int, int]]:
+    """The rules of Comm.all_gather_shards, checked on the tensors' metadata (no device, no communicator): raises ValueError, returns
+    [(rows, width, shard_rows)] per tensor. fulls: 1 to 64 contiguous tensors; rows d is dim 0 and width W the product of the other
+    dims. shard_rows p: None (FSDP2's ceil(d / nranks)), one int, or one per tensor, with nranks * p >= d. shards: contiguous, with the
+    full's trailing shape and at least n_r = clamp(d - rank * p, 0, p) rows. Dtypes (shard -> full): one dtype in and out (bfloat16,
+    float16, float32, float8_e4m3fn or float8_e5m2), or float32 -> bfloat16 or float16. p * W and d * W whole multiples of 16 bytes in
+    both dtypes, pointers 16-byte aligned, at most 2^31 - 1 16-byte vectors per side and in sum p * W; no output may overlap a source
+    or another output."""
+    return _check_shards(nranks, rank, shards, fulls, shard_rows, True)
+
+
+def check_reduce_scatter_shards(nranks: int, rank: int, fulls, shards, shard_rows=None) -> list[tuple[int, int, int]]:
+    """The rules of Comm.reduce_scatter_shards, checked on the tensors' metadata: raises ValueError, returns as check_all_gather_shards.
+    Dtypes (full -> shard): bfloat16, float16 or float32 to the same, or bfloat16 or float16 to float32. Everything else as the
+    gather."""
+    return _check_shards(nranks, rank, shards, fulls, shard_rows, False)
+
+
 def _check_routed(nranks: int, x, topk_idx, num_experts: int, recv, expert_counts, route, dropped, fp8=None) -> None:
     """The rules of both device-routed dispatches; fp8 is None (check_expert_dispatch) or (recv_scales, block), which adds the FP8
     call's rules, as routed_prepare in coll/src/dispatch.cu takes a RoutedQuant."""
@@ -1334,6 +1436,49 @@ class Comm:
         shards = list(shards)
         B, S_l, per = check_reduce_scatter_context(self.nranks, fulls, shards, chunks)
         self._context(load().b200collReduceScatterContext, "ReduceScatterContext", shards, fulls, per, B, S_l, chunks, stream)
+        return shards
+
+    def _shard_tensors(self, shards, fulls, per):
+        return (ShardTensor * len(fulls))(*[ShardTensor(x.data_ptr(), f.data_ptr(), d, w, p) for x, f, (d, w, p) in zip(shards, fulls, per)])
+
+    def all_gather_shards(self, shards, fulls=None, *, shard_rows=None, stream=None):
+        """FSDP's parameter all-gather before forward, one kernel for up to 64 tensors (one unit): this rank's dim-0 shard of each
+        parameter (rows [rank * p, rank * p + n_r) of the unsharded tensor, p = shard_rows, by default ceil(rows / N)) is cast on this
+        rank (float32 -> bfloat16 or float16, or kept as it is) and stored into its rows of the unsharded tensor in fulls on every rank.
+        Bit for bit as coll/include/b200coll.h's b200collAllGatherShards states. Returns fulls. With more than one rank fulls must be
+        given, as arena tensors (`empty()` or the communicator's `mem_pool()`) at the same offsets on every rank; with one rank None
+        allocates them in the shards' dtype."""
+        shards = list(shards)
+        if fulls is None:
+            if self.nranks > 1:
+                raise ValueError("all_gather_shards with more than one rank needs fulls: arena tensors (Comm.empty or Comm.mem_pool) of the "
+                                 "unsharded shapes, the same on every rank")
+            fulls = [x.new_empty(x.shape) for x in shards]
+        fulls = list(fulls)
+        per = check_all_gather_shards(self.nranks, self.rank, shards, fulls, shard_rows)
+        arr = self._shard_tensors(shards, fulls, per)
+        _check(load().b200collAllGatherShards(arr, len(fulls), torch_dtype_code(shards[0].dtype), torch_dtype_code(fulls[0].dtype), self._h,
+                                              self._stream(stream)), "AllGatherShards")
+        return fulls
+
+    def reduce_scatter_shards(self, fulls, shards=None, *, scale: float = 1.0, accumulate: bool = False, shard_rows=None, stream=None):
+        """FSDP's gradient reduce-scatter after backward, one kernel for up to 64 tensors: every rank's unsharded gradients in fulls
+        are summed in fp32 in rank order, multiplied by scale (1 / N for a mean), added to the gradient already in shards if
+        accumulate, rounded once and stored into this rank's rows of each shard (bfloat16 or float16 gradients may go to float32
+        shards). Bit for bit as b200collReduceScatterShards states. Returns shards. With more than one rank fulls must be arena tensors
+        at the same offsets on every rank and shards must be given (any device tensors); with one rank None allocates them in the
+        fulls' dtype, unless accumulate asks for the old values."""
+        fulls = list(fulls)
+        if shards is None:
+            if self.nranks > 1 or accumulate:
+                raise ValueError("reduce_scatter_shards needs shards with more than one rank or with accumulate: this rank's sharded "
+                                 "gradients, one per full")
+            shards = [f.new_empty(f.shape) for f in fulls]
+        shards = list(shards)
+        per = check_reduce_scatter_shards(self.nranks, self.rank, fulls, shards, shard_rows)
+        arr = self._shard_tensors(shards, fulls, per)
+        _check(load().b200collReduceScatterShards(arr, len(fulls), torch_dtype_code(fulls[0].dtype), torch_dtype_code(shards[0].dtype),
+                                                  float(scale), int(bool(accumulate)), self._h, self._stream(stream)), "ReduceScatterShards")
         return shards
 
     def _rows(self, xs):
