@@ -79,6 +79,8 @@ typedef enum {
  *   P2P reduce-scatter (16- and 32-bit inputs)              receiving rank r sums r, r+1, .., N-1, 0, .., r-1
  *   context-parallel reduce-scatter                         ranks 0 .. N-1
  *   FSDP shard reduce-scatter (ReduceScatterShards)         ranks 0 .. N-1, then * scale, then + the old shard
+ *   vocab-parallel cross-entropy (VocabParallelCrossEntropy) ranks 0 .. N-1 for S = sum_r s_r * exp(m_r - M); in a rank's slice, its
+ *                                                           16-element chunk sums folded as RMSNorm's (see the entry below)
  *   NVLS (multimem.ld_reduce)                               the switch's order: within an ulp of the exact sum, not bit-reproducible
  * Rounding to FP8 saturates to the finite range (+-inf becomes +-max, NaN stays NaN); fp16 overflows to inf.
  * All-gather, broadcast and all-to-all(v) apply the same epilogue per element: round((0 + x) * scale) (e4m3 in, bf16 out, scale =
@@ -690,6 +692,46 @@ b200collResult_t b200collAllGatherShards(const b200collShardTensor* tensors, int
 b200collResult_t b200collReduceScatterShards(const b200collShardTensor* tensors, int ntensors, b200collDataType_t full_dtype,
                                              b200collDataType_t shard_dtype, float scale, int accumulate, b200collComm_t comm,
                                              b200collStream_t stream);
+
+/* Vocab-parallel cross-entropy for a tensor-parallel LM head (Megatron's vocab_parallel_cross_entropy), one kernel per direction
+ * (src/xent.cu). N ranks, this rank r, Vl = vocab_local. logits: this rank's dense [rows, Vl] of `dtype` (bf16, fp16 or fp32), its
+ * columns being the global vocabulary ids [r * Vl, (r + 1) * Vl) (Megatron's uniform split). target: [rows] int64 global ids, THE SAME
+ * ON EVERY RANK (the caller's condition; nothing checks it). loss, lse, dloss: [rows] fp32. Every product and sum is an IEEE fp32 op
+ * rounded on its own (no fused multiply-add); exp and log are the library's own fixed sequences of fp32 multiplies, adds, rint and
+ * exponent-bit arithmetic (no hardware approximation), within 1 ulp of the exact value, exp(0) == 1, exp(x) == +0 for x < -87,
+ * exp(x) == +inf for x > 88.7228317, log(1) == 0, log(+0) == -inf; tests/coll_xent_reference.py mirrors both in numpy. Per row t:
+ *   1. On rank r, with x the widened logits of the row:
+ *        m_r = max_j x_j, NaN if any x_j is NaN (+inf if any is +inf and none is NaN);
+ *        s_r = sum_j exp(x_j - m_r): the sums of the 16-element chunks (columns 16c .. 16c+15, the last one short) in column order from
+ *              +0, padded with +0 to a power of two P and folded p = p[:P/2] + p[P/2:] until one value is left; s_r = +0 if m_r = -inf;
+ *        z_r = x_{target - r * Vl} if 0 <= target - r * Vl < Vl (this rank owns the target).
+ *      (m_r, s_r, z_r, owns) is pushed as one 16-byte record into row t of every rank's mailbox.
+ *   2. Every rank combines the N records in rank order: M = max_r m_r (NaN-aware), S = ((+0 + e_0) + e_1) + .. + e_{N-1} with
+ *      e_r = s_r * exp(m_r - M) (e_r = +0 if m_r = -inf), lse = M + log(S), loss = lse - z with z from the owning rank. If
+ *      target == ignore_index, loss = +0; else if target is outside [0, N * Vl), loss = NaN, and nothing outside the row is read. lse is
+ *      stored for every row.
+ *   Backward (no communication): grad[t, j] = round_dtype((exp(x_j - lse[t]) - [r * Vl + j == target]) * dloss[t]), RNE; +0 on rows with
+ *   target == ignore_index, NaN on rows whose target is out of range. grad == logits (the whole buffer) runs in place.
+ * Every rank holds the same loss and lse. The result depends only on the values and N, not on the launch shape.
+ * Arguments (InvalidArgument, message in b200collGetLastError, nothing launched): dtype not bf16, fp16 or fp32; Vl == 0 or Vl * sizeof(dtype)
+ * not a multiple of 16; N * Vl >= 2^31; rows >= 2^31; a null pointer when rows > 0; logits or grad not 16-byte aligned, target not
+ * 8-byte aligned, loss, lse or dloss not 4-byte aligned; any overlap among the outputs (loss and lse; grad) and the inputs other than
+ * grad == logits. A poisoned communicator gives RemoteError.
+ * Placement: every buffer may be any device memory, as only its own rank reads or writes it. The only cross-rank memory is the mailbox,
+ * rows * N * 16 bytes of the quantising collectives' scratch (a collective contract like b200collMemAlloc: every rank makes the same
+ * calls in the same order; OutOfMemory, before anything is launched, when the arena cannot hold it; a superseded scratch is kept until
+ * CommDestroy, so a captured CUDA graph stays valid). rows, Vl, ignore_index and dtype must be equal on every rank; B200COLL_CHECK=1
+ * cross-checks them and the mailbox offset on multi-process communicators. The forward starts with a relaxed barrier (every rank has
+ * finished the previous user of its mailbox) and publishes the records with a releasing one; rows == 0 still launches on every rank.
+ * The host reads no device data, so both calls can be captured in a CUDA graph. One rank: a local kernel, no barrier, no mailbox.
+ * b200collStats count the forward as an allreduce of rows * 16 bytes under twoshot (copy with one rank), one kernel launch; the
+ * backward as one kernel launch and no operation (rows == 0: nothing). The tuner and b200collCommSetAlgo do not apply. */
+b200collResult_t b200collVocabParallelCrossEntropy(const void* logits, const int64_t* target, float* loss, float* lse, size_t rows,
+                                                   size_t vocab_local, int64_t ignore_index, b200collDataType_t dtype, b200collComm_t comm,
+                                                   b200collStream_t stream);
+b200collResult_t b200collVocabParallelCrossEntropyBackward(const void* logits, const int64_t* target, const float* lse, const float* dloss,
+                                                           void* grad, size_t rows, size_t vocab_local, int64_t ignore_index,
+                                                           b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
 
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.

@@ -169,6 +169,8 @@ def load() -> C.CDLL:
     L.b200collReduceScatterContext.argtypes = [C.POINTER(ContextTensor), ci, sz, sz, ci, ci, vp, vp]
     L.b200collAllGatherShards.argtypes = [C.POINTER(ShardTensor), ci, ci, ci, vp, vp]
     L.b200collReduceScatterShards.argtypes = [C.POINTER(ShardTensor), ci, ci, ci, C.c_float, ci, vp, vp]
+    L.b200collVocabParallelCrossEntropy.argtypes = [vp, vp, vp, vp, sz, sz, C.c_int64, ci, vp, vp]
+    L.b200collVocabParallelCrossEntropyBackward.argtypes = [vp, vp, vp, vp, vp, sz, sz, C.c_int64, ci, vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -884,6 +886,62 @@ def check_reduce_scatter_shards(nranks: int, rank: int, fulls, shards, shard_row
     return _check_shards(nranks, rank, shards, fulls, shard_rows, False)
 
 
+def _xent_overlap(a, b) -> bool:
+    return a[1] > 0 and b[1] > 0 and a[0] < b[0] + b[1] and b[0] < a[0] + a[1]
+
+
+def check_vocab_parallel_cross_entropy(nranks: int, logits, target, loss=None, lse=None, dloss=None, grad=None) -> tuple[int, int]:
+    """The rules of Comm.vocab_parallel_cross_entropy (and, with dloss given, of its backward), checked on the tensors' metadata (no
+    device, no communicator), as xent_check in coll/src/xent.cu: raises ValueError, returns (rows, vocab_local). logits: a contiguous
+    [rows, Vl] bfloat16, float16 or float32 tensor, Vl > 0 and Vl * itemsize a multiple of 16 bytes, nranks * Vl < 2^31, rows < 2^31;
+    target: contiguous [rows] int64; loss, lse, dloss: contiguous [rows] float32; grad: logits' dtype and shape. Alignment: logits and
+    grad 16 bytes, target 8, the float32 arrays 4. No output (loss and lse; grad) may overlap an input or another output, except
+    grad is logits (the in-place backward)."""
+    import torch
+    what = "vocab_parallel_cross_entropy" + ("_backward" if dloss is not None else "")
+    if logits.dtype not in (torch.bfloat16, torch.float16, torch.float32):
+        raise ValueError(f"{what}: logits must be bfloat16, float16 or float32, got {logits.dtype}")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError(f"{what}: logits must be a contiguous [rows, vocab_local] tensor, got shape {list(logits.shape)}")
+    rows, vl = logits.shape
+    es = logits.element_size()
+    if vl == 0 or (vl * es) % 16:
+        raise ValueError(f"{what}: vocab_local must be positive and vocab_local * itemsize a multiple of 16 bytes, got {vl} x {es}")
+    if nranks * vl >= 2 ** 31:
+        raise ValueError(f"{what}: nranks * vocab_local must be below 2^31, got {nranks} x {vl}")
+    if rows >= 2 ** 31:
+        raise ValueError(f"{what}: rows must be below 2^31, got {rows}")
+    if target.dtype != torch.int64 or tuple(target.shape) != (rows,) or not target.is_contiguous():
+        raise ValueError(f"{what}: target must be a contiguous [{rows}] int64 tensor, got {target.dtype} {list(target.shape)}")
+    f32 = {"loss": loss, "lse": lse, "dloss": dloss}
+    for name, t in f32.items():
+        if t is not None and (t.dtype != torch.float32 or tuple(t.shape) != (rows,) or not t.is_contiguous()):
+            raise ValueError(f"{what}: {name} must be a contiguous [{rows}] float32 tensor, got {t.dtype} {list(t.shape)}")
+    if grad is not None and (grad.dtype != logits.dtype or tuple(grad.shape) != (rows, vl) or not grad.is_contiguous()):
+        raise ValueError(f"{what}: grad must be a contiguous {logits.dtype} [{rows}, {vl}] tensor, got {grad.dtype} {list(grad.shape)}")
+    if logits.data_ptr() % 16 or (grad is not None and grad.data_ptr() % 16):
+        raise ValueError(f"{what}: logits and grad must be 16-byte aligned")
+    if target.data_ptr() % 8:
+        raise ValueError(f"{what}: target must be 8-byte aligned")
+    if any(t is not None and t.data_ptr() % 4 for t in f32.values()):
+        raise ValueError(f"{what}: loss, lse and dloss must be 4-byte aligned")
+    if rows:
+        span = lambda t: (t.data_ptr(), t.numel() * t.element_size())     # noqa: E731
+        ins = [span(logits), span(target)]
+        if dloss is not None:
+            outs, ins = [span(grad)] if grad is not None else [], ins + [span(lse), span(dloss)]
+        else:
+            outs = [span(t) for t in (loss, lse) if t is not None]
+        for i, o in enumerate(outs):
+            for j, x in enumerate(ins):
+                if _xent_overlap(o, x) and not (dloss is not None and j == 0 and o == x):
+                    raise ValueError(f"{what}: outputs must not overlap the inputs (grad is logits is the one overlap allowed)")
+            for o2 in outs[i + 1:]:
+                if _xent_overlap(o, o2):
+                    raise ValueError(f"{what}: outputs must not overlap each other")
+    return rows, vl
+
+
 def _check_routed(nranks: int, x, topk_idx, num_experts: int, recv, expert_counts, route, dropped, fp8=None) -> None:
     """The rules of both device-routed dispatches; fp8 is None (check_expert_dispatch) or (recv_scales, block), which adds the FP8
     call's rules, as routed_prepare in coll/src/dispatch.cu takes a RoutedQuant."""
@@ -1481,6 +1539,39 @@ class Comm:
                                                   float(scale), int(bool(accumulate)), self._h, self._stream(stream)), "ReduceScatterShards")
         return shards
 
+    def vocab_parallel_cross_entropy(self, logits, target, ignore_index: int = -100, *, loss=None, lse=None, stream=None):
+        """The tensor-parallel LM head's cross-entropy, one kernel: logits is this rank's [rows, Vl] slice of the vocabulary (global
+        columns [rank * Vl, (rank + 1) * Vl)), target the [rows] int64 global labels, the same on every rank. Returns (loss, lse), [rows]
+        float32 each, the same on every rank, bit for bit as coll/include/b200coll.h's b200collVocabParallelCrossEntropy states: loss =
+        logsumexp over the whole vocabulary minus the target logit, +0 where target == ignore_index, NaN where the target is out of
+        range. Any device tensors; only a 16-byte record per row and rank crosses NVLink."""
+        import torch
+        rows = logits.shape[0] if logits.dim() else 0
+        loss = logits.new_empty(rows, dtype=torch.float32) if loss is None else loss
+        lse = logits.new_empty(rows, dtype=torch.float32) if lse is None else lse
+        rows, vl = check_vocab_parallel_cross_entropy(self.nranks, logits, target, loss, lse)
+        _check(load().b200collVocabParallelCrossEntropy(logits.data_ptr(), target.data_ptr(), loss.data_ptr(), lse.data_ptr(), rows, vl,
+                                                        int(ignore_index), torch_dtype_code(logits.dtype), self._h, self._stream(stream)),
+               "VocabParallelCrossEntropy")
+        return loss, lse
+
+    def vocab_parallel_cross_entropy_backward(self, logits, target, lse, dloss, grad=None, ignore_index: int = -100, *, stream=None):
+        """The gradient of vocab_parallel_cross_entropy's loss with respect to this rank's logits, one elementwise kernel, no
+        communication: grad = round((exp(logits - lse) - onehot(target)) * dloss), +0 on ignored rows. grad=logits runs in place
+        (Megatron's way of not keeping a second [rows, Vl] buffer); grad=None allocates it. Returns grad."""
+        grad = logits.new_empty(logits.shape) if grad is None else grad
+        rows, vl = check_vocab_parallel_cross_entropy(self.nranks, logits, target, lse=lse, dloss=dloss, grad=grad)
+        _check(load().b200collVocabParallelCrossEntropyBackward(logits.data_ptr(), target.data_ptr(), lse.data_ptr(), dloss.data_ptr(),
+                                                                grad.data_ptr(), rows, vl, int(ignore_index), torch_dtype_code(logits.dtype),
+                                                                self._h, self._stream(stream)), "VocabParallelCrossEntropyBackward")
+        return grad
+
+    def vocab_parallel_cross_entropy_loss(self, logits, target, ignore_index: int = -100, *, inplace_backward: bool = False, stream=None):
+        """vocab_parallel_cross_entropy as an autograd function: returns the [rows] float32 loss; .backward() runs
+        vocab_parallel_cross_entropy_backward on this communicator. Only the logits, target and lse are saved. inplace_backward writes
+        the gradient over the logits (they must not be needed afterwards)."""
+        return _vocab_xent_fn().apply(logits, target, self, int(ignore_index), bool(inplace_backward), stream)
+
     def _rows(self, xs):
         """A host list of nranks row counts or offsets, as the library's int64[nranks]."""
         return (C.c_int64 * self.nranks)(*[int(x) for x in xs])
@@ -1710,3 +1801,33 @@ class Comm:
         rc = load().b200collCommGetAsyncError(self._h, C.byref(f))
         if rc != SUCCESS:
             raise B200CollError(rc, "watchdog", f"code={f.code} rank={f.rank} peer={f.peer} block={f.block} expected={f.expected} observed={f.observed} op={f.op}")
+
+
+_VOCAB_XENT_FN = None
+
+
+def _vocab_xent_fn():
+    """The torch.autograd.Function behind Comm.vocab_parallel_cross_entropy_loss, built on first use (torch is imported lazily here)."""
+    global _VOCAB_XENT_FN
+    if _VOCAB_XENT_FN is None:
+        import torch
+
+        class VocabParallelCrossEntropy(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, logits, target, comm, ignore_index, inplace, stream):
+                logits = logits.contiguous()
+                loss, lse = comm.vocab_parallel_cross_entropy(logits, target, ignore_index, stream=stream)
+                ctx.save_for_backward(logits, target, lse)
+                ctx.comm, ctx.ignore_index, ctx.inplace, ctx.stream = comm, ignore_index, inplace, stream
+                return loss
+
+            @staticmethod
+            def backward(ctx, dloss):
+                logits, target, lse = ctx.saved_tensors
+                grad = logits if ctx.inplace else None
+                grad = ctx.comm.vocab_parallel_cross_entropy_backward(logits, target, lse, dloss.float().contiguous(), grad,
+                                                                      ctx.ignore_index, stream=ctx.stream)
+                return grad, None, None, None, None, None
+
+        _VOCAB_XENT_FN = VocabParallelCrossEntropy
+    return _VOCAB_XENT_FN
