@@ -81,6 +81,9 @@ typedef enum {
  *   FSDP shard reduce-scatter (ReduceScatterShards)         ranks 0 .. N-1, then * scale, then + the old shard
  *   vocab-parallel cross-entropy (VocabParallelCrossEntropy) ranks 0 .. N-1 for S = sum_r s_r * exp(m_r - M); in a rank's slice, its
  *                                                           16-element chunk sums folded as RMSNorm's (see the entry below)
+ *   vocab-parallel embedding backward                       per row of dweight: its tokens in ascending token order, from +0 (or
+ *   (VocabParallelEmbeddingBackward)                        the old dweight with accumulate); no sum crosses ranks
+ *   vocab-parallel embedding (VocabParallelEmbedding)       no sum: each output row is a bit copy of one table row
  *   NVLS (multimem.ld_reduce)                               the switch's order: within an ulp of the exact sum, not bit-reproducible
  * Rounding to FP8 saturates to the finite range (+-inf becomes +-max, NaN stays NaN); fp16 overflows to inf.
  * All-gather, broadcast and all-to-all(v) apply the same epilogue per element: round((0 + x) * scale) (e4m3 in, bf16 out, scale =
@@ -732,6 +735,50 @@ b200collResult_t b200collVocabParallelCrossEntropy(const void* logits, const int
 b200collResult_t b200collVocabParallelCrossEntropyBackward(const void* logits, const int64_t* target, const float* lse, const float* dloss,
                                                            void* grad, size_t rows, size_t vocab_local, int64_t ignore_index,
                                                            b200collDataType_t dtype, b200collComm_t comm, b200collStream_t stream);
+
+/* Vocab-parallel embedding for a tensor-parallel input layer (Megatron's VocabParallelEmbedding), src/embedding.cu. N ranks, this rank
+ * r, Vl = vocab_local, T = tokens, H = hidden. weight: this rank's dense [Vl, H] of `dtype` (bf16, fp16 or fp32), its rows being the
+ * global ids [r * Vl, (r + 1) * Vl) (Megatron's uniform split). ids: [T] int64 global ids, THE SAME ON EVERY RANK (the caller's
+ * condition; nothing checks it). sequence_parallel = 0: out is [T, H] on every rank, and the backward's dout is [T, H], the same on every
+ * rank. sequence_parallel = 1: T must be a multiple of N, out is this rank's rows [r * T / N, (r + 1) * T / N) as a dense [T / N, H],
+ * and dout is this rank's [T / N, H] shard of the output gradient in the same rows.
+ *   Forward: out[t] = W_full[ids[t]], a bit copy (NaN payloads and -0 kept), with W_full the N tables stacked in rank order; out[t] = +0
+ *   when ids[t] is outside [0, N * Vl), and nothing is read for that row (Megatron's masked lookup gives the same).
+ *   Backward: for each local row j, in fp32, every add an IEEE fp32 add rounded on its own (no fused multiply-add):
+ *     acc = accumulate ? widen(dweight[j]) : +0;  for t = 0 .. T-1 ascending with ids[t] == r * Vl + j: acc = acc + widen(dout[t]);
+ *     dweight[j] = round_{dweight_dtype}(acc) (RNE; fp16 overflows to inf).
+ *   Rows no token hits get +0 (accumulate: unchanged in value); ids outside [0, N * Vl) contribute nothing. dweight_dtype is fp32 (the
+ *   fp32 main_grad) or dout_dtype. Under sequence parallelism the rank owning row j pulls row t of dout from rank t / (T / N).
+ * The result depends only on the values and N, not on the launch shape, on timing or on the distribution of the ids: the tokens of each
+ * row are grouped on the device by a stable radix sort (no atomic hands out a place, no floating-point atomic anywhere, no host sync).
+ * Arguments (InvalidArgument, message in b200collGetLastError, nothing launched): dtype, dout_dtype not bf16, fp16 or fp32; dweight_dtype
+ * not fp32 or dout_dtype; H == 0 or H * sizeof(t) not a multiple of 16 for any dtype t of the call; Vl == 0; N * Vl >= 2^31; T >= 2^31;
+ * sequence_parallel and T not a multiple of N; more than 2^31 - 1 16-byte vectors in out, dout or dweight; weight (dweight) null, or ids
+ * or out (dout) null when T > 0; ids not 8-byte aligned, weight, out, dout or dweight not 16-byte aligned; out overlapping weight or
+ * ids; dweight overlapping dout or ids; with N > 1 and T > 0, weight (forward) or the sequence-parallel dout (backward) not arena memory
+ * at the same offset on every rank (b200collMemAlloc). A poisoned communicator gives RemoteError.
+ * Placement: with one rank every buffer may be any device memory. ids, out and dweight are only ever touched by their own rank. The
+ * backward's sort buffers (16 T + 1024 * ceil(T / 2048) + 4 (Vl + 1) bytes, rounded to 16-byte parts) are this rank's own, taken from the
+ * quantising collectives' scratch when T > 0 (a collective contract like b200collMemAlloc: every rank makes the same calls in the same
+ * order; OutOfMemory, before anything is launched, when the arena cannot hold it; a superseded scratch is kept until CommDestroy, so a
+ * captured CUDA graph stays valid). T, H, Vl, sequence_parallel, the dtypes and accumulate must be equal on every rank; B200COLL_CHECK=1
+ * cross-checks them and the weight, dout and scratch arena offsets on multi-process communicators.
+ * Ordering: with N > 1 the forward, and the sequence-parallel backward, start with a relaxed barrier (every rank's stream has reached the
+ * call, so its weight or dout is written) and end with a releasing one (no rank changes its weight or dout before every peer has pulled
+ * its rows). The tensor-parallel backward moves nothing between ranks and takes no barrier. T == 0: the forward launches nothing, the
+ * backward one kernel that writes dweight (+0 or unchanged). The host reads no device data, so both calls can be captured in a CUDA graph.
+ * Launch shapes: the forward and the fold follow the P2P kind of b200collCommSetLaunchShape ("p2p"); the sort's tiles are fixed.
+ * b200collStats: the forward counts an allgather of the out bytes (T / N or T rows of H) under twoshot (copy with one rank), one kernel
+ * launch; the backward counts one kernel launch per kernel (3 per 8-bit digit of the value Vl for the sort, one for the row bounds, one for the fold),
+ * and, under sequence parallelism with N > 1, an allgather of this rank's dout bytes under twoshot. The tuner and b200collCommSetAlgo do
+ * not apply. */
+b200collResult_t b200collVocabParallelEmbedding(const int64_t* ids, const void* weight, void* out, size_t tokens, size_t hidden,
+                                                size_t vocab_local, int sequence_parallel, b200collDataType_t dtype,
+                                                b200collComm_t comm, b200collStream_t stream);
+b200collResult_t b200collVocabParallelEmbeddingBackward(const int64_t* ids, const void* dout, void* dweight, size_t tokens, size_t hidden,
+                                                        size_t vocab_local, int sequence_parallel, b200collDataType_t dout_dtype,
+                                                        b200collDataType_t dweight_dtype, int accumulate, b200collComm_t comm,
+                                                        b200collStream_t stream);
 
 /* --- host path (src/hostpath.cu). CommInitRank binds the calling thread to the CPUs of the GPU's NUMA node (B200COLL_AFFINITY=0:
  * leave it alone, 2: restore the previous mask after init). HostAlloc returns pinned, device-mapped host memory on that node.

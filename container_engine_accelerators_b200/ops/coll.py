@@ -171,6 +171,8 @@ def load() -> C.CDLL:
     L.b200collReduceScatterShards.argtypes = [C.POINTER(ShardTensor), ci, ci, ci, C.c_float, ci, vp, vp]
     L.b200collVocabParallelCrossEntropy.argtypes = [vp, vp, vp, vp, sz, sz, C.c_int64, ci, vp, vp]
     L.b200collVocabParallelCrossEntropyBackward.argtypes = [vp, vp, vp, vp, vp, sz, sz, C.c_int64, ci, vp, vp]
+    L.b200collVocabParallelEmbedding.argtypes = [vp, vp, vp, sz, sz, sz, ci, ci, vp, vp]
+    L.b200collVocabParallelEmbeddingBackward.argtypes = [vp, vp, vp, sz, sz, sz, ci, ci, ci, ci, vp, vp]
     L.b200collHostAlloc.argtypes = [vp, C.POINTER(vp), sz]
     L.b200collHostFree.argtypes = [vp, vp]
     L.b200collAllReduceHost.argtypes = [vp, vp, sz, C.POINTER(Epilogue), ci, vp, vp]
@@ -942,6 +944,64 @@ def check_vocab_parallel_cross_entropy(nranks: int, logits, target, loss=None, l
     return rows, vl
 
 
+def check_vocab_parallel_embedding(nranks: int, ids, table, rows=None, *, sequence_parallel: bool = False, backward: bool = False,
+                                   symmetric=None) -> tuple[int, int, int]:
+    """The rules of Comm.vocab_parallel_embedding (table = weight, rows = out) and, with backward=True, of its backward (table =
+    dweight, rows = grad_out), checked on the tensors' metadata as emb_check in coll/src/embedding.cu: raises ValueError, returns (T, H,
+    Vl). ids: contiguous [T] int64, T < 2^31 and, under sequence parallelism, a multiple of nranks. table: contiguous [Vl, H], Vl > 0,
+    nranks * Vl < 2^31; weight bfloat16, float16 or float32; dweight float32 or grad_out's dtype. rows: contiguous [T / nranks or T, H]
+    (bfloat16, float16 or float32, weight's dtype in the forward). H > 0 and H * itemsize a multiple of 16 bytes for every dtype; at most
+    2^31 - 1 16-byte vectors in each tensor. Alignment: ids 8 bytes, the others 16. out must not overlap weight or ids, dweight not
+    grad_out or ids. symmetric(tensor) -> bool, given with nranks > 1: weight (forward) or the sequence-parallel grad_out (backward) must
+    be arena memory when T > 0."""
+    import torch
+    what = "vocab_parallel_embedding" + ("_backward" if backward else "")
+    wide = (torch.bfloat16, torch.float16, torch.float32)
+    if ids.dtype != torch.int64 or ids.dim() != 1 or not ids.is_contiguous():
+        raise ValueError(f"{what}: ids must be a contiguous [tokens] int64 tensor, got {ids.dtype} {list(ids.shape)}")
+    T = ids.shape[0]
+    if table.dim() != 2 or not table.is_contiguous():
+        raise ValueError(f"{what}: {'dweight' if backward else 'weight'} must be a contiguous [vocab_local, hidden] tensor, got shape {list(table.shape)}")
+    vl, h = table.shape
+    rdt = rows.dtype if rows is not None else table.dtype
+    if rdt not in wide or (not backward and table.dtype not in wide):
+        raise ValueError(f"{what}: {'grad_out' if backward else 'weight'} must be bfloat16, float16 or float32, got {rdt if backward else table.dtype}")
+    if backward and table.dtype not in (torch.float32, rdt):
+        raise ValueError(f"{what}: dweight must be float32 or grad_out's dtype {rdt}, got {table.dtype}")
+    if not backward and rows is not None and rows.dtype != table.dtype:
+        raise ValueError(f"{what}: out must have weight's dtype {table.dtype}, got {rows.dtype}")
+    ers, ets = torch.empty((), dtype=rdt).element_size(), table.element_size()
+    if h == 0 or (h * ers) % 16 or (h * ets) % 16:
+        raise ValueError(f"{what}: hidden must be positive and hidden * itemsize a multiple of 16 bytes for every dtype, got {h}")
+    if vl == 0:
+        raise ValueError(f"{what}: vocab_local must be positive")
+    if nranks * vl >= 2 ** 31:
+        raise ValueError(f"{what}: nranks * vocab_local must be below 2^31, got {nranks} x {vl}")
+    if T >= 2 ** 31:
+        raise ValueError(f"{what}: tokens must be below 2^31, got {T}")
+    if sequence_parallel and T % nranks:
+        raise ValueError(f"{what}: tokens must be a multiple of nranks under sequence parallelism, got {T} and {nranks}")
+    nr = T // nranks if sequence_parallel else T
+    if max(nr * h * ers, vl * h * ers, vl * h * ets) // 16 > 2 ** 31 - 1:
+        raise ValueError(f"{what}: more than 2^31 - 1 16-byte vectors in one tensor")
+    if rows is not None and (tuple(rows.shape) != (nr, h) or not rows.is_contiguous()):
+        raise ValueError(f"{what}: {'grad_out' if backward else 'out'} must be a contiguous [{nr}, {h}] tensor, got {list(rows.shape)}")
+    if ids.data_ptr() % 8:
+        raise ValueError(f"{what}: ids must be 8-byte aligned")
+    if table.data_ptr() % 16 or (rows is not None and rows.data_ptr() % 16):
+        raise ValueError(f"{what}: {'dout and dweight' if backward else 'weight and out'} must be 16-byte aligned")
+    if T and rows is not None:
+        span = lambda t: (t.data_ptr(), t.numel() * t.element_size())     # noqa: E731
+        o, ins = (span(table), [span(rows), span(ids)]) if backward else (span(rows), [span(table), span(ids)])
+        if any(_xent_overlap(o, x) for x in ins):
+            raise ValueError(f"{what}: " + ("dweight must not overlap dout or ids" if backward else "out must not overlap weight or ids"))
+    if nranks > 1 and T and symmetric is not None and (not backward or sequence_parallel):
+        t = rows if backward else table
+        if t is not None and not symmetric(t):
+            raise ValueError(f"{what}: {'grad_out' if backward else 'weight'} must lie in the symmetric arena (Comm.empty), at the same offset on every rank")
+    return T, h, vl
+
+
 def _check_routed(nranks: int, x, topk_idx, num_experts: int, recv, expert_counts, route, dropped, fp8=None) -> None:
     """The rules of both device-routed dispatches; fp8 is None (check_expert_dispatch) or (recv_scales, block), which adds the FP8
     call's rules, as routed_prepare in coll/src/dispatch.cu takes a RoutedQuant."""
@@ -1572,6 +1632,72 @@ class Comm:
         the gradient over the logits (they must not be needed afterwards)."""
         return _vocab_xent_fn().apply(logits, target, self, int(ignore_index), bool(inplace_backward), stream)
 
+    def vocab_parallel_embedding(self, ids, weight, *, sequence_parallel: bool = False, out=None, stream=None):
+        """The tensor-parallel input embedding, one kernel: weight is this rank's [Vl, H] rows of the table (global ids
+        [rank * Vl, (rank + 1) * Vl)), ids the [T] int64 global ids, the same on every rank. Returns out = the unsplit table's rows of ids
+        (+0 rows for ids outside [0, nranks * Vl)), bit for bit: [T, H] on every rank, or with sequence_parallel this rank's rows
+        [rank * T / N, (rank + 1) * T / N). With more than one rank weight must be arena memory (Comm.empty); each rank pulls its rows
+        from their owners over NVLink."""
+        T = ids.shape[0] if ids.dim() == 1 else 0
+        nr = T // self.nranks if sequence_parallel else T
+        if out is None:
+            out = weight.new_empty((nr, weight.shape[1] if weight.dim() == 2 else 0))
+        T, h, vl = check_vocab_parallel_embedding(self.nranks, ids, weight, out, sequence_parallel=sequence_parallel,
+                                                  symmetric=self.is_symmetric)
+        _check(load().b200collVocabParallelEmbedding(ids.data_ptr(), weight.data_ptr(), out.data_ptr(), T, h, vl, int(bool(sequence_parallel)),
+                                                     torch_dtype_code(weight.dtype), self._h, self._stream(stream)), "VocabParallelEmbedding")
+        return out
+
+    def vocab_parallel_embedding_backward(self, ids, grad_out, grad_weight=None, *, vocab_local: Optional[int] = None,
+                                          sequence_parallel: bool = False, accumulate: bool = False, stream=None):
+        """The gradient of vocab_parallel_embedding with respect to this rank's weight: grad_weight[j] = the sum, in fp32 and in token
+        order, of grad_out's rows of the tokens whose id is rank * Vl + j, rounded once (added to grad_weight's old value with
+        accumulate). grad_out is [T, H] (the same on every rank), or with sequence_parallel this rank's [T / N, H] shard, which must then
+        be arena memory with more than one rank. grad_weight: a [Vl, H] float32 (a main_grad) or grad_out-dtype tensor, or None to
+        allocate a float32 one (vocab_local required then). Returns grad_weight."""
+        import torch
+        if grad_weight is None:
+            if vocab_local is None:
+                raise ValueError("vocab_parallel_embedding_backward: give grad_weight or vocab_local")
+            grad_weight = grad_out.new_empty((int(vocab_local), grad_out.shape[-1]), dtype=torch.float32)
+        T, h, vl = check_vocab_parallel_embedding(self.nranks, ids, grad_weight, grad_out, sequence_parallel=sequence_parallel, backward=True,
+                                                  symmetric=self.is_symmetric)
+        _check(load().b200collVocabParallelEmbeddingBackward(ids.data_ptr(), grad_out.data_ptr(), grad_weight.data_ptr(), T, h, vl,
+                                                             int(bool(sequence_parallel)), torch_dtype_code(grad_out.dtype),
+                                                             torch_dtype_code(grad_weight.dtype), int(bool(accumulate)), self._h,
+                                                             self._stream(stream)), "VocabParallelEmbeddingBackward")
+        return grad_weight
+
+    def vocab_parallel_embedding_lookup(self, ids, weight, *, sequence_parallel: bool = False, stream=None):
+        """vocab_parallel_embedding as an autograd function: returns out; .backward() runs vocab_parallel_embedding_backward on this
+        communicator into a fresh grad_weight of weight's dtype. Under sequence parallelism the backward needs its incoming gradient
+        in arena memory, so with more than one rank it is always copied into the communicator's arena staging buffer first (one
+        [T / N, H] copy on the call's stream; the same decision on every rank keeps the arena allocations in step)."""
+        return _vocab_embedding_fn().apply(ids, weight, self, bool(sequence_parallel), stream)
+
+    def _embedding_stage(self, g, stream=None):
+        """g copied into this communicator's arena staging buffer for the sequence-parallel embedding gradient (one [T / N, H] copy on
+        the call's stream), returned as a view of the buffer. One buffer per communicator, grown to at least twice its size when a
+        call needs more; a superseded buffer is kept until the communicator is destroyed (a kernel already queued, or a peer's pull of
+        it, may still read it), so all of them together stay below twice the largest. Every rank stages the same sizes in the same
+        order, which keeps the arena allocations, a collective contract, the same on every rank. Reusing the buffer on one stream is
+        safe: the backward's closing barrier ends every peer's reads before the stream moves on."""
+        import torch
+        need = g.numel() * g.element_size()
+        buf = self.__dict__.get("_emb_stage")
+        if buf is None or buf.numel() < need:
+            if buf is not None:
+                self.__dict__.setdefault("_emb_stage_retired", []).append(buf)
+            buf = self.empty(max(need, 2 * (buf.numel() if buf is not None else 0)), torch.uint8)
+            self._emb_stage = buf
+        staged = buf[:need].view(g.dtype).view(g.shape)
+        s = stream if stream is not None else torch.cuda.current_stream(g.device)
+        s.wait_stream(torch.cuda.current_stream(g.device))
+        with torch.cuda.stream(s):
+            staged.copy_(g)
+        g.record_stream(s)
+        return staged
+
     def _rows(self, xs):
         """A host list of nranks row counts or offsets, as the library's int64[nranks]."""
         return (C.c_int64 * self.nranks)(*[int(x) for x in xs])
@@ -1831,3 +1957,37 @@ def _vocab_xent_fn():
 
         _VOCAB_XENT_FN = VocabParallelCrossEntropy
     return _VOCAB_XENT_FN
+
+
+_VOCAB_EMBEDDING_FN = None
+
+
+def _vocab_embedding_fn():
+    """The torch.autograd.Function behind Comm.vocab_parallel_embedding_lookup, built on first use (torch is imported lazily here)."""
+    global _VOCAB_EMBEDDING_FN
+    if _VOCAB_EMBEDDING_FN is None:
+        import torch
+
+        class VocabParallelEmbedding(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, ids, weight, comm, sequence_parallel, stream):
+                out = comm.vocab_parallel_embedding(ids, weight, sequence_parallel=sequence_parallel, stream=stream)
+                ctx.save_for_backward(ids)
+                ctx.comm, ctx.sp, ctx.stream = comm, sequence_parallel, stream
+                ctx.vl, ctx.wdtype = weight.shape[0], weight.dtype
+                return out
+
+            @staticmethod
+            def backward(ctx, grad_out):
+                (ids,) = ctx.saved_tensors
+                comm = ctx.comm
+                g = grad_out.to(ctx.wdtype).contiguous()
+                if ctx.sp and comm.nranks > 1 and ids.shape[0]:
+                    # always staged (never decided per rank from where g happens to lie): the staging buffer is an arena allocation
+                    g = comm._embedding_stage(g, ctx.stream)
+                gw = torch.empty((ctx.vl, g.shape[1]), dtype=ctx.wdtype, device=g.device)
+                comm.vocab_parallel_embedding_backward(ids, g, gw, sequence_parallel=ctx.sp, stream=ctx.stream)
+                return None, gw, None, None, None
+
+        _VOCAB_EMBEDDING_FN = VocabParallelEmbedding
+    return _VOCAB_EMBEDDING_FN
